@@ -5,6 +5,7 @@
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference --steps 2 --warmup 1      # CPU arm (oracle port of the reference's BA)
+    python bench.py --gpus 1 --steps 5 --warmup 3 --dump-outputs DIR    # + the last step's results as DIR/*.npy
 
 One "step" = one bundle-adjustment solve of ITERS Levenberg-Marquardt iterations (residual/Jacobian ->
 Schur -> Cholesky -> back-substitution -> candidate evaluation -> accept/reject) on configuration C3
@@ -49,21 +50,21 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 def load_tensor_peak():
-    """Measured dense bf16 TFLOP/s of this pool's B200s (burst: a kernel timed alone), else the profiling recipe's figure."""
+    """Measured dense bf16 TFLOP/s (burst: a kernel timed alone), else the H100 SXM data sheet's dense figure."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         if "bf16_tflops" in d:
             return float(d["bf16_tflops"]), "measured cuBLAS bf16 (MEASURED_PEAKS.json)"
-    return 1650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, "H100 SXM data sheet (dense bf16)"
 
 
 class ClockSampler:
-    """SM clock and throttle reasons DURING the timed region (B200_PROFILING.md recipe), sampled in-process through
+    """SM clock and throttle reasons DURING the timed region, sampled in-process through
     NVML every 250 ms (an `nvidia-smi -lms` child process was measured to slow the timed region by ~30 %)."""
 
     def __init__(self, index=0):
@@ -148,24 +149,11 @@ def cpu_ba_sample(sc, extr, K, extra, pts, iters):
 
 
 def cpu_tri_sample(sc, ntracks):
-    """CPU triangulate_tracks (256 hypotheses) on the first `ntracks` tracks of C3; returns (tracks/s, seconds, kind).
-    kind = "reference": the reference's own triangulate_tracks (vggsfm/utils/triangulation.py:677) imported from
-    /root/reference with stub third-party modules (build container only -- the path does not exist on the GPU box);
-    kind = "port": oracle/tri_oracle.py (numpy restatement pinned to the reference's goldens)."""
+    """CPU triangulate_tracks (256 hypotheses) on the first `ntracks` tracks of C3 with oracle/tri_oracle.py (the numpy
+    restatement pinned to the reference's goldens); returns (tracks/s, seconds, kind)."""
     import torch
-    from oracle import reference_shim, tri_oracle as to
+    from oracle import tri_oracle as to
     tn = to.cam_from_img(sc.tracks[:, :ntracks].astype(np.float64), sc.intrinsics, sc.extra_params)
-    if reference_shim.available():
-        reference_shim.install()
-        from vggsfm.utils.triangulation import triangulate_tracks as ref_tt
-        torch.set_num_threads(os.cpu_count() or 1)
-        E = torch.from_numpy(sc.extrinsics)
-        tnt = reference_shim.contiguous_tracks(torch.from_numpy(tn))
-        torch.manual_seed(0)
-        t0 = time.perf_counter()
-        ref_tt(E, tnt, track_vis=torch.from_numpy(sc.vis[:, :ntracks]), track_score=torch.from_numpy(sc.score[:, :ntracks]))
-        dt = time.perf_counter() - t0
-        return ntracks / dt, dt, "reference"
     torch.manual_seed(0)
     pairs = to.draw_pairs(S_FRAMES, 256)
     t0 = time.perf_counter()
@@ -216,9 +204,9 @@ def run_reference(args):
 def syrk_roofline(D, K3, dev, clocks):
     import torch
     from vggsfm_b200 import _lib
-    """Times vgg_syrk_ozaki (slice + tcgen05 SYRK) at this rank's Schur shape with CUDA events.  Algorithmic work =
-    28 int8 GEMM pairs x 2 K Dpad (Dpad+128)/2 ops on the lower tiles; peak = 148 SMs x 8192 MAC/clk (the kind::i8 rate
-    measured with N=256, tools/syrk_i8_check.py rate) x 2 x the SM clock sampled during the run."""
+    """Times vgg_syrk_ozaki (slice + wgmma SYRK) at this rank's Schur shape with CUDA events.  Algorithmic work =
+    28 int8 GEMM pairs x 2 K Dpad (Dpad+128)/2 ops on the lower tiles; peak = 132 SMs x 4096 dense int8 MAC/clk/SM (the
+    H100 SXM data sheet's 1979 TOP/s at its 1830 MHz boost clock) x 2 x the SM clock sampled during the run."""
     import ctypes
     L = _lib.lib()
     Dpad = (D + 2 + 127) // 128 * 128
@@ -247,12 +235,12 @@ def syrk_roofline(D, K3, dev, clocks):
     ms = a.elapsed_time(b) / reps
     pairs = slices * (slices + 1) // 2
     ops = pairs * 2.0 * Kpad * Dpad * (Dpad + 128) / 2
-    sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
-    peak = 148 * 8192 * 2 * sm_mhz * 1e6 / 1e12
+    sm_mhz = (clocks or {}).get("sm_mhz") or 1830.0
+    peak = 132 * 4096 * 2 * sm_mhz * 1e6 / 1e12
     ach = ops / (ms * 1e-3) / 1e12
-    return {"kernel": "oz_slice_kernel + oz_syrk_kernel (tcgen05.mma kind::i8, 7 Ozaki slices)", "bound": "tensor",
+    return {"kernel": "oz_slice_kernel + oz_syrk_kernel (wgmma s8, 7 Ozaki slices)", "bound": "tensor",
             "achieved": ach, "peak": peak, "unit": "TOP/s", "frac": ach / peak, "ms_per_call": ms,
-            "peak_source": "148 SMs x 8192 int8 MAC/clk/SM (measured kind::i8 N=256 issue rate) x sampled SM clock",
+            "peak_source": "132 SMs x 4096 int8 MAC/clk/SM (H100 SXM data sheet, dense) x sampled SM clock",
             "fp64_equivalent_tflops": 2.0 * Kpad * Dpad * (Dpad + 128) / 2 / (ms * 1e-3) / 1e12,
             "note": "time includes the column-max and slicing kernels; in the LM loop the column max is fused into z_build"}
 
@@ -299,14 +287,13 @@ def corr_section(dev, hbm_peak):
             rec = {"shape": [B, S, C, H, W], "queries": N, "levels": L, "radius": r, "ms_fused": ms,
                    "pairs_per_s": B * S * N / (ms * 1e-3)}
             if getattr(ours._pyr, "tc_tiles", None) is not None:
-                # tcgen05 path (csrc/corr_tc.cu): the dense per-level correlation runs on the tensor cores (kind::f16,
-                # fp32 accumulators in TMEM) and is sampled from TMEM -- tensor-bound, not HBM-bound
+                # tensor-core path (csrc/corr_tc.cu): the dense per-level correlation runs on wgmma (f16 operands, fp32
+                # register accumulators) and is sampled from the accumulators -- tensor-bound, not HBM-bound
                 fl = 2.0 * B * S * N * C * sum((H >> l) * (W >> l) for l in range(L))
                 tpk, tsrc = load_tensor_peak()
-                rec.update({"kernel": "corr_tc_kernel (tcgen05.mma kind::f16, M=128 N=256, TMEM accumulators)", "bound": "tensor",
+                rec.update({"kernel": "corr_tc_kernel (wgmma m64n256k16 f16, register accumulators)", "bound": "tensor",
                             "flops": fl, "achieved_tflops": fl / (ms * 1e-3) / 1e12, "tensor_peak_tflops": tpk,
-                            "tensor_peak_source": tsrc, "frac_of_tensor_peak": fl / (ms * 1e-3) / 1e12 / tpk,
-                            "ncu": "profiles/r02_ncu_corr_tc8.txt: sm__pipe_tensor_subpipe_hmma_cycles_active 38.7 %"})
+                            "tensor_peak_source": tsrc, "frac_of_tensor_peak": fl / (ms * 1e-3) / 1e12 / tpk})
             else:
                 rec.update({"kernel": ("corr_sample_c32_kernel (CUDA cores, one footprint position per lane)" if C == 32
                                        else "corr_sample_kernel (CUDA cores, channels across lanes)"),
@@ -382,6 +369,15 @@ def small_problem_section(dev):
     return out
 
 
+def dump_outputs(out_dir, arrays, rank, world):
+    """What the timed path returned in its last step, as float64 .npy files (a few MB at C3).  With several ranks each
+    rank writes its own shard of the per-track arrays under a rank suffix."""
+    os.makedirs(out_dir, exist_ok=True)
+    suffix = f".rank{rank}" if world > 1 else ""
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + suffix + ".npy"), t.detach().to("cpu").double().numpy())
+
+
 def run_gpu(args):
     import torch
     import torch.distributed as dist
@@ -436,16 +432,20 @@ def run_gpu(args):
                          "(csrc/fabric.cu; no NCCL call and no host callback inside the LM loop)")
         else:
             reduction = "fabric v1: multimem.red all-reduce fused into the Schur kernels (NVSwitch multicast) + host-hook barriers"
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 50 MB L2
 
     def barrier():
         if world > 1:
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = {}
+
     def ba_step():
         poses, intr, X = poses0.clone(), intr0.clone(), pts0.clone()
-        return ba.lm_solve(uv, mask, poses, intr, X, model, mode, param_const, None, opt, hook)
+        summary = ba.lm_solve(uv, mask, poses, intr, X, model, mode, param_const, None, opt, hook)
+        last.update(ba_poses=poses, ba_intrinsics=intr, ba_points3d=X)
+        return summary
 
     # ---- timed region 1: BA
     launches = 0
@@ -498,7 +498,7 @@ def run_gpu(args):
     e0.record()
     for _ in range(args.steps):
         flush.fill_(1.0)
-        p3, num, _ = tri_pass()
+        p3, num, inl = tri_pass()
         launches += 6
     e1.record()
     barrier()
@@ -508,6 +508,9 @@ def run_gpu(args):
     tri_ms = float(tms.item())
     tracks_per_s = N_TRACKS * args.steps / (tri_ms * 1e-3)
     tri_median_err = float(np.median(np.linalg.norm(p3.cpu().numpy() - sc.points3d[lo:hi], axis=1)))
+    if args.dump_outputs:
+        last.update(tri_points3d=p3, tri_inlier_count=num, tri_inlier_mask=inl)
+        dump_outputs(args.dump_outputs, last, rank, world)
 
     # ---- e2e: public API with host (pinned) buffers, copies inside the timed region
     h_tracks = torch.from_numpy(sc.tracks[:, lo:hi].copy()).pin_memory()
@@ -593,9 +596,6 @@ def run_gpu(args):
         ach = ab / (ms * 1e-3) / 1e9
         roof = {"kernel": "ba_blocks_kernel<SIMPLE_RADIAL,INTR_SHARED,TMA>", "bound": "hbm", "achieved": ach,
                 "peak": peak, "peak_source": peak_src, "unit": "GB/s", "frac": ach / peak,
-                # dram__bytes_read.sum + dram__bytes_write.sum of this launch from the ncu --set full capture
-                # profiles/r02_ncu_blocks_c3b.txt (16.0 MB + 176.7 MB; part of W is still in the 126 MB L2 when the counters stop)
-                "traffic": 1.927e8 if n_loc == N_TRACKS else None,
                 "bytes_per_launch": ab, "ms_per_launch": ms, "ms_per_call": ms_call, "observations": obs,
                 "note": "ms_per_launch: CUDA event pair on the launching stream directly around the kernel; ms_per_call adds "
                         "the accumulator memset and the W-tail memset2D of one build_blocks call; 256 MB L2 flush before each"}
@@ -611,10 +611,7 @@ def run_gpu(args):
             ab_s = algo_bytes(S_FRAMES, NS_)
             ach_s = ab_s / (ms_s * 1e-3) / 1e9
             roof["scaled"] = {"workload": "400 x 131072 tracks", "achieved": ach_s, "frac": ach_s / peak,
-                              "bytes_per_launch": ab_s, "ms_per_launch": ms_s, "ms_per_call": ms_s_call,
-                              # dram__bytes_read.sum + dram__bytes_write.sum of this launch shape from the ncu --set full
-                              # capture kept in profiles/r01_ncu_full_summary_k1_scaled.txt (0.58 GB + 7.51 GB)
-                              "traffic": 8.09e9}
+                              "bytes_per_launch": ab_s, "ms_per_launch": ms_s, "ms_per_call": ms_s_call}
             del uv_s, mk_s, X_s
         except Exception as e:     # out of memory on a shared box: keep the C3-size number
             roof["scaled"] = {"error": str(e)[:200]}
@@ -662,14 +659,14 @@ def run_gpu(args):
             "dtype": "f64", "data": "synthetic",
             "config": {"workload": WORKLOAD, "lm_iterations_per_step": ITERS, "parallelism": f"track-shard x{world}",
                        "reduction": reduction,
-                       "tracks_per_rank": n_loc, "l2": "256 MB flush write between steps; working set ~0.8 GB > 126 MB L2",
+                       "tracks_per_rank": n_loc, "l2": "256 MB flush write between steps; working set ~0.8 GB > 50 MB L2",
                        "final_cost": final_cost},
             "tracks_per_s": tracks_per_s, "tri_ms_per_pass": tri_ms / args.steps, "tri_median_point_error": tri_median_err,
             "e2e": {"value": e2e_value, "unit": "it/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
             "gpu_launches": int(launches), "clocks": clocks, "roofline": roof, "roofline_syrk": roof_syrk,
             "cpu_baseline": cpu_base, "corr": corr, "small_problems": small, "c5": c5,
         }
-        line["config"]["syrk"] = os.environ.get("VGG_SYRK", "ozaki:7") + " (default: tcgen05 kind::i8, 7 Ozaki slices, FP64-equivalent)"
+        line["config"]["syrk"] = os.environ.get("VGG_SYRK", "ozaki:7") + " (default: wgmma s8, 7 Ozaki slices, FP64-equivalent)"
         if hook is not None:
             line["config"]["allreduce_calls"] = hook.calls
             line["config"]["allreduce_bytes"] = hook.bytes
@@ -688,6 +685,9 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-corr", action="store_true", help="skip the C4 correlation section (rank 0, N=1 only)")
     ap.add_argument("--no-c5", action="store_true", help="skip the C5 sequential-video section (rank 0, N=1 only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed BA step's refined poses / intrinsics / points and the last triangulation "
+                         "pass's points / inlier counts / inlier mask as DIR/<name>.npy (float64; inputs are seeded)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * vggsfm_b200 -- C ABI of the B200-native geometry hot path for VGGSfM.
+ * vggsfm_b200 -- C ABI of the H100-native (sm_90a) geometry hot path for VGGSfM.
  *
  * The reference (facebookresearch/vggsfm @ e1d9d2e) has no FFI of its own: its seam for this path
  * is ordinary Python symbols plus the pycolmap object API (SURVEY.md section 8b).  Every entry
@@ -142,7 +142,7 @@ int vgg_cholesky_lower(int n, int lda, double* A, void* workspace, size_t ws_byt
 
 /* The same SYRK step on the tensor cores (csrc/syrk_i8.cu): Cmat[Dpad,Dpad] -= Zt^T Zt for Zt double [Kpad,Dpad]
  * (Dpad a multiple of 128), FP64-equivalent through `slices` (3..7; 7 = 54 fractional bits) int8
- * Ozaki slices on tcgen05.mma kind::i8 with exact int32 accumulation in TMEM.  The row-major LOWER triangle is written.
+ * Ozaki slices on wgmma s8 with exact int32 accumulation in registers.  The row-major LOWER triangle is written.
  * Selected inside vgg_ba_solve by VGG_SYRK=ozaki[:slices]; exposed for the parity tests and profiling. */
 int vgg_syrk_ozaki_workspace_bytes(int Kpad, int Dpad, int slices, size_t* bytes);
 int vgg_syrk_ozaki(int Kpad, int Dpad, const double* Zt, double* Cmat, int slices, void* workspace, size_t ws_bytes,
@@ -277,8 +277,8 @@ int vgg_corr_sample(int BS, int N, int C, int H, int W, int num_levels, int radi
                     const float* targets, const float* coords, int border_padding, float* out, void* stream);
 
 /* The same CorrBlock.corr + CorrBlock.sample for the coarse tracker's C = 128 maps ON THE TENSOR CORES
- * (csrc/corr_tc.cu: tcgen05.mma kind::f16 M=128 x N=256 x K=128 into TMEM, footprint extraction from TMEM in the
- * epilogue; the dense fp16 product of blocks.py:413 without ever storing the volume).  Zero padding only; map width a
+ * (csrc/corr_tc.cu: wgmma f16 M=64 x N=256 x K=128 per warpgroup into registers, footprint extraction from the register
+ * accumulators; the dense fp16 product of blocks.py:413 without ever storing the volume).  Zero padding only; map width a
  * power of two.  vgg_corr_tc_build turns the HALF channels-last pyramid of vgg_corr_build_pyramid into operand tile
  * images once per CorrBlock (tile_bytes from vgg_corr_tc_bytes); vgg_corr_tc_sample needs `target_bytes` of scratch for
  * the fp16 target tiles of the call.  Same targets / coords / out layout as vgg_corr_sample. */

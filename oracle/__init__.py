@@ -10,7 +10,7 @@ Modules
   ba_oracle    numpy float64 restatement of COLMAP 3.10's bundle adjustment
                (``ReprojErrorCostFunction`` + Ceres 2.x Levenberg-Marquardt with a
                direct Schur solve).  PARITY UNPINNED: pycolmap/pyceres are absent from
-               this container and from /root/reference, and the reference holds no golden
+               this environment and from the reference, and the reference holds no golden
                vectors for this boundary (SURVEY.md section 8c).  Self-validated against
                scipy.optimize.least_squares and finite differences instead.
   tri_oracle   numpy float64 restatement of the reference's pure-torch triangulation

@@ -1,8 +1,8 @@
 """CPU oracle for the bundle-adjustment half of the hot path -- TEST INFRASTRUCTURE ONLY.
 
 PARITY UNPINNED.  The arithmetic restated here lives in third-party engines that are not
-under /root/reference and are not installable in this container:
-  * pycolmap 3.10.0 (pin: /root/reference/install.sh:41) -- COLMAP 3.10
+in the reference and could not be installed:
+  * pycolmap 3.10.0 (pin: the reference's install.sh:41) -- COLMAP 3.10
     ``BundleAdjustmentController::Run`` / ``BundleAdjuster`` / ``ReprojErrorCostFunction`` /
     ``SimplePinholeCameraModel`` / ``SimpleRadialCameraModel`` / ``Reconstruction::Normalize``
   * pyceres 2.3 (install.sh:42) -- Ceres 2.x ``TrustRegionMinimizer`` +

@@ -74,7 +74,7 @@ class TorchCorrBlock:
     with every spatial position (fp16 under autocast on a GPU, as the reference runs it, runners/runner.py:418), the
     [B,S,N,H,W] volume in memory, then F.grid_sample (align_corners=True, zeros padding) at the (2r+1)^2 taps.  This is
     what the reference executes on a GPU; bench.py times it as the C4 baseline (kind "port": written from the reference's
-    description, not imported -- /root/reference does not exist on the GPU box)."""
+    description, not imported from it)."""
 
     def __init__(self, fmaps, num_levels=4, radius=4, padding_mode="zeros"):
         B, S, C, H, W = fmaps.shape

@@ -1,8 +1,8 @@
 """CPU oracle for absolute-pose refinement (motion-only BA) -- TEST INFRASTRUCTURE ONLY.
 
-PARITY UNPINNED.  ``pycolmap.pose_refinement`` (pycolmap 3.10.0, pin /root/reference/install.sh:41)
+PARITY UNPINNED.  ``pycolmap.pose_refinement`` (pycolmap 3.10.0, pin: the reference's install.sh:41)
 is COLMAP 3.10 ``RefineAbsolutePose`` (src/colmap/estimators/pose.cc) on Ceres 2.x; neither is
-under /root/reference nor installable here, and the reference holds no golden vectors for it.
+in the reference nor installable, and the reference holds no golden vectors for it.
 Restated from the published algorithm [3P-memory]:
   * one ``ReprojErrorConstantPoint3DCostFunction<CameraModel>`` per inlier correspondence,
     wrapped in ``ceres::CauchyLoss(1.0)``;

@@ -1,19 +1,18 @@
-"""Import the UNMODIFIED reference (/root/reference) with stub third-party modules -- TEST INFRASTRUCTURE ONLY.
+"""Import the UNMODIFIED reference (a facebookresearch/vggsfm checkout named by $VGGSFM_REFERENCE) with stub
+third-party modules -- GOLDEN GENERATION ONLY.
 
-Used in the build container (where /root/reference exists) to validate the oracle restatements and to
-generate the golden fixtures under tests/golden/ (tools/make_golden.py).  /root/reference does not exist
-on the GPU box: nothing in the `-m gpu` tests, smoke() or bench.py calls this module.
-Recipe: SURVEY.md Appendix C.
+The tools/make_golden*.py scripts use it to run the reference and store what the tests compare against under
+tests/golden/; no test, smoke() or bench.py calls this module.  Recipe: SURVEY.md Appendix C.
 """
 import os
 import sys
 import types
 
-REFERENCE_ROOT = "/root/reference"
+REFERENCE_ROOT = os.environ.get("VGGSFM_REFERENCE", "")
 
 
 def available() -> bool:
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "vggsfm"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "vggsfm"))
 
 
 class _Stub(types.ModuleType):
@@ -38,7 +37,7 @@ _STUBS = ["hydra", "hydra.utils", "pycolmap", "pyceres", "kornia", "kornia.core"
 def install():
     """Put the reference on sys.path with stubs for the absent third-party packages."""
     if not available():
-        raise RuntimeError("/root/reference is not present on this machine")
+        raise RuntimeError("set VGGSFM_REFERENCE to a facebookresearch/vggsfm checkout")
     import torch
     for name in _STUBS:
         sys.modules.setdefault(name, _Stub(name))

@@ -4,7 +4,7 @@ numpy float64 restatement of the reference's pure-torch geometry functions.  PIN
 the reference itself (imported in the build container through oracle/reference_shim.py) by
 tests/test_tri_oracle.py and through the committed fixtures in tests/golden/.
 
-Follows (all under /root/reference):
+Follows (all in the reference):
   triangulate_tracks_single_chunk     vggsfm/utils/triangulation.py:776-956
   local_refine_and_compute_error      vggsfm/utils/triangulation.py:959-1017
   local_refinement_tri                vggsfm/utils/triangulation_helpers.py:648-725

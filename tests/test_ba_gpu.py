@@ -202,7 +202,7 @@ def test_c2_full_solve_matches_oracle(cuda_dev):
 def test_c3_bench_config_matches_oracle(cuda_dev):
     """The configuration bench.py publishes numbers on (C3: 400 x 4096, SIMPLE_RADIAL, shared camera, dense visibility;
     the same scene and perturbed start as bench.make_problem): first 3 LM iterations on the default product path
-    (tcgen05 Ozaki SYRK + the in-repo Cholesky) against the oracle."""
+    (wgmma Ozaki SYRK + the in-repo Cholesky) against the oracle."""
     c = ba_case(400, 4096, "SIMPLE_RADIAL", bo.INTR_SHARED, seed=0, invisible_frac=0.0)
     ref, got = _solve_both(c, cuda_dev, 3, use_c=bo._load_c() is not None)
     assert got[3].iterations == 3

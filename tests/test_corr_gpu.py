@@ -73,7 +73,7 @@ def test_c4_shape_linearity(cuda_dev):
 
 @pytest.mark.parametrize("H,W,N,L,r", [(32, 32, 130, 3, 4), (24, 64, 256, 4, 3), (128, 128, 128, 5, 4)])
 def test_tensor_core_path_matches_cuda_core_path(cuda_dev, H, W, N, L, r):
-    """csrc/corr_tc.cu (tcgen05 kind::f16, footprint extraction from TMEM) against csrc/corr.cu on the same half
+    """csrc/corr_tc.cu (wgmma f16, footprint extraction from the register accumulators) against csrc/corr.cu on the same half
     pyramid: both round targets and features to fp16 and accumulate in fp32, only the summation order differs (1e-3 of
     the value range); queries on, near and beyond the border, a ragged last 128-query tile, non-square maps."""
     import torch

@@ -1,5 +1,5 @@
 """CPU: the triangulation oracle (oracle/tri_oracle.py) against the committed golden fixtures produced by
-the reference itself (tools/make_golden.py), and -- when /root/reference is present -- against a live run."""
+the reference itself (tools/make_golden.py, tools/make_golden_live.py)."""
 import glob
 import os
 
@@ -48,36 +48,17 @@ def test_oracle_matches_reference_golden(path):
 
 
 def test_oracle_matches_live_reference():
-    from oracle import reference_shim as rs
-    if not rs.available():
-        pytest.skip("/root/reference not present on this machine")
-    import warnings
+    """The reference's triangulate_tracks (stable sort, torch seed 3) on a 10 x 40 scene, stored by
+    tools/make_golden_live.py; the oracle draws the same pairs from the same seed."""
     import torch
-    warnings.filterwarnings("ignore")
-    rs.install()
-    from vggsfm.utils import triangulation as rt
-    from vggsfm.utils import triangulation_helpers as rh
     from vggsfm_b200.synthetic import make_scene
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_triangulate_10x40.npz"))
     sc = make_scene(10, 40, "SIMPLE_RADIAL", seed=21, invisible_frac=0.2, outlier_frac=0.1)
-    K, E, ex = torch.from_numpy(sc.intrinsics), torch.from_numpy(sc.extrinsics), torch.from_numpy(sc.extra_params)
-    tn = rh.cam_from_img(torch.from_numpy(sc.tracks), K, ex)
-    _sort = torch.sort
-
-    def stable(*a, **k):
-        k["stable"] = True
-        return _sort(*a, **k)
-    torch.manual_seed(3)
-    torch.sort = stable
-    try:
-        p, n, m = rt.triangulate_tracks(E, rs.contiguous_tracks(tn), track_vis=torch.from_numpy(sc.vis),
-                                        track_score=torch.from_numpy(sc.score))
-    finally:
-        torch.sort = _sort
     torch.manual_seed(3)
     pairs = to.draw_pairs(10, 256)
-    po, no, mo = to.triangulate_tracks(sc.extrinsics, tn.numpy(), pairs, sc.vis, sc.score)
-    assert np.array_equal(no, n.numpy()) and np.array_equal(mo, m.numpy())
-    assert np.abs(po - p.numpy()).max() < 1e-9
+    po, no, mo = to.triangulate_tracks(sc.extrinsics, g["tn"], pairs, sc.vis, sc.score)
+    assert np.array_equal(no, g["num"]) and np.array_equal(mo, g["mask"])
+    assert np.abs(po - g["points"]).max() < 1e-9
 
 
 def test_undistortion_quirk_is_reproduced():

@@ -23,7 +23,7 @@ def test_band_hint_does_not_change_the_joint_ba(cuda_dev):
     """The tile / k-range skipping of the tensor-core SYRK (band hint from the visibility mask, csrc/ba_solve.cu) must
     leave the solve unchanged: same minimum (final cost to 1e-9 relative).  The iteration COUNT is not compared: the
     last iterations of these solves sit on the gradient / function tolerance and the count moves by a few from run to
-    run in either mode (f64 RED order; profiles/r02_c5_band_parity.log, tools/band_parity_check.py: 40-42 in both modes, costs equal to 13 digits)."""
+    run in either mode (f64 RED order; tools/band_parity_check.py shows it)."""
     import video_c5
     from vggsfm_b200 import video
     res = {}

@@ -1,4 +1,4 @@
-"""Generate tests/golden/*.npz by running the UNMODIFIED reference (/root/reference, imported with stub
+"""Generate tests/golden/*.npz by running the UNMODIFIED reference ($VGGSFM_REFERENCE, imported with stub
 third-party modules) on seeded synthetic inputs.  Run in the build container only:
 
     python tools/make_golden.py

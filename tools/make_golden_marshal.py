@@ -6,7 +6,7 @@ inverse ``pycolmap_to_batch_matrix`` (:163-214) with ``vggsfm_b200.reconstructio
 ``pycolmap`` module -- i.e. the reference's own O(S*P) Python loops decide ids, point2D order, the 3000 clamp and the
 camera sharing, and only the passive container classes are ours.  The flattened result is what
 ``Reconstruction.from_batch_matrix`` (the vectorised product path) must reproduce exactly.  Also pins the pure-torch
-``get_valid_frame_mask`` (vggsfm/utils/triangulation.py:1222-1242).  Needs /root/reference; run in the build container:
+``get_valid_frame_mask`` (vggsfm/utils/triangulation.py:1222-1242).  Needs $VGGSFM_REFERENCE (a reference checkout):
 
     python tools/make_golden_marshal.py
 """

@@ -5,7 +5,7 @@
 learned transformer is replaced on both sides by the deterministic stand-in tests/helpers.py:tiny_former (it is not on
 the hot path and its weights would not fit a fixture), the fine feature net by one 3x3 convolution.  kornia is absent:
 its two tiny functions used by compute_score_fn (create_meshgrid, dsnt.spatial_expectation2d) are restated here
-[3P-memory].  Needs /root/reference:   python tools/make_golden_tracker.py"""
+[3P-memory].  Needs $VGGSFM_REFERENCE:   python tools/make_golden_tracker.py"""
 import os
 import sys
 import types

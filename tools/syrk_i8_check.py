@@ -1,4 +1,4 @@
-"""Accuracy / timing check of the tcgen05 INT8 (Ozaki) SYRK against numpy float64 and the DMMA kernel path.
+"""Accuracy / timing check of the wgmma INT8 (Ozaki) SYRK against numpy float64 and the DMMA kernel path.
    python tools/syrk_i8_check.py [Dpad Kpad slices]"""
 import ctypes
 import os
@@ -12,23 +12,6 @@ sys.path.insert(0, ROOT)
 from vggsfm_b200 import _lib       # noqa: E402
 
 dev = torch.device("cuda:0")
-if len(sys.argv) > 1 and sys.argv[1] == "probe":
-    L = _lib.lib()
-    torch.zeros(1, device=dev)
-    o = (ctypes.c_int * 3)()
-    _lib.check(L.vgg_probe_remote_mbarrier(o, None), "probe")
-    print("remote-mbarrier probe: leader barrier completed =", o[0], " peer bytes landed =", o[1], " leader bytes landed =", o[2])
-    sys.exit(0)
-if len(sys.argv) > 1 and sys.argv[1] == "rate":
-    L = _lib.lib()
-    torch.zeros(1, device=dev)
-    for mode, name in [(0, "SW64  N=128"), (1, "SW64  N=256"), (2, "SW128 N=128"), (3, "SW128 N=256"), (4, "none  N=128"), (5, "none  N=256"),
-                       (8, "SW64  N=128 A-in-TMEM"), (9, "SW64  N=256 A-in-TMEM")]:
-        c = ctypes.c_double()
-        _lib.check(L.vgg_syrk_ozaki_mma_rate(4096, mode, ctypes.byref(c), None), "rate")
-        n = 256 if mode & 1 else 128
-        print(f"kind::i8 M=128 {name} K=32: {c.value:7.1f} cycles/MMA -> {128 * n * 32 / c.value:7.0f} MAC/clk/SM")
-    sys.exit(0)
 Dpad = int(sys.argv[1]) if len(sys.argv) > 1 else 256
 Kpad = int(sys.argv[2]) if len(sys.argv) > 2 else 640
 s = int(sys.argv[3]) if len(sys.argv) > 3 else 7

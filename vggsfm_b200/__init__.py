@@ -1,1 +1,1 @@
-"""vggsfm_b200 -- B200-native geometry hot path for VGGSfM (see DESIGN.md)."""
+"""vggsfm_b200 -- H100-native (sm_90a) geometry hot path for VGGSfM (see DESIGN.md)."""

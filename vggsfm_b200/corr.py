@@ -40,7 +40,7 @@ class _Pyramid:
                                                 scratch.data_ptr() if sb.value else None, _stream(dev)),
                        "vgg_corr_build_pyramid")
         self.dev = dev
-        # coarse tracker (C = 128, power-of-two maps, half pyramid): operand tile images for the tcgen05 kernel
+        # coarse tracker (C = 128, power-of-two maps, half pyramid): operand tile images for the wgmma kernel
         # (csrc/corr_tc.cu); VGG_CORR_TC=0 keeps the CUDA-core footprint kernel for A/B
         import os
         self.tc_tiles = None

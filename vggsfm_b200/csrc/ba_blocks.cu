@@ -404,7 +404,7 @@ static int launch_blocks(const vgg_ba_problem* p, double* cost, double* camrec, 
     static int slots_cache[2] = {0, 0};
     int& slots = slots_cache[minb == 3];
     if (slots == 0) {
-      int dev = 0, sms = 148, per_sm = minb;
+      int dev = 0, sms = 132, per_sm = minb;
       cudaGetDevice(&dev);
       cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
       // the occupancy query needs the opt-in shared-memory limit in place (r02: without it the query returned 0, the

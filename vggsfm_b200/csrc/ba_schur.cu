@@ -665,8 +665,8 @@ int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc
   const int nb = Dpad / SY_BM;
   const int ntiles = nb * (nb + 1) / 2;
   const int nslab = Kpad / SY_BK;
-  // split K so that the grid covers the 148 SMs a few times over
-  int splits = (148 * 3 + ntiles - 1) / ntiles;
+  // split K so that the grid covers the 132 SMs of an H100 SXM a few times over
+  int splits = (132 * 3 + ntiles - 1) / ntiles;
   if (splits < 1) splits = 1;
   if (splits > nslab) splits = nslab;
   int slabs_per = (nslab + splits - 1) / splits;

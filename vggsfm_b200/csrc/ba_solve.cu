@@ -181,8 +181,8 @@ struct Layout {
   size_t bytes;
 };
 
-// The Schur SYRK runs on the tensor cores by default (tcgen05 INT8 Ozaki slices, csrc/syrk_i8.cu: r01 A/B at C3
-// 2.46 ms -> 1.10 ms per iteration, 238 -> 348 it/s, same iterates).  VGG_SYRK=ozaki:N picks 3..7 slices (default 7 =
+// The Schur SYRK runs on the tensor cores by default (INT8 wgmma Ozaki slices, csrc/syrk_i8.cu; same iterates as the
+// FP64 kernels).  VGG_SYRK=ozaki:N picks 3..7 slices (default 7 =
 // 54 fractional bits, FP64-equivalent); VGG_SYRK=fp64 selects the FP64-pipe kernels (DMMA / DFMA).
 static int syrk_i8_slices() {
   static int slices = -1;

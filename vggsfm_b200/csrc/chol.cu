@@ -627,7 +627,7 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
 //            fused panel kernel of the next step is adding into at the same time); mode 4 = tile columns 2 and 3 only
 //            (REDs), mode 5 = tile columns >= 4 (REDs on 4 and 5): the two halves of mode 3 with different deadlines.
 //   TM = 32 (mode 1, the next panel's 128 columns = tile columns 0 and 1, ON the critical path): twice as many CTAs so
-//            the ~140 tiles of a 2400-row matrix fill the 148 SMs with one short tile each; warps 1x8, warp tile 32x8.
+//            the ~140 tiles of a 2400-row matrix fill the SMs with one short tile each; warps 1x8, warp tile 32x8.
 // Shared memory holds ONE K half (64 panel columns) of both operands at a time, row stride 68 doubles (fragment loads
 // conflict-free like stride 132): 68 KB per CTA instead of 135 KB, so an update CTA fits on an SM NEXT TO a panel CTA
 // (152 KB) and two or three fit on a free SM.  r02 launch list of the previous version (whole K resident, one CTA per
@@ -838,7 +838,7 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
   static const int persist_ctas = [] {
     const char* e = getenv("VGG_CHOL_PERSIST");
     if (!(e && e[0] == '1')) return 0;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     return sms;

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the vggsfm_b200 kernels (sm_100a only).
+// Shared device/host helpers for the vggsfm_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -124,6 +124,15 @@ __device__ __forceinline__ void tma_store_wait_all() {
 }
 // make generic-proxy shared-memory writes visible to the async proxy (TMA)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// wgmma (sm_90a): shared-memory matrix descriptor of a K-major operand in the 64-byte swizzle (Swizzle<2,4,3>; 8-row
+// core-matrix groups 512 B apart, tile base 512-byte aligned), and the warpgroup fence / commit / wait
+__device__ __forceinline__ uint64_t wgmma_desc_sw64(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (2ull << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
 // cp.async 16B (LDGSTS)
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {

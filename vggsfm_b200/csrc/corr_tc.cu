@@ -1,19 +1,17 @@
-// Coarse-tracker correlation on the 5th-generation tensor cores (tcgen05.mma kind::f16, TMEM accumulators).
+// Coarse-tracker correlation on the tensor cores (wgmma f16, fp32 register accumulators).
 //
 // CorrBlock.corr + CorrBlock.sample of the coarse tracker (vggsfm/models/track_modules/blocks.py:363-416: per level one
 // torch.matmul of the [N,C] targets with all H*W positions, fp16 under autocast, then (2r+1)^2 bilinear taps) for
-// C = 128 channels.  r02 measurement at BASELINE's C4 shape (128 frames x 1024 queries, 128x128 maps, 5 levels, r = 4):
-// the CUDA-core footprint kernel (csrc/corr.cu) needs 11.9 ms per refinement iteration -- 16.8 GB of L2 gathers, 0.2 of
-// the HBM roofline -- and loses to the reference's own GPU path (dense fp16 GEMM + grid_sample: 4.7 ms).  The dense
-// product is the right shape for this chip after all, as long as the 5.7 GB volume is never written: here one CTA per
-// SM walks work items (frame, 128 queries); per level and per tile of 256 positions it issues
-// tcgen05.mma M=128 x N=256 x K=128 (8 instructions of K=16) from shared memory into one of two 256-column TMEM
-// accumulators, while eight epilogue warps (thread = query = TMEM lane, two warps per lane quarter) drain the other one with tcgen05.ld and keep
-// only the (2r+2)^2 footprint values each query needs, in a shared-memory footprint table; after a level's last tile the
-// same warps interpolate the (2r+1)^2 taps and write them.  The correlation volume lives 2 us in TMEM.
+// C = 128 channels.  The CUDA-core footprint kernel (csrc/corr.cu) gathers the footprints through L2, which at the C4
+// shape (128 frames x 1024 queries, 128x128 maps, 5 levels, r = 4) is slower than the dense product itself.  Here the
+// dense product runs on the tensor cores, and the 5.7 GB volume is never written: one CTA per SM walks work items
+// (frame, 128 queries); per level and per tile of 256 positions each of two consumer warpgroups (64 queries) issues
+// wgmma M=64 x N=256 x K=128 (8 instructions of K=16) from shared memory into registers and keeps only the (2r+2)^2
+// footprint values each query needs, in a shared-memory footprint table; after a level's last tile the same warps
+// interpolate the (2r+1)^2 taps and write them.  While one warpgroup extracts, the other one's MMAs run.
 //   operands: K-major, 64-byte swizzle (k-blocks of 32 fp16 channels), stored in global memory as ready-made tile
 //   images -- B (feature positions) once per CorrBlock, A (targets) once per call -- so the producer warp moves a whole
-//   256 x 128 operand tile with ONE 64 KB bulk copy (cp.async.bulk -> UBLKCP), no tensor map.
+//   256 x 128 operand tile with ONE 64 KB bulk copy (cp.async.bulk), no tensor map.
 // grid_sample semantics kept: align_corners=True, padding "zeros" (taps outside the map read 0), tap order
 // out[a*(2r+1)+b] at x = cx + (a-r), y = cy + (b-r).  Maps whose width is a power of two (128 -> 8 at C4).
 #include <cuda_fp16.h>
@@ -24,14 +22,14 @@ namespace vgg {
 
 namespace {
 
-constexpr int CT_M = 128;                 // queries per work item (TMEM lanes)
-constexpr int CT_N = 256;                 // positions per tile (TMEM columns)
+constexpr int CT_M = 128;                 // queries per work item (two consumer warpgroups of 64)
+constexpr int CT_N = 256;                 // positions per tile
 constexpr int CT_C = 128;                 // channels
 constexpr int CT_KB = 4;                  // k-blocks of 32 channels (64 bytes)
 constexpr int CT_A_BYTES = CT_M * CT_C * 2;          // 32 KB
 constexpr int CT_B_BYTES = CT_N * CT_C * 2;          // 64 KB
 constexpr int CT_STAGES = 2;
-constexpr int CT_THREADS = 320;           // warp 0 producer, warp 1 MMA, warps 2..9 epilogue (TMEM quarter = warp & 3, two per quarter)
+constexpr int CT_THREADS = 384;           // warpgroup 0 producer, warpgroups 1..2 MMA + footprint extraction (64 queries each)
 constexpr int CT_FB_LD = 101;             // footprint table row stride (floats): 10*10 (+1: conflict-free per-query rows)
 constexpr size_t CT_SMEM = 1024 + CT_A_BYTES + (size_t)CT_STAGES * CT_B_BYTES + (size_t)CT_M * CT_FB_LD * 4 + 256;
 
@@ -41,41 +39,47 @@ struct CtLevels {
   size_t img_stride;                      // bytes of tile images per image (all levels)
 };
 
-__device__ __forceinline__ void tcf_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcf_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ uint64_t desc_sw64(uint32_t saddr) {
-  // K-major, 64-byte swizzle, 8-row atoms 512 B apart, sm_100 descriptor version (as csrc/syrk_i8.cu)
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)(512 >> 4) << 32) | (1ull << 46) | (4ull << 61);
-}
-// D = f32, A = B = f16, both K-major, N = 256, M = 128
-constexpr uint32_t CT_IDESC = (1u << 4) | (0u << 7) | (0u << 10) | ((256u >> 3) << 17) | ((128u >> 4) << 24);
-
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(CT_IDESC), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_to(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 __device__ __forceinline__ void mbar_arrive1(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+__device__ __forceinline__ void wg_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// d[64 x 256] (+)= A[64 x 16] * B[256 x 16]^T, f16 x f16 -> f32, both operands K-major in shared memory; accumulate = 0
+// overwrites d.  Fragment of thread (warp w of the warpgroup, lane l): d[j] is row 16 w + l / 4 + 8 ((j >> 1) & 1), column
+// 8 (j >> 2) + 2 (l & 3) + (j & 1).
+__device__ __forceinline__ void wgmma_f16(float (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,"
-      "%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-        "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21,"
+      "%22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41,"
+      "%42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61,"
+      "%62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81,"
+      "%82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100,"
+      "%101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116,"
+      "%117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]),
+        "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]),
+        "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]),
+        "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]),
+        "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]),
+        "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]),
+        "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]),
+        "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]),
+        "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(accumulate)
+      : "memory");
 }
 
 // byte offset of (row r, channel c) inside a k-block tile image of `rows` x 64 B (64-byte swizzle, Swizzle<2,4,3>)
@@ -146,36 +150,24 @@ __global__ void __launch_bounds__(CT_THREADS, 1)
   uint64_t* a_empty = bars + 1;       // 1
   uint64_t* b_full = bars + 2;        // [2]
   uint64_t* b_empty = bars + 4;       // [2]
-  uint64_t* t_full = bars + 6;        // [2]
-  uint64_t* t_empty = bars + 8;       // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 10);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
   if (threadIdx.x == 0) {
     mbar_init(a_full, 1);
-    mbar_init(a_empty, 1);
+    mbar_init(a_empty, 8);
     for (int s = 0; s < CT_STAGES; ++s) {
       mbar_init(&b_full[s], 1);
-      mbar_init(&b_empty[s], 1);
-      mbar_init(&t_full[s], 1);
-      mbar_init(&t_empty[s], 8);
+      mbar_init(&b_empty[s], 8);      // one arrive per consumer warp
     }
     mbar_fence_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcf_before();
   __syncthreads();
-  tcf_after();
-  const uint32_t tmem_base = *tmem_ptr;
   const int nitems = BS * mtiles;
-  int tiles_per_item = 0;
-  for (int l = 0; l < L; ++l) tiles_per_item += lv.ntiles[l];
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===== producer: one bulk copy per operand tile =====
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");     // registers go to the consumers' accumulators
+    if (threadIdx.x == 0) {
       int stage = 0, phase = 0, item_no = 0;
       for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++item_no) {
         const int img = item / mtiles;
@@ -193,124 +185,96 @@ __global__ void __launch_bounds__(CT_THREADS, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      int stage = 0, phase = 0, item_no = 0;
-      uint32_t tile_no = 0;
-      for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++item_no) {
-        mbar_wait(a_full, (uint32_t)(item_no & 1));
-        tcf_after();
-        const uint32_t a_addr = smem_u32(a_sm);
-        for (int t = 0; t < tiles_per_item; ++t, ++tile_no) {
-          const uint32_t buf = tile_no & 1u;
-          mbar_wait(&t_empty[buf], (uint32_t)(((tile_no >> 1) & 1u) ^ 1u));
-          mbar_wait(&b_full[stage], (uint32_t)phase);
-          tcf_after();
-          const uint32_t b_addr = smem_u32(b_sm + (size_t)stage * CT_B_BYTES);
-#pragma unroll
-          for (int kb = 0; kb < CT_KB; ++kb)
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks)
-              umma_f16(tmem_base + buf * CT_N, desc_sw64(a_addr + kb * (CT_M * 64) + ks * 32),
-                       desc_sw64(b_addr + kb * (CT_N * 64) + ks * 32), (kb | ks) ? 1u : 0u);
-          umma_commit_to(&b_empty[stage]);       // the stage may be refilled once these MMAs have read it
-          umma_commit_to(&t_full[buf]);          // ... and the accumulator is complete
-          if (++stage == CT_STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_to(a_empty);                 // all MMAs of the item have consumed A
-      }
-    }
-  } else {
-    // ===== epilogue: thread = query row = TMEM lane; two warps per lane quarter (quarter = warp & 3), warp `sub` of a
-    //       pair drains the 32-column chunks with (chunk & 1) == sub; the pair meets on a named barrier per level =====
-    const int quarter = warp & 3, sub = (warp - 2) >> 2;
-    const int row = quarter * 32 + lane;                       // 0..127
-    float* myfb = fb + row * CT_FB_LD;
-    const float inv_sqrt_c = rsqrtf((float)CT_C);
-    uint32_t tile_no = 0;
-    for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
-      const int img = item / mtiles, m = item % mtiles;
-      const int n = m * CT_M + row;
-      float cx0 = 0.f, cy0 = 0.f;
-      if (n < N) {
-        cx0 = coords[((size_t)img * N + n) * 2];
-        cy0 = coords[((size_t)img * N + n) * 2 + 1];
-      }
-      for (int l = 0; l < L; ++l) {
-        const int W = lv.W[l], logW = lv.logW[l];
-        const float scale = 1.0f / (float)(1 << l);
-        const float cx = cx0 * scale, cy = cy0 * scale;
-        const float fxf = floorf(cx), fyf = floorf(cy);
-        const int x0 = (int)fxf - R, y0 = (int)fyf - R;        // footprint origin
-        for (int i = sub; i < FP * FP; i += 2) myfb[i] = 0.f;
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");       // table zeroed by both warps of the pair
-        for (int t = 0; t < lv.ntiles[l]; ++t, ++tile_no) {
-          const uint32_t buf = tile_no & 1u;
-          mbar_wait(&t_full[buf], (uint32_t)((tile_no >> 1) & 1u));
-          tcf_after();
-#pragma unroll 1
-          for (int ch = sub; ch < CT_N / 32; ch += 2) {
-            const int p0 = t * CT_N + ch * 32;
-            bool need;
-            int dy = 0, xc = 0;
-            if (W >= 32) {
-              dy = (p0 >> logW) - y0;
-              xc = p0 & (W - 1);
-              need = (unsigned)dy < (unsigned)FP && xc + 31 >= x0 && xc < x0 + FP;
-            } else {
-              const int ya = p0 >> logW, yb = (p0 + 31) >> logW;
-              need = yb >= y0 && ya < y0 + FP;
-            }
-            if (!__any_sync(0xffffffffu, need)) continue;
-            uint32_t v[32];
-            tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + buf * CT_N + ch * 32, v);
-            if (need) {
-              if (W >= 32) {
-                float* dstrow = myfb + dy * FP - x0 + xc;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                  const int dx = xc + j - x0;
-                  if ((unsigned)dx < (unsigned)FP) dstrow[j] = __uint_as_float(v[j]) * inv_sqrt_c;
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                  const int p = p0 + j;
-                  const int ddy = (p >> logW) - y0, dx = (p & (W - 1)) - x0;
-                  if ((unsigned)ddy < (unsigned)FP && (unsigned)dx < (unsigned)FP)
-                    myfb[ddy * FP + dx] = __uint_as_float(v[j]) * inv_sqrt_c;
-                }
-              }
-            }
-          }
-          tcf_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive1(&t_empty[buf]);
-        }
-        // ---- interpolation of the K*K taps: the pair shares its 32 queries (even / odd), one query at a time so that
-        //      the stores of a query are contiguous
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");       // both halves of every footprint are in
-        for (int qq = sub; qq < 32; qq += 2) {
-          const int nq = m * CT_M + quarter * 32 + qq;
-          if (nq >= N) break;
-          const float qcx = __shfl_sync(0xffffffffu, cx, qq), qcy = __shfl_sync(0xffffffffu, cy, qq);
-          const float wx = qcx - floorf(qcx), wy = qcy - floorf(qcy);
-          const float* f = fb + (quarter * 32 + qq) * CT_FB_LD;
-          float* orow = out + ((size_t)img * N + nq) * (size_t)(L * K * K) + (size_t)l * K * K;
-          for (int o = lane; o < K * K; o += 32) {
-            const int a = o / K, b = o % K;
-            const float d00 = f[b * FP + a], d01 = f[b * FP + a + 1], d10 = f[(b + 1) * FP + a], d11 = f[(b + 1) * FP + a + 1];
-            orow[o] = d00 * (1.f - wx) * (1.f - wy) + d01 * wx * (1.f - wy) + d10 * (1.f - wx) * wy + d11 * wx * wy;
-          }
-        }
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + quarter) : "memory");       // tables are re-zeroed next level
-      }
-    }
+    return;
   }
-  tcf_before();
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
+
+  // ===== consumers: warpgroup half (= wg - 1) owns queries 64 half .. 64 half + 63 of the item; a thread holds the
+  //       accumulators of queries q0 and q0 + 8 =====
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int half = wg - 1, wq = warp & 3;
+  const int q0 = half * 64 + wq * 16 + (lane >> 2);
+  const int cbase = 2 * (lane & 3);
+  const float inv_sqrt_c = rsqrtf((float)CT_C);
+  float acc[128];
+  int stage = 0, phase = 0, item_no = 0;
+  for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++item_no) {
+    const int img = item / mtiles, m = item % mtiles;
+    float cx0[2] = {0.f, 0.f}, cy0[2] = {0.f, 0.f};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int n = m * CT_M + q0 + 8 * h;
+      if (n < N) {
+        cx0[h] = coords[((size_t)img * N + n) * 2];
+        cy0[h] = coords[((size_t)img * N + n) * 2 + 1];
+      }
+    }
+    mbar_wait(a_full, (uint32_t)(item_no & 1));
+    const uint32_t a_addr = smem_u32(a_sm) + (uint32_t)half * 64u * 64u;   // 64 rows = 8 swizzle atoms
+    for (int l = 0; l < L; ++l) {
+      const int W = lv.W[l], logW = lv.logW[l];
+      const float scale = 1.0f / (float)(1 << l);
+      int x0[2], y0[2];                                                   // footprint origins of the two queries
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        x0[h] = (int)floorf(cx0[h] * scale) - R;
+        y0[h] = (int)floorf(cy0[h] * scale) - R;
+      }
+      for (int i = (threadIdx.x & 127); i < 64 * FP * FP; i += 128)
+        fb[(half * 64 + i / (FP * FP)) * CT_FB_LD + i % (FP * FP)] = 0.f;
+      wg_bar(1 + half);                                                   // table zeroed by the whole warpgroup
+      for (int t = 0; t < lv.ntiles[l]; ++t) {
+        mbar_wait(&b_full[stage], (uint32_t)phase);
+        const uint32_t b_addr = smem_u32(b_sm + (size_t)stage * CT_B_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int kb = 0; kb < CT_KB; ++kb)
+#pragma unroll
+          for (int ks = 0; ks < 2; ++ks)
+            wgmma_f16(acc, wgmma_desc_sw64(a_addr + kb * (CT_M * 64) + ks * 32), wgmma_desc_sw64(b_addr + kb * (CT_N * 64) + ks * 32),
+                      (kb | ks) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait_all();
+        __syncwarp();
+        if (lane == 0) mbar_arrive1(&b_empty[stage]);                    // the stage may be refilled
+        if (++stage == CT_STAGES) { stage = 0; phase ^= 1; }
+        // keep the footprint values: position p = t * 256 + column
+        const int p_lo = t * CT_N, p_hi = p_lo + CT_N - 1;
+        bool need[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          need[h] = (p_hi >> logW) >= y0[h] && (p_lo >> logW) < y0[h] + FP;
+        if (!__any_sync(0xffffffffu, need[0] || need[1])) continue;
+#pragma unroll
+        for (int j = 0; j < 128; ++j) {
+          const int h = (j >> 1) & 1;
+          const int p = p_lo + 8 * (j >> 2) + cbase + (j & 1);
+          const int dy = (p >> logW) - y0[h], dx = (p & (W - 1)) - x0[h];
+          if ((unsigned)dy < (unsigned)FP && (unsigned)dx < (unsigned)FP)
+            fb[(q0 + 8 * h) * CT_FB_LD + dy * FP + dx] = acc[j] * inv_sqrt_c;
+        }
+      }
+      // ---- interpolation of the K*K taps: warp wq takes its 16 queries one at a time, lanes across the taps, so that
+      //      the stores of a query are contiguous
+      wg_bar(1 + half);                                                   // every footprint of the warpgroup is in
+      for (int qq = 0; qq < 16; ++qq) {
+        const int ql = half * 64 + wq * 16 + qq;
+        const int nq = m * CT_M + ql;
+        if (nq >= N) break;
+        const float qcx = coords[((size_t)img * N + nq) * 2] * scale, qcy = coords[((size_t)img * N + nq) * 2 + 1] * scale;
+        const float wx = qcx - floorf(qcx), wy = qcy - floorf(qcy);
+        const float* f = fb + ql * CT_FB_LD;
+        float* orow = out + ((size_t)img * N + nq) * (size_t)(L * K * K) + (size_t)l * K * K;
+        for (int o = lane; o < K * K; o += 32) {
+          const int a = o / K, b = o % K;
+          const float d00 = f[b * FP + a], d01 = f[b * FP + a + 1], d10 = f[(b + 1) * FP + a], d11 = f[(b + 1) * FP + a + 1];
+          orow[o] = d00 * (1.f - wx) * (1.f - wy) + d01 * wx * (1.f - wy) + d10 * (1.f - wx) * wy + d11 * wx * wy;
+        }
+      }
+      wg_bar(1 + half);                                                   // tables are re-zeroed next level
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive1(a_empty);                                // all MMAs of the item have consumed A
+  }
 }
 
 int ct_levels(int H, int W, int L, CtLevels* lv) {

@@ -4,12 +4,6 @@
 #ifdef __cplusplus
 extern "C" {
 #endif
-/* Tensor-pipe probe used for the SYRK's roofline: cycles per back-to-back tcgen05.mma.kind::i8 (M=128, K=32); mode
- * bit0 selects N=256 (else 128), mode>>1 the shared-memory layout (0 = 64 B swizzle, 1 = 128 B swizzle, 2 = none).
- * out_cycles is a host pointer. */
-int vgg_syrk_ozaki_mma_rate(int iters, int mode, double* out_cycles, void* stream);
-/* Cluster hardware-rule probe used while developing the CTA-pair SYRK (bounded, cannot hang): out_host[0..2] int. */
-int vgg_probe_remote_mbarrier(int* out_host, void* stream);
 /* Kernel-only timing of ba_blocks_kernel: while enabled, every build_blocks call records a CUDA event pair on its stream
  * directly around the kernel launch (the accumulator memsets before it are outside); last_ms waits for the second event
  * and returns the elapsed milliseconds of the most recent launch. */

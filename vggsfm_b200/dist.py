@@ -3,7 +3,7 @@
 The reference has no distributed code (SURVEY.md section 2.2); this is new.  One process per GPU:
 every rank holds all S cameras and a contiguous slice of the N tracks; point blocks, coupling blocks
 and the Schur products are local; the reduced system [D x Dpad | rhs | diag | g] is summed across
-ranks once per LM iteration (NCCL over NVLink 5 / NVSwitch), after which every rank factors the same
+ranks once per LM iteration (NCCL over NVLink / NVSwitch), after which every rank factors the same
 small system redundantly and back-substitutes its own points.  A second, tiny all-reduce carries the
 candidate cost and gradient so all ranks take the same accept/reject decision.
 """
@@ -30,7 +30,7 @@ def shard_range(N: int, rank: int, world: int, multiple: int = 16):
 
 class FabricBuffer:
     """Reduced-system buffer in symmetric (peer-mapped, NVSwitch-multicast) memory for the fused reduction
-    (include/vggsfm_b200.h: vgg_ba_fabric).  v2 (default): the tcgen05 SYRK's epilogue REDs every 128-row block of the
+    (include/vggsfm_b200.h: vgg_ba_fabric).  v2 (default): the tensor-core SYRK's epilogue REDs every 128-row block of the
     lower triangle into its owner's copy over NVLink (reduce-scatter), every rank then pulls the blocks it does not own
     (csrc/fabric.cu), and the barriers / small all-reduces of the LM loop are kernels on the same allocation -- no NCCL
     call and no host callback inside the loop.  v1 (``VGG_FABRIC=1``): multimem.red into every copy + barriers and

@@ -1,4 +1,4 @@
-"""``pycolmap``-shaped entry points on the B200 kernels -- the reference's own third-party seam.
+"""``pycolmap``-shaped entry points on the CUDA kernels -- the reference's own third-party seam.
 
 Every BA / pose call of the reference is a call into ``pycolmap`` (SURVEY section 0.2): ``pycolmap.bundle_adjustment``
 (vggsfm/utils/triangulation.py:213,1050,1142; runners/video_runner.py:508), ``pycolmap.pose_refinement``

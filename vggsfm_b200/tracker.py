@@ -4,7 +4,7 @@
 and ``refine_track`` / ``compute_score_fn`` are vggsfm/models/track_modules/refine_track.py:24-187 / :190-294, with the
 reference's arguments and return values.  The learned modules stay the caller's (``predictor.updateformer``, ``.norm``,
 ``.ffeat_updater``, ``.vis_predictor``, ``fine_fnet``: stock PyTorch layers holding the reference's checkpoints); what
-moves onto the B200 kernels is everything between them:
+moves onto the CUDA kernels is everything between them:
 
   * correlation + local sampling: ``vggsfm_b200.corr.CorrBlock`` / ``EfficientCorrBlock`` (csrc/corr.cu, fused; the
     [B,S,N,H,W] volume of blocks.py:396-416 is never built);

@@ -1,4 +1,4 @@
-"""``Triangulator`` -- the reference's triangulation + bundle-adjustment stage on the B200 kernels.
+"""``Triangulator`` -- the reference's triangulation + bundle-adjustment stage on the CUDA kernels.
 
 Drop-in for ``vggsfm.models.triangulator.Triangulator`` (hydra ``cfg.MODEL.TRIANGULAE._target_``,
 cfgs/demo.yaml:105-106): same ``forward`` arguments and the same 9-tuple back
