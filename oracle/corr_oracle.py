@@ -6,7 +6,13 @@ pyramid by repeated avg_pool2d(2,2) (:352-361), full correlation volume per leve
 (:363-394 via models/utils.py:347-412); and of EfficientCorrBlock.sample (:433-471, border padding).
 The bilinear gather is written out by hand (no grid_sample) so it is an independent statement.
 PINNED against the reference through tests/golden/corr_*.npz (tools/make_golden_corr.py).
+
+corr_reference is the float64 statement the CUDA kernels are checked against: it takes the pyramid levels and targets
+already rounded to the kernel's precision (kernel_pyramid rebuilds the kernels' pyramid bit for bit), and returns with
+every output the same bilinear combination of sum_c |t_c f_c| / sqrt(C), the scale of the kernel's rounding error.
 """
+import math
+
 import torch
 import torch.nn.functional as F
 
@@ -23,8 +29,8 @@ def build_pyramid(fmaps, num_levels):
 
 
 def _bilinear_gather(vol, x, y, border):
-    """vol [Q,H,W]; x,y [Q,T] pixel coords -> [Q,T]."""
-    Q, H, W = vol.shape
+    """vol [Q,H,W,...]; x,y [Q,T] pixel coords -> [Q,T,...]."""
+    Q, H, W = vol.shape[:3]
     if border:
         x = x.clamp(0, W - 1)
         y = y.clamp(0, H - 1)
@@ -34,8 +40,8 @@ def _bilinear_gather(vol, x, y, border):
     wy = y - y0
     x0 = x0.long()
     y0 = y0.long()
-    out = torch.zeros_like(x)
-    qi = torch.arange(Q)[:, None].expand_as(x0)
+    out = torch.zeros(x.shape + vol.shape[3:], dtype=vol.dtype, device=vol.device)
+    qi = torch.arange(Q, device=vol.device)[:, None].expand_as(x0)
     for dy, wyv in ((0, 1 - wy), (1, wy)):
         for dx, wxv in ((0, 1 - wx), (1, wx)):
             xi = x0 + dx
@@ -47,7 +53,8 @@ def _bilinear_gather(vol, x, y, border):
             else:
                 inside = (xi >= 0) & (xi < W) & (yi >= 0) & (yi < H)
             v = vol[qi, yi.clamp(0, H - 1), xi.clamp(0, W - 1)]
-            out = out + torch.where(inside, v, torch.zeros_like(v)) * wxv * wyv
+            w = torch.where(inside, wxv * wyv, torch.zeros_like(wxv)).to(vol.dtype)
+            out = out + v * w.reshape(w.shape + (1,) * (vol.dim() - 3))
     return out
 
 
@@ -107,3 +114,56 @@ class TorchCorrBlock:
             s = F.grid_sample(v.reshape(B * S * N, 1, H, W), g.to(v.dtype), align_corners=True, padding_mode=self.padding_mode)
             out.append(s.reshape(B, S, N, -1))
         return torch.cat(out, dim=-1).contiguous()
+
+
+def kernel_pyramid(fmaps, num_levels, half=True):
+    """The pyramid csrc/corr.cu builds, bit for bit: float32 levels pooled as ((a + b) + c) + d then * 0.25 from the
+    float32 level above (odd sizes floored), each rounded to float16 round-to-nearest-even when `half`.
+    fmaps [B,S,C,H,W] (any device) -> list of [B,S,C,h,w] float32 (half-valued when `half`)."""
+    f = fmaps.float()
+    levels = [f.half().float() if half else f]
+    for _ in range(num_levels - 1):
+        h, w = f.shape[-2] // 2, f.shape[-1] // 2
+        a, b = f[..., 0:2 * h:2, 0:2 * w:2], f[..., 0:2 * h:2, 1:2 * w:2]
+        c, d = f[..., 1:2 * h:2, 0:2 * w:2], f[..., 1:2 * h:2, 1:2 * w:2]
+        f = (((a + b) + c) + d) * 0.25
+        levels.append(f.half().float() if half else f)
+    return levels
+
+
+def corr_reference(levels, targets, coords, radius, border=False, frames=4):
+    """float64 correlation + sampling: levels [B,S,C,h,w] per level, targets [B,S,N,C] and coords [B,S,N,2] float32, all
+    on one device.  Returns (out, bound) [B,S,N,L*(2r+1)^2] float64, bound = the bilinear combination of
+    sum_c |t_c f_c| / sqrt(C).  Tap positions as the kernels form them: for zeros padding floor(c) + d plus the
+    float32 fraction c - floor(c), once per query (c = coords / 2^l); for border padding c + d rounded to float32,
+    then clamped."""
+    B, S, N, C = targets.shape
+    r = radius
+    K = 2 * r + 1
+    dev = targets.device
+    out = torch.empty(B, S, N, len(levels) * K * K, dtype=torch.float64, device=dev)
+    bound = torch.empty_like(out)
+    d = torch.arange(-r, r + 1, dtype=torch.float64, device=dev)
+    for s0 in range(0, S, frames):
+        s1 = min(S, s0 + frames)
+        t = targets[:, s0:s1].double()
+        for i, fm in enumerate(levels):
+            H, W = fm.shape[-2:]
+            f = fm[:, s0:s1].double()
+            vol = torch.stack([torch.einsum("bsnc,bschw->bsnhw", t, f), torch.einsum("bsnc,bschw->bsnhw", t.abs(), f.abs())],
+                              dim=-1) / math.sqrt(C)
+            c = coords[:, s0:s1].float().reshape(-1, 2) / 2 ** i
+            if border:
+                x = (c[:, 0:1, None] + d.float()[None, :, None]).double()
+                y = (c[:, 1:2, None] + d.float()[None, None, :]).double()
+            else:
+                fl = torch.floor(c)
+                pos = fl.double() + (c - fl).double()          # the float32 fraction: inexact for c in (-0.5, 0)
+                x = pos[:, 0:1, None] + d[None, :, None]
+                y = pos[:, 1:2, None] + d[None, None, :]
+            x = x.expand(-1, K, K).reshape(-1, K * K)
+            y = y.expand(-1, K, K).reshape(-1, K * K)
+            g = _bilinear_gather(vol.reshape(-1, H, W, 2), x, y, border).reshape(B, s1 - s0, N, K * K, 2)
+            out[:, s0:s1, :, i * K * K:(i + 1) * K * K] = g[..., 0]
+            bound[:, s0:s1, :, i * K * K:(i + 1) * K * K] = g[..., 1]
+    return out, bound

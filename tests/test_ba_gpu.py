@@ -56,14 +56,21 @@ def test_blocks_match_oracle(cuda_dev, S, N, cam, mode):
         assert relerr(H_ss, ref["H_ss"]) < tol
 
 
-@pytest.mark.parametrize("S,N,cam,mode", CASES[:4])
+@pytest.mark.parametrize("S,N,cam,mode", CASES[:4] + [
+    (50, 2048, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME),     # D = 350: three 128-column tiles
+    (400, 4096, "SIMPLE_RADIAL", bo.INTR_SHARED),        # C3: D = 2402, 19 row blocks
+])
 def test_schur_matches_oracle(cuda_dev, S, N, cam, mode):
+    """Sraw = H_cc - Z Z^T through z_build (which also produces the SYRK's column maxima) and the Ozaki SYRK, per entry
+    within 1e-12 sqrt(S_ii S_jj) -- the accuracy the Cholesky of the reduced system needs (largest observed on an
+    H100 80GB HBM3: 7.9e-14, at C3)."""
     import torch
     from vggsfm_b200 import bundle_adjustment as ba
     c = ba_case(S, N, cam, mode, seed=3 * S + N)
     dc, ns = bo.dims(c["model"], mode)
     D = S * dc + ns
-    blk = bo.build_blocks(c["poses"], c["intr"], c["points"], c["uv"], c["mask"], c["model"], mode)
+    blocks = bo.build_blocks_c if bo._load_c() is not None else bo.build_blocks
+    blk = blocks(c["poses"], c["intr"], c["points"], c["uv"], c["mask"], c["model"], mode)
     Hc, gc = bo._assemble_camera_system(blk, S, dc, ns)
     radius = 37.0
     sc_p = 1.0 / (1.0 + np.sqrt(np.einsum("nii->ni", blk["H_pp"])))
@@ -86,8 +93,11 @@ def test_schur_matches_oracle(cuda_dev, S, N, cam, mode):
     torch.cuda.synchronize()
     Sraw = Sraw.cpu().numpy()[:, :D]
     low = np.tril_indices(D)
-    scale = np.abs(S_ref).max()
-    assert np.abs(Sraw[low] - S_ref[low]).max() < 1e-9 * scale
+    d = np.sqrt(np.diag(S_ref))
+    assert (d > 0).all()
+    ratio = (np.abs(Sraw - S_ref) / np.outer(d, d))[low].max()
+    print(f"schur S={S} N={N}: max |dS_ij| / sqrt(S_ii S_jj) = {ratio:.3g}")
+    assert ratio < 1e-12
     assert np.abs(rhs.cpu().numpy() - rhs_ref).max() < 1e-9 * np.abs(rhs_ref).max()
 
 
