@@ -10,7 +10,7 @@ LIB := vggsfm_b200/libvggsfm_b200.so
 
 all: $(LIB) oracle
 
-$(BUILD)/%.o: $(CSRC)/%.cu $(CSRC)/common.cuh include/vggsfm_b200.h
+$(BUILD)/%.o: $(CSRC)/%.cu $(CSRC)/common.cuh $(wildcard $(CSRC)/*.h) include/vggsfm_b200.h
 	@mkdir -p $(BUILD)
 	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> $(BUILD)/$*.ptxas.log || (cat $(BUILD)/$*.ptxas.log; exit 1)
 

@@ -140,10 +140,11 @@ int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double*
  * INT_MAX if the in-kernel hand-off between CTAs stalled (bounded spin; never seen, reported instead of hanging). */
 int vgg_cholesky_lower(int n, int lda, double* A, void* workspace, size_t ws_bytes, int* info_host, void* stream);
 
-/* The same SYRK step on the tensor cores (csrc/syrk_i8.cu): Cmat[Dpad,Dpad] -= Zt^T Zt for Zt double [Kpad,Dpad]
+/* The Schur SYRK step on the INT8 tensor cores (csrc/syrk_i8.cu): Cmat[Dpad,Dpad] -= Zt^T Zt for Zt double [Kpad,Dpad]
  * (Dpad a multiple of 128), FP64-equivalent through `slices` (3..7; 7 = 54 fractional bits) int8
  * Ozaki slices on wgmma s8 with exact int32 accumulation in registers.  The row-major LOWER triangle is written.
- * Selected inside vgg_ba_solve by VGG_SYRK=ozaki[:slices]; exposed for the parity tests and profiling. */
+ * vgg_ba_solve runs the FP64 tensor-core SYRK of csrc/ba_schur.cu instead (faster on H100); this one is kept for the
+ * parity tests and profiling. */
 int vgg_syrk_ozaki_workspace_bytes(int Kpad, int Dpad, int slices, size_t* bytes);
 int vgg_syrk_ozaki(int Kpad, int Dpad, const double* Zt, double* Cmat, int slices, void* workspace, size_t ws_bytes,
                    void* stream);

@@ -1,5 +1,5 @@
 """CUDA-event micro-benchmarks for A/B runs (env switches are read once per process):
-   python tools/microbench.py chol | ba | blocks [N] | pose [S N] | pipeline [S N]"""
+   python tools/microbench.py chol | ba | blocks [N] | pose [S N] | pipeline [S N] | syrk [S N]"""
 import ctypes
 import os
 import sys
@@ -111,6 +111,51 @@ if mode == "trsv":
         hand = (see[b - 1] - pub[b]) / 1e3 if b > 0 else float("nan")
         print(f"  {b:5d}  {(see[b] - t0) / 1e3:10.2f}  {(pub[b] - t0) / 1e3:12.2f}  {(pub[b] - see[b]) / 1e3:10.2f}  {hand:10.2f}")
     print(f"  total chain {(pub[0] - t0) / 1e3:.1f} us after the last block row published")
+    sys.exit(0)
+
+if mode == "syrk":
+    # The Schur SYRK at the C3 shape (default 400 x 4096, SIMPLE_RADIAL, shared camera: D = 6 S + 2): the FP64 tensor-core
+    # kernel of the LM loop (vgg_dev_syrk_f64) and the INT8 Ozaki call (vgg_syrk_ozaki, slicing included), alternated in
+    # rounds of 10 calls each.  FP64 TFLOP/s counts the 128 x 128 tiles on and below the diagonal; the peak is
+    # 132 SMs x 256 flop/clk/SM (DMMA) x the SM clock sampled by NVML during the timed rounds.
+    import ctypes
+    sys.path.insert(0, ROOT)
+    from bench import ClockSampler                             # noqa: E402
+    S = int(sys.argv[2]) if len(sys.argv) > 2 else 400
+    N = int(sys.argv[3]) if len(sys.argv) > 3 else 4096
+    D = 6 * S + 2
+    Dpad, Kpad = (D + 2 + 127) // 128 * 128, (3 * N + 15) // 16 * 16
+    L = _lib.lib()
+    g = torch.Generator(device=dev).manual_seed(0)
+    Zt = torch.randn(Kpad, Dpad, dtype=torch.float64, device=dev, generator=g)
+    Zt[:, D:] = 0
+    C = torch.zeros(Dpad, Dpad, dtype=torch.float64, device=dev)
+    nb = ctypes.c_size_t()
+    _lib.check(L.vgg_syrk_ozaki_workspace_bytes(Kpad, Dpad, 7, ctypes.byref(nb)), "ws")
+    ws = torch.empty(nb.value, dtype=torch.uint8, device=dev)
+    st = torch.cuda.current_stream().cuda_stream
+    calls = {"f64": lambda: _lib.check(L.vgg_dev_syrk_f64(Kpad, Dpad, Zt.data_ptr(), C.data_ptr(), st), "syrk_f64"),
+             "ozaki7": lambda: _lib.check(L.vgg_syrk_ozaki(Kpad, Dpad, Zt.data_ptr(), C.data_ptr(), 7, ws.data_ptr(), ws.numel(), st),
+                                          "ozaki")}
+    cs = ClockSampler()
+    cs.prepare()
+    cs.start()
+    times = {k: [] for k in calls}
+    for rnd in range(6):
+        for k, fn in calls.items():
+            t_ms = timeit(fn, reps=10, warm=2 if rnd == 0 else 0)
+            if rnd > 0:
+                times[k].append(t_ms)
+    clk = cs.stop()
+    nbk = Dpad // 128
+    flop = 2.0 * Kpad * 128 * 128 * nbk * (nbk + 1) / 2
+    mhz = clk.get("sm_mhz") or float("nan")
+    peak = 132 * 256 * mhz * 1e6 / 1e12
+    for k, v in times.items():
+        ms = float(np.median(v))
+        print(f"[{tag}] syrk {k} Kpad={Kpad} Dpad={Dpad}: {ms:.3f} ms/call (rounds {min(v):.3f}..{max(v):.3f})  "
+              f"{flop / ms / 1e9:.1f} FP64 TFLOP/s = {flop / ms / 1e9 / peak:.2f} of the DMMA peak {peak:.1f} at {mhz:.0f} MHz "
+              f"(throttle: {','.join(clk.get('reasons', [])) or 'none'})")
     sys.exit(0)
 
 if mode == "chol128":

@@ -26,7 +26,7 @@ EXPORTS = [
 
 
 # development probes (csrc/dev_probes.h): exported, not part of the public header
-DEV_EXPORTS = ["vgg_dev_blocks_timing", "vgg_dev_blocks_last_ms", "vgg_dev_chol128_probe", "vgg_dev_set_syrk_ranges", "vgg_dev_trsv_probe", "vgg_dev_set_chol_band"]
+DEV_EXPORTS = ["vgg_dev_blocks_timing", "vgg_dev_blocks_last_ms", "vgg_dev_chol128_probe", "vgg_dev_set_syrk_ranges", "vgg_dev_syrk_f64", "vgg_dev_trsv_probe", "vgg_dev_set_chol_band"]
 
 
 class BAProblem(ctypes.Structure):
@@ -143,6 +143,7 @@ def lib() -> ctypes.CDLL:
     L.vgg_dev_blocks_last_ms.argtypes = [ctypes.POINTER(cd)]
     L.vgg_dev_chol128_probe.argtypes = [ci, ci, vp, vp, vp]
     L.vgg_dev_set_syrk_ranges.argtypes = [vp, ci]
+    L.vgg_dev_syrk_f64.argtypes = [ci, ci, vp, vp, vp]
     L.vgg_dev_trsv_probe.argtypes = [ci, ci, vp, vp, vp, vp]
     L.vgg_dev_set_chol_band.argtypes = [vp, ci, ci]
     L.vgg_syrk_ozaki.argtypes = [ci, ci, vp, vp, ci, vp, cs, vp]

@@ -8,13 +8,16 @@
 //   assemble_hc     camera Hessian/gradient from the per-frame records into the dense reduced system
 //   z_build         Zt[3n+c][row] = (W[n][row][:] M_n)[c]   (k-major operand for the SYRK; W is track-major,
 //                   so this is a straight streaming pass), rhs[row] += Z[row] . q
-//   syrk            Sraw -= Zt^T Zt on the lower-triangular 128x128 tiles: FP64 FMA pipe, 8x8 register
-//                   tiles, cp.async double-buffered k-slabs, split-K with f64 RED epilogue
+//   syrk_f64        Sraw -= Zt^T Zt on the upper 128x128 tiles, mirrored into the lower triangle: FP64 tensor cores
+//                   (DMMA 16x8x16), bulk-copy/mbarrier ring, persistent over a k-split work list, f64 RED epilogue
 //   scale_damp      A = Dc Sraw Dc + diag(clamp(diag(Dc Hcc Dc)))/radius, constant parameters pinned
 //   cam_step / backsub_partial / point_step / cam_update   back-substitution and the candidate state
 #include <stddef.h>
-#include <stdlib.h>
+#include <algorithm>
+#include <vector>
 #include "common.cuh"
+#include "dev_probes.h"
+#include "syrk_work.h"
 
 namespace vgg {
 
@@ -168,8 +171,7 @@ constexpr int ZB_NT = 32;
 __global__ void __launch_bounds__(128) z_build_kernel(int D, int N, int Dpad, size_t pitch, const double* __restrict__ W,
                                                       const double* __restrict__ M, const double* __restrict__ q,
                                                       double* __restrict__ Zt, double* __restrict__ rhs,
-                                                      ptrdiff_t mc_off, unsigned long long* __restrict__ amax,
-                                                      const int* __restrict__ rb_range) {
+                                                      ptrdiff_t mc_off, const int* __restrict__ rb_range) {
   __shared__ double sm[ZB_NT][12];
   const int row = blockIdx.x * 128 + threadIdx.x;
   const int n0 = blockIdx.y * ZB_NT;
@@ -187,7 +189,6 @@ __global__ void __launch_bounds__(128) z_build_kernel(int D, int N, int Dpad, si
   __syncthreads();
   if (row >= D) return;
   double zq = 0.0;
-  double zmax = 0.0;                  // running max |z| of this row (NaN / Inf stick): the tensor-core SYRK's column scale
   const double* wp = W + ((size_t)n0 * pitch + row) * 3;
 #pragma unroll 4
   for (int t = 0; t < nt; ++t, wp += pitch * 3) {
@@ -201,222 +202,131 @@ __global__ void __launch_bounds__(128) z_build_kernel(int D, int N, int Dpad, si
     zo[Dpad] = z1;
     zo[2 * (size_t)Dpad] = z2;
     zq += z0 * m[9] + z1 * m[10] + z2 * m[11];
-    const double a0 = fabs(z0), a1 = fabs(z1), a2 = fabs(z2);
-    zmax = (a0 > zmax || a0 != a0) ? a0 : zmax;
-    zmax = (a1 > zmax || a1 != a1) ? a1 : zmax;
-    zmax = (a2 > zmax || a2 != a2) ? a2 : zmax;
-  }
-  if (amax) {
-    if (!(zmax <= 1.7976931348623157e308)) zmax = __longlong_as_double(0x7ff0000000000000LL);
-    if (zmax > 0.0) atomicMax(&amax[row], (unsigned long long)__double_as_longlong(zmax));
   }
   if (zq != 0.0) ar_add(&rhs[row], mc_off ? &rhs[row] + mc_off : nullptr, zq);
 }
 
 // ------------------------------------------------------------------------------------------------
-// SYRK on lower-triangular tiles: C[bi,bj] -= Zt[:, bi]^T Zt[:, bj]
-constexpr int SY_BM = 128, SY_BK = 16, SY_THREADS = 256, SY_STAGES = 3;
+// Schur SYRK on the FP64 tensor cores: Sraw -= Zt^T Zt with mma.sync.m16n8k16.f64 (SASS DMMA.16x8x16, the full-rate FP64
+// MMA of sm_90a; m8n8k4 issues at half of it).  Persistent, one CTA per SM, over a host-built list of (upper tile
+// bi <= bj, k range) items:
+//   warp 0      producer: one 1 KB bulk copy (cp.async.bulk) per k-row and operand into a ring of SF_STAGES stages of
+//               SF_BK k-rows, completing on the stage's mbarrier; Zt is read as z_build wrote it ([Kpad][Dpad]).  The
+//               rest of its warpgroup only hands its registers over (setmaxnreg)
+//   warps 4-11  2 x 4 warps of 64 x 32 outputs (4 x 4 MMA tiles, 64 accumulator doubles per lane), then syrk_red_upper
+// Diagonal tiles load one operand.  The row stride of SF_LDS = 132 doubles is 4 doubles (mod the 128-byte bank row), so
+// the four k-rows one fragment load touches fall into disjoint quarters of the banks.
+constexpr int SF_BM = 128, SF_BK = 16, SF_LDS = 132, SF_STAGES = 4, SF_MMA_WARPS = 8;
+constexpr int SF_THREADS = 128 + SF_MMA_WARPS * 32;
+constexpr int SF_STAGE_DOUBLES = 2 * SF_BK * SF_LDS;
+constexpr size_t SF_SMEM_BYTES = sizeof(double) * SF_STAGES * SF_STAGE_DOUBLES + sizeof(uint64_t) * 2 * SF_STAGES;
 
-__global__ void __launch_bounds__(SY_THREADS) syrk_kernel(int Kpad, int Dpad, int k_per_split,
-                                                          const double* __restrict__ Zt, double* __restrict__ Cmat,
-                                                          ptrdiff_t mc_off, int fill_upper) {
-  extern __shared__ __align__(16) double sy_smem[];
-  // tile decode: blockIdx.x -> (bi >= bj)
-  int t = blockIdx.x;
-  int bi = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-  while ((bi + 1) * (bi + 2) / 2 <= t) ++bi;
-  while (bi * (bi + 1) / 2 > t) --bi;
-  const int bj = t - bi * (bi + 1) / 2;
-  const bool diag = (bi == bj);
-  const int kbeg = blockIdx.y * k_per_split;
-  const int kend = min(Kpad, kbeg + k_per_split);
-  const int nslab = (kend - kbeg + SY_BK - 1) / SY_BK;
-  if (nslab <= 0) return;
+struct SyrkWork {
+  int bi, bj, kb0, kb1;        // upper tile (row block bi <= column block bj), k blocks of 64 rows [kb0, kb1)
+};
 
-  double* As = sy_smem;                                   // [STAGES][BK][BM]
-  double* Bs = sy_smem + SY_STAGES * SY_BK * SY_BM;       // [STAGES][BK][BM]
-  const int tid = threadIdx.x;
-  const int ty = tid >> 4, tx = tid & 15;
-
-  auto load_slab = [&](int slab, int stage) {
-    const int k0 = kbeg + slab * SY_BK;
-    // each operand slab: BK x BM doubles = 1024 x 16B chunks; 256 threads x 4
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int chunk = tid + i * SY_THREADS;          // 0..1023
-      const int kk = chunk >> 6;                       // 64 chunks of 16 B per k-row
-      const int cc = (chunk & 63) * 2;
-      const size_t grow = (size_t)(k0 + kk) * Dpad;
-      cp_async16(As + (stage * SY_BK + kk) * SY_BM + cc, Zt + grow + bi * SY_BM + cc);
-      if (!diag) cp_async16(Bs + (stage * SY_BK + kk) * SY_BM + cc, Zt + grow + bj * SY_BM + cc);
-    }
-    cp_async_commit();
-  };
-
-  double acc[8][8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[i][j] = 0.0;
-
-  // prologue
-#pragma unroll
-  for (int s = 0; s < SY_STAGES - 1; ++s) {
-    if (s < nslab) load_slab(s, s);
-    else cp_async_commit();
-  }
-  for (int slab = 0; slab < nslab; ++slab) {
-    cp_async_wait<SY_STAGES - 2>();
-    __syncthreads();
-    {
-      const int nxt = slab + SY_STAGES - 1;
-      if (nxt < nslab) load_slab(nxt, nxt % SY_STAGES);
-      else cp_async_commit();
-    }
-    const int stage = slab % SY_STAGES;
-    const double* as = As + stage * SY_BK * SY_BM;
-    const double* bs = diag ? as : (Bs + stage * SY_BK * SY_BM);
-#pragma unroll
-    for (int kk = 0; kk < SY_BK; ++kk) {
-      double a[8], b[8];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const double2 av = *reinterpret_cast<const double2*>(as + kk * SY_BM + ty * 2 + 32 * i);
-        a[2 * i] = av.x; a[2 * i + 1] = av.y;
-        const double2 bv = *reinterpret_cast<const double2*>(bs + kk * SY_BM + tx * 2 + 32 * i);
-        b[2 * i] = bv.x; b[2 * i + 1] = bv.y;
-      }
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[i][j] = fma(a[i], b[j], acc[i][j]);
-    }
-  }
-  cp_async_wait<0>();
-  // epilogue: C -= acc  (f64 RED; split-K partials and H_cc already in C)
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int r = bi * SY_BM + ty * 2 + (i & 1) + 32 * (i >> 1);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int c = bj * SY_BM + tx * 2 + (j & 1) + 32 * (j >> 1);
-      if (acc[i][j] != 0.0) {
-        // row-major LOWER triangle (what csrc/chol.cu factors; in fabric mode one multimem op per element); the mirror
-        // only for the library factorisation A/B (fill_upper: cuSOLVER's fast path reads the column-major lower view)
-        if (!diag || c <= r) {
-          double* q = &Cmat[(size_t)r * Dpad + c];
-          ar_add(q, mc_off ? q + mc_off : nullptr, -acc[i][j]);
-        }
-        if (fill_upper && (!diag || c < r)) atomicAdd(&Cmat[(size_t)c * Dpad + r], -acc[i][j]);
-      }
-    }
-  }
+// d[16 x 8] += a[16 x 16] b[16 x 8]; lane (g = lane / 4, t = lane % 4) holds a[i] = A[g + 8 (i & 1)][t + 4 (i >> 1)],
+// b[j] = B[t + 4 j][g], d = (g, 2t), (g, 2t + 1), (g + 8, 2t), (g + 8, 2t + 1)
+__device__ __forceinline__ void dmma_m16n8k16(double (&d)[4], const double (&a)[8], const double (&b)[4]) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, "
+      "{%0,%1,%2,%3};"
+      : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]),
+        "d"(b[2]), "d"(b[3]));
 }
 
-// ------------------------------------------------------------------------------------------------
-// Same SYRK on the FP64 tensor path: mma.sync.m8n8k4.f64 (SASS DMMA).  CTA tile 128x128, 8 warps as 4x2,
-// warp tile 32x64 = 4x8 MMA tiles (64 accumulator doubles per lane); operands k-major in shared memory with a
-// 136-double row stride so the four k-rows of a fragment load fall into disjoint bank halves.
-constexpr int SD_LDS = 136;
-
-__device__ __forceinline__ void dmma_m8n8k4(double& d0, double& d1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-               : "+d"(d0), "+d"(d1)
-               : "d"(a), "d"(b));
-}
-
-__global__ void __launch_bounds__(SY_THREADS) syrk_dmma_kernel(int Kpad, int Dpad, int k_per_split,
-                                                               const double* __restrict__ Zt,
-                                                               double* __restrict__ Cmat, ptrdiff_t mc_off,
-                                                               int fill_upper) {
-  extern __shared__ __align__(16) double sd_smem[];
-  int t = blockIdx.x;
-  int bi = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-  while ((bi + 1) * (bi + 2) / 2 <= t) ++bi;
-  while (bi * (bi + 1) / 2 > t) --bi;
-  const int bj = t - bi * (bi + 1) / 2;
-  const bool diag = (bi == bj);
-  const int kbeg = blockIdx.y * k_per_split;
-  const int kend = min(Kpad, kbeg + k_per_split);
-  const int nslab = (kend - kbeg + SY_BK - 1) / SY_BK;
-  if (nslab <= 0) return;
-  double* As = sd_smem;                                      // [STAGES][BK][SD_LDS]
-  double* Bs = sd_smem + SY_STAGES * SY_BK * SD_LDS;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int wm = warp >> 1, wn = warp & 1;                   // 4 x 2 warps
-  const int g = lane >> 2, q = lane & 3;
-
-  auto load_slab = [&](int slab, int stage) {
-    const int k0 = kbeg + slab * SY_BK;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int chunk = tid + i * SY_THREADS;
-      const int kk = chunk >> 6;
-      const int cc = (chunk & 63) * 2;
-      const size_t grow = (size_t)(k0 + kk) * Dpad;
-      cp_async16(As + (stage * SY_BK + kk) * SD_LDS + cc, Zt + grow + bi * SY_BM + cc);
-      if (!diag) cp_async16(Bs + (stage * SY_BK + kk) * SD_LDS + cc, Zt + grow + bj * SY_BM + cc);
+__global__ void __launch_bounds__(SF_THREADS, 1)
+    syrk_f64_kernel(const SyrkWork* __restrict__ work, int nwork, int Kpad, int Dpad, const double* __restrict__ Zt,
+                    double* __restrict__ Cmat, ptrdiff_t mc_off, int fill_upper, const __grid_constant__ FabricDev fd) {
+  extern __shared__ __align__(16) double sf_smem[];
+  uint64_t* full = reinterpret_cast<uint64_t*>(sf_smem + SF_STAGES * SF_STAGE_DOUBLES);
+  uint64_t* empty = full + SF_STAGES;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < SF_STAGES; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], SF_MMA_WARPS);        // one arrive per MMA warp
     }
-    cp_async_commit();
-  };
-
-  double c[4][8][2];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) c[i][j][0] = c[i][j][1] = 0.0;
-
-#pragma unroll
-  for (int s = 0; s < SY_STAGES - 1; ++s) {
-    if (s < nslab) load_slab(s, s);
-    else cp_async_commit();
+    mbar_fence_init();
   }
-  for (int slab = 0; slab < nslab; ++slab) {
-    cp_async_wait<SY_STAGES - 2>();
-    __syncthreads();
-    {
-      const int nxt = slab + SY_STAGES - 1;
-      if (nxt < nslab) load_slab(nxt, nxt % SY_STAGES);
-      else cp_async_commit();
-    }
-    const int stage = slab % SY_STAGES;
-    const double* as = As + stage * SY_BK * SD_LDS;
-    const double* bs = diag ? as : (Bs + stage * SY_BK * SD_LDS);
-#pragma unroll
-    for (int k4 = 0; k4 < SY_BK / 4; ++k4) {
-      double a[4], b[8];
-      const double* arow = as + (k4 * 4 + q) * SD_LDS + wm * 32 + g;
-      const double* brow = bs + (k4 * 4 + q) * SD_LDS + wn * 64 + g;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) a[i] = arow[i * 8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) b[j] = brow[j * 8];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) dmma_m8n8k4(c[i][j][0], c[i][j][1], a[i], b[j]);
-    }
-  }
-  cp_async_wait<0>();
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = bi * SY_BM + wm * 32 + i * 8 + g;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int cc = bj * SY_BM + wn * 64 + j * 8 + 2 * q;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const double v = c[i][j][h];
-        const int col = cc + h;
-        if (v != 0.0) {
-          if (!diag || col <= r) {
-            double* q = &Cmat[(size_t)r * Dpad + col];
-            ar_add(q, mc_off ? q + mc_off : nullptr, -v);
-          }
-          if (fill_upper && (!diag || col < r)) atomicAdd(&Cmat[(size_t)col * Dpad + r], -v);   // library A/B only
+  __syncthreads();
+
+  int stage = 0, phase = 0;
+  if (warp < 4) {
+    // ===== producer: lanes 0-15 copy the k-rows of operand bi, lanes 16-31 those of bj =====
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp > 0) return;
+    const int row = lane & (SF_BK - 1), opnd = lane / SF_BK;
+    for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
+      const SyrkWork wk = work[w];
+      const bool diag = wk.bi == wk.bj;
+      const int k1 = min(Kpad, wk.kb1 * 64);
+      for (int k = wk.kb0 * 64; k < k1; k += SF_BK) {
+        mbar_wait(&empty[stage], phase ^ 1);
+        if (lane == 0) mbar_expect_tx(&full[stage], (diag ? 1u : 2u) * SF_BK * SF_BM * (uint32_t)sizeof(double));
+        __syncwarp();
+        if (opnd == 0 || !diag)
+          tma_load_1d(sf_smem + stage * SF_STAGE_DOUBLES + (opnd * SF_BK + row) * SF_LDS,
+                      Zt + (size_t)(k + row) * Dpad + (opnd ? wk.bj : wk.bi) * SF_BM, SF_BM * sizeof(double), &full[stage]);
+        if (++stage == SF_STAGES) {
+          stage = 0;
+          phase ^= 1;
         }
       }
     }
+    return;
+  }
+
+  // ===== MMA warps =====
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int wm = (warp - 4) >> 2, wn = warp & 3;
+  const int g = lane >> 2, t = lane & 3;
+  for (int w = blockIdx.x; w < nwork; w += gridDim.x) {
+    const SyrkWork wk = work[w];
+    const bool diag = wk.bi == wk.bj;
+    const int k1 = min(Kpad, wk.kb1 * 64);
+    double acc[4][4][4];
+#pragma unroll
+    for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int h = 0; h < 4; ++h) acc[mt][nt][h] = 0.0;
+    for (int k = wk.kb0 * 64; k < k1; k += SF_BK) {
+      mbar_wait(&full[stage], phase);
+      const double* as = sf_smem + stage * SF_STAGE_DOUBLES + t * SF_LDS + wm * 64 + g;
+      const double* bs = sf_smem + stage * SF_STAGE_DOUBLES + (diag ? 0 : SF_BK * SF_LDS) + t * SF_LDS + wn * 32 + g;
+      double b[4][4];
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) b[nt][j] = bs[4 * j * SF_LDS + nt * 8];
+#pragma unroll
+      for (int mt = 0; mt < 4; ++mt) {
+        double a[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) a[i] = as[4 * (i >> 1) * SF_LDS + mt * 16 + 8 * (i & 1)];
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) dmma_m16n8k16(acc[mt][nt], a, b[nt]);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[stage]);
+      if (++stage == SF_STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+#pragma unroll
+    for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+        for (int h = 0; h < 4; ++h) {
+          const int r = wk.bi * SF_BM + wm * 64 + mt * 16 + g + 8 * (h >> 1);
+          const int col = wk.bj * SF_BM + wn * 32 + nt * 8 + 2 * t + (h & 1);
+          syrk_red_upper(Cmat, Dpad, r, col, wk.bj, diag, acc[mt][nt][h], mc_off, fill_upper, fd);
+        }
   }
 }
 
@@ -647,10 +557,10 @@ int launch_assemble_hc(int S, int dc, int ns, int KR, int Dpad, const double* ca
   return VGG_OK;
 }
 int launch_z_transpose(int D, int N, int Dpad, const double* W, const double* M, const double* q, double* Zt,
-                       double* rhs, ptrdiff_t mc_off, cudaStream_t st, unsigned long long* amax) {
+                       double* rhs, ptrdiff_t mc_off, cudaStream_t st) {
   const size_t pitch = (size_t)(D + (D & 1));
   dim3 grid((D + 127) / 128, (N + ZB_NT - 1) / ZB_NT);
-  z_build_kernel<<<grid, 128, 0, st>>>(D, N, Dpad, pitch, W, M, q, Zt, rhs, mc_off, amax, g_band_dev.rb_range);
+  z_build_kernel<<<grid, 128, 0, st>>>(D, N, Dpad, pitch, W, M, q, Zt, rhs, mc_off, g_band_dev.rb_range);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
@@ -661,30 +571,55 @@ int g_fill_upper = 0;
 // reduce-scatter destinations of the running multi-GPU solve (set per iteration by csrc/ba_solve.cu; world <= 1: off)
 FabricDev g_fabric_dev = {0, 0, {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}};
 
+// Band hint of the current solve (csrc/syrk_i8.cu; set by csrc/ba_solve.cu or vgg_dev_set_syrk_ranges): [lo, hi) k-block
+// range per 128-column row block of Zt outside which the block is exactly zero; empty = dense.
+extern std::vector<int> g_syrk_kb_ranges;
+
+// work list of the last shape / band hint, kept on the device until either changes
+struct SyrkF64State {
+  int dev = -1, Kpad = -1, Dpad = -1, sms = 0, nwork = 0;
+  std::vector<int> ranges;
+  SyrkWork* work_dev = nullptr;
+  size_t work_cap = 0;
+};
+thread_local SyrkF64State g_sf;
+
+// Cmat -= Zt^T Zt: Zt [Kpad][Dpad] (Dpad % 128 == 0, Kpad % 16 == 0), Cmat [Dpad][Dpad] row-major, LOWER triangle (plus
+// the mirror when g_fill_upper; into the fabric destinations of g_fabric_dev / mc_off, see syrk_red_upper)
 int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc_off, cudaStream_t st) {
-  const int nb = Dpad / SY_BM;
-  const int ntiles = nb * (nb + 1) / 2;
-  const int nslab = Kpad / SY_BK;
-  // split K so that the grid covers the 132 SMs of an H100 SXM a few times over
-  int splits = (132 * 3 + ntiles - 1) / ntiles;
-  if (splits < 1) splits = 1;
-  if (splits > nslab) splits = nslab;
-  int slabs_per = (nslab + splits - 1) / splits;
-  splits = (nslab + slabs_per - 1) / slabs_per;
-  const size_t smem = sizeof(double) * 2 * SY_STAGES * SY_BK * SY_BM;
-  const size_t smem_d = sizeof(double) * 2 * SY_STAGES * SY_BK * SD_LDS;
-  static bool attr_set = false;
-  static int use_dmma = 0;
-  if (!attr_set) {
-    VGG_CUDA_CHECK(cudaFuncSetAttribute(syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    VGG_CUDA_CHECK(cudaFuncSetAttribute(syrk_dmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_d));
-    const char* e = getenv("VGG_SYRK_DMMA");
-    use_dmma = (e && e[0] == '0') ? 0 : 1;     // DMMA is the default (r01 A/B: 3.1 ms -> 2.4 ms at C3); VGG_SYRK_DMMA=0 selects the DFMA kernel
-    attr_set = true;
+  VGG_REQUIRE(Dpad % SF_BM == 0 && Kpad % SF_BK == 0, "syrk: Dpad must be a multiple of 128 and Kpad of 16");
+  const int nb = Dpad / SF_BM, KB = (Kpad + 63) / 64;
+  SyrkF64State& hs = g_sf;
+  const std::vector<int> ranges = (int)g_syrk_kb_ranges.size() == 2 * nb ? g_syrk_kb_ranges : std::vector<int>();
+  int dev = 0;
+  VGG_CUDA_CHECK(cudaGetDevice(&dev));
+  if (hs.dev != dev || hs.Kpad != Kpad || hs.Dpad != Dpad || hs.ranges != ranges) {
+    VGG_CUDA_CHECK(cudaDeviceGetAttribute(&hs.sms, cudaDevAttrMultiProcessorCount, dev));
+    VGG_CUDA_CHECK(cudaFuncSetAttribute(syrk_f64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SF_SMEM_BYTES));
+    // equal-length items, longest first: the CTAs of a wave advance through k together, so Zt is read from HBM about
+    // once and from L2 by the other tiles of its column block
+    std::vector<SyrkWork> work;
+    build_work_list<SyrkWork>({1}, syrk_tile_jobs(nb, ranges), KB, hs.sms, KB, 1,
+                              [](const SyrkTileJob& j, int, int k0, int k1) { return SyrkWork{j.bi, j.bj, k0, k1}; }, &work);
+    // a kernel in flight (on any stream) may still read the previous list
+    VGG_CUDA_CHECK(cudaDeviceSynchronize());
+    if (hs.dev != dev || work.size() > hs.work_cap) {
+      if (hs.work_dev) cudaFree(hs.work_dev);
+      hs.work_dev = nullptr;
+      hs.work_cap = std::max<size_t>(work.size(), 1);
+      VGG_CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&hs.work_dev), sizeof(SyrkWork) * hs.work_cap));
+    }
+    if (!work.empty())
+      VGG_CUDA_CHECK(cudaMemcpy(hs.work_dev, work.data(), sizeof(SyrkWork) * work.size(), cudaMemcpyHostToDevice));
+    hs.nwork = (int)work.size();
+    hs.dev = dev;
+    hs.Kpad = Kpad;
+    hs.Dpad = Dpad;
+    hs.ranges = ranges;
   }
-  dim3 grid(ntiles, splits);
-  if (use_dmma) syrk_dmma_kernel<<<grid, SY_THREADS, smem_d, st>>>(Kpad, Dpad, slabs_per * SY_BK, Zt, Cmat, mc_off, g_fill_upper);
-  else syrk_kernel<<<grid, SY_THREADS, smem, st>>>(Kpad, Dpad, slabs_per * SY_BK, Zt, Cmat, mc_off, g_fill_upper);
+  if (hs.nwork == 0) return VGG_OK;
+  syrk_f64_kernel<<<std::min(hs.sms, hs.nwork), SF_THREADS, SF_SMEM_BYTES, st>>>(hs.work_dev, hs.nwork, Kpad, Dpad, Zt, Cmat,
+                                                                               mc_off, g_fill_upper, g_fabric_dev);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
@@ -737,3 +672,15 @@ int launch_gradmax(int D, int N, const double* gvec, const uint8_t* pconst, cons
 }
 
 }  // namespace vgg
+
+extern "C" {
+
+/* development probe (csrc/dev_probes.h): the in-loop Schur SYRK on its own, with the band hint of vgg_dev_set_syrk_ranges */
+int vgg_dev_syrk_f64(int Kpad, int Dpad, const double* Zt, double* Cmat, void* stream) {
+  using namespace vgg;
+  g_launch_count = 0;
+  VGG_REQUIRE(Zt && Cmat && Kpad > 0 && Dpad > 0, "bad argument");
+  return launch_syrk(Kpad, Dpad, Zt, Cmat, 0, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

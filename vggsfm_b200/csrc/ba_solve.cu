@@ -34,13 +34,8 @@ int launch_point_prep(int N, const double* H_pp, const double* g_p, const double
 int launch_assemble_hc(int S, int dc, int ns, int KR, int Dpad, const double* camrec, const double* shared_in,
                        double* Sraw, double* rhs, double* hdiag, double* gvec, ptrdiff_t mc_off, cudaStream_t st);
 int launch_z_transpose(int D, int N, int Dpad, const double* W, const double* M, const double* q, double* Zt,
-                       double* rhs, ptrdiff_t mc_off, cudaStream_t st, unsigned long long* amax);
+                       double* rhs, ptrdiff_t mc_off, cudaStream_t st);
 int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc_off, cudaStream_t st);
-size_t syrk_i8_workspace_bytes(int Kpad, int Dpad, int slices);
-int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc_off, int slices, void* ws,
-                   size_t ws_bytes, cudaStream_t st, bool amax_ready);
-unsigned long long* syrk_i8_amax(void* ws);
-int syrk_i8_reset_amax(void* ws, int Dpad, cudaStream_t st);
 int launch_scale_damp(int D, int Dpad, double* A, const double* rhs, const double* hdiag, const double* sc,
                       const uint8_t* pconst, double radius, double min_diag, double max_diag, double* bvec,
                       cudaStream_t st);
@@ -175,28 +170,9 @@ struct Layout {
   double *chol_diag;
   int *dev_info;
   int *trsv_flags;
-  uint8_t* oz_ws;    // int8 slices + scales of the tensor-core SYRK (csrc/syrk_i8.cu)
-  size_t oz_bytes;
   size_t potrf_lwork;
   size_t bytes;
 };
-
-// The Schur SYRK runs on the tensor cores by default (INT8 wgmma Ozaki slices, csrc/syrk_i8.cu; same iterates as the
-// FP64 kernels).  VGG_SYRK=ozaki:N picks 3..7 slices (default 7 =
-// 54 fractional bits, FP64-equivalent); VGG_SYRK=fp64 selects the FP64-pipe kernels (DMMA / DFMA).
-static int syrk_i8_slices() {
-  static int slices = -1;
-  if (slices < 0) {
-    slices = 7;
-    const char* e = getenv("VGG_SYRK");
-    if (e && strncmp(e, "ozaki", 5) == 0) {
-      if (e[5] == ':' && e[6] >= '3' && e[6] <= '7') slices = e[6] - '0';
-    } else if (e && e[0]) {
-      slices = 0;
-    }
-  }
-  return slices;
-}
 
 static int make_layout(int S, int N, int model, int mode, void* base, size_t cap, size_t potrf_lwork, Layout* L) {
   int dc, ns, KR;
@@ -238,9 +214,6 @@ static int make_layout(int S, int N, int model, int mode, void* base, size_t cap
   L->chol_diag = c.take<double>(chol_workspace_doubles(L->D + 1));
   L->dev_info = c.take<int>(4);
   L->trsv_flags = c.take<int>(trsv_workspace_ints(L->D));
-  L->oz_bytes = syrk_i8_workspace_bytes(L->Kpad, L->Dpad, 7);
-  c.off = align_up(c.off, 1024);
-  L->oz_ws = c.take<uint8_t>(L->oz_bytes);
   L->bytes = align_up(c.off, 256);
   if (base && c.off > cap) {
     set_error("workspace too small: need %zu bytes, have %zu", c.off, cap);
@@ -328,7 +301,7 @@ struct Fabric2 {
   }
 };
 
-extern std::vector<int> g_syrk_kb_ranges;     // csrc/syrk_i8.cu: band hint of the current solve
+extern std::vector<int> g_syrk_kb_ranges;     // csrc/syrk_i8.cu: band hint of the current solve (both SYRK kernels)
 extern std::vector<int> g_chol_band_end;      // csrc/chol.cu: block structure of the reduced system (banded + arrow)
 extern int g_chol_arrow_blk;
 extern BandDev g_band_dev;                    // csrc/ba_schur.cu: device tables for ba_blocks / z_build / backsub
@@ -512,13 +485,8 @@ static int schur_build(const Layout& L, const BlockSet& b, const uint8_t* point_
   // fabric mode: every rank's copy must be zero before anyone's multimem reductions land in it
   if (mc_off && barrier && (rc = (*barrier)())) return rc;
   if ((rc = launch_assemble_hc(L.S, L.dc, L.ns, L.KR, L.Dpad, b.camrec, b.shared, Sraw, rhs, hdiag, gvec, mc_off, st))) return rc;
-  const int oz = L.oz_bytes ? syrk_i8_slices() : 0;
-  if (oz && (rc = syrk_i8_reset_amax(L.oz_ws, L.Dpad, st))) return rc;
-  if ((rc = launch_z_transpose(L.D, L.N, L.Dpad, b.W, L.M, L.q, L.Zt, rhs, mc_off, st, oz ? syrk_i8_amax(L.oz_ws) : nullptr)))
-    return rc;
-  if (oz) rc = launch_syrk_i8(L.Kpad, L.Dpad, L.Zt, Sraw, mc_off, oz, L.oz_ws, L.oz_bytes, st, true);
-  else rc = launch_syrk(L.Kpad, L.Dpad, L.Zt, Sraw, mc_off, st);
-  if (rc) return rc;
+  if ((rc = launch_z_transpose(L.D, L.N, L.Dpad, b.W, L.M, L.q, L.Zt, rhs, mc_off, st))) return rc;
+  if ((rc = launch_syrk(L.Kpad, L.Dpad, L.Zt, Sraw, mc_off, st))) return rc;
   // ... and all reductions must have landed before anyone reads its copy
   if (mc_off && barrier && (rc = (*barrier)())) return rc;
   return VGG_OK;
@@ -707,8 +675,7 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     // barriers and small all-reduces through the host hook) for A/B
     static const bool want_v2 = [] { const char* e = getenv("VGG_FABRIC"); return !(e && e[0] == '1'); }();
     const FabricLayout lay = fabric_layout(D, L.Dpad);
-    if (want_v2 && fabric->world > 1 && fabric->world <= 8 && fabric->peer_base[0] && fabric->total_doubles >= lay.total &&
-        L.oz_bytes && syrk_i8_slices() > 0) {
+    if (want_v2 && fabric->world > 1 && fabric->world <= 8 && fabric->peer_base[0] && fabric->total_doubles >= lay.total) {
       fab2.on = true;
       fab2.lay = lay;
       fab2.base.world = fabric->world;
@@ -720,7 +687,7 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
       VGG_REQUIRE(allreduce, "fabric v1 needs the hook for its barrier (op 2)");
     }
   }
-  if (L.oz_bytes && (rc = compute_band_hint(prob, dc, D, L.Dpad, L.Kpad, allreduce != nullptr || fabric != nullptr, st))) return rc;
+  if ((rc = compute_band_hint(prob, dc, D, L.Dpad, L.Kpad, allreduce != nullptr || fabric != nullptr, st))) return rc;
   if (g_band_dev.fg_tracks) {
     // the kernels skip the (track chunk, frame group) regions no observation falls into: their W blocks must read as zero
     const size_t w_doubles = (size_t)N * (size_t)(D + (D & 1)) * 3;

@@ -86,6 +86,9 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
       "{\n"
@@ -176,6 +179,30 @@ __device__ __forceinline__ double warp_max(double r) {
 #pragma unroll
   for (int off = 16; off >= 1; off >>= 1) r = fmax(r, __shfl_xor_sync(0xffffffffu, r, off));
   return r;
+}
+
+// Epilogue of the Schur SYRK kernels (csrc/ba_schur.cu, csrc/syrk_i8.cu): subtract v = (Zt^T Zt)[r][col] of an UPPER
+// tile (row block of r <= column block bj of col; diag: the two blocks are the same).  The element goes to its mirror
+// (col, r) of the row-major LOWER triangle, which is what csrc/chol.cu factors; the direct element (r, col) is only
+// written for the library factorisation A/B (fill_upper).  Destinations of the lower triangle:
+//   fd.world > 1   reduce-scatter: row block bj lives on rank (bj mod world) until the gather (csrc/fabric.cu); one
+//                  system-scope RED over NVLink per element, only into the owner's copy
+//   mc_off != 0    one multimem RED on the NVSwitch multicast address, landing in every rank's copy
+//   otherwise      a local f64 RED
+__device__ __forceinline__ void syrk_red_upper(double* Cmat, int Dpad, int r, int col, int bj, bool diag, double v,
+                                               ptrdiff_t mc_off, int fill_upper, const FabricDev& fd) {
+  if (v == 0.0) return;
+  if (!diag || col >= r) {
+    const size_t off = (size_t)col * Dpad + r;
+    if (fd.world > 1) {
+      asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(fd.peer[bj % fd.world] + off), "d"(-v) : "memory");
+    } else if (mc_off) {
+      asm volatile("multimem.red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(Cmat + off + mc_off), "d"(-v) : "memory");
+    } else {
+      atomicAdd(Cmat + off, -v);
+    }
+  }
+  if (fill_upper && (!diag || col > r)) atomicAdd(&Cmat[(size_t)r * Dpad + col], -v);
 }
 #endif  // __CUDACC__
 

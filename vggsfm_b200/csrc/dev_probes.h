@@ -1,5 +1,5 @@
 // Development probes (NOT part of the public C ABI in include/vggsfm_b200.h): exported from the library for
-// tools/syrk_i8_check.py, tools/microbench.py and bench.py's roofline only.
+// tools/syrk_i8_check.py, tools/microbench.py, bench.py's roofline and the tests only.
 #pragma once
 #ifdef __cplusplus
 extern "C" {
@@ -18,6 +18,9 @@ int vgg_dev_chol128_probe(int leaf, int reps, const double* A_host, double* L_ho
  * 128-column row block rb of Zt is exactly zero (count = 2 * Dpad/128; count = 0 clears it).  vgg_ba_solve computes the
  * same thing from the visibility mask and clears it when it returns. */
 int vgg_dev_set_syrk_ranges(const int* ranges_host, int count);
+/* The Schur SYRK of the LM loop (csrc/ba_schur.cu, FP64 tensor cores): Cmat -= Zt^T Zt into the row-major LOWER triangle
+ * of Cmat [Dpad][Dpad] for Zt [Kpad][Dpad] (device pointers; Dpad % 128 == 0, Kpad % 16 == 0), honouring the band hint. */
+int vgg_dev_syrk_f64(int Kpad, int Dpad, const double* Zt, double* Cmat, void* stream);
 /* Backward substitution (csrc/trsv.cu) with per-block-row timestamps (ns): stamps_host[2 b] = block row b (64 rows) has
  * consumed every x_j it needs, [2 b + 1] = x_b published.  A_dev: row-major upper triangle, lda columns. */
 int vgg_dev_trsv_probe(int n, int lda, const double* A_dev, const double* y_dev, double* x_dev, long long* stamps_host);

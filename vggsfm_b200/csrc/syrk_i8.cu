@@ -1,8 +1,8 @@
-// Schur SYRK on the tensor cores: Sraw -= Zt^T Zt in FP64-equivalent precision computed with INT8 wgmma (Ozaki
-// splitting), the step SURVEY section 0.6 / DESIGN section 4.2 name as the dominant cost of a bundle-adjustment
-// iteration (76.5 GFLOP at 400 x 4096).
-//
-// INT8 wgmma accumulates exactly in int32 at about 30x the FP64 tensor-core rate of sm_90a (data-sheet figures).
+// Schur SYRK on the INT8 tensor cores: Sraw -= Zt^T Zt in FP64-equivalent precision computed with INT8 wgmma (Ozaki
+// splitting), exposed as vgg_syrk_ozaki.  The LM loop runs the FP64 tensor-core kernel of csrc/ba_schur.cu instead:
+// INT8 wgmma has 32x the FP64 tensor-core rate of sm_90a (4096 int8 MAC against 128 DMMA FMA per clock and SM), and
+// s = 7 slices need 28 int8 products per FP64-equivalent product, so even at peak this path is only 32/28 = 1.14x
+// the DMMA rate before the slicing pass; at 400 x 4096 it measured 2x slower (DESIGN section 4.2).
 //   1. every column d of Z (a reduced camera parameter) gets a power-of-two scale 2^e_d >= max_k |Z[k][d]|;
 //      x = Z 2^-e_d is rounded to B = 8s-2 fractional bits and written as s balanced base-256 digits
 //      (int8 "slices", most significant first): x = 2^-B sum_p d_p 256^(s-p)          (oz_slice_kernel)
@@ -10,7 +10,7 @@
 //      every C_t is an exact int32 (|d| <= 128, at most 7 pairs and 16384 k per work item: |C_t| < 2^31); orders t > s+1 are below
 //      the rounding of step 1 and are dropped, leaving s(s+1)/2 int8 GEMMs (28 for s = 7)  (oz_syrk_kernel)
 //   3. the epilogue recombines the C_t of a tile in FP64 registers and adds -value into Sraw with f64 RED
-//      (or multimem.red in fabric mode), exactly like the DMMA kernel's epilogue.
+//      (or multimem.red in fabric mode) through syrk_red_upper, the epilogue of the FP64 kernel too.
 //
 // oz_syrk_kernel is a persistent, warp-specialised wgmma kernel (one CTA per SM):
 //   warpgroup 0    producer: the int8 slices are stored in HBM as 8 KB tile images that are already in the 64-byte
@@ -22,6 +22,7 @@
 // Work items (tile, order group, k range) are built on the host, longest first, and strided over the CTAs.
 #include "common.cuh"
 #include "dev_probes.h"
+#include "syrk_work.h"
 
 #include <algorithm>
 #include <vector>
@@ -149,9 +150,6 @@ __global__ void __launch_bounds__(512) oz_slice_kernel(int Kpad, int Dpad, int K
 // pull a global range into L2 ahead of the bulk copy that will read it (hides the HBM latency of first-touch tiles)
 __device__ __forceinline__ void l2_prefetch(const void* gptr, uint32_t bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gptr), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 // d[64 x 128] (+)= A[64 x 32] * B[128 x 32]^T, int8 x int8 -> int32, both operands K-major in shared memory.
@@ -283,7 +281,7 @@ __global__ void __launch_bounds__(OZ_THREADS, 1)
         phase ^= 1;
       }
     }
-    // combine the orders, scale and accumulate into Sraw (same triangle rules as syrk_dmma_kernel)
+    // combine the orders, scale and accumulate into Sraw (syrk_red_upper, common.cuh)
     const int row_base = wk.bi * OZ_BM + half * 64 + wq * 16 + (lane >> 2);
     const int col_base = wk.bj * OZ_BM + 2 * (lane & 3);
 #pragma unroll
@@ -307,24 +305,7 @@ __global__ void __launch_bounds__(OZ_THREADS, 1)
           if (er == OZ_EXPO_BAD || ec == OZ_EXPO_BAD) v = __longlong_as_double(0x7ff8000000000000LL);
           else if (tame && ec > -400 && ec < 400) v = v * sr * pow2[col];
           else v = ldexp(v, er + ec + g.exp_base);
-          if (v != 0.0) {
-            // The work list holds UPPER tiles (bi <= bj): element (r, col) goes to its mirror (col, r) of the row-major
-            // LOWER triangle, which is what csrc/chol.cu factors (fabric mode: one multimem op per element).  The direct
-            // element (r, col) is only written for the library factorisation A/B.
-            if (!diag || col >= r) {
-              const size_t off = (size_t)col * Dpad + r;
-              if (fd.world > 1) {
-                // reduce-scatter: row block wk.bj of the lower triangle lives on rank (wk.bj mod world) until the gather
-                // (csrc/fabric.cu); one system-scope RED over NVLink per element, only into the owner's copy
-                asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(fd.peer[wk.bj % fd.world] + off), "d"(-v) : "memory");
-              } else if (mc_off) {
-                asm volatile("multimem.red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(Cmat + off + mc_off), "d"(-v) : "memory");
-              } else {
-                atomicAdd(Cmat + off, -v);
-              }
-            }
-            if (fill_upper && (!diag || col > r)) atomicAdd(&Cmat[(size_t)r * Dpad + col], -v);
-          }
+          syrk_red_upper(Cmat, Dpad, r, col, wk.bj, diag, v, mc_off, fill_upper, fd);
         }
     }
   }
@@ -379,50 +360,6 @@ bool build_plan(int s, OzPlan* plan, int max_acc) {
 }
 
 
-// Work items are handed out statically (item w goes to CTA / cluster w mod n, longest first), so the finishing time is
-// the heaviest residue class.  The k-split granularity is chosen by simulating that assignment for a few candidate
-// targets and keeping the best makespan (+ a small charge per item for its epilogue).
-struct OzTileJob {
-  int bi, bj;
-  int kb0 = 0, kb1 = -1;       // k-block range in which BOTH row blocks can be non-zero (kb1 < 0: all of K)
-};
-template <class Work, class Make>
-void build_work_list(const OzPlan& plan, const std::vector<OzTileJob>& jobs, int KB, int nworkers, Make make,
-                     std::vector<Work>* out) {
-  long long total = 0, pairs_all = 0;
-  for (int g = 0; g < plan.n_groups; ++g) pairs_all += plan.g[g].n_pairs;
-  for (const OzTileJob& jb : jobs) total += pairs_all * (long long)((jb.kb1 < 0 ? KB : jb.kb1) - jb.kb0);
-  const long long epilogue_cost = 24;            // pair-kblock equivalents of one item's epilogue (order combination + REDs)
-  long long best = -1;
-  for (int div = 2; div <= 10; ++div) {
-    const long long target = std::max<long long>(1, total / ((long long)nworkers * div));
-    std::vector<std::pair<long long, Work>> items;
-    for (const OzTileJob& jb : jobs) {
-      const int jk0 = jb.kb0, jk1 = jb.kb1 < 0 ? KB : jb.kb1, len = jk1 - jk0;
-      if (len <= 0) continue;
-      for (int g = 0; g < plan.n_groups; ++g) {
-        const long long cost = (long long)plan.g[g].n_pairs * len;
-        int parts = (int)std::min<long long>(16, std::max<long long>(1, (cost + target / 2) / target));
-        parts = std::max(parts, (len + OZ_MAX_ITEM_KB - 1) / OZ_MAX_ITEM_KB);      // int32 accumulators stay exact
-        parts = std::min(parts, len);
-        for (int p = 0; p < parts; ++p) {
-          const int k0 = jk0 + (int)((long long)len * p / parts), k1 = jk0 + (int)((long long)len * (p + 1) / parts);
-          items.push_back({(long long)plan.g[g].n_pairs * (k1 - k0), make(jb, g, k0, k1)});
-        }
-      }
-    }
-    std::stable_sort(items.begin(), items.end(), [](const auto& a, const auto& b) { return a.first > b.first; });
-    std::vector<long long> load(nworkers, 0);
-    for (size_t i = 0; i < items.size(); ++i) load[i % nworkers] += items[i].first + epilogue_cost;
-    const long long makespan = *std::max_element(load.begin(), load.end());
-    if (best < 0 || makespan < best) {
-      best = makespan;
-      out->clear();
-      for (auto& it : items) out->push_back(it.second);
-    }
-  }
-}
-
 struct OzHostState {
   int Kpad = -1, Dpad = -1, slices = -1, sms = 0;
   std::vector<int> ranges;        // k-block range per row block the cached work list was built for (empty: dense)
@@ -454,14 +391,6 @@ size_t oz_workspace_bytes(int Kpad, int Dpad, int s) {
 
 size_t syrk_i8_workspace_bytes(int Kpad, int Dpad, int slices) { return oz_workspace_bytes(Kpad, Dpad, slices); }
 
-// The column maxima can be produced by whoever writes Zt (z_build_kernel does): zero them with syrk_i8_reset_amax,
-// hand syrk_i8_amax(ws) to the producer, then call launch_syrk_i8 with amax_ready = true.
-unsigned long long* syrk_i8_amax(void* ws) { return static_cast<unsigned long long*>(ws); }
-int syrk_i8_reset_amax(void* ws, int Dpad, cudaStream_t st) {
-  VGG_CUDA_CHECK(cudaMemsetAsync(ws, 0, sizeof(unsigned long long) * Dpad, st));
-  return VGG_OK;
-}
-
 // Sraw -= Zt^T Zt with s int8 slices.  Zt [Kpad][Dpad] (Dpad % 128 == 0), Cmat [Dpad][Dpad] row-major, LOWER triangle
 // written (plus the mirror when g_fill_upper), same contract as launch_syrk.
 extern int g_fill_upper;      // csrc/ba_schur.cu
@@ -471,7 +400,7 @@ std::vector<int> g_syrk_kb_ranges;
 extern FabricDev g_fabric_dev;  // csrc/ba_schur.cu: reduce-scatter destinations of the current multi-GPU solve (world <= 1: off)
 
 int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc_off, int s, void* ws,
-                   size_t ws_bytes, cudaStream_t st, bool amax_ready) {
+                   size_t ws_bytes, cudaStream_t st) {
   VGG_REQUIRE(Dpad % OZ_BM == 0, "syrk_i8: Dpad must be a multiple of 128");
   VGG_REQUIRE(ws_bytes >= oz_workspace_bytes(Kpad, Dpad, s), "syrk_i8: workspace too small");
   const int KB = (Kpad + OZ_BK - 1) / OZ_BK;
@@ -496,19 +425,12 @@ int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t
     VGG_CUDA_CHECK(cudaFuncSetAttribute(oz_syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OZ_SMEM_BYTES));
     // work items: (tile, group, k range), longest first (build_work_list picks the k-split granularity)
     {
-      std::vector<OzTileJob> jobs;
-      for (int bi = 0; bi < nb; ++bi)
-        for (int bj = 0; bj <= bi; ++bj) {                                    // upper tile (row block bj <= column block bi)
-          OzTileJob jb{bj, bi};
-          if (banded) {
-            jb.kb0 = std::max(hs.ranges[2 * bi], hs.ranges[2 * bj]);
-            jb.kb1 = std::min(hs.ranges[2 * bi + 1], hs.ranges[2 * bj + 1]);
-            if (jb.kb1 <= jb.kb0) continue;
-          }
-          jobs.push_back(jb);
-        }
-      build_work_list<OzWork>(hs.plan, jobs, KB, hs.sms,
-                              [](const OzTileJob& j, int g, int k0, int k1) { return OzWork{j.bi, j.bj, g, k0, k1}; }, &hs.work);
+      std::vector<int> pairs;
+      for (int g = 0; g < hs.plan.n_groups; ++g) pairs.push_back(hs.plan.g[g].n_pairs);
+      // epilogue_cost: pair-kblock equivalents of one item's epilogue (order combination + REDs); OZ_MAX_ITEM_KB keeps
+      // the int32 accumulators exact
+      build_work_list<OzWork>(pairs, syrk_tile_jobs(nb, hs.ranges), KB, hs.sms, OZ_MAX_ITEM_KB, 24,
+                              [](const SyrkTileJob& j, int g, int k0, int k1) { return OzWork{j.bi, j.bj, g, k0, k1}; }, &hs.work);
     }
     if (hs.work.size() > hs.pinned_cap) {
       if (hs.pinned) cudaFreeHost(hs.pinned);
@@ -531,8 +453,8 @@ int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t
   const int nwork = (int)hs.work.size();
 
   VGG_CUDA_CHECK(cudaMemcpyAsync(work_d, hs.pinned, sizeof(OzWork) * nwork, cudaMemcpyHostToDevice, st));
-  if (!amax_ready) {
-    VGG_CUDA_CHECK(cudaMemsetAsync(amax, 0, sizeof(unsigned long long) * Dpad, st));
+  VGG_CUDA_CHECK(cudaMemsetAsync(amax, 0, sizeof(unsigned long long) * Dpad, st));
+  {
     const int ksplit = 64;
     const int k_per = (Kpad + ksplit - 1) / ksplit;
     oz_rowmax_kernel<<<dim3(Dpad / 128, ksplit), 128, 0, st>>>(Kpad, Dpad, k_per, Zt, amax);
@@ -571,7 +493,7 @@ int vgg_syrk_ozaki(int Kpad, int Dpad, const double* Zt, double* Cmat, int slice
   using namespace vgg;
   g_launch_count = 0;
   VGG_REQUIRE(Zt && Cmat && workspace, "null pointer");
-  return launch_syrk_i8(Kpad, Dpad, Zt, Cmat, 0, slices, workspace, ws_bytes, static_cast<cudaStream_t>(stream), false);
+  return launch_syrk_i8(Kpad, Dpad, Zt, Cmat, 0, slices, workspace, ws_bytes, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"
