@@ -225,17 +225,6 @@ struct SyrkWork {
   int bi, bj, kb0, kb1;        // upper tile (row block bi <= column block bj), k blocks of 64 rows [kb0, kb1)
 };
 
-// d[16 x 8] += a[16 x 16] b[16 x 8]; lane (g = lane / 4, t = lane % 4) holds a[i] = A[g + 8 (i & 1)][t + 4 (i >> 1)],
-// b[j] = B[t + 4 j][g], d = (g, 2t), (g, 2t + 1), (g + 8, 2t), (g + 8, 2t + 1)
-__device__ __forceinline__ void dmma_m16n8k16(double (&d)[4], const double (&a)[8], const double (&b)[4]) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, "
-      "{%0,%1,%2,%3};"
-      : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
-      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]),
-        "d"(b[2]), "d"(b[3]));
-}
-
 __global__ void __launch_bounds__(SF_THREADS, 1)
     syrk_f64_kernel(const SyrkWork* __restrict__ work, int nwork, int Kpad, int Dpad, const double* __restrict__ Zt,
                     double* __restrict__ Cmat, ptrdiff_t mc_off, int fill_upper, const __grid_constant__ FabricDev fd) {

@@ -3,17 +3,19 @@
 // serial piece of a bundle-adjustment iteration: n = 2403 at 400 frames (bordered with the right-hand side), 4.6 GFLOP
 // of float64 whose cost is a dependency chain, not arithmetic.  128-column panels; per panel
 //   chol_panel_kernel   EVERY CTA re-factors the 128x128 diagonal block in shared memory (cta_chol128 below) with its
-//                       own 16 panel rows riding along, so no CTA waits for another one and the rows come out solved;
+//                       own xr panel rows riding along, so no CTA waits for another one and the rows come out solved;
 //                       it writes them back together with their transpose (the upper triangle ends up holding L^T,
 //                       which is what the backward substitution kernel, csrc/trsv.cu, streams row by row), then --
-//                       fused schedule -- waits for the eight CTAs that own block row k+1, loads those 128 rows and
-//                       applies this panel's update to its own rows of block column k+1 with DMMA + f64 REDs.  The
-//                       next panel kernel follows on the same stream.  <= 143 CTAs: one wave.
-//   chol_update_kernel  A22 -= P P^T on 64x64 tiles with mma.sync.m8n8k4.f64 (SASS DMMA) for block columns >= k+2, on a
-//                       low-priority side stream; one K half of both operands in shared memory at a time (68 KB) so that
-//                       its CTAs run NEXT TO the panel CTAs of the following step (152 KB) on the same SMs.
+//                       fused schedule -- waits for the CTAs that own block row k+1, loads those 128 rows and applies
+//                       this panel's update to its own rows of block column k+1 with DMMA + f64 REDs.  The next panel
+//                       kernel follows on the same stream.  Each CTA needs a whole SM's worth of shared memory, so xr
+//                       (16, 20, ... 32 rows) is chosen per panel such that the 1 + chunks CTAs fit on the device's SMs
+//                       in one wave: a second wave would repeat the whole POTRF128 on the critical path.
+//   chol_update_kernel  A22 -= P P^T on 64x64 tiles for block columns >= k+2, on low-priority side streams; one K half of
+//                       both operands in shared memory at a time (68 KB) so that its CTAs run NEXT TO the panel CTAs of
+//                       the following step (<= 155 KB with xr <= 20) on the same SMs.
+// Every MMA is mma.sync.m16n8k16.f64 (dmma_m16n8k16, full FP64 tensor rate on sm_90; m8n8k4 runs at half of it).
 // The whole launch sequence is captured once per (matrix, order) into a CUDA graph.  Switches for A/B runs:
-// VGG_CHOL_FUSE=0 (separate critical-path update kernel + panel on a side stream, the first r02 schedule),
 // VGG_CHOL_LOOKAHEAD=0 (everything in program order), VGG_CHOL_GRAPH=0, VGG_CHOL_LEAF=0.
 #include <stdlib.h>
 #include <algorithm>
@@ -26,15 +28,10 @@ namespace vgg {
 
 constexpr int CB = 128;       // panel width
 constexpr int CLD = 132;      // shared-memory row stride (doubles): rows 16-byte aligned, DMMA fragment loads conflict-free
-constexpr int C_RPC = 16;     // panel rows per CTA in the triangular solve
+constexpr int C_RPC = 16;     // panel rows per CTA riding along in the POTRF128: the least ...
+constexpr int C_RPC_MAX = 32; // ... and the most (the rank-32 update covers them with one 32-row tile)
 constexpr int CT = 64;        // trailing-update tile
 constexpr int C_THREADS = 256;
-
-__device__ __forceinline__ void chol_dmma(double& d0, double& d1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-               : "+d"(d0), "+d"(d1)
-               : "d"(a), "d"(b));
-}
 
 // Cholesky of the 128x128 block in shared memory Ls (row stride CLD) by the whole CTA (256 threads).  Lower triangle
 // in, L out (entries above the diagonal are left undefined).  dinv[j] = 1 / L[j][j].  Returns 0 or 1 + first bad pivot.
@@ -44,9 +41,10 @@ __device__ __forceinline__ void chol_dmma(double& d0, double& d1, double a, doub
 //     columns through shuffles, two pivots per step), (b) one thread per row below solves its 8 entries against the
 //     pre-scaled leaf, (c) rank-8 update of the REST OF THE SUB-PANEL only (<= 24 columns), two threads per row, by warps
 //     1..7 WHILE warp 0 already prepares and factors the next leaf (the pivot chain is the critical path);
-//   * after each sub-panel ONE rank-32 update of everything to its right with mma.sync.m8n8k4.f64 (DMMA), 32x16 warp
-//     tiles straight from the row-major block (row stride 132: conflict-free fragments), tiles handed out through a
-//     shared counter; warp 0 takes the tile with the next leaf first and factors it under the other warps' tiles.
+//   * after each sub-panel ONE rank-32 update of everything to its right with dmma_m16n8k16, 32x16 warp tiles straight
+//     from the row-major block (row stride 132 = 4 mod 16 doubles: lane (g, t) reads rows g and g+8 at columns t + 4e,
+//     conflict-free), tiles dealt round-robin; warp 0 takes the tile with the next leaf first and factors it under the
+//     other warps' tiles.
 // r02 one-CTA probe (tools/microbench.py chol128, cycles): 55.5 k with the first leaf -> 47.9 k (hardware f64 rsqrt seed,
 // two-pivot leaf, per-lane look-ahead prep, overlapped sub-panel leaves); floor from the FP64 pipe alone: ~13 k.
 // 1/sqrt(p) for normal p > 0: the hardware's double-precision seed (rsqrt.approx.ftz.f64 -> MUFU.RSQ64H, relative error
@@ -68,9 +66,9 @@ constexpr double CHOL_PMIN = 2.2250738585072014e-308;      // smallest normal do
 // LEAF selects the 8x8 leaf (0: one pivot per step, 1: two pivots per step); PROBE adds clock64 phase counters for
 // tools/microbench.py chol128 (threads 0 and 32 = warp 0 / warp 1; prof[warp][phase], see the MARK sites).
 //
-// xr (0 or C_RPC) extra rows stored right below the block (rows 128 .. 128+xr-1 of Ls) ride along: they take part in the
-// micro-panel solves and in the rank-8 / rank-32 updates, so when the block is factored they hold X = A_ik L^-T -- the
-// panel rows this CTA owns -- with no separate triangular solve afterwards (r02: that solve was a 128-step
+// xr (0 or C_RPC .. C_RPC_MAX) extra rows stored right below the block (rows 128 .. 128+xr-1 of Ls) ride along: they
+// take part in the micro-panel solves and in the rank-8 / rank-32 updates, so when the block is factored they hold
+// X = A_ik L^-T -- the panel rows this CTA owns -- with no separate triangular solve afterwards (r02: that solve was a 128-step
 // multiply/shuffle/FMA chain, ~3 us after every POTRF128, plus a transposing pass over the block to feed it).
 template <int LEAF, bool PROBE>
 __device__ __forceinline__ int cta_chol128(double* Ls, double* dinv, int* fail_sm, int tid, int xr,
@@ -338,7 +336,8 @@ __device__ __forceinline__ int cta_chol128(double* Ls, double* dinv, int* fail_s
     const int nrb = (CB - t0) / 32;                  // 32-row blocks: 3, 2, 1, 0
     if (nrb > 0) {
       const int ntile = nrb * (nrb + 1);             // sum over rb of (2 rb + 2) 16-column tiles
-      const int nxt = xr ? (CB - t0) / 16 : 0;       // 16 x 16 tiles of the ride-along rows (two 8-row MMA blocks)
+      const int nxt = xr ? (CB - t0) / 16 : 0;       // xr x 16 tiles of the ride-along rows (one or two 16-row MMA blocks)
+      const int rend = CB + xr;                      // rows >= rend are not in the buffer: their fragments read as zero
       const int g = lane >> 2, q = lane & 3;
       // warp 0 updates tile 0 (it holds the next sub-panel's first 8 x 8 block), then factors that block while warps
       // 1..7 work through the remaining tiles round-robin (r02 probe: the three unoverlapped leaves were 9 % of the
@@ -346,7 +345,7 @@ __device__ __forceinline__ int cta_chol128(double* Ls, double* dinv, int* fail_s
       // warp 0 then picks up a late tile after its leaf and becomes the straggler of the phase.
       bool leaf_pending = warp == 0;
       for (int t = warp == 0 ? 0 : warp; t < ntile + nxt; t += (warp == 0 ? ntile + nxt : C_THREADS / 32 - 1)) {
-        int R0, C0, nrow8 = 4;
+        int R0, C0, nrow16 = 2;
         if (t < ntile) {
           int rb = 0, cb = t;
           while (cb >= 2 * rb + 2) { cb -= 2 * rb + 2; ++rb; }
@@ -355,46 +354,54 @@ __device__ __forceinline__ int cta_chol128(double* Ls, double* dinv, int* fail_s
         } else {
           R0 = CB;
           C0 = t0 + (t - ntile) * 16;
-          nrow8 = 2;
+          nrow16 = (xr + 15) / 16;
         }
-        double c[4][2][2];
+        // 32 x 16 warp tile = two m16 x two n8 DMMA tiles, k = 32 in two steps
+        double c[2][2][4];
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < 2; ++i)
 #pragma unroll
-          for (int j = 0; j < 2; ++j) c[i][j][0] = c[i][j][1] = 0.0;
-        const double* arow = Ls + (R0 + g) * CLD + c32 + q;
-        const double* brow = Ls + (C0 + g) * CLD + c32 + q;
+          for (int j = 0; j < 2; ++j) c[i][j][0] = c[i][j][1] = c[i][j][2] = c[i][j][3] = 0.0;
 #pragma unroll
-        for (int k4 = 0; k4 < 8; ++k4) {
-          double a[4], b[2];
+        for (int kk = c32; kk < c32 + 32; kk += 16) {
+          double a[2][8], b[2][4];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) a[i] = (i < nrow8) ? arow[i * 8 * CLD + k4 * 4] : 0.0;
+          for (int j = 0; j < 2; ++j)
 #pragma unroll
-          for (int j = 0; j < 2; ++j) b[j] = brow[j * 8 * CLD + k4 * 4];
+            for (int e = 0; e < 4; ++e) b[j][e] = Ls[(C0 + j * 8 + g) * CLD + kk + q + 4 * e];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            if (i < nrow8) {                               // warp-uniform
+          for (int i = 0; i < 2; ++i) {
+            if (i < nrow16) {                              // warp-uniform
 #pragma unroll
-              for (int j = 0; j < 2; ++j) chol_dmma(c[i][j][0], c[i][j][1], a[i], b[j]);
+              for (int e = 0; e < 8; ++e) {
+                const int r = R0 + i * 16 + g + 8 * (e & 1);
+                a[i][e] = r < rend ? Ls[r * CLD + kk + q + 4 * (e >> 1)] : 0.0;
+              }
+#pragma unroll
+              for (int j = 0; j < 2; ++j) dmma_m16n8k16(c[i][j], a[i], b[j]);
             }
           }
         }
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          if (i >= nrow8) continue;
-          const int r = R0 + i * 8 + g;
+        for (int i = 0; i < 2; ++i) {
+          if (i >= nrow16) continue;
 #pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const int col = C0 + j * 8 + 2 * q;
-            if (col > r) continue;
-            double* pp = Ls + r * CLD + col;
-            if (col + 1 <= r) {
-              double2 v = *reinterpret_cast<double2*>(pp);
-              v.x -= c[i][j][0];
-              v.y -= c[i][j][1];
-              *reinterpret_cast<double2*>(pp) = v;
-            } else {
-              *pp -= c[i][j][0];
+          for (int h = 0; h < 2; ++h) {
+            const int r = R0 + i * 16 + g + 8 * h;
+            if (r >= rend) continue;
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              const int col = C0 + j * 8 + 2 * q;
+              if (col > r) continue;
+              double* pp = Ls + r * CLD + col;
+              if (col + 1 <= r) {
+                double2 v = *reinterpret_cast<double2*>(pp);
+                v.x -= c[i][j][2 * h];
+                v.y -= c[i][j][2 * h + 1];
+                *reinterpret_cast<double2*>(pp) = v;
+              } else {
+                *pp -= c[i][j][2 * h];
+              }
             }
           }
         }
@@ -440,8 +447,9 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol128_probe_kernel(const doubl
   for (int e = tid; e < CB * CB; e += C_THREADS) L[e] = ((e & 127) <= (e >> 7)) ? cp_smem[(e >> 7) * CLD + (e & 127)] : 0.0;
 }
 
-// grid.x = 1 + number of 16-row chunks below the diagonal block; block 256.  Every CTA factors the diagonal block
-// redundantly with its own 16 panel rows riding along (xr = C_RPC), so those rows come out solved.  CTA 0 stores the
+// grid.x = 1 + number of xr-row chunks below the diagonal block; block 256; dynamic shared memory (128 + xr) rows of CLD
+// doubles.  Every CTA factors the diagonal block redundantly with its own xr panel rows riding along, so those rows come
+// out solved.  CTA 0 stores the
 // factored block: L^T into the strict upper triangle in place (nobody reads it), L itself into the side buffer Ldiag --
 // the other CTAs of this launch may still be loading the unfactored block; CTA 0 of the NEXT panel's launch moves it
 // into place (the last panel, a single CTA, writes its block directly).
@@ -450,7 +458,7 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol128_probe_kernel(const doubl
 //   A[r0.., t0..t0+127] -= X P^T,   X = its solved rows,  P = L[t0..t0+127][k0..k0+127]  (block row k+1 of the panel),
 // so that column is complete when the kernel ends and the next panel kernel can follow directly (r02: the separate
 // critical-path update kernel and its two cross-stream graph edges cost ~12 us per panel step on top of the ~9 us the
-// kernel ran).  P is produced by CTAs 1..8 of this launch: they publish their rows (fence + flags[panel]++), everyone
+// kernel ran).  P is produced by CTAs 1..ceil(128 / xr) of this launch: they publish their rows (fence + flags[panel]++), everyone
 // spins on the counter (bounded), then loads P through L2.  A CTA only ever waits for lower-numbered CTAs, which the
 // hardware dispatched before it, so the wait cannot deadlock even when the grid is not co-resident.  The subtraction
 // uses f64 REDs: the trailing-update kernel of the PREVIOUS panel may still be adding into the same tiles.
@@ -461,22 +469,25 @@ template <int LEAF>
 __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda, int k0, double* __restrict__ A,
                                                                    double* __restrict__ Ldiag /*[nblk][128*128]*/,
                                                                    int* __restrict__ info, int* __restrict__ flags,
-                                                                   int fuse, int band_end, int arrow_lo) {
+                                                                   int fuse, int band_end, int arrow_lo, int xr) {
   // Rows below the diagonal block that can be non-zero in this block column: [k0+128, band_end) and [arrow_lo, n)
-  // (band_end = arrow_lo = n: everything, the dense case).  The CTAs cover exactly these rows, 16 each.
+  // (band_end = arrow_lo = n: everything, the dense case).  The CTAs cover exactly these rows, xr each; a chunk ends
+  // early at the end of its range (nrows < xr), its remaining rows are zero.
   extern __shared__ __align__(16) double cp_smem[];
   double* Ls = cp_smem;                        // [128][CLD]
-  double* Ts = cp_smem + CB * CLD;             // [16][CLD]: rows 128.. of the same array (ride-along rows)
+  double* Ts = cp_smem + CB * CLD;             // [xr][CLD]: rows 128.. of the same array (ride-along rows)
   __shared__ double dinv[CB];
   __shared__ int fail_sm;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int nb = min(CB, n - k0);
   const bool solver = blockIdx.x > 0;
-  const int chunks1r = (max(0, min(band_end, n) - (k0 + CB)) + C_RPC - 1) / C_RPC;   // banded: band_end is a multiple of 128
+  const int band_hi = min(band_end, n);
+  const int chunks1r = (max(0, band_hi - (k0 + CB)) + xr - 1) / xr;
   const int cidx = (int)blockIdx.x - 1;
-  const int r0 = cidx < chunks1r ? k0 + CB + cidx * C_RPC : arrow_lo + (cidx - chunks1r) * C_RPC;
+  const int r0 = cidx < chunks1r ? k0 + CB + cidx * xr : arrow_lo + (cidx - chunks1r) * xr;
+  const int nrows = solver ? min(xr, (cidx < chunks1r ? band_hi : n) - r0) : 0;
   // diagonal block (rows < nb: whole 128-double rows, the part above the diagonal is never read; identity padding
-  // beyond nb) and this CTA's 16 panel rows: cp.async, all 16-byte chunks in flight at once (r02: the plain
+  // beyond nb) and this CTA's xr panel rows: cp.async, all 16-byte chunks in flight at once (r02: the plain
   // load -> store loop serialised 32 L2 round trips per thread, a third of the kernel)
   for (int e = tid; e < CB * (CB / 2); e += C_THREADS) {
     const int i = e >> 6, j = (e & 63) * 2;
@@ -486,15 +497,15 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
       *reinterpret_cast<double2*>(Ls + i * CLD + j) = make_double2(j == i ? 1.0 : 0.0, j + 1 == i ? 1.0 : 0.0);
     }
   }
-  for (int e = tid; e < C_RPC * (CB / 2); e += C_THREADS) {
+  for (int e = tid; e < xr * (CB / 2); e += C_THREADS) {
     const int r = e >> 6, j = (e & 63) * 2;
-    if (solver && r0 + r < n) cp_async16(Ts + r * CLD + j, A + (size_t)(r0 + r) * lda + k0 + j);
+    if (r < nrows) cp_async16(Ts + r * CLD + j, A + (size_t)(r0 + r) * lda + k0 + j);
     else *reinterpret_cast<double2*>(Ts + r * CLD + j) = make_double2(0.0, 0.0);
   }
   cp_async_commit();
   cp_async_wait<0>();
   __syncthreads();
-  const int fail = cta_chol128<LEAF, false>(Ls, dinv, &fail_sm, tid, C_RPC);
+  const int fail = cta_chol128<LEAF, false>(Ls, dinv, &fail_sm, tid, xr);
   if (fail && blockIdx.x == 0 && tid == 0) atomicCAS(info, 0, k0 + fail);
   if (!solver) {
     // the last panel has no other CTA that could still be loading the block: its factor goes straight into place
@@ -532,14 +543,14 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
     return;
   }
   // row-major store of the solved rows ...
-  for (int e = tid; e < C_RPC * CB; e += C_THREADS) {
+  for (int e = tid; e < nrows * CB; e += C_THREADS) {
     const int r = e >> 7, c = e & 127;
-    if (r0 + r < n && c < nb) A[(size_t)(r0 + r) * lda + k0 + c] = Ts[r * CLD + c];
+    if (c < nb) A[(size_t)(r0 + r) * lda + k0 + c] = Ts[r * CLD + c];
   }
-  // ... and their transpose into the upper triangle (16 consecutive doubles = one 128-byte segment per column c)
-  for (int e = tid; e < C_RPC * CB; e += C_THREADS) {
-    const int c = e >> 4, r = e & 15;
-    if (r0 + r < n && c < nb) A[(size_t)(k0 + c) * lda + r0 + r] = Ts[r * CLD + c];
+  // ... and their transpose into the upper triangle (nrows consecutive doubles per column c)
+  for (int e = tid; e < nrows * CB; e += C_THREADS) {
+    const int c = e / nrows, r = e - c * nrows;
+    if (c < nb) A[(size_t)(k0 + c) * lda + r0 + r] = Ts[r * CLD + c];
   }
   if (!fuse) return;
 
@@ -548,7 +559,7 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
   // CTAs 1..nprod own block row k+1 (the band's first block, or the arrow block when it is the next one); a block
   // row that is structurally zero in this column has no producers and there is nothing to subtract
   const bool p_active = band_end > t0 || arrow_lo == t0;
-  const int nprod = p_active ? min(CB / C_RPC, (int)gridDim.x - 1) : 0;
+  const int nprod = p_active ? min((CB + xr - 1) / xr, (int)gridDim.x - 1) : 0;
   if (nprod == 0) return;
   int* flag = flags + k0 / CB;
   __threadfence();
@@ -580,81 +591,83 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
     cp_async_commit();
   }
   {
+    // warp w: the xr rows x columns t0 + 16 w .. +15, i.e. one or two m16 x two n8 DMMA tiles, k = 128
     const int g = lane >> 2, q = lane & 3;
-    double c[2][2][2];
+    const int nrow16 = (xr + 15) / 16;
+    double c[2][2][4];
 #pragma unroll
     for (int i = 0; i < 2; ++i)
 #pragma unroll
-      for (int j = 0; j < 2; ++j) c[i][j][0] = c[i][j][1] = 0.0;
-    const double* arow = Ts + g * CLD + q;
-    const double* brow = Ls + (warp * 16 + g) * CLD + q;
+      for (int j = 0; j < 2; ++j) c[i][j][0] = c[i][j][1] = c[i][j][2] = c[i][j][3] = 0.0;
 #pragma unroll
     for (int half = 0; half < 2; ++half) {
       if (half == 0) cp_async_wait<1>();
       else cp_async_wait<0>();
       __syncthreads();
-#pragma unroll 4
-      for (int k4 = half * 16; k4 < half * 16 + 16; ++k4) {
-        double a[2], b[2];
+#pragma unroll 2
+      for (int kk = half * 64; kk < half * 64 + 64; kk += 16) {
+        double a[2][8], b[2][4];
 #pragma unroll
-        for (int i = 0; i < 2; ++i) a[i] = arow[i * 8 * CLD + k4 * 4];
+        for (int j = 0; j < 2; ++j)
 #pragma unroll
-        for (int j = 0; j < 2; ++j) b[j] = brow[j * 8 * CLD + k4 * 4];
+          for (int e = 0; e < 4; ++e) b[j][e] = Ls[(warp * 16 + j * 8 + g) * CLD + kk + q + 4 * e];
 #pragma unroll
-        for (int i = 0; i < 2; ++i)
+        for (int i = 0; i < 2; ++i) {
+          if (i < nrow16) {                              // warp-uniform
 #pragma unroll
-          for (int j = 0; j < 2; ++j) chol_dmma(c[i][j][0], c[i][j][1], a[i], b[j]);
+            for (int e = 0; e < 8; ++e) {
+              const int r = i * 16 + g + 8 * (e & 1);
+              a[i][e] = r < xr ? Ts[r * CLD + kk + q + 4 * (e >> 1)] : 0.0;
+            }
+#pragma unroll
+            for (int j = 0; j < 2; ++j) dmma_m16n8k16(c[i][j], a[i], b[j]);
+          }
+        }
       }
     }
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      const int r = r0 + i * 8 + g;
-      if (r >= n) continue;
 #pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int col = t0 + warp * 16 + j * 8 + 2 * q;
-        double* p = A + (size_t)r * lda + col;
-        if (col <= r) atomicAdd(p, -c[i][j][0]);
-        if (col + 1 <= r) atomicAdd(p + 1, -c[i][j][1]);
+      for (int h = 0; h < 2; ++h) {
+        const int rr = i * 16 + g + 8 * h;
+        if (i >= nrow16 || rr >= nrows) continue;
+        const int r = r0 + rr;
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int col = t0 + warp * 16 + j * 8 + 2 * q;
+          double* p = A + (size_t)r * lda + col;
+          if (col <= r) atomicAdd(p, -c[i][j][2 * h]);
+          if (col + 1 <= r) atomicAdd(p + 1, -c[i][j][2 * h + 1]);
+        }
       }
     }
   }
 }
 
-// A[t0.., t0..] -= P P^T (lower part), P = A[t0.., k0..k0+127].  Tiles of TM rows x 64 columns, 8 warps.
-//   TM = 64 (trailing update off the critical path): tile (bi, bj), bj <= bi, warps 2x4, warp tile 32x16; mode 2 = tile
-//            columns >= 2, mode 0 = all; mode 3 = mode 2 with f64 REDs on tile columns 2 and 3 (the block column the
-//            fused panel kernel of the next step is adding into at the same time); mode 4 = tile columns 2 and 3 only
-//            (REDs), mode 5 = tile columns >= 4 (REDs on 4 and 5): the two halves of mode 3 with different deadlines.
-//   TM = 32 (mode 1, the next panel's 128 columns = tile columns 0 and 1, ON the critical path): twice as many CTAs so
-//            the ~140 tiles of a 2400-row matrix fill the SMs with one short tile each; warps 1x8, warp tile 32x8.
-// Shared memory holds ONE K half (64 panel columns) of both operands at a time, row stride 68 doubles (fragment loads
-// conflict-free like stride 132): 68 KB per CTA instead of 135 KB, so an update CTA fits on an SM NEXT TO a panel CTA
-// (152 KB) and two or three fit on a free SM.  r02 launch list of the previous version (whole K resident, one CTA per
-// SM): the panel kernel's <= 143 latency-bound CTAs held their SMs for the whole step and the trailing update ran
-// after them, not beside them -- the factorisation took the SUM of all its kernels (0.90 ms).
+// A[t0.., t0..] -= P P^T (lower part), P = A[t0.., k0..k0+127]: one 64 x 64 tile (bi, bj), bj <= bi, per CTA; 8 warps
+// 2 x 4, warp tile 32 x 16 = two m16 x two n8 DMMA tiles.  Which tiles (tile columns counted from t0):
+//   CU_ALL   every tile (the program-order schedule, VGG_CHOL_LOOKAHEAD=0)
+//   CU_NEXT  tile columns 2 and 3 = block column k+2, which the fused panel kernel of the next step is adding into at
+//            the same time: f64 REDs
+//   CU_REST  tile columns >= 4 (REDs on 4 and 5: block column k+3 is shared with CU_NEXT of the next step)
+// all_red: banded matrices, whose tile columns no longer line up with block columns, write every tile with REDs.
+// Shared memory holds ONE K half (64 panel columns) of both operands at a time, row stride 68 doubles (= 4 mod 16, so
+// the m16n8k16 fragment loads are conflict-free like stride 132): 68 KB per CTA instead of 135 KB, so an update CTA fits
+// on an SM NEXT TO a panel CTA (<= 155 KB with xr <= 20) and two or three fit on a free SM.  r02 launch list of the
+// previous version (whole K resident, one CTA per SM): the panel kernel's latency-bound CTAs held their SMs for the
+// whole step and the trailing update ran after them, not beside them -- the factorisation took the SUM of all its kernels.
 constexpr int CUD = 68;
-template <int TM>
+enum { CU_ALL = 0, CU_NEXT = 1, CU_REST = 2 };
 __global__ void __launch_bounds__(C_THREADS, 2) chol_update_kernel(int n, int lda, int k0, int t0, int mode,
                                                                     double* __restrict__ A, int band_end, int arrow_lo,
-                                                                    int all_red, int ntiles) {
-  constexpr int WN = TM == 64 ? 4 : 8;            // warps along the 64 tile columns
-  constexpr int NJ = 64 / WN / 8;                 // 8-column MMA tiles per warp: 2 or 1
+                                                                    int all_red) {
   extern __shared__ __align__(16) double cu_smem[];
-  double* As = cu_smem;                         // [TM][CUD]
-  double* Bs = cu_smem + TM * CUD;              // [64][CUD]
-  // gridDim.x == ntiles: one tile per CTA (default); gridDim.x < ntiles (VGG_CHOL_PERSIST=1): a persistent CTA per SM walks
-  // the tiles, so that never more than one update CTA sits on an SM and a panel CTA of the next step always finds room.
-  // Measured r02: 0.920 ms against 0.890 -- one update CTA per SM hides its own latencies worse than it helps the panels.
-  for (int tile_t = blockIdx.x; tile_t < ntiles; tile_t += gridDim.x) {
+  double* As = cu_smem;                         // [64][CUD]
+  double* Bs = cu_smem + CT * CUD;              // [64][CUD]
   int bi, bj;
   {
-    int t = tile_t;
-    if (TM == 32) {
-      const int T = (n - t0 + 31) / 32;           // 32-row tiles; tile column 1 starts at row tile 2
-      if (t < T) { bi = t; bj = 0; }
-      else { bi = t - T + 2; bj = 1; }
-    } else if (mode == 4) {                         // tile columns 2 and 3 only (= block column k+2)
+    const int t = blockIdx.x;
+    if (mode == CU_NEXT) {
       const int T = (max(0, min(band_end, n) - t0) + 63) / 64 + (band_end >= n ? 0 : (n - arrow_lo + 63) / 64);
       if (t < T - 2) { bi = 2 + t; bj = 2; }
       else { bi = 3 + (t - (T - 2)); bj = 3; }
@@ -663,38 +676,38 @@ __global__ void __launch_bounds__(C_THREADS, 2) chol_update_kernel(int n, int ld
       while ((bi + 1) * (bi + 2) / 2 <= t) ++bi;
       while (bi * (bi + 1) / 2 > t) --bi;
       bj = t - bi * (bi + 1) / 2;
-      const int skip = mode == 5 ? 4 : (mode >= 2 ? 2 : 0);
+      const int skip = mode == CU_REST ? 4 : 0;
       bi += skip;
       bj += skip;
     }
   }
-  const bool diag = TM == 64 && bi == bj;
+  const bool diag = bi == bj;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   // banded matrices: 64-row tile v of the ACTIVE rows -- the band part [t0, band_end) first, then the arrow part
   // [arrow_lo, n) (band_end = n: the plain dense mapping)
   const int T1v = band_end >= n ? (1 << 30) : (band_end - t0) / 64;
   auto vrow = [&](int v) { return v < T1v ? t0 + v * 64 : arrow_lo + (v - T1v) * 64; };
-  const int ri = TM == 64 ? vrow(bi) : t0 + bi * TM, rj = TM == 64 ? vrow(bj) : t0 + bj * 64;
+  const int ri = vrow(bi), rj = vrow(bj);
   const double* bs = diag ? As : Bs;
-  const int wm = warp / WN, wn = warp % WN;
+  const int wm = warp / 4, wn = warp % 4;
   const int g = lane >> 2, q = lane & 3;
-  double c[4][NJ][2];
+  double c[2][2][4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i)
+  for (int i = 0; i < 2; ++i)
 #pragma unroll
-    for (int j = 0; j < NJ; ++j) c[i][j][0] = c[i][j][1] = 0.0;
+    for (int j = 0; j < 2; ++j) c[i][j][0] = c[i][j][1] = c[i][j][2] = c[i][j][3] = 0.0;
   const double* arow = As + (wm * 32 + g) * CUD + q;
-  const double* brow = bs + (wn * (8 * NJ) + g) * CUD + q;
+  const double* brow = bs + (wn * 16 + g) * CUD + q;
 #pragma unroll 1
   for (int half = 0; half < 2; ++half) {
     if (half) __syncthreads();                      // everyone is done with the first half's fragments
     // panel rows, row-major (k contiguous)
-    for (int e = tid; e < (TM + 64) * 16; e += C_THREADS) {
+    for (int e = tid; e < 2 * CT * 16; e += C_THREADS) {
       const int row = e >> 4, ch = (e & 15) * 4;     // 4 doubles (two 16-byte chunks) per thread-step
-      const bool isA = row < TM;
+      const bool isA = row < CT;
       if (!isA && diag) continue;
-      const int grow = isA ? ri + row : rj + (row - TM);
-      double* dst = (isA ? As + row * CUD : Bs + (row - TM) * CUD) + ch;
+      const int grow = isA ? ri + row : rj + (row - CT);
+      double* dst = (isA ? As + row * CUD : Bs + (row - CT) * CUD) + ch;
       if (grow < n) {
         const double* src = A + (size_t)grow * lda + k0 + half * 64 + ch;
         cp_async16(dst, src);
@@ -707,42 +720,49 @@ __global__ void __launch_bounds__(C_THREADS, 2) chol_update_kernel(int n, int ld
     cp_async_commit();
     cp_async_wait<0>();
     __syncthreads();
-#pragma unroll 4
-    for (int k4 = 0; k4 < 16; ++k4) {
-      double a[4], b[NJ];
+#pragma unroll 2
+    for (int kk = 0; kk < 64; kk += 16) {
+      double a[2][8], b[2][4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) a[i] = arow[i * 8 * CUD + k4 * 4];
+      for (int i = 0; i < 2; ++i)
 #pragma unroll
-      for (int j = 0; j < NJ; ++j) b[j] = brow[j * 8 * CUD + k4 * 4];
+        for (int e = 0; e < 8; ++e) a[i][e] = arow[(i * 16 + 8 * (e & 1)) * CUD + kk + 4 * (e >> 1)];
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
+      for (int j = 0; j < 2; ++j)
 #pragma unroll
-        for (int j = 0; j < NJ; ++j) chol_dmma(c[i][j][0], c[i][j][1], a[i], b[j]);
+        for (int e = 0; e < 4; ++e) b[j][e] = brow[j * 8 * CUD + kk + 4 * e];
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j) dmma_m16n8k16(c[i][j], a[i], b[j]);
     }
   }
+  const bool red = all_red || mode == CU_NEXT || (mode == CU_REST && bj < 6);
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = ri + wm * 32 + i * 8 + g;
-    if (r >= n) continue;
+  for (int i = 0; i < 2; ++i) {
 #pragma unroll
-    for (int j = 0; j < NJ; ++j) {
-      const int col = rj + wn * (8 * NJ) + j * 8 + 2 * q;
-      if (col > r) continue;                         // lower triangle only (col <= r < n)
-      double* p = A + (size_t)r * lda + col;
-      if (TM == 64 && (all_red || (mode == 3 && bj < 4) || mode == 4 || (mode == 5 && bj < 6))) {
-        atomicAdd(p, -c[i][j][0]);
-        if (col + 1 <= r) atomicAdd(p + 1, -c[i][j][1]);
-      } else if (col + 1 <= r) {
-        double2 v = *reinterpret_cast<double2*>(p);
-        v.x -= c[i][j][0];
-        v.y -= c[i][j][1];
-        *reinterpret_cast<double2*>(p) = v;
-      } else {
-        *p -= c[i][j][0];
+    for (int h = 0; h < 2; ++h) {
+      const int r = ri + wm * 32 + i * 16 + g + 8 * h;
+      if (r >= n) continue;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int col = rj + wn * 16 + j * 8 + 2 * q;
+        if (col > r) continue;                         // lower triangle only (col <= r < n)
+        double* p = A + (size_t)r * lda + col;
+        const double v0 = c[i][j][2 * h], v1 = c[i][j][2 * h + 1];
+        if (red) {
+          atomicAdd(p, -v0);
+          if (col + 1 <= r) atomicAdd(p + 1, -v1);
+        } else if (col + 1 <= r) {
+          double2 v = *reinterpret_cast<double2*>(p);
+          v.x -= v0;
+          v.y -= v1;
+          *reinterpret_cast<double2*>(p) = v;
+        } else {
+          *p -= v0;
+        }
       }
     }
-  }
-  __syncthreads();                                  // the next tile's loads overwrite the operand buffers
   }
 }
 
@@ -757,8 +777,8 @@ size_t chol_workspace_doubles(int n) {
 namespace {
 
 struct CholStreams {
-  cudaStream_t side = nullptr, side_lo = nullptr, side_mid = nullptr, cap = nullptr;
-  cudaEvent_t ev_col = nullptr, ev_panel = nullptr, ev_upd[2] = {nullptr, nullptr}, ev_bulk[3] = {nullptr, nullptr, nullptr};
+  cudaStream_t side_lo = nullptr, side_mid = nullptr, cap = nullptr;
+  cudaEvent_t ev_col = nullptr, ev_upd[2] = {nullptr, nullptr}, ev_bulk[3] = {nullptr, nullptr, nullptr};
   bool ready = false;
 };
 
@@ -770,12 +790,10 @@ int chol_streams(CholStreams** out) {
     // lo = least, hi = greatest priority.  The critical chain (panel steps) is captured on `cap` at the greatest
     // priority; the fused schedule's bulk updates go to side_lo at the least, so that a panel CTA is placed as soon as
     // an SM has room for it instead of queueing behind the remaining update CTAs.
-    VGG_CUDA_CHECK(cudaStreamCreateWithPriority(&s.side, cudaStreamNonBlocking, hi));
     VGG_CUDA_CHECK(cudaStreamCreateWithPriority(&s.side_lo, cudaStreamNonBlocking, lo));
     VGG_CUDA_CHECK(cudaStreamCreateWithPriority(&s.side_mid, cudaStreamNonBlocking, (lo + hi) / 2));
     VGG_CUDA_CHECK(cudaStreamCreateWithPriority(&s.cap, cudaStreamNonBlocking, hi));
     VGG_CUDA_CHECK(cudaEventCreateWithFlags(&s.ev_col, cudaEventDisableTiming));
-    VGG_CUDA_CHECK(cudaEventCreateWithFlags(&s.ev_panel, cudaEventDisableTiming));
     VGG_CUDA_CHECK(cudaEventCreateWithFlags(&s.ev_upd[0], cudaEventDisableTiming));
     VGG_CUDA_CHECK(cudaEventCreateWithFlags(&s.ev_upd[1], cudaEventDisableTiming));
     for (int i = 0; i < 3; ++i) VGG_CUDA_CHECK(cudaEventCreateWithFlags(&s.ev_bulk[i], cudaEventDisableTiming));
@@ -791,17 +809,26 @@ int chol_leaf() {
   return v;
 }
 
+// SMs of the current device, queried once: the panel kernel's grid is sized to fit them in one wave
+int chol_sms() {
+  static const int v = [] {
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+      sms = 0;
+    return sms > 0 ? sms : 132;
+  }();
+  return v;
+}
+
 int chol_set_attrs() {
   static bool done = false;
   if (done) return VGG_OK;
   VGG_CUDA_CHECK(cudaFuncSetAttribute(chol_panel_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)(sizeof(double) * (CB + C_RPC) * CLD)));
+                                      (int)(sizeof(double) * (CB + C_RPC_MAX) * CLD)));
   VGG_CUDA_CHECK(cudaFuncSetAttribute(chol_panel_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)(sizeof(double) * (CB + C_RPC) * CLD)));
-  VGG_CUDA_CHECK(cudaFuncSetAttribute(chol_update_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)(sizeof(double) * (CB + C_RPC_MAX) * CLD)));
+  VGG_CUDA_CHECK(cudaFuncSetAttribute(chol_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)(sizeof(double) * 2 * CT * CUD)));
-  VGG_CUDA_CHECK(cudaFuncSetAttribute(chol_update_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)(sizeof(double) * (32 + CT) * CUD)));
   done = true;
   return VGG_OK;
 }
@@ -817,36 +844,31 @@ int g_chol_arrow_blk = 0;
 
 namespace {
 
-// VGG_CHOL_FUSE=0 (A/B): the r02 schedule with a separate critical-path update kernel per panel
-bool chol_fuse() {
-  static const bool v = [] { const char* e = getenv("VGG_CHOL_FUSE"); return !(e && e[0] == '0'); }();
-  return v;
+// Ride-along rows per panel CTA for `rows` rows below the diagonal block (in `segs` separately chunked ranges): the
+// least multiple of 4 from C_RPC up such that the 1 + chunks CTAs, each needing a whole SM's shared memory, run in one
+// wave (a second wave repeats the whole POTRF128 on the critical path).  C_RPC_MAX is the most the POTRF128's
+// ride-along tiles cover; beyond it the grid takes a second wave.  Up to 20 rows a panel CTA (156 KB + 1.5 KB static +
+// 1 KB reserved) still shares an SM with one 68 KB update CTA within the 228 KB per SM.
+int chol_panel_rows(int below1, int below2, int* chunks) {
+  const int sms = chol_sms();
+  int xr = C_RPC;
+  for (;; xr += 4) {
+    *chunks = (below1 + xr - 1) / xr + (below2 + xr - 1) / xr;
+    if (1 + *chunks <= sms || xr >= C_RPC_MAX) return xr;
+  }
 }
 
-// The launch sequence on (st, side).
-//   fused (default): step(b) = panel b + its update of block column b+1, all on st back to back; the rest of panel b's
-//     trailing update (block columns >= b+2) runs on the side stream behind step(b) and has to be finished before
-//     step(b+2) -- it shares block column b+2 with step(b+1)'s fused update, both sides use REDs there.
-//   unfused lookahead: update<32>(b) [critical tiles] -> panel(b+1) on the side stream, update<64>(b) on st.
-//   lookahead == false: everything on st in program order.
+// The launch sequence on st (+ the side streams).
+//   lookahead (default): step(b) = panel b + its fused update of block column b+1, on st back to back; the rest of
+//     panel b's trailing update runs on the side streams behind step(b): U1(b) = block column b+2 (CU_NEXT, needed by
+//     step(b+2)) and U2(b) = block columns >= b+3 (CU_REST, needed by step(b+3)).
+//   lookahead == false: everything on st in program order (one CU_ALL update per panel, no fused update).
 int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags, cudaStream_t st, CholStreams* cs,
                  bool lookahead) {
   const int nblk = (n + CB - 1) / CB;
-  const size_t smem_p = sizeof(double) * (CB + C_RPC) * CLD;
   const size_t smem_u = sizeof(double) * 2 * CT * CUD;
-  const bool fuse = lookahead && chol_fuse();
-  static const int persist_ctas = [] {
-    const char* e = getenv("VGG_CHOL_PERSIST");
-    if (!(e && e[0] == '1')) return 0;
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    return sms;
-  }();
-  auto upd_grid = [&](int tiles) { return persist_ctas > 0 ? std::min(tiles, persist_ctas) : tiles; };
-  static const bool split = [] { const char* e = getenv("VGG_CHOL_SPLIT"); return !(e && e[0] == '0'); }();
-  // the band structure is honoured by the default (fused + split) schedule only; the A/B schedules treat the matrix as dense
-  const bool banded = fuse && split && (int)g_chol_band_end.size() >= nblk && g_chol_arrow_blk > 0;
+  // the band structure is honoured by the lookahead schedule only; the program-order schedule treats the matrix as dense
+  const bool banded = lookahead && (int)g_chol_band_end.size() >= nblk && g_chol_arrow_blk > 0;
   auto band_rows = [&](int b, int* band_end, int* arrow_lo) {
     if (!banded) {
       *band_end = *arrow_lo = n;
@@ -856,101 +878,75 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
     *arrow_lo = std::min(n, std::max(g_chol_arrow_blk * CB, *band_end));
     if (*band_end >= n || *arrow_lo <= *band_end) *band_end = *arrow_lo = n;      // no gap left: plain dense rows
   };
-  auto panel = [&](int b, cudaStream_t s2) -> int {
+  auto panel = [&](int b) -> int {
     const int k0 = b * CB;
-    int band_end, arrow_lo;
+    int band_end, arrow_lo, chunks;
     band_rows(b, &band_end, &arrow_lo);
     const int below1 = std::max(0, std::min(band_end, n) - (k0 + CB));
     const int below2 = band_end >= n ? 0 : n - arrow_lo;
-    const int chunks = (below1 + C_RPC - 1) / C_RPC + (below2 + C_RPC - 1) / C_RPC;
+    const int xr = chol_panel_rows(below1, below2, &chunks);
+    const size_t smem_p = sizeof(double) * (CB + xr) * CLD;
+    const int fuse = lookahead ? 1 : 0;
     if (chol_leaf() == 1)
-      chol_panel_kernel<1><<<1 + chunks, C_THREADS, smem_p, s2>>>(n, lda, k0, A, Ldiag, info, flags, fuse ? 1 : 0, band_end, arrow_lo);
+      chol_panel_kernel<1><<<1 + chunks, C_THREADS, smem_p, st>>>(n, lda, k0, A, Ldiag, info, flags, fuse, band_end, arrow_lo, xr);
     else
-      chol_panel_kernel<0><<<1 + chunks, C_THREADS, smem_p, s2>>>(n, lda, k0, A, Ldiag, info, flags, fuse ? 1 : 0, band_end, arrow_lo);
+      chol_panel_kernel<0><<<1 + chunks, C_THREADS, smem_p, st>>>(n, lda, k0, A, Ldiag, info, flags, fuse, band_end, arrow_lo, xr);
     VGG_LAUNCH_CHECK();
     return VGG_OK;
   };
   int rc;
-  if ((rc = panel(0, st))) return rc;
-  if (fuse) {
-    // Panel b's trailing update in two pieces with different deadlines: U1(b) = block column b+2 (needed by step(b+2),
-    // one step of slack, medium priority) and U2(b) = block columns >= b+3 (needed by step(b+3), two steps of slack,
-    // lowest priority).  r02: as ONE kernel with one step of slack the update of the first six panels did not fit
-    // next to the following step and 0.15 ms of it showed up on the critical path.
-    static const bool skip_bulk = getenv("VGG_CHOL_TIMING_SKIP_BULK") != nullptr;   // timing experiment only: WRONG factor
-    bool have_u1[2] = {false, false}, have_u2[3] = {false, false, false};
+  if ((rc = panel(0))) return rc;
+  if (!lookahead) {
     for (int b = 0; b + 1 < nblk; ++b) {
       const int k0 = b * CB, t0 = k0 + CB;
-      int band_end, arrow_lo;
-      band_rows(b, &band_end, &arrow_lo);
-      const int T = (std::max(0, std::min(band_end, n) - t0) + CT - 1) / CT + (band_end >= n ? 0 : (n - arrow_lo + CT - 1) / CT);
-      const int all_red = band_end >= n ? 0 : 1;     // banded: tile columns no longer map to consecutive block columns
-      const int n_u1 = T > 2 ? (T - 2) + (T > 3 ? T - 3 : 0) : 0;
-      const int n_u2 = T > 4 ? (T - 4) * (T - 3) / 2 : 0;
-      const int n_rest = T > 2 ? (T - 2) * (T - 1) / 2 : 0;
-      have_u1[b & 1] = false;
-      have_u2[b % 3] = false;
-      if (n_rest > 0 && !skip_bulk) {
-        VGG_CUDA_CHECK(cudaEventRecord(cs->ev_col, st));                 // step(b) done
-        if (split) {
-          VGG_CUDA_CHECK(cudaStreamWaitEvent(cs->side_mid, cs->ev_col, 0));
-          // U2(b-2) still writes block column b+2 with plain read-modify-writes (only its first block column uses REDs)
-          if (b >= 2 && have_u2[(b - 2) % 3]) VGG_CUDA_CHECK(cudaStreamWaitEvent(cs->side_mid, cs->ev_bulk[(b - 2) % 3], 0));
-          chol_update_kernel<64><<<upd_grid(n_u1), C_THREADS, smem_u, cs->side_mid>>>(n, lda, k0, t0, 4, A, band_end, arrow_lo, all_red, n_u1);
-          VGG_LAUNCH_CHECK();
-          VGG_CUDA_CHECK(cudaEventRecord(cs->ev_upd[b & 1], cs->side_mid));
-          have_u1[b & 1] = true;
-          if (n_u2 > 0) {
-            VGG_CUDA_CHECK(cudaStreamWaitEvent(cs->side_lo, cs->ev_col, 0));
-            chol_update_kernel<64><<<upd_grid(n_u2), C_THREADS, smem_u, cs->side_lo>>>(n, lda, k0, t0, 5, A, band_end, arrow_lo, all_red, n_u2);
-            VGG_LAUNCH_CHECK();
-            VGG_CUDA_CHECK(cudaEventRecord(cs->ev_bulk[b % 3], cs->side_lo));
-            have_u2[b % 3] = true;
-          }
-        } else {
-          VGG_CUDA_CHECK(cudaStreamWaitEvent(cs->side_lo, cs->ev_col, 0));
-          chol_update_kernel<64><<<upd_grid(n_rest), C_THREADS, smem_u, cs->side_lo>>>(n, lda, k0, t0, 3, A, n, n, 0, n_rest);
-          VGG_LAUNCH_CHECK();
-          VGG_CUDA_CHECK(cudaEventRecord(cs->ev_upd[b & 1], cs->side_lo));
-          have_u1[b & 1] = true;
-        }
-      }
-      // step(b+1) factors block column b+1: U1(b-1) (the last update of panel b-1 that touches it) and U2(b-2) must be done
-      if (b >= 1 && have_u1[(b - 1) & 1]) VGG_CUDA_CHECK(cudaStreamWaitEvent(st, cs->ev_upd[(b - 1) & 1], 0));
-      if (b >= 2 && have_u2[(b - 2) % 3]) VGG_CUDA_CHECK(cudaStreamWaitEvent(st, cs->ev_bulk[(b - 2) % 3], 0));
-      if ((rc = panel(b + 1, st))) return rc;
+      const int T = (n - t0 + CT - 1) / CT;
+      chol_update_kernel<<<T * (T + 1) / 2, C_THREADS, smem_u, st>>>(n, lda, k0, t0, CU_ALL, A, n, n, 0);
+      VGG_LAUNCH_CHECK();
+      if ((rc = panel(b + 1))) return rc;
     }
-    // join whatever the last two panels left on the side streams (capture needs every forked stream back)
-    for (int i = 0; i < 2; ++i)
-      if (have_u1[i]) VGG_CUDA_CHECK(cudaStreamWaitEvent(st, cs->ev_upd[i], 0));
-    for (int i = 0; i < 3; ++i)
-      if (have_u2[i]) VGG_CUDA_CHECK(cudaStreamWaitEvent(st, cs->ev_bulk[i], 0));
     return VGG_OK;
   }
+  // U1 gets one step of slack at medium priority, U2 two steps at the lowest.  r02: as ONE kernel with one step of
+  // slack the update of the first six panels did not fit next to the following step and 0.15 ms of it showed up on the
+  // critical path.
+  bool have_u1[2] = {false, false}, have_u2[3] = {false, false, false};
   for (int b = 0; b + 1 < nblk; ++b) {
     const int k0 = b * CB, t0 = k0 + CB;
-    const int T = (n - t0 + CT - 1) / CT;
-    const int T32 = (n - t0 + 31) / 32;
-    const int n_col = T32 + (T32 > 2 ? T32 - 2 : 0);       // 32-row tiles of tile columns 0 and 1
-    const int n_rest = T > 2 ? (T - 2) * (T - 1) / 2 : 0;
-    if (!lookahead) {
-      chol_update_kernel<64><<<upd_grid(T * (T + 1) / 2), C_THREADS, smem_u, st>>>(n, lda, k0, t0, 0, A, n, n, 0, T * (T + 1) / 2);
+    int band_end, arrow_lo;
+    band_rows(b, &band_end, &arrow_lo);
+    const int T = (std::max(0, std::min(band_end, n) - t0) + CT - 1) / CT + (band_end >= n ? 0 : (n - arrow_lo + CT - 1) / CT);
+    const int all_red = band_end >= n ? 0 : 1;     // banded: tile columns no longer map to consecutive block columns
+    const int n_u1 = T > 2 ? (T - 2) + (T > 3 ? T - 3 : 0) : 0;
+    const int n_u2 = T > 4 ? (T - 4) * (T - 3) / 2 : 0;
+    have_u1[b & 1] = false;
+    have_u2[b % 3] = false;
+    if (n_u1 > 0) {
+      VGG_CUDA_CHECK(cudaEventRecord(cs->ev_col, st));                 // step(b) done
+      VGG_CUDA_CHECK(cudaStreamWaitEvent(cs->side_mid, cs->ev_col, 0));
+      // U2(b-2) still writes block column b+2 with plain read-modify-writes (only its first block column uses REDs)
+      if (b >= 2 && have_u2[(b - 2) % 3]) VGG_CUDA_CHECK(cudaStreamWaitEvent(cs->side_mid, cs->ev_bulk[(b - 2) % 3], 0));
+      chol_update_kernel<<<n_u1, C_THREADS, smem_u, cs->side_mid>>>(n, lda, k0, t0, CU_NEXT, A, band_end, arrow_lo, all_red);
       VGG_LAUNCH_CHECK();
-      if ((rc = panel(b + 1, st))) return rc;
-      continue;
+      VGG_CUDA_CHECK(cudaEventRecord(cs->ev_upd[b & 1], cs->side_mid));
+      have_u1[b & 1] = true;
+      if (n_u2 > 0) {
+        VGG_CUDA_CHECK(cudaStreamWaitEvent(cs->side_lo, cs->ev_col, 0));
+        chol_update_kernel<<<n_u2, C_THREADS, smem_u, cs->side_lo>>>(n, lda, k0, t0, CU_REST, A, band_end, arrow_lo, all_red);
+        VGG_LAUNCH_CHECK();
+        VGG_CUDA_CHECK(cudaEventRecord(cs->ev_bulk[b % 3], cs->side_lo));
+        have_u2[b % 3] = true;
+      }
     }
-    chol_update_kernel<32><<<n_col, C_THREADS, sizeof(double) * (32 + CT) * CUD, st>>>(n, lda, k0, t0, 1, A, n, n, 0, n_col);
-    VGG_LAUNCH_CHECK();
-    VGG_CUDA_CHECK(cudaEventRecord(cs->ev_col, st));
-    VGG_CUDA_CHECK(cudaStreamWaitEvent(cs->side, cs->ev_col, 0));
-    if ((rc = panel(b + 1, cs->side))) return rc;
-    VGG_CUDA_CHECK(cudaEventRecord(cs->ev_panel, cs->side));
-    if (n_rest > 0) {
-      chol_update_kernel<64><<<upd_grid(n_rest), C_THREADS, smem_u, st>>>(n, lda, k0, t0, 2, A, n, n, 0, n_rest);
-      VGG_LAUNCH_CHECK();
-    }
-    VGG_CUDA_CHECK(cudaStreamWaitEvent(st, cs->ev_panel, 0));
+    // step(b+1) factors block column b+1: U1(b-1) (the last update of panel b-1 that touches it) and U2(b-2) must be done
+    if (b >= 1 && have_u1[(b - 1) & 1]) VGG_CUDA_CHECK(cudaStreamWaitEvent(st, cs->ev_upd[(b - 1) & 1], 0));
+    if (b >= 2 && have_u2[(b - 2) % 3]) VGG_CUDA_CHECK(cudaStreamWaitEvent(st, cs->ev_bulk[(b - 2) % 3], 0));
+    if ((rc = panel(b + 1))) return rc;
   }
+  // join whatever the last two panels left on the side streams (capture needs every forked stream back)
+  for (int i = 0; i < 2; ++i)
+    if (have_u1[i]) VGG_CUDA_CHECK(cudaStreamWaitEvent(st, cs->ev_upd[i], 0));
+  for (int i = 0; i < 3; ++i)
+    if (have_u2[i]) VGG_CUDA_CHECK(cudaStreamWaitEvent(st, cs->ev_bulk[i], 0));
   return VGG_OK;
 }
 

@@ -150,6 +150,18 @@ __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
+// FP64 tensor-core MMA at the full sm_90 rate (the m8n8k4 shape runs at half of it).
+// d[16 x 8] += a[16 x 16] b[16 x 8]; lane (g = lane / 4, t = lane % 4) holds a[i] = A[g + 8 (i & 1)][t + 4 (i >> 1)],
+// b[j] = B[t + 4 j][g], d = (g, 2t), (g, 2t + 1), (g + 8, 2t), (g + 8, 2t + 1)
+__device__ __forceinline__ void dmma_m16n8k16(double (&d)[4], const double (&a)[8], const double (&b)[4]) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, "
+      "{%0,%1,%2,%3};"
+      : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]),
+        "d"(b[2]), "d"(b[3]));
+}
+
 // Warp reduce-scatter: every lane contributes v[0..KP), KP a power of two <= 32.  Returns in lane l
 // the warp-wide sum of v[l & (KP-1)].  Costs KP-1 (+log2(32/KP)) 64-bit shuffles instead of 5*KP.
 template <int KP>
