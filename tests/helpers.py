@@ -21,6 +21,25 @@ def ba_case(S, N, camera_type, mode, seed=0, invisible_frac=0.2, noise_px=0.3):
                 uv=sc.tracks.astype(np.float64), mask=sc.mask, K=K, extra=extra)
 
 
+def banded_mask(S, N, life, seed, holes=0.2):
+    """Sequential (video-like) visibility: point n is born in a frame (births sorted, so storage order = creation
+    order) and seen for `life` to 1.5 `life` frames, with a fraction `holes` of those observations missing."""
+    rng = np.random.default_rng(seed)
+    m = np.zeros((S, N), dtype=bool)
+    births = np.sort(rng.integers(0, max(1, S - life // 2), size=N))        # creation order = storage order
+    for n, b in enumerate(births):
+        m[b:min(S, b + life + rng.integers(0, life // 2 + 1)), n] = True
+    m &= rng.uniform(size=m.shape) > holes
+    return m
+
+
+def banded_ba_case(S, N, camera_type, mode, life, seed=0, mask_seed=0):
+    """ba_case with a banded visibility mask: the scene's observations stay, only which of them are used changes."""
+    c = ba_case(S, N, camera_type, mode, seed=seed, invisible_frac=0.0)
+    c["mask"] = banded_mask(S, N, life, mask_seed)
+    return c
+
+
 def to_dev(a, dev, dtype=None):
     import torch
     t = torch.from_numpy(np.ascontiguousarray(a))

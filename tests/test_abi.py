@@ -36,6 +36,33 @@ def test_host_only_entry_points():
     assert o.max_num_iterations == 100 and o.gradient_tolerance == 1e-4
 
 
+def test_build_blocks_rejects_unaligned_tracks_per_warp():
+    """vgg_ba_build_blocks: tracks_per_warp must be 0 (choose) or a positive multiple of 4, else a warp's vectorised
+    observation loads would be misaligned.  The check comes before any CUDA call, so it needs no GPU: the buffers are
+    host memory of the right sizes that nothing may touch."""
+    import ctypes
+    import numpy as np
+    L = _lib.lib()
+    S, N = 2, 5
+    dc, ns = ctypes.c_int(), ctypes.c_int()
+    assert L.vgg_ba_dims(0, 1, ctypes.byref(dc), ctypes.byref(ns)) == 0
+    D = S * dc.value + ns.value
+    arrays = dict(uv=np.zeros((S, N, 2), np.float32), mask=np.ones((S, N), np.uint8), poses=np.zeros((S, 12)),
+                  intr=np.zeros((S, 4)), points=np.zeros((N, 3)))
+    outs = [np.zeros(8), np.zeros(S * L.vgg_ba_camrec_len(0, 1)), np.zeros(N * 3), np.zeros(N * 6),
+            np.zeros(N * (D + (D & 1)) * 3), np.zeros(8)]
+    p = _lib.BAProblem()
+    p.S, p.N, p.camera_model, p.intr_mode = S, N, 0, 1
+    for k, a in arrays.items():
+        setattr(p, k, a.ctypes.data)
+    sentinel = [o.copy() for o in outs]
+    for tpw in (-4, -1, 1, 2, 6, 30, 102):
+        rc = L.vgg_ba_build_blocks(ctypes.byref(p), *[o.ctypes.data for o in outs], tpw, None)
+        assert rc == -1, tpw                                         # VGG_EINVAL
+        assert b"tracks_per_warp" in L.vgg_last_error()
+    assert all(np.array_equal(a, b) for a, b in zip(outs, sentinel))
+
+
 def test_fails_loudly_without_the_library_or_a_gpu(monkeypatch, tmp_path):
     """No fallback path: a missing .so raises NativeLibraryMissing, CPU tensors raise, on every public entry."""
     import pytest

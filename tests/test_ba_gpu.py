@@ -3,6 +3,8 @@
 Tolerances: the kernels compute in float64 with a different summation order than numpy, so block
 sums are compared at 1e-10 relative; a whole LM solve (tens of Cholesky solves) at 1e-7 on the
 trajectory and 1e-6 on the final parameters (rotation geodesic in degrees, translation/point L2)."""
+import functools
+
 import numpy as np
 import pytest
 
@@ -21,21 +23,48 @@ CASES = [
 ]
 
 
+BLOCK_CASES = CASES + [
+    (45, 300, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME),    # frame group 1: nf = 13 frames of dc = 7 -> plain-store W path
+    (70, 1000, "SIMPLE_RADIAL", bo.INTR_SHARED),       # 3 frame groups
+    (33, 130, "SIMPLE_RADIAL", bo.INTR_PER_FRAME),     # frame group 1 has nf = 1
+    (70, 1001, "SIMPLE_PINHOLE", bo.INTR_SHARED),      # N % 4 != 0: scalar observation loads, several groups
+]
+
+
 def relerr(a, b):
     return np.abs(a - b).max() / max(1e-300, np.abs(b).max())
 
 
-@pytest.mark.parametrize("S,N,cam,mode", CASES)
-def test_blocks_match_oracle(cuda_dev, S, N, cam, mode):
-    import torch
-    from vggsfm_b200 import bundle_adjustment as ba
+@functools.lru_cache(maxsize=None)
+def _blocks_oracle(S, N, cam, mode):
     c = ba_case(S, N, cam, mode, seed=S + N)
     pconst = np.zeros(N, dtype=bool)
     pconst[::7] = True
     ref = bo.build_blocks(c["poses"], c["intr"], c["points"], c["uv"], c["mask"], c["model"], mode, pconst)
+    return c, pconst, ref
+
+
+@pytest.mark.parametrize("S,N,cam,mode", BLOCK_CASES)
+def test_blocks_match_oracle(cuda_dev, S, N, cam, mode):
+    """the library's own warp sizing (tracks_per_warp = 0)"""
+    _check_blocks(cuda_dev, S, N, cam, mode, 0)
+
+
+# 36 and 100 put warp chunk boundaries inside a 32-track point tile; 64 is the sizing of banded problems
+@pytest.mark.parametrize("tracks_per_warp", [4, 36, 64, 100])
+@pytest.mark.parametrize("S,N,cam,mode", BLOCK_CASES)
+def test_blocks_tracks_per_warp_match_oracle(cuda_dev, S, N, cam, mode, tracks_per_warp):
+    _check_blocks(cuda_dev, S, N, cam, mode, tracks_per_warp)
+
+
+def _check_blocks(cuda_dev, S, N, cam, mode, tracks_per_warp):
+    import torch
+    from vggsfm_b200 import bundle_adjustment as ba
+    c, pconst, ref = _blocks_oracle(S, N, cam, mode)
     out = ba.build_blocks(to_dev(c["uv"], cuda_dev, torch.float32), to_dev(c["mask"].astype(np.uint8), cuda_dev),
                           to_dev(c["poses"], cuda_dev), to_dev(c["intr"], cuda_dev), to_dev(c["points"], cuda_dev),
-                          c["model"], mode, point_const=to_dev(pconst.astype(np.uint8), cuda_dev))
+                          c["model"], mode, point_const=to_dev(pconst.astype(np.uint8), cuda_dev),
+                          tracks_per_warp=tracks_per_warp)
     torch.cuda.synchronize()
     dc, ns = bo.dims(c["model"], mode)
     g_c, H_cc, H_cs, g_s, H_ss = unpack_camrec(out["camrec"].cpu().numpy(), out["shared"].cpu().numpy(), S, dc, ns)

@@ -4,16 +4,7 @@ import numpy as np
 import pytest
 
 from oracle import band_oracle as bo
-
-
-def _banded_mask(S, N, life, seed, holes=0.2):
-    rng = np.random.default_rng(seed)
-    m = np.zeros((S, N), dtype=bool)
-    births = np.sort(rng.integers(0, max(1, S - life // 2), size=N))        # creation order = storage order
-    for n, b in enumerate(births):
-        m[b:min(S, b + life + rng.integers(0, life // 2 + 1)), n] = True
-    m &= rng.uniform(size=m.shape) > holes
-    return m
+from tests.helpers import banded_mask as _banded_mask
 
 
 @pytest.mark.parametrize("S,N,life,dc,ns,seed", [(160, 1400, 24, 6, 1, 0), (220, 2000, 40, 6, 2, 1), (130, 1100, 16, 7, 0, 2),

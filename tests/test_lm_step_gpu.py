@@ -1,0 +1,272 @@
+"""One LM iteration of vgg_ba_solve against the oracle's damped system at the start point.
+
+The whole-solve tests (test_ba_gpu.py, test_video_c5_gpu.py) compare costs, and Levenberg-Marquardt corrects itself: a
+wrong Schur complement, camera step or point step still reaches the same minimum, only in more iterations.  Here the
+solver runs ONE iteration from a perturbed start and the step it took is read back from the parameters it updated in
+place.  That step is checked in the FULL damped system (cameras and points, Jacobi-scaled variables, constant parameters
+and points removed, built by oracle/ba_oracle.py from the same blocks the oracle's own LM uses), by its normwise
+backward error
+
+    eta = |H d + g|_inf / (|H|_inf (|d|_inf + |u|_inf) + |g|_inf)  <=  1e-12,
+
+u being the rounding of the parameter update it was recovered from (2^-52 max(|old|, |new|) per entry).  A dropped
+coupling block or observation gives eta of 1e-4 or more; rounding gives about 1e-15.  Also checked: the initial cost,
+the model change and the step norm the solver reported (trace columns 3 and 6) at the recovered step, and the candidate
+cost (column 2) against the oracle's cost at the returned parameters.
+
+Banded (video-like) problems run with the band hint off (VGG_BAND=0), for the SYRK and factorisation only (VGG_BAND=2) and
+fully on (unset); each run is checked against the oracle on its own, and the hint the solver computed is read back through
+a development probe and compared with oracle/band_oracle.py table by table."""
+import ctypes
+
+import numpy as np
+import pytest
+
+from oracle import ba_oracle as bo
+from oracle import band_oracle
+from tests.helpers import ba_case, banded_ba_case, to_dev
+
+pytestmark = pytest.mark.gpu
+
+EPS = 2.0 ** -52
+RADIUS = 1e4                # initial_trust_region_radius of the default options
+MIN_DIAG, MAX_DIAG = 1e-6, 1e32
+
+
+def _so3_log(R):
+    """rotation vectors of [..., 3, 3] rotations, accurate for small angles"""
+    w = 0.5 * np.stack([R[..., 2, 1] - R[..., 1, 2], R[..., 0, 2] - R[..., 2, 0], R[..., 1, 0] - R[..., 0, 1]], -1)
+    s = np.linalg.norm(w, axis=-1)
+    th = np.arctan2(s, 0.5 * (np.trace(R, axis1=-2, axis2=-1) - 1.0))
+    return w * np.where(s > 0, th / np.where(s > 0, s, 1.0), 1.0)[..., None]
+
+
+def _recovered_step(old, new, S, dc, ns, model, mode):
+    """(camera step [D], its uncertainty [D], point step [N,3], its uncertainty [N,3]) from the parameters before and after
+    the iteration: R_new = Exp(2 delta) R_old, everything else additive."""
+    (p0, i0, x0), (p1, i1, x1) = old, new
+    D = S * dc + ns
+    d, u = np.zeros(D), np.zeros(D)
+    dcam, ucam = d[:S * dc].reshape(S, dc), u[:S * dc].reshape(S, dc)
+    R0, R1 = p0[:, :, :3], p1[:, :, :3]
+    dcam[:, 0:3] = 0.5 * _so3_log(R1 @ R0.transpose(0, 2, 1))
+    ucam[:, 0:3] = EPS * np.maximum(np.abs(R0).max(axis=(1, 2)), np.abs(R1).max(axis=(1, 2)))[:, None]
+    dcam[:, 3:6] = p1[:, :, 3] - p0[:, :, 3]
+    ucam[:, 3:6] = EPS * np.maximum(np.abs(p0[:, :, 3]), np.abs(p1[:, :, 3]))
+    for j, col in enumerate([0, 3][:bo.n_intr(model)]):
+        if mode == bo.INTR_PER_FRAME:
+            dcam[:, 6 + j] = i1[:, col] - i0[:, col]
+            ucam[:, 6 + j] = EPS * np.maximum(np.abs(i0[:, col]), np.abs(i1[:, col]))
+        elif mode == bo.INTR_SHARED:
+            d[S * dc + j] = i1[0, col] - i0[0, col]
+            u[S * dc + j] = EPS * max(abs(i0[0, col]), abs(i1[0, col]))
+    return d, u, x1 - x0, EPS * np.maximum(np.abs(x0), np.abs(x1))
+
+
+def _reference_system(c, param_const, point_const):
+    """The damped system of the first iteration in scaled variables (oracle/ba_oracle.py lm_solve): camera block A [D,D],
+    coupling B [D,N,3], point blocks V [N,3,3], gradients; rows and columns of constant parameters / points zeroed."""
+    S, N = c["mask"].shape
+    model, mode = c["model"], c["mode"]
+    dc, ns = bo.dims(model, mode)
+    blocks = bo.build_blocks_c if bo._load_c() is not None else bo.build_blocks
+    blk = blocks(c["poses"], c["intr"], c["points"], c["uv"], c["mask"], model, mode, point_const)
+    Hc, gc = bo._assemble_camera_system(blk, S, dc, ns)
+    W = bo._full_W(blk, S, dc, ns)
+    fc, fp = ~param_const, ~point_const
+    sc_c = 1.0 / (1.0 + np.sqrt(np.diag(Hc)))
+    sc_p = 1.0 / (1.0 + np.sqrt(np.einsum("nii->ni", blk["H_pp"])))
+    dcc = np.clip(np.diag(Hc) * sc_c * sc_c, MIN_DIAG, MAX_DIAG)
+    Hps = blk["H_pp"] * sc_p[:, :, None] * sc_p[:, None, :]
+    dpp = np.clip(np.einsum("nii->ni", Hps), MIN_DIAG, MAX_DIAG)
+    A = (Hc * np.outer(sc_c, sc_c) + np.diag(dcc / RADIUS)) * np.outer(fc, fc)
+    B = W * (sc_c * fc)[:, None, None] * (sc_p * fp[:, None])[None]
+    V = Hps + dpp[:, :, None] * np.eye(3) / RADIUS
+    return dict(cost=blk["cost"], gc=gc, gp=blk["g_p"], sc_c=sc_c, sc_p=sc_p, dcc=dcc, dpp=dpp, fc=fc, fp=fp, A=A,
+                B=B.reshape(A.shape[0], 3 * N), V=V, gcs=gc * sc_c * fc, gps=blk["g_p"] * sc_p * fp[:, None])
+
+
+def _backward_error(ref, dcs, ucs, dps, ups):
+    """normwise backward error of the scaled step (dcs [D], dps [N,3]) in the full damped system, evaluated blockwise"""
+    A, B, V, fc, fp = ref["A"], ref["B"], ref["V"], ref["fc"], ref["fp"]
+    N = V.shape[0]
+    rc = A @ dcs + B @ dps.reshape(-1) + ref["gcs"]
+    rp = (B.T @ dcs).reshape(N, 3) + np.einsum("nij,nj->ni", V, dps) + ref["gps"]
+    absB = np.abs(B)
+    row_c = np.abs(A).sum(1) + absB.sum(1)
+    row_p = absB.sum(0).reshape(N, 3) + np.abs(V).sum(2)
+    res = max(np.abs(rc[fc]).max(initial=0.0), np.abs(rp[fp]).max(initial=0.0))
+    normH = max(row_c[fc].max(initial=0.0), row_p[fp].max(initial=0.0))
+    nd = max(np.abs(dcs[fc]).max(initial=0.0), np.abs(dps[fp]).max(initial=0.0))
+    nu = max(np.abs(ucs[fc]).max(initial=0.0), np.abs(ups[fp]).max(initial=0.0))
+    ng = max(np.abs(ref["gcs"]).max(initial=0.0), np.abs(ref["gps"]).max(initial=0.0))
+    return res / (normH * (nd + nu) + ng)
+
+
+def _oracle_step(ref):
+    """the oracle's own scaled step (Schur complement + Cholesky) and the 2-norm condition number of the reduced matrix"""
+    A, B, V, fc = ref["A"], ref["B"], ref["V"], ref["fc"]
+    N = V.shape[0]
+    Vi = np.linalg.inv(V)
+    T = np.einsum("dnk,nkj->dnj", B.reshape(-1, N, 3), Vi).reshape(B.shape)
+    Sred = (A - T @ B.T)[np.ix_(fc, fc)]
+    b = (-ref["gcs"] + T @ ref["gps"].reshape(-1))[fc]
+    Lc = np.linalg.cholesky(Sred)
+    dcs = np.zeros(A.shape[0])
+    dcs[fc] = np.linalg.solve(Lc.T, np.linalg.solve(Lc, b))
+    dps = np.einsum("nij,nj->ni", Vi, -ref["gps"] - (B.T @ dcs).reshape(N, 3))
+    ev = np.linalg.eigvalsh(Sred)
+    return dcs, dps, ev[-1] / ev[0]
+
+
+def _band_record():
+    """the band hint of the most recent solve (vgg_dev_last_band_hint)"""
+    from vggsfm_b200 import _lib
+    L = _lib.lib()
+    meta = np.zeros(8, dtype=np.int32)
+    _lib.check(L.vgg_dev_last_band_hint(meta.ctypes.data, None, None, None, None), "vgg_dev_last_band_hint")
+    nb, KB, ng = int(meta[3]), int(meta[4]), int(meta[5])
+    rec = dict(active=bool(meta[0]), chol=bool(meta[1]), tables=bool(meta[2]), arrow_blk=int(meta[6]),
+               rb_range=np.zeros((nb, 2), np.int32), end_blk=np.zeros(nb, np.int32), kb_rows=np.zeros((KB, 2), np.int32),
+               fg_tracks=np.zeros((ng, 2), np.int32))
+    _lib.check(L.vgg_dev_last_band_hint(meta.ctypes.data, rec["rb_range"].ctypes.data, rec["end_blk"].ctypes.data,
+                                        rec["kb_rows"].ctypes.data, rec["fg_tracks"].ctypes.data), "vgg_dev_last_band_hint")
+    return rec
+
+
+def _check_band(c, band):
+    """banded problem: the hint the solver took equals band_oracle.band_tables; band None = dense expected"""
+    rec = _band_record()
+    if band is None:
+        assert not (rec["active"] or rec["chol"] or rec["tables"]), rec
+        return
+    dc, ns = bo.dims(c["model"], c["mode"])
+    t = band_oracle.band_tables(c["mask"], dc, ns)
+    if band == "0":
+        assert not (rec["active"] or rec["chol"] or rec["tables"]), rec
+        return
+    assert rec["active"] and rec["chol"], rec
+    assert rec["tables"] == (band == "1")
+    assert np.array_equal(rec["rb_range"], t["rb_range"])
+    assert np.array_equal(rec["end_blk"], t["end_blk"]) and rec["arrow_blk"] == t["arrow_blk"]
+    if band == "1":
+        assert np.array_equal(rec["kb_rows"], t["kb_rows"])
+        assert np.array_equal(rec["fg_tracks"], t["fg_tracks"])
+
+
+def _one_step(c, dev, param_const=None, point_const=None, label=""):
+    """run one LM iteration on the GPU and check it against the oracle's system; returns eta"""
+    import torch
+    from vggsfm_b200 import bundle_adjustment as ba
+    S, N = c["mask"].shape
+    model, mode = c["model"], c["mode"]
+    dc, ns = bo.dims(model, mode)
+    if param_const is None:
+        param_const = bo.default_param_const(S, model, mode)
+    if point_const is None:
+        point_const = np.zeros(N, dtype=bool)
+    poses, intr, pts = to_dev(c["poses"], dev), to_dev(c["intr"], dev), to_dev(c["points"], dev)
+    o = ba.default_options()
+    o.max_num_iterations = 1
+    o.function_tolerance = o.gradient_tolerance = o.parameter_tolerance = 0.0
+    s = ba.lm_solve(to_dev(c["uv"], dev, torch.float32), to_dev(c["mask"].astype(np.uint8), dev), poses, intr, pts, model,
+                    mode, param_const=to_dev(param_const.astype(np.uint8), dev),
+                    point_const=to_dev(point_const.astype(np.uint8), dev), options=o, want_trace=True)
+    new = (poses.cpu().numpy(), intr.cpu().numpy(), pts.cpu().numpy())
+    tr = s.trace.numpy()
+    assert s.iterations == 1 and tr[0, 7] == 1, (label, tr)            # the step was accepted
+    assert tr[0, 5] == RADIUS
+
+    ref = _reference_system(c, param_const, point_const)
+    assert abs(s.initial_cost - ref["cost"]) <= 1e-12 * ref["cost"], (label, s.initial_cost, ref["cost"])
+    d_c, u_c, d_p, u_p = _recovered_step((c["poses"], c["intr"], c["points"]), new, S, dc, ns, model, mode)
+    assert not d_c[param_const].any() and not d_p[point_const].any()
+    dcs, ucs = d_c / ref["sc_c"], u_c / ref["sc_c"]
+    dps, ups = d_p / ref["sc_p"], u_p / ref["sc_p"]
+    eta = _backward_error(ref, dcs, ucs, dps, ups)
+    # model change (oracle/ba_oracle.py lm_solve) and step norm at the recovered step
+    quad = (np.sum(dcs * dcs * ref["dcc"] / RADIUS * ref["fc"]) - np.sum(d_c * ref["gc"]) +
+            np.sum(dps * dps * ref["dpp"] / RADIUS * ref["fp"][:, None]) - np.sum(d_p * ref["gp"]))
+    model_change = 0.5 * quad
+    step_norm = np.sqrt(np.sum(d_c * d_c) + np.sum(d_p * d_p))
+    c_cost = bo.cost_only(*new, c["uv"], c["mask"], model)
+    ref_dcs, ref_dps, kappa = _oracle_step(ref)
+    fwd = max(np.abs(dcs - ref_dcs).max(), np.abs(dps - ref_dps).max()) / max(np.abs(ref_dcs).max(), np.abs(ref_dps).max())
+    print(f"lm step {label}: eta = {eta:.2e}  forward error vs oracle step = {fwd:.2e}  kappa2(reduced) = {kappa:.2e}  "
+          f"model change {abs(tr[0, 3] / model_change - 1):.1e}  step norm {abs(tr[0, 6] / step_norm - 1):.1e}  "
+          f"candidate cost {abs(tr[0, 2] / c_cost - 1):.1e}")
+    assert eta <= 1e-12, (label, eta)
+    assert abs(tr[0, 3] - model_change) <= 1e-10 * abs(model_change), (label, tr[0, 3], model_change)
+    assert abs(tr[0, 6] - step_norm) <= 1e-10 * step_norm, (label, tr[0, 6], step_norm)
+    assert abs(tr[0, 2] - c_cost) <= 1e-12 * c_cost, (label, tr[0, 2], c_cost)
+    return eta
+
+
+def _dense_case(name):
+    if name == "8x256":          # D = 56: one trsv block, factorisation order 57
+        return ba_case(8, 256, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME, seed=21), None, None
+    if name == "64x1000":        # D = 448 = 7 x 64: the last trsv block is full
+        return ba_case(64, 1000, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME, seed=22), None, None
+    if name == "45x700":         # frame group 1 has nf = 13 frames of dc = 7: W goes out with plain stores
+        c = ba_case(45, 700, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME, seed=23)
+        const_pose = np.zeros(45, dtype=bool)
+        const_pose[40] = True
+        pc = bo.default_param_const(45, c["model"], c["mode"], const_pose=const_pose)
+        ptc = np.zeros(700, dtype=bool)
+        ptc[::7] = True
+        return c, pc, ptc
+    if name == "C3":             # the benchmark configuration
+        return ba_case(400, 4096, "SIMPLE_RADIAL", bo.INTR_SHARED, seed=0, invisible_frac=0.0), None, None
+    raise KeyError(name)
+
+
+def _banded_case(name, mask_seed=0):
+    if name == "160x4003":
+        # partial last k block (3 N % 64 != 0) and partial last 32-track z_build tile; frame 77 sees nothing, point 1234
+        # is seen by no frame, and point 5 is also seen by the last 3 frames (one long track widens the ranges)
+        c = banded_ba_case(160, 4003, "SIMPLE_RADIAL", bo.INTR_SHARED, life=24, seed=31, mask_seed=mask_seed)
+        c["mask"][77] = False
+        c["mask"][:, 1234] = False
+        c["mask"][-3:, 5] = True
+        return c
+    if name == "130x2500":       # dc = 7: frames straddle the 128-row blocks; no shared columns
+        return banded_ba_case(130, 2500, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME, life=20, seed=32, mask_seed=mask_seed)
+    if name == "128x2048":       # S dc = 768: the arrow starts exactly at a block boundary, ns = 0
+        return banded_ba_case(128, 2048, "SIMPLE_RADIAL", bo.INTR_CONST, life=20, seed=33, mask_seed=mask_seed)
+    raise KeyError(name)
+
+
+@pytest.mark.parametrize("name", ["8x256", "64x1000", "45x700", "C3"])
+def test_dense_step_matches_oracle(cuda_dev, monkeypatch, name):
+    monkeypatch.delenv("VGG_BAND", raising=False)
+    c, pc, ptc = _dense_case(name)
+    _one_step(c, cuda_dev, pc, ptc, label=name)
+    _check_band(c, None)
+
+
+@pytest.mark.parametrize("band", ["0", "2", "1"])
+@pytest.mark.parametrize("name", ["160x4003", "130x2500", "128x2048"])
+def test_banded_step_matches_oracle(cuda_dev, monkeypatch, name, band):
+    """band "1" = VGG_BAND unset (every band skip on)"""
+    if band == "1":
+        monkeypatch.delenv("VGG_BAND", raising=False)
+    else:
+        monkeypatch.setenv("VGG_BAND", band)
+    c = _banded_case(name)
+    _one_step(c, cuda_dev, label=f"{name} VGG_BAND={band}")
+    _check_band(c, band)
+
+
+def test_back_to_back_band_dense_band(cuda_dev, monkeypatch):
+    """One process, one workspace: banded, then dense, then banded with another mask (a new hint): the workspace cache,
+    the SYRK work-list cache and the thread-local band tables must follow."""
+    monkeypatch.delenv("VGG_BAND", raising=False)
+    c = _banded_case("160x4003", mask_seed=0)
+    _one_step(c, cuda_dev, label="160x4003 first")
+    _check_band(c, "1")
+    c, pc, ptc = _dense_case("45x700")
+    _one_step(c, cuda_dev, pc, ptc, label="45x700 between")
+    _check_band(c, None)
+    c = _banded_case("160x4003", mask_seed=7)
+    _one_step(c, cuda_dev, label="160x4003 second mask")
+    _check_band(c, "1")

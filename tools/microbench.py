@@ -95,7 +95,7 @@ if mode == "trsv":
     nb = (n + 63) // 64
     st = np.zeros(6 * nb, dtype=np.int64)
     for _ in range(3):
-        _lib.check(L.vgg_dev_trsv_probe(n, lda, Ad.data_ptr(), yd.data_ptr(), xd.data_ptr(), st.ctypes.data), "probe")
+        _lib.check(L.vgg_dev_trsv_probe(n, lda, Ad.data_ptr(), yd.data_ptr(), 1, xd.data_ptr(), st.ctypes.data), "probe")
     x = xd.cpu().numpy()
     print(f"[{tag}] trsv n={n}: |Ux-y|/|y| = {np.linalg.norm(U @ x - y) / np.linalg.norm(y):.2e}")
     ent, lod, inv, see, pub, rhs = st[0::6], st[1::6], st[2::6], st[3::6], st[4::6], st[5::6]

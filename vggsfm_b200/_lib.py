@@ -26,7 +26,8 @@ EXPORTS = [
 
 
 # development probes (csrc/dev_probes.h): exported, not part of the public header
-DEV_EXPORTS = ["vgg_dev_blocks_timing", "vgg_dev_blocks_last_ms", "vgg_dev_chol128_probe", "vgg_dev_set_syrk_ranges", "vgg_dev_syrk_f64", "vgg_dev_trsv_probe", "vgg_dev_set_chol_band"]
+DEV_EXPORTS = ["vgg_dev_blocks_timing", "vgg_dev_blocks_last_ms", "vgg_dev_chol128_probe", "vgg_dev_set_syrk_ranges", "vgg_dev_syrk_f64", "vgg_dev_trsv_probe", "vgg_dev_set_chol_band",
+               "vgg_dev_last_band_hint"]
 
 
 class BAProblem(ctypes.Structure):
@@ -144,8 +145,9 @@ def lib() -> ctypes.CDLL:
     L.vgg_dev_chol128_probe.argtypes = [ci, ci, vp, vp, vp]
     L.vgg_dev_set_syrk_ranges.argtypes = [vp, ci]
     L.vgg_dev_syrk_f64.argtypes = [ci, ci, vp, vp, vp]
-    L.vgg_dev_trsv_probe.argtypes = [ci, ci, vp, vp, vp, vp]
+    L.vgg_dev_trsv_probe.argtypes = [ci, ci, vp, vp, cs, vp, vp]
     L.vgg_dev_set_chol_band.argtypes = [vp, ci, ci]
+    L.vgg_dev_last_band_hint.argtypes = [vp, vp, vp, vp, vp]
     L.vgg_syrk_ozaki.argtypes = [ci, ci, vp, vp, ci, vp, cs, vp]
     L.vgg_cholesky_lower.argtypes = [ci, ci, vp, vp, cs, ctypes.POINTER(ci), vp]
     L.vgg_tri_workspace_bytes.argtypes = [ci, ci, ci, ci, ctypes.POINTER(cs)]

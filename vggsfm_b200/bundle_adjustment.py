@@ -121,7 +121,8 @@ def _problem(uv, mask, poses, intr, points, model, mode, param_const, point_cons
 def build_blocks(uv, mask, poses, intr, points, model, mode, point_const=None, tracks_per_warp=0):
     """One launch of the fused residual+Jacobian+block kernel (vgg_ba_build_blocks).  Returns a dict of
     device tensors: cost[1], camrec[S,KR], g_p[N,3], H_pp[N,6], W[N,pitch,3] (track-major, pitch = D rounded
-    up to even), shared[8]."""
+    up to even), shared[8].  ``tracks_per_warp``: 0 lets the library choose; otherwise a positive multiple of 4
+    (the kernel loads the observations of 4 tracks at a time), anything else raises."""
     L = _lib.lib()
     S, N = mask.shape
     dc, ns = dims(model, mode)

@@ -11,6 +11,7 @@
 #include <map>
 #include <vector>
 #include "common.cuh"
+#include "dev_probes.h"
 
 namespace vgg {
 
@@ -25,7 +26,7 @@ void set_error(const char* fmt, ...) {
 
 // kernels (ba_blocks.cu / ba_schur.cu)
 int ba_build_blocks(const vgg_ba_problem* p, double* cost, double* camrec, double* g_p, double* H_pp, double* W,
-                    double* shared_out, int frames_per_cta, cudaStream_t stream, bool outputs_zeroed = false);
+                    double* shared_out, int tracks_per_warp, cudaStream_t stream, bool outputs_zeroed = false);
 int launch_jacobi_scale_points(int N, const double* H_pp, double* sc_p, int enable, cudaStream_t st);
 int launch_jacobi_scale_cams(int D, const double* hdiag, double* sc_c, int enable, cudaStream_t st);
 int launch_point_prep(int N, const double* H_pp, const double* g_p, const double* sc_p, const uint8_t* point_const,
@@ -318,6 +319,15 @@ struct SolveGuard {
   }
 };
 
+// What compute_band_hint decided for the most recent solve, kept after SolveGuard has cleared the live globals
+// (vgg_dev_last_band_hint, csrc/dev_probes.h): the tests compare it with oracle/band_oracle.py
+struct BandRecord {
+  int nb = 0, KB = 0, ngroups = 0, arrow_blk = 0;
+  bool active = false, chol = false, tables = false;
+  std::vector<int> rb_range, end_blk, kb_rows, fg_tracks;
+};
+static thread_local BandRecord g_band_last;
+
 // first / last visible point of every frame (N / -1 when the frame sees nothing): the band structure of sequential
 // (video) problems, where a point lives for a few windows and the dense [S, N] grid is mostly masked out
 __global__ void __launch_bounds__(256) frame_point_range_kernel(int S, int N, const uint8_t* __restrict__ mask,
@@ -357,6 +367,11 @@ static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad
   const char* env = getenv("VGG_BAND");                 // read per solve so that a test can compare both paths in one process
   const bool off = env && env[0] == '0';
   const int S = prob->S, N = prob->N, nb = Dpad / 128, KB = (Kpad + 63) / 64;
+  BandRecord& rec = g_band_last;
+  rec = BandRecord{};
+  rec.nb = nb;
+  rec.KB = KB;
+  rec.ngroups = (S + 31) / 32;
   if (off || nb < 6 || N < 1024) return VGG_OK;
   static thread_local int* dev = nullptr;
   static thread_local int cap = 0;
@@ -399,6 +414,8 @@ static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad
     }
   if (kept < 0.7 * all) {
     g_syrk_kb_ranges = rg;
+    rec.active = true;
+    rec.rb_range = rg;
     // the same structure for the factorisation: block (i, b) of the reduced system is non-zero iff the k ranges of row
     // blocks i and b meet; the blocks from the first shared-intrinsics column on (and the bordered right-hand-side row)
     // are the dense "arrow".  end[b] = one past the last band block of column b, made non-decreasing (the envelope
@@ -425,6 +442,9 @@ static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad
       }
       g_chol_band_end = end;
       g_chol_arrow_blk = arrow;
+      rec.chol = true;
+      rec.end_blk = end;
+      rec.arrow_blk = arrow;
       // device tables for the kernels that walk the dense [frames, points] grid (VGG_BAND=2: SYRK/Cholesky hint only)
       if (!(env && env[0] == '2')) {
         const int ngroups = (S + 31) / 32;
@@ -463,6 +483,9 @@ static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad
         VGG_CUDA_CHECK(cudaMemcpyAsync(tdev, tab.data(), sizeof(int) * tab.size(), cudaMemcpyHostToDevice, st));
         VGG_CUDA_CHECK(cudaStreamSynchronize(st));           // pageable source
         g_band_dev = BandDev{tdev, tdev + 2 * nb, tdev + 2 * (nb + KB), arrow * 128};
+        rec.tables = true;
+        rec.kb_rows.assign(t_kb, t_kb + 2 * KB);
+        rec.fg_tracks.assign(t_fg, t_fg + 2 * ngroups);
       }
     }
   }
@@ -546,10 +569,12 @@ int vgg_ba_workspace_bytes(int S, int N, int camera_model, int intr_mode, size_t
 }
 
 int vgg_ba_build_blocks(const vgg_ba_problem* prob, double* cost, double* camrec, double* g_p, double* H_pp, double* W,
-                        double* shared_out, int frames_per_cta, void* stream) {
+                        double* shared_out, int tracks_per_warp, void* stream) {
   VGG_REQUIRE(prob && cost && camrec && g_p && H_pp && W && shared_out, "null pointer");
+  // a warp's first track t0 = chunk * tracks_per_warp + 4k is the 16-byte (uv) / 4-byte (mask) cp.async offset
+  VGG_REQUIRE(tracks_per_warp >= 0 && tracks_per_warp % 4 == 0, "tracks_per_warp must be 0 (choose) or a multiple of 4");
   g_launch_count = 0;
-  return ba_build_blocks(prob, cost, camrec, g_p, H_pp, W, shared_out, frames_per_cta, (cudaStream_t)stream);
+  return ba_build_blocks(prob, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, (cudaStream_t)stream);
 }
 
 int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double* g_p, const double* H_pp,
@@ -1017,6 +1042,22 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
   summary->final_radius = radius;
   summary->device_ms = ms;
   summary->kernel_launches = g_launch_count;
+  return VGG_OK;
+}
+
+/* development probe (csrc/dev_probes.h): the band hint of the most recent solve on this thread */
+int vgg_dev_last_band_hint(int* meta, int* rb_range, int* end_blk, int* kb_rows, int* fg_tracks) {
+  VGG_REQUIRE(meta, "null pointer");
+  const BandRecord& r = g_band_last;
+  const int m[8] = {r.active, r.chol, r.tables, r.nb, r.KB, r.ngroups, r.arrow_blk, 0};
+  memcpy(meta, m, sizeof(m));
+  auto put = [](int* dst, const std::vector<int>& v) {
+    if (dst && !v.empty()) memcpy(dst, v.data(), sizeof(int) * v.size());
+  };
+  put(rb_range, r.rb_range);
+  put(end_blk, r.end_blk);
+  put(kb_rows, r.kb_rows);
+  put(fg_tracks, r.fg_tracks);
   return VGG_OK;
 }
 

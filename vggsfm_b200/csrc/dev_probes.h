@@ -21,9 +21,18 @@ int vgg_dev_set_syrk_ranges(const int* ranges_host, int count);
 /* The Schur SYRK of the LM loop (csrc/ba_schur.cu, FP64 tensor cores): Cmat -= Zt^T Zt into the row-major LOWER triangle
  * of Cmat [Dpad][Dpad] for Zt [Kpad][Dpad] (device pointers; Dpad % 128 == 0, Kpad % 16 == 0), honouring the band hint. */
 int vgg_dev_syrk_f64(int Kpad, int Dpad, const double* Zt, double* Cmat, void* stream);
-/* Backward substitution (csrc/trsv.cu) with per-block-row timestamps (ns): stamps_host[2 b] = block row b (64 rows) has
- * consumed every x_j it needs, [2 b + 1] = x_b published.  A_dev: row-major upper triangle, lda columns. */
-int vgg_dev_trsv_probe(int n, int lda, const double* A_dev, const double* y_dev, double* x_dev, long long* stamps_host);
+/* Backward substitution U x = y (csrc/trsv.cu).  A_dev: row-major upper triangle, lda columns (the strictly lower
+ * triangle is never read); y_dev[i * y_stride] = y_i.  stamps_host == NULL: the launcher of the LM loop (sentinel fill +
+ * kernel), then a device synchronise.  Otherwise the kernel alone with per-block-row timestamps (ns, 6 per block row of
+ * 64 rows: entry, diagonal block loaded, inverse ready, every x_j consumed, x_b published, right-hand side ready). */
+int vgg_dev_trsv_probe(int n, int lda, const double* A_dev, const double* y_dev, size_t y_stride, double* x_dev,
+                       long long* stamps_host);
+/* Band hint of the most recent vgg_ba_solve on the calling thread (csrc/ba_solve.cu, compute_band_hint), kept after the
+ * solve has cleared it.  meta_host[0..7] = {SYRK k-range hint active, factorisation band set, device tables for
+ * ba_blocks / z_build / backsub made, nb (128-column row blocks), KB (64-row k blocks), frame groups of 32, arrow_blk, 0}.
+ * Each non-null array receives its table if it was made: rb_range[2 nb], end_blk[nb], kb_rows[2 KB],
+ * fg_tracks[2 groups]. */
+int vgg_dev_last_band_hint(int* meta_host, int* rb_range, int* end_blk, int* kb_rows, int* fg_tracks);
 /* Block structure for the in-repo Cholesky (tests): end_blk_host[b] = one past the last band block (128 rows) of block
  * column b, arrow_blk = first block of the dense arrow; count = 0 clears it (dense). */
 int vgg_dev_set_chol_band(const int* end_blk_host, int count, int arrow_blk);

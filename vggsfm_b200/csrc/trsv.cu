@@ -12,6 +12,7 @@
 // Critical path per block: one 64 x 64 tile update + one 64 x 64 mat-vec + one flag hand-off (~1.5 us), 38 blocks.
 // U is the row-major upper triangle (what a column-major LOWER potrf leaves in a row-major buffer): U[i][j] = A[i*lda+j].
 #include "common.cuh"
+#include "dev_probes.h"
 
 namespace vgg {
 
@@ -232,10 +233,12 @@ int launch_trsv_upper(int n, int lda, const double* A, const double* y, size_t y
 
 }  // namespace vgg
 
-// tools/microbench.py trsv: the backward substitution on a random well-conditioned upper triangle, with per-block-row
-// timestamps (ns, globaltimer): stamps_host[2 b] = block row b has consumed every x_j it needs, [2 b + 1] = x_b published
-extern "C" int vgg_dev_trsv_probe(int n, int lda, const double* A_dev, const double* y_dev, double* x_dev, long long* stamps_host) {
+// tests/test_trsv_gpu.py (stamps_host == NULL): the production launcher on its own.  tools/microbench.py trsv: the kernel
+// with per-block-row timestamps (ns, globaltimer), 6 per block row (see csrc/dev_probes.h)
+extern "C" int vgg_dev_trsv_probe(int n, int lda, const double* A_dev, const double* y_dev, size_t y_stride, double* x_dev,
+                                  long long* stamps_host) {
   using namespace vgg;
+  VGG_REQUIRE(n > 0 && lda >= n && A_dev && y_dev && x_dev && y_stride > 0, "bad argument");
   const int nb = (n + TS_NB - 1) / TS_NB;
   static long long* d = nullptr;                      // allocated once: a cudaMalloc / cudaFree pair per call would put
   static int d_cap = 0;                                // allocator work (and its TLB effects) right in front of the kernel
@@ -245,10 +248,17 @@ extern "C" int vgg_dev_trsv_probe(int n, int lda, const double* A_dev, const dou
     d_cap = 6 * nb;
   }
   VGG_CUDA_CHECK(cudaMemset(d, 0, sizeof(long long) * 6 * nb));
+  if (!stamps_host) {
+    // the zeroed stamp buffer doubles as the flag workspace (>= trsv_workspace_ints(n) ints)
+    const int rc = launch_trsv_upper(n, lda, A_dev, y_dev, y_stride, x_dev, reinterpret_cast<int*>(d), 1, 0);
+    if (rc) return rc;
+    VGG_CUDA_CHECK(cudaDeviceSynchronize());
+    return VGG_OK;
+  }
   const size_t smem = sizeof(double) * (2 * TS_NB * (TS_NB + 1) + 2 * TS_NB);
   VGG_CUDA_CHECK(cudaFuncSetAttribute(trsv_upper_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   VGG_CUDA_CHECK(cudaMemset(x_dev, 0xFF, sizeof(double) * (size_t)n));
-  trsv_upper_kernel<<<nb, TS_THREADS, smem>>>(n, lda, A_dev, y_dev, 1, x_dev, reinterpret_cast<int*>(d), 1, 2);
+  trsv_upper_kernel<<<nb, TS_THREADS, smem>>>(n, lda, A_dev, y_dev, y_stride, x_dev, reinterpret_cast<int*>(d), 1, 2);
   VGG_LAUNCH_CHECK();
   VGG_CUDA_CHECK(cudaDeviceSynchronize());
   VGG_CUDA_CHECK(cudaMemcpy(stamps_host, d, sizeof(long long) * 6 * nb, cudaMemcpyDeviceToHost));
