@@ -159,9 +159,10 @@ def tri_angle_deg(c1, c2, X, eps=1e-12):
     return t * (180.0 / PI)
 
 
-def any_pair_tri_angle(centers, X, min_deg, inl=None):
+def any_pair_tri_angle_exhaustive(centers, X, min_deg, inl=None):
     """exists (a,b) [both flagged by inl if given] with triangulation angle >= min_deg.
-    centers [S,3], X [P,3], inl [S,P]|None -> [P] bool.  NaN angles compare False like torch."""
+    centers [S,3], X [P,3], inl [S,P]|None -> [P] bool.  NaN angles compare False like torch.
+    The reference's full S x S table; kept as the definition any_pair_tri_angle is tested against."""
     S = centers.shape[0]
     out = np.zeros(X.shape[0], dtype=bool)
     for a in range(S):
@@ -171,6 +172,48 @@ def any_pair_tri_angle(centers, X, min_deg, inl=None):
         if inl is not None:
             ok = ok & inl[a][None, :] & inl
         out |= ok.any(axis=0)
+    return out
+
+
+def separation_order(S):
+    """Frame-index separations d of the pairs (a, a+d), wide baselines first as the kernels visit them:
+    S/2, ..., S-1, S/2-1, ..., 1, then 0 (the self pairs, which only pass when min_deg <= 0)."""
+    mid = max(S // 2, 1)
+    return list(range(mid, S)) + list(range(mid - 1, 0, -1)) + [0]
+
+
+def any_pair_tri_angle(centers, X, min_deg, inl=None, margin=0.0, return_best=False):
+    """Same answer as any_pair_tri_angle_exhaustive, found faster: pairs are visited by separation, wide first,
+    vectorised over the points still undecided, and a point leaves the search as soon as one of its pairs reaches
+    min_deg + margin.  The points that never do (the False answers, and the True ones whose best pair lies in
+    [min_deg, min_deg + margin)) run through every pair.  tri_angle_deg is symmetric in its two centres and gives
+    exactly 0 for a self pair, so the unordered pairs plus the self pairs are the whole S x S table.
+
+    With return_best also returns, per point, the largest angle over the pairs visited (ignoring NaN, -inf if
+    none): the exact maximum when it is below min_deg + margin, a lower bound at or above it otherwise."""
+    S = centers.shape[0]
+    P = X.shape[0]
+    out = np.zeros(P, dtype=bool)
+    best = np.full(P, -np.inf)
+    block = max(1, (1 << 21) // max(S, 1))
+    for p0 in range(0, P, block):
+        live = np.arange(p0, min(P, p0 + block))
+        for d in separation_order(S):
+            if live.size == 0:
+                break
+            a = np.arange(S - d)
+            ang = tri_angle_deg(centers[a][:, None, :], centers[a + d][:, None, :], X[live][None, :, :])   # [S-d,U]
+            with np.errstate(invalid="ignore"):
+                ok = ang >= min_deg
+            if inl is not None:
+                pair_inl = inl[a][:, live] & inl[a + d][:, live]
+                ok &= pair_inl
+                ang = np.where(pair_inl, ang, -np.inf)
+            out[live] |= ok.any(axis=0)
+            best[live] = np.maximum(best[live], np.where(np.isnan(ang), -np.inf, ang).max(axis=0))
+            live = live[best[live] < min_deg + margin]
+    if return_best:
+        return out, best
     return out
 
 
@@ -203,28 +246,32 @@ def residual_indicator(err, thr, nanvalue):
     return (thres - m) / thres + cnt.astype(np.float64), cnt, inl
 
 
+# A refined hypothesis whose best camera pair lies within this many degrees above min_tri_angle keeps searching, so
+# that its reported best pair angle is exact there (see any_pair_tri_angle); the answer itself does not depend on it.
+TRI_TIE_DEG = 1e-6
+
+
 def _refine(tn_t, cams, centers, inl, order, lo, min_tri_angle, invalid_vis, thr):
     """local_refine_and_compute_error for the top-`lo` hypotheses.  tn_t [N,S,2], inl [N,H,S] bool,
-    order [N,H] ranking -> (X [N,lo,3], err [N,lo,S])."""
+    order [N,H] ranking -> (X [N,lo,3], err [N,lo,S], best pair angle - min_tri_angle [N,lo])."""
     N, S, _ = tn_t.shape
     X = np.zeros((N, lo, 3))
-    invalid = np.zeros((N, lo), dtype=bool)
     camsB = np.broadcast_to(cams[None], (N, S, 3, 4))
     for j in range(lo):
         mk = inl[np.arange(N), order[:, j]]                       # [N,S]
         pts = np.where(mk[..., None], tn_t, 0.0)                  # masked-out observations are zeroed (:670-672)
-        Xj = dlt(camsB, pts, mk.astype(np.float64))
-        X[:, j] = Xj
-        with np.errstate(invalid="ignore"):
-            z = np.einsum("sj,nj->ns", cams[:, 2, :3], Xj) + cams[None, :, 2, 3]
-            bad_che = (z <= 0).any(axis=1)                        # all S cameras (:100-115)
-        ok_tri = any_pair_tri_angle(centers, Xj, min_tri_angle)    # all S^2 camera pairs (:117-120)
-        invalid[:, j] = (~ok_tri) | bad_che
+        X[:, j] = dlt(camsB, pts, mk.astype(np.float64))
+    with np.errstate(invalid="ignore"):
+        z = np.einsum("sj,nlj->nls", cams[:, 2, :3], X) + cams[None, None, :, 2, 3]
+        bad_che = (z <= 0).any(axis=2)                            # all S cameras (:100-115)
+    ok_tri, best = any_pair_tri_angle(centers, X.reshape(-1, 3), min_tri_angle, margin=TRI_TIE_DEG,
+                                      return_best=True)           # all S^2 camera pairs (:117-120)
+    invalid = (~ok_tri.reshape(N, lo)) | bad_che
     err = angular_error(np.transpose(tn_t, (1, 0, 2)), np.transpose(X, (1, 0, 2)), cams)   # [lo,S,N]
     err = np.transpose(err, (2, 0, 1))
     err = np.where(np.isfinite(err), err, 100 * PI)               # nan_to_num(100*pi) (:1001-1006)
     err = err + PI * invalid[:, :, None] + PI * invalid_vis[:, None, :]
-    return X, err
+    return X, err, best.reshape(N, lo) - min_tri_angle
 
 
 def triangulate_tracks(extrinsics, tn, pairs, track_vis, track_score=None, lo_num=50, max_angular_error=2.0,
@@ -263,11 +310,11 @@ def triangulate_tracks(extrinsics, tn, pairs, track_vis, track_score=None, lo_nu
         inl = err <= thr
     # -- local refinement, two rounds
     order = np.argsort(-inl.sum(axis=-1), axis=1, kind="stable")
-    X1, err1 = _refine(tn_t, extrinsics, centers, inl, order, lo, min_tri_angle, invalid_vis, thr)
+    X1, err1, tri1 = _refine(tn_t, extrinsics, centers, inl, order, lo, min_tri_angle, invalid_vis, thr)
     lo2 = 10 if lo > 10 else lo
     inl1 = err1 <= thr
     order1 = np.argsort(-inl1.sum(axis=-1), axis=1, kind="stable")
-    X2, err2 = _refine(tn_t, extrinsics, centers, inl1, order1, lo2, min_tri_angle, invalid_vis, thr)
+    X2, err2, tri2 = _refine(tn_t, extrinsics, centers, inl1, order1, lo2, min_tri_angle, invalid_vis, thr)
     allX = np.concatenate([X0, X1, X2], axis=1)
     allE = np.concatenate([err, err1, err2], axis=1)
     score, cnt, mask = residual_indicator(allE, thr, 2 * PI)
@@ -275,7 +322,24 @@ def triangulate_tracks(extrinsics, tn, pairs, track_vis, track_score=None, lo_nu
     ar = np.arange(N)
     out = allX[ar, best], cnt[ar, best].astype(np.int64), mask[ar, best]
     if return_debug:
-        return out + (dict(allX=allX, allE=allE, score=score, best=best, order=order, order1=order1),)
+        # near-tie information: how far each decision that selects or counts something is from flipping
+        Xb = allX[ar, best][:, None, :]
+        with np.errstate(invalid="ignore"):
+            same_point = np.all(np.abs(allX - Xb) <= 1e-9 * (1.0 + np.abs(Xb)), axis=-1)   # NaN -> different
+            gate = np.abs(allE - thr)
+        gate = np.where(np.isnan(gate), np.inf, gate)                # a NaN error is never an inlier
+        other = np.where(same_point, -np.inf, score).max(axis=1)
+        return out + (dict(allX=allX, allE=allE, score=score, best=best, order=order, order1=order1, cnt=cnt,
+                           mask=mask,
+                           # best score minus the best score of a hypothesis with a different point (inf if none)
+                           score_margin=score[ar, best] - other,
+                           # |angular error - gate| of the chosen hypothesis per observation [N,S], and the
+                           # smallest such distance over every hypothesis of the track [N]
+                           gate_dist=gate[ar, best], gate_dist_min=gate.min(axis=(1, 2)),
+                           # triangulation angle of the two-view pair [N,H0], and of the best camera pair of each
+                           # refined hypothesis [N,lo+lo2], minus min_tri_angle (exact within TRI_TIE_DEG of 0)
+                           tri_dist0=ang.reshape(N, H0) - min_tri_angle,
+                           tri_dist=np.concatenate([tri1, tri2], axis=1)),)
     return out
 
 
