@@ -251,7 +251,9 @@ int vgg_undistort_simple_radial(int S, int N, const double* tracks_normalized, c
  * frame_flags uint8 [S] (0 = skip the frame), points double [P,3], intr double [S,4] = f,cx,cy,k.
  * Out: pose_out double [S,12] (R|t, written for successful frames only), focal_out double [S] (prior focal x best
  * factor), num_inliers_out int32 [S] (0 = no model: the reference's `None`), inlier_out uint8 [S,P].
- * The non-linear refinement COLMAP runs afterwards is vgg_pose_refinement.  P <= ~9700 per call. */
+ * The non-linear refinement COLMAP runs afterwards is vgg_pose_refinement.  P <= 9751 per call: the
+ * frame's usable points live in 21 P + 16 bytes of dynamic shared memory, capped at 200 KB; a larger P returns
+ * VGG_EINVAL before anything is launched. */
 int vgg_pnp_workspace_bytes(int S, int estimate_focal_length, size_t* bytes);
 int vgg_absolute_pose_estimation(int S, int P, int camera_model, const float* uv, const uint8_t* mask,
                                  const uint8_t* frame_flags, const double* points, const double* intr,

@@ -221,58 +221,126 @@ def gauss_newton(P, X, xn, steps=GN_STEPS):
     return P
 
 
-def lo_ransac(X, xn, thr2, u_samples):
+def new_debug():
+    """Decision record filled by ``lo_ransac(..., debug=d)``:
+      nsol_hist [5]     trials by number of P3P solutions (0..4); trials with a repeated index are counted in ``skipped``;
+      best_from_lo      the returned pose is a local-optimisation iterate (False: a raw P3P candidate);
+      lo_not_last       local optimisations started from a candidate that was not the last of its trial (the kernel
+                        must then restore the supports of the later candidates);
+      thr_margin        smallest |res - thr2| / thr2 over the finite residuals of every scored pose (P3P candidates
+                        and local-optimisation iterates), i.e. of every inlier decision the support depends on;
+      tie_gap           smallest |s_a - s_b| / max(s_a, s_b) over the support comparisons with equal inlier counts of at
+                        least 4 whose two poses differ by more than 1e-8 (closer poses are interchangeable at the 1e-8
+                        bar).  With 3 inliers every candidate fits its own sample exactly, the sums are rounding noise,
+                        and such a support never starts a local optimisation: any larger support replaces it, and a
+                        final count of 3 leaves the pose ambiguous."""
+    return {"nsol_hist": np.zeros(5, dtype=np.int64), "skipped": 0, "lo_not_last": 0, "thr_margin": np.inf,
+            "tie_gap": np.inf, "best_from_lo": False}
+
+
+def _note_margin(debug, res, thr2):
+    if debug is not None:
+        fin = res[np.isfinite(res)]
+        if len(fin):
+            debug["thr_margin"] = min(debug["thr_margin"], float(np.min(np.abs(fin - thr2))) / thr2)
+
+
+def _note_tie(debug, Pa, cnt, rs, Pb, bcnt, bs):
+    if debug is not None and Pb is not None and cnt == bcnt >= 4 and np.abs(Pa - Pb).max() > 1e-8:
+        den = max(abs(rs), abs(bs))
+        debug["tie_gap"] = min(debug["tie_gap"], abs(rs - bs) / den if den > 0 else 0.0)
+
+
+def lo_ransac(X, xn, thr2, u_samples, debug=None):
     """LO-RANSAC over the host-drawn minimal samples.  X [n,3], xn [n,2] (usable points only).
-    Returns (pose, num_inliers, residual_sum, inlier mask) or None."""
+    Returns (pose, num_inliers, residual_sum, inlier mask) or None.  ``debug``: a ``new_debug()`` dict to accumulate
+    into."""
     n = len(X)
     if n < 3:
         return None
     best = (None, 0, np.inf, np.zeros(n, dtype=bool))
+    from_lo = False
     for us in u_samples:
         idx = np.minimum((us * n).astype(np.int64), n - 1)
         if len(set(idx.tolist())) < 3:
+            if debug is not None:
+                debug["skipped"] += 1
             continue
         b = np.concatenate([xn[idx], np.ones((3, 1))], axis=1)
         b = b / np.linalg.norm(b, axis=1, keepdims=True)
-        for P in p3p(b, X[idx]):
-            cnt, rs, inl = _support(residuals(P, X, xn), thr2)
+        sols = p3p(b, X[idx])
+        if debug is not None:
+            debug["nsol_hist"][len(sols)] += 1
+        for q, P in enumerate(sols):
+            res = residuals(P, X, xn)
+            _note_margin(debug, res, thr2)
+            cnt, rs, inl = _support(res, thr2)
+            _note_tie(debug, P, cnt, rs, best[0], best[1], best[2])
             if not _better(cnt, rs, best[1], best[2]):
                 continue
             best = (P, cnt, rs, inl)
+            from_lo = False
             if cnt >= 4:
+                if debug is not None and q < len(sols) - 1:
+                    debug["lo_not_last"] += 1
                 for _ in range(MAX_LOCAL_TRIALS):
                     prev = best[1]
                     Pl = gauss_newton(best[0], X[best[3]], xn[best[3]])
-                    c2, r2, i2 = _support(residuals(Pl, X, xn), thr2)
+                    res = residuals(Pl, X, xn)
+                    _note_margin(debug, res, thr2)
+                    c2, r2, i2 = _support(res, thr2)
+                    _note_tie(debug, Pl, c2, r2, best[0], best[1], best[2])
                     if _better(c2, r2, best[1], best[2]):
                         best = (Pl, c2, r2, i2)
+                        from_lo = True
                     if best[1] <= prev:
                         break
+    if debug is not None:
+        debug["best_from_lo"] = from_lo
     if best[0] is None or best[1] < 3:
         return None
     return best
 
 
 def absolute_pose_estimation(points2D, points3D, intr4, model, u_samples, estimate_focal_length=False, max_error=12.0,
-                             mask=None):
-    """-> dict(pose [3,4], focal, num_inliers, inliers [P] bool) before the non-linear refinement, or None."""
+                             mask=None, return_debug=False):
+    """-> dict(pose [3,4], focal, num_inliers, inliers [P] bool) before the non-linear refinement, or None.
+
+    ``return_debug``: returns (result or None, debug) where debug is ``new_debug()`` accumulated over every factor plus
+    ``factors``: per focal factor a dict(focal, num_inliers (0 when nothing was found), residual_sum, pose, inliers [P],
+    from_lo); ``best_from_lo`` then refers to the winning factor."""
     P = len(points3D)
     mask = np.ones(P, dtype=bool) if mask is None else np.asarray(mask, dtype=bool)
     idx = np.nonzero(mask)[0]
     X = np.asarray(points3D, dtype=np.float64)[idx]
     uv = np.asarray(points2D, dtype=np.float64)[idx]
     f0, cx, cy, k = [float(v) for v in intr4]
+    debug = new_debug() if return_debug else None
+    if debug is not None:
+        debug["factors"] = []
     best, best_f = None, f0
     for fac in focal_length_factors(estimate_focal_length):
         f = f0 * fac
         xn = (uv - np.array([cx, cy])) / f
         if model == SIMPLE_RADIAL:
             xn = undistort_radial(xn, k)
-        r = lo_ransac(X, xn, (max_error / f) ** 2, u_samples)
+        r = lo_ransac(X, xn, (max_error / f) ** 2, u_samples, debug)
+        if debug is not None:
+            m = np.zeros(P, dtype=bool)
+            if r is not None:
+                m[idx[r[3]]] = True
+            debug["factors"].append({"focal": f, "num_inliers": 0 if r is None else r[1],
+                                     "residual_sum": np.inf if r is None else r[2],
+                                     "pose": np.zeros((3, 4)) if r is None else r[0], "inliers": m,
+                                     "from_lo": debug["best_from_lo"]})
         if r is not None and (best is None or r[1] > best[1]):        # across factors: inlier count only, first wins ties
             best, best_f = r, f
-    if best is None:
-        return None
-    inl = np.zeros(P, dtype=bool)
-    inl[idx[best[3]]] = True
-    return {"pose": best[0], "focal": best_f, "num_inliers": best[1], "inliers": inl}
+    out = None
+    if debug is not None:
+        debug["best_from_lo"] = best is not None and debug["factors"][int(np.argmax(
+            [fc["num_inliers"] for fc in debug["factors"]]))]["from_lo"]
+    if best is not None:
+        inl = np.zeros(P, dtype=bool)
+        inl[idx[best[3]]] = True
+        out = {"pose": best[0], "focal": best_f, "num_inliers": best[1], "inliers": inl}
+    return (out, debug) if return_debug else out

@@ -144,13 +144,20 @@ def pose_refinement(pose, intr, points3D, points2D, inlier_mask, model, refine_f
         return pose, intr, summary
     cost, H, g = evaluate(pose, intr)
     summary["initial_cost"] = cost
-    sc = 1.0 / (1.0 + np.sqrt(np.diag(H)))
     radius = opt.initial_trust_region_radius
+    if not (np.isfinite(cost) and np.isfinite(g[free]).all()):
+        # Ceres: the initial residual / Jacobian evaluation fails -> FAILURE before the first iteration [3P-memory]
+        summary.update(final_cost=cost, final_radius=radius, termination=FAILURE)
+        return pose, intr, summary
+    sc = 1.0 / (1.0 + np.sqrt(np.diag(H)))
     decrease_factor = 2.0
     invalid = 0
     it = 0
-    if np.max(np.abs(g[free])) <= opt.gradient_tolerance:
-        summary.update(final_cost=cost, termination=CONV_GRADIENT)
+    grad_max = float(np.max(np.abs(g[free])))
+    if trace is not None:
+        trace.append({"it": 0, "accepted": True, "cost": cost, "grad_max": grad_max})
+    if grad_max <= opt.gradient_tolerance:
+        summary.update(final_cost=cost, final_radius=radius, termination=CONV_GRADIENT)
         return pose, intr, summary
     while True:
         if it >= opt.max_num_iterations:
@@ -197,7 +204,7 @@ def pose_refinement(pose, intr, points3D, points2D, inlier_mask, model, refine_f
         rho = cost_change / model_change
         if trace is not None:
             trace.append({"it": it, "cost": cost, "candidate_cost": c_cost, "model_change": model_change, "rho": rho,
-                          "radius": radius, "step_norm": step_norm})
+                          "radius": radius, "step_norm": step_norm, "x_norm": x_norm})
         if step_norm <= opt.parameter_tolerance * (x_norm + opt.parameter_tolerance):
             summary["termination"] = CONV_PARAMETER
             break
@@ -211,7 +218,10 @@ def pose_refinement(pose, intr, points3D, points2D, inlier_mask, model, refine_f
             summary["successful"] += 1
             radius = min(opt.max_trust_region_radius, radius / max(1.0 / 3.0, 1.0 - (2.0 * rho - 1.0) ** 3))
             decrease_factor = 2.0
-            if np.max(np.abs(g[free])) <= opt.gradient_tolerance:
+            grad_max = float(np.max(np.abs(g[free])))
+            if trace is not None:
+                trace.append({"it": it, "accepted": True, "cost": cost, "grad_max": grad_max})
+            if grad_max <= opt.gradient_tolerance:
                 summary["termination"] = CONV_GRADIENT
                 break
         else:
@@ -241,7 +251,7 @@ def pose_refinement_batched(poses, intr, points3D, tracks2D, inlier, model, acti
 
 
 def frame_loop(poses, intr, points3D, tracks2D, inlier, active, model, shared_camera, max_reproj_error=0.0,
-               min_inliers=0, options: PoseOptions | None = None):
+               min_inliers=0, options: PoseOptions | None = None, traces: list | None = None):
     """The python frame loop both reference callers share (triangulation.py:341-441, :542-608) in array form.
 
     * pre-filter (refine_pose only, :298-315): inlier AND depth > 0 AND squared reprojection error <= max^2,
@@ -249,7 +259,8 @@ def frame_loop(poses, intr, points3D, tracks2D, inlier, active, model, shared_ca
     * a frame is refined when active and its inlier count is > min_inliers;
     * shared camera: one camera object, created from frame 0's intrinsics, refined by frame 0 only
       (refine flags are switched off for ridx > 0, :373-375) and read back for every frame.
-    Returns (poses, intr, used_mask, summaries)."""
+    Returns (poses, intr, used_mask, summaries).  ``traces``: a list that receives one ``pose_refinement`` trace per
+    frame (empty for a frame that is not refined)."""
     poses = np.array(poses, dtype=np.float64).copy()
     intr = np.array(intr, dtype=np.float64).copy()
     S = len(poses)
@@ -267,8 +278,12 @@ def frame_loop(poses, intr, points3D, tracks2D, inlier, active, model, shared_ca
         if shared_camera:
             intr[s] = cam
         rf = (not shared_camera) or s == 0
+        trace = []
+        if traces is not None:
+            traces.append(trace)
         if active[s] and used[s].sum() > min_inliers:
-            poses[s], intr[s], sm = pose_refinement(poses[s], intr[s], points3D, tracks2D[s], used[s], model, rf, rf, options)
+            poses[s], intr[s], sm = pose_refinement(poses[s], intr[s], points3D, tracks2D[s], used[s], model, rf, rf, options,
+                                                    trace)
             if shared_camera:
                 cam = intr[s].copy()
         else:

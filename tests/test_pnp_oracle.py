@@ -71,3 +71,48 @@ def test_recovers_pose_with_outliers(cam, est_f):
 def test_returns_none_without_enough_points():
     us = np.random.default_rng(0).uniform(size=(8, 3))
     assert po.absolute_pose_estimation(np.zeros((2, 2)), np.zeros((2, 3)), (1000.0, 512.0, 512.0, 0.0), 0, us) is None
+
+
+def test_debug_record():
+    """absolute_pose_estimation(return_debug=True): per-factor results agree with a direct lo_ransac at that focal,
+    the winner is the first factor with the highest count, and the decision record is filled."""
+    sc = make_scene(2, 300, "SIMPLE_PINHOLE", seed=5, noise_px=0.3, outlier_frac=0.3)
+    us = np.random.default_rng(4).uniform(size=(48, 3))
+    us[5] = [0.1, 0.1, 0.7]                                       # a repeated index: the trial is skipped
+    intr = (1300.0, 512.0, 512.0, 0.0)
+    r, dbg = po.absolute_pose_estimation(sc.tracks[1], sc.points3d, intr, 0, us, estimate_focal_length=True,
+                                         mask=sc.mask[1], return_debug=True)
+    facs = dbg["factors"]
+    assert len(facs) == 31 and dbg["skipped"] == 31
+    assert dbg["nsol_hist"].sum() == 31 * 47 and dbg["nsol_hist"][1:].sum() > 0
+    counts = [f["num_inliers"] for f in facs]
+    k = int(np.argmax(counts))
+    assert r["focal"] == facs[k]["focal"] and r["num_inliers"] == counts[k]
+    assert np.array_equal(r["inliers"], facs[k]["inliers"]) and np.array_equal(r["pose"], facs[k]["pose"])
+    assert 0 < dbg["thr_margin"] < 1 and dbg["tie_gap"] > 0
+    for j in (0, 17, 30):
+        f = facs[j]["focal"]
+        idx = np.nonzero(sc.mask[1])[0]
+        xn = (sc.tracks[1][idx].astype(np.float64) - 512.0) / f
+        d = po.new_debug()
+        got = po.lo_ransac(sc.points3d[idx], xn, (12.0 / f) ** 2, us, d)
+        if got is None:
+            assert facs[j]["num_inliers"] == 0 and not facs[j]["inliers"].any()
+            continue
+        assert got[1] == facs[j]["num_inliers"] and got[2] == facs[j]["residual_sum"]
+        assert np.array_equal(got[0], facs[j]["pose"]) and facs[j]["inliers"].sum() == got[1]
+        assert d["nsol_hist"].sum() == 47 and d["thr_margin"] >= dbg["thr_margin"]
+    # without the debug flag the result is the same
+    r2 = po.absolute_pose_estimation(sc.tracks[1], sc.points3d, intr, 0, us, estimate_focal_length=True, mask=sc.mask[1])
+    assert r2["focal"] == r["focal"] and np.array_equal(r2["pose"], r["pose"])
+
+
+def test_debug_sees_lo_on_an_earlier_candidate():
+    """Over a few hundred random trials some P3P samples have 3 or 4 solutions and local optimisation runs on a candidate
+    that is not the last of its trial (the case in which the kernel restores the later candidates' supports)."""
+    sc = make_scene(1, 400, "SIMPLE_PINHOLE", seed=11, noise_px=0.3, outlier_frac=0.2)
+    us = np.random.default_rng(12).uniform(size=(400, 3))
+    _, dbg = po.absolute_pose_estimation(sc.tracks[0], sc.points3d, (1000.0, 512.0, 512.0, 0.0), 0, us,
+                                         mask=sc.mask[0], return_debug=True)
+    assert dbg["nsol_hist"][2] > 0 and dbg["nsol_hist"][3:].sum() > 0
+    assert dbg["lo_not_last"] > 0 and len(dbg["factors"]) == 1

@@ -95,3 +95,41 @@ def test_frame_loop_shared_camera_semantics():
     uv_bad[1, :10] += 50.0
     _, _, used2, _ = po.frame_loop(poses, intr, X, uv_bad, inl, np.zeros(S, bool), 0, False, 12.0, 0)
     assert not used2[1, :10].any() and used2[1, 10:].all()
+
+
+@pytest.mark.parametrize("bad", ["nan", "camera_plane"])
+def test_non_finite_start_fails_at_iteration_zero(bad):
+    """A non-finite residual at the starting point (a NaN observation, or a point exactly on the camera plane; nothing
+    filters them when max_reproj_error is 0, as in init_refine_pose) ends the solve with FAILURE before the first
+    iteration and leaves pose and intrinsics untouched -- Ceres' failed initial evaluation [3P-memory]."""
+    _, _, X, uv, p0, i0 = _case(1)
+    X, uv = X.copy(), uv.copy()
+    if bad == "nan":
+        uv[7, 0] = np.nan
+    else:
+        p0 = p0.copy()
+        p0[2, 3] = 0.0                                    # the world origin is then exactly at depth 0
+        X[7] = 0.0
+    trace = []
+    p1, i1, sm = po.pose_refinement(p0, i0, X, uv, np.ones(len(X), bool), 1, trace=trace)
+    assert sm["termination"] == po.FAILURE and sm["iterations"] == 0 and sm["successful"] == 0
+    assert not np.isfinite(sm["initial_cost"]) and not np.isfinite(sm["final_cost"])
+    assert sm["final_radius"] == po.PoseOptions().initial_trust_region_radius
+    assert np.array_equal(p1, p0) and np.array_equal(i1, i0) and trace == []
+    # the same observation outside the inlier set does not matter
+    m = np.ones(len(X), bool)
+    m[7] = False
+    _, _, sm2 = po.pose_refinement(p0, i0, X, uv, m, 1)
+    assert sm2["termination"] in (po.CONV_GRADIENT, po.CONV_FUNCTION, po.CONV_PARAMETER) and sm2["iterations"] > 0
+
+
+def test_trace_records_gradient_at_every_accepted_point():
+    _, _, X, uv, p0, i0 = _case(0)
+    trace = []
+    _, _, sm = po.pose_refinement(p0, i0, X, uv, np.ones(len(X), bool), 0, trace=trace)
+    acc = [t for t in trace if t.get("accepted")]
+    assert acc[0]["it"] == 0 and abs(acc[0]["cost"] - sm["initial_cost"]) == 0
+    assert len(acc) == sm["successful"] + 1 and acc[-1]["cost"] == sm["final_cost"]
+    assert all(a["grad_max"] > 0 for a in acc)
+    steps = [t for t in trace if "step_norm" in t]
+    assert len(steps) == sm["iterations"] and all(t["x_norm"] > 1 for t in steps)

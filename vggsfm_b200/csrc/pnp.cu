@@ -21,6 +21,14 @@ constexpr int PNP_LOCAL_TRIALS = 10;
 
 __device__ __forceinline__ double cbrt_signed(double x) { return cbrt(x); }
 
+// COLMAP's focal-length ladder 0.2 + 4.8 (k / 30)^2, rounded step by step: a contracted FMA would move a factor by an
+// ulp, and with it the focal length the frame reports
+__device__ __forceinline__ double focal_factor(int k, int nfac) {
+  if (nfac <= 1) return 1.0;
+  const double i = (double)k / (double)(nfac - 1);
+  return __dadd_rn(0.2, __dmul_rn(__dmul_rn(5.0 - 0.2, i), i));
+}
+
 // real roots of A4 x^4 + A3 x^3 + A2 x^2 + A1 x + A0 (same steps as oracle/pnp_oracle.py:solve_quartic_real)
 __device__ int solve_quartic_real(double A4, double A3, double A2, double A1, double A0, double* roots) {
   if (!(isfinite(A4) && isfinite(A3) && isfinite(A2) && isfinite(A1) && isfinite(A0)) || fabs(A4) < 1e-300) return 0;
@@ -284,12 +292,7 @@ __global__ void __launch_bounds__(PNP_THREADS) pnp_ransac_kernel(
   if (!frame_flags[s]) return;
   const double f0 = intr[(size_t)s * 4], cx = intr[(size_t)s * 4 + 1], cy = intr[(size_t)s * 4 + 2];
   const double kdist = model == VGG_SIMPLE_RADIAL ? intr[(size_t)s * 4 + 3] : 0.0;
-  double fac = 1.0;
-  if (nfac > 1) {
-    const double i = (double)kf / (double)(nfac - 1);
-    fac = 0.2 + (5.0 - 0.2) * i * i;
-  }
-  const double f = f0 * fac;
+  const double f = f0 * focal_factor(kf, nfac);
   const double thr = max_error / f, thr2 = thr * thr;
   // ---- compaction of the usable points (order preserved) + normalised coordinates
   if (tid == 0) sh.n_usable = 0;
@@ -508,12 +511,7 @@ __global__ void pnp_select_kernel(int S, int P, int model, int nfac, double max_
   }
   const double f0 = intr[(size_t)s * 4], cx = intr[(size_t)s * 4 + 1], cy = intr[(size_t)s * 4 + 2];
   const double kdist = model == VGG_SIMPLE_RADIAL ? intr[(size_t)s * 4 + 3] : 0.0;
-  double fac = 1.0;
-  if (nfac > 1) {
-    const double i = (double)bk / (double)(nfac - 1);
-    fac = 0.2 + (5.0 - 0.2) * i * i;
-  }
-  const double f = f0 * fac, thr = max_error / f, thr2 = thr * thr;
+  const double f = f0 * focal_factor(bk, nfac), thr = max_error / f, thr2 = thr * thr;
   const double* Pb = res_pose + ((size_t)s * nfac + bk) * 12;
   if (tid < 12) pose_out[(size_t)s * 12 + tid] = Pb[tid];
   if (tid == 0) focal_out[s] = f;
@@ -569,7 +567,7 @@ int vgg_absolute_pose_estimation(int S, int P, int camera_model, const float* uv
     return VGG_EWORKSPACE;
   }
   const size_t smem = (size_t)P * (sizeof(double2) + sizeof(int) + 1) + 16;
-  VGG_REQUIRE(smem <= 200 * 1024, "absolute pose estimation: at most ~9700 points per call (shared-memory resident)");
+  VGG_REQUIRE(smem <= 200 * 1024, "absolute pose estimation: at most 9751 points per call (shared-memory resident)");
   cudaStream_t st = (cudaStream_t)stream;
   Carver c(workspace, ws_bytes);
   double* res_pose = c.take<double>((size_t)S * nfac * 12);

@@ -267,7 +267,15 @@ __global__ void __launch_bounds__(PT) pose_refine_kernel(int S, int P, const flo
     sh.it = 0; sh.invalid = 0; sh.successful = 0; sh.termination = VGG_BA_NO_CONVERGENCE;
     summary_d[s * 4 + 0] = sh.cost;
     sh.state = ST_EVAL_CAND;
-    if (grad_max() <= opt.gradient_tolerance) {
+    // a non-finite residual at the start (NaN observation, point on the camera plane) fails the solve before the first
+    // iteration, as Ceres' initial evaluation does; grad_max() would drop the NaNs (fmax) and report convergence
+    bool finite = isfinite(sh.cost);
+    for (int i = 0; i < 8; ++i)
+      if (i < 6 || (i == 6 ? free_f : free_k)) finite = finite && isfinite(sh.g[i]);
+    if (!finite) {
+      sh.termination = VGG_BA_FAILURE;
+      sh.state = ST_DONE;
+    } else if (grad_max() <= opt.gradient_tolerance) {
       sh.termination = VGG_BA_CONVERGENCE_GRADIENT;
       sh.state = ST_DONE;
     }

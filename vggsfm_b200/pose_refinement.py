@@ -43,6 +43,7 @@ class PoseReport:
     termination: torch.Tensor           # [S] int32 (TERMINATION)
     initial_cost: torch.Tensor          # [S] f64
     final_cost: torch.Tensor            # [S] f64
+    final_radius: torch.Tensor          # [S] f64 trust-region radius at the end (0 for frames that were not refined)
     num_inliers: torch.Tensor           # [S] int64 effective inliers per frame
     inlier_used: torch.Tensor           # [S,P] bool
     needs_absolute_pose: Optional[torch.Tensor] = None   # [S] bool (refine_pose only)
@@ -63,7 +64,7 @@ def pose_refinement_batched(poses, intr4, points3D, tracks2D, inlier, frame_flag
     if S == 0 or P == 0:                     # nothing to refine: every frame is reported as having too few inliers
         z = torch.zeros(S, dtype=torch.float64, device=dev)
         return PoseReport(torch.zeros(S, dtype=torch.int32, device=dev), torch.zeros(S, dtype=torch.int32, device=dev),
-                          torch.full((S,), 7, dtype=torch.int32, device=dev), z, z.clone(),
+                          torch.full((S,), 7, dtype=torch.int32, device=dev), z, z.clone(), z.clone(),
                           torch.zeros(S, dtype=torch.int64, device=dev), torch.zeros(S, P, dtype=torch.bool, device=dev))
     assert poses.dtype == torch.float64 and poses.is_contiguous() and intr4.dtype == torch.float64 and intr4.is_contiguous()
     pts = points3D.double().contiguous()
@@ -79,7 +80,7 @@ def pose_refinement_batched(poses, intr4, points3D, tracks2D, inlier, frame_flag
         _lib.check(L.vgg_pose_refinement(S, P, model, uv.data_ptr(), inl.data_ptr(), flags.data_ptr(), pts.data_ptr(),
                                      poses.data_ptr(), intr4.data_ptr(), ctypes.byref(opt), used.data_ptr(),
                                      sd.data_ptr(), si.data_ptr(), stream), "vgg_pose_refinement")
-    return PoseReport(si[:, 0], si[:, 1], si[:, 2], sd[:, 0], sd[:, 1], sd[:, 3].round().long(), used.bool(),
+    return PoseReport(si[:, 0], si[:, 1], si[:, 2], sd[:, 0], sd[:, 1], sd[:, 2], sd[:, 3].round().long(), used.bool(),
                       kernel_launches=1 if S > 0 else 0)
 
 
@@ -149,7 +150,8 @@ def _calibration_matrix(intr4):
 
 
 def _merge(dst: PoseReport, src: PoseReport, rows):
-    for f in ("iterations", "successful", "termination", "initial_cost", "final_cost", "num_inliers", "inlier_used"):
+    for f in ("iterations", "successful", "termination", "initial_cost", "final_cost", "final_radius", "num_inliers",
+              "inlier_used"):
         getattr(dst, f)[rows] = getattr(src, f)
     dst.kernel_launches += src.kernel_launches
 
