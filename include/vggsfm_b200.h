@@ -262,6 +262,36 @@ int vgg_absolute_pose_estimation(int S, int P, int camera_model, const float* uv
                                  void* workspace, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------- */
+/* Two-view stage (float64 arithmetic; float or double tracks)                                 */
+/* ------------------------------------------------------------------------------------------- */
+
+/* estimate_fundamental (vggsfm/two_view_geo/fundamental.py:43-183) for B pairs at once: 7-point minimal solves on
+ * caller-drawn samples (int32 [T,7], HOST memory: generate_samples, utils.py:39-60), Sampson scoring, two rounds of
+ * 8-point local refinement from the top lo_num (then lo_num/2) candidates, the residual indicator with its batch-wide
+ * threshold (utils.py:63-87), first argmax.  points1/points2 [B,N,2] float (points_are_f64 = 0) or double,
+ * valid_mask uint8 [B,N] or NULL, threshold = max_error^2 (squared) or max_error.  Outputs: fmat_out double [B,3,3],
+ * inlier_num_out int32 [B], inlier_mask_out uint8 [B,N], residuals_out double [B,N] (1e6 at invalid matches).
+ * VGG_EINVAL before any launch when N < 7, T < 7, lo_num outside [1, 3T], N > 190000 or a sample is outside [0, N). */
+int vgg_twoview_workspace_bytes(int B, int N, int T, int lo_num, size_t* bytes);
+int vgg_estimate_fundamental(int B, int N, const void* points1, const void* points2, int points_are_f64,
+                             const uint8_t* valid_mask, const int32_t* samples, int T, int lo_num, double threshold,
+                             int squared, int second_refine, double* fmat_out, int32_t* inlier_num_out,
+                             uint8_t* inlier_mask_out, double* residuals_out, void* workspace, size_t ws_bytes,
+                             void* stream);
+
+/* inlier_by_fundamental (utils.py:300-322): inlier_mask_out uint8 [B,N] = Sampson residual of (points1, points2)
+ * under fmat double [B,3,3] <= threshold (squared distance, or its square root + eps when squared = 0). */
+int vgg_fundamental_inliers(int B, int N, const void* points1, const void* points2, int points_are_f64,
+                            const double* fmat, double threshold, int squared, uint8_t* inlier_mask_out, void* stream);
+
+/* estimate_preliminary.py:148-164: E = K^T F K with the default K (f = max(W, H), principal point (W/2, H/2)),
+ * decompose_essential_matrix (essential.py:36-83) and remove_cheirality (utils.py:325-448) over all N matches of the
+ * pair.  Out: R_out double [B,3,3], t_out double [B,3], E_out double [B,3,3]. */
+int vgg_relative_pose_from_fundamental(int B, int N, const void* points1, const void* points2, int points_are_f64,
+                                       const double* fmat, double width, double height, double* R_out, double* t_out,
+                                       double* E_out, void* stream);
+
+/* ------------------------------------------------------------------------------------------- */
 /* Tracker correlation inner loop (float32 math on float or half feature pyramids)             */
 /* ------------------------------------------------------------------------------------------- */
 

@@ -22,6 +22,8 @@ EXPORTS = [
     "vgg_project_points", "vgg_normalize_tracks", "vgg_undistort_simple_radial",
     "vgg_corr_pyramid_bytes", "vgg_corr_build_pyramid", "vgg_corr_sample", "vgg_sample_features4d",
     "vgg_corr_tc_supported", "vgg_corr_tc_bytes", "vgg_corr_tc_build", "vgg_corr_tc_sample",
+    "vgg_twoview_workspace_bytes", "vgg_estimate_fundamental", "vgg_relative_pose_from_fundamental",
+    "vgg_fundamental_inliers",
 ]
 
 
@@ -165,6 +167,10 @@ def lib() -> ctypes.CDLL:
     L.vgg_corr_tc_bytes.argtypes = [ci, ci, ci, ci, ci, ci, ctypes.POINTER(cs), ctypes.POINTER(cs)]
     L.vgg_corr_tc_build.argtypes = [ci, ci, ci, ci, ci, vp, vp, vp]
     L.vgg_corr_tc_sample.argtypes = [ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp]
+    L.vgg_twoview_workspace_bytes.argtypes = [ci, ci, ci, ci, ctypes.POINTER(cs)]
+    L.vgg_estimate_fundamental.argtypes = [ci, ci, vp, vp, ci, vp, vp, ci, ci, cd, ci, ci, vp, vp, vp, vp, vp, cs, vp]
+    L.vgg_fundamental_inliers.argtypes = [ci, ci, vp, vp, ci, vp, cd, ci, vp, vp]
+    L.vgg_relative_pose_from_fundamental.argtypes = [ci, ci, vp, vp, ci, vp, cd, cd, vp, vp, vp, vp]
     _lib = L
     return L
 
