@@ -127,7 +127,7 @@ int vgg_ba_build_blocks(const vgg_ba_problem* prob, double* cost, double* camrec
 
 /* Schur complement of the point blocks onto the camera system (second kernel of the path):
  * given the blocks above, the Jacobi scales and the trust-region radius, writes
- * Sraw[D,Dpad] (symmetric, both triangles written) = H_cc - sum_j W_j V_j^-1 W_j^T and rhs[Dpad] =
+ * Sraw[D,Dpad] (symmetric, only the row-major lower triangle valid) = H_cc - sum_j W_j V_j^-1 W_j^T and rhs[Dpad] =
  * -(g_c - sum_j W_j V_j^-1 g_pj).  Exposed for the parity tests and profiling. */
 int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double* g_p,
                  const double* H_pp, const double* W, const double* shared, const double* scale_p,

@@ -36,6 +36,29 @@ def test_host_only_entry_points():
     assert o.max_num_iterations == 100 and o.gradient_tolerance == 1e-4
 
 
+def test_ba_workspace_bytes_is_host_only():
+    """vgg_ba_workspace_bytes is a pure size computation: it succeeds without a GPU for the C1, C2 and C3 shapes and
+    every camera model / intrinsics mode, and covers at least the Schur operand Zt [Kpad][Dpad] and the reduced system
+    [D+3][Dpad] (matrix rows, right-hand side, diagonal, gradient) in float64."""
+    import ctypes
+    L = _lib.lib()
+    for S, N in ((8, 256), (50, 2048), (400, 4096)):
+        for model in (0, 1):
+            for mode in (0, 1, 2):
+                dc, ns = ctypes.c_int(), ctypes.c_int()
+                assert L.vgg_ba_dims(model, mode, ctypes.byref(dc), ctypes.byref(ns)) == 0
+                D = S * dc.value + ns.value
+                Dpad = (D + 2 + 127) // 128 * 128
+                Kpad = (3 * N + 15) // 16 * 16
+                red = ctypes.c_size_t()
+                assert L.vgg_ba_reduced_system_doubles(S, model, mode, ctypes.byref(red)) == 0
+                assert red.value == (D + 3) * Dpad
+                n = ctypes.c_size_t()
+                rc = L.vgg_ba_workspace_bytes(S, N, model, mode, ctypes.byref(n))
+                assert rc == 0, (S, N, model, mode, rc, L.vgg_last_error())
+                assert n.value >= 8 * (Kpad * Dpad + (D + 3) * Dpad), (S, N, model, mode, n.value)
+
+
 def test_build_blocks_rejects_unaligned_tracks_per_warp():
     """vgg_ba_build_blocks: tracks_per_warp must be 0 (choose) or a positive multiple of 4, else a warp's vectorised
     observation loads would be misaligned.  The check comes before any CUDA call, so it needs no GPU: the buffers are

@@ -1,5 +1,6 @@
-"""CUDA-event micro-benchmarks for A/B runs (env switches are read once per process):
-   python tools/microbench.py chol | ba | blocks [N] | pose [S N] | pipeline [S N] | syrk [S N]"""
+"""CUDA-event micro-benchmarks of single kernels and solver stages (the VGG_* environment variables set for the run
+label every line):
+   python tools/microbench.py ba [N] | blocks [N] | chol [n] | chol128 | trsv [n] | pose [S N] | pipeline [S N] | syrk [S N]"""
 import ctypes
 import os
 import sys
@@ -166,14 +167,13 @@ if mode == "chol128":
     B = rng.standard_normal((128, 160))
     A = np.ascontiguousarray(B @ B.T / 160 + 0.5 * np.eye(128))
     names = ["leaf(0)", "trsm(b)", "lookahead work", "lookahead wait", "dmma rank-32", "leaf(t0)"]
-    for leaf in (0, 1):
-        Lo = np.zeros((128, 128))
-        prof = np.zeros(13, dtype=np.int64)
-        _lib.check(L.vgg_dev_chol128_probe(leaf, 5, A.ctypes.data, Lo.ctypes.data, prof.ctypes.data), "probe")
-        err = np.abs(Lo @ Lo.T - A).max() / np.abs(A).max()
-        print(f"[{tag}] POTRF128 leaf={leaf}: {prof[12]} cycles  |LL^T-A|/|A| = {err:.2e}")
-        for w in (0, 1):
-            print("    warp %d: " % w + "  ".join(f"{n} {prof[w * 6 + i]}" for i, n in enumerate(names)))
+    Lo = np.zeros((128, 128))
+    prof = np.zeros(13, dtype=np.int64)
+    _lib.check(L.vgg_dev_chol128_probe(5, A.ctypes.data, Lo.ctypes.data, prof.ctypes.data), "probe")
+    err = np.abs(Lo @ Lo.T - A).max() / np.abs(A).max()
+    print(f"[{tag}] POTRF128: {prof[12]} cycles  |LL^T-A|/|A| = {err:.2e}")
+    for w in (0, 1):
+        print("    warp %d: " % w + "  ".join(f"{n} {prof[w * 6 + i]}" for i, n in enumerate(names)))
     sys.exit(0)
 
 if mode == "chol":

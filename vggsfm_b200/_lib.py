@@ -144,7 +144,7 @@ def lib() -> ctypes.CDLL:
     L.vgg_syrk_ozaki_workspace_bytes.argtypes = [ci, ci, ci, ctypes.POINTER(cs)]
     L.vgg_dev_blocks_timing.argtypes = [ci]
     L.vgg_dev_blocks_last_ms.argtypes = [ctypes.POINTER(cd)]
-    L.vgg_dev_chol128_probe.argtypes = [ci, ci, vp, vp, vp]
+    L.vgg_dev_chol128_probe.argtypes = [ci, vp, vp, vp]
     L.vgg_dev_set_syrk_ranges.argtypes = [vp, ci]
     L.vgg_dev_syrk_f64.argtypes = [ci, ci, vp, vp, vp]
     L.vgg_dev_trsv_probe.argtypes = [ci, ci, vp, vp, cs, vp, vp]

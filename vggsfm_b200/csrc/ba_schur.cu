@@ -227,7 +227,7 @@ struct SyrkWork {
 
 __global__ void __launch_bounds__(SF_THREADS, 1)
     syrk_f64_kernel(const SyrkWork* __restrict__ work, int nwork, int Kpad, int Dpad, const double* __restrict__ Zt,
-                    double* __restrict__ Cmat, ptrdiff_t mc_off, int fill_upper, const __grid_constant__ FabricDev fd) {
+                    double* __restrict__ Cmat, ptrdiff_t mc_off, const __grid_constant__ FabricDev fd) {
   extern __shared__ __align__(16) double sf_smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(sf_smem + SF_STAGES * SF_STAGE_DOUBLES);
   uint64_t* empty = full + SF_STAGES;
@@ -314,21 +314,20 @@ __global__ void __launch_bounds__(SF_THREADS, 1)
         for (int h = 0; h < 4; ++h) {
           const int r = wk.bi * SF_BM + wm * 64 + mt * 16 + g + 8 * (h >> 1);
           const int col = wk.bj * SF_BM + wn * 32 + nt * 8 + 2 * t + (h & 1);
-          syrk_red_upper(Cmat, Dpad, r, col, wk.bj, diag, acc[mt][nt][h], mc_off, fill_upper, fd);
+          syrk_red_upper(Cmat, Dpad, r, col, wk.bj, diag, acc[mt][nt][h], mc_off, fd);
         }
   }
 }
 
 // ------------------------------------------------------------------------------------------------
-// A (in place) = sc_i sc_j Sraw + diag; constant parameters pinned; b = sc * rhs.  Lower triangle only unless
-// fill_upper (library factorisation A/B, which reads the mirror).
+// A (in place) = sc_i sc_j Sraw + diag; constant parameters pinned; b = sc * rhs.  Lower triangle only.
 __global__ void scale_damp_kernel(int D, int Dpad, double* __restrict__ A, const double* __restrict__ rhs,
                                   const double* __restrict__ hdiag, const double* __restrict__ sc,
                                   const uint8_t* __restrict__ pconst, double radius, double min_diag, double max_diag,
-                                  double* __restrict__ bvec, int fill_upper) {
+                                  double* __restrict__ bvec) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const int i = blockIdx.y;
-  if (j >= D || (!fill_upper && j > i)) return;
+  if (j >= D || j > i) return;
   const bool ci = pconst[i] != 0, cj = pconst[j] != 0;
   double v;
   if (ci || cj) {
@@ -340,13 +339,12 @@ __global__ void scale_damp_kernel(int D, int Dpad, double* __restrict__ A, const
   A[(size_t)i * Dpad + j] = v;
   if (i == j) {
     // The scaled right-hand side also becomes row D of the matrix (in the workspace rhs IS row D, so this scales it in
-    // place; the library A/B wants it as column D = row D of its column-major view): the factorisation of the bordered
-    // matrix [[A, b], [b^T, c]] = [[L, 0], [y^T, .]] leaves y = L^-1 b there, i.e. the forward substitution comes out
-    // of the factorisation for free (csrc/ba_solve.cu).  c only has to exceed y^T y.
+    // place): the factorisation of the bordered matrix [[A, b], [b^T, c]] = [[L, 0], [y^T, .]] leaves y = L^-1 b there,
+    // i.e. the forward substitution comes out of the factorisation for free (csrc/ba_solve.cu).  c only has to exceed
+    // y^T y.
     const double b = ci ? 0.0 : rhs[i] * sc[i];
     bvec[i] = b;
-    if (fill_upper) A[(size_t)i * Dpad + D] = b;
-    else A[(size_t)D * Dpad + i] = b;
+    A[(size_t)D * Dpad + i] = b;
     if (i == 0) A[(size_t)D * Dpad + D] = 1e300;
   }
 }
@@ -553,10 +551,6 @@ int launch_z_transpose(int D, int N, int Dpad, const double* W, const double* M,
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
-// 0 (default): the reduced system is kept as a row-major LOWER triangle (csrc/chol.cu); 1: both triangles, for the
-// library factorisation A/B (set by csrc/ba_solve.cu from VGG_CHOL)
-int g_fill_upper = 0;
-
 // reduce-scatter destinations of the running multi-GPU solve (set per iteration by csrc/ba_solve.cu; world <= 1: off)
 FabricDev g_fabric_dev = {0, 0, {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}};
 
@@ -573,8 +567,8 @@ struct SyrkF64State {
 };
 thread_local SyrkF64State g_sf;
 
-// Cmat -= Zt^T Zt: Zt [Kpad][Dpad] (Dpad % 128 == 0, Kpad % 16 == 0), Cmat [Dpad][Dpad] row-major, LOWER triangle (plus
-// the mirror when g_fill_upper; into the fabric destinations of g_fabric_dev / mc_off, see syrk_red_upper)
+// Cmat -= Zt^T Zt: Zt [Kpad][Dpad] (Dpad % 128 == 0, Kpad % 16 == 0), Cmat [Dpad][Dpad] row-major, LOWER triangle (or
+// the fabric destinations of g_fabric_dev / mc_off, see syrk_red_upper)
 int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc_off, cudaStream_t st) {
   VGG_REQUIRE(Dpad % SF_BM == 0 && Kpad % SF_BK == 0, "syrk: Dpad must be a multiple of 128 and Kpad of 16");
   const int nb = Dpad / SF_BM, KB = (Kpad + 63) / 64;
@@ -608,7 +602,7 @@ int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc
   }
   if (hs.nwork == 0) return VGG_OK;
   syrk_f64_kernel<<<std::min(hs.sms, hs.nwork), SF_THREADS, SF_SMEM_BYTES, st>>>(hs.work_dev, hs.nwork, Kpad, Dpad, Zt, Cmat,
-                                                                               mc_off, g_fill_upper, g_fabric_dev);
+                                                                               mc_off, g_fabric_dev);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
@@ -616,7 +610,7 @@ int launch_scale_damp(int D, int Dpad, double* A, const double* rhs, const doubl
                       const uint8_t* pconst, double radius, double min_diag, double max_diag, double* bvec,
                       cudaStream_t st) {
   dim3 grid((D + 255) / 256, D);
-  scale_damp_kernel<<<grid, 256, 0, st>>>(D, Dpad, A, rhs, hdiag, sc, pconst, radius, min_diag, max_diag, bvec, g_fill_upper);
+  scale_damp_kernel<<<grid, 256, 0, st>>>(D, Dpad, A, rhs, hdiag, sc, pconst, radius, min_diag, max_diag, bvec);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }

@@ -3,7 +3,6 @@
 // iteration on one stream and ONE small device->host read (accept/reject scalars); track shards on
 // other GPUs join through the caller's all-reduce hook (NCCL over NVLink, see vggsfm_b200/dist.py).
 #include <cublas_v2.h>
-#include <cusolverDn.h>
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -53,12 +52,10 @@ int launch_extract_gvec(int S, int dc, int ns, int KR, const double* camrec, con
 int launch_gradmax(int D, int N, const double* gvec, const uint8_t* pconst, const double* g_p,
                    const uint8_t* point_const, double* scal, cudaStream_t st);
 
-size_t trsv_workspace_ints(int n);
-int launch_trsv_upper(int n, int lda, const double* A, const double* y, size_t y_stride, double* x, int* flags, int epoch,
+int launch_trsv_upper(int n, int lda, const double* A, const double* y, size_t y_stride, double* x, long long* stamps,
                       cudaStream_t st);
 size_t chol_workspace_doubles(int n);
 int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, cudaStream_t st);
-extern int g_fill_upper;       // csrc/ba_schur.cu: 1 = also write the mirror triangle (library factorisation A/B)
 extern FabricDev g_fabric_dev; // csrc/ba_schur.cu: reduce-scatter destinations read by the SYRK epilogue
 int launch_fabric_barrier(const FabricDev& fd, size_t flags_off, unsigned long long epoch, int* err, cudaStream_t st);
 int launch_fabric_gather(const FabricDev& fd, int nrows, int nmat, int ncols_vec, int lda, cudaStream_t st);
@@ -66,7 +63,7 @@ int launch_fabric_allreduce(const FabricDev& fd, size_t flags_off, size_t mail_o
                             unsigned long long epoch, double* vec, int count, int max_slot, int* err, cudaStream_t st);
 
 // gathers the accept/reject scalars into one 24-double record so the host reads them with ONE copy:
-// [0..7] = scal[0..7], [8..15] = small[0..7], [16] = potrf info, [17] = potrs info, [18] = |x|^2
+// [0..7] = scal[0..7], [8..15] = small[0..7], [16] = factorisation info, [17] = substitution info, [18] = |x|^2
 __global__ void pack_scalars_kernel(const double* __restrict__ scal, const double* __restrict__ small,
                                     const int* __restrict__ info, double* __restrict__ out) {
   const int i = threadIdx.x;
@@ -167,15 +164,12 @@ struct Layout {
   double *small;     // [8 scalars | gvec_candidate Dpad]           (one small all-reduce)
   double *scal;      // [16]
   double *packed;    // [24] scalars gathered for the host
-  double *potrf_work;
   double *chol_diag;
   int *dev_info;
-  int *trsv_flags;
-  size_t potrf_lwork;
   size_t bytes;
 };
 
-static int make_layout(int S, int N, int model, int mode, void* base, size_t cap, size_t potrf_lwork, Layout* L) {
+static int make_layout(int S, int N, int model, int mode, void* base, size_t cap, Layout* L) {
   int dc, ns, KR;
   if (dims_of(model, mode, &dc, &ns, &KR) != VGG_OK) {
     set_error("bad camera_model/intr_mode");
@@ -210,11 +204,8 @@ static int make_layout(int S, int N, int model, int mode, void* base, size_t cap
   L->small = c.take<double>(8 + (size_t)L->Dpad);
   L->scal = c.take<double>(16);
   L->packed = c.take<double>(32);
-  L->potrf_lwork = potrf_lwork;
-  L->potrf_work = c.take<double>(potrf_lwork);
   L->chol_diag = c.take<double>(chol_workspace_doubles(L->D + 1));
   L->dev_info = c.take<int>(4);
-  L->trsv_flags = c.take<int>(trsv_workspace_ints(L->D));
   L->bytes = align_up(c.off, 256);
   if (base && c.off > cap) {
     set_error("workspace too small: need %zu bytes, have %zu", c.off, cap);
@@ -223,44 +214,12 @@ static int make_layout(int S, int N, int model, int mode, void* base, size_t cap
   return VGG_OK;
 }
 
-static cusolverDnHandle_t get_cusolver() {
-  static thread_local cusolverDnHandle_t h = nullptr;
-  if (!h) {
-    if (cusolverDnCreate(&h) != CUSOLVER_STATUS_SUCCESS) h = nullptr;
-  }
-  return h;
-}
-
 static cublasHandle_t get_cublas() {
   static thread_local cublasHandle_t h = nullptr;
   if (!h) {
     if (cublasCreate(&h) != CUBLAS_STATUS_SUCCESS) h = nullptr;
   }
   return h;
-}
-
-// Doubles of device scratch the factorisation needs at order D+1 (bordered system): the larger of the 32-bit
-// cusolverDnDpotrf and the 64-bit cusolverDnXpotrf requirement, so one carved region serves either call.
-static int potrf_lwork(int D, int Dpad, size_t* lwork) {
-  cusolverDnHandle_t h = get_cusolver();
-  if (!h) {
-    set_error("cusolverDnCreate failed");
-    return VGG_ESOLVER;
-  }
-  int lw = 0;
-  if (cusolverDnDpotrf_bufferSize(h, CUBLAS_FILL_MODE_LOWER, D + 1, nullptr, Dpad, &lw) != CUSOLVER_STATUS_SUCCESS) {
-    set_error("cusolverDnDpotrf_bufferSize failed");
-    return VGG_ESOLVER;
-  }
-  size_t need = (size_t)lw;
-  static thread_local cusolverDnParams_t xp = nullptr;
-  if (!xp) cusolverDnCreateParams(&xp);
-  size_t db = 0, hb = 0;
-  if (xp && cusolverDnXpotrf_bufferSize(h, xp, CUBLAS_FILL_MODE_LOWER, D + 1, CUDA_R_64F, nullptr, Dpad, CUDA_R_64F, &db, &hb) ==
-                CUSOLVER_STATUS_SUCCESS)
-    need = need > (db + 7) / 8 ? need : (db + 7) / 8;
-  *lwork = need;
-  return VGG_OK;
 }
 
 // Layout of the symmetric allocation of fabric v2 (doubles): two copies of the reduced system (iteration parity, so a
@@ -311,7 +270,6 @@ extern BandDev g_band_dev;                    // csrc/ba_schur.cu: device tables
 struct SolveGuard {
   ~SolveGuard() {
     g_fabric_dev.world = 0;
-    g_fill_upper = 0;
     g_syrk_kb_ranges.clear();
     g_chol_band_end.clear();
     g_chol_arrow_blk = 0;
@@ -552,17 +510,8 @@ int vgg_ba_camrec_len(int camera_model, int intr_mode) {
 
 int vgg_ba_workspace_bytes(int S, int N, int camera_model, int intr_mode, size_t* bytes) {
   VGG_REQUIRE(S > 0 && N > 0 && bytes, "S, N must be positive");
-  int dc, ns;
-  if (dims_of(camera_model, intr_mode, &dc, &ns, nullptr) != VGG_OK) {
-    set_error("bad camera_model/intr_mode");
-    return VGG_EINVAL;
-  }
-  const int D = S * dc + ns;
-  size_t lwork = 0;
-  int rc = potrf_lwork(D, (int)align_up((size_t)D + 2, 128), &lwork);
-  if (rc) return rc;
   Layout L;
-  rc = make_layout(S, N, camera_model, intr_mode, nullptr, 0, lwork, &L);
+  const int rc = make_layout(S, N, camera_model, intr_mode, nullptr, 0, &L);
   if (rc) return rc;
   *bytes = L.bytes;
   return VGG_OK;
@@ -584,13 +533,8 @@ int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double*
   VGG_REQUIRE(prob && workspace && Sraw && rhs, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   g_launch_count = 0;
-  size_t lwork = 0;
-  int dc, ns;
-  dims_of(prob->camera_model, prob->intr_mode, &dc, &ns, nullptr);
-  int rc = potrf_lwork(prob->S * dc + ns, (int)align_up((size_t)(prob->S * dc + ns) + 2, 128), &lwork);
-  if (rc) return rc;
   Layout L;
-  rc = make_layout(prob->S, prob->N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, lwork, &L);
+  int rc = make_layout(prob->S, prob->N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L);
   if (rc) return rc;
   BlockSet b;
   b.cost = nullptr;
@@ -674,17 +618,9 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     return VGG_EINVAL;
   }
   const int D = S * dc + ns;
-  size_t lwork = 0;
-  int rc = potrf_lwork(D, (int)align_up((size_t)D + 2, 128), &lwork);
-  if (rc) return rc;
   Layout L;
-  rc = make_layout(S, N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, lwork, &L);
+  int rc = make_layout(S, N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L);
   if (rc) return rc;
-  cusolverDnHandle_t cs = get_cusolver();
-  if (cusolverDnSetStream(cs, st) != CUSOLVER_STATUS_SUCCESS) {
-    set_error("cusolverDnSetStream failed");
-    return VGG_ESOLVER;
-  }
   const size_t ar_count = (size_t)D * L.Dpad + 3 * (size_t)L.Dpad;
   // fabric mode: the reduced system lives in symmetric (peer-mapped) memory and is reduced by multimem operations
   // issued from the producing kernels; mc_off is the distance from a local address to its multicast twin
@@ -733,14 +669,6 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     if (allreduce) return allreduce(ar_user, vec, count, op, st);
     return VGG_OK;
   };
-  // factorisation: 2 = csrc/chol.cu (default), 0 = cuSOLVER Xpotrf (VGG_CHOL=lib), 1 = cuSOLVER Dpotrf (VGG_CHOL=legacy)
-  static const int chol_mode = [] {
-    const char* e = getenv("VGG_CHOL");
-    if (!e || !e[0] || e[0] == 'o') return 2;
-    return (e[0] == 'l' && e[1] == 'e') ? 1 : 0;
-  }();
-  const int cm = mc_off ? 2 : chol_mode;           // fabric mode reduces the lower triangle only
-  g_fill_upper = cm != 2;
 
   EventPair evs;
   VGG_CUDA_CHECK(cudaEventCreate(&evs.a));
@@ -850,59 +778,17 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     if ((rc = launch_scale_damp(D, L.Dpad, Sraw, rhs, hdiag, L.sc_c, prob->param_const, radius, opt.min_lm_diagonal,
                                 opt.max_lm_diagonal, L.bvec, st)))
       return rc;
-    // Factor the reduced system.  Default: the in-repo blocked Cholesky (csrc/chol.cu) on the row-major LOWER triangle,
-    // of the BORDERED matrix of order D+1 -- scale_damp put the scaled right-hand side into row D, so the factorisation
-    // leaves y = L^-1 b there (and, mirrored like every panel, in column D): the forward substitution costs nothing and
-    // only the backward substitution L^T x = y remains.  VGG_CHOL=lib (cuSOLVER 64-bit potrf on the column-major LOWER
-    // view, r01 default, 1.05 ms at n = 2403) and VGG_CHOL=legacy (32-bit potrf) are kept for A/B; they need the mirror
-    // triangle (g_fill_upper) and are not available in fabric mode.
-    const int nfac = D + 1;
-    if (cm == 2) {
-      if ((rc = chol_lower_inplace(nfac, L.Dpad, Sraw, L.chol_diag, L.dev_info, st))) return rc;
-    } else if (cm == 0) {
-      static thread_local cusolverDnParams_t xp = nullptr;
-      static thread_local void* xdev_fallback = nullptr;
-      static thread_local void* xhost = nullptr;
-      static thread_local size_t xdev_b = 0, xhost_b = 0;
-      if (!xp) cusolverDnCreateParams(&xp);
-      size_t db = 0, hb = 0;
-      if (cusolverDnXpotrf_bufferSize(cs, xp, CUBLAS_FILL_MODE_LOWER, nfac, CUDA_R_64F, Sraw, L.Dpad, CUDA_R_64F, &db, &hb) !=
-          CUSOLVER_STATUS_SUCCESS) {
-        set_error("cusolverDnXpotrf_bufferSize failed");
-        return VGG_ESOLVER;
-      }
-      // device scratch comes out of the caller's workspace (sized by potrf_lwork); the cudaMalloc below only runs if
-      // a library version asks for more at solve time than it reported when the workspace was sized
-      void* xdev = L.potrf_work;
-      if (db > L.potrf_lwork * sizeof(double)) {
-        if (db > xdev_b) { if (xdev_fallback) cudaFree(xdev_fallback); VGG_CUDA_CHECK(cudaMalloc(&xdev_fallback, db)); xdev_b = db; }
-        xdev = xdev_fallback;
-      }
-      if (hb > xhost_b) { free(xhost); xhost = malloc(hb); xhost_b = hb; }
-      if (cusolverDnXpotrf(cs, xp, CUBLAS_FILL_MODE_LOWER, nfac, CUDA_R_64F, Sraw, L.Dpad, CUDA_R_64F, xdev, db, xhost, hb,
-                           L.dev_info) != CUSOLVER_STATUS_SUCCESS) {
-        set_error("cusolverDnXpotrf failed to launch");
-        return VGG_ESOLVER;
-      }
-      g_launch_count += 1;
-    } else {
-      if (cusolverDnDpotrf(cs, CUBLAS_FILL_MODE_LOWER, nfac, Sraw, L.Dpad, L.potrf_work, (int)L.potrf_lwork, L.dev_info) !=
-          CUSOLVER_STATUS_SUCCESS) {
-        set_error("cusolverDnDpotrf failed to launch");
-        return VGG_ESOLVER;
-      }
-      g_launch_count += 1;
-    }
-    // Backward substitution on U = L^T (the row-major upper triangle in every mode), y = column D of the buffer.
+    // Factor the reduced system with the in-repo blocked Cholesky (csrc/chol.cu) on the row-major LOWER triangle of the
+    // BORDERED matrix of order D+1 -- scale_damp put the scaled right-hand side into row D, so the factorisation leaves
+    // y = L^-1 b there (and, mirrored like every panel, in column D): the forward substitution costs nothing and only the
+    // backward substitution L^T x = y remains.  (cuSOLVER potrf on the same matrix took 1.05 ms at n = 2403, this 0.93.)
+    if ((rc = chol_lower_inplace(D + 1, L.Dpad, Sraw, L.chol_diag, L.dev_info, st))) return rc;
+    // Backward substitution on U = L^T (the row-major upper triangle), y = column D of the buffer.
     const double* dcs = L.bvec;
     size_t dcs_stride = 1;
     {
-      static const bool lib_trsv = [] {
-        const char* e = getenv("VGG_TRSV");
-        return e && e[0] == 'c';                     // VGG_TRSV=cublas keeps the library call for A/B
-      }();
       VGG_CUDA_CHECK(cudaMemsetAsync(L.dev_info + 1, 0, sizeof(int), st));
-      if (lib_trsv || D > 7000) {                     // own kernel: one co-resident wave of D/64 CTAs
+      if (D > 7000) {                                 // beyond the own kernel's one co-resident wave of D/64 CTAs
         cublasHandle_t cb = get_cublas();
         if (!cb || cublasSetStream(cb, st) != CUBLAS_STATUS_SUCCESS) {
           set_error("cublasCreate / cublasSetStream failed");
@@ -917,8 +803,8 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
         dcs = Sraw + D;
         dcs_stride = (size_t)L.Dpad;
       } else {
-        // own backward substitution (csrc/trsv.cu): one launch, block rows chained through flags
-        if ((rc = launch_trsv_upper(D, L.Dpad, Sraw, Sraw + D, (size_t)L.Dpad, L.bvec, L.trsv_flags, 1, st))) return rc;
+        // own backward substitution (csrc/trsv.cu): one launch, block rows chained through the solution itself
+        if ((rc = launch_trsv_upper(D, L.Dpad, Sraw, Sraw + D, (size_t)L.Dpad, L.bvec, nullptr, st))) return rc;
       }
     }
     if ((rc = launch_cam_step(D, dcs, dcs_stride, L.sc_c, hdiag, gvec, prob->param_const, radius, opt.min_lm_diagonal,

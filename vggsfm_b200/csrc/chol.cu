@@ -15,8 +15,8 @@
 //                       both operands in shared memory at a time (68 KB) so that its CTAs run NEXT TO the panel CTAs of
 //                       the following step (<= 155 KB with xr <= 20) on the same SMs.
 // Every MMA is mma.sync.m16n8k16.f64 (dmma_m16n8k16, full FP64 tensor rate on sm_90; m8n8k4 runs at half of it).
-// The whole launch sequence is captured once per (matrix, order) into a CUDA graph.  Switches for A/B runs:
-// VGG_CHOL_LOOKAHEAD=0 (everything in program order), VGG_CHOL_GRAPH=0, VGG_CHOL_LEAF=0.
+// The whole launch sequence is captured once per (matrix, order) into a CUDA graph; VGG_CHOL_GRAPH=0 launches it
+// directly instead.  Matrices of fewer than three blocks are factored in program order (no fused update, no side streams).
 #include <stdlib.h>
 #include <algorithm>
 #include <map>
@@ -63,14 +63,14 @@ __device__ __forceinline__ double fast_rsqrt(double p) {
 }
 constexpr double CHOL_PMIN = 2.2250738585072014e-308;      // smallest normal double: pivots below it count as non-positive
 
-// LEAF selects the 8x8 leaf (0: one pivot per step, 1: two pivots per step); PROBE adds clock64 phase counters for
-// tools/microbench.py chol128 (threads 0 and 32 = warp 0 / warp 1; prof[warp][phase], see the MARK sites).
+// PROBE adds clock64 phase counters for tools/microbench.py chol128 (threads 0 and 32 = warp 0 / warp 1;
+// prof[warp][phase], see the MARK sites).
 //
 // xr (0 or C_RPC .. C_RPC_MAX) extra rows stored right below the block (rows 128 .. 128+xr-1 of Ls) ride along: they
 // take part in the micro-panel solves and in the rank-8 / rank-32 updates, so when the block is factored they hold
 // X = A_ik L^-T -- the panel rows this CTA owns -- with no separate triangular solve afterwards (r02: that solve was a 128-step
 // multiply/shuffle/FMA chain, ~3 us after every POTRF128, plus a transposing pass over the block to feed it).
-template <int LEAF, bool PROBE>
+template <bool PROBE>
 __device__ __forceinline__ int cta_chol128(double* Ls, double* dinv, int* fail_sm, int tid, int xr,
                                            long long* prof = nullptr) {
   const int lane = tid & 31, warp = tid >> 5;
@@ -105,7 +105,7 @@ __device__ __forceinline__ int cta_chol128(double* Ls, double* dinv, int* fail_s
   // back to the sequential formula (warp-uniform branch).  A shuffle-free variant (every lane holds the whole
   // 36-element triangle) measured SLOWER: panel 51.6 vs 48.6 us -- 36 broadcast loads + 64 predicated stores per leaf
   // cost more than the shuffles they replace.
-  auto leaf1 = [&](int c0) {
+  auto leaf = [&](int c0) {
     double a[8];
     const int r = c0 + (lane & 7);
 #pragma unroll
@@ -166,49 +166,6 @@ __device__ __forceinline__ int cta_chol128(double* Ls, double* dinv, int* fail_s
       for (int c = 0; c < 8; ++c) Lh[lane * 8 + c] = (c < lane) ? a[c] * mydinv : 0.0;
     }
     if (lane == 0 && fail && *fail_sm == 0) *fail_sm = fail;
-  };
-  // one pivot per step (the r02 default until the two-pivot leaf; kept for A/B through the probe)
-  auto leaf0 = [&](int c0) {
-    double a[8];
-    const int r = c0 + (lane & 7);
-#pragma unroll
-    for (int c = 0; c < 8; c += 2) {
-      const double2 v = *reinterpret_cast<const double2*>(Ls + r * CLD + c0 + c);
-      a[c] = v.x;
-      a[c + 1] = v.y;
-    }
-    int fail = 0;
-    double mydinv = 1.0;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const double pj = __shfl_sync(0xffffffffu, a[j], j);
-      double inv = fast_rsqrt(pj);
-      if (!(pj >= CHOL_PMIN)) {                               // uniform; tested in the shadow of the rsqrt chain
-        if (fail == 0) fail = c0 + j + 1;
-        inv = 1.0;
-      }
-      a[j] = a[j] * inv;                                      // lane j: pj * inv = sqrt(pj)
-      if (lane == j) {
-        dinv[c0 + j] = inv;
-        mydinv = inv;
-      }
-#pragma unroll
-      for (int c = j + 1; c < 8; ++c) {
-        const double lc = __shfl_sync(0xffffffffu, a[j], c);
-        if (lane >= c) a[c] = fma(-a[j], lc, a[c]);
-      }
-    }
-    if (lane < 8) {
-#pragma unroll
-      for (int c = 0; c < 8; ++c) Ls[r * CLD + c0 + c] = (c <= lane) ? a[c] : 0.0;
-#pragma unroll
-      for (int c = 0; c < 8; ++c) Lh[lane * 8 + c] = (c < lane) ? a[c] * mydinv : 0.0;
-    }
-    if (lane == 0 && fail && *fail_sm == 0) *fail_sm = fail;
-  };
-  auto leaf = [&](int c0) {
-    if constexpr (LEAF == 0) leaf0(c0);
-    else leaf1(c0);
   };
   // C[r][j] -= sum_k L[r][c0+k] L[j][c0+k] for j = jb, jb+js, ... <= jend (two columns in flight)
   auto row_update = [&](int r, int c0, int jb, int js, int jend) {
@@ -425,7 +382,6 @@ __device__ __forceinline__ int cta_chol128(double* Ls, double* dinv, int* fail_s
 }
 
 // one-CTA probe: factor a 128 x 128 block `reps` times (reloading it each time), report the cycles of the last pass
-template <int LEAF>
 __global__ void __launch_bounds__(C_THREADS, 1) chol128_probe_kernel(const double* __restrict__ A, double* __restrict__ L,
                                                                       long long* __restrict__ prof, int reps, int xr) {
   extern __shared__ __align__(16) double cp_smem[];
@@ -439,7 +395,7 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol128_probe_kernel(const doubl
       cp_smem[(CB + (e >> 7)) * CLD + (e & 127)] = A[(CB - xr + (e >> 7)) * CB + (e & 127)];
     __syncthreads();
     const long long t0 = clock64();
-    cta_chol128<LEAF, true>(cp_smem, dinv, &fail_sm, tid, xr, prof);
+    cta_chol128<true>(cp_smem, dinv, &fail_sm, tid, xr, prof);
     __syncthreads();
     total = clock64() - t0;
   }
@@ -465,7 +421,6 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol128_probe_kernel(const doubl
 constexpr int CHOL_SPIN_LIMIT = 1 << 22;
 constexpr int CHOL_INFO_STALLED = 0x7fffffff;
 
-template <int LEAF>
 __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda, int k0, double* __restrict__ A,
                                                                    double* __restrict__ Ldiag /*[nblk][128*128]*/,
                                                                    int* __restrict__ info, int* __restrict__ flags,
@@ -505,7 +460,7 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
   cp_async_commit();
   cp_async_wait<0>();
   __syncthreads();
-  const int fail = cta_chol128<LEAF, false>(Ls, dinv, &fail_sm, tid, xr);
+  const int fail = cta_chol128<false>(Ls, dinv, &fail_sm, tid, xr);
   if (fail && blockIdx.x == 0 && tid == 0) atomicCAS(info, 0, k0 + fail);
   if (!solver) {
     // the last panel has no other CTA that could still be loading the block: its factor goes straight into place
@@ -646,7 +601,7 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
 
 // A[t0.., t0..] -= P P^T (lower part), P = A[t0.., k0..k0+127]: one 64 x 64 tile (bi, bj), bj <= bi, per CTA; 8 warps
 // 2 x 4, warp tile 32 x 16 = two m16 x two n8 DMMA tiles.  Which tiles (tile columns counted from t0):
-//   CU_ALL   every tile (the program-order schedule, VGG_CHOL_LOOKAHEAD=0)
+//   CU_ALL   every tile (the program-order schedule of matrices with fewer than three blocks)
 //   CU_NEXT  tile columns 2 and 3 = block column k+2, which the fused panel kernel of the next step is adding into at
 //            the same time: f64 REDs
 //   CU_REST  tile columns >= 4 (REDs on 4 and 5: block column k+3 is shared with CU_NEXT of the next step)
@@ -803,12 +758,6 @@ int chol_streams(CholStreams** out) {
   return VGG_OK;
 }
 
-// VGG_CHOL_LEAF=0|1 (A/B): 8x8 leaf with one / two (default) pivots per step
-int chol_leaf() {
-  static const int v = [] { const char* e = getenv("VGG_CHOL_LEAF"); return (e && e[0] == '0') ? 0 : 1; }();
-  return v;
-}
-
 // SMs of the current device, queried once: the panel kernel's grid is sized to fit them in one wave
 int chol_sms() {
   static const int v = [] {
@@ -823,9 +772,7 @@ int chol_sms() {
 int chol_set_attrs() {
   static bool done = false;
   if (done) return VGG_OK;
-  VGG_CUDA_CHECK(cudaFuncSetAttribute(chol_panel_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)(sizeof(double) * (CB + C_RPC_MAX) * CLD)));
-  VGG_CUDA_CHECK(cudaFuncSetAttribute(chol_panel_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  VGG_CUDA_CHECK(cudaFuncSetAttribute(chol_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)(sizeof(double) * (CB + C_RPC_MAX) * CLD)));
   VGG_CUDA_CHECK(cudaFuncSetAttribute(chol_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)(sizeof(double) * 2 * CT * CUD)));
@@ -859,9 +806,9 @@ int chol_panel_rows(int below1, int below2, int* chunks) {
 }
 
 // The launch sequence on st (+ the side streams).
-//   lookahead (default): step(b) = panel b + its fused update of block column b+1, on st back to back; the rest of
-//     panel b's trailing update runs on the side streams behind step(b): U1(b) = block column b+2 (CU_NEXT, needed by
-//     step(b+2)) and U2(b) = block columns >= b+3 (CU_REST, needed by step(b+3)).
+//   lookahead (three or more blocks): step(b) = panel b + its fused update of block column b+1, on st back to back; the
+//     rest of panel b's trailing update runs on the side streams behind step(b): U1(b) = block column b+2 (CU_NEXT,
+//     needed by step(b+2)) and U2(b) = block columns >= b+3 (CU_REST, needed by step(b+3)).
 //   lookahead == false: everything on st in program order (one CU_ALL update per panel, no fused update).
 int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags, cudaStream_t st, CholStreams* cs,
                  bool lookahead) {
@@ -887,10 +834,7 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
     const int xr = chol_panel_rows(below1, below2, &chunks);
     const size_t smem_p = sizeof(double) * (CB + xr) * CLD;
     const int fuse = lookahead ? 1 : 0;
-    if (chol_leaf() == 1)
-      chol_panel_kernel<1><<<1 + chunks, C_THREADS, smem_p, st>>>(n, lda, k0, A, Ldiag, info, flags, fuse, band_end, arrow_lo, xr);
-    else
-      chol_panel_kernel<0><<<1 + chunks, C_THREADS, smem_p, st>>>(n, lda, k0, A, Ldiag, info, flags, fuse, band_end, arrow_lo, xr);
+    chol_panel_kernel<<<1 + chunks, C_THREADS, smem_p, st>>>(n, lda, k0, A, Ldiag, info, flags, fuse, band_end, arrow_lo, xr);
     VGG_LAUNCH_CHECK();
     return VGG_OK;
   };
@@ -954,7 +898,7 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
 
 // In-place Cholesky of the row-major lower triangle of A[n x n] (lda even, A 16-byte aligned): on return the lower
 // triangle holds L and the strict upper triangle L^T.  info (device int): 0 or the 1-based index of the first
-// non-positive pivot.  VGG_CHOL_LOOKAHEAD=0 / VGG_CHOL_GRAPH=0 switch the side stream / the CUDA graph off (A/B).
+// non-positive pivot.  VGG_CHOL_GRAPH=0 switches the CUDA graph off.
 int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, cudaStream_t st) {
   VGG_REQUIRE((lda % 2) == 0, "lda must be even");
   int rc;
@@ -963,24 +907,23 @@ int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, cuda
   const int nblk0 = (n + CB - 1) / CB;
   int* flags = reinterpret_cast<int*>(Ldiag + (size_t)nblk0 * CB * CB);
   VGG_CUDA_CHECK(cudaMemsetAsync(flags, 0, sizeof(int) * (size_t)nblk0, st));
-  static const bool lookahead = [] { const char* e = getenv("VGG_CHOL_LOOKAHEAD"); return !(e && e[0] == '0'); }();
   static const bool use_graph = [] { const char* e = getenv("VGG_CHOL_GRAPH"); return !(e && e[0] == '0'); }();
   const int nblk = (n + CB - 1) / CB;
   CholStreams* cs = nullptr;
   if ((rc = chol_streams(&cs))) return rc;
-  if (nblk < 3 || !use_graph) return chol_enqueue(n, lda, A, Ldiag, info, flags, st, cs, lookahead && nblk >= 3);
+  if (nblk < 3 || !use_graph) return chol_enqueue(n, lda, A, Ldiag, info, flags, st, cs, nblk >= 3);
   // one captured graph per (matrix, order): ~60 launches + events become a single cudaGraphLaunch
-  typedef std::tuple<double*, int, int, int*, double*, bool, unsigned long long> Key;
+  typedef std::tuple<double*, int, int, int*, double*, unsigned long long> Key;
   static thread_local std::map<Key, cudaGraphExec_t> cache;
   unsigned long long band_hash = (unsigned long long)g_chol_arrow_blk;
   for (int v : g_chol_band_end) band_hash = band_hash * 1000003ull + (unsigned long long)(v + 1);
-  const Key key(A, n, lda, info, Ldiag, lookahead, band_hash);
+  const Key key(A, n, lda, info, Ldiag, band_hash);
   auto it = cache.find(key);
   if (it == cache.end()) {
     const long long launches_before = g_launch_count;
     cudaGraph_t graph = nullptr;
     VGG_CUDA_CHECK(cudaStreamBeginCapture(cs->cap, cudaStreamCaptureModeThreadLocal));
-    rc = chol_enqueue(n, lda, A, Ldiag, info, flags, cs->cap, cs, lookahead);
+    rc = chol_enqueue(n, lda, A, Ldiag, info, flags, cs->cap, cs, true);
     const cudaError_t ce = cudaStreamEndCapture(cs->cap, &graph);
     g_launch_count = launches_before;
     if (rc) {
@@ -1005,7 +948,7 @@ int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, cuda
 }  // namespace vgg
 
 // tools/microbench.py chol128: one CTA, POTRF128 of A (host, row-major SPD 128 x 128), cycles per phase
-extern "C" int vgg_dev_chol128_probe(int leaf, int reps, const double* A_host, double* L_host, long long* prof13_host) {
+extern "C" int vgg_dev_chol128_probe(int reps, const double* A_host, double* L_host, long long* prof13_host) {
   using namespace vgg;
   VGG_REQUIRE(A_host && L_host && prof13_host && reps > 0, "chol128 probe: bad arguments");
   double *dA = nullptr, *dL = nullptr;
@@ -1016,13 +959,8 @@ extern "C" int vgg_dev_chol128_probe(int leaf, int reps, const double* A_host, d
   VGG_CUDA_CHECK(cudaMemcpy(dA, A_host, sizeof(double) * CB * CB, cudaMemcpyHostToDevice));
   VGG_CUDA_CHECK(cudaMemset(dP, 0, sizeof(long long) * 13));
   const int smem = (int)(sizeof(double) * (CB + C_RPC) * CLD);
-  if (leaf == 1) {
-    VGG_CUDA_CHECK(cudaFuncSetAttribute(chol128_probe_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    chol128_probe_kernel<1><<<1, C_THREADS, smem>>>(dA, dL, dP, reps, C_RPC);
-  } else {
-    VGG_CUDA_CHECK(cudaFuncSetAttribute(chol128_probe_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    chol128_probe_kernel<0><<<1, C_THREADS, smem>>>(dA, dL, dP, reps, C_RPC);
-  }
+  VGG_CUDA_CHECK(cudaFuncSetAttribute(chol128_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  chol128_probe_kernel<<<1, C_THREADS, smem>>>(dA, dL, dP, reps, C_RPC);
   VGG_LAUNCH_CHECK();
   VGG_CUDA_CHECK(cudaDeviceSynchronize());
   VGG_CUDA_CHECK(cudaMemcpy(L_host, dL, sizeof(double) * CB * CB, cudaMemcpyDeviceToHost));

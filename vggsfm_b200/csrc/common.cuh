@@ -195,26 +195,23 @@ __device__ __forceinline__ double warp_max(double r) {
 
 // Epilogue of the Schur SYRK kernels (csrc/ba_schur.cu, csrc/syrk_i8.cu): subtract v = (Zt^T Zt)[r][col] of an UPPER
 // tile (row block of r <= column block bj of col; diag: the two blocks are the same).  The element goes to its mirror
-// (col, r) of the row-major LOWER triangle, which is what csrc/chol.cu factors; the direct element (r, col) is only
-// written for the library factorisation A/B (fill_upper).  Destinations of the lower triangle:
+// (col, r) of the row-major LOWER triangle, which is what csrc/chol.cu factors; nothing is written above the diagonal.
+// Destinations of the lower triangle:
 //   fd.world > 1   reduce-scatter: row block bj lives on rank (bj mod world) until the gather (csrc/fabric.cu); one
 //                  system-scope RED over NVLink per element, only into the owner's copy
 //   mc_off != 0    one multimem RED on the NVSwitch multicast address, landing in every rank's copy
 //   otherwise      a local f64 RED
 __device__ __forceinline__ void syrk_red_upper(double* Cmat, int Dpad, int r, int col, int bj, bool diag, double v,
-                                               ptrdiff_t mc_off, int fill_upper, const FabricDev& fd) {
-  if (v == 0.0) return;
-  if (!diag || col >= r) {
-    const size_t off = (size_t)col * Dpad + r;
-    if (fd.world > 1) {
-      asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(fd.peer[bj % fd.world] + off), "d"(-v) : "memory");
-    } else if (mc_off) {
-      asm volatile("multimem.red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(Cmat + off + mc_off), "d"(-v) : "memory");
-    } else {
-      atomicAdd(Cmat + off, -v);
-    }
+                                               ptrdiff_t mc_off, const FabricDev& fd) {
+  if (v == 0.0 || (diag && col < r)) return;
+  const size_t off = (size_t)col * Dpad + r;
+  if (fd.world > 1) {
+    asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(fd.peer[bj % fd.world] + off), "d"(-v) : "memory");
+  } else if (mc_off) {
+    asm volatile("multimem.red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(Cmat + off + mc_off), "d"(-v) : "memory");
+  } else {
+    atomicAdd(Cmat + off, -v);
   }
-  if (fill_upper && (!diag || col > r)) atomicAdd(&Cmat[(size_t)r * Dpad + col], -v);
 }
 #endif  // __CUDACC__
 

@@ -320,10 +320,9 @@ static int launch_corr(int BS, int N, int C, int L, int R, const CorrLevels& lv,
     VGG_LAUNCH_CHECK();                                                                                            \
     return VGG_OK;                                                                                                 \
   }
-  // C = 32: position-per-lane kernel (VGG_CORR_C32=0 keeps the channel-per-lane one for A/B); pointers must be 16-byte
-  // aligned, which every level of an NHWC pyramid with C = 32 is
-  static const bool c32 = [] { const char* e = getenv("VGG_CORR_C32"); return !(e && e[0] == '0'); }();
-  if (C == 32 && c32 && (R == 3 || R == 4) && (reinterpret_cast<uintptr_t>(targets) & 15) == 0) {
+  // C = 32: position-per-lane kernel; pointers must be 16-byte aligned, which every level of an NHWC pyramid with C = 32
+  // is (otherwise the channel-per-lane kernel below)
+  if (C == 32 && (R == 3 || R == 4) && (reinterpret_cast<uintptr_t>(targets) & 15) == 0) {
     bool aligned = true;
     for (int l = 0; l < L; ++l) aligned = aligned && (reinterpret_cast<uintptr_t>(lv.fmap[l]) & 15) == 0;
     if (aligned) {

@@ -9,11 +9,11 @@ extern "C" {
  * and returns the elapsed milliseconds of the most recent launch. */
 int vgg_dev_blocks_timing(int enable);
 int vgg_dev_blocks_last_ms(double* ms);
-/* One-CTA probe of the in-shared-memory POTRF128 of csrc/chol.cu (leaf 0|1 = one / two pivots per 8x8 leaf step):
- * A_host row-major SPD 128 x 128, L_host its factor, prof13_host[0..5] = cycles per phase seen by warp 0, [6..11] by
- * warp 1 (0 first leaf, 1 TRSM of the micro-panel, 2 look-ahead section work, 3 wait at its barrier, 4 rank-32 DMMA
- * update, 5 first leaf of the next sub-panel), [12] = total cycles of the last of `reps` passes. */
-int vgg_dev_chol128_probe(int leaf, int reps, const double* A_host, double* L_host, long long* prof13_host);
+/* One-CTA probe of the in-shared-memory POTRF128 of csrc/chol.cu: A_host row-major SPD 128 x 128, L_host its factor,
+ * prof13_host[0..5] = cycles per phase seen by warp 0, [6..11] by warp 1 (0 first leaf, 1 TRSM of the micro-panel,
+ * 2 look-ahead section work, 3 wait at its barrier, 4 rank-32 DMMA update, 5 first leaf of the next sub-panel),
+ * [12] = total cycles of the last of `reps` passes. */
+int vgg_dev_chol128_probe(int reps, const double* A_host, double* L_host, long long* prof13_host);
 /* Band hint of the tensor-core SYRK for tests: ranges_host[2*rb], [2*rb+1] = the 64-row k-block range outside which the
  * 128-column row block rb of Zt is exactly zero (count = 2 * Dpad/128; count = 0 clears it).  vgg_ba_solve computes the
  * same thing from the visibility mask and clears it when it returns. */

@@ -191,7 +191,7 @@ __global__ void __launch_bounds__(OZ_THREADS, 1)
     oz_syrk_kernel(const __grid_constant__ OzPlan plan, const OzWork* __restrict__ work, int nwork, int KB,
                    const int8_t* __restrict__ slices, size_t slice_stride, const int* __restrict__ expo,
                    const double* __restrict__ pow2, int Dpad, double* __restrict__ Cmat, ptrdiff_t mc_off,
-                   int fill_upper, const __grid_constant__ FabricDev fd) {
+                   const __grid_constant__ FabricDev fd) {
   extern __shared__ __align__(1024) uint8_t oz_smem[];
   uint8_t* tiles = reinterpret_cast<uint8_t*>(align_up(reinterpret_cast<size_t>(oz_smem), 1024));
   uint64_t* full = reinterpret_cast<uint64_t*>(tiles + (size_t)OZ_STAGES * OZ_STAGE_BYTES);
@@ -305,7 +305,7 @@ __global__ void __launch_bounds__(OZ_THREADS, 1)
           if (er == OZ_EXPO_BAD || ec == OZ_EXPO_BAD) v = __longlong_as_double(0x7ff8000000000000LL);
           else if (tame && ec > -400 && ec < 400) v = v * sr * pow2[col];
           else v = ldexp(v, er + ec + g.exp_base);
-          syrk_red_upper(Cmat, Dpad, r, col, wk.bj, diag, v, mc_off, fill_upper, fd);
+          syrk_red_upper(Cmat, Dpad, r, col, wk.bj, diag, v, mc_off, fd);
         }
     }
   }
@@ -392,8 +392,7 @@ size_t oz_workspace_bytes(int Kpad, int Dpad, int s) {
 size_t syrk_i8_workspace_bytes(int Kpad, int Dpad, int slices) { return oz_workspace_bytes(Kpad, Dpad, slices); }
 
 // Sraw -= Zt^T Zt with s int8 slices.  Zt [Kpad][Dpad] (Dpad % 128 == 0), Cmat [Dpad][Dpad] row-major, LOWER triangle
-// written (plus the mirror when g_fill_upper), same contract as launch_syrk.
-extern int g_fill_upper;      // csrc/ba_schur.cu
+// written, same contract as launch_syrk.
 // Band hint of the current solve (csrc/ba_solve.cu): [lo, hi) k-block range per 128-column row block of Zt outside which
 // the block is exactly zero; empty = dense.  Tiles whose two ranges do not intersect are skipped, the others shortened.
 std::vector<int> g_syrk_kb_ranges;
@@ -465,7 +464,7 @@ int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t
   VGG_LAUNCH_CHECK();
   const int grid = std::min(hs.sms, nwork);
   oz_syrk_kernel<<<grid, OZ_THREADS, OZ_SMEM_BYTES, st>>>(hs.plan, work_d, nwork, KB, slices, slice_stride, expo, pow2, Dpad,
-                                                          Cmat, mc_off, g_fill_upper, g_fabric_dev);
+                                                          Cmat, mc_off, g_fabric_dev);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }

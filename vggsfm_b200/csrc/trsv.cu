@@ -10,7 +10,7 @@
 //   * x_b = inv(U_bb) acc (four threads per row), stored element-wise with volatile 8-byte stores.
 // Block rows are handed out in reverse CTA order, so a CTA waits only for CTAs the hardware dispatched before it.
 // Critical path per block: one 64 x 64 tile update + one 64 x 64 mat-vec + one flag hand-off (~1.5 us), 38 blocks.
-// U is the row-major upper triangle (what a column-major LOWER potrf leaves in a row-major buffer): U[i][j] = A[i*lda+j].
+// U is the row-major upper triangle (L^T, which csrc/chol.cu writes above the diagonal): U[i][j] = A[i*lda+j].
 #include "common.cuh"
 #include "dev_probes.h"
 
@@ -22,9 +22,11 @@ constexpr int TS_NB = 64;
 constexpr int TS_THREADS = 256;
 constexpr unsigned long long TS_SENTINEL = 0xffffffffffffffffull;   // x is pre-filled with this NaN pattern
 
+// stamps != nullptr (tools/microbench.py trsv): globaltimer stamps, 6 per block row: kernel entry, diagonal block loaded,
+// inverse ready, every x_j consumed, x_b published, right-hand side ready
 __global__ void __launch_bounds__(TS_THREADS, 1)
     trsv_upper_kernel(int n, int lda, const double* __restrict__ A, const double* __restrict__ y, size_t y_stride,
-                      double* __restrict__ x, int* flags, int epoch, int use_flag) {
+                      double* __restrict__ x, long long* __restrict__ stamps) {
   extern __shared__ __align__(16) double ts_smem[];
   double(*Ud)[TS_NB + 1] = reinterpret_cast<double(*)[TS_NB + 1]>(ts_smem);                            // diagonal block
   double(*Vi)[TS_NB + 1] = reinterpret_cast<double(*)[TS_NB + 1]>(ts_smem + TS_NB * (TS_NB + 1));      // its inverse
@@ -36,15 +38,14 @@ __global__ void __launch_bounds__(TS_THREADS, 1)
   const int rows = min(TS_NB, n - r0);
   const int tid = threadIdx.x;
   const int r = tid >> 2, seg = tid & 3;      // row of the block, 16-column segment
-  // use_flag == 2 (tools/microbench.py trsv): globaltimer stamps into flags (as int64, 5 per block row): kernel entry,
-  // diagonal block loaded, inverse ready, every x_j consumed, x_b published
-  long long* stamps = reinterpret_cast<long long*>(flags);
-  auto now_ns = []() {
-    long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
+  auto stamp = [&](int k) {
+    if (stamps && tid == 0) {
+      long long t;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+      stamps[6 * b + k] = t;
+    }
   };
-  if (use_flag == 2 && tid == 0) stamps[6 * b] = now_ns();
+  stamp(0);
   // this block row's right-hand side, requested FIRST: r02 timestamps showed this one 8-byte load per thread taking
   // ~19 us when it was issued after the inversion (every block row, same absolute completion time) -- and the whole
   // chain waits for the last block row.  Issued here it completes under the block load and the inversion.
@@ -59,7 +60,7 @@ __global__ void __launch_bounds__(TS_THREADS, 1)
     Ud[i][j] = v;
   }
   __syncthreads();
-  if (use_flag == 2 && tid == 0) stamps[6 * b + 1] = now_ns();
+  stamp(1);
   if (tid < TS_NB) xs[tid] = 1.0 / Ud[tid][tid];       // reciprocal pivots (xs is free until the first hop)
   __syncthreads();
   {
@@ -80,11 +81,11 @@ __global__ void __launch_bounds__(TS_THREADS, 1)
     }
   }
   __syncthreads();
-  if (use_flag == 2 && tid == 0) stamps[6 * b + 2] = now_ns();
+  stamp(2);
   // ---- right-hand side rows of this block
   if (tid < TS_NB) accs[tid] = y_mine;
   __syncthreads();
-  if (use_flag == 2 && tid == 0) stamps[6 * b + 5] = now_ns();
+  stamp(5);
 
   // ---- block columns to the right, last first; tile j+... prefetched into registers before its x is awaited
   // three tiles are kept in flight in registers (tiles do not depend on x, only x_j does)
@@ -98,22 +99,10 @@ __global__ void __launch_bounds__(TS_THREADS, 1)
   double acc = 0.0;                            // this thread's partial of row r (its 16-column segment), over all j
   auto hop = [&](const double (&tile)[16], int j) {
     // x_j arrives as data: the buffer was pre-filled with a sentinel NaN pattern, every element is polled by one thread
-    // (8-byte stores are single-copy atomic, so no flag, no fence and no second round trip are needed)
-    if (use_flag == 1) {
-      // ONE thread of the CTA watches block j's flag (with a short back-off), then 64 threads fetch the block through L2.
-      // The data-as-flag variant below has every waiting CTA poll 64 elements: up to 37 CTAs x 64 threads hammer the
-      // four L2 lines of the newest block, and the producer's stores queue behind them.
-      if (tid == 0) {
-        int seen;
-        while (true) {
-          asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(seen) : "l"(flags + j) : "memory");
-          if (seen == epoch) break;
-          __nanosleep(40);
-        }
-      }
-      __syncthreads();
-      if (tid < TS_NB) xs[tid] = (j * TS_NB + tid < n) ? __ldcg(&x[j * TS_NB + tid]) : 0.0;
-    } else if (tid < TS_NB) {
+    // (8-byte stores are single-copy atomic, so no flag, no fence and no second round trip are needed).  One flag per
+    // block row, watched by one thread per CTA, measured slower (160.6 vs 150.6 us at n = 2402): the fence and the flag
+    // round trip cost more than the 64-thread polling they remove.
+    if (tid < TS_NB) {
       double v = 0.0;
       if (j * TS_NB + tid < n) {
         const volatile unsigned long long* src = reinterpret_cast<const volatile unsigned long long*>(&x[j * TS_NB + tid]);
@@ -159,7 +148,7 @@ __global__ void __launch_bounds__(TS_THREADS, 1)
     --j;
   }
   }
-  if (use_flag == 2 && tid == 0) stamps[6 * b + 3] = now_ns();      // every x_j this block row needs has been consumed
+  stamp(3);                                    // every x_j this block row needs has been consumed
   // reduce the four segments of a row, subtract from the right-hand side
   acc += __shfl_xor_sync(0xffffffffu, acc, 1);
   acc += __shfl_xor_sync(0xffffffffu, acc, 2);
@@ -185,28 +174,17 @@ __global__ void __launch_bounds__(TS_THREADS, 1)
       *reinterpret_cast<volatile unsigned long long*>(&x[r0 + r]) = bits;
     }
   }
-  if (use_flag == 2) {
+  if (stamps) {
     __syncthreads();
-    if (tid == 0) stamps[6 * b + 4] = now_ns();
-    return;
-  }
-  if (use_flag) {
-    __syncthreads();                                    // all 64 stores issued
-    if (tid == 0) {
-      __threadfence();
-      asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(flags + b), "r"(epoch) : "memory");
-    }
+    stamp(4);
   }
 }
 
 }  // namespace
 
-size_t trsv_workspace_ints(int n) { return (size_t)((n + TS_NB - 1) / TS_NB) + 1; }
-
-// x = U^-1 y; flags: workspace of trsv_workspace_ints(n) ints that must be zero before the first call and is
-// otherwise left to this function (the last int counts calls so that no reset is needed between them).
-int launch_trsv_upper(int n, int lda, const double* A, const double* y, size_t y_stride, double* x, int* flags,
-                      int epoch, cudaStream_t st) {
+// x = U^-1 y; stamps: nullptr, or 6 int64 per 64-row block row for the timestamps of trsv_upper_kernel
+int launch_trsv_upper(int n, int lda, const double* A, const double* y, size_t y_stride, double* x, long long* stamps,
+                      cudaStream_t st) {
   const int nb = (n + TS_NB - 1) / TS_NB;
   VGG_REQUIRE(nb <= 120, "trsv_upper: n too large for one co-resident wave");
   const size_t smem = sizeof(double) * (2 * TS_NB * (TS_NB + 1) + 2 * TS_NB);
@@ -215,26 +193,16 @@ int launch_trsv_upper(int n, int lda, const double* A, const double* y, size_t y
     VGG_CUDA_CHECK(cudaFuncSetAttribute(trsv_upper_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = true;
   }
-  // VGG_TRSV_POLL=flag: one flag per block row and one polling thread per CTA instead of polling the solution elements
-  // themselves.  Measured r02: 160.6 us against 150.6 us for the data hand-off -- the fence + flag round trip costs more
-  // than the 64-thread polling it removes, so the default stays the data hand-off.
-  static const bool use_flag = [] { const char* e = getenv("VGG_TRSV_POLL"); return e && e[0] == 'f'; }();
-  if (use_flag) {
-    VGG_REQUIRE(flags, "trsv_upper: flag workspace missing");
-    epoch = 1;
-    VGG_CUDA_CHECK(cudaMemsetAsync(flags, 0, sizeof(int) * (size_t)nb, st));    // nobody has published anything yet
-  } else {
-    VGG_CUDA_CHECK(cudaMemsetAsync(x, 0xFF, sizeof(double) * (size_t)n, st));   // sentinel fill: x_j is polled as data
-  }
-  trsv_upper_kernel<<<nb, TS_THREADS, smem, st>>>(n, lda, A, y, y_stride, x, flags, epoch, use_flag ? 1 : 0);
+  VGG_CUDA_CHECK(cudaMemsetAsync(x, 0xFF, sizeof(double) * (size_t)n, st));     // sentinel fill: x_j is polled as data
+  trsv_upper_kernel<<<nb, TS_THREADS, smem, st>>>(n, lda, A, y, y_stride, x, stamps);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
 
 }  // namespace vgg
 
-// tests/test_trsv_gpu.py (stamps_host == NULL): the production launcher on its own.  tools/microbench.py trsv: the kernel
-// with per-block-row timestamps (ns, globaltimer), 6 per block row (see csrc/dev_probes.h)
+// tests/test_trsv_gpu.py (stamps_host == NULL): the production launcher on its own.  tools/microbench.py trsv: the same
+// launch with per-block-row timestamps (ns, globaltimer), 6 per block row (see csrc/dev_probes.h)
 extern "C" int vgg_dev_trsv_probe(int n, int lda, const double* A_dev, const double* y_dev, size_t y_stride, double* x_dev,
                                   long long* stamps_host) {
   using namespace vgg;
@@ -242,25 +210,15 @@ extern "C" int vgg_dev_trsv_probe(int n, int lda, const double* A_dev, const dou
   const int nb = (n + TS_NB - 1) / TS_NB;
   static long long* d = nullptr;                      // allocated once: a cudaMalloc / cudaFree pair per call would put
   static int d_cap = 0;                                // allocator work (and its TLB effects) right in front of the kernel
-  if (d_cap < 6 * nb) {
+  if (stamps_host && d_cap < 6 * nb) {
     if (d) cudaFree(d);
     VGG_CUDA_CHECK(cudaMalloc(&d, sizeof(long long) * 6 * nb));
     d_cap = 6 * nb;
   }
-  VGG_CUDA_CHECK(cudaMemset(d, 0, sizeof(long long) * 6 * nb));
-  if (!stamps_host) {
-    // the zeroed stamp buffer doubles as the flag workspace (>= trsv_workspace_ints(n) ints)
-    const int rc = launch_trsv_upper(n, lda, A_dev, y_dev, y_stride, x_dev, reinterpret_cast<int*>(d), 1, 0);
-    if (rc) return rc;
-    VGG_CUDA_CHECK(cudaDeviceSynchronize());
-    return VGG_OK;
-  }
-  const size_t smem = sizeof(double) * (2 * TS_NB * (TS_NB + 1) + 2 * TS_NB);
-  VGG_CUDA_CHECK(cudaFuncSetAttribute(trsv_upper_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  VGG_CUDA_CHECK(cudaMemset(x_dev, 0xFF, sizeof(double) * (size_t)n));
-  trsv_upper_kernel<<<nb, TS_THREADS, smem>>>(n, lda, A_dev, y_dev, y_stride, x_dev, reinterpret_cast<int*>(d), 1, 2);
-  VGG_LAUNCH_CHECK();
+  if (stamps_host) VGG_CUDA_CHECK(cudaMemset(d, 0, sizeof(long long) * 6 * nb));
+  const int rc = launch_trsv_upper(n, lda, A_dev, y_dev, y_stride, x_dev, stamps_host ? d : nullptr, 0);
+  if (rc) return rc;
   VGG_CUDA_CHECK(cudaDeviceSynchronize());
-  VGG_CUDA_CHECK(cudaMemcpy(stamps_host, d, sizeof(long long) * 6 * nb, cudaMemcpyDeviceToHost));
+  if (stamps_host) VGG_CUDA_CHECK(cudaMemcpy(stamps_host, d, sizeof(long long) * 6 * nb, cudaMemcpyDeviceToHost));
   return VGG_OK;
 }
