@@ -291,6 +291,24 @@ int vgg_relative_pose_from_fundamental(int B, int N, const void* points1, const 
                                        const double* fmat, double width, double height, double* R_out, double* t_out,
                                        double* E_out, void* stream);
 
+/* poselib.estimate_fundamental as estimate_preliminary_cameras_poselib (vggsfm/two_view_geo/estimate_preliminary.py:37-95)
+ * calls it, for B pairs at once: LO-MSAC over the valid matches with PoseLib's seeded sampler, the real-root 7-point
+ * solver with the real focal check, truncated-loss LM local optimisation, PoseLib's dynamic stopping rule, and a
+ * Cauchy polish on the inliers (restated in oracle/poselib_oracle.py).  points1/points2 [B,N,2] float
+ * (points_are_f64 = 0) or double pixels, valid_mask uint8 [B,N] or NULL (all valid), max_error = the epipolar threshold
+ * in pixels (Sampson distance), max_iterations / min_iterations as RansacOptions, seed = RansacOptions.seed (the
+ * reference uses the defaults: min_iterations 1000, seed 0).  Outputs: fmat_out double [B,3,3] (|F|_F = 1, entry of
+ * largest magnitude positive; 0 when a pair has fewer than 7 valid matches or no model), inlier_num_out int32 [B],
+ * inlier_mask_out uint8 [B,N] (invalid matches 0), iterations_out int32 [B] (RANSAC iterations run).  The call
+ * synchronises with `stream` once per chunk of trials.  VGG_EINVAL before any launch when B or N is negative,
+ * B * N >= 2^31, max_iterations < 1, min_iterations < 0 or max_error is not positive and finite. */
+int vgg_msac_fundamental_workspace_bytes(int B, int N, int max_iterations, int min_iterations, size_t* bytes);
+int vgg_estimate_fundamental_msac(int B, int N, const void* points1, const void* points2, int points_are_f64,
+                                  const uint8_t* valid_mask, double max_error, int max_iterations, int min_iterations,
+                                  unsigned long long seed, double* fmat_out, int32_t* inlier_num_out,
+                                  uint8_t* inlier_mask_out, int32_t* iterations_out, void* workspace, size_t ws_bytes,
+                                  void* stream);
+
 /* ------------------------------------------------------------------------------------------- */
 /* Tracker correlation inner loop (float32 math on float or half feature pyramids)             */
 /* ------------------------------------------------------------------------------------------- */

@@ -23,13 +23,13 @@ EXPORTS = [
     "vgg_corr_pyramid_bytes", "vgg_corr_build_pyramid", "vgg_corr_sample", "vgg_sample_features4d",
     "vgg_corr_tc_supported", "vgg_corr_tc_bytes", "vgg_corr_tc_build", "vgg_corr_tc_sample",
     "vgg_twoview_workspace_bytes", "vgg_estimate_fundamental", "vgg_relative_pose_from_fundamental",
-    "vgg_fundamental_inliers",
+    "vgg_fundamental_inliers", "vgg_msac_fundamental_workspace_bytes", "vgg_estimate_fundamental_msac",
 ]
 
 
 # development probes (csrc/dev_probes.h): exported, not part of the public header
 DEV_EXPORTS = ["vgg_dev_blocks_timing", "vgg_dev_blocks_last_ms", "vgg_dev_chol128_probe", "vgg_dev_set_syrk_ranges", "vgg_dev_syrk_f64", "vgg_dev_trsv_probe", "vgg_dev_set_chol_band",
-               "vgg_dev_last_band_hint"]
+               "vgg_dev_last_band_hint", "vgg_dev_msac_trace"]
 
 
 class BAProblem(ctypes.Structure):
@@ -171,6 +171,10 @@ def lib() -> ctypes.CDLL:
     L.vgg_estimate_fundamental.argtypes = [ci, ci, vp, vp, ci, vp, vp, ci, ci, cd, ci, ci, vp, vp, vp, vp, vp, cs, vp]
     L.vgg_fundamental_inliers.argtypes = [ci, ci, vp, vp, ci, vp, cd, ci, vp, vp]
     L.vgg_relative_pose_from_fundamental.argtypes = [ci, ci, vp, vp, ci, vp, cd, cd, vp, vp, vp, vp]
+    cu64 = ctypes.c_ulonglong
+    L.vgg_msac_fundamental_workspace_bytes.argtypes = [ci, ci, ci, ci, ctypes.POINTER(cs)]
+    L.vgg_estimate_fundamental_msac.argtypes = [ci, ci, vp, vp, ci, vp, cd, ci, ci, cu64, vp, vp, vp, vp, vp, cs, vp]
+    L.vgg_dev_msac_trace.argtypes = [ci, ci, ci, ci, vp, ci, vp, vp, vp]
     _lib = L
     return L
 

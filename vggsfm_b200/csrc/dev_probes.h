@@ -36,6 +36,11 @@ int vgg_dev_last_band_hint(int* meta_host, int* rb_range, int* end_blk, int* kb_
 /* Block structure for the in-repo Cholesky (tests): end_blk_host[b] = one past the last band block (128 rows) of block
  * column b, arrow_blk = first block of the dense arrow; count = 0 clears it (dense). */
 int vgg_dev_set_chol_band(const int* end_blk_host, int count, int arrow_blk);
+/* Trace of the most recent vgg_estimate_fundamental_msac on `workspace` (same B, N and iteration limits; waits for the
+ * device): per pair the number of trials that ran local optimisation, the trial whose model won (-1: none) and the
+ * first min(cap, 64) of those trials in order (-1 padded), all host arrays. */
+int vgg_dev_msac_trace(int B, int N, int max_iterations, int min_iterations, const void* workspace, int cap,
+                       int32_t* lo_runs_host, int32_t* win_trial_host, int32_t* lo_trials_host);
 
 #ifdef __cplusplus
 }

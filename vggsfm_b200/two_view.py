@@ -9,7 +9,9 @@ The minimal samples are drawn on the host with the reference's own ``np.random.r
 the reference's 7-point sets.  There is no fallback path: CPU tensors raise.
 
 ``vggsfm.runners.runner.estimate_preliminary_cameras`` (with ``use_poselib: False``) can be rebound to
-``estimate_preliminary_cameras`` below.
+``estimate_preliminary_cameras`` below, and ``estimate_preliminary_cameras_poselib`` (the default configurations,
+``use_poselib: True``) to ``estimate_preliminary_cameras_poselib``: PoseLib's LO-MSAC restated as
+csrc/twoview_msac.cu (``vgg_estimate_fundamental_msac``), so the default configuration runs without PoseLib.
 """
 from __future__ import annotations
 
@@ -189,3 +191,53 @@ def estimate_preliminary_cameras(tracks, tracks_vis, width, height, tracks_score
         "fmat_residuals": fres.to(dt).reshape(B, S - 1, -1),
     }
     return pred_cameras, preliminary_dict
+
+
+def estimate_fundamental_msac(points1, points2, valid_mask=None, max_error=0.5, max_iterations=20000,
+                              min_iterations=1000, seed=0, workspace=None):
+    """poselib.estimate_fundamental (LO-MSAC, real focal check, no progressive sampling) for every pair at once.
+    points1/points2 [B,N,2] CUDA float32 or float64 pixels, valid_mask [B,N] bool or None.  Returns (fmat [B,3,3] f64,
+    inlier_num [B] int64, inlier_mask [B,N] bool, iterations [B] int64).  ``workspace`` (a uint8 CUDA tensor) is
+    used instead of a fresh one when it is large enough."""
+    _need_cuda(points1, "estimate_fundamental_msac")
+    L = _lib.lib()
+    B, N, _ = points1.shape
+    dev = points1.device
+    p1, f64 = _points(points1)
+    p2, _ = _points(points2.to(p1.dtype))
+    vm = valid_mask.to(torch.uint8).contiguous() if valid_mask is not None else None
+    fmat = torch.empty(B, 3, 3, dtype=torch.float64, device=dev)
+    num = torch.empty(B, dtype=torch.int32, device=dev)
+    mask = torch.empty(B, N, dtype=torch.uint8, device=dev)
+    iters = torch.empty(B, dtype=torch.int32, device=dev)
+    nb = ctypes.c_size_t()
+    _lib.check(L.vgg_msac_fundamental_workspace_bytes(B, N, int(max_iterations), int(min_iterations), ctypes.byref(nb)),
+               "vgg_msac_fundamental_workspace_bytes")
+    ws = workspace if workspace is not None and workspace.numel() >= nb.value else \
+        torch.empty(max(nb.value, 256), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(L.vgg_estimate_fundamental_msac(B, N, p1.data_ptr(), p2.data_ptr(), f64,
+                                                   vm.data_ptr() if vm is not None else None, float(max_error),
+                                                   int(max_iterations), int(min_iterations), int(seed),
+                                                   fmat.data_ptr(), num.data_ptr(), mask.data_ptr(), iters.data_ptr(),
+                                                   ws.data_ptr(), ws.numel(), stream), "vgg_estimate_fundamental_msac")
+    return fmat, num.long(), mask.bool(), iters.long()
+
+
+def estimate_preliminary_cameras_poselib(tracks, tracks_vis, width, height, tracks_score=None, max_error=0.5,
+                                         max_ransac_iters=20000, predict_essential=False, lo_num=None,
+                                         predict_homo=False, loopresidual=False):
+    """estimate_preliminary.py:37-95.  tracks [B,S,N,2] CUDA, tracks_vis [B,S,N].  Returns (None, {"fmat":
+    [1, B(S-1), 3, 3] f64, "fmat_inlier_mask": [1, B(S-1), N] bool}).  As in the reference, the left points of every
+    pair are tracks[0, 0] (batch 0's query frame, also for the pairs of later batches), only matches with
+    tracks_vis >= 0.05 take part, and tracks_score, predict_essential, lo_num, predict_homo and loopresidual are
+    accepted and ignored.  A pair with fewer than 7 valid matches gets F = 0 and an empty mask (the reference fails)."""
+    _need_cuda(tracks, "estimate_preliminary_cameras_poselib")
+    B, S, N, _ = tracks.shape
+    left = tracks[0, 0][None].expand(B * (S - 1), N, 2)
+    right = tracks[:, 1:].reshape(B * (S - 1), N, 2)
+    valid = (tracks_vis >= 0.05)[:, 1:].reshape(B * (S - 1), N)
+    fmat, _, mask, _ = estimate_fundamental_msac(left, right, valid, max_error=max_error,
+                                                 max_iterations=max_ransac_iters, min_iterations=1000, seed=0)
+    return None, {"fmat": fmat[None], "fmat_inlier_mask": mask[None]}
