@@ -25,6 +25,23 @@ State layout (shared with the CUDA path, see DESIGN.md):
   uv      [S,N,2] float32-representable pixel observations, mask [S,N] bool
 Camera tangent block (dc columns): [delta(3) half-angle left perturbation, t(3), f, k];
 reduced-system index of frame s, column i is s*dc+i; shared intrinsics follow at S*dc.
+
+LM control (lm_solve), as the CUDA loop (csrc/ba_solve.cu) must follow it:
+  * terminations NO_CONVERGENCE, CONVERGENCE_GRADIENT / _FUNCTION / _PARAMETER, MIN_TRUST_REGION_RADIUS and
+    FAILURE_INVALID_STEPS (max_num_consecutive_invalid_steps invalid steps in a row); the Python binding of the CUDA
+    solver reports the same names.
+  * a step is invalid when the linear solve fails or gives a non-finite step, or when the model change is not > 0;
+    the radius then halves and decrease_factor is kept.
+  * the gradient max-norm propagates NaN, so a NaN gradient never reads as converged.
+  * trace: one dict per iteration with "outcome" 1 accepted / 0 rejected or terminating / 2 invalid and the radius
+    the iteration ran with (an invalid step's halving shows in the next row); valid steps also carry cost_change and
+    x_norm (|x| of ParameterToleranceReached), accepted steps the new gmax.  summary["initial_gmax"] is iteration 0's.
+  * known differences from Ceres 2.x [3P-memory]: Ceres ends with FAILURE at iteration 0 when the initial residual
+    evaluation fails (a NaN or inf observation); here such a problem runs into invalid steps instead (same
+    termination, parameters unchanged).  Ceres gives a candidate that fails to evaluate the cost DBL_MAX, which
+    rejects the step; here a non-finite candidate cost also makes rho non-finite and rejects it, but the CUDA loop
+    counts it as an invalid step.  No input with a finite initial cost and float32 observations was found that makes
+    the candidate cost non-finite, so that branch has no test (tests/test_ba_lm_edges_gpu.py).
 """
 from __future__ import annotations
 
@@ -397,13 +414,14 @@ def lm_solve(poses, intr, points, uv, mask, model, mode, param_const=None, point
     def grad_max_norm(gc_glob, gp):
         a = np.max(np.abs(gc_glob[free_c])) if free_c.any() else 0.0
         b = np.max(np.abs(gp[~point_const])) if (~point_const).any() else 0.0
-        return float(armax(max(a, b)))
+        return float(armax(np.max([a, b])))          # NaN propagates (Python's max() drops a NaN second argument)
 
     radius = opt.initial_trust_region_radius
     decrease_factor = 2.0
     summary = {"iterations": 0, "successful": 0, "initial_cost": cost, "termination": "NO_CONVERGENCE",
                "initial_eval_s": _t_init}
     gmax = grad_max_norm(gc_glob, blk["g_p"])
+    summary["initial_gmax"] = gmax
     if gmax <= opt.gradient_tolerance:
         summary.update(termination="CONVERGENCE_GRADIENT", final_cost=cost)
         return poses, intr, points, summary
@@ -452,12 +470,12 @@ def lm_solve(poses, intr, points, uv, mask, model, mode, param_const=None, point
             ok = False
         if not ok:
             invalid_steps += 1
+            if trace is not None:
+                trace.append({"it": it, "invalid": True, "outcome": 2, "cost": cost, "radius": radius})
             if invalid_steps >= opt.max_num_consecutive_invalid_steps:
                 summary["termination"] = "FAILURE_INVALID_STEPS"
                 break
             radius *= 0.5
-            if trace is not None:
-                trace.append({"it": it, "invalid": True, "radius": radius})
             continue
         d_c = dcs * sc_c                                           # unscaled camera step
         # ---- back-substitution: dp = M M^T (-(g_p + W^T d_c))
@@ -473,12 +491,13 @@ def lm_solve(poses, intr, points, uv, mask, model, mode, param_const=None, point
         model_change = 0.5 * quad
         if not (model_change > 0):
             invalid_steps += 1
+            if trace is not None:
+                trace.append({"it": it, "invalid": True, "outcome": 2, "cost": cost, "radius": radius,
+                              "model_change": model_change})
             if invalid_steps >= opt.max_num_consecutive_invalid_steps:
                 summary["termination"] = "FAILURE_INVALID_STEPS"
                 break
             radius *= 0.5
-            if trace is not None:
-                trace.append({"it": it, "invalid": True, "radius": radius})
             continue
         invalid_steps = 0
         d_cam = d_c[:S * dc].reshape(S, dc)
@@ -489,11 +508,12 @@ def lm_solve(poses, intr, points, uv, mask, model, mode, param_const=None, point
         step_norm = float(np.sqrt(np.sum(d_c * d_c) + pt_terms[1]))
         cost_change = cost - c_cost
         rho = cost_change / model_change
+        x_norm = _x_norm(poses, intr, points, S, dc, ns, param_const, point_const)
+        rec = {"it": it, "cost": cost, "candidate_cost": c_cost, "model_change": model_change, "rho": rho,
+               "radius": radius, "step_norm": step_norm, "cost_change": cost_change, "x_norm": x_norm, "outcome": 0}
         if trace is not None:
-            trace.append({"it": it, "cost": cost, "candidate_cost": c_cost, "model_change": model_change,
-                          "rho": rho, "radius": radius, "step_norm": step_norm})
-        if step_norm <= opt.parameter_tolerance * (_x_norm(poses, intr, points, S, dc, ns, param_const, point_const)
-                                                   + opt.parameter_tolerance):
+            trace.append(rec)
+        if step_norm <= opt.parameter_tolerance * (x_norm + opt.parameter_tolerance):
             summary["termination"] = "CONVERGENCE_PARAMETER"
             break
         if abs(cost_change) <= opt.function_tolerance * cost:
@@ -501,6 +521,7 @@ def lm_solve(poses, intr, points, uv, mask, model, mode, param_const=None, point
             summary["termination"] = "CONVERGENCE_FUNCTION"
             break
         if rho > opt.min_relative_decrease:
+            rec["outcome"] = 1
             poses, intr, points, cost = c_poses, c_intr, c_points, c_cost
             blk, Hc, gc = c_blk, c_Hc, c_gc
             Hc_diag = ar(np.diag(Hc).copy())
@@ -509,6 +530,7 @@ def lm_solve(poses, intr, points, uv, mask, model, mode, param_const=None, point
             radius = min(opt.max_trust_region_radius, radius / max(1.0 / 3.0, 1.0 - (2.0 * rho - 1.0) ** 3))
             decrease_factor = 2.0
             gmax = grad_max_norm(gc_glob, blk["g_p"])
+            rec["gmax"] = gmax
             if gmax <= opt.gradient_tolerance:
                 summary["termination"] = "CONVERGENCE_GRADIENT"
                 break

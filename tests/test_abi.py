@@ -38,11 +38,11 @@ def test_host_only_entry_points():
 
 def test_ba_workspace_bytes_is_host_only():
     """vgg_ba_workspace_bytes is a pure size computation: it succeeds without a GPU for the C1, C2 and C3 shapes and
-    every camera model / intrinsics mode, and covers at least the Schur operand Zt [Kpad][Dpad] and the reduced system
+    every camera model / intrinsics mode, and for 1001 frames (D = 7007 with per-frame SIMPLE_PINHOLE), and covers at least the Schur operand Zt [Kpad][Dpad] and the reduced system
     [D+3][Dpad] (matrix rows, right-hand side, diagonal, gradient) in float64."""
     import ctypes
     L = _lib.lib()
-    for S, N in ((8, 256), (50, 2048), (400, 4096)):
+    for S, N in ((8, 256), (50, 2048), (400, 4096), (1001, 2048), (1001, 6000)):     # the last two: D > 7000
         for model in (0, 1):
             for mode in (0, 1, 2):
                 dc, ns = ctypes.c_int(), ctypes.c_int()

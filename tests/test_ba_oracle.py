@@ -92,3 +92,43 @@ def test_c_restatement_matches_numpy(cam, mode):
     for k in a:
         if k != "cost":
             assert np.abs(a[k] - b[k]).max() <= 1e-11 * max(1.0, np.abs(a[k]).max()), k
+
+
+def test_lm_trace_fields():
+    """lm_solve's trace: the outcome of every iteration, cost_change, x_norm and (after a success) gmax as the solver
+    decided with them; an invalid step records the radius it ran with; a NaN gradient is not convergence."""
+    c = ba_case(8, 60, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME, seed=4)
+    S, N = c["mask"].shape
+    pc = bo.default_param_const(S, c["model"], c["mode"])
+    ptc = np.zeros(N, dtype=bool)
+    trace = []
+    o = bo.LMOptions()
+    o.max_num_iterations = 6
+    p, i, x, summ = bo.lm_solve(c["poses"], c["intr"], c["points"], c["uv"], c["mask"], c["model"], c["mode"],
+                                options=o, trace=trace)
+    assert len(trace) == summ["iterations"] and sum(r["outcome"] == 1 for r in trace) == summ["successful"]
+    dc, ns = bo.dims(c["model"], c["mode"])
+    for r in trace:
+        assert r["cost_change"] == r["cost"] - r["candidate_cost"] and r["outcome"] == int(r["rho"] > 1e-3)
+        assert ("gmax" in r) == (r["outcome"] == 1)
+    assert trace[0]["x_norm"] == bo._x_norm(c["poses"], c["intr"], c["points"], S, dc, ns, pc, ptc)
+    assert trace[-1]["outcome"] == 1                 # the returned state is the last row's candidate
+    blk = bo.build_blocks(p, i, x, c["uv"], c["mask"], c["model"], c["mode"])
+    _, gc = bo._assemble_camera_system(blk, S, dc, ns)
+    g = max(np.abs(gc[~pc]).max(), np.abs(blk["g_p"]).max())
+    assert abs(trace[-1]["gmax"] - g) <= 1e-12 * g
+    # NaN observation: invalid steps, each recording the radius it ran with; no convergence on a NaN gradient
+    uv = c["uv"].copy()
+    uv[2, 7] = np.nan
+    mask = c["mask"].copy()
+    mask[2, 7] = True
+    trace = []
+    o = bo.LMOptions()
+    o.gradient_tolerance = 1e30
+    o.max_num_consecutive_invalid_steps = 4
+    p2, _, _, summ = bo.lm_solve(c["poses"], c["intr"], c["points"], uv, mask, c["model"], c["mode"], options=o,
+                                 trace=trace)
+    assert np.isnan(summ["initial_gmax"]) and summ["termination"] == "FAILURE_INVALID_STEPS"
+    assert [r["outcome"] for r in trace] == [2, 2, 2, 2]
+    assert [r["radius"] for r in trace] == [1e4, 5e3, 2.5e3, 1.25e3]
+    assert np.array_equal(p2, c["poses"])

@@ -24,83 +24,11 @@ import pytest
 
 from oracle import ba_oracle as bo
 from oracle import band_oracle
-from tests.helpers import ba_case, banded_ba_case, to_dev
+from tests.helpers import ba_case, backward_error, banded_ba_case, recovered_step, reference_system, to_dev
 
 pytestmark = pytest.mark.gpu
 
-EPS = 2.0 ** -52
 RADIUS = 1e4                # initial_trust_region_radius of the default options
-MIN_DIAG, MAX_DIAG = 1e-6, 1e32
-
-
-def _so3_log(R):
-    """rotation vectors of [..., 3, 3] rotations, accurate for small angles"""
-    w = 0.5 * np.stack([R[..., 2, 1] - R[..., 1, 2], R[..., 0, 2] - R[..., 2, 0], R[..., 1, 0] - R[..., 0, 1]], -1)
-    s = np.linalg.norm(w, axis=-1)
-    th = np.arctan2(s, 0.5 * (np.trace(R, axis1=-2, axis2=-1) - 1.0))
-    return w * np.where(s > 0, th / np.where(s > 0, s, 1.0), 1.0)[..., None]
-
-
-def _recovered_step(old, new, S, dc, ns, model, mode):
-    """(camera step [D], its uncertainty [D], point step [N,3], its uncertainty [N,3]) from the parameters before and after
-    the iteration: R_new = Exp(2 delta) R_old, everything else additive."""
-    (p0, i0, x0), (p1, i1, x1) = old, new
-    D = S * dc + ns
-    d, u = np.zeros(D), np.zeros(D)
-    dcam, ucam = d[:S * dc].reshape(S, dc), u[:S * dc].reshape(S, dc)
-    R0, R1 = p0[:, :, :3], p1[:, :, :3]
-    dcam[:, 0:3] = 0.5 * _so3_log(R1 @ R0.transpose(0, 2, 1))
-    ucam[:, 0:3] = EPS * np.maximum(np.abs(R0).max(axis=(1, 2)), np.abs(R1).max(axis=(1, 2)))[:, None]
-    dcam[:, 3:6] = p1[:, :, 3] - p0[:, :, 3]
-    ucam[:, 3:6] = EPS * np.maximum(np.abs(p0[:, :, 3]), np.abs(p1[:, :, 3]))
-    for j, col in enumerate([0, 3][:bo.n_intr(model)]):
-        if mode == bo.INTR_PER_FRAME:
-            dcam[:, 6 + j] = i1[:, col] - i0[:, col]
-            ucam[:, 6 + j] = EPS * np.maximum(np.abs(i0[:, col]), np.abs(i1[:, col]))
-        elif mode == bo.INTR_SHARED:
-            d[S * dc + j] = i1[0, col] - i0[0, col]
-            u[S * dc + j] = EPS * max(abs(i0[0, col]), abs(i1[0, col]))
-    return d, u, x1 - x0, EPS * np.maximum(np.abs(x0), np.abs(x1))
-
-
-def _reference_system(c, param_const, point_const):
-    """The damped system of the first iteration in scaled variables (oracle/ba_oracle.py lm_solve): camera block A [D,D],
-    coupling B [D,N,3], point blocks V [N,3,3], gradients; rows and columns of constant parameters / points zeroed."""
-    S, N = c["mask"].shape
-    model, mode = c["model"], c["mode"]
-    dc, ns = bo.dims(model, mode)
-    blocks = bo.build_blocks_c if bo._load_c() is not None else bo.build_blocks
-    blk = blocks(c["poses"], c["intr"], c["points"], c["uv"], c["mask"], model, mode, point_const)
-    Hc, gc = bo._assemble_camera_system(blk, S, dc, ns)
-    W = bo._full_W(blk, S, dc, ns)
-    fc, fp = ~param_const, ~point_const
-    sc_c = 1.0 / (1.0 + np.sqrt(np.diag(Hc)))
-    sc_p = 1.0 / (1.0 + np.sqrt(np.einsum("nii->ni", blk["H_pp"])))
-    dcc = np.clip(np.diag(Hc) * sc_c * sc_c, MIN_DIAG, MAX_DIAG)
-    Hps = blk["H_pp"] * sc_p[:, :, None] * sc_p[:, None, :]
-    dpp = np.clip(np.einsum("nii->ni", Hps), MIN_DIAG, MAX_DIAG)
-    A = (Hc * np.outer(sc_c, sc_c) + np.diag(dcc / RADIUS)) * np.outer(fc, fc)
-    B = W * (sc_c * fc)[:, None, None] * (sc_p * fp[:, None])[None]
-    V = Hps + dpp[:, :, None] * np.eye(3) / RADIUS
-    return dict(cost=blk["cost"], gc=gc, gp=blk["g_p"], sc_c=sc_c, sc_p=sc_p, dcc=dcc, dpp=dpp, fc=fc, fp=fp, A=A,
-                B=B.reshape(A.shape[0], 3 * N), V=V, gcs=gc * sc_c * fc, gps=blk["g_p"] * sc_p * fp[:, None])
-
-
-def _backward_error(ref, dcs, ucs, dps, ups):
-    """normwise backward error of the scaled step (dcs [D], dps [N,3]) in the full damped system, evaluated blockwise"""
-    A, B, V, fc, fp = ref["A"], ref["B"], ref["V"], ref["fc"], ref["fp"]
-    N = V.shape[0]
-    rc = A @ dcs + B @ dps.reshape(-1) + ref["gcs"]
-    rp = (B.T @ dcs).reshape(N, 3) + np.einsum("nij,nj->ni", V, dps) + ref["gps"]
-    absB = np.abs(B)
-    row_c = np.abs(A).sum(1) + absB.sum(1)
-    row_p = absB.sum(0).reshape(N, 3) + np.abs(V).sum(2)
-    res = max(np.abs(rc[fc]).max(initial=0.0), np.abs(rp[fp]).max(initial=0.0))
-    normH = max(row_c[fc].max(initial=0.0), row_p[fp].max(initial=0.0))
-    nd = max(np.abs(dcs[fc]).max(initial=0.0), np.abs(dps[fp]).max(initial=0.0))
-    nu = max(np.abs(ucs[fc]).max(initial=0.0), np.abs(ups[fp]).max(initial=0.0))
-    ng = max(np.abs(ref["gcs"]).max(initial=0.0), np.abs(ref["gps"]).max(initial=0.0))
-    return res / (normH * (nd + nu) + ng)
 
 
 def _oracle_step(ref):
@@ -177,13 +105,13 @@ def _one_step(c, dev, param_const=None, point_const=None, label=""):
     assert s.iterations == 1 and tr[0, 7] == 1, (label, tr)            # the step was accepted
     assert tr[0, 5] == RADIUS
 
-    ref = _reference_system(c, param_const, point_const)
+    ref = reference_system(c, param_const, point_const, RADIUS)
     assert abs(s.initial_cost - ref["cost"]) <= 1e-12 * ref["cost"], (label, s.initial_cost, ref["cost"])
-    d_c, u_c, d_p, u_p = _recovered_step((c["poses"], c["intr"], c["points"]), new, S, dc, ns, model, mode)
+    d_c, u_c, d_p, u_p = recovered_step((c["poses"], c["intr"], c["points"]), new, S, dc, ns, model, mode)
     assert not d_c[param_const].any() and not d_p[point_const].any()
     dcs, ucs = d_c / ref["sc_c"], u_c / ref["sc_c"]
     dps, ups = d_p / ref["sc_p"], u_p / ref["sc_p"]
-    eta = _backward_error(ref, dcs, ucs, dps, ups)
+    eta = backward_error(ref, dcs, ucs, dps, ups)
     # model change (oracle/ba_oracle.py lm_solve) and step norm at the recovered step
     quad = (np.sum(dcs * dcs * ref["dcc"] / RADIUS * ref["fc"]) - np.sum(d_c * ref["gc"]) +
             np.sum(dps * dps * ref["dpp"] / RADIUS * ref["fp"][:, None]) - np.sum(d_p * ref["gp"]))

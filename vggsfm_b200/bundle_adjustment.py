@@ -26,7 +26,7 @@ INTR_PER_FRAME = 1
 INTR_SHARED = 2
 
 TERMINATION = {0: "NO_CONVERGENCE", 1: "CONVERGENCE_GRADIENT", 2: "CONVERGENCE_FUNCTION",
-               3: "CONVERGENCE_PARAMETER", 4: "MIN_TRUST_REGION_RADIUS", 5: "FAILURE"}
+               3: "CONVERGENCE_PARAMETER", 4: "MIN_TRUST_REGION_RADIUS", 5: "FAILURE_INVALID_STEPS"}
 
 
 def camera_model_id(camera_type: str) -> int:

@@ -499,19 +499,24 @@ __global__ void extract_gvec_kernel(int S, int dc, int ns, int KR, const double*
   gvec[i] = (i < S * dc) ? camrec[(size_t)(i / dc) * KR + (i % dc)] : shared_in[i - S * dc];
 }
 
-// scal[4] = max |gvec| over free parameters, scal[5] = max |g_p| over variable points
+// scal[4] = max |gvec| over free parameters, scal[5] = max |g_p| over variable points.  The maximum is taken over the
+// bit patterns: non-negative doubles order like them, and fabs(NaN) is a positive NaN, which orders above +inf -- so a
+// NaN gradient entry gives a NaN max-norm (that never passes gradient_tolerance) where fmax would drop it.
 __global__ void gradmax_kernel(int D, int N, const double* __restrict__ gvec, const uint8_t* __restrict__ pconst,
                                const double* __restrict__ g_p, const uint8_t* __restrict__ point_const,
                                double* __restrict__ scal) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  double mc = 0, mp = 0;
-  if (i < D && !pconst[i]) mc = fabs(gvec[i]);
-  if (i < N * 3 && !(point_const && point_const[i / 3])) mp = fabs(g_p[i]);
-  mc = warp_max(mc); mp = warp_max(mp);
+  unsigned long long mc = 0, mp = 0;
+  if (i < D && !pconst[i]) mc = (unsigned long long)__double_as_longlong(fabs(gvec[i]));
+  if (i < N * 3 && !(point_const && point_const[i / 3])) mp = (unsigned long long)__double_as_longlong(fabs(g_p[i]));
+#pragma unroll
+  for (int off = 16; off >= 1; off >>= 1) {
+    mc = max(mc, __shfl_xor_sync(0xffffffffu, mc, off));
+    mp = max(mp, __shfl_xor_sync(0xffffffffu, mp, off));
+  }
   if ((threadIdx.x & 31) == 0) {
-    // non-negative doubles order like their bit patterns
-    atomicMax(reinterpret_cast<unsigned long long*>(&scal[4]), (unsigned long long)__double_as_longlong(mc));
-    atomicMax(reinterpret_cast<unsigned long long*>(&scal[5]), (unsigned long long)__double_as_longlong(mp));
+    atomicMax(reinterpret_cast<unsigned long long*>(&scal[4]), mc);
+    atomicMax(reinterpret_cast<unsigned long long*>(&scal[5]), mp);
   }
 }
 

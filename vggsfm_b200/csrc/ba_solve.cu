@@ -127,6 +127,10 @@ struct EventPair {
   }
 };
 
+// max of the camera and point gradient max-norms; a NaN in either (gradmax_kernel keeps them) stays NaN, so that a NaN
+// gradient is never taken for convergence
+static double grad_max_norm(double gc, double gp) { return isnan(gc) || isnan(gp) ? NAN : fmax(gc, gp); }
+
 static double* pinned_scalars() {
   static thread_local double* h = nullptr;
   if (!h) {
@@ -724,7 +728,7 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
       return VGG_ECUDA;
     }
     *cost_out = h_scal[8];
-    *gmax_out = fmax(h_scal[4], h_scal[5]);
+    *gmax_out = grad_max_norm(h_scal[4], h_scal[5]);
     return VGG_OK;
   };
 
@@ -905,7 +909,7 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
       if (tr) tr[7] = 1;
       radius = fmin(opt.max_trust_region_radius, radius / fmax(1.0 / 3.0, 1.0 - pow(2.0 * rho - 1.0, 3.0)));
       decrease_factor = 2.0;
-      gmax = fmax(h_scal[4], h_scal[5]);
+      gmax = grad_max_norm(h_scal[4], h_scal[5]);
       if (gmax <= opt.gradient_tolerance) {
         summary->termination = VGG_BA_CONVERGENCE_GRADIENT;
         break;
