@@ -323,12 +323,9 @@ def test_cholesky_band_plus_arrow_matches_lapack(cuda_dev, nblk, bw, tail):
     ws = torch.empty(nb_all * 131072 + 1024, dtype=torch.uint8, device=cuda_dev)
     info = ctypes.c_int(-1)
     L = _lib.lib()
-    _lib.check(L.vgg_dev_set_chol_band(end.ctypes.data, end.size, arrow), "band")
-    try:
-        _lib.check(L.vgg_cholesky_lower(n, lda, buf.data_ptr(), ws.data_ptr(), ws.numel(), ctypes.byref(info),
-                                        torch.cuda.current_stream().cuda_stream), "vgg_cholesky_lower")
-    finally:
-        L.vgg_dev_set_chol_band(None, 0, 0)
+    _lib.check(L.vgg_dev_cholesky_band(n, lda, buf.data_ptr(), ws.data_ptr(), ws.numel(), ctypes.byref(info),
+                                       torch.cuda.current_stream().cuda_stream, end.ctypes.data, end.size, arrow),
+               "vgg_dev_cholesky_band")
     assert info.value == 0
     ref = np.linalg.cholesky(A)
     got = np.tril(buf.cpu().numpy()[:, :n])

@@ -19,14 +19,11 @@ def _factor(cuda_dev, A, band=None):
     ws = torch.empty(((n + 127) // 128) * 131072 + 1024, dtype=torch.uint8, device=cuda_dev)
     info = ctypes.c_int(-1)
     L = _lib.lib()
-    if band is not None:
-        _lib.check(L.vgg_dev_set_chol_band(band[0].ctypes.data, band[0].size, band[1]), "band")
-    try:
-        _lib.check(L.vgg_cholesky_lower(n, lda, buf.data_ptr(), ws.data_ptr(), ws.numel(), ctypes.byref(info),
-                                        torch.cuda.current_stream().cuda_stream), "vgg_cholesky_lower")
-    finally:
-        if band is not None:
-            L.vgg_dev_set_chol_band(None, 0, 0)
+    args = (n, lda, buf.data_ptr(), ws.data_ptr(), ws.numel(), ctypes.byref(info), torch.cuda.current_stream().cuda_stream)
+    if band is None:
+        _lib.check(L.vgg_cholesky_lower(*args), "vgg_cholesky_lower")
+    else:
+        _lib.check(L.vgg_dev_cholesky_band(*args, band[0].ctypes.data, band[0].size, band[1]), "vgg_dev_cholesky_band")
     return info.value, buf.cpu().numpy()[:, :n]
 
 

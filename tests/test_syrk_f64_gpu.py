@@ -21,16 +21,13 @@ def _syrk(Z, C0, dev, ranges=None):
     Zt = torch.from_numpy(np.ascontiguousarray(Z)).to(dev)
     C = torch.from_numpy(np.ascontiguousarray(C0)).to(dev)
     with torch.cuda.device(dev):
-        if ranges is not None:
+        args = (Kpad, Dpad, Zt.data_ptr(), C.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        if ranges is None:
+            _lib.check(L.vgg_dev_syrk_f64(*args), "vgg_dev_syrk_f64")
+        else:
             r = np.ascontiguousarray(ranges, dtype=np.int32)
-            _lib.check(L.vgg_dev_set_syrk_ranges(r.ctypes.data, r.size), "vgg_dev_set_syrk_ranges")
-        try:
-            _lib.check(L.vgg_dev_syrk_f64(Kpad, Dpad, Zt.data_ptr(), C.data_ptr(), torch.cuda.current_stream().cuda_stream),
-                       "vgg_dev_syrk_f64")
-            torch.cuda.synchronize()
-        finally:
-            if ranges is not None:
-                _lib.check(L.vgg_dev_set_syrk_ranges(None, 0), "vgg_dev_set_syrk_ranges")
+            _lib.check(L.vgg_dev_syrk_f64_band(*args, r.ctypes.data, r.size), "vgg_dev_syrk_f64_band")
+        torch.cuda.synchronize()
     return C.cpu().numpy()
 
 

@@ -20,7 +20,8 @@ from oracle import ozaki_oracle as oz
 pytestmark = pytest.mark.gpu
 
 
-def _run(Z, s, dev):
+def _run(Z, s, dev, rg=None):
+    """rg: band hint (k-block range per 128-column row block of Z), None = dense"""
     import torch
     from vggsfm_b200 import _lib
     L = _lib.lib()
@@ -31,8 +32,11 @@ def _run(Z, s, dev):
     _lib.check(L.vgg_syrk_ozaki_workspace_bytes(Kpad, Dpad, s, ctypes.byref(nb)), "vgg_syrk_ozaki_workspace_bytes")
     ws = torch.empty(nb.value, dtype=torch.uint8, device=dev)
     with torch.cuda.device(dev):
-        _lib.check(L.vgg_syrk_ozaki(Kpad, Dpad, Zt.data_ptr(), C.data_ptr(), s, ws.data_ptr(), ws.numel(),
-                                    torch.cuda.current_stream().cuda_stream), "vgg_syrk_ozaki")
+        args = (Kpad, Dpad, Zt.data_ptr(), C.data_ptr(), s, ws.data_ptr(), ws.numel(), torch.cuda.current_stream().cuda_stream)
+        if rg is None:
+            _lib.check(L.vgg_syrk_ozaki(*args), "vgg_syrk_ozaki")
+        else:
+            _lib.check(L.vgg_dev_syrk_ozaki_band(*args, rg.ctypes.data, rg.size), "vgg_dev_syrk_ozaki_band")
         torch.cuda.synchronize()
     full = C.cpu().numpy()
     del Zt, C, ws
@@ -163,25 +167,15 @@ def _banded(Dpad, KB, seed):
     return Z, rg
 
 
-def _run_banded(Z, rg, s, dev):
-    from vggsfm_b200 import _lib
-    L = _lib.lib()
-    _lib.check(L.vgg_dev_set_syrk_ranges(rg.ctypes.data, rg.size), "ranges")
-    try:
-        return _run(Z, s, dev)
-    finally:
-        L.vgg_dev_set_syrk_ranges(None, 0)
-
-
 def test_band_hint_skips_only_zero_blocks(cuda_dev):
-    """With the band hint installed (k-block range per 128-column row block outside which Zt is zero) the kernel skips
-    tiles whose ranges do not meet and shortens the rest: the result must equal the dense product of the same Z."""
+    """With the band hint (k-block range per 128-column row block outside which Zt is zero) the kernel skips tiles
+    whose ranges do not meet and shortens the rest: the result must equal the dense product of the same Z."""
     Z, rg = _banded(1024, 24, 11)
     dense = _run(Z, 7, cuda_dev)
-    got = _run_banded(Z, rg, 7, cuda_dev)
+    got = _run(Z, 7, cuda_dev, rg)
     _check(Z, dense, 7, cuda_dev, "band: dense")
     _check(Z, got, 7, cuda_dev, "band: hint")
-    again = _run(Z, 7, cuda_dev)                       # and the plan goes back to dense when the hint is gone
+    again = _run(Z, 7, cuda_dev)                       # and the cached plan goes back to dense without the hint
     _check(Z, again, 7, cuda_dev, "band: dense again")
 
 
@@ -192,7 +186,7 @@ def test_plan_cache_alternating_shapes(cuda_dev):
     cases = {"a": (_case(256, 640, 21), 7), "b": (_case(384, 1040, 22), 5), "c": (_case(256, 700, 23), 4)}
     for key in ["a", "b", "band", "a", "band-dense", "c", "band", "b", "c"]:
         if key.startswith("band"):
-            got = _run(Zb, 7, cuda_dev) if key == "band-dense" else _run_banded(Zb, rg, 7, cuda_dev)
+            got = _run(Zb, 7, cuda_dev, None if key == "band-dense" else rg)
             _check(Zb, got, 7, cuda_dev, f"plan cache {key}")
         else:
             Z, s = cases[key]

@@ -28,7 +28,7 @@ EXPORTS = [
 
 
 # development probes (csrc/dev_probes.h): exported, not part of the public header
-DEV_EXPORTS = ["vgg_dev_blocks_timing", "vgg_dev_blocks_last_ms", "vgg_dev_chol128_probe", "vgg_dev_set_syrk_ranges", "vgg_dev_syrk_f64", "vgg_dev_trsv_probe", "vgg_dev_set_chol_band",
+DEV_EXPORTS = ["vgg_dev_blocks_timing", "vgg_dev_blocks_last_ms", "vgg_dev_chol128_probe", "vgg_dev_syrk_f64", "vgg_dev_syrk_f64_band", "vgg_dev_syrk_ozaki_band", "vgg_dev_trsv_probe", "vgg_dev_cholesky_band",
                "vgg_dev_last_band_hint", "vgg_dev_msac_trace"]
 
 
@@ -145,13 +145,14 @@ def lib() -> ctypes.CDLL:
     L.vgg_dev_blocks_timing.argtypes = [ci]
     L.vgg_dev_blocks_last_ms.argtypes = [ctypes.POINTER(cd)]
     L.vgg_dev_chol128_probe.argtypes = [ci, vp, vp, vp]
-    L.vgg_dev_set_syrk_ranges.argtypes = [vp, ci]
     L.vgg_dev_syrk_f64.argtypes = [ci, ci, vp, vp, vp]
+    L.vgg_dev_syrk_f64_band.argtypes = L.vgg_dev_syrk_f64.argtypes + [vp, ci]
     L.vgg_dev_trsv_probe.argtypes = [ci, ci, vp, vp, cs, vp, vp]
-    L.vgg_dev_set_chol_band.argtypes = [vp, ci, ci]
     L.vgg_dev_last_band_hint.argtypes = [vp, vp, vp, vp, vp]
     L.vgg_syrk_ozaki.argtypes = [ci, ci, vp, vp, ci, vp, cs, vp]
+    L.vgg_dev_syrk_ozaki_band.argtypes = L.vgg_syrk_ozaki.argtypes + [vp, ci]
     L.vgg_cholesky_lower.argtypes = [ci, ci, vp, vp, cs, ctypes.POINTER(ci), vp]
+    L.vgg_dev_cholesky_band.argtypes = L.vgg_cholesky_lower.argtypes + [vp, ci, ci]
     L.vgg_tri_workspace_bytes.argtypes = [ci, ci, ci, ci, ctypes.POINTER(cs)]
     L.vgg_triangulate_tracks.argtypes = [ci, ci, vp, vp, vp, vp, vp, ci, ci, cd, cd, vp, vp, vp, vp, cs, vp]
     L.vgg_triangulate_by_pair.argtypes = [ci, ci, vp, vp, vp, vp, vp, vp, cs, vp]

@@ -32,7 +32,6 @@ namespace vgg {
 
 // kernel-only timing for bench.py's roofline (csrc/dev_probes.h): an event pair on the launching stream, directly
 // around the ba_blocks_kernel launch (the accumulator memsets stay outside)
-extern BandDev g_band_dev;         // csrc/ba_schur.cu
 static bool g_blocks_timing = false;
 static cudaEvent_t g_blocks_ev[2] = {nullptr, nullptr};
 
@@ -383,7 +382,8 @@ __global__ void __launch_bounds__(BT, USE_TMA ? 2 : 3) ba_blocks_kernel(
 
 template <int MODEL, int MODE>
 static int launch_blocks(const vgg_ba_problem* p, double* cost, double* camrec, double* g_p, double* H_pp,
-                         double* W, double* shared_out, int tracks_per_warp, cudaStream_t stream, bool outputs_zeroed) {
+                         double* W, double* shared_out, int tracks_per_warp, const int* fg_tracks, cudaStream_t stream,
+                         bool outputs_zeroed) {
   using C = BlkCfg<MODEL, MODE>;
   const int S = p->S, N = p->N;
   const int D = S * C::DC + C::NS;
@@ -393,7 +393,7 @@ static int launch_blocks(const vgg_ba_problem* p, double* cost, double* camrec, 
   const bool tma_ok = ((reinterpret_cast<uintptr_t>(W) & 15) == 0);
   const int ngroups = (S + 31) / 32;
   const auto kern = tma_ok ? ba_blocks_kernel<MODEL, MODE, true> : ba_blocks_kernel<MODEL, MODE, false>;
-  if (tracks_per_warp <= 0 && g_band_dev.fg_tracks) {
+  if (tracks_per_warp <= 0 && fg_tracks) {
     // banded (sequential) problems: most (frame group, track chunk) warps return at once, so the chunks must be small
     // enough for the few that do not to spread over the machine (r02 launch list at 1000 frames x 32 k points: with the
     // dense sizing ~220 warps of 500 tracks each did all the work, 0.43 ms; the visible part is 0.5 GB)
@@ -457,22 +457,23 @@ static int launch_blocks(const vgg_ba_problem* p, double* cost, double* camrec, 
   if (g_blocks_timing) VGG_CUDA_CHECK(cudaEventRecord(g_blocks_ev[0], stream));
   VGG_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<grid, BT, smem, stream>>>(S, N, tracks_per_warp, p->uv, p->mask, p->poses, p->intr, p->points, p->point_const,
-                                   cost, camrec, g_p, H_pp, W, shared_out, g_band_dev.fg_tracks);
+                                   cost, camrec, g_p, H_pp, W, shared_out, fg_tracks);
   VGG_LAUNCH_CHECK();
   if (g_blocks_timing) VGG_CUDA_CHECK(cudaEventRecord(g_blocks_ev[1], stream));
   return VGG_OK;
 }
 
 int ba_build_blocks(const vgg_ba_problem* p, double* cost, double* camrec, double* g_p, double* H_pp, double* W,
-                    double* shared_out, int tracks_per_warp, cudaStream_t stream, bool outputs_zeroed) {
+                    double* shared_out, int tracks_per_warp, const int* fg_tracks, cudaStream_t stream,
+                    bool outputs_zeroed) {
   const int key = p->camera_model * 3 + p->intr_mode;
   switch (key) {
-    case 0: return launch_blocks<0, 0>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, stream, outputs_zeroed);
-    case 1: return launch_blocks<0, 1>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, stream, outputs_zeroed);
-    case 2: return launch_blocks<0, 2>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, stream, outputs_zeroed);
-    case 3: return launch_blocks<1, 0>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, stream, outputs_zeroed);
-    case 4: return launch_blocks<1, 1>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, stream, outputs_zeroed);
-    case 5: return launch_blocks<1, 2>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, stream, outputs_zeroed);
+    case 0: return launch_blocks<0, 0>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks, stream, outputs_zeroed);
+    case 1: return launch_blocks<0, 1>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks, stream, outputs_zeroed);
+    case 2: return launch_blocks<0, 2>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks, stream, outputs_zeroed);
+    case 3: return launch_blocks<1, 0>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks, stream, outputs_zeroed);
+    case 4: return launch_blocks<1, 1>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks, stream, outputs_zeroed);
+    case 5: return launch_blocks<1, 2>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks, stream, outputs_zeroed);
   }
   set_error("bad camera_model/intr_mode %d/%d", p->camera_model, p->intr_mode);
   return VGG_EINVAL;

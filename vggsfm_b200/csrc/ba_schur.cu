@@ -21,9 +21,6 @@
 
 namespace vgg {
 
-// band structure of the running solve (csrc/ba_solve.cu, compute_band_hint); null pointers: dense
-BandDev g_band_dev = {nullptr, nullptr, nullptr, 0};
-
 // Add v to one element of the reduced-system buffer.  Single GPU: plain f64 RED on the local copy.  Track-sharded
 // multi-GPU ("fabric" mode): ONE multimem reduction on the NVSwitch multicast address, which lands the addend in every
 // rank's copy of the buffer -- the all-reduce of the reduced camera system happens inside the kernels that
@@ -549,19 +546,13 @@ int launch_assemble_hc(int S, int dc, int ns, int KR, int Dpad, const double* ca
   return VGG_OK;
 }
 int launch_z_transpose(int D, int N, int Dpad, const double* W, const double* M, const double* q, double* Zt,
-                       double* rhs, ptrdiff_t mc_off, cudaStream_t st) {
+                       double* rhs, ptrdiff_t mc_off, const int* rb_range, cudaStream_t st) {
   const size_t pitch = (size_t)(D + (D & 1));
   dim3 grid((D + 127) / 128, (N + ZB_NT - 1) / ZB_NT);
-  z_build_kernel<<<grid, 128, 0, st>>>(D, N, Dpad, pitch, W, M, q, Zt, rhs, mc_off, g_band_dev.rb_range);
+  z_build_kernel<<<grid, 128, 0, st>>>(D, N, Dpad, pitch, W, M, q, Zt, rhs, mc_off, rb_range);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
-// reduce-scatter destinations of the running multi-GPU solve (set per iteration by csrc/ba_solve.cu; world <= 1: off)
-FabricDev g_fabric_dev = {0, 0, {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}};
-
-// Band hint of the current solve (csrc/syrk_i8.cu; set by csrc/ba_solve.cu or vgg_dev_set_syrk_ranges): [lo, hi) k-block
-// range per 128-column row block of Zt outside which the block is exactly zero; empty = dense.
-extern std::vector<int> g_syrk_kb_ranges;
 
 // work list of the last shape / band hint, kept on the device until either changes
 struct SyrkF64State {
@@ -573,12 +564,14 @@ struct SyrkF64State {
 thread_local SyrkF64State g_sf;
 
 // Cmat -= Zt^T Zt: Zt [Kpad][Dpad] (Dpad % 128 == 0, Kpad % 16 == 0), Cmat [Dpad][Dpad] row-major, LOWER triangle (or
-// the fabric destinations of g_fabric_dev / mc_off, see syrk_red_upper)
-int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc_off, cudaStream_t st) {
+// the fabric destinations of fd / mc_off, see syrk_red_upper).  kb_ranges: [lo, hi) k-block range per 128-column row
+// block of Zt outside which the block is exactly zero (csrc/ba_solve.cu, compute_band_hint); any other size = dense.
+int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc_off, const std::vector<int>& kb_ranges,
+                const FabricDev& fd, cudaStream_t st) {
   VGG_REQUIRE(Dpad % SF_BM == 0 && Kpad % SF_BK == 0, "syrk: Dpad must be a multiple of 128 and Kpad of 16");
   const int nb = Dpad / SF_BM, KB = (Kpad + 63) / 64;
   SyrkF64State& hs = g_sf;
-  const std::vector<int> ranges = (int)g_syrk_kb_ranges.size() == 2 * nb ? g_syrk_kb_ranges : std::vector<int>();
+  const std::vector<int> ranges = (int)kb_ranges.size() == 2 * nb ? kb_ranges : std::vector<int>();
   int dev = 0;
   VGG_CUDA_CHECK(cudaGetDevice(&dev));
   if (hs.dev != dev || hs.Kpad != Kpad || hs.Dpad != Dpad || hs.ranges != ranges) {
@@ -607,7 +600,7 @@ int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc
   }
   if (hs.nwork == 0) return VGG_OK;
   syrk_f64_kernel<<<std::min(hs.sms, hs.nwork), SF_THREADS, SF_SMEM_BYTES, st>>>(hs.work_dev, hs.nwork, Kpad, Dpad, Zt, Cmat,
-                                                                               mc_off, g_fabric_dev);
+                                                                               mc_off, fd);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
@@ -626,9 +619,10 @@ int launch_cam_step(int D, const double* dcs, size_t dcs_stride, const double* s
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
-int launch_backsub(int D, int N, const double* W, const double* d_c, double* wacc, cudaStream_t st) {
+int launch_backsub(int D, int N, const double* W, const double* d_c, double* wacc, const int* kb_rows, int arrow_row,
+                   cudaStream_t st) {
   const size_t pitch = (size_t)(D + (D & 1));
-  backsub_kernel<<<(N + 7) / 8, 256, 0, st>>>(D, N, pitch, W, d_c, wacc, g_band_dev.kb_rows, g_band_dev.arrow_row);
+  backsub_kernel<<<(N + 7) / 8, 256, 0, st>>>(D, N, pitch, W, d_c, wacc, kb_rows, arrow_row);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
@@ -663,12 +657,17 @@ int launch_gradmax(int D, int N, const double* gvec, const uint8_t* pconst, cons
 
 extern "C" {
 
-/* development probe (csrc/dev_probes.h): the in-loop Schur SYRK on its own, with the band hint of vgg_dev_set_syrk_ranges */
+/* development probes (csrc/dev_probes.h): the in-loop Schur SYRK on its own, dense / with the given band hint */
 int vgg_dev_syrk_f64(int Kpad, int Dpad, const double* Zt, double* Cmat, void* stream) {
+  return vgg_dev_syrk_f64_band(Kpad, Dpad, Zt, Cmat, stream, nullptr, 0);
+}
+
+int vgg_dev_syrk_f64_band(int Kpad, int Dpad, const double* Zt, double* Cmat, void* stream, const int* ranges, int count) {
   using namespace vgg;
   g_launch_count = 0;
-  VGG_REQUIRE(Zt && Cmat && Kpad > 0 && Dpad > 0, "bad argument");
-  return launch_syrk(Kpad, Dpad, Zt, Cmat, 0, static_cast<cudaStream_t>(stream));
+  VGG_REQUIRE(Zt && Cmat && Kpad > 0 && Dpad > 0 && (ranges || count <= 0), "bad argument");
+  return launch_syrk(Kpad, Dpad, Zt, Cmat, 0, std::vector<int>(ranges, ranges + std::max(count, 0)), FabricDev{},
+                     static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

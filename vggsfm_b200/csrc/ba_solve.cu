@@ -25,7 +25,8 @@ void set_error(const char* fmt, ...) {
 
 // kernels (ba_blocks.cu / ba_schur.cu)
 int ba_build_blocks(const vgg_ba_problem* p, double* cost, double* camrec, double* g_p, double* H_pp, double* W,
-                    double* shared_out, int tracks_per_warp, cudaStream_t stream, bool outputs_zeroed = false);
+                    double* shared_out, int tracks_per_warp, const int* fg_tracks, cudaStream_t stream,
+                    bool outputs_zeroed = false);
 int launch_jacobi_scale_points(int N, const double* H_pp, double* sc_p, int enable, cudaStream_t st);
 int launch_jacobi_scale_cams(int D, const double* hdiag, double* sc_c, int enable, cudaStream_t st);
 int launch_point_prep(int N, const double* H_pp, const double* g_p, const double* sc_p, const uint8_t* point_const,
@@ -34,15 +35,17 @@ int launch_point_prep(int N, const double* H_pp, const double* g_p, const double
 int launch_assemble_hc(int S, int dc, int ns, int KR, int Dpad, const double* camrec, const double* shared_in,
                        double* Sraw, double* rhs, double* hdiag, double* gvec, ptrdiff_t mc_off, cudaStream_t st);
 int launch_z_transpose(int D, int N, int Dpad, const double* W, const double* M, const double* q, double* Zt,
-                       double* rhs, ptrdiff_t mc_off, cudaStream_t st);
-int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc_off, cudaStream_t st);
+                       double* rhs, ptrdiff_t mc_off, const int* rb_range, cudaStream_t st);
+int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc_off, const std::vector<int>& kb_ranges,
+                const FabricDev& fd, cudaStream_t st);
 int launch_scale_damp(int D, int Dpad, double* A, const double* rhs, const double* hdiag, const double* sc,
                       const uint8_t* pconst, double radius, double min_diag, double max_diag, double* bvec,
                       cudaStream_t st);
 int launch_cam_step(int D, const double* dcs, size_t dcs_stride, const double* sc, const double* hdiag, const double* gvec,
                     const uint8_t* pconst, double radius, double min_diag, double max_diag, double* d_c, double* scal,
                     cudaStream_t st);
-int launch_backsub(int D, int N, const double* W, const double* d_c, double* wacc, cudaStream_t st);
+int launch_backsub(int D, int N, const double* W, const double* d_c, double* wacc, const int* kb_rows, int arrow_row,
+                   cudaStream_t st);
 int launch_point_step(int N, const double* M, const double* g_p, const double* wacc, const double* sc_p,
                       const double* dpp, const double* X, double radius, double* Xc, double* scal, cudaStream_t st);
 int launch_cam_update(int S, int dc, int ns, int model, const double* d_c, const double* poses, const double* intr,
@@ -55,8 +58,8 @@ int launch_gradmax(int D, int N, const double* gvec, const uint8_t* pconst, cons
 int launch_trsv_upper(int n, int lda, const double* A, const double* y, size_t y_stride, double* x, long long* stamps,
                       cudaStream_t st);
 size_t chol_workspace_doubles(int n);
-int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, cudaStream_t st);
-extern FabricDev g_fabric_dev; // csrc/ba_schur.cu: reduce-scatter destinations read by the SYRK epilogue
+int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, const std::vector<int>& end_blk,
+                       int arrow_blk, cudaStream_t st);
 int launch_fabric_barrier(const FabricDev& fd, size_t flags_off, unsigned long long epoch, int* err, cudaStream_t st);
 int launch_fabric_gather(const FabricDev& fd, int nrows, int nmat, int ncols_vec, int lda, cudaStream_t st);
 int launch_fabric_allreduce(const FabricDev& fd, size_t flags_off, size_t mail_off, int mail_len, int parity,
@@ -265,30 +268,18 @@ struct Fabric2 {
   }
 };
 
-extern std::vector<int> g_syrk_kb_ranges;     // csrc/syrk_i8.cu: band hint of the current solve (both SYRK kernels)
-extern std::vector<int> g_chol_band_end;      // csrc/chol.cu: block structure of the reduced system (banded + arrow)
-extern int g_chol_arrow_blk;
-extern BandDev g_band_dev;                    // csrc/ba_schur.cu: device tables for ba_blocks / z_build / backsub
-
-// resets the process-wide kernel switches when a solve ends, on every exit path
-struct SolveGuard {
-  ~SolveGuard() {
-    g_fabric_dev.world = 0;
-    g_syrk_kb_ranges.clear();
-    g_chol_band_end.clear();
-    g_chol_arrow_blk = 0;
-    g_band_dev = BandDev{nullptr, nullptr, nullptr, 0};
-  }
-};
-
-// What compute_band_hint decided for the most recent solve, kept after SolveGuard has cleared the live globals
-// (vgg_dev_last_band_hint, csrc/dev_probes.h): the tests compare it with oracle/band_oracle.py
-struct BandRecord {
+// The band structure of one solve (compute_band_hint), passed to the launchers that use it; empty / null = dense.
+//   kb_ranges             SYRK k-block range per 128-column row block of Zt (launch_syrk)
+//   end_blk, arrow_blk    block structure of the reduced system (chol_lower_inplace)
+//   dev                   device tables for ba_blocks / z_build / backsub; kb_rows, fg_tracks: host copies of two of them
+struct BandPlan {
   int nb = 0, KB = 0, ngroups = 0, arrow_blk = 0;
-  bool active = false, chol = false, tables = false;
-  std::vector<int> rb_range, end_blk, kb_rows, fg_tracks;
+  std::vector<int> kb_ranges, end_blk, kb_rows, fg_tracks;
+  BandDev dev{nullptr, nullptr, nullptr, 0};
 };
-static thread_local BandRecord g_band_last;
+// the plan of the most recent solve on this thread (vgg_dev_last_band_hint): the tests compare it with
+// oracle/band_oracle.py
+static thread_local BandPlan g_band_last;
 
 // first / last visible point of every frame (N / -1 when the frame sees nothing): the band structure of sequential
 // (video) problems, where a point lives for a few windows and the dense [S, N] grid is mostly masked out
@@ -320,20 +311,15 @@ __global__ void __launch_bounds__(256) frame_point_range_kernel(int S, int N, co
 
 // Per 128-column row block of Zt: the 64-row k-block range outside which the block is exactly zero (Zt row 3n+c belongs to
 // point n; column d < S*dc to frame d / dc; the shared-intrinsics columns see every point).  Leaves the hint empty when
-// the grid is (nearly) dense.  One small kernel + a 8 S byte read-back per solve.
-static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad, int Kpad, bool multi_rank, cudaStream_t st) {
-  g_syrk_kb_ranges.clear();
-  g_chol_band_end.clear();
-  g_chol_arrow_blk = 0;
-  g_band_dev = BandDev{nullptr, nullptr, nullptr, 0};
+// the grid is (nearly) dense.  One small kernel + a 8 S byte read-back per solve.  *plan must come in empty (dense).
+static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad, int Kpad, bool multi_rank, cudaStream_t st,
+                             BandPlan* plan) {
   const char* env = getenv("VGG_BAND");                 // read per solve so that a test can compare both paths in one process
   const bool off = env && env[0] == '0';
   const int S = prob->S, N = prob->N, nb = Dpad / 128, KB = (Kpad + 63) / 64;
-  BandRecord& rec = g_band_last;
-  rec = BandRecord{};
-  rec.nb = nb;
-  rec.KB = KB;
-  rec.ngroups = (S + 31) / 32;
+  plan->nb = nb;
+  plan->KB = KB;
+  plan->ngroups = (S + 31) / 32;
   if (off || nb < 6 || N < 1024) return VGG_OK;
   static thread_local int* dev = nullptr;
   static thread_local int cap = 0;
@@ -375,9 +361,7 @@ static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad
       kept += std::max(0, std::min(rg[2 * bi + 1], rg[2 * bj + 1]) - std::max(rg[2 * bi], rg[2 * bj]));
     }
   if (kept < 0.7 * all) {
-    g_syrk_kb_ranges = rg;
-    rec.active = true;
-    rec.rb_range = rg;
+    plan->kb_ranges = rg;
     // the same structure for the factorisation: block (i, b) of the reduced system is non-zero iff the k ranges of row
     // blocks i and b meet; the blocks from the first shared-intrinsics column on (and the bordered right-hand-side row)
     // are the dense "arrow".  end[b] = one past the last band block of column b, made non-decreasing (the envelope
@@ -402,11 +386,8 @@ static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad
         end[b] = e;
         prev = e;
       }
-      g_chol_band_end = end;
-      g_chol_arrow_blk = arrow;
-      rec.chol = true;
-      rec.end_blk = end;
-      rec.arrow_blk = arrow;
+      plan->end_blk = end;
+      plan->arrow_blk = arrow;
       // device tables for the kernels that walk the dense [frames, points] grid (VGG_BAND=2: SYRK/Cholesky hint only)
       if (!(env && env[0] == '2')) {
         const int ngroups = (S + 31) / 32;
@@ -444,20 +425,20 @@ static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad
         }
         VGG_CUDA_CHECK(cudaMemcpyAsync(tdev, tab.data(), sizeof(int) * tab.size(), cudaMemcpyHostToDevice, st));
         VGG_CUDA_CHECK(cudaStreamSynchronize(st));           // pageable source
-        g_band_dev = BandDev{tdev, tdev + 2 * nb, tdev + 2 * (nb + KB), arrow * 128};
-        rec.tables = true;
-        rec.kb_rows.assign(t_kb, t_kb + 2 * KB);
-        rec.fg_tracks.assign(t_fg, t_fg + 2 * ngroups);
+        plan->dev = BandDev{tdev, tdev + 2 * nb, tdev + 2 * (nb + KB), arrow * 128};
+        plan->kb_rows.assign(t_kb, t_kb + 2 * KB);
+        plan->fg_tracks.assign(t_fg, t_fg + 2 * ngroups);
       }
     }
   }
   return VGG_OK;
 }
 
-// Schur complement of blk onto AR (Sraw, rhs, hdiag, gvec) at the given radius
-static int schur_build(const Layout& L, const BlockSet& b, const uint8_t* point_const, double radius, double min_diag,
-                       double max_diag, cudaStream_t st, ptrdiff_t mc_off = 0,
-                       const std::function<int()>* barrier = nullptr) {
+// Schur complement of blk onto AR (Sraw, rhs, hdiag, gvec) at the given radius; fd: where the SYRK epilogue sends each
+// row block in a fabric v2 solve
+static int schur_build(const Layout& L, const BlockSet& b, const BandPlan& band, const FabricDev& fd,
+                       const uint8_t* point_const, double radius, double min_diag, double max_diag, cudaStream_t st,
+                       ptrdiff_t mc_off = 0, const std::function<int()>* barrier = nullptr) {
   int rc;
   double* Sraw = L.AR;
   double* rhs = L.AR + (size_t)L.D * L.Dpad;
@@ -470,8 +451,8 @@ static int schur_build(const Layout& L, const BlockSet& b, const uint8_t* point_
   // fabric mode: every rank's copy must be zero before anyone's multimem reductions land in it
   if (mc_off && barrier && (rc = (*barrier)())) return rc;
   if ((rc = launch_assemble_hc(L.S, L.dc, L.ns, L.KR, L.Dpad, b.camrec, b.shared, Sraw, rhs, hdiag, gvec, mc_off, st))) return rc;
-  if ((rc = launch_z_transpose(L.D, L.N, L.Dpad, b.W, L.M, L.q, L.Zt, rhs, mc_off, st))) return rc;
-  if ((rc = launch_syrk(L.Kpad, L.Dpad, L.Zt, Sraw, mc_off, st))) return rc;
+  if ((rc = launch_z_transpose(L.D, L.N, L.Dpad, b.W, L.M, L.q, L.Zt, rhs, mc_off, band.dev.rb_range, st))) return rc;
+  if ((rc = launch_syrk(L.Kpad, L.Dpad, L.Zt, Sraw, mc_off, band.kb_ranges, fd, st))) return rc;
   // ... and all reductions must have landed before anyone reads its copy
   if (mc_off && barrier && (rc = (*barrier)())) return rc;
   return VGG_OK;
@@ -527,7 +508,7 @@ int vgg_ba_build_blocks(const vgg_ba_problem* prob, double* cost, double* camrec
   // a warp's first track t0 = chunk * tracks_per_warp + 4k is the 16-byte (uv) / 4-byte (mask) cp.async offset
   VGG_REQUIRE(tracks_per_warp >= 0 && tracks_per_warp % 4 == 0, "tracks_per_warp must be 0 (choose) or a multiple of 4");
   g_launch_count = 0;
-  return ba_build_blocks(prob, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, (cudaStream_t)stream);
+  return ba_build_blocks(prob, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, nullptr, (cudaStream_t)stream);
 }
 
 int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double* g_p, const double* H_pp,
@@ -550,7 +531,7 @@ int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double*
   VGG_CUDA_CHECK(cudaMemcpyAsync(L.sc_p, scale_p, sizeof(double) * (size_t)L.N * 3, cudaMemcpyDeviceToDevice, st));
   VGG_CUDA_CHECK(cudaMemsetAsync(L.Zt, 0, sizeof(double) * (size_t)L.Kpad * L.Dpad, st));
   VGG_CUDA_CHECK(cudaMemsetAsync(L.scal, 0, sizeof(double) * 16, st));
-  rc = schur_build(L, b, prob->point_const, radius, min_diag, max_diag, st);
+  rc = schur_build(L, b, BandPlan{}, FabricDev{}, prob->point_const, radius, min_diag, max_diag, st);
   if (rc) return rc;
   VGG_CUDA_CHECK(cudaMemcpyAsync(Sraw, L.AR, sizeof(double) * (size_t)L.D * L.Dpad, cudaMemcpyDeviceToDevice, st));
   VGG_CUDA_CHECK(cudaMemcpyAsync(rhs, L.AR + (size_t)L.D * L.Dpad, sizeof(double) * L.Dpad, cudaMemcpyDeviceToDevice, st));
@@ -559,7 +540,13 @@ int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double*
 }
 
 int vgg_cholesky_lower(int n, int lda, double* A, void* workspace, size_t ws_bytes, int* info_host, void* stream) {
-  VGG_REQUIRE(A && workspace && n > 0 && lda >= n, "bad arguments");
+  return vgg_dev_cholesky_band(n, lda, A, workspace, ws_bytes, info_host, stream, nullptr, 0, 0);
+}
+
+/* development probe (csrc/dev_probes.h): vgg_cholesky_lower of a banded + arrow matrix */
+int vgg_dev_cholesky_band(int n, int lda, double* A, void* workspace, size_t ws_bytes, int* info_host, void* stream,
+                          const int* end_blk, int count, int arrow_blk) {
+  VGG_REQUIRE(A && workspace && n > 0 && lda >= n && (end_blk || count <= 0), "bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
   g_launch_count = 0;
   const size_t need = sizeof(double) * chol_workspace_doubles(n) + 256;
@@ -569,7 +556,8 @@ int vgg_cholesky_lower(int n, int lda, double* A, void* workspace, size_t ws_byt
   }
   int* info = reinterpret_cast<int*>(workspace);
   double* diag = reinterpret_cast<double*>(reinterpret_cast<char*>(workspace) + 256);
-  int rc = chol_lower_inplace(n, lda, A, diag, info, st);
+  int rc = chol_lower_inplace(n, lda, A, diag, info, std::vector<int>(end_blk, end_blk + std::max(count, 0)),
+                              count > 0 ? arrow_blk : 0, st);
   if (rc) return rc;
   if (info_host) {
     VGG_CUDA_CHECK(cudaMemcpyAsync(info_host, info, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -630,7 +618,6 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
   // issued from the producing kernels; mc_off is the distance from a local address to its multicast twin
   ptrdiff_t mc_off = 0;
   Fabric2 fab2;
-  SolveGuard guard;
   static thread_local std::map<const double*, unsigned long long> fabric_epochs;
   if (fabric && fabric->ar_local && fabric->ar_multicast) {
     VGG_REQUIRE(fabric->ar_doubles >= ar_count, "fabric buffer too small (vgg_ba_reduced_system_doubles)");
@@ -652,8 +639,10 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
       VGG_REQUIRE(allreduce, "fabric v1 needs the hook for its barrier (op 2)");
     }
   }
-  if ((rc = compute_band_hint(prob, dc, D, L.Dpad, L.Kpad, allreduce != nullptr || fabric != nullptr, st))) return rc;
-  if (g_band_dev.fg_tracks) {
+  BandPlan band;
+  if ((rc = compute_band_hint(prob, dc, D, L.Dpad, L.Kpad, allreduce != nullptr || fabric != nullptr, st, &band))) return rc;
+  g_band_last = band;
+  if (band.dev.fg_tracks) {
     // the kernels skip the (track chunk, frame group) regions no observation falls into: their W blocks must read as zero
     const size_t w_doubles = (size_t)N * (size_t)(D + (D & 1)) * 3;
     VGG_CUDA_CHECK(cudaMemsetAsync(L.blk[0].W, 0, sizeof(double) * w_doubles, st));
@@ -696,7 +685,7 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     // cost | shared | camrec | g_p | H_pp are carved back to back: one memset covers all accumulators
     const size_t acc_bytes = reinterpret_cast<char*>(b.H_pp + (size_t)N * 6) - reinterpret_cast<char*>(b.cost);
     VGG_CUDA_CHECK(cudaMemsetAsync(b.cost, 0, acc_bytes, st));
-    return ba_build_blocks(&p, b.cost, b.camrec, b.g_p, b.H_pp, b.W, b.shared, 0, st, true);
+    return ba_build_blocks(&p, b.cost, b.camrec, b.g_p, b.H_pp, b.W, b.shared, 0, band.dev.fg_tracks, st, true);
   };
   // global cost + gradient max-norm of block set `which`; result lands in host h[0..2] = cost, gmax_c, gmax_p
   double* h_scal = pinned_scalars();
@@ -756,6 +745,7 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     ++it;
     const int cand = cur ^ 1;
     VGG_CUDA_CHECK(cudaMemsetAsync(L.scal, 0, sizeof(double) * 16, st));
+    FabricDev fd{};
     if (fab2.on) {
       // this iteration's copy of the reduced system (parity) and where the SYRK epilogue sends each row block
       const size_t off = (size_t)(it & 1) * fab2.lay.arc;
@@ -764,16 +754,13 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
       rhs = L.AR + (size_t)D * L.Dpad;
       hdiag = rhs + L.Dpad;
       gvec = hdiag + L.Dpad;
-      g_fabric_dev = fab2.at(off);
+      fd = fab2.at(off);
     }
-    if ((rc = schur_build(L, L.blk[cur], prob->point_const, radius, opt.min_lm_diagonal, opt.max_lm_diagonal, st, mc_off,
-                          (fab2.on || allreduce) ? &barrier_fn : nullptr)))
+    if ((rc = schur_build(L, L.blk[cur], band, fd, prob->point_const, radius, opt.min_lm_diagonal, opt.max_lm_diagonal, st,
+                          mc_off, (fab2.on || allreduce) ? &barrier_fn : nullptr)))
       return rc;
-    if (fab2.on) {
-      // every row block is complete on its owner: pull the others (matrix rows 0..D incl. the rhs row, then hdiag, gvec)
-      if ((rc = launch_fabric_gather(g_fabric_dev, D + 3, D + 1, D, L.Dpad, st))) return rc;
-      g_fabric_dev.world = 0;
-    }
+    // every row block is complete on its owner: pull the others (matrix rows 0..D incl. the rhs row, then hdiag, gvec)
+    if (fab2.on && (rc = launch_fabric_gather(fd, D + 3, D + 1, D, L.Dpad, st))) return rc;
     if (allreduce && !mc_off && (rc = allreduce(ar_user, L.AR, ar_count, 0, st))) return rc;
     if (!have_scale_c) {
       if ((rc = launch_jacobi_scale_cams(D, hdiag, L.sc_c, opt.jacobi_scaling, st))) return rc;
@@ -786,7 +773,7 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     // BORDERED matrix of order D+1 -- scale_damp put the scaled right-hand side into row D, so the factorisation leaves
     // y = L^-1 b there (and, mirrored like every panel, in column D): the forward substitution costs nothing and only the
     // backward substitution L^T x = y remains.  (cuSOLVER potrf on the same matrix took 1.05 ms at n = 2403, this 0.93.)
-    if ((rc = chol_lower_inplace(D + 1, L.Dpad, Sraw, L.chol_diag, L.dev_info, st))) return rc;
+    if ((rc = chol_lower_inplace(D + 1, L.Dpad, Sraw, L.chol_diag, L.dev_info, band.end_blk, band.arrow_blk, st))) return rc;
     // Backward substitution on U = L^T (the row-major upper triangle), y = column D of the buffer.
     const double* dcs = L.bvec;
     size_t dcs_stride = 1;
@@ -823,7 +810,7 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
       if ((rc = allreduce(ar_user, L.d_c, (size_t)L.Dpad, 1, st))) return rc;
       VGG_CUDA_CHECK(cudaMemcpyAsync(L.scal, L.d_c + L.Dpad - 2, sizeof(double) * 2, cudaMemcpyDeviceToDevice, st));
     }
-    if ((rc = launch_backsub(D, N, L.blk[cur].W, L.d_c, L.wacc, st))) return rc;
+    if ((rc = launch_backsub(D, N, L.blk[cur].W, L.d_c, L.wacc, band.dev.kb_rows, band.dev.arrow_row, st))) return rc;
     if ((rc = launch_point_step(N, L.M, L.blk[cur].g_p, L.wacc, L.sc_p, L.dpp, L.points[cur], radius, L.points[cand],
                                 L.scal, st)))
       return rc;
@@ -938,13 +925,13 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
 /* development probe (csrc/dev_probes.h): the band hint of the most recent solve on this thread */
 int vgg_dev_last_band_hint(int* meta, int* rb_range, int* end_blk, int* kb_rows, int* fg_tracks) {
   VGG_REQUIRE(meta, "null pointer");
-  const BandRecord& r = g_band_last;
-  const int m[8] = {r.active, r.chol, r.tables, r.nb, r.KB, r.ngroups, r.arrow_blk, 0};
+  const BandPlan& r = g_band_last;
+  const int m[8] = {!r.kb_ranges.empty(), !r.end_blk.empty(), !r.fg_tracks.empty(), r.nb, r.KB, r.ngroups, r.arrow_blk, 0};
   memcpy(meta, m, sizeof(m));
   auto put = [](int* dst, const std::vector<int>& v) {
     if (dst && !v.empty()) memcpy(dst, v.data(), sizeof(int) * v.size());
   };
-  put(rb_range, r.rb_range);
+  put(rb_range, r.kb_ranges);
   put(end_blk, r.end_blk);
   put(kb_rows, r.kb_rows);
   put(fg_tracks, r.fg_tracks);

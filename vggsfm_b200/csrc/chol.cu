@@ -780,17 +780,6 @@ int chol_set_attrs() {
   return VGG_OK;
 }
 
-}  // namespace
-
-// Block structure of a banded + arrow matrix (sequential / video problems; set by csrc/ba_solve.cu for the duration of
-// a solve, empty = dense): in block column b the rows that can be non-zero below the diagonal block are the band
-// [128 (b+1), 128 end_blk[b]) and the arrow [128 arrow_blk, n).  end_blk is non-decreasing (the envelope the
-// factorisation fills) and end_blk[b] >= b + 2 while b + 1 < arrow_blk, so block row b+1 is always in the band.
-std::vector<int> g_chol_band_end;
-int g_chol_arrow_blk = 0;
-
-namespace {
-
 // Ride-along rows per panel CTA for `rows` rows below the diagonal block (in `segs` separately chunked ranges): the
 // least multiple of 4 from C_RPC up such that the 1 + chunks CTAs, each needing a whole SM's shared memory, run in one
 // wave (a second wave repeats the whole POTRF128 on the critical path).  C_RPC_MAX is the most the POTRF128's
@@ -810,19 +799,19 @@ int chol_panel_rows(int below1, int below2, int* chunks) {
 //     rest of panel b's trailing update runs on the side streams behind step(b): U1(b) = block column b+2 (CU_NEXT,
 //     needed by step(b+2)) and U2(b) = block columns >= b+3 (CU_REST, needed by step(b+3)).
 //   lookahead == false: everything on st in program order (one CU_ALL update per panel, no fused update).
-int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags, cudaStream_t st, CholStreams* cs,
-                 bool lookahead) {
+int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags, const std::vector<int>& end_blk,
+                 int arrow_blk, cudaStream_t st, CholStreams* cs, bool lookahead) {
   const int nblk = (n + CB - 1) / CB;
   const size_t smem_u = sizeof(double) * 2 * CT * CUD;
   // the band structure is honoured by the lookahead schedule only; the program-order schedule treats the matrix as dense
-  const bool banded = lookahead && (int)g_chol_band_end.size() >= nblk && g_chol_arrow_blk > 0;
+  const bool banded = lookahead && (int)end_blk.size() >= nblk && arrow_blk > 0;
   auto band_rows = [&](int b, int* band_end, int* arrow_lo) {
     if (!banded) {
       *band_end = *arrow_lo = n;
       return;
     }
-    *band_end = std::min(n, g_chol_band_end[b] * CB);
-    *arrow_lo = std::min(n, std::max(g_chol_arrow_blk * CB, *band_end));
+    *band_end = std::min(n, end_blk[b] * CB);
+    *arrow_lo = std::min(n, std::max(arrow_blk * CB, *band_end));
     if (*band_end >= n || *arrow_lo <= *band_end) *band_end = *arrow_lo = n;      // no gap left: plain dense rows
   };
   auto panel = [&](int b) -> int {
@@ -899,7 +888,12 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
 // In-place Cholesky of the row-major lower triangle of A[n x n] (lda even, A 16-byte aligned): on return the lower
 // triangle holds L and the strict upper triangle L^T.  info (device int): 0 or the 1-based index of the first
 // non-positive pivot.  VGG_CHOL_GRAPH=0 switches the CUDA graph off.
-int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, cudaStream_t st) {
+// Block structure of a banded + arrow matrix (sequential / video problems; empty end_blk = dense): in block column b
+// the rows that can be non-zero below the diagonal block are the band [128 (b+1), 128 end_blk[b]) and the arrow
+// [128 arrow_blk, n).  end_blk is non-decreasing (the envelope the factorisation fills) and end_blk[b] >= b + 2 while
+// b + 1 < arrow_blk, so block row b+1 is always in the band.
+int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, const std::vector<int>& end_blk,
+                       int arrow_blk, cudaStream_t st) {
   VGG_REQUIRE((lda % 2) == 0, "lda must be even");
   int rc;
   if ((rc = chol_set_attrs())) return rc;
@@ -911,19 +905,19 @@ int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, cuda
   const int nblk = (n + CB - 1) / CB;
   CholStreams* cs = nullptr;
   if ((rc = chol_streams(&cs))) return rc;
-  if (nblk < 3 || !use_graph) return chol_enqueue(n, lda, A, Ldiag, info, flags, st, cs, nblk >= 3);
+  if (nblk < 3 || !use_graph) return chol_enqueue(n, lda, A, Ldiag, info, flags, end_blk, arrow_blk, st, cs, nblk >= 3);
   // one captured graph per (matrix, order): ~60 launches + events become a single cudaGraphLaunch
   typedef std::tuple<double*, int, int, int*, double*, unsigned long long> Key;
   static thread_local std::map<Key, cudaGraphExec_t> cache;
-  unsigned long long band_hash = (unsigned long long)g_chol_arrow_blk;
-  for (int v : g_chol_band_end) band_hash = band_hash * 1000003ull + (unsigned long long)(v + 1);
+  unsigned long long band_hash = (unsigned long long)arrow_blk;
+  for (int v : end_blk) band_hash = band_hash * 1000003ull + (unsigned long long)(v + 1);
   const Key key(A, n, lda, info, Ldiag, band_hash);
   auto it = cache.find(key);
   if (it == cache.end()) {
     const long long launches_before = g_launch_count;
     cudaGraph_t graph = nullptr;
     VGG_CUDA_CHECK(cudaStreamBeginCapture(cs->cap, cudaStreamCaptureModeThreadLocal));
-    rc = chol_enqueue(n, lda, A, Ldiag, info, flags, cs->cap, cs, true);
+    rc = chol_enqueue(n, lda, A, Ldiag, info, flags, end_blk, arrow_blk, cs->cap, cs, true);
     const cudaError_t ce = cudaStreamEndCapture(cs->cap, &graph);
     g_launch_count = launches_before;
     if (rc) {
@@ -968,15 +962,6 @@ extern "C" int vgg_dev_chol128_probe(int reps, const double* A_host, double* L_h
   cudaFree(dA);
   cudaFree(dL);
   cudaFree(dP);
-  return VGG_OK;
-}
-
-// tests: install / clear (count = 0) the block structure the next factorisations assume (csrc/ba_solve.cu sets the same
-// globals from the visibility mask for the duration of a solve)
-extern "C" int vgg_dev_set_chol_band(const int* end_blk_host, int count, int arrow_blk) {
-  using namespace vgg;
-  g_chol_band_end.assign(end_blk_host, end_blk_host + (count > 0 ? count : 0));
-  g_chol_arrow_blk = count > 0 ? arrow_blk : 0;
   return VGG_OK;
 }
 

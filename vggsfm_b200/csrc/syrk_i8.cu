@@ -392,22 +392,19 @@ size_t oz_workspace_bytes(int Kpad, int Dpad, int s) {
 size_t syrk_i8_workspace_bytes(int Kpad, int Dpad, int slices) { return oz_workspace_bytes(Kpad, Dpad, slices); }
 
 // Sraw -= Zt^T Zt with s int8 slices.  Zt [Kpad][Dpad] (Dpad % 128 == 0), Cmat [Dpad][Dpad] row-major, LOWER triangle
-// written, same contract as launch_syrk.
-// Band hint of the current solve (csrc/ba_solve.cu): [lo, hi) k-block range per 128-column row block of Zt outside which
-// the block is exactly zero; empty = dense.  Tiles whose two ranges do not intersect are skipped, the others shortened.
-std::vector<int> g_syrk_kb_ranges;
-extern FabricDev g_fabric_dev;  // csrc/ba_schur.cu: reduce-scatter destinations of the current multi-GPU solve (world <= 1: off)
-
-int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc_off, int s, void* ws,
-                   size_t ws_bytes, cudaStream_t st) {
+// written, same contract as launch_syrk.  kb_ranges: [lo, hi) k-block range per 128-column row block of Zt outside which
+// the block is exactly zero; any other size = dense.  Tiles whose two ranges do not intersect are skipped, the others
+// shortened.
+int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, int s, void* ws, size_t ws_bytes,
+                   const std::vector<int>& kb_ranges, cudaStream_t st) {
   VGG_REQUIRE(Dpad % OZ_BM == 0, "syrk_i8: Dpad must be a multiple of 128");
   VGG_REQUIRE(ws_bytes >= oz_workspace_bytes(Kpad, Dpad, s), "syrk_i8: workspace too small");
   const int KB = (Kpad + OZ_BK - 1) / OZ_BK;
   const int nb = Dpad / OZ_BM;
   OzHostState& hs = g_oz;
-  const bool banded = (int)g_syrk_kb_ranges.size() == 2 * nb;
-  if (hs.Kpad != Kpad || hs.Dpad != Dpad || hs.slices != s || (banded ? hs.ranges != g_syrk_kb_ranges : !hs.ranges.empty())) {
-    hs.ranges = banded ? g_syrk_kb_ranges : std::vector<int>();
+  const bool banded = (int)kb_ranges.size() == 2 * nb;
+  if (hs.Kpad != Kpad || hs.Dpad != Dpad || hs.slices != s || (banded ? hs.ranges != kb_ranges : !hs.ranges.empty())) {
+    hs.ranges = banded ? kb_ranges : std::vector<int>();
     if (banded) {
       if (hs.ranges_cap < hs.ranges.size()) {
         if (hs.ranges_dev) cudaFree(hs.ranges_dev);
@@ -464,7 +461,7 @@ int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t
   VGG_LAUNCH_CHECK();
   const int grid = std::min(hs.sms, nwork);
   oz_syrk_kernel<<<grid, OZ_THREADS, OZ_SMEM_BYTES, st>>>(hs.plan, work_d, nwork, KB, slices, slice_stride, expo, pow2, Dpad,
-                                                          Cmat, mc_off, g_fabric_dev);
+                                                          Cmat, 0, FabricDev{});
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
@@ -472,13 +469,6 @@ int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t
 }  // namespace vgg
 
 extern "C" {
-
-/* development probe (csrc/dev_probes.h): install / clear (count = 0) the band hint the next SYRK calls plan with */
-int vgg_dev_set_syrk_ranges(const int* ranges_host, int count) {
-  using namespace vgg;
-  g_syrk_kb_ranges.assign(ranges_host, ranges_host + (count > 0 ? count : 0));
-  return VGG_OK;
-}
 
 int vgg_syrk_ozaki_workspace_bytes(int Kpad, int Dpad, int slices, size_t* bytes) {
   using namespace vgg;
@@ -489,10 +479,17 @@ int vgg_syrk_ozaki_workspace_bytes(int Kpad, int Dpad, int slices, size_t* bytes
 
 int vgg_syrk_ozaki(int Kpad, int Dpad, const double* Zt, double* Cmat, int slices, void* workspace, size_t ws_bytes,
                    void* stream) {
+  return vgg_dev_syrk_ozaki_band(Kpad, Dpad, Zt, Cmat, slices, workspace, ws_bytes, stream, nullptr, 0);
+}
+
+/* development probe (csrc/dev_probes.h): vgg_syrk_ozaki with a band hint */
+int vgg_dev_syrk_ozaki_band(int Kpad, int Dpad, const double* Zt, double* Cmat, int slices, void* workspace,
+                            size_t ws_bytes, void* stream, const int* ranges, int count) {
   using namespace vgg;
   g_launch_count = 0;
-  VGG_REQUIRE(Zt && Cmat && workspace, "null pointer");
-  return launch_syrk_i8(Kpad, Dpad, Zt, Cmat, 0, slices, workspace, ws_bytes, static_cast<cudaStream_t>(stream));
+  VGG_REQUIRE(Zt && Cmat && workspace && (ranges || count <= 0), "null pointer");
+  return launch_syrk_i8(Kpad, Dpad, Zt, Cmat, slices, workspace, ws_bytes,
+                        std::vector<int>(ranges, ranges + std::max(count, 0)), static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"
