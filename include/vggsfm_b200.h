@@ -346,6 +346,61 @@ int vgg_corr_tc_sample(int BS, int N, int C, int H, int W, int num_levels, int r
 int vgg_sample_features4d(int B, int C, int H, int W, int R, const float* input_nchw, const float* coords, float* out,
                           void* stream);
 
+/* ------------------------------------------------------------------------------------------- */
+/* Dense depth stage (align_dense_depth_maps, vggsfm/utils/utils.py:635-770), all frames per call */
+/* ------------------------------------------------------------------------------------------- */
+
+/* Frames' disparity maps are one CSR: frame f is float32 [H_f, W_f] row-major at map_offsets[f] (int64 [F+1]),
+ * map_hw int32 [F,2] = (H_f, W_f).  Sparse samples are a CSR too: int32 offsets [F+1] into the per-sample arrays. */
+
+/* utils.py:669-690: per observation i of frame uvd_frame[i], uvd double [n,3] = (u, v, depth): np.round (half to
+ * even) of (u, v), bounds 0 <= u < W, 0 <= v < H, nearest-pixel disparity x_out (0 when out of bounds),
+ * y_out = 1 / clip(depth, depth_min, depth_max), keep_out = x_out > 0. */
+int vgg_depth_sparse_samples(int n_total, const int32_t* uvd_frame, const double* uvd, double depth_min,
+                             double depth_max, const int64_t* map_offsets, const int32_t* map_hw, const float* disp,
+                             float* x_out, double* y_out, uint8_t* keep_out, void* stream);
+
+/* np.median(y) / divisor per frame (utils.py:695; the median is the mean of the two middle values for an even count,
+ * NaN for none), each step one IEEE double operation.  y >= 0. */
+int vgg_depth_median(int F, const int32_t* offsets, const double* y, double divisor, double* median_out,
+                     void* stream);
+
+/* RANSACRegressor(LinearRegression(), min_samples=2, residual_threshold=threshold[f], max_trials, loss=
+ * "squared_error").fit(x[:, None], y) per frame (utils.py:700-709), x float32, y double.  begin() resets every frame;
+ * each chunk() evaluates T trials (T <= vgg_depth_ransac_max_chunk()) of the R live frames `frames` int32 [R], the
+ * trial's two sample indices in samples int32 [R,T,2] (drawn by the caller), and writes running_out uint8 [F] for
+ * those frames (1 while n_trials < max_trials).  finish() writes scale / shift float32 [F] (coef_[0], intercept_),
+ * n_trials / n_inliers int32 [F] (n_inliers -1 when no trial was kept: sklearn's "could not find a valid consensus
+ * set") and inlier_mask uint8 in the sample CSR.  The workspace holds the per-frame state and one chunk's trials. */
+int vgg_depth_ransac_workspace_bytes(int F, size_t* bytes);
+int vgg_depth_ransac_max_chunk(void);
+int vgg_depth_ransac_begin(int F, int max_trials, void* workspace, size_t ws_bytes, void* stream);
+int vgg_depth_ransac_chunk(int F, const int32_t* offsets, const float* x, const double* y, const double* threshold,
+                           int R, const int32_t* frames, int T, const int32_t* samples, uint8_t* running_out,
+                           void* workspace, size_t ws_bytes, void* stream);
+int vgg_depth_ransac_finish(int F, const int32_t* offsets, const float* x, const double* y, const double* threshold,
+                            float* scale_out, float* shift_out, int32_t* n_trials_out, int32_t* n_inliers_out,
+                            uint8_t* inlier_mask_out, void* workspace, size_t ws_bytes, void* stream);
+
+/* utils.py:712-724 in one pass: disp != 0 -> disp * scale[f] + shift[f] (float32 ops, written back in place),
+ * kept where 0 < disp <= 10000 and 0 elsewhere; depth_out = float32(1 / disp), 0 where disp == 0.  Frame f spans
+ * the tiles tile_offsets[f] .. tile_offsets[f+1] (int64 [F+1]) of vgg_depth_tile_pixels() pixels each;
+ * tile_counts int32 [n_tiles] (may be NULL) receives each tile's valid-pixel count. */
+int vgg_depth_tile_pixels(void);
+int vgg_depth_apply(int F, int64_t n_tiles, const int64_t* map_offsets, const int64_t* tile_offsets,
+                    const float* scale, const float* shift, float* disp, float* depth_out, int32_t* tile_counts,
+                    void* stream);
+
+/* utils.py:728-765 (visual_dense_point_cloud): valid pixels (depth != 0) in row-major order, compacted by
+ * tile_base int64 [n_tiles + 1] (exclusive prefix of tile_counts): pixel (x, y) without +0.5 through cam_from_img
+ * (cam_model VGG_SIMPLE_*, cam_params double [F,4] = f, cx, cy, k), times depth, through world_from_cam double
+ * [F,3,4] (cam_from_world.inverse()).  Frame f's M_f points are one [2, M_f, 3] block of `out` double starting at
+ * 6 * tile_base[tile_offsets[f]]: the world points, then rgb uint8 [pixels,3] / 255. */
+int vgg_depth_unproject(int F, int64_t n_tiles, const int64_t* map_offsets, const int32_t* map_hw,
+                        const int64_t* tile_offsets, const int64_t* tile_base, const float* depth, const uint8_t* rgb,
+                        const int32_t* cam_model, const double* cam_params, const double* world_from_cam,
+                        double* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

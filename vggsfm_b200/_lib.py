@@ -24,6 +24,9 @@ EXPORTS = [
     "vgg_corr_tc_supported", "vgg_corr_tc_bytes", "vgg_corr_tc_build", "vgg_corr_tc_sample",
     "vgg_twoview_workspace_bytes", "vgg_estimate_fundamental", "vgg_relative_pose_from_fundamental",
     "vgg_fundamental_inliers", "vgg_msac_fundamental_workspace_bytes", "vgg_estimate_fundamental_msac",
+    "vgg_depth_sparse_samples", "vgg_depth_median", "vgg_depth_ransac_workspace_bytes", "vgg_depth_ransac_max_chunk",
+    "vgg_depth_ransac_begin", "vgg_depth_ransac_chunk", "vgg_depth_ransac_finish", "vgg_depth_tile_pixels",
+    "vgg_depth_apply", "vgg_depth_unproject",
 ]
 
 
@@ -176,6 +179,17 @@ def lib() -> ctypes.CDLL:
     L.vgg_msac_fundamental_workspace_bytes.argtypes = [ci, ci, ci, ci, ctypes.POINTER(cs)]
     L.vgg_estimate_fundamental_msac.argtypes = [ci, ci, vp, vp, ci, vp, cd, ci, ci, cu64, vp, vp, vp, vp, vp, cs, vp]
     L.vgg_dev_msac_trace.argtypes = [ci, ci, ci, ci, vp, ci, vp, vp, vp]
+    i64 = ctypes.c_int64
+    L.vgg_depth_sparse_samples.argtypes = [ci, vp, vp, cd, cd, vp, vp, vp, vp, vp, vp, vp]
+    L.vgg_depth_median.argtypes = [ci, vp, vp, cd, vp, vp]
+    L.vgg_depth_ransac_workspace_bytes.argtypes = [ci, ctypes.POINTER(cs)]
+    L.vgg_depth_ransac_max_chunk.argtypes = []
+    L.vgg_depth_ransac_begin.argtypes = [ci, ci, vp, cs, vp]
+    L.vgg_depth_ransac_chunk.argtypes = [ci, vp, vp, vp, vp, ci, vp, ci, vp, vp, vp, cs, vp]
+    L.vgg_depth_ransac_finish.argtypes = [ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, cs, vp]
+    L.vgg_depth_tile_pixels.argtypes = []
+    L.vgg_depth_apply.argtypes = [ci, i64, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.vgg_depth_unproject.argtypes = [ci, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     _lib = L
     return L
 

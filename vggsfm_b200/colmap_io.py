@@ -122,3 +122,22 @@ def read_model(path):
             points[vals[0]] = {"xyz": np.array(vals[1:4]), "rgb": np.array(vals[4:7], dtype=np.uint8), "error": vals[7],
                                "track": [tuple(int(v) for v in t) for t in tr]}
     return {"cameras": cameras, "images": images, "points3D": points}
+
+
+def write_array(array, path):
+    """COLMAP's dense map format (``colmap::mvs::Mat<T>::Write``) as vggsfm/utils/utils.py:359-389 writes it, byte for
+    byte: the ASCII header ``width&height&channels&``, then the float32 values little-endian in column-major order
+    (x fastest within a row of the transposed map, channels slowest)."""
+    assert array.dtype == np.float32
+    if array.ndim == 2:
+        height, width = array.shape
+        channels = 1
+        trans = array.T
+    elif array.ndim == 3:
+        height, width, channels = array.shape
+        trans = np.transpose(array, (1, 0, 2))
+    else:
+        raise AssertionError("write_array takes a 2-D or 3-D array")
+    with open(path, "wb") as fid:
+        fid.write(f"{width}&{height}&{channels}&".encode())
+        fid.write(trans.reshape(-1, order="F").astype("<f4", copy=False).tobytes())

@@ -60,6 +60,24 @@ class Rigid3d:
     def matrix(self):
         return np.concatenate([self.rotation.matrix(), self.translation[:, None]], axis=1)
 
+    def inverse(self):
+        """pycolmap.Rigid3d.inverse(): rotation R^T, translation -R^T t."""
+        Ri = self.rotation.matrix().T
+        return Rigid3d(Rotation3d(Ri), -_apply(Ri, np.zeros(3), self.translation))
+
+    def __mul__(self, x):
+        """``Rigid3d * point`` for a 3-vector or an [N,3] array: R x + t (pycolmap 3.10)."""
+        if isinstance(x, Rigid3d):
+            R = self.rotation.matrix()
+            return Rigid3d(Rotation3d(R @ x.rotation.matrix()), _apply(R, self.translation, x.translation))
+        return _apply(self.rotation.matrix(), self.translation, np.asarray(x, dtype=np.float64))
+
+
+def _apply(R, t, p):
+    """R p + t with each row's terms added left to right, for p of shape [3] or [N,3] (the same rounding either way,
+    which the vectorised dense-depth code relies on)."""
+    return p[..., 0, None] * R[:, 0] + p[..., 1, None] * R[:, 1] + p[..., 2, None] * R[:, 2] + t
+
 
 class Camera:
     """pycolmap.Camera for the two models the reference supports (tensor_to_pycolmap.py:78-110)."""
@@ -82,6 +100,57 @@ class Camera:
     def calibration_matrix(self):
         f, cx, cy = self.params[:3]
         return np.array([[f, 0.0, cx], [0.0, f, cy], [0.0, 0.0, 1.0]])
+
+    def img_from_cam(self, cam_points):
+        """pycolmap 3.10 ``Camera.img_from_cam`` [3P-memory]: a 3-vector (or [N,3]) is divided by its z, then the
+        model maps it to pixels (SIMPLE_RADIAL: f (u + u k r^2) + cx); a 2-vector (or [N,2]) is taken as already
+        normalised.  runner.py:769 passes the 3-vector ``cam_from_world * xyz``."""
+        p = np.asarray(cam_points, dtype=np.float64)
+        if p.shape[-1] == 3:
+            u, v = p[..., 0] / p[..., 2], p[..., 1] / p[..., 2]
+        else:
+            u, v = p[..., 0], p[..., 1]
+        f, cx, cy = self.params[:3]
+        if self.model == "SIMPLE_RADIAL":
+            rad = self.params[3] * (u * u + v * v)
+            u, v = u + u * rad, v + v * rad
+        return np.stack([f * u + cx, f * v + cy], axis=-1)
+
+    def cam_from_img(self, image_points):
+        """pycolmap 3.10 ``Camera.cam_from_img``: pixels [N,2] (or a 2-vector) -> normalised [N,2].  SIMPLE_RADIAL
+        inverts the distortion with COLMAP's iterative undistortion [3P-memory]."""
+        xy = np.asarray(image_points, dtype=np.float64)
+        f, cx, cy = self.params[:3]
+        u, v = (xy[..., 0] - cx) / f, (xy[..., 1] - cy) / f
+        if self.model == "SIMPLE_RADIAL":
+            u, v = _iterative_undistortion(self.params[3], u, v)
+        return np.stack([u, v], axis=-1)
+
+
+def _iterative_undistortion(k, u, v):
+    """COLMAP BaseCameraModel::IterativeUndistortion for SIMPLE_RADIAL (Newton, central-difference Jacobian with
+    relative step 1e-6, at most 100 iterations, stop once the squared step is below 1e-10) [3P-memory]."""
+    u, v = np.array(u, dtype=np.float64, ndmin=1), np.array(v, dtype=np.float64, ndmin=1)
+    shape = np.shape(u)
+    u, v = u.reshape(-1).copy(), v.reshape(-1).copy()
+    x0, y0 = u.copy(), v.copy()
+    eps = np.finfo(np.float64).eps
+    for i in range(len(u)):
+        x, y = u[i], v[i]
+        for _ in range(100):
+            s0, s1 = max(eps, abs(1e-6 * x)), max(eps, abs(1e-6 * y))
+            d = [(a * k * (a * a + b * b), b * k * (a * a + b * b))
+                 for a, b in ((x, y), (x - s0, y), (x + s0, y), (x, y - s1), (x, y + s1))]
+            J00, J01 = 1 + (d[2][0] - d[1][0]) / (2 * s0), (d[4][0] - d[3][0]) / (2 * s1)
+            J10, J11 = (d[2][1] - d[1][1]) / (2 * s0), 1 + (d[4][1] - d[3][1]) / (2 * s1)
+            r0, r1 = x + d[0][0] - x0[i], y + d[0][1] - y0[i]
+            det = J00 * J11 - J01 * J10
+            st0, st1 = (J11 * r0 - J01 * r1) / det, (J00 * r1 - J10 * r0) / det
+            x, y = x - st0, y - st1
+            if st0 * st0 + st1 * st1 < 1e-10:
+                break
+        u[i], v[i] = x, y
+    return u.reshape(shape), v.reshape(shape)
 
 
 class Point2D:
