@@ -135,8 +135,9 @@ int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double*
                  double* Sraw, double* rhs, int* Dpad_out, void* stream);
 
 /* Blocked Cholesky of the reduced camera system (csrc/chol.cu): in-place factorisation of the row-major
- * lower triangle of A [n x n], leading dimension lda (even), replacing the potrf inside Ceres' DENSE_SCHUR.  On
- * return the lower triangle holds L and the strict upper triangle L^T.
+ * lower triangle of A [n x n], leading dimension lda (any even lda >= n, A 16-byte aligned), replacing the potrf inside
+ * Ceres' DENSE_SCHUR.  On return the lower triangle holds L and the strict upper triangle L^T.  Nothing outside the
+ * n x n matrix is read or written, and the input in the strict upper triangle is never used (it may hold anything).
  * workspace >= ceil(n/128)*131072 + 1024 bytes (n <= 24000); *info_host = 0, the 1-based index of the failing pivot, or
  * INT_MAX if the in-kernel hand-off between CTAs stalled (bounded spin; never seen, reported instead of hanging). */
 int vgg_cholesky_lower(int n, int lda, double* A, void* workspace, size_t ws_bytes, int* info_host, void* stream);

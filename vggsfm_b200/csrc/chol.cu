@@ -124,7 +124,13 @@ __device__ __forceinline__ int cta_chol128(double* Ls, double* dinv, int* fail_s
       const double AC = A * C;
       const double det = fma(-B, B, AC);
       double ia = fast_rsqrt(A);
-      double ib = (A * ia) * fast_rsqrt(det);
+      const double rdet = fast_rsqrt(det);
+      double ib = (A * ia) * rdet;
+      // L11 itself as sqrt(det / A) from the same two reciprocal roots, so that L11 * ib = 1 to a few roundings.  The
+      // rows below are scaled by ib; an L11 taken from C - l10^2 instead differs from 1 / ib by the rounding of det
+      // relative to the pivot, ~eps C / (C - B^2/A), and a nearly dependent pair then leaves that much backward error
+      // in every entry of its second column (the diagonal itself is fine either way)
+      double d11 = (det * rdet) * ia;
       double l10 = B * ia;
       // the tests run in the shadow of the two rsqrt chains; the branch is warp-uniform (every lane holds A, B, C)
       const bool good = A >= CHOL_PMIN && det >= CHOL_PMIN && AC < 1e280 && AC > 1e-280;
@@ -141,9 +147,10 @@ __device__ __forceinline__ int cta_chol128(double* Ls, double* dinv, int* fail_s
         } else {
           ib = rsqrt(p1);
         }
+        d11 = p1 * ib;                                      // sequential: consistent with ib = rsqrt(p1)
       }
       const double x0 = a[j] * ia;                          // lane j: A * ia = sqrt(A)
-      const double x1 = fma(-x0, l10, a[j + 1]) * ib;       // lane j+1: (C - l10^2) / sqrt(C - l10^2)
+      const double x1 = lane == j + 1 ? d11 : fma(-x0, l10, a[j + 1]) * ib;   // lane j+1: L11; lanes > j+1: L[lane][j+1]
       a[j] = x0;
       a[j + 1] = x1;
       if (lane == j) {
@@ -441,13 +448,17 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
   const int cidx = (int)blockIdx.x - 1;
   const int r0 = cidx < chunks1r ? k0 + CB + cidx * xr : arrow_lo + (cidx - chunks1r) * xr;
   const int nrows = solver ? min(xr, (cidx < chunks1r ? band_hi : n) - r0) : 0;
-  // diagonal block (rows < nb: whole 128-double rows, the part above the diagonal is never read; identity padding
-  // beyond nb) and this CTA's xr panel rows: cp.async, all 16-byte chunks in flight at once (r02: the plain
-  // load -> store loop serialised 32 L2 round trips per thread, a third of the kernel)
+  // diagonal block (rows < nb: columns < nb, the part above the diagonal is never read; identity padding beyond nb)
+  // and this CTA's xr panel rows: cp.async, all 16-byte chunks in flight at once (r02: the plain load -> store loop
+  // serialised 32 L2 round trips per thread, a third of the kernel).  Columns >= n are not loaded: in the last panel
+  // k0 + 127 may lie beyond the row (lda >= n is all the caller promises), and for the last row beyond the matrix;
+  // they are above the diagonal, so zeros do.  The chunk straddling column n (odd n) loads its one matrix element.
   for (int e = tid; e < CB * (CB / 2); e += C_THREADS) {
     const int i = e >> 6, j = (e & 63) * 2;
-    if (i < nb) {
+    if (i < nb && j + 1 < nb) {
       cp_async16(Ls + i * CLD + j, A + (size_t)(k0 + i) * lda + k0 + j);
+    } else if (i < nb) {
+      *reinterpret_cast<double2*>(Ls + i * CLD + j) = make_double2(j < nb ? A[(size_t)(k0 + i) * lda + k0 + j] : 0.0, 0.0);
     } else {
       *reinterpret_cast<double2*>(Ls + i * CLD + j) = make_double2(j == i ? 1.0 : 0.0, j + 1 == i ? 1.0 : 0.0);
     }
@@ -885,7 +896,7 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
 
 }  // namespace
 
-// In-place Cholesky of the row-major lower triangle of A[n x n] (lda even, A 16-byte aligned): on return the lower
+// In-place Cholesky of the row-major lower triangle of A[n x n] (any even lda >= n, A 16-byte aligned): on return the lower
 // triangle holds L and the strict upper triangle L^T.  info (device int): 0 or the 1-based index of the first
 // non-positive pivot.  VGG_CHOL_GRAPH=0 switches the CUDA graph off.
 // Block structure of a banded + arrow matrix (sequential / video problems; empty end_blk = dense): in block column b
