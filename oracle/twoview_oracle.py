@@ -378,8 +378,10 @@ def decompose_essential_matrix(E):
     return np.stack([R1, R1, R2, R2], 1), np.stack([T, -T, T, -T], 1)
 
 
-def cheirality_counts(R, t, x1, x2):
-    """R [3,3], t [3], x1/x2 [N,2] normalised -> number of points in front of both cameras inside the depth window."""
+def cheirality_counts(R, t, x1, x2, return_margin=False):
+    """R [3,3], t [3], x1/x2 [N,2] normalised -> number of points in front of both cameras inside the depth window.
+    With return_margin: (count, margin), margin = the smallest relative distance of a finite depth (either camera) to
+    K_MIN_DEPTH or to the window 1000 |R^T t|."""
     N = x1.shape[0]
     P1 = np.eye(3, 4)
     P2 = np.concatenate([R, t[:, None]], 1)
@@ -397,11 +399,25 @@ def cheirality_counts(R, t, x1, x2):
         d1 = X[:, 2]
         d2 = X @ R[2] + t[2]
     max_depth = 1000.0 * np.linalg.norm(R.T @ t)
-    return int(((d1 > K_MIN_DEPTH) & (d1 < max_depth) & (d2 > K_MIN_DEPTH) & (d2 < max_depth)).sum())
+    cnt = int(((d1 > K_MIN_DEPTH) & (d1 < max_depth) & (d2 > K_MIN_DEPTH) & (d2 < max_depth)).sum())
+    if not return_margin:
+        return cnt
+    d = np.concatenate([d1, d2])
+    d = d[np.isfinite(d)]
+    margin = np.inf
+    if d.size:
+        margin = float(np.min(np.abs(d - K_MIN_DEPTH)) / K_MIN_DEPTH)
+        if max_depth > 0:
+            margin = min(margin, float(np.min(np.abs(d - max_depth)) / max_depth))
+    return cnt, margin
 
 
-def relative_pose(fmat, points1, points2, width, height):
-    """fmat [B,3,3], points [B,N,2] -> (R [B,3,3], t [B,3], E [B,3,3], counts [B,4])."""
+def relative_pose(fmat, points1, points2, width, height, return_debug=False):
+    """fmat [B,3,3], points [B,N,2] -> (R [B,3,3], t [B,3], E [B,3,3], counts [B,4]).  With return_debug a fifth
+    element: per pair a dict with the candidates (Rs [4,3,3], ts [4,3]), the chosen index `k` (first maximum), the
+    singular values `sigma` of E, `depth_margin` (the smallest relative distance of any finite triangulated depth, over
+    the four candidates and both cameras, to K_MIN_DEPTH or to the depth window) and `count_gap` (the smallest count
+    difference between the winner and a candidate with a different (R, t); inf when there is none)."""
     K = default_kmat(width, height)
     E = K.T @ fmat @ K
     Rs, ts = decompose_essential_matrix(E)
@@ -411,10 +427,66 @@ def relative_pose(fmat, points1, points2, width, height):
     R = np.zeros((B, 3, 3))
     t = np.zeros((B, 3))
     counts = np.zeros((B, 4), np.int64)
+    debug = []
     for b in range(B):
         x1 = (np.asarray(points1[b], np.float64) - pp) / f
         x2 = (np.asarray(points2[b], np.float64) - pp) / f
-        counts[b] = [cheirality_counts(Rs[b, k], ts[b, k], x1, x2) for k in range(4)]
+        cm = [cheirality_counts(Rs[b, k], ts[b, k], x1, x2, return_margin=True) for k in range(4)]
+        counts[b] = [c for c, _ in cm]
         k = int(np.argmax(counts[b]))
         R[b], t[b] = Rs[b, k], ts[b, k]
+        if return_debug:
+            gap = np.inf
+            for j in range(4):
+                same = np.abs(Rs[b, j] - Rs[b, k]).max() <= 1e-12 and np.abs(ts[b, j] - ts[b, k]).max() <= 1e-12
+                if j != k and not same:
+                    gap = min(gap, float(counts[b, k] - counts[b, j]))
+            debug.append(dict(Rs=Rs[b], ts=ts[b], k=k, sigma=np.linalg.svd(E[b], compute_uv=False),
+                              depth_margin=min(m for _, m in cm), count_gap=gap))
+    if return_debug:
+        return R, t, E, counts, debug
     return R, t, E, counts
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# conditioning of the decomposition
+# ---------------------------------------------------------------------------------------------------------------------
+EPS = 2.0 ** -52
+POSE_BAR_C = 96.0
+
+
+def pose_bar(sigma):
+    """Bar on max |R - R_ref| and max |t - t_ref| between two float64 decompositions of the same F:
+    POSE_BAR_C * eps * sigma_1 / sigma_2 (eps = 2^-52; inf when sigma_2 = 0).
+
+    Derivation, with u = 2^-53 the unit roundoff and sigma_3 << sigma_2 (E is within rounding of rank 2):
+      * forming E = K^T F K takes two length-3 inner products per entry, so |dE| <= 6u |K^T| |F| |K|.  With the default
+        K (c_x, c_y <= f / 2) the entries of |K^T| |K^-T| and |K^-1| |K| are at most 2 and their 2-norms below 1.9,
+        and F = K^-T E K^-1, so || |K^T| |F| |K| ||_2 <= 1.9^2 ||E||_F <= 3.7 sqrt(2) sigma_1: ||dE|| <= 32u sigma_1;
+      * a backward-stable 3 x 3 SVD (LAPACK's, or a few sweeps of one-sided Jacobi, each rotation exact to a few u)
+        returns the exact SVD of E + dE' with ||dE'|| <= 16u sigma_1;
+      * R = U W V^T is the orthogonal factor of the rank-2 part of E, and t its left null vector: to first order both
+        move by at most 2 ||dE|| / sigma_2 (polar-factor and singular-subspace perturbation with the gap
+        sigma_2 - sigma_3 ~ sigma_2; the gap sigma_1 - sigma_2 does not enter, since R is the same for every
+        rotation of the leading singular pair);
+      * two independent decompositions differ by the sum: 2 * 2 (32 + 16) u sigma_1 / sigma_2 = 192 u sigma_1 / sigma_2
+        = 96 eps sigma_1 / sigma_2.
+    A decomposition through the normal matrix E^T E instead loses eps sigma_1^2 / sigma_2^2 (the eigenvector gap of
+    E^T E is sigma_2^2 while its rounding is eps sigma_1^2), which exceeds this bar once sigma_2 / sigma_1 <~ 1e-3."""
+    s = np.asarray(sigma, np.float64)
+    return POSE_BAR_C * EPS * s[0] / s[1] if s[1] > 0 else np.inf
+
+
+def random_rotation(rng):
+    Q, Rr = np.linalg.qr(rng.normal(size=(3, 3)))
+    Q = Q * np.sign(np.diag(Rr))
+    return Q if np.linalg.det(Q) > 0 else -Q
+
+
+def fundamental_with_singular_values(sigma, width, height, rng):
+    """F = K^-T E K^-1 for E = U diag(sigma) V^T with random rotations U, V and the default K of (width, height).
+    -> (F [3,3], E [3,3], U, V).  sigma = (1, r, 0) plants an E whose second singular value is r."""
+    U, V = random_rotation(rng), random_rotation(rng)
+    E = U @ np.diag(np.asarray(sigma, np.float64)) @ V.T
+    Ki = np.linalg.inv(default_kmat(width, height))
+    return Ki.T @ E @ Ki, E, U, V

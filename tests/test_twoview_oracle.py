@@ -157,6 +157,118 @@ def test_einval_before_launch():
     assert L.vgg_twoview_workspace_bytes(400, 4096, 4096, 300, ctypes.byref(nb)) == 0 and nb.value < 200 * 2 ** 20
 
 
+_W = np.array([[0.0, -1.0, 0.0], [1.0, 0.0, 0.0], [0.0, 0.0, 1.0]])
+
+
+def _pinned_candidates(U, V):
+    """The four (R, t) of decompose_essential_matrix from rotations U, V, with its orientation pin."""
+    t = U[:, 2]
+    if t[np.argmax(np.abs(t))] < 0:
+        P = np.array([-1.0, 1.0, -1.0])
+        U, V = U * P, V * P
+    R1, R2, T = U @ _W @ V.T, U @ _W.T @ V.T, U[:, 2]
+    return np.stack([R1, R1, R2, R2]), np.stack([T, -T, T, -T])
+
+
+def _normal_matrix_route(E):
+    """Float64 restatement of the decomposition through E^T E that tv_pose_kernel used before it moved to one-sided
+    Jacobi: V = eigenvectors of E^T E (descending), u_i = E v_i / |E v_i|, u1 re-orthogonalised, u2 = u0 x u1."""
+    w, Wv = np.linalg.eigh(E.T @ E)
+    V = Wv[:, np.argsort(-w, kind="stable")]
+    u0, u1 = (E @ V[:, i] for i in range(2))
+    u0, u1 = u0 / np.linalg.norm(u0), u1 / np.linalg.norm(u1)
+    u1 = u1 - (u0 @ u1) * u0
+    u1 = u1 / np.linalg.norm(u1)
+    if np.linalg.det(V) < 0:
+        V[:, 2] = -V[:, 2]
+    return _pinned_candidates(np.stack([u0, u1, np.cross(u0, u1)], 1), V)
+
+
+@pytest.mark.parametrize("r", [1.0, 1 - 1e-12, 1e-2, 1e-4, 1e-6, 1e-8])
+def test_singular_value_generator_plants_what_it_claims(r):
+    rng = np.random.default_rng(int(-np.log10(r)) if r < 1 else 99)
+    for width, height in ((1024, 1024), (1920, 1080), (480, 640)):
+        F, E, U, V = tvo.fundamental_with_singular_values((1.0, r, 0.0), width, height, rng)
+        assert np.linalg.det(U) > 0 and np.linalg.det(V) > 0
+        assert np.abs(U.T @ U - np.eye(3)).max() < 1e-15 and np.abs(V.T @ V - np.eye(3)).max() < 1e-15
+        K = tvo.default_kmat(width, height)
+        Ek = K.T @ F @ K
+        assert np.abs(Ek - E).max() < 1e-13
+        s = np.linalg.svd(Ek, compute_uv=False)
+        assert abs(s[0] - 1) < 1e-14 and abs(s[1] - r) < 1e-14 and s[2] < 1e-14
+        Rs, ts = _pinned_candidates(U, V)
+        for R in Rs:
+            assert np.abs(R.T @ R - np.eye(3)).max() < 1e-14 and abs(np.linalg.det(R) - 1) < 1e-14
+        assert np.abs(Ek.T @ ts[0]).max() < 1e-14            # t spans the left null space
+
+
+@pytest.mark.parametrize("r", [1.0, 1 - 1e-12, 1e-2, 1e-4, 1e-6, 1e-8])
+def test_pose_bar_passes_lapack_and_rejects_the_normal_matrix_route(r):
+    """LAPACK's decomposition of K^T F K stays inside pose_bar around the planted candidates (all four, in order: the
+    determinant fixes and the orientation pin make the order canonical); the E^T E route of the old kernel leaves it
+    at sigma_2 / sigma_1 <= 1e-4 on every draw."""
+    rng = np.random.default_rng(7)
+    worst_lapack, best_normal = 0.0, np.inf
+    for _ in range(12):
+        F, E, U, V = tvo.fundamental_with_singular_values((1.0, r, 0.0), 1024, 768, rng)
+        K = tvo.default_kmat(1024, 768)
+        Ek = K.T @ F @ K
+        bar = tvo.pose_bar(np.linalg.svd(Ek, compute_uv=False))
+        Rp, tp = _pinned_candidates(U, V)
+        Rs, ts = tvo.decompose_essential_matrix(Ek[None])
+        worst_lapack = max(worst_lapack, max(np.abs(Rs[0] - Rp).max(), np.abs(ts[0] - tp).max()) / bar)
+        Rn, tn = _normal_matrix_route(Ek)
+        best_normal = min(best_normal, max(np.abs(Rn - Rp).max(), np.abs(tn - tp).max()) / bar)
+    assert worst_lapack <= 0.25, worst_lapack
+    if r <= 1e-4:
+        assert best_normal > 1.0, best_normal
+
+
+def test_pose_bar_is_inf_at_rank_one():
+    assert tvo.pose_bar([1.0, 0.0, 0.0]) == np.inf
+    assert tvo.pose_bar([2.0, 1e-3, 0.0]) == pytest.approx(96 * 2.0 ** -52 * 2e3)
+
+
+def test_lapack_basis_of_rank_deficient_e():
+    """What the oracle decomposes F = 0 and a rank-1 F into: F = 0 gives U = V = I, so R = W, W^T and t = e2; a rank-1
+    E = a b^T gives rotations with t orthogonal to a (LAPACK's completion of the basis, not unique)."""
+    Rs, ts = tvo.decompose_essential_matrix(np.zeros((1, 3, 3)))
+    assert np.array_equal(Rs[0, 0], _W) and np.array_equal(Rs[0, 2], _W.T) and np.array_equal(ts[0, 0], [0, 0, 1])
+    a, b = np.array([0.3, -0.5, 0.8]), np.array([1.0, 0.2, -0.4])
+    Rs, ts = tvo.decompose_essential_matrix(np.outer(a, b)[None])
+    for R in Rs[0]:
+        assert np.isfinite(R).all() and np.abs(R.T @ R - np.eye(3)).max() < 1e-14 and abs(np.linalg.det(R) - 1) < 1e-14
+    assert abs(ts[0, 0] @ a) < 1e-14 and abs(np.linalg.norm(ts[0, 0]) - 1) < 1e-14
+
+
+def test_cheirality_margin_fields_on_a_hand_built_pair():
+    """R = I, t = (1, 0, 0): window 1000.  Points at depth 2, 500 and 999.5 -> margins 0.998, 0.5, 5e-4; a point
+    behind both cameras at -3 is not counted and its margin is (3 + eps32) / 1000 + 1 against the window, far larger."""
+    R, t = np.eye(3), np.array([1.0, 0.0, 0.0])
+    X = np.array([[0.1, 0.2, 2.0], [0.5, -0.3, 500.0], [1.0, 1.0, 999.5], [0.2, 0.1, -3.0]])
+    Y = X @ R.T + t
+    x1, x2 = X[:, :2] / X[:, 2:], Y[:, :2] / Y[:, 2:]
+    for n, want_cnt, want_margin in ((1, 1, 0.998), (2, 2, 0.5), (3, 3, 5e-4), (4, 3, 5e-4)):
+        cnt, margin = tvo.cheirality_counts(R, t, x1[:n], x2[:n], return_margin=True)
+        assert cnt == want_cnt and margin == pytest.approx(want_margin, rel=1e-9), (n, cnt, margin)
+    assert tvo.cheirality_counts(R, t, x1, x2) == 3
+    # the relative pose of the same pair in pixels: the winner has every point in front, count_gap against the others
+    f, w, h = 1000.0, 1000, 800
+    K = tvo.default_kmat(w, h)
+    Ki = np.linalg.inv(K)
+    tx = np.array([[0, -t[2], t[1]], [t[2], 0, -t[0]], [-t[1], t[0], 0]])
+    F = (Ki.T @ tx @ R @ Ki)[None]
+    p1 = (x1 * f + [w / 2, h / 2])[None]
+    p2 = (x2 * f + [w / 2, h / 2])[None]
+    Rr, tr, _, counts, dbg = tvo.relative_pose(F, p1, p2, w, h, return_debug=True)
+    d = dbg[0]
+    assert d["k"] == int(np.argmax(counts[0])) and counts[0, d["k"]] == 3
+    assert np.abs(Rr[0] - np.eye(3)).max() < 1e-12 and np.abs(tr[0] - t).max() < 1e-12
+    others = [counts[0, j] for j in range(4) if j != d["k"]]
+    assert d["count_gap"] == 3 - max(others)
+    assert d["depth_margin"] <= 5e-4 * (1 + 1e-9) and np.allclose(d["sigma"], [1, 1, 0], atol=1e-12)
+
+
 def test_mirror_refuses_cpu_tensors():
     import torch
     from vggsfm_b200 import two_view as tv

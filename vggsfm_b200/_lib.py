@@ -32,7 +32,7 @@ EXPORTS = [
 
 # development probes (csrc/dev_probes.h): exported, not part of the public header
 DEV_EXPORTS = ["vgg_dev_blocks_timing", "vgg_dev_blocks_last_ms", "vgg_dev_chol128_probe", "vgg_dev_syrk_f64", "vgg_dev_syrk_f64_band", "vgg_dev_syrk_ozaki_band", "vgg_dev_trsv_probe", "vgg_dev_cholesky_band",
-               "vgg_dev_last_band_hint", "vgg_dev_msac_trace"]
+               "vgg_dev_last_band_hint", "vgg_dev_msac_trace", "vgg_dev_relative_pose_counts"]
 
 
 class BAProblem(ctypes.Structure):
@@ -175,6 +175,7 @@ def lib() -> ctypes.CDLL:
     L.vgg_estimate_fundamental.argtypes = [ci, ci, vp, vp, ci, vp, vp, ci, ci, cd, ci, ci, vp, vp, vp, vp, vp, cs, vp]
     L.vgg_fundamental_inliers.argtypes = [ci, ci, vp, vp, ci, vp, cd, ci, vp, vp]
     L.vgg_relative_pose_from_fundamental.argtypes = [ci, ci, vp, vp, ci, vp, cd, cd, vp, vp, vp, vp]
+    L.vgg_dev_relative_pose_counts.argtypes = [ci, ci, vp, vp, ci, vp, cd, cd, vp, vp, vp, vp, vp]
     cu64 = ctypes.c_ulonglong
     L.vgg_msac_fundamental_workspace_bytes.argtypes = [ci, ci, ci, ci, ctypes.POINTER(cs)]
     L.vgg_estimate_fundamental_msac.argtypes = [ci, ci, vp, vp, ci, vp, cd, ci, ci, cu64, vp, vp, vp, vp, vp, cs, vp]

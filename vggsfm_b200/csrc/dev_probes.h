@@ -46,6 +46,11 @@ int vgg_dev_cholesky_band(int n, int lda, double* A, void* workspace, size_t ws_
  * first min(cap, 64) of those trials in order (-1 padded), all host arrays. */
 int vgg_dev_msac_trace(int B, int N, int max_iterations, int min_iterations, const void* workspace, int cap,
                        int32_t* lo_runs_host, int32_t* win_trial_host, int32_t* lo_trials_host);
+/* vgg_relative_pose_from_fundamental that also writes the cheirality vote: counts_dev[4 b + k] = points in front of both
+ * cameras inside the depth window for candidate k (R1 t, R1 -t, R2 t, R2 -t) of pair b (device int32 [B, 4]). */
+int vgg_dev_relative_pose_counts(int B, int N, const void* points1, const void* points2, int points_are_f64,
+                                 const double* fmat, double width, double height, double* R_out, double* t_out,
+                                 double* E_out, int32_t* counts_dev, void* stream);
 
 #ifdef __cplusplus
 }

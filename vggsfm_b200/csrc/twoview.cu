@@ -19,6 +19,7 @@
 #include <float.h>
 #include <math.h>
 #include "common.cuh"
+#include "dev_probes.h"
 #include "twoview_geom.h"
 
 namespace vgg {
@@ -444,34 +445,86 @@ __device__ __forceinline__ void cross3(const double* a, const double* b, double*
   o[2] = a[0] * b[1] - a[1] * b[0];
 }
 
-// 3x3 SVD of E by Jacobi on E^T E; U, V row-major with singular vectors in the columns, descending order.  The third
-// left vector is u0 x u1 (E has rank <= 2); the determinant fixes of the reference are then no-ops for U.
+// One-sided (Hestenes) Jacobi on the m x n row-major A: plane rotations V make the columns of A V mutually orthogonal
+// (to 4 eps relative), and A is overwritten by A V.  Working on A itself rather than on A^T A keeps the singular
+// vectors accurate to about eps sigma_1 / gap instead of eps (sigma_1 / gap)^2.  A pair whose columns are already
+// orthogonal, zero or not finite is left alone.
+template <int m, int n>
+__device__ void jacobi_svd(double* A, double* V) {
+#pragma unroll
+  for (int i = 0; i < n * n; ++i) V[i] = (i % (n + 1) == 0) ? 1.0 : 0.0;
+  for (int sweep = 0; sweep < 30; ++sweep) {
+    bool rotated = false;
+#pragma unroll
+    for (int p = 0; p < n; ++p)
+#pragma unroll
+      for (int q = p + 1; q < n; ++q) {
+        double al = 0.0, be = 0.0, ga = 0.0;
+#pragma unroll
+        for (int k = 0; k < m; ++k) {
+          al += A[k * n + p] * A[k * n + p];
+          be += A[k * n + q] * A[k * n + q];
+          ga += A[k * n + p] * A[k * n + q];
+        }
+        if (!(fabs(ga) > 4.0 * DBL_EPSILON * sqrt(al) * sqrt(be))) continue;
+        const double zeta = (be - al) / (2.0 * ga);
+        const double t = fabs(zeta) > 1e150 ? 0.5 / zeta
+                                             : (zeta >= 0.0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+        const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
+#pragma unroll
+        for (int k = 0; k < m; ++k) {
+          const double ap = A[k * n + p], aq = A[k * n + q];
+          A[k * n + p] = c * ap - s * aq;
+          A[k * n + q] = s * ap + c * aq;
+        }
+#pragma unroll
+        for (int k = 0; k < n; ++k) {
+          const double vp = V[k * n + p], vq = V[k * n + q];
+          V[k * n + p] = c * vp - s * vq;
+          V[k * n + q] = s * vp + c * vq;
+        }
+        rotated = true;
+      }
+    if (!rotated) break;
+  }
+}
+
+// 3x3 SVD of E by one-sided Jacobi; U, V row-major with singular vectors in the columns, descending order.  The third
+// left vector is u0 x u1 (E has rank <= 2); the determinant fixes of the reference are then no-ops for U.  Where
+// E v_i vanishes (rank <= 1, E = 0) the left vectors are completed to an orthonormal basis: u0 = e0 when E = 0, u1
+// from the coordinate axis least aligned with u0 (E = 0 then gives U = V = I, as LAPACK does).
 __device__ void svd3(const double* E, double* U, double* V) {
-  double A[9], W[9], w[3];
-  for (int r = 0; r < 3; ++r)
-    for (int q = 0; q < 3; ++q) A[r * 3 + q] = E[r] * E[q] + E[3 + r] * E[3 + q] + E[6 + r] * E[6 + q];
-  jacobi_eig<3>(A, W, w);
+  double A[9], nrm[3];
+  for (int i = 0; i < 9; ++i) A[i] = E[i];
+  jacobi_svd<3, 3>(A, V);
+  for (int i = 0; i < 3; ++i) nrm[i] = sqrt(A[i] * A[i] + A[3 + i] * A[3 + i] + A[6 + i] * A[6 + i]);
   int o[3] = {0, 1, 2};
   for (int i = 0; i < 3; ++i)
     for (int k = i + 1; k < 3; ++k)
-      if (w[o[k]] > w[o[i]]) { const int t = o[i]; o[i] = o[k]; o[k] = t; }
+      if (nrm[o[k]] > nrm[o[i]]) { const int t = o[i]; o[i] = o[k]; o[k] = t; }
+  double W[9];
+  for (int i = 0; i < 9; ++i) W[i] = V[i];
   for (int i = 0; i < 3; ++i)
     for (int r = 0; r < 3; ++r) V[r * 3 + i] = W[r * 3 + o[i]];
   double u[3][3];
-  for (int i = 0; i < 2; ++i) {
-    double nn = 0.0;
-    for (int r = 0; r < 3; ++r) {
-      u[i][r] = E[r * 3] * V[i] + E[r * 3 + 1] * V[3 + i] + E[r * 3 + 2] * V[6 + i];
-      nn += u[i][r] * u[i][r];
-    }
+  for (int i = 0; i < 2; ++i)
+    for (int r = 0; r < 3; ++r) u[i][r] = nrm[o[i]] != 0.0 ? A[r * 3 + o[i]] / nrm[o[i]] : 0.0;   // NaN stays NaN
+  if (nrm[o[0]] == 0.0) { u[0][0] = 1.0; u[0][1] = 0.0; u[0][2] = 0.0; }
+  // re-orthogonalise u1 against u0 (equal singular values of an essential matrix), or complete it
+  for (int pass = 0; pass < 2; ++pass) {
+    double dp = u[0][0] * u[1][0] + u[0][1] * u[1][1] + u[0][2] * u[1][2], nn = 0.0;
+    for (int r = 0; r < 3; ++r) { u[1][r] -= dp * u[0][r]; nn += u[1][r] * u[1][r]; }
     nn = sqrt(nn);
-    for (int r = 0; r < 3; ++r) u[i][r] /= nn;
+    if (pass == 0 && nn <= 0.5) {              // E v1 vanished (or lay along u0): the axis least aligned with u0
+      int k = 0;
+      for (int r = 1; r < 3; ++r)
+        if (fabs(u[0][r]) < fabs(u[0][k])) k = r;
+      for (int r = 0; r < 3; ++r) u[1][r] = r == k ? 1.0 : 0.0;
+      continue;
+    }
+    for (int r = 0; r < 3; ++r) u[1][r] /= nn;
+    break;
   }
-  // re-orthogonalise u1 against u0 (equal singular values of an essential matrix)
-  double dp = u[0][0] * u[1][0] + u[0][1] * u[1][1] + u[0][2] * u[1][2], nn = 0.0;
-  for (int r = 0; r < 3; ++r) { u[1][r] -= dp * u[0][r]; nn += u[1][r] * u[1][r]; }
-  nn = sqrt(nn);
-  for (int r = 0; r < 3; ++r) u[1][r] /= nn;
   cross3(u[0], u[1], u[2]);
   for (int i = 0; i < 3; ++i)
     for (int r = 0; r < 3; ++r) U[r * 3 + i] = u[i][r];
@@ -481,7 +534,7 @@ template <typename TP>
 __global__ void __launch_bounds__(128) tv_pose_kernel(int N, double width, double height, const TP* __restrict__ p1,
                                                       const TP* __restrict__ p2, const double* __restrict__ fmat,
                                                       double* __restrict__ R_out, double* __restrict__ t_out,
-                                                      double* __restrict__ E_out) {
+                                                      double* __restrict__ E_out, int* __restrict__ counts_out) {
   __shared__ double Rs[4][9], ts[4][3], maxd[4];
   __shared__ double red[4 * 4];
   const int b = blockIdx.x, tid = threadIdx.x;
@@ -583,6 +636,8 @@ __global__ void __launch_bounds__(128) tv_pose_kernel(int N, double width, doubl
       if (cnt[k] > cnt[kb]) kb = k;
     for (int i = 0; i < 9; ++i) R_out[(size_t)b * 9 + i] = Rs[kb][i];
     for (int i = 0; i < 3; ++i) t_out[(size_t)b * 3 + i] = ts[kb][i];
+    if (counts_out)
+      for (int k = 0; k < 4; ++k) counts_out[(size_t)b * 4 + k] = (int)(cnt[k] + 0.5);
   }
 }
 
@@ -730,6 +785,13 @@ int vgg_fundamental_inliers(int B, int N, const void* points1, const void* point
 int vgg_relative_pose_from_fundamental(int B, int N, const void* points1, const void* points2, int points_are_f64,
                                        const double* fmat, double width, double height, double* R_out, double* t_out,
                                        double* E_out, void* stream) {
+  return vgg_dev_relative_pose_counts(B, N, points1, points2, points_are_f64, fmat, width, height, R_out, t_out, E_out,
+                                      nullptr, stream);
+}
+
+int vgg_dev_relative_pose_counts(int B, int N, const void* points1, const void* points2, int points_are_f64,
+                                 const double* fmat, double width, double height, double* R_out, double* t_out,
+                                 double* E_out, int32_t* counts_out, void* stream) {
   VGG_REQUIRE(B >= 0 && N >= 0 && width > 0 && height > 0, "bad arguments");
   g_launch_count = 0;
   if (B == 0) return VGG_OK;
@@ -737,10 +799,10 @@ int vgg_relative_pose_from_fundamental(int B, int N, const void* points1, const 
   cudaStream_t st = (cudaStream_t)stream;
   if (points_are_f64)
     tv_pose_kernel<double><<<B, 128, 0, st>>>(N, width, height, (const double*)points1, (const double*)points2, fmat,
-                                              R_out, t_out, E_out);
+                                              R_out, t_out, E_out, counts_out);
   else
     tv_pose_kernel<float><<<B, 128, 0, st>>>(N, width, height, (const float*)points1, (const float*)points2, fmat,
-                                             R_out, t_out, E_out);
+                                             R_out, t_out, E_out, counts_out);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
