@@ -87,24 +87,24 @@ typedef struct vgg_ba_summary {
 #define VGG_BA_FAILURE 5
 
 /* Sum/max all-reduce hook over track shards (one process per GPU).  `buf` is a device pointer
- * inside the caller's workspace; op 0 = sum, 1 = max, 2 = barrier across ranks on `stream` (buf NULL).
- * NULL = single GPU. */
+ * inside the caller's workspace; op 0 = sum, 1 = max, on `stream`.  NULL = single GPU. */
 typedef int (*vgg_allreduce_fn)(void* user, double* buf, size_t count, int op, void* stream);
 
-/* Fused reduction over NVLink/NVSwitch: the reduced camera system lives in symmetric (peer-mapped) memory and
- * every rank's assemble / Schur kernels add their contributions with multimem.red on the multicast address,
- * so the per-iteration all-reduce of [D x Dpad | rhs | diag | g] needs no separate collective.  ar_local and
- * ar_multicast address the same allocation (e.g. torch.distributed._symmetric_memory). */
+/* Fused reduction over NVLink/NVSwitch: the reduced camera system [D x Dpad | rhs | diag | g] lives in symmetric
+ * (peer-mapped) memory and is reduced by the kernels that produce it, so the LM loop needs no separate collective.
+ * ar_local and ar_multicast address the same allocation (e.g. torch.distributed._symmetric_memory); the assemble /
+ * Schur kernels add the small blocks with multimem.red on the multicast address.  The SYRK reduce-scatters the lower
+ * triangle's 128-row blocks onto their owners (block b -> rank b mod world) with system-scope REDs over NVLink, every
+ * rank gathers the others by peer loads, and the barriers and the small cost/gradient all-reduces are kernels on the
+ * same allocation -- no NCCL call, no host callback inside the LM loop, inbound traffic per GPU independent of the
+ * number of ranks, bit-identical systems on all ranks.  The all-reduce hook is not called. */
 typedef struct vgg_ba_fabric {
   double* ar_local;
   double* ar_multicast;
   size_t ar_doubles;     /* >= vgg_ba_reduced_system_doubles() */
-  /* v2 (optional; world = 0 keeps v1): reduce-scatter of the lower triangle's 128-row blocks onto their owners
-   * (block b -> rank b mod world) with system-scope REDs over NVLink, gather by peer loads, barriers and the small
-   * cost/gradient all-reduces as kernels on the same allocation -- no NCCL call, no host callback inside the LM loop,
-   * inbound traffic per GPU independent of the number of ranks, bit-identical systems on all ranks.
-   * peer_base[r] = rank r's base address of the SAME symmetric allocation (ar_local == peer_base[rank]), which must
-   * hold total_doubles >= vgg_ba_fabric_doubles() and be zero-filled once when it is created. */
+  /* world in 2..8, rank = this process.  peer_base[r] = rank r's base address of the SAME symmetric allocation
+   * (ar_local == peer_base[rank]), which must hold total_doubles >= vgg_ba_fabric_doubles() and be zero-filled once
+   * when it is created.  vgg_ba_solve_fabric returns VGG_EINVAL without them. */
   int32_t world, rank;
   double* peer_base[8];
   size_t total_doubles;

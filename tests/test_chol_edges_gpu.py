@@ -12,12 +12,9 @@ Cases: orders across the one-block / program-order / lookahead boundaries and ev
 failing pivots (negative, NaN, subnormal, +inf, two of them, both of a pair, in band and arrow) at every leaf position
 class of the first, a middle and the last block, each followed by a good matrix on the same buffer; graded scales whose
 pivot pairs leave the two-pivot range; ill-conditioned and nearly dependent pairs; the bordered matrix of the LM loop;
-NaN sentinels around the matrix and lda = n; the direct-launch schedule (VGG_CHOL_GRAPH=0, in a subprocess); the
-graph cache; band shapes.  Each case prints its backward-error ratio and worst ulp count."""
+NaN sentinels around the matrix and lda = n; the graph cache; band shapes.  Each case prints its backward-error ratio
+and worst ulp count."""
 import functools
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -28,7 +25,6 @@ pytestmark = pytest.mark.gpu
 
 ORDERS = [1, 2, 7, 8, 9, 31, 32, 33, 127, 128, 129, 255, 256, 257, 383, 384, 385, 2402, 2403]
 POSITIONS = [0, 1, 6, 7, 8, 9, 30, 31, 32, 33, 126, 127]
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _r128(n):
@@ -309,7 +305,7 @@ def _band_case():
     return co.band_arrow(12, 2, 77, 5)
 
 
-def representative_set():
+def test_representative_set_graph(cuda_dev):
     """257 (program order), 2403, 4500 (second wave) and a band + arrow matrix under bars 1 and 2, with a failure and
     a recovery on each buffer"""
     for n in (257, 2403, 4500):
@@ -320,25 +316,11 @@ def representative_set():
         assert s.factor(bad)[0] == n - 2
         info, full = s.factor(A)
         assert info == 0
-        check(f"schedule VGG_CHOL_GRAPH={os.environ.get('VGG_CHOL_GRAPH', '1')}", A, full)
+        check("schedule", A, full)
     A, keep, end, arrow = _band_case()
     info, full = Slot(len(A)).factor(A, band=(end, arrow))
     assert info == 0
-    check(f"schedule band+arrow VGG_CHOL_GRAPH={os.environ.get('VGG_CHOL_GRAPH', '1')}", A, full)
-
-
-def test_representative_set_graph(cuda_dev):
-    representative_set()
-
-
-def test_representative_set_direct_launch(cuda_dev):
-    """VGG_CHOL_GRAPH=0 is read once per process: the direct-launch schedule runs in a child process"""
-    env = dict(os.environ, VGG_CHOL_GRAPH="0")
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
-        "-c", "import torch; from tests.test_chol_edges_gpu import representative_set as r; r(); print('direct-launch ok')"]
-    p = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=900)
-    print(p.stdout[-4000:])
-    assert p.returncode == 0 and "direct-launch ok" in p.stdout, p.stderr[-4000:]
+    check("schedule band+arrow", A, full)
 
 
 def test_graph_cache_eviction_and_reuse(cuda_dev):

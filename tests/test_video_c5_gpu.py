@@ -27,16 +27,15 @@ def test_band_hint_does_not_change_the_joint_ba(cuda_dev):
     import video_c5
     from vggsfm_b200 import video
     res = {}
-    for band in ("0", "2", "1"):          # dense / SYRK + Cholesky hint only / + ba_blocks, z_build, backsub skips
+    for band in ("0", "1"):               # dense / SYRK, Cholesky, ba_blocks, z_build and backsub skips
         os.environ["VGG_BAND"] = band
         try:
             out = video_c5.final_problem(frames=320, new_per_window=128, dev=cuda_dev, reps=1)
             res[band] = (out["lm_iterations"][0], float(video.last_joint_summary.final_cost))
         finally:
             os.environ.pop("VGG_BAND", None)
-    for band in ("2", "1"):
-        assert res["0"][0] > 5 and res[band][0] > 5
-        assert abs(res["0"][1] - res[band][1]) <= 1e-9 * abs(res["0"][1]), band
+    assert res["0"][0] > 5 and res["1"][0] > 5
+    assert abs(res["0"][1] - res["1"][1]) <= 1e-9 * abs(res["0"][1])
 
 
 def test_band_detection_is_safe_for_unordered_points(cuda_dev):

@@ -6,7 +6,6 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
-#include <functional>
 #include <map>
 #include <vector>
 #include "common.cuh"
@@ -184,7 +183,7 @@ static int make_layout(int S, int N, int model, int mode, void* base, size_t cap
   }
   L->S = S; L->N = N; L->dc = dc; L->ns = ns; L->KR = KR;
   L->D = S * dc + ns;
-  L->Dpad = (int)align_up((size_t)L->D + 2, 128);      // >= 2 spare slots after D (fabric-mode scalar sync)
+  L->Dpad = (int)align_up((size_t)L->D + 2, 128);      // >= 2 spare slots after D (row D: the bordered right-hand side)
   L->Kpad = (int)align_up((size_t)3 * N, 16);
   Carver c(base, cap);
   for (int b = 0; b < 2; ++b) {
@@ -229,7 +228,7 @@ static cublasHandle_t get_cublas() {
   return h;
 }
 
-// Layout of the symmetric allocation of fabric v2 (doubles): two copies of the reduced system (iteration parity, so a
+// Layout of the symmetric allocation of the fabric (doubles): two copies of the reduced system (iteration parity, so a
 // rank may zero the next copy while a slow peer still pulls from the previous one), the mailboxes of the small
 // all-reduce (2 parities x 8 source ranks), one row of 64-bit barrier flags.
 struct FabricLayout {
@@ -246,9 +245,9 @@ static FabricLayout fabric_layout(int D, int Dpad) {
   return f;
 }
 
-// Run-time state of fabric v2 (csrc/fabric.cu): reduce-scatter + gather of the reduced system, in-kernel barriers and
+// Run-time state of the fabric (csrc/fabric.cu): reduce-scatter + gather of the reduced system, in-kernel barriers and
 // small all-reduces -- no NCCL call and no host callback inside the LM loop.
-struct Fabric2 {
+struct Fabric {
   bool on = false;
   FabricDev base{};                 // peer[r] = base of rank r's symmetric allocation
   FabricLayout lay{};
@@ -388,57 +387,55 @@ static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad
       }
       plan->end_blk = end;
       plan->arrow_blk = arrow;
-      // device tables for the kernels that walk the dense [frames, points] grid (VGG_BAND=2: SYRK/Cholesky hint only)
-      if (!(env && env[0] == '2')) {
-        const int ngroups = (S + 31) / 32;
-        std::vector<int> tab(2 * (size_t)(nb + KB + ngroups), 0);
-        int* t_rb = tab.data();
-        int* t_kb = t_rb + 2 * nb;
-        int* t_fg = t_kb + 2 * KB;
-        for (int i = 0; i < 2 * nb; ++i) t_rb[i] = rg[i];
-        for (int kb = 0; kb < KB; ++kb) {
-          int first = -1, last = -1;
-          for (int rb = 0; rb < arrow; ++rb)
-            if (rg[2 * rb] <= kb && kb < rg[2 * rb + 1]) {
-              if (first < 0) first = rb;
-              last = rb;
-            }
-          t_kb[2 * kb] = first < 0 ? 0 : first * 128;
-          t_kb[2 * kb + 1] = first < 0 ? 0 : (last + 1) * 128;
-        }
-        for (int g = 0; g < ngroups; ++g) {
-          int lo = N, hi = 0;
-          for (int f = 32 * g; f < std::min(S, 32 * g + 32); ++f) {
-            if (fr[2 * f + 1] < 0) continue;
-            lo = std::min(lo, fr[2 * f]);
-            hi = std::max(hi, fr[2 * f + 1] + 1);
+      // device tables for the kernels that walk the dense [frames, points] grid
+      const int ngroups = (S + 31) / 32;
+      std::vector<int> tab(2 * (size_t)(nb + KB + ngroups), 0);
+      int* t_rb = tab.data();
+      int* t_kb = t_rb + 2 * nb;
+      int* t_fg = t_kb + 2 * KB;
+      for (int i = 0; i < 2 * nb; ++i) t_rb[i] = rg[i];
+      for (int kb = 0; kb < KB; ++kb) {
+        int first = -1, last = -1;
+        for (int rb = 0; rb < arrow; ++rb)
+          if (rg[2 * rb] <= kb && kb < rg[2 * rb + 1]) {
+            if (first < 0) first = rb;
+            last = rb;
           }
-          t_fg[2 * g] = hi > lo ? lo : 0;
-          t_fg[2 * g + 1] = hi > lo ? hi : 0;
-        }
-        static thread_local int* tdev = nullptr;
-        static thread_local size_t tcap = 0;
-        if (tcap < tab.size()) {
-          if (tdev) cudaFree(tdev);
-          VGG_CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&tdev), sizeof(int) * tab.size()));
-          tcap = tab.size();
-        }
-        VGG_CUDA_CHECK(cudaMemcpyAsync(tdev, tab.data(), sizeof(int) * tab.size(), cudaMemcpyHostToDevice, st));
-        VGG_CUDA_CHECK(cudaStreamSynchronize(st));           // pageable source
-        plan->dev = BandDev{tdev, tdev + 2 * nb, tdev + 2 * (nb + KB), arrow * 128};
-        plan->kb_rows.assign(t_kb, t_kb + 2 * KB);
-        plan->fg_tracks.assign(t_fg, t_fg + 2 * ngroups);
+        t_kb[2 * kb] = first < 0 ? 0 : first * 128;
+        t_kb[2 * kb + 1] = first < 0 ? 0 : (last + 1) * 128;
       }
+      for (int g = 0; g < ngroups; ++g) {
+        int lo = N, hi = 0;
+        for (int f = 32 * g; f < std::min(S, 32 * g + 32); ++f) {
+          if (fr[2 * f + 1] < 0) continue;
+          lo = std::min(lo, fr[2 * f]);
+          hi = std::max(hi, fr[2 * f + 1] + 1);
+        }
+        t_fg[2 * g] = hi > lo ? lo : 0;
+        t_fg[2 * g + 1] = hi > lo ? hi : 0;
+      }
+      static thread_local int* tdev = nullptr;
+      static thread_local size_t tcap = 0;
+      if (tcap < tab.size()) {
+        if (tdev) cudaFree(tdev);
+        VGG_CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&tdev), sizeof(int) * tab.size()));
+        tcap = tab.size();
+      }
+      VGG_CUDA_CHECK(cudaMemcpyAsync(tdev, tab.data(), sizeof(int) * tab.size(), cudaMemcpyHostToDevice, st));
+      VGG_CUDA_CHECK(cudaStreamSynchronize(st));           // pageable source
+      plan->dev = BandDev{tdev, tdev + 2 * nb, tdev + 2 * (nb + KB), arrow * 128};
+      plan->kb_rows.assign(t_kb, t_kb + 2 * KB);
+      plan->fg_tracks.assign(t_fg, t_fg + 2 * ngroups);
     }
   }
   return VGG_OK;
 }
 
 // Schur complement of blk onto AR (Sraw, rhs, hdiag, gvec) at the given radius; fd: where the SYRK epilogue sends each
-// row block in a fabric v2 solve
+// row block in a fabric solve, fab: that solve's fabric (null otherwise)
 static int schur_build(const Layout& L, const BlockSet& b, const BandPlan& band, const FabricDev& fd,
                        const uint8_t* point_const, double radius, double min_diag, double max_diag, cudaStream_t st,
-                       ptrdiff_t mc_off = 0, const std::function<int()>* barrier = nullptr) {
+                       ptrdiff_t mc_off = 0, Fabric* fab = nullptr) {
   int rc;
   double* Sraw = L.AR;
   double* rhs = L.AR + (size_t)L.D * L.Dpad;
@@ -448,13 +445,13 @@ static int schur_build(const Layout& L, const BlockSet& b, const BandPlan& band,
                               L.scal, st)))
     return rc;
   VGG_CUDA_CHECK(cudaMemsetAsync(L.AR, 0, sizeof(double) * ((size_t)L.D * L.Dpad + 3 * (size_t)L.Dpad), st));
-  // fabric mode: every rank's copy must be zero before anyone's multimem reductions land in it
-  if (mc_off && barrier && (rc = (*barrier)())) return rc;
+  // fabric mode: every rank's copy must be zero before anyone's reductions land in it
+  if (fab && (rc = fab->barrier(st))) return rc;
   if ((rc = launch_assemble_hc(L.S, L.dc, L.ns, L.KR, L.Dpad, b.camrec, b.shared, Sraw, rhs, hdiag, gvec, mc_off, st))) return rc;
   if ((rc = launch_z_transpose(L.D, L.N, L.Dpad, b.W, L.M, L.q, L.Zt, rhs, mc_off, band.dev.rb_range, st))) return rc;
   if ((rc = launch_syrk(L.Kpad, L.Dpad, L.Zt, Sraw, mc_off, band.kb_ranges, fd, st))) return rc;
   // ... and all reductions must have landed before anyone reads its copy
-  if (mc_off && barrier && (rc = (*barrier)())) return rc;
+  if (fab && (rc = fab->barrier(st))) return rc;
   return VGG_OK;
 }
 
@@ -614,30 +611,26 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
   int rc = make_layout(S, N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L);
   if (rc) return rc;
   const size_t ar_count = (size_t)D * L.Dpad + 3 * (size_t)L.Dpad;
-  // fabric mode: the reduced system lives in symmetric (peer-mapped) memory and is reduced by multimem operations
-  // issued from the producing kernels; mc_off is the distance from a local address to its multicast twin
+  // fabric mode: the reduced system lives in symmetric (peer-mapped) memory and is reduced by the producing kernels
+  // (multimem operations for the small blocks, the SYRK's reduce-scatter for the rest); mc_off is the distance from a
+  // local address to its multicast twin
   ptrdiff_t mc_off = 0;
-  Fabric2 fab2;
+  Fabric fab;
   static thread_local std::map<const double*, unsigned long long> fabric_epochs;
   if (fabric && fabric->ar_local && fabric->ar_multicast) {
     VGG_REQUIRE(fabric->ar_doubles >= ar_count, "fabric buffer too small (vgg_ba_reduced_system_doubles)");
+    const FabricLayout lay = fabric_layout(D, L.Dpad);
+    VGG_REQUIRE(fabric->world > 1 && fabric->world <= 8 && fabric->peer_base[0] && fabric->total_doubles >= lay.total,
+                "fabric needs its peer table: world in 2..8, peer_base set, total_doubles >= vgg_ba_fabric_doubles");
     L.AR = fabric->ar_local;
     mc_off = fabric->ar_multicast - fabric->ar_local;
-    // v2 (default when the caller passed the peer table): VGG_FABRIC=1 keeps v1 (multimem all-reduce into every copy,
-    // barriers and small all-reduces through the host hook) for A/B
-    static const bool want_v2 = [] { const char* e = getenv("VGG_FABRIC"); return !(e && e[0] == '1'); }();
-    const FabricLayout lay = fabric_layout(D, L.Dpad);
-    if (want_v2 && fabric->world > 1 && fabric->world <= 8 && fabric->peer_base[0] && fabric->total_doubles >= lay.total) {
-      fab2.on = true;
-      fab2.lay = lay;
-      fab2.base.world = fabric->world;
-      fab2.base.rank = fabric->rank;
-      for (int r = 0; r < fabric->world; ++r) fab2.base.peer[r] = fabric->peer_base[r];
-      fab2.epoch = &fabric_epochs[fabric->peer_base[fabric->rank]];
-      fab2.err = L.dev_info + 2;
-    } else {
-      VGG_REQUIRE(allreduce, "fabric v1 needs the hook for its barrier (op 2)");
-    }
+    fab.on = true;
+    fab.lay = lay;
+    fab.base.world = fabric->world;
+    fab.base.rank = fabric->rank;
+    for (int r = 0; r < fabric->world; ++r) fab.base.peer[r] = fabric->peer_base[r];
+    fab.epoch = &fabric_epochs[fabric->peer_base[fabric->rank]];
+    fab.err = L.dev_info + 2;
   }
   BandPlan band;
   if ((rc = compute_band_hint(prob, dc, D, L.Dpad, L.Kpad, allreduce != nullptr || fabric != nullptr, st, &band))) return rc;
@@ -652,13 +645,9 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
   double* rhs = L.AR + (size_t)D * L.Dpad;
   double* hdiag = rhs + L.Dpad;
   double* gvec = hdiag + L.Dpad;
-  const std::function<int()> barrier_fn = [&]() -> int {
-    if (fab2.on) return fab2.barrier(st);
-    return allreduce(ar_user, nullptr, 0, 2, st);
-  };
   // sum (and one max slot) of a small vector over the ranks: in-kernel over the fabric, else through the host hook
   auto reduce_small = [&](double* vec, size_t count, int op) -> int {
-    if (fab2.on) return fab2.allreduce(vec, (int)count, op == 1 ? 0 : -1, st);
+    if (fab.on) return fab.allreduce(vec, (int)count, op == 1 ? 0 : -1, st);
     if (allreduce) return allreduce(ar_user, vec, count, op, st);
     return VGG_OK;
   };
@@ -746,21 +735,21 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     const int cand = cur ^ 1;
     VGG_CUDA_CHECK(cudaMemsetAsync(L.scal, 0, sizeof(double) * 16, st));
     FabricDev fd{};
-    if (fab2.on) {
+    if (fab.on) {
       // this iteration's copy of the reduced system (parity) and where the SYRK epilogue sends each row block
-      const size_t off = (size_t)(it & 1) * fab2.lay.arc;
+      const size_t off = (size_t)(it & 1) * fab.lay.arc;
       L.AR = fabric->ar_local + off;
       Sraw = L.AR;
       rhs = L.AR + (size_t)D * L.Dpad;
       hdiag = rhs + L.Dpad;
       gvec = hdiag + L.Dpad;
-      fd = fab2.at(off);
+      fd = fab.at(off);
     }
     if ((rc = schur_build(L, L.blk[cur], band, fd, prob->point_const, radius, opt.min_lm_diagonal, opt.max_lm_diagonal, st,
-                          mc_off, (fab2.on || allreduce) ? &barrier_fn : nullptr)))
+                          mc_off, fab.on ? &fab : nullptr)))
       return rc;
     // every row block is complete on its owner: pull the others (matrix rows 0..D incl. the rhs row, then hdiag, gvec)
-    if (fab2.on && (rc = launch_fabric_gather(fd, D + 3, D + 1, D, L.Dpad, st))) return rc;
+    if (fab.on && (rc = launch_fabric_gather(fd, D + 3, D + 1, D, L.Dpad, st))) return rc;
     if (allreduce && !mc_off && (rc = allreduce(ar_user, L.AR, ar_count, 0, st))) return rc;
     if (!have_scale_c) {
       if ((rc = launch_jacobi_scale_cams(D, hdiag, L.sc_c, opt.jacobi_scaling, st))) return rc;
@@ -801,15 +790,6 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     if ((rc = launch_cam_step(D, dcs, dcs_stride, L.sc_c, hdiag, gvec, prob->param_const, radius, opt.min_lm_diagonal,
                               opt.max_lm_diagonal, L.d_c, L.scal, st)))
       return rc;
-    if (mc_off && !fab2.on) {
-      // Fabric v1: the multimem reductions reach each rank's copy in a different order, so the copies (and with
-      // them the factorisation and the camera step) differ in the last bits.  Keep the replicated camera state
-      // and the accept/reject scalars bit-identical on every rank: element-wise MAX over ranks of
-      // [d_c | quad_c | |d_c|^2] (one 19 KB collective; any rank-consistent choice within rounding would do).
-      VGG_CUDA_CHECK(cudaMemcpyAsync(L.d_c + L.Dpad - 2, L.scal, sizeof(double) * 2, cudaMemcpyDeviceToDevice, st));
-      if ((rc = allreduce(ar_user, L.d_c, (size_t)L.Dpad, 1, st))) return rc;
-      VGG_CUDA_CHECK(cudaMemcpyAsync(L.scal, L.d_c + L.Dpad - 2, sizeof(double) * 2, cudaMemcpyDeviceToDevice, st));
-    }
     if ((rc = launch_backsub(D, N, L.blk[cur].W, L.d_c, L.wacc, band.dev.kb_rows, band.dev.arrow_row, st))) return rc;
     if ((rc = launch_point_step(N, L.M, L.blk[cur].g_p, L.wacc, L.sc_p, L.dpp, L.points[cur], radius, L.points[cand],
                                 L.scal, st)))
@@ -824,11 +804,11 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + 1, L.scal + 2, sizeof(double) * 2, cudaMemcpyDeviceToDevice, st));
     VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + 3, L.scal + 6, sizeof(double), cudaMemcpyDeviceToDevice, st));
     if ((rc = launch_extract_gvec(S, dc, ns, L.KR, L.blk[cand].camrec, L.blk[cand].shared, L.small + 8, st))) return rc;
-    if (fab2.on) {
+    if (fab.on) {
       // one in-kernel all-reduce for everything: the point-gradient max rides in slot 4 (max), the rest is summed
       if ((rc = launch_gradmax(D, N, L.small + 8, prob->param_const, L.blk[cand].g_p, prob->point_const, L.scal, st))) return rc;
       VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + 4, L.scal + 5, sizeof(double), cudaMemcpyDeviceToDevice, st));
-      if ((rc = fab2.allreduce(L.small, 8 + L.Dpad, 4, st))) return rc;
+      if ((rc = fab.allreduce(L.small, 8 + L.Dpad, 4, st))) return rc;
       VGG_CUDA_CHECK(cudaMemsetAsync(L.scal + 4, 0, sizeof(double) * 2, st));
       if ((rc = launch_gradmax(D, N, L.small + 8, prob->param_const, L.blk[cand].g_p, prob->point_const, L.scal, st))) return rc;
       VGG_CUDA_CHECK(cudaMemcpyAsync(L.scal + 5, L.small + 4, sizeof(double), cudaMemcpyDeviceToDevice, st));

@@ -15,9 +15,8 @@
 //                       both operands in shared memory at a time (68 KB) so that its CTAs run NEXT TO the panel CTAs of
 //                       the following step (<= 155 KB with xr <= 20) on the same SMs.
 // Every MMA is mma.sync.m16n8k16.f64 (dmma_m16n8k16, full FP64 tensor rate on sm_90; m8n8k4 runs at half of it).
-// The whole launch sequence is captured once per (matrix, order) into a CUDA graph; VGG_CHOL_GRAPH=0 launches it
-// directly instead.  Matrices of fewer than three blocks are factored in program order (no fused update, no side streams).
-#include <stdlib.h>
+// The whole launch sequence is captured once per (matrix, order) into a CUDA graph.  Matrices of fewer than three blocks
+// are factored in program order (no fused update, no side streams), launched directly.
 #include <algorithm>
 #include <map>
 #include <vector>
@@ -898,7 +897,7 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
 
 // In-place Cholesky of the row-major lower triangle of A[n x n] (any even lda >= n, A 16-byte aligned): on return the lower
 // triangle holds L and the strict upper triangle L^T.  info (device int): 0 or the 1-based index of the first
-// non-positive pivot.  VGG_CHOL_GRAPH=0 switches the CUDA graph off.
+// non-positive pivot.
 // Block structure of a banded + arrow matrix (sequential / video problems; empty end_blk = dense): in block column b
 // the rows that can be non-zero below the diagonal block are the band [128 (b+1), 128 end_blk[b]) and the arrow
 // [128 arrow_blk, n).  end_blk is non-decreasing (the envelope the factorisation fills) and end_blk[b] >= b + 2 while
@@ -912,11 +911,10 @@ int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, cons
   const int nblk0 = (n + CB - 1) / CB;
   int* flags = reinterpret_cast<int*>(Ldiag + (size_t)nblk0 * CB * CB);
   VGG_CUDA_CHECK(cudaMemsetAsync(flags, 0, sizeof(int) * (size_t)nblk0, st));
-  static const bool use_graph = [] { const char* e = getenv("VGG_CHOL_GRAPH"); return !(e && e[0] == '0'); }();
   const int nblk = (n + CB - 1) / CB;
   CholStreams* cs = nullptr;
   if ((rc = chol_streams(&cs))) return rc;
-  if (nblk < 3 || !use_graph) return chol_enqueue(n, lda, A, Ldiag, info, flags, end_blk, arrow_blk, st, cs, nblk >= 3);
+  if (nblk < 3) return chol_enqueue(n, lda, A, Ldiag, info, flags, end_blk, arrow_blk, st, cs, false);
   // one captured graph per (matrix, order): ~60 launches + events become a single cudaGraphLaunch
   typedef std::tuple<double*, int, int, int*, double*, unsigned long long> Key;
   static thread_local std::map<Key, cudaGraphExec_t> cache;

@@ -30,11 +30,11 @@ def shard_range(N: int, rank: int, world: int, multiple: int = 16):
 
 class FabricBuffer:
     """Reduced-system buffer in symmetric (peer-mapped, NVSwitch-multicast) memory for the fused reduction
-    (include/vggsfm_b200.h: vgg_ba_fabric).  v2 (default): the tensor-core SYRK's epilogue REDs every 128-row block of the
-    lower triangle into its owner's copy over NVLink (reduce-scatter), every rank then pulls the blocks it does not own
+    (include/vggsfm_b200.h: vgg_ba_fabric).  The tensor-core SYRK's epilogue REDs every 128-row block of the lower
+    triangle into its owner's copy over NVLink (reduce-scatter), every rank then pulls the blocks it does not own
     (csrc/fabric.cu), and the barriers / small all-reduces of the LM loop are kernels on the same allocation -- no NCCL
-    call and no host callback inside the loop.  v1 (``VGG_FABRIC=1``): multimem.red into every copy + barriers and
-    small all-reduces through the AllReduceHook."""
+    call and no host callback inside the loop.  ``ok`` is False when the group lacks multicast or a peer table for
+    2..8 ranks; AllReduceHook then reduces through NCCL instead."""
 
     def __init__(self, S: int, model: int, mode: int, device, group=None):
         import torch.distributed._symmetric_memory as symm_mem
@@ -52,33 +52,28 @@ class FabricBuffer:
         self.world, self.rank = dist.get_world_size(group), dist.get_rank(group)
         ptrs = getattr(self.handle, "buffer_ptrs", None)
         self.peer_ptrs = [int(p) for p in ptrs] if ptrs is not None else []
-        self.ok = self.multicast_ptr != 0
-        self.v2 = self.ok and len(self.peer_ptrs) == self.world and 1 < self.world <= 8
-
-    def barrier(self):
-        self.handle.barrier(channel=0)
+        self.ok = self.multicast_ptr != 0 and len(self.peer_ptrs) == self.world and 1 < self.world <= 8
+        self.v2 = self.ok                             # bench.py reads this name
 
     def struct(self):
         f = _lib.BAFabric()
         f.ar_local, f.ar_multicast, f.ar_doubles = self.tensor.data_ptr(), self.multicast_ptr, self.count
-        if self.v2:
-            f.world, f.rank, f.total_doubles = self.world, self.rank, self.total
-            for r, p in enumerate(self.peer_ptrs):
-                f.peer_base[r] = p
+        f.world, f.rank, f.total_doubles = self.world, self.rank, self.total
+        for r, p in enumerate(self.peer_ptrs):
+            f.peer_base[r] = p
         return f
 
 
 class AllReduceHook:
-    """vgg_allreduce_fn implemented with torch.distributed on views of the solver workspace.  With a FabricBuffer
-    attached, the big per-iteration reduction is done by the kernels themselves and this hook only provides the
-    cross-rank barrier (op 2) and the small cost/gradient reductions."""
+    """vgg_allreduce_fn implemented with torch.distributed on views of the solver workspace.  With a usable FabricBuffer
+    attached, every reduction of the LM loop is done by the kernels themselves and the solver never calls this hook."""
 
     def __init__(self, group=None, fabric: "FabricBuffer | None" = None):
         self.group = group
         self.fabric = fabric if (fabric is not None and fabric.ok) else None
         self.calls = 0
         self.bytes = 0
-        self.barriers = 0
+        self.barriers = 0                             # always 0 (the barriers are kernels); bench.py reports it
         self._ws = None
         self._cb = None
 
@@ -88,10 +83,6 @@ class AllReduceHook:
 
         def _fn(user, buf, count, op, stream):
             try:
-                if op == 2:
-                    self.fabric.barrier()
-                    self.barriers += 1
-                    return 0
                 off = buf - base
                 view = self._ws[off:off + count * 8].view(torch.float64)
                 dist.all_reduce(view, op=dist.ReduceOp.SUM if op == 0 else dist.ReduceOp.MAX, group=self.group)
