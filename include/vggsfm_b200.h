@@ -126,11 +126,12 @@ int vgg_ba_build_blocks(const vgg_ba_problem* prob, double* cost, double* camrec
                         double* H_pp, double* W, double* shared, int tracks_per_warp, void* stream);
 
 /* Schur complement of the point blocks onto the camera system (second kernel of the path):
- * given the blocks above, the Jacobi scales and the trust-region radius, writes
+ * given the blocks above (without W: the coupling blocks are rebuilt from prob's observations and state), the Jacobi
+ * scales and the trust-region radius, writes
  * Sraw[D,Dpad] (symmetric, only the row-major lower triangle valid) = H_cc - sum_j W_j V_j^-1 W_j^T and rhs[Dpad] =
  * -(g_c - sum_j W_j V_j^-1 g_pj).  Exposed for the parity tests and profiling. */
 int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double* g_p,
-                 const double* H_pp, const double* W, const double* shared, const double* scale_p,
+                 const double* H_pp, const double* shared, const double* scale_p,
                  double radius, double min_diag, double max_diag, void* workspace, size_t ws_bytes,
                  double* Sraw, double* rhs, int* Dpad_out, void* stream);
 

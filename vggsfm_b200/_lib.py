@@ -128,7 +128,7 @@ def lib() -> ctypes.CDLL:
                                          ctypes.POINTER(ctypes.c_size_t)]
     L.vgg_ba_camrec_len.argtypes = [ctypes.c_int, ctypes.c_int]
     L.vgg_ba_build_blocks.argtypes = [ctypes.POINTER(BAProblem)] + [ctypes.c_void_p] * 6 + [ctypes.c_int, ctypes.c_void_p]
-    L.vgg_ba_schur.argtypes = ([ctypes.POINTER(BAProblem)] + [ctypes.c_void_p] * 6 +
+    L.vgg_ba_schur.argtypes = ([ctypes.POINTER(BAProblem)] + [ctypes.c_void_p] * 5 +
                                [ctypes.c_double] * 3 + [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p,
                                                         ctypes.c_void_p, ctypes.POINTER(ctypes.c_int), ctypes.c_void_p])
     L.vgg_ba_solve.argtypes = [ctypes.POINTER(BAProblem), ctypes.POINTER(BAOptions), ctypes.c_void_p, ctypes.c_size_t,

@@ -156,7 +156,8 @@ def build_blocks(uv, mask, poses, intr, points, model, mode, point_const=None, t
 
 def schur(uv, mask, poses, intr, points, model, mode, blocks, scale_p, radius, min_diag=1e-6, max_diag=1e32,
           point_const=None):
-    """Schur complement of `blocks` (vgg_ba_schur).  Returns (Sraw[D,Dpad] lower-valid, rhs[D])."""
+    """Schur complement of `blocks` (vgg_ba_schur; the coupling blocks are rebuilt from the observations and the
+    state, so blocks["W"] is not read).  Returns (Sraw[D,Dpad] lower-valid, rhs[D])."""
     L = _lib.lib()
     S, N = mask.shape
     dc, ns = dims(model, mode)
@@ -171,7 +172,7 @@ def schur(uv, mask, poses, intr, points, model, mode, blocks, scale_p, radius, m
     with torch.cuda.device(dev):
         st = torch.cuda.current_stream().cuda_stream
         _lib.check(L.vgg_ba_schur(ctypes.byref(p), blocks["camrec"].data_ptr(), blocks["g_p"].data_ptr(),
-                                  blocks["H_pp"].data_ptr(), blocks["W"].data_ptr(), blocks["shared"].data_ptr(),
+                                  blocks["H_pp"].data_ptr(), blocks["shared"].data_ptr(),
                                   scale_p.data_ptr(), radius, min_diag, max_diag, ws.data_ptr(), ws.numel(),
                                   Sraw.data_ptr(), rhs.data_ptr(), ctypes.byref(dpad), st), "vgg_ba_schur")
     assert dpad.value == Dpad

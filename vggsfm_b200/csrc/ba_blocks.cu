@@ -23,8 +23,11 @@
 //   * observations (uv 8 B + mask 1 B) are read with 32-byte vector loads, 4 tracks per lane at a time,
 //     prefetched one batch ahead; poses/intrinsics sit transposed in shared memory (one frame per lane).
 // Algorithmic HBM bytes per observation: 9 + 24*dc (+ amortised per-frame/per-point terms), see DESIGN.md.
+// The LM solve runs the variant without W (WRITE_W = false): 9 B per observation.  z_build and backsub (ba_schur.cu)
+// rebuild each block from its observation with the same obs_math (ba_obs.h), so W never goes through HBM there.
 #include <stdlib.h>
 #include <utility>
+#include "ba_obs.h"
 #include "common.cuh"
 #include "dev_probes.h"
 
@@ -40,16 +43,6 @@ constexpr int BT = BW * 32;      // threads per CTA
 constexpr int TB = 4;            // tracks per prefetch batch (32 B of uv per lane)
 constexpr int XT = 32;           // tracks per shared-memory point tile (one per lane)
 constexpr int PVS = 33;          // row stride of the per-point scratch (odd: conflict-free column sums)
-
-template <int MODEL, int MODE>
-struct BlkCfg {
-  static constexpr int NI = (MODEL == VGG_SIMPLE_PINHOLE) ? 1 : 2;
-  static constexpr int DC = (MODE == VGG_INTR_PER_FRAME) ? 6 + NI : 6;
-  static constexpr int NS = (MODE == VGG_INTR_SHARED) ? NI : 0;
-  static constexpr int NPACK = DC * (DC + 1) / 2;
-  static constexpr int KR = DC + NPACK + 6 * NS;   // per-frame camera record length
-  static constexpr int NP = 9 + 3 * NS;            // per-point reduced values: g_p 3, H_pp 6, W_s 3*NS
-};
 
 // ---- compile-time layout of the per-frame camera record: g_c[DC] | H_cc upper-packed | H_cs[6][NS] ----
 __host__ __device__ constexpr int pack_row(int dc, int p) {
@@ -84,77 +77,24 @@ __device__ __forceinline__ void cam_accumulate(double (&acc)[KR], const double* 
   (cam_accumulate_one<DC, NS, K, KR>(acc, jc0, jc1, rx, ry), ...);
 }
 
-// One observation, branch-free: residual and Jacobian columns, all scaled by the validity mask (an invalid
-// observation computes on a safe depth and contributes exact zeros).  jc: delta(3), t(3), f, k; jx: point(3).
-template <int MODEL>
-__device__ __forceinline__ void obs_math(const double* pw, int lane, const double* xt, float ox, float oy, bool valid,
-                                         double* jc0, double* jc1, double* jx0, double* jx1, double& rx, double& ry) {
-  const double2 xa = *reinterpret_cast<const double2*>(xt);
-  const double2 xb = *reinterpret_cast<const double2*>(xt + 2);
-  const double X0 = xa.x, X1 = xa.y, X2 = xb.x;
-  const double m = valid ? 1.0 : 0.0;
-  const double mp = (xb.y != 0.0) ? 0.0 : m;                    // constant point: no point columns
-  const double R00 = pw[0 * 32 + lane], R01 = pw[1 * 32 + lane], R02 = pw[2 * 32 + lane], t0_ = pw[3 * 32 + lane];
-  const double R10 = pw[4 * 32 + lane], R11 = pw[5 * 32 + lane], R12 = pw[6 * 32 + lane], t1_ = pw[7 * 32 + lane];
-  const double R20 = pw[8 * 32 + lane], R21 = pw[9 * 32 + lane], R22 = pw[10 * 32 + lane], t2_ = pw[11 * 32 + lane];
-  const double fo = pw[12 * 32 + lane], cx = pw[13 * 32 + lane], cy = pw[14 * 32 + lane];
-  const double kk = (MODEL == VGG_SIMPLE_RADIAL) ? pw[15 * 32 + lane] : 0.0;
-  const double a1 = R00 * X0 + R01 * X1 + R02 * X2;
-  const double a2 = R10 * X0 + R11 * X1 + R12 * X2;
-  const double a3 = R20 * X0 + R21 * X1 + R22 * X2;
-  const double px = a1 + t0_, py = a2 + t1_;
-  const double pz = valid ? (a3 + t2_) : 1.0;
-  const double iz = 1.0 / pz;
-  const double u = px * iz, w_ = py * iz;
-  const double r2 = u * u + w_ * w_;
-  const double d = 1.0 + kk * r2;
-  rx = valid ? (fo * d * u + cx - (double)ox) : 0.0;            // select, not multiply: ox/oy of a masked slot may be anything
-  ry = valid ? (fo * d * w_ + cy - (double)oy) : 0.0;
-  double a00, a01, a11;
-  if (MODEL == VGG_SIMPLE_RADIAL) {
-    a00 = fo * (d + 2.0 * kk * u * u);
-    a01 = fo * (2.0 * kk * u * w_);
-    a11 = fo * (d + 2.0 * kk * w_ * w_);
-  } else {
-    a00 = fo; a01 = 0.0; a11 = fo;
-  }
-  // Jproj (2x3) = f*A * iz*[[1,0,-u],[0,1,-v]], masked
-  const double izm = iz * m;
-  const double j00 = a00 * izm, j01 = a01 * izm, j02 = -(a00 * u + a01 * w_) * izm;
-  const double j10 = a01 * izm, j11 = a11 * izm, j12 = -(a01 * u + a11 * w_) * izm;
-  const double b1 = 2.0 * a1, b2 = 2.0 * a2, b3 = 2.0 * a3;
-  jc0[0] = b2 * j02 - b3 * j01;  jc1[0] = b2 * j12 - b3 * j11;
-  jc0[1] = b3 * j00 - b1 * j02;  jc1[1] = b3 * j10 - b1 * j12;
-  jc0[2] = b1 * j01 - b2 * j00;  jc1[2] = b1 * j11 - b2 * j10;
-  jc0[3] = j00; jc0[4] = j01; jc0[5] = j02;
-  jc1[3] = j10; jc1[4] = j11; jc1[5] = j12;
-  jc0[6] = m * d * u;            jc1[6] = m * d * w_;
-  jc0[7] = m * fo * u * r2;      jc1[7] = m * fo * w_ * r2;
-  const double mq = (xb.y != 0.0) ? 0.0 : 1.0;
-  jx0[0] = mq * (j00 * R00 + j01 * R10 + j02 * R20);
-  jx0[1] = mq * (j00 * R01 + j01 * R11 + j02 * R21);
-  jx0[2] = mq * (j00 * R02 + j01 * R12 + j02 * R22);
-  jx1[0] = mq * (j10 * R00 + j11 * R10 + j12 * R20);
-  jx1[1] = mq * (j10 * R01 + j11 * R11 + j12 * R21);
-  jx1[2] = mq * (j10 * R02 + j11 * R12 + j12 * R22);
-  (void)mp;
-}
-
-// coupling block (DC rows x 3, 16-byte stores into the staging buffer) and per-point values (scratch column)
-template <int DC, int NS, int WB>
+// coupling block (DC rows x 3, 16-byte stores into the staging buffer; only when W is written) and per-point values
+// (scratch column)
+template <int DC, int NS, int WB, bool WRITE_W>
 __device__ __forceinline__ void emit_blocks(double* wt, double* pvw, int lane, const double* jc0, const double* jc1,
                                             const double* jx0, const double* jx1, double rx, double ry) {
-  double wb[WB];
+  if (WRITE_W) {
+    double wb[WB];
 #pragma unroll
-  for (int i = 0; i < DC; ++i)
+    for (int i = 0; i < DC; ++i)
 #pragma unroll
-    for (int c = 0; c < 3; ++c) wb[i * 3 + c] = jc0[i] * jx0[c] + jc1[i] * jx1[c];
-  if ((WB & 1) == 0) {
+      for (int c = 0; c < 3; ++c) wb[i * 3 + c] = w_entry(jc0, jc1, jx0, jx1, i, c);
+    if ((WB & 1) == 0) {
 #pragma unroll
-    for (int e = 0; e < WB; e += 2) *reinterpret_cast<double2*>(wt + e) = make_double2(wb[e], wb[e + 1]);
-  } else {
+      for (int e = 0; e < WB; e += 2) *reinterpret_cast<double2*>(wt + e) = make_double2(wb[e], wb[e + 1]);
+    } else {
 #pragma unroll
-    for (int e = 0; e < WB; ++e) wt[e] = wb[e];
+      for (int e = 0; e < WB; ++e) wt[e] = wb[e];
+    }
   }
   pvw[0 * PVS + lane] = jx0[0] * rx + jx1[0] * ry;
   pvw[1 * PVS + lane] = jx0[1] * rx + jx1[1] * ry;
@@ -165,26 +105,32 @@ __device__ __forceinline__ void emit_blocks(double* wt, double* pvw, int lane, c
   pvw[6 * PVS + lane] = jx0[1] * jx0[1] + jx1[1] * jx1[1];
   pvw[7 * PVS + lane] = jx0[1] * jx0[2] + jx1[1] * jx1[2];
   pvw[8 * PVS + lane] = jx0[2] * jx0[2] + jx1[2] * jx1[2];
+  if (WRITE_W) {
 #pragma unroll
-  for (int j = 0; j < NS; ++j)
+    for (int j = 0; j < NS; ++j)
 #pragma unroll
-    for (int c = 0; c < 3; ++c) pvw[(9 + j * 3 + c) * PVS + lane] = jc0[6 + j] * jx0[c] + jc1[6 + j] * jx1[c];
+      for (int c = 0; c < 3; ++c) pvw[(9 + j * 3 + c) * PVS + lane] = w_entry(jc0, jc1, jx0, jx1, 6 + j, c);
+  }
 }
 
 // W row pitch (rows of 3 doubles) of one track: D rounded up to even so every track starts 16-B aligned
 __host__ __device__ inline size_t w_pitch(int D) { return (size_t)(D + (D & 1)); }
 
 // Two CTAs per SM let ptxas use ~250 registers (no spills, 8 warps/SM); three cap them at 168 (12 warps/SM) and spill.
-// The TMA variant runs at two, the non-TMA fallback (W not 16-byte aligned) at three.
-template <int MODEL, int MODE, bool USE_TMA>
-__global__ void __launch_bounds__(BT, USE_TMA ? 2 : 3) ba_blocks_kernel(
+// The TMA variant runs at two, the non-TMA fallback (W not 16-byte aligned) at three.  The variant of the LM solve
+// (WRITE_W = false) stores no W -- z_build and backsub rebuild each block from its observation (ba_obs.h) -- which
+// drops the staging buffers and the 24-double block from the live registers: it runs at BLK_NOW_CTAS CTAs per SM.
+constexpr int BLK_NOW_CTAS = 2;
+template <int MODEL, int MODE, bool WRITE_W, bool USE_TMA>
+__global__ void __launch_bounds__(BT, WRITE_W ? (USE_TMA ? 2 : 3) : BLK_NOW_CTAS) ba_blocks_kernel(
     int S, int N, int tracks_per_warp, const float* __restrict__ uv, const uint8_t* __restrict__ mask,
     const double* __restrict__ poses, const double* __restrict__ intr, const double* __restrict__ points,
     const uint8_t* __restrict__ point_const, double* __restrict__ cost, double* __restrict__ camrec,
     double* __restrict__ g_p, double* __restrict__ H_pp, double* __restrict__ W, double* __restrict__ shared_out,
     const int* __restrict__ fg_tracks) {
   using C = BlkCfg<MODEL, MODE>;
-  constexpr int DC = C::DC, NS = C::NS, KR = C::KR, NP = C::NP;
+  constexpr int DC = C::DC, NS = C::NS, KR = C::KR;
+  constexpr int NP = WRITE_W ? 9 + 3 * NS : 9;     // per-point reduced values: g_p 3, H_pp 6, W_s 3*NS
   constexpr int WB = DC * 3;                       // doubles per observation block
   extern __shared__ __align__(128) unsigned char smem_raw[];
   // per warp: pose/intrinsics transposed [16][32], two W staging buffers [32][WB]
@@ -192,7 +138,7 @@ __global__ void __launch_bounds__(BT, USE_TMA ? 2 : 3) ba_blocks_kernel(
   double* sm_x = sm_pose + BW * 16 * 32;                                 // [BW][XT][4]: X,Y,Z,const flag per track
   double* sm_pv = sm_x + BW * XT * 4;                                    // [BW][2 tracks x 16][PVS]: per-point values, one column per lane
   double* sm_w = sm_pv + BW * 32 * PVS;                                  // [BW][2][32*WB]
-  float* sm_obs = reinterpret_cast<float*>(sm_w + (size_t)BW * 2 * 32 * WB);   // [BW][2 stages][32 lanes][12]
+  float* sm_obs = reinterpret_cast<float*>(sm_w + (WRITE_W ? (size_t)BW * 2 * 32 * WB : 0));   // [BW][2 stages][32 lanes][12]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int D = S * DC + NS;
   const size_t pitch = w_pitch(D);
@@ -207,8 +153,8 @@ __global__ void __launch_bounds__(BT, USE_TMA ? 2 : 3) ba_blocks_kernel(
   const int chunk = wid / ngroups;
   const int t_begin = (int)min((long long)N, (long long)chunk * tracks_per_warp);
   const int t_end = min(N, t_begin + tracks_per_warp);
-  // banded (sequential) problems: none of this warp's tracks is visible in its 32 frames.  Their W blocks stay at the zero
-  // the solver wrote once per solve, and z_build / backsub skip the same region (csrc/ba_solve.cu, compute_band_hint).
+  // banded (sequential) problems (solve only): none of this warp's tracks is visible in its 32 frames, so they add
+  // nothing; z_build and backsub skip the same region (csrc/ba_solve.cu, compute_band_hint).
   if (fg_tracks && (t_end <= fg_tracks[2 * g] || t_begin >= fg_tracks[2 * g + 1])) return;
   const int s = g * 32 + lane;
   const bool frame_ok = s < S;
@@ -294,28 +240,34 @@ __global__ void __launch_bounds__(BT, USE_TMA ? 2 : 3) ba_blocks_kernel(
       {
         const float ox = k == 0 ? ca.x : cb.x, oy = k == 0 ? ca.y : cb.y;
         const bool valid = frame_ok && ((cm >> (8 * k)) & 0xffu) != 0;
-        obs_math<MODEL>(pw, lane, xw + ((nA - t_begin) & (XT - 1)) * 4, ox, oy, valid, jcA0, jcA1, jxA0, jxA1, rxA, ryA);
+        const double* xt = xw + ((nA - t_begin) & (XT - 1)) * 4;
+        const double2 xa = *reinterpret_cast<const double2*>(xt), xb = *reinterpret_cast<const double2*>(xt + 2);
+        obs_math<MODEL>(pw + lane, 32, xa.x, xa.y, xb.x, xb.y != 0.0, ox, oy, valid, jcA0, jcA1, jxA0, jxA1, rxA, ryA);
       }
       {
         const float ox = k == 0 ? ca.z : cb.z, oy = k == 0 ? ca.w : cb.w;
         const bool valid = hasB && frame_ok && ((cm >> (8 * (k + 1))) & 0xffu) != 0;
-        obs_math<MODEL>(pw, lane, xw + ((nA + 1 - t_begin) & (XT - 1)) * 4, ox, oy, valid, jcB0, jcB1, jxB0, jxB1, rxB, ryB);
+        const double* xt = xw + ((nA + 1 - t_begin) & (XT - 1)) * 4;
+        const double2 xa = *reinterpret_cast<const double2*>(xt), xb = *reinterpret_cast<const double2*>(xt + 2);
+        obs_math<MODEL>(pw + lane, 32, xa.x, xa.y, xb.x, xb.y != 0.0, ox, oy, valid, jcB0, jcB1, jxB0, jxB1, rxB, ryB);
       }
       cost_acc += 0.5 * (rxA * rxA + ryA * ryA) + 0.5 * (rxB * rxB + ryB * ryB);
       // ---- both staging buffers must have been read out by the previous step's bulk stores
-      if (USE_TMA) {
+      if (WRITE_W && USE_TMA) {
         if (lane == 0) tma_store_wait_read<0>();
         __syncwarp();
       }
       double* wA = wbuf + lane * WB;
       double* wB = wbuf + 32 * WB + lane * WB;
-      emit_blocks<DC, NS, WB>(wA, pvw, lane, jcA0, jcA1, jxA0, jxA1, rxA, ryA);
-      emit_blocks<DC, NS, WB>(wB, pvw + 16 * PVS, lane, jcB0, jcB1, jxB0, jxB1, rxB, ryB);
+      emit_blocks<DC, NS, WB, WRITE_W>(wA, pvw, lane, jcA0, jcA1, jxA0, jxA1, rxA, ryA);
+      emit_blocks<DC, NS, WB, WRITE_W>(wB, pvw + 16 * PVS, lane, jcB0, jcB1, jxB0, jxB1, rxB, ryB);
       // ---- ship the 32 frames' blocks of each track: contiguous runs W[n][g*32*DC .. +nf*DC][3]
       double* dstA = W + ((size_t)nA * pitch + (size_t)g * 32 * DC) * 3;
       double* dstB = dstA + pitch * 3;
       const uint32_t bytes = (uint32_t)nf * WB * 8u;
-      if (USE_TMA && (bytes & 15u) == 0) {
+      if (!WRITE_W) {
+        __syncwarp();
+      } else if (USE_TMA && (bytes & 15u) == 0) {
         fence_proxy_async();
         __syncwarp();
         if (lane == 0) {
@@ -363,7 +315,7 @@ __global__ void __launch_bounds__(BT, USE_TMA ? 2 : 3) ba_blocks_kernel(
       __syncwarp();        // the scratch and the staging buffers are rewritten next step
     }
   }
-  if (USE_TMA && lane == 0) tma_store_wait_all<0>();
+  if (WRITE_W && USE_TMA && lane == 0) tma_store_wait_all<0>();
 
   // flush this lane's camera record
   if (frame_ok && t_begin < t_end) {
@@ -388,11 +340,15 @@ static int launch_blocks(const vgg_ba_problem* p, double* cost, double* camrec, 
   const int S = p->S, N = p->N;
   const int D = S * C::DC + C::NS;
   const size_t pitch = w_pitch(D);
-  const size_t smem = sizeof(double) * (BW * 16 * 32 + BW * XT * 4 + BW * 32 * PVS + (size_t)BW * 2 * 32 * C::DC * 3) +
+  const bool write_w = W != nullptr;
+  const size_t smem = sizeof(double) * (BW * 16 * 32 + BW * XT * 4 + BW * 32 * PVS +
+                                        (write_w ? (size_t)BW * 2 * 32 * C::DC * 3 : 0)) +
                       sizeof(float) * BW * 2 * 32 * 12;
   const bool tma_ok = ((reinterpret_cast<uintptr_t>(W) & 15) == 0);
   const int ngroups = (S + 31) / 32;
-  const auto kern = tma_ok ? ba_blocks_kernel<MODEL, MODE, true> : ba_blocks_kernel<MODEL, MODE, false>;
+  const auto kern = !write_w ? ba_blocks_kernel<MODEL, MODE, false, false>
+                    : tma_ok ? ba_blocks_kernel<MODEL, MODE, true, true>
+                             : ba_blocks_kernel<MODEL, MODE, true, false>;
   if (tracks_per_warp <= 0 && fg_tracks) {
     // banded (sequential) problems: most (frame group, track chunk) warps return at once, so the chunks must be small
     // enough for the few that do not to spread over the machine (r02 launch list at 1000 frames x 32 k points: with the
@@ -403,15 +359,18 @@ static int launch_blocks(const vgg_ba_problem* p, double* cost, double* camrec, 
     // Every warp does the same amount of work, so the grid must be a whole number of waves: resident warps =
     // SMs x CTAs/SM (occupancy query) x BW.  Pick the smallest wave count that keeps >= 32 tracks per warp
     // amortising the per-warp camera flush (32 x KR REDs), capped at 4 waves; tracks per warp multiple of TB.
-    static int slots = 0;
+    // (one figure for the solve's variant without W, one for the W-writing variants)
+    static int slots_of[2] = {0, 0};
+    int& slots = slots_of[write_w];
     if (slots == 0) {
       int dev = 0, sms = 132, per_sm = 2;
       cudaGetDevice(&dev);
       cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
       // the occupancy query needs the opt-in shared-memory limit in place (r02: without it the query returned 0, the
       // grid was sized for ONE CTA per SM and the 400 x 4096 launch ran as a single wave of 147 CTAs, half the warps)
-      cudaFuncSetAttribute(ba_blocks_kernel<MODEL, MODE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ba_blocks_kernel<MODEL, MODE, true>, BT, smem);
+      const auto qk = write_w ? ba_blocks_kernel<MODEL, MODE, true, true> : kern;
+      cudaFuncSetAttribute(qk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, qk, BT, smem);
       if (per_sm < 1) per_sm = 1;
       slots = sms * per_sm;
     }
@@ -449,7 +408,7 @@ static int launch_blocks(const vgg_ba_problem* p, double* cost, double* camrec, 
       VGG_CUDA_CHECK(cudaMemsetAsync(shared_out, 0, sizeof(double) * 8, stream));
     }
   }
-  if (pitch > (size_t)S * C::DC) {
+  if (write_w && pitch > (size_t)S * C::DC) {
     // shared-intrinsics rows (accumulated with REDs) and the pitch padding row of every track
     const size_t tail = pitch - (size_t)S * C::DC;
     VGG_CUDA_CHECK(cudaMemset2DAsync(W + (size_t)S * C::DC * 3, pitch * 24, 0, tail * 24, (size_t)N, stream));

@@ -1,0 +1,78 @@
+// The Jacobian of one observation, shared by every bundle-adjustment kernel that needs one: ba_blocks (cost, camera
+// records, point blocks), z_build (the Schur operand Zt = W M) and backsub (W^T d_c).  W = J_c^T J_p is never stored
+// in the solve; the kernels that use it rebuild it from the observation with this one function, so every copy of a
+// block is the same arithmetic.
+#pragma once
+#include "common.cuh"
+
+namespace vgg {
+
+template <int MODEL, int MODE>
+struct BlkCfg {
+  static constexpr int NI = (MODEL == VGG_SIMPLE_PINHOLE) ? 1 : 2;
+  static constexpr int DC = (MODE == VGG_INTR_PER_FRAME) ? 6 + NI : 6;
+  static constexpr int NS = (MODE == VGG_INTR_SHARED) ? NI : 0;
+  static constexpr int NPACK = DC * (DC + 1) / 2;
+  static constexpr int KR = DC + NPACK + 6 * NS;   // per-frame camera record length
+};
+
+// One observation, branch-free: residual and Jacobian columns, all scaled by the validity mask (an invalid
+// observation computes on a safe depth and contributes exact zeros).  jc: delta(3), t(3), f, k; jx: point(3).
+// cam: R (row-major 3x4 with t), f, cx, cy, k at cam[0], cam[cs], ..., cam[15 cs]; pc: the point is held constant.
+template <int MODEL>
+__device__ __forceinline__ void obs_math(const double* cam, int cs, double X0, double X1, double X2, bool pc, float ox,
+                                         float oy, bool valid, double* jc0, double* jc1, double* jx0, double* jx1,
+                                         double& rx, double& ry) {
+  const double m = valid ? 1.0 : 0.0;
+  const double R00 = cam[0 * cs], R01 = cam[1 * cs], R02 = cam[2 * cs], t0_ = cam[3 * cs];
+  const double R10 = cam[4 * cs], R11 = cam[5 * cs], R12 = cam[6 * cs], t1_ = cam[7 * cs];
+  const double R20 = cam[8 * cs], R21 = cam[9 * cs], R22 = cam[10 * cs], t2_ = cam[11 * cs];
+  const double fo = cam[12 * cs], cx = cam[13 * cs], cy = cam[14 * cs];
+  const double kk = (MODEL == VGG_SIMPLE_RADIAL) ? cam[15 * cs] : 0.0;
+  const double a1 = R00 * X0 + R01 * X1 + R02 * X2;
+  const double a2 = R10 * X0 + R11 * X1 + R12 * X2;
+  const double a3 = R20 * X0 + R21 * X1 + R22 * X2;
+  const double px = a1 + t0_, py = a2 + t1_;
+  const double pz = valid ? (a3 + t2_) : 1.0;
+  const double iz = 1.0 / pz;
+  const double u = px * iz, w_ = py * iz;
+  const double r2 = u * u + w_ * w_;
+  const double d = 1.0 + kk * r2;
+  rx = valid ? (fo * d * u + cx - (double)ox) : 0.0;            // select, not multiply: ox/oy of a masked slot may be anything
+  ry = valid ? (fo * d * w_ + cy - (double)oy) : 0.0;
+  double a00, a01, a11;
+  if (MODEL == VGG_SIMPLE_RADIAL) {
+    a00 = fo * (d + 2.0 * kk * u * u);
+    a01 = fo * (2.0 * kk * u * w_);
+    a11 = fo * (d + 2.0 * kk * w_ * w_);
+  } else {
+    a00 = fo; a01 = 0.0; a11 = fo;
+  }
+  // Jproj (2x3) = f*A * iz*[[1,0,-u],[0,1,-v]], masked
+  const double izm = iz * m;
+  const double j00 = a00 * izm, j01 = a01 * izm, j02 = -(a00 * u + a01 * w_) * izm;
+  const double j10 = a01 * izm, j11 = a11 * izm, j12 = -(a01 * u + a11 * w_) * izm;
+  const double b1 = 2.0 * a1, b2 = 2.0 * a2, b3 = 2.0 * a3;
+  jc0[0] = b2 * j02 - b3 * j01;  jc1[0] = b2 * j12 - b3 * j11;
+  jc0[1] = b3 * j00 - b1 * j02;  jc1[1] = b3 * j10 - b1 * j12;
+  jc0[2] = b1 * j01 - b2 * j00;  jc1[2] = b1 * j11 - b2 * j10;
+  jc0[3] = j00; jc0[4] = j01; jc0[5] = j02;
+  jc1[3] = j10; jc1[4] = j11; jc1[5] = j12;
+  jc0[6] = m * d * u;            jc1[6] = m * d * w_;
+  jc0[7] = m * fo * u * r2;      jc1[7] = m * fo * w_ * r2;
+  const double mq = pc ? 0.0 : 1.0;                              // constant point: no point columns
+  jx0[0] = mq * (j00 * R00 + j01 * R10 + j02 * R20);
+  jx0[1] = mq * (j00 * R01 + j01 * R11 + j02 * R21);
+  jx0[2] = mq * (j00 * R02 + j01 * R12 + j02 * R22);
+  jx1[0] = mq * (j10 * R00 + j11 * R10 + j12 * R20);
+  jx1[1] = mq * (j10 * R01 + j11 * R11 + j12 * R21);
+  jx1[2] = mq * (j10 * R02 + j11 * R12 + j12 * R22);
+}
+
+// one entry of the coupling block W = J_c^T J_p: row i of the camera columns (6 + intrinsics), point column c
+__device__ __forceinline__ double w_entry(const double* jc0, const double* jc1, const double* jx0, const double* jx1,
+                                          int i, int c) {
+  return jc0[i] * jx0[c] + jc1[i] * jx1[c];
+}
+
+}  // namespace vgg

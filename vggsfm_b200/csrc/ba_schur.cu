@@ -6,8 +6,8 @@
 //   point_prep      per point: V = Dp H_pp Dp + diag(clamp(diag))/radius, 3x3 Cholesky,
 //                   M = Dp L^-T, q = M^T g_p
 //   assemble_hc     camera Hessian/gradient from the per-frame records into the dense reduced system
-//   z_build         Zt[3n+c][row] = (W[n][row][:] M_n)[c]   (k-major operand for the SYRK; W is track-major,
-//                   so this is a straight streaming pass), rhs[row] += Z[row] . q
+//   z_build         Zt[3n+c][row] = (W[n][row][:] M_n)[c]   (k-major operand for the SYRK), W rebuilt per observation,
+//                   rhs[row] += Z[row] . q
 //   syrk_f64        Sraw -= Zt^T Zt on the upper 128x128 tiles, mirrored into the lower triangle: FP64 tensor cores
 //                   (DMMA 16x8x16), bulk-copy/mbarrier ring, persistent over a k-split work list, f64 RED epilogue
 //   scale_damp      A = Dc Sraw Dc + diag(clamp(diag(Dc Hcc Dc)))/radius, constant parameters pinned
@@ -15,6 +15,7 @@
 #include <stddef.h>
 #include <algorithm>
 #include <vector>
+#include "ba_obs.h"
 #include "common.cuh"
 #include "dev_probes.h"
 #include "syrk_work.h"
@@ -160,47 +161,135 @@ __global__ void assemble_hc_kernel(int S, int dc, int ns, int KR, int Dpad, cons
 }
 
 // ------------------------------------------------------------------------------------------------
-// Schur operand: Zt[(3n+c)*Dpad + row] = sum_c' W[n][row][c'] M[n][c'][c];  rhs[row] += sum_{n,c} Z q.
-// W is track-major ([N][pitch][3]), so for a fixed track both the read (24 B per row) and the three writes
-// (8 B per row into three k-rows of Zt) are contiguous across threads: no transpose, no shared-memory tile.
-// block = 128 rows x ZB_NT tracks.
-constexpr int ZB_NT = 32;
-__global__ void __launch_bounds__(128) z_build_kernel(int D, int N, int Dpad, size_t pitch, const double* __restrict__ W,
-                                                      const double* __restrict__ M, const double* __restrict__ q,
-                                                      double* __restrict__ Zt, double* __restrict__ rhs,
-                                                      ptrdiff_t mc_off, const int* __restrict__ rb_range) {
-  __shared__ double sm[ZB_NT][12];
-  const int row = blockIdx.x * 128 + threadIdx.x;
-  const int n0 = blockIdx.y * ZB_NT;
-  const int nt = min(ZB_NT, N - n0);
-  // banded problems: these 32 tracks' rows of Zt lie outside the k range in which this 128-column block is non-zero --
-  // W is zero here (never written after the per-solve memset), nobody reads this part of Zt, nothing to add to rhs
-  if (rb_range) {
-    const int kb_first = (3 * n0) >> 6, kb_last = (3 * (n0 + nt - 1) + 2) >> 6;
-    if (kb_last < rb_range[2 * blockIdx.x] || kb_first >= rb_range[2 * blockIdx.x + 1]) return;
+// Schur operand straight from the observations: Zt[(3n+c)*Dpad + s*dc+i] = (W_sn M_n)[i][c], W_sn = J_c^T J_p of
+// observation (s, n) rebuilt by obs_math (ba_obs.h) -- no stored coupling blocks -- and rhs[row] += sum_{n,c} Z q.
+// A CTA owns ZB_NT tracks and all frames; its warps take the 32-frame groups in turn, one lane per frame, so the blocks
+// of one (track, group) are 32*dc contiguous doubles of each of the three Zt rows: staged in shared memory, written
+// with 16-byte stores.  A lane reads the ZB_NT observations of its frame, 8 B each and consecutive in uv, so every
+// sector it pulls from HBM is used whole.  The shared-intrinsics columns are sums over all frames: each warp reduces
+// its groups' share per track, the CTA adds the warps' shares at the end.
+// Rows that no observation reaches (masked everywhere in a frame group; band skip of sequential problems) are not
+// written: the mask is fixed during a solve and Zt is zeroed once before it, so they hold the zero they would get.
+constexpr int ZB_NT = 8;     // tracks per CTA
+constexpr int ZB_W = 4;      // warps per CTA
+template <int MODEL, int MODE>
+__global__ void __launch_bounds__(ZB_W * 32) z_build_kernel(
+    int S, int N, int Dpad, const float* __restrict__ uv, const uint8_t* __restrict__ mask,
+    const double* __restrict__ poses, const double* __restrict__ intr, const double* __restrict__ points,
+    const uint8_t* __restrict__ point_const, const double* __restrict__ M, const double* __restrict__ q,
+    double* __restrict__ Zt, double* __restrict__ rhs, ptrdiff_t mc_off, const int* __restrict__ fg_tracks) {
+  using C = BlkCfg<MODEL, MODE>;
+  constexpr int DC = C::DC, NS = C::NS;
+  constexpr int ZR = 32 * DC;                      // Zt columns of one frame group
+  __shared__ __align__(16) double s_cam[ZB_W][16 * 32];   // per warp: pose | f, cx, cy, k, transposed (one frame per lane)
+  __shared__ __align__(16) double s_z[ZB_W][3 * ZR];      // per warp: the three Zt rows of one (track, frame group)
+  __shared__ double s_pt[ZB_NT][16];                      // per track: X, Y, Z, constant flag | M (9) | q (3)
+  __shared__ double s_ws[ZB_W][ZB_NT][3 * (NS > 0 ? NS : 1)];   // per warp and track: its frames' share of W_s
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int n0 = blockIdx.x * ZB_NT, nt = min(ZB_NT, N - n0);
+  const int ngroups = (S + 31) / 32;
+  for (int e = threadIdx.x; e < ZB_NT * 16; e += blockDim.x) {
+    const int t = e >> 4, k = e & 15, n = n0 + t;
+    double v = 0.0;
+    if (t < nt) {
+      if (k < 3) v = points[(size_t)n * 3 + k];
+      else if (k == 3) v = (point_const && point_const[n]) ? 1.0 : 0.0;
+      else if (k < 13) v = M[(size_t)n * 9 + (k - 4)];
+      else v = q[(size_t)n * 3 + (k - 13)];
+    }
+    s_pt[t][k] = v;
   }
-  for (int e = threadIdx.x; e < nt * 12; e += 128) {
-    const int t = e / 12, k = e % 12;
-    sm[t][k] = k < 9 ? M[(size_t)(n0 + t) * 9 + k] : q[(size_t)(n0 + t) * 3 + (k - 9)];
-  }
+  if (NS > 0)
+    for (int e = threadIdx.x; e < ZB_W * ZB_NT * 3 * NS; e += blockDim.x) (&s_ws[0][0][0])[e] = 0.0;
   __syncthreads();
-  if (row >= D) return;
-  double zq = 0.0;
-  const double* wp = W + ((size_t)n0 * pitch + row) * 3;
-#pragma unroll 4
-  for (int t = 0; t < nt; ++t, wp += pitch * 3) {
-    const double w0 = wp[0], w1 = wp[1], w2 = wp[2];
-    const double* m = sm[t];
-    const double z0 = w0 * m[0];                              // M upper triangular (row-major)
-    const double z1 = w0 * m[1] + w1 * m[4];
-    const double z2 = w0 * m[2] + w1 * m[5] + w2 * m[8];
-    double* zo = Zt + (size_t)(3 * (n0 + t)) * Dpad + row;
-    zo[0] = z0;
-    zo[Dpad] = z1;
-    zo[2 * (size_t)Dpad] = z2;
-    zq += z0 * m[9] + z1 * m[10] + z2 * m[11];
+  double* pw = s_cam[warp];
+  double* zs = s_z[warp];
+  const float2* uv2 = reinterpret_cast<const float2*>(uv);
+  for (int g = warp; g < ngroups; g += ZB_W) {
+    if (fg_tracks && (n0 + nt <= fg_tracks[2 * g] || n0 >= fg_tracks[2 * g + 1])) continue;
+    const int s = g * 32 + lane;
+    const bool frame_ok = s < S;
+    const int cnt = min(32, S - g * 32) * DC;      // Zt columns of the frames of this group that exist
+    __syncwarp();
+#pragma unroll
+    for (int i = 0; i < 12; ++i) pw[i * 32 + lane] = frame_ok ? poses[(size_t)s * 12 + i] : 0.0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) pw[(12 + i) * 32 + lane] = frame_ok ? intr[(size_t)s * 4 + i] : 0.0;
+    __syncwarp();
+    double zq[DC];
+#pragma unroll
+    for (int i = 0; i < DC; ++i) zq[i] = 0.0;
+    for (int t = 0; t < nt; ++t) {
+      const size_t o = (size_t)s * N + n0 + t;
+      const bool valid = frame_ok && mask[o] != 0;
+      if (!__any_sync(0xffffffffu, valid)) continue;
+      const float2 ob = frame_ok ? uv2[o] : make_float2(0.f, 0.f);
+      const double* pt = s_pt[t];
+      const double* m = pt + 4;                    // M upper triangular (row-major), then q
+      double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry;
+      obs_math<MODEL>(pw + lane, 32, pt[0], pt[1], pt[2], pt[3] != 0.0, ob.x, ob.y, valid, jc0, jc1, jx0, jx1, rx, ry);
+#pragma unroll
+      for (int i = 0; i < DC; ++i) {
+        const double w0 = w_entry(jc0, jc1, jx0, jx1, i, 0), w1 = w_entry(jc0, jc1, jx0, jx1, i, 1),
+                     w2 = w_entry(jc0, jc1, jx0, jx1, i, 2);
+        const double z0 = w0 * m[0];
+        const double z1 = w0 * m[1] + w1 * m[4];
+        const double z2 = w0 * m[2] + w1 * m[5] + w2 * m[8];
+        zs[lane * DC + i] = z0;
+        zs[ZR + lane * DC + i] = z1;
+        zs[2 * ZR + lane * DC + i] = z2;
+        zq[i] += z0 * m[9] + z1 * m[10] + z2 * m[11];
+      }
+      if (NS > 0) {
+        double a[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) a[k] = k < 3 * NS ? w_entry(jc0, jc1, jx0, jx1, 6 + k / 3, k % 3) : 0.0;
+        const double r = warp_reduce_scatter<8>(a, lane);
+        if (lane < 3 * NS) s_ws[warp][t][lane] += r;
+      }
+      __syncwarp();
+      double* dst = Zt + (size_t)(3 * (n0 + t)) * Dpad + (size_t)g * ZR;
+#pragma unroll
+      for (int c = 0; c < 3; ++c, dst += Dpad) {
+        const double* src = zs + c * ZR;
+        for (int e = 2 * lane; e + 1 < cnt; e += 64)
+          *reinterpret_cast<double2*>(dst + e) = *reinterpret_cast<const double2*>(src + e);
+        if ((cnt & 1) && lane == 0) dst[cnt - 1] = src[cnt - 1];
+      }
+      __syncwarp();
+    }
+    if (frame_ok) {
+#pragma unroll
+      for (int i = 0; i < DC; ++i) {
+        double* r = &rhs[(size_t)s * DC + i];
+        if (zq[i] != 0.0) ar_add(r, mc_off ? r + mc_off : nullptr, zq[i]);
+      }
+    }
   }
-  if (zq != 0.0) ar_add(&rhs[row], mc_off ? &rhs[row] + mc_off : nullptr, zq);
+  if (NS > 0) {
+    __syncthreads();
+    if ((int)threadIdx.x < nt * NS) {
+      const int t = threadIdx.x / NS, j = threadIdx.x % NS;
+      double w[3];
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        w[c] = 0.0;
+#pragma unroll
+        for (int v = 0; v < ZB_W; ++v) w[c] += s_ws[v][t][j * 3 + c];
+      }
+      const double* m = s_pt[t] + 4;
+      const double z0 = w[0] * m[0];
+      const double z1 = w[0] * m[1] + w[1] * m[4];
+      const double z2 = w[0] * m[2] + w[1] * m[5] + w[2] * m[8];
+      double* zo = Zt + (size_t)(3 * (n0 + t)) * Dpad + (size_t)S * DC + j;
+      zo[0] = z0;
+      zo[Dpad] = z1;
+      zo[2 * (size_t)Dpad] = z2;
+      const double zq = z0 * m[9] + z1 * m[10] + z2 * m[11];
+      double* r = &rhs[(size_t)S * DC + j];
+      if (zq != 0.0) ar_add(r, mc_off ? r + mc_off : nullptr, zq);
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -370,38 +459,72 @@ __global__ void cam_step_kernel(int D, const double* __restrict__ dcs, size_t dc
   }
 }
 
-// wacc[n][c] = sum_row W[n][row][c] d_c[row]: one warp per track, lanes stride over the contiguous rows
-__global__ void __launch_bounds__(256) backsub_kernel(int D, int N, size_t pitch, const double* __restrict__ W,
-                                                      const double* __restrict__ d_c, double* __restrict__ wacc,
-                                                      const int* __restrict__ kb_rows, int arrow_row) {
-  const int lane = threadIdx.x & 31;
-  const int n = blockIdx.x * 8 + (threadIdx.x >> 5);
-  if (n >= N) return;
-  const double* wp = W + (size_t)n * pitch * 3;
-  double w0 = 0, w1 = 0, w2 = 0;
-  auto span = [&](int r0, int r1) {
-#pragma unroll 4
-    for (int r = r0 + lane; r < r1; r += 32) {
-      const double d = __ldg(d_c + r);
-      w0 = fma(wp[(size_t)r * 3], d, w0);
-      w1 = fma(wp[(size_t)r * 3 + 1], d, w1);
-      w2 = fma(wp[(size_t)r * 3 + 2], d, w2);
-    }
-  };
-  if (kb_rows) {
-    // banded problems: the rows this point can touch (its two k-blocks' row ranges) and the dense arrow
-    const int ka = (3 * n) >> 6, kb = (3 * n + 2) >> 6;
-    const int lo = min(kb_rows[2 * ka], kb_rows[2 * kb]), hi = min(max(kb_rows[2 * ka + 1], kb_rows[2 * kb + 1]), arrow_row);
-    if (lo < hi) span(lo, hi);
-    span(min(arrow_row, D), D);
-  } else {
-    span(0, D);
+// wacc[n] = W_n^T d_c = sum_s J_p,sn^T (J_c,sn d_c,s + J_intr,sn d_shared), each block rebuilt from its observation
+// (obs_math, ba_obs.h).  One lane per track, so the observation loads are coalesced and the sum stays in the lane; the
+// warps of a CTA take the frames in turn (a frame's camera and step are broadcasts) and add up at the end.  Frames in
+// which none of the CTA's tracks is visible (band skip of sequential problems, or all masked) are passed over.
+constexpr int BS_W = 16;     // warps per CTA
+template <int MODEL, int MODE>
+__global__ void __launch_bounds__(BS_W * 32) backsub_kernel(
+    int S, int N, const float* __restrict__ uv, const uint8_t* __restrict__ mask, const double* __restrict__ poses,
+    const double* __restrict__ intr, const double* __restrict__ points, const uint8_t* __restrict__ point_const,
+    const double* __restrict__ d_c, double* __restrict__ wacc, const int* __restrict__ fg_tracks) {
+  using C = BlkCfg<MODEL, MODE>;
+  constexpr int DC = C::DC, NS = C::NS;
+  __shared__ double s_cam[BS_W][16];
+  __shared__ double s_acc[3][BS_W][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  const int nlo = blockIdx.x * 32, nhi = min(N, nlo + 32);
+  const int n = nlo + lane;
+  const bool track_ok = n < N;
+  double X0 = 0.0, X1 = 0.0, X2 = 0.0;
+  bool pc = true;
+  if (track_ok) {
+    X0 = points[(size_t)n * 3]; X1 = points[(size_t)n * 3 + 1]; X2 = points[(size_t)n * 3 + 2];
+    pc = point_const && point_const[n] != 0;
   }
-  w0 = warp_sum(w0); w1 = warp_sum(w1); w2 = warp_sum(w2);
-  if (lane == 0) {
-    wacc[(size_t)n * 3] = w0;
-    wacc[(size_t)n * 3 + 1] = w1;
-    wacc[(size_t)n * 3 + 2] = w2;
+  double dsh[2] = {0.0, 0.0};
+#pragma unroll
+  for (int j = 0; j < NS; ++j) dsh[j] = d_c[(size_t)S * DC + j];
+  const float2* uv2 = reinterpret_cast<const float2*>(uv);
+  double* cam = s_cam[warp];
+  double w0 = 0.0, w1 = 0.0, w2 = 0.0;
+  for (int s = warp; s < S; s += nw) {
+    if (fg_tracks && (nhi <= fg_tracks[2 * (s >> 5)] || nlo >= fg_tracks[2 * (s >> 5) + 1])) continue;
+    const size_t o = (size_t)s * N + n;
+    const bool valid = track_ok && mask[o] != 0;
+    if (!__any_sync(0xffffffffu, valid)) continue;
+    const float2 ob = valid ? uv2[o] : make_float2(0.f, 0.f);
+    __syncwarp();
+    if (lane < 16) cam[lane] = lane < 12 ? poses[(size_t)s * 12 + lane] : intr[(size_t)s * 4 + (lane - 12)];
+    __syncwarp();
+    double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry;
+    obs_math<MODEL>(cam, 1, X0, X1, X2, pc, ob.x, ob.y, valid, jc0, jc1, jx0, jx1, rx, ry);
+    const double* d = d_c + (size_t)s * DC;
+#pragma unroll
+    for (int i = 0; i < DC; ++i) {
+      const double di = __ldg(d + i);
+      w0 = fma(w_entry(jc0, jc1, jx0, jx1, i, 0), di, w0);
+      w1 = fma(w_entry(jc0, jc1, jx0, jx1, i, 1), di, w1);
+      w2 = fma(w_entry(jc0, jc1, jx0, jx1, i, 2), di, w2);
+    }
+#pragma unroll
+    for (int j = 0; j < NS; ++j) {
+      w0 = fma(w_entry(jc0, jc1, jx0, jx1, 6 + j, 0), dsh[j], w0);
+      w1 = fma(w_entry(jc0, jc1, jx0, jx1, 6 + j, 1), dsh[j], w1);
+      w2 = fma(w_entry(jc0, jc1, jx0, jx1, 6 + j, 2), dsh[j], w2);
+    }
+  }
+  s_acc[0][warp][lane] = w0;
+  s_acc[1][warp][lane] = w1;
+  s_acc[2][warp][lane] = w2;
+  __syncthreads();
+  // 3 x 32 sums; a CTA of fewer than three warps (S < 3) takes several
+  for (int e = threadIdx.x; e < 96; e += blockDim.x) {
+    const int c = e >> 5, t = e & 31;
+    double r = 0.0;
+    for (int v = 0; v < nw; ++v) r += s_acc[c][v][t];
+    if (nlo + t < N) wacc[(size_t)(nlo + t) * 3 + c] = r;
   }
 }
 
@@ -545,11 +668,25 @@ int launch_assemble_hc(int S, int dc, int ns, int KR, int Dpad, const double* ca
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
-int launch_z_transpose(int D, int N, int Dpad, const double* W, const double* M, const double* q, double* Zt,
-                       double* rhs, ptrdiff_t mc_off, const int* rb_range, cudaStream_t st) {
-  const size_t pitch = (size_t)(D + (D & 1));
-  dim3 grid((D + 127) / 128, (N + ZB_NT - 1) / ZB_NT);
-  z_build_kernel<<<grid, 128, 0, st>>>(D, N, Dpad, pitch, W, M, q, Zt, rhs, mc_off, rb_range);
+// the instantiation of a bundle-adjustment kernel template for the problem's camera model and intrinsics mode
+#define VGG_PICK_BA_KERNEL(kern, tmpl, p)                 \
+  decltype(&tmpl<0, 0>) kern = nullptr;                   \
+  switch ((p)->camera_model * 3 + (p)->intr_mode) {       \
+    case 0: kern = tmpl<0, 0>; break;                     \
+    case 1: kern = tmpl<0, 1>; break;                     \
+    case 2: kern = tmpl<0, 2>; break;                     \
+    case 3: kern = tmpl<1, 0>; break;                     \
+    case 4: kern = tmpl<1, 1>; break;                     \
+    case 5: kern = tmpl<1, 2>; break;                     \
+  }                                                       \
+  VGG_REQUIRE(kern, "bad camera_model/intr_mode")
+
+int launch_z_build(const vgg_ba_problem* p, int Dpad, const double* M, const double* q, double* Zt, double* rhs,
+                   ptrdiff_t mc_off, const int* fg_tracks, cudaStream_t st) {
+  VGG_PICK_BA_KERNEL(kern, z_build_kernel, p);
+  const int nw = std::min(ZB_W, (p->S + 31) / 32);
+  kern<<<(p->N + ZB_NT - 1) / ZB_NT, nw * 32, 0, st>>>(p->S, p->N, Dpad, p->uv, p->mask, p->poses, p->intr, p->points,
+                                                        p->point_const, M, q, Zt, rhs, mc_off, fg_tracks);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
@@ -619,10 +756,11 @@ int launch_cam_step(int D, const double* dcs, size_t dcs_stride, const double* s
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
-int launch_backsub(int D, int N, const double* W, const double* d_c, double* wacc, const int* kb_rows, int arrow_row,
-                   cudaStream_t st) {
-  const size_t pitch = (size_t)(D + (D & 1));
-  backsub_kernel<<<(N + 7) / 8, 256, 0, st>>>(D, N, pitch, W, d_c, wacc, kb_rows, arrow_row);
+int launch_backsub(const vgg_ba_problem* p, const double* d_c, double* wacc, const int* fg_tracks, cudaStream_t st) {
+  VGG_PICK_BA_KERNEL(kern, backsub_kernel, p);
+  const int nw = std::min(BS_W, p->S);
+  kern<<<(p->N + 31) / 32, nw * 32, 0, st>>>(p->S, p->N, p->uv, p->mask, p->poses, p->intr, p->points, p->point_const,
+                                             d_c, wacc, fg_tracks);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }

@@ -33,8 +33,8 @@ int launch_point_prep(int N, const double* H_pp, const double* g_p, const double
                       double* scal, cudaStream_t st);
 int launch_assemble_hc(int S, int dc, int ns, int KR, int Dpad, const double* camrec, const double* shared_in,
                        double* Sraw, double* rhs, double* hdiag, double* gvec, ptrdiff_t mc_off, cudaStream_t st);
-int launch_z_transpose(int D, int N, int Dpad, const double* W, const double* M, const double* q, double* Zt,
-                       double* rhs, ptrdiff_t mc_off, const int* rb_range, cudaStream_t st);
+int launch_z_build(const vgg_ba_problem* p, int Dpad, const double* M, const double* q, double* Zt, double* rhs,
+                   ptrdiff_t mc_off, const int* fg_tracks, cudaStream_t st);
 int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc_off, const std::vector<int>& kb_ranges,
                 const FabricDev& fd, cudaStream_t st);
 int launch_scale_damp(int D, int Dpad, double* A, const double* rhs, const double* hdiag, const double* sc,
@@ -43,8 +43,7 @@ int launch_scale_damp(int D, int Dpad, double* A, const double* rhs, const doubl
 int launch_cam_step(int D, const double* dcs, size_t dcs_stride, const double* sc, const double* hdiag, const double* gvec,
                     const uint8_t* pconst, double radius, double min_diag, double max_diag, double* d_c, double* scal,
                     cudaStream_t st);
-int launch_backsub(int D, int N, const double* W, const double* d_c, double* wacc, const int* kb_rows, int arrow_row,
-                   cudaStream_t st);
+int launch_backsub(const vgg_ba_problem* p, const double* d_c, double* wacc, const int* fg_tracks, cudaStream_t st);
 int launch_point_step(int N, const double* M, const double* g_p, const double* wacc, const double* sc_p,
                       const double* dpp, const double* X, double radius, double* Xc, double* scal, cudaStream_t st);
 int launch_cam_update(int S, int dc, int ns, int model, const double* d_c, const double* poses, const double* intr,
@@ -158,8 +157,10 @@ static int dims_of(int model, int mode, int* dc, int* ns, int* KR) {
 // ------------------------------------------------------------------------------------------------
 // workspace layout
 // ------------------------------------------------------------------------------------------------
+// Accumulators of one evaluation.  The coupling blocks W are not among them: z_build and backsub rebuild each one from
+// its observation (csrc/ba_obs.h).
 struct BlockSet {
-  double *cost, *camrec, *g_p, *H_pp, *W, *shared;
+  double *cost, *camrec, *g_p, *H_pp, *shared;
 };
 struct Layout {
   int S, N, dc, ns, KR, D, Dpad, Kpad;
@@ -192,7 +193,6 @@ static int make_layout(int S, int N, int model, int mode, void* base, size_t cap
     L->blk[b].camrec = c.take<double>((size_t)S * KR);
     L->blk[b].g_p = c.take<double>((size_t)N * 3);
     L->blk[b].H_pp = c.take<double>((size_t)N * 6);
-    L->blk[b].W = c.take<double>((size_t)(L->D + (L->D & 1)) * N * 3);   // track-major [N][pitch][3]
     L->poses[b] = c.take<double>((size_t)S * 12);
     L->intr[b] = c.take<double>((size_t)S * 4);
     L->points[b] = c.take<double>((size_t)N * 3);
@@ -270,11 +270,12 @@ struct Fabric {
 // The band structure of one solve (compute_band_hint), passed to the launchers that use it; empty / null = dense.
 //   kb_ranges             SYRK k-block range per 128-column row block of Zt (launch_syrk)
 //   end_blk, arrow_blk    block structure of the reduced system (chol_lower_inplace)
-//   dev                   device tables for ba_blocks / z_build / backsub; kb_rows, fg_tracks: host copies of two of them
+//   dev                   device table for ba_blocks / z_build / backsub (fg_tracks, also kept on the host)
+//   kb_rows               reduced-system row range per k-block (vgg_dev_last_band_hint only)
 struct BandPlan {
   int nb = 0, KB = 0, ngroups = 0, arrow_blk = 0;
   std::vector<int> kb_ranges, end_blk, kb_rows, fg_tracks;
-  BandDev dev{nullptr, nullptr, nullptr, 0};
+  BandDev dev{nullptr};
 };
 // the plan of the most recent solve on this thread (vgg_dev_last_band_hint): the tests compare it with
 // oracle/band_oracle.py
@@ -387,13 +388,10 @@ static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad
       }
       plan->end_blk = end;
       plan->arrow_blk = arrow;
-      // device tables for the kernels that walk the dense [frames, points] grid
+      // the per-k-block row ranges (reported by vgg_dev_last_band_hint) and the per-frame-group track ranges, the device
+      // table of the kernels that walk the dense [frames, points] grid
       const int ngroups = (S + 31) / 32;
-      std::vector<int> tab(2 * (size_t)(nb + KB + ngroups), 0);
-      int* t_rb = tab.data();
-      int* t_kb = t_rb + 2 * nb;
-      int* t_fg = t_kb + 2 * KB;
-      for (int i = 0; i < 2 * nb; ++i) t_rb[i] = rg[i];
+      std::vector<int> t_kb(2 * (size_t)KB, 0), t_fg(2 * (size_t)ngroups, 0);
       for (int kb = 0; kb < KB; ++kb) {
         int first = -1, last = -1;
         for (int rb = 0; rb < arrow; ++rb)
@@ -416,39 +414,40 @@ static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad
       }
       static thread_local int* tdev = nullptr;
       static thread_local size_t tcap = 0;
-      if (tcap < tab.size()) {
+      if (tcap < t_fg.size()) {
         if (tdev) cudaFree(tdev);
-        VGG_CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&tdev), sizeof(int) * tab.size()));
-        tcap = tab.size();
+        VGG_CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&tdev), sizeof(int) * t_fg.size()));
+        tcap = t_fg.size();
       }
-      VGG_CUDA_CHECK(cudaMemcpyAsync(tdev, tab.data(), sizeof(int) * tab.size(), cudaMemcpyHostToDevice, st));
+      VGG_CUDA_CHECK(cudaMemcpyAsync(tdev, t_fg.data(), sizeof(int) * t_fg.size(), cudaMemcpyHostToDevice, st));
       VGG_CUDA_CHECK(cudaStreamSynchronize(st));           // pageable source
-      plan->dev = BandDev{tdev, tdev + 2 * nb, tdev + 2 * (nb + KB), arrow * 128};
-      plan->kb_rows.assign(t_kb, t_kb + 2 * KB);
-      plan->fg_tracks.assign(t_fg, t_fg + 2 * ngroups);
+      plan->dev = BandDev{tdev};
+      plan->kb_rows = t_kb;
+      plan->fg_tracks = t_fg;
     }
   }
   return VGG_OK;
 }
 
-// Schur complement of blk onto AR (Sraw, rhs, hdiag, gvec) at the given radius; fd: where the SYRK epilogue sends each
-// row block in a fabric solve, fab: that solve's fabric (null otherwise)
-static int schur_build(const Layout& L, const BlockSet& b, const BandPlan& band, const FabricDev& fd,
-                       const uint8_t* point_const, double radius, double min_diag, double max_diag, cudaStream_t st,
+// Schur complement of blk onto AR (Sraw, rhs, hdiag, gvec) at the given radius; p: the problem at the state blk was
+// evaluated at (z_build rebuilds the coupling blocks from it); fd: where the SYRK epilogue sends each row block in a
+// fabric solve, fab: that solve's fabric (null otherwise)
+static int schur_build(const Layout& L, const vgg_ba_problem& p, const BlockSet& b, const BandPlan& band,
+                       const FabricDev& fd, double radius, double min_diag, double max_diag, cudaStream_t st,
                        ptrdiff_t mc_off = 0, Fabric* fab = nullptr) {
   int rc;
   double* Sraw = L.AR;
   double* rhs = L.AR + (size_t)L.D * L.Dpad;
   double* hdiag = rhs + L.Dpad;
   double* gvec = hdiag + L.Dpad;
-  if ((rc = launch_point_prep(L.N, b.H_pp, b.g_p, L.sc_p, point_const, radius, min_diag, max_diag, L.M, L.q, L.dpp,
+  if ((rc = launch_point_prep(L.N, b.H_pp, b.g_p, L.sc_p, p.point_const, radius, min_diag, max_diag, L.M, L.q, L.dpp,
                               L.scal, st)))
     return rc;
   VGG_CUDA_CHECK(cudaMemsetAsync(L.AR, 0, sizeof(double) * ((size_t)L.D * L.Dpad + 3 * (size_t)L.Dpad), st));
   // fabric mode: every rank's copy must be zero before anyone's reductions land in it
   if (fab && (rc = fab->barrier(st))) return rc;
   if ((rc = launch_assemble_hc(L.S, L.dc, L.ns, L.KR, L.Dpad, b.camrec, b.shared, Sraw, rhs, hdiag, gvec, mc_off, st))) return rc;
-  if ((rc = launch_z_transpose(L.D, L.N, L.Dpad, b.W, L.M, L.q, L.Zt, rhs, mc_off, band.dev.rb_range, st))) return rc;
+  if ((rc = launch_z_build(&p, L.Dpad, L.M, L.q, L.Zt, rhs, mc_off, band.dev.fg_tracks, st))) return rc;
   if ((rc = launch_syrk(L.Kpad, L.Dpad, L.Zt, Sraw, mc_off, band.kb_ranges, fd, st))) return rc;
   // ... and all reductions must have landed before anyone reads its copy
   if (fab && (rc = fab->barrier(st))) return rc;
@@ -509,7 +508,7 @@ int vgg_ba_build_blocks(const vgg_ba_problem* prob, double* cost, double* camrec
 }
 
 int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double* g_p, const double* H_pp,
-                 const double* W, const double* shared_in, const double* scale_p, double radius, double min_diag,
+                 const double* shared_in, const double* scale_p, double radius, double min_diag,
                  double max_diag, void* workspace, size_t ws_bytes, double* Sraw, double* rhs, int* Dpad_out,
                  void* stream) {
   VGG_REQUIRE(prob && workspace && Sraw && rhs, "null pointer");
@@ -523,12 +522,11 @@ int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double*
   b.camrec = const_cast<double*>(camrec);
   b.g_p = const_cast<double*>(g_p);
   b.H_pp = const_cast<double*>(H_pp);
-  b.W = const_cast<double*>(W);
   b.shared = const_cast<double*>(shared_in);
   VGG_CUDA_CHECK(cudaMemcpyAsync(L.sc_p, scale_p, sizeof(double) * (size_t)L.N * 3, cudaMemcpyDeviceToDevice, st));
   VGG_CUDA_CHECK(cudaMemsetAsync(L.Zt, 0, sizeof(double) * (size_t)L.Kpad * L.Dpad, st));
   VGG_CUDA_CHECK(cudaMemsetAsync(L.scal, 0, sizeof(double) * 16, st));
-  rc = schur_build(L, b, BandPlan{}, FabricDev{}, prob->point_const, radius, min_diag, max_diag, st);
+  rc = schur_build(L, *prob, b, BandPlan{}, FabricDev{}, radius, min_diag, max_diag, st);
   if (rc) return rc;
   VGG_CUDA_CHECK(cudaMemcpyAsync(Sraw, L.AR, sizeof(double) * (size_t)L.D * L.Dpad, cudaMemcpyDeviceToDevice, st));
   VGG_CUDA_CHECK(cudaMemcpyAsync(rhs, L.AR + (size_t)L.D * L.Dpad, sizeof(double) * L.Dpad, cudaMemcpyDeviceToDevice, st));
@@ -635,12 +633,6 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
   BandPlan band;
   if ((rc = compute_band_hint(prob, dc, D, L.Dpad, L.Kpad, allreduce != nullptr || fabric != nullptr, st, &band))) return rc;
   g_band_last = band;
-  if (band.dev.fg_tracks) {
-    // the kernels skip the (track chunk, frame group) regions no observation falls into: their W blocks must read as zero
-    const size_t w_doubles = (size_t)N * (size_t)(D + (D & 1)) * 3;
-    VGG_CUDA_CHECK(cudaMemsetAsync(L.blk[0].W, 0, sizeof(double) * w_doubles, st));
-    VGG_CUDA_CHECK(cudaMemsetAsync(L.blk[1].W, 0, sizeof(double) * w_doubles, st));
-  }
   double* Sraw = L.AR;
   double* rhs = L.AR + (size_t)D * L.Dpad;
   double* hdiag = rhs + L.Dpad;
@@ -665,16 +657,21 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
   VGG_CUDA_CHECK(cudaMemsetAsync(L.Zt, 0, sizeof(double) * (size_t)L.Kpad * L.Dpad, st));
   VGG_CUDA_CHECK(cudaMemsetAsync(L.d_c, 0, sizeof(double) * L.Dpad, st));
 
-  auto eval = [&](int which) -> int {
+  // the problem at state `which` (buffer set of the current state or the candidate)
+  auto state = [&](int which) {
     vgg_ba_problem p = *prob;
     p.poses = L.poses[which];
     p.intr = L.intr[which];
     p.points = L.points[which];
+    return p;
+  };
+  auto eval = [&](int which) -> int {
+    const vgg_ba_problem p = state(which);
     const BlockSet& b = L.blk[which];
     // cost | shared | camrec | g_p | H_pp are carved back to back: one memset covers all accumulators
     const size_t acc_bytes = reinterpret_cast<char*>(b.H_pp + (size_t)N * 6) - reinterpret_cast<char*>(b.cost);
     VGG_CUDA_CHECK(cudaMemsetAsync(b.cost, 0, acc_bytes, st));
-    return ba_build_blocks(&p, b.cost, b.camrec, b.g_p, b.H_pp, b.W, b.shared, 0, band.dev.fg_tracks, st, true);
+    return ba_build_blocks(&p, b.cost, b.camrec, b.g_p, b.H_pp, nullptr, b.shared, 0, band.dev.fg_tracks, st, true);
   };
   // global cost + gradient max-norm of block set `which`; result lands in host h[0..2] = cost, gmax_c, gmax_p
   double* h_scal = pinned_scalars();
@@ -745,8 +742,9 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
       gvec = hdiag + L.Dpad;
       fd = fab.at(off);
     }
-    if ((rc = schur_build(L, L.blk[cur], band, fd, prob->point_const, radius, opt.min_lm_diagonal, opt.max_lm_diagonal, st,
-                          mc_off, fab.on ? &fab : nullptr)))
+    const vgg_ba_problem pcur = state(cur);
+    if ((rc = schur_build(L, pcur, L.blk[cur], band, fd, radius, opt.min_lm_diagonal, opt.max_lm_diagonal, st, mc_off,
+                          fab.on ? &fab : nullptr)))
       return rc;
     // every row block is complete on its owner: pull the others (matrix rows 0..D incl. the rhs row, then hdiag, gvec)
     if (fab.on && (rc = launch_fabric_gather(fd, D + 3, D + 1, D, L.Dpad, st))) return rc;
@@ -790,7 +788,7 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     if ((rc = launch_cam_step(D, dcs, dcs_stride, L.sc_c, hdiag, gvec, prob->param_const, radius, opt.min_lm_diagonal,
                               opt.max_lm_diagonal, L.d_c, L.scal, st)))
       return rc;
-    if ((rc = launch_backsub(D, N, L.blk[cur].W, L.d_c, L.wacc, band.dev.kb_rows, band.dev.arrow_row, st))) return rc;
+    if ((rc = launch_backsub(&pcur, L.d_c, L.wacc, band.dev.fg_tracks, st))) return rc;
     if ((rc = launch_point_step(N, L.M, L.blk[cur].g_p, L.wacc, L.sc_p, L.dpp, L.points[cur], radius, L.points[cand],
                                 L.scal, st)))
       return rc;

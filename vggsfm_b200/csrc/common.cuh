@@ -51,16 +51,11 @@ struct Carver {
   bool ok() const { return base == nullptr || off <= cap; }
 };
 
-// Band structure of a sequential (video) problem on the device (csrc/ba_solve.cu, compute_band_hint); all pointers
-// null = dense.  Points are stored in creation order, so every range is contiguous.
-//   rb_range[2 rb]  .. [2 rb + 1]   64-row k-block range of Zt outside which 128-column row block rb is zero
-//   kb_rows[2 kb]   .. [2 kb + 1]   reduced-system row range [lo, hi) that the points of k-block kb can touch (band part)
+// Band structure of a sequential (video) problem on the device (csrc/ba_solve.cu, compute_band_hint); null = dense.
+// Points are stored in creation order, so every range is contiguous.
 //   fg_tracks[2 g]  .. [2 g + 1]    track range [lo, hi) visible to the 32-frame group g
 struct BandDev {
-  const int* rb_range;
-  const int* kb_rows;
   const int* fg_tracks;
-  int arrow_row;                     // first row of the dense arrow (shared intrinsics ...): always processed
 };
 
 // Destination table of the fused multi-GPU reduction (csrc/fabric.cu): world <= 1 means "not in use".
