@@ -326,7 +326,9 @@ int vgg_corr_build_pyramid(int BS, int C, int H, int W, int num_levels, const fl
 
 /* CorrBlock.corr + CorrBlock.sample fused (blocks.py:363-416; border_padding=1 gives
  * EfficientCorrBlock.sample, :433-471).  targets float [BS,N,C], coords float [BS,N,2] (x,y) in level-0
- * pixels, out float [BS,N,num_levels*(2r+1)^2] with out[a*(2r+1)+b] sampled at (x+a-r, y+b-r). */
+ * pixels, out float [BS,N,num_levels*(2r+1)^2] with out[a*(2r+1)+b] sampled at (x+a-r, y+b-r).  Coordinates follow
+ * grid_sample on CUDA: a NaN or ±inf coordinate reads 0 with zero padding; border padding clamps it (NaN -> 0).
+ * BS * N == 0 returns VGG_OK without a launch, and the pointers may then be null (also for vgg_corr_tc_sample). */
 int vgg_corr_sample(int BS, int N, int C, int H, int W, int num_levels, int radius, const void* pyramid, int elem_size,
                     const float* targets, const float* coords, int border_padding, float* out, void* stream);
 

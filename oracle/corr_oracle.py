@@ -10,6 +10,8 @@ PINNED against the reference through tests/golden/corr_*.npz (tools/make_golden_
 corr_reference is the float64 statement the CUDA kernels are checked against: it takes the pyramid levels and targets
 already rounded to the kernel's precision (kernel_pyramid rebuilds the kernels' pyramid bit for bit), and returns with
 every output the same bilinear combination of sum_c |t_c f_c| / sqrt(C), the scale of the kernel's rounding error.
+sample_features4d_reference is the float64 statement of sample_features4d, with the same kind of bound.  Both follow
+grid_sample's coordinate rule on CUDA for non-finite and far-away coordinates (_source_coordinate).
 """
 import math
 
@@ -28,12 +30,23 @@ def build_pyramid(fmaps, num_levels):
     return pyr
 
 
+def _source_coordinate(x, size, border):
+    """grid_sample's coordinate rule on CUDA (ATen/native/cuda/GridSampler.cuh compute_coordinates): border padding clips
+    with fmaxf semantics (NaN -> 0, -inf -> 0, +inf -> size - 1); then a non-finite coordinate, or one beyond INT_MAX - 1
+    or below INT_MIN, becomes -100 (safe_downgrade_to_int_range), outside the map, so with zeros padding it contributes
+    nothing.  CPU grid_sample, and on CUDA the cuDNN sampler that torch uses by default for zeros / bilinear /
+    align_corners=True, return NaN at a NaN coordinate with zeros padding; ATen's CUDA kernel is the rule here."""
+    if border:
+        x = torch.nan_to_num(x, nan=0.0, posinf=float(size - 1), neginf=0.0).clamp(0, size - 1)
+    bad = ~torch.isfinite(x) | (x > 2.0 ** 31 - 2) | (x < -2.0 ** 31)
+    return torch.where(bad, torch.full_like(x, -100.0), x)
+
+
 def _bilinear_gather(vol, x, y, border):
     """vol [Q,H,W,...]; x,y [Q,T] pixel coords -> [Q,T,...]."""
     Q, H, W = vol.shape[:3]
-    if border:
-        x = x.clamp(0, W - 1)
-        y = y.clamp(0, H - 1)
+    x = _source_coordinate(x, W, border)
+    y = _source_coordinate(y, H, border)
     x0 = torch.floor(x)
     y0 = torch.floor(y)
     wx = x - x0
@@ -166,4 +179,34 @@ def corr_reference(levels, targets, coords, radius, border=False, frames=4):
             g = _bilinear_gather(vol.reshape(-1, H, W, 2), x, y, border).reshape(B, s1 - s0, N, K * K, 2)
             out[:, s0:s1, :, i * K * K:(i + 1) * K * K] = g[..., 0]
             bound[:, s0:s1, :, i * K * K:(i + 1) * K * K] = g[..., 1]
+    return out, bound
+
+
+def sample_features4d_reference(inp, coords):
+    """float64 sample_features4d (models/utils.py:415-447: bilinear_sampler, align_corners=True, border padding):
+    inp [B,C,H,W], coords [B,R,2] (x, y) float32, on one device -> (out, bound) [B,R,C] float64.  The sample position is
+    the reference's float32 round trip, x * float32(2 / max(W - 1, 1)) - 1, then ((g + 1) / 2) * (W - 1), each step
+    rounded; it is clipped by grid_sample's CUDA rule (_source_coordinate) and interpolated in float64.
+    bound = sum_i w_i |v_i|, the scale of a float32 kernel's rounding error."""
+    B, C, H, W = inp.shape
+    c = coords.float()
+    pos = []
+    for k, size in ((0, W), (1, H)):
+        s = torch.tensor(2 / max(size - 1, 1), dtype=torch.float32, device=c.device)
+        g = c[..., k] * s - 1
+        pos.append(_source_coordinate((((g + 1) / 2) * (size - 1)).double(), size, True))
+    x, y = pos
+    x0, y0 = torch.floor(x), torch.floor(y)
+    wx, wy = (x - x0)[..., None], (y - y0)[..., None]
+    x0, y0 = x0.long(), y0.long()
+    x1, y1 = (x0 + 1).clamp(max=W - 1), (y0 + 1).clamp(max=H - 1)
+    v = inp.double().permute(0, 2, 3, 1)
+    bi = torch.arange(B, device=inp.device)[:, None]
+    out = torch.zeros(B, x.shape[1], C, dtype=torch.float64, device=inp.device)
+    bound = torch.zeros_like(out)
+    for yi, wyv in ((y0, 1 - wy), (y1, wy)):
+        for xi, wxv in ((x0, 1 - wx), (x1, wx)):
+            t = v[bi, yi, xi]
+            out = out + wxv * wyv * t
+            bound = bound + wxv * wyv * t.abs()
     return out, bound

@@ -61,6 +61,8 @@ class _Pyramid:
         r = self.radius
         K = 2 * r + 1
         out = torch.empty(B, S, N, self.num_levels * K * K, dtype=torch.float32, device=self.dev)
+        if out.numel() == 0:                # no query (N = 0): the reference returns the empty [B,S,0,L*K*K] tensor
+            return out
         tg = targets.float().contiguous()
         co = coords.float().contiguous()
         if self.tc_tiles is not None and not border:

@@ -65,6 +65,16 @@ struct FabricDev {
 };
 
 #ifdef __CUDACC__
+// Correlation sampling (csrc/corr.cu, csrc/corr_tc.cu): a query's coordinate on a level of `size` positions, clamped
+// into [-(R+2), size+R+1] before its footprint origin (int)floorf(c) is formed.  Inside that window the clamp is the
+// identity.  Beyond it every tap c + d (|d| <= R) lies outside the map either way, so zeros padding still reads only
+// zeros and border padding still reads the clamped edge.  NaN goes to the low end (fmaxf): 0 with zeros padding and
+// column / row 0 with border padding, which is what grid_sample on CUDA returns for a NaN tap.  The int conversion and
+// the footprint arithmetic on it are then defined for every input, ±inf and |c| >= 2^31 included.
+__device__ __forceinline__ float corr_window(float c, int R, int size) {
+  return fminf(fmaxf(c, -(float)(R + 2)), (float)(size + R + 1));
+}
+
 // ---------------------------------------------------------------------------------------------
 // TMA 1-D bulk copies + mbarrier (PTX ISA 8.x, sm_90+; SASS: UBLKCP / SYNCS)
 // ---------------------------------------------------------------------------------------------

@@ -116,8 +116,9 @@ __global__ void __launch_bounds__(256) corr_sample_kernel(int BS, int N, int L, 
     const int H = lv.H[l], W = lv.W[l];
     const T* fm = reinterpret_cast<const T*>(lv.fmap[l]) + img * (size_t)H * W * C;
     const float scale = 1.0f / (float)(1 << l);
-    // reference: coords/2^l + delta, then x*(2/(W-1)) - 1 and grid_sample's un-normalisation ((x+1)/2*(W-1))
-    const float cx = cx0 * scale, cy = cy0 * scale;
+    // reference: coords/2^l + delta, then x*(2/(W-1)) - 1 and grid_sample's un-normalisation ((x+1)/2*(W-1));
+    // non-finite and far-away coordinates: corr_window (common.cuh)
+    const float cx = corr_window(cx0 * scale, R, W), cy = corr_window(cy0 * scale, R, H);
     const float fxf = floorf(cx), fyf = floorf(cy);
     const int fx = (int)fxf, fy = (int)fyf;
     // Every footprint position is loaded UNCONDITIONALLY from a clamped address and masked afterwards: the loads of a
@@ -265,7 +266,7 @@ __global__ void __launch_bounds__(256, 4) corr_sample_c32_kernel(int BS, int N, 
     const int H = lv.H[l], W = lv.W[l];
     const T* fm = reinterpret_cast<const T*>(lv.fmap[l]) + img * (size_t)H * W * C;
     const float scale = 1.0f / (float)(1 << l);
-    const float cx = cx0 * scale, cy = cy0 * scale;
+    const float cx = corr_window(cx0 * scale, R, W), cy = corr_window(cy0 * scale, R, H);
     const float fxf = floorf(cx), fyf = floorf(cy);
     const int fx = (int)fxf, fy = (int)fyf;
 #pragma unroll
@@ -354,10 +355,11 @@ __global__ void sample_features_kernel(int B, int C, int H, int W, int R, const 
   if (gw >= B * R) return;
   const int b = gw / R;
   float x = coords[(size_t)gw * 2], y = coords[(size_t)gw * 2 + 1];
-  // grid_sample's unnormalise(normalise(x)) round trip, then the border clamp
+  // grid_sample's unnormalise(normalise(x)) round trip, rounded step by step as the reference does (__fmul_rn: x * s - 1
+  // is not contracted into one FMA), then the border clamp
   const float sx = 2.0f / (float)max(W - 1, 1), sy = 2.0f / (float)max(H - 1, 1);
-  x = ((x * sx - 1.0f) + 1.0f) * 0.5f * (float)(W - 1);
-  y = ((y * sy - 1.0f) + 1.0f) * 0.5f * (float)(H - 1);
+  x = ((__fmul_rn(x, sx) - 1.0f) + 1.0f) * 0.5f * (float)(W - 1);
+  y = ((__fmul_rn(y, sy) - 1.0f) + 1.0f) * 0.5f * (float)(H - 1);
   x = fminf(fmaxf(x, 0.0f), (float)(W - 1));
   y = fminf(fmaxf(y, 0.0f), (float)(H - 1));
   const float fx = floorf(x), fy = floorf(y);
@@ -433,10 +435,12 @@ int vgg_corr_build_pyramid(int BS, int C, int H, int W, int num_levels, const fl
 
 int vgg_corr_sample(int BS, int N, int C, int H, int W, int num_levels, int radius, const void* pyramid, int elem_size,
                     const float* targets, const float* coords, int border_padding, float* out, void* stream) {
-  VGG_REQUIRE(pyramid && targets && coords && out, "null pointer");
+  VGG_REQUIRE(BS >= 0 && N >= 0, "bad sizes");
   VGG_REQUIRE(num_levels >= 1 && num_levels <= 8, "num_levels must be in [1,8]");
   cudaStream_t st = (cudaStream_t)stream;
   g_launch_count = 0;
+  if ((size_t)BS * N == 0) return VGG_OK;              // nothing to sample (a zero grid is not a valid launch)
+  VGG_REQUIRE(pyramid && targets && coords && out, "null pointer");
   CorrLevels lv;
   const char* p = reinterpret_cast<const char*>(pyramid);
   int h = H, w = W;

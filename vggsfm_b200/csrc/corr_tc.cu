@@ -12,8 +12,9 @@
 //   operands: K-major, 64-byte swizzle (k-blocks of 32 fp16 channels), stored in global memory as ready-made tile
 //   images -- B (feature positions) once per CorrBlock, A (targets) once per call -- so the producer warp moves a whole
 //   256 x 128 operand tile with ONE 64 KB bulk copy (cp.async.bulk), no tensor map.
-// grid_sample semantics kept: align_corners=True, padding "zeros" (taps outside the map read 0), tap order
-// out[a*(2r+1)+b] at x = cx + (a-r), y = cy + (b-r).  Maps whose width is a power of two (128 -> 8 at C4).
+// grid_sample semantics kept: align_corners=True, padding "zeros" (taps outside the map read 0, and so do non-finite
+// coordinates, as on CUDA: corr_window in common.cuh), tap order out[a*(2r+1)+b] at x = cx + (a-r), y = cy + (b-r).
+// Maps whose width is a power of two (128 -> 8 at C4).
 #include <cuda_fp16.h>
 #include <algorithm>
 #include "common.cuh"
@@ -211,13 +212,13 @@ __global__ void __launch_bounds__(CT_THREADS, 1)
     mbar_wait(a_full, (uint32_t)(item_no & 1));
     const uint32_t a_addr = smem_u32(a_sm) + (uint32_t)half * 64u * 64u;   // 64 rows = 8 swizzle atoms
     for (int l = 0; l < L; ++l) {
-      const int W = lv.W[l], logW = lv.logW[l];
+      const int H = lv.H[l], W = lv.W[l], logW = lv.logW[l];
       const float scale = 1.0f / (float)(1 << l);
       int x0[2], y0[2];                                                   // footprint origins of the two queries
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        x0[h] = (int)floorf(cx0[h] * scale) - R;
-        y0[h] = (int)floorf(cy0[h] * scale) - R;
+        x0[h] = (int)floorf(corr_window(cx0[h] * scale, R, W)) - R;
+        y0[h] = (int)floorf(corr_window(cy0[h] * scale, R, H)) - R;
       }
       for (int i = (threadIdx.x & 127); i < 64 * FP * FP; i += 128)
         fb[(half * 64 + i / (FP * FP)) * CT_FB_LD + i % (FP * FP)] = 0.f;
@@ -260,7 +261,8 @@ __global__ void __launch_bounds__(CT_THREADS, 1)
         const int ql = half * 64 + wq * 16 + qq;
         const int nq = m * CT_M + ql;
         if (nq >= N) break;
-        const float qcx = coords[((size_t)img * N + nq) * 2] * scale, qcy = coords[((size_t)img * N + nq) * 2 + 1] * scale;
+        const float qcx = corr_window(coords[((size_t)img * N + nq) * 2] * scale, R, W);
+        const float qcy = corr_window(coords[((size_t)img * N + nq) * 2 + 1] * scale, R, H);
         const float wx = qcx - floorf(qcx), wy = qcy - floorf(qcy);
         const float* f = fb + ql * CT_FB_LD;
         float* orow = out + ((size_t)img * N + nq) * (size_t)(L * K * K) + (size_t)l * K * K;
@@ -341,13 +343,14 @@ int vgg_corr_tc_build(int BS, int C, int H, int W, int num_levels, const void* p
 
 int vgg_corr_tc_sample(int BS, int N, int C, int H, int W, int num_levels, int radius, const void* tiles, const float* targets,
                        const float* coords, void* target_tiles, float* out, void* stream) {
-  VGG_REQUIRE(tiles && targets && coords && target_tiles && out, "null pointer");
+  VGG_REQUIRE(BS >= 0 && N >= 0, "bad sizes");
   VGG_REQUIRE(radius == 3 || radius == 4, "tensor-core correlation: radius 3 or 4");
   CtLevels lv;
   VGG_REQUIRE(C == CT_C && ct_levels(H, W, num_levels, &lv) == 0, "tensor-core correlation: unsupported shape");
   cudaStream_t st = (cudaStream_t)stream;
   g_launch_count = 0;
-  if (BS == 0 || N == 0) return VGG_OK;
+  if (BS == 0 || N == 0) return VGG_OK;                // nothing to sample: empty tensors may pass null pointers
+  VGG_REQUIRE(tiles && targets && coords && target_tiles && out, "null pointer");
   const int mtiles = (N + CT_M - 1) / CT_M;
   {
     const size_t total = (size_t)BS * mtiles * CT_M * 16;
