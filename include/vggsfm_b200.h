@@ -375,7 +375,8 @@ int vgg_depth_median(int F, const int32_t* offsets, const double* y, double divi
  * trial's two sample indices in samples int32 [R,T,2] (drawn by the caller), and writes running_out uint8 [F] for
  * those frames (1 while n_trials < max_trials).  finish() writes scale / shift float32 [F] (coef_[0], intercept_),
  * n_trials / n_inliers int32 [F] (n_inliers -1 when no trial was kept: sklearn's "could not find a valid consensus
- * set") and inlier_mask uint8 in the sample CSR.  The workspace holds the per-frame state and one chunk's trials. */
+ * set") and inlier_mask uint8 in the sample CSR.  The final fit centres on numpy's float32 pairwise means of the
+ * inliers, bitwise.  The workspace holds the per-frame state and one chunk's trials. */
 int vgg_depth_ransac_workspace_bytes(int F, size_t* bytes);
 int vgg_depth_ransac_max_chunk(void);
 int vgg_depth_ransac_begin(int F, int max_trials, void* workspace, size_t ws_bytes, void* stream);
@@ -387,7 +388,8 @@ int vgg_depth_ransac_finish(int F, const int32_t* offsets, const float* x, const
                             uint8_t* inlier_mask_out, void* workspace, size_t ws_bytes, void* stream);
 
 /* utils.py:712-724 in one pass: disp != 0 -> disp * scale[f] + shift[f] (float32 ops, written back in place),
- * kept where 0 < disp <= 10000 and 0 elsewhere; depth_out = float32(1 / disp), 0 where disp == 0.  Frame f spans
+ * kept where 0 < disp <= 10000 and 0 elsewhere; depth_out = float32(1 / disp), 0 where disp == 0 or where 1 / disp
+ * overflows to +inf (the reference zeroes infinite depths).  Frame f spans
  * the tiles tile_offsets[f] .. tile_offsets[f+1] (int64 [F+1]) of vgg_depth_tile_pixels() pixels each;
  * tile_counts int32 [n_tiles] (may be NULL) receives each tile's valid-pixel count. */
 int vgg_depth_tile_pixels(void);
@@ -395,13 +397,15 @@ int vgg_depth_apply(int F, int64_t n_tiles, const int64_t* map_offsets, const in
                     const float* scale, const float* shift, float* disp, float* depth_out, int32_t* tile_counts,
                     void* stream);
 
-/* utils.py:728-765 (visual_dense_point_cloud): valid pixels (depth != 0) in row-major order, compacted by
+/* utils.py:728-765 (visual_dense_point_cloud): valid pixels (disp != 0: the rescaled disparity that
+ * vgg_depth_apply wrote, so a valid pixel whose depth is 0 is still a point) in row-major order, compacted by
  * tile_base int64 [n_tiles + 1] (exclusive prefix of tile_counts): pixel (x, y) without +0.5 through cam_from_img
  * (cam_model VGG_SIMPLE_*, cam_params double [F,4] = f, cx, cy, k), times depth, through world_from_cam double
  * [F,3,4] (cam_from_world.inverse()).  Frame f's M_f points are one [2, M_f, 3] block of `out` double starting at
  * 6 * tile_base[tile_offsets[f]]: the world points, then rgb uint8 [pixels,3] / 255. */
 int vgg_depth_unproject(int F, int64_t n_tiles, const int64_t* map_offsets, const int32_t* map_hw,
-                        const int64_t* tile_offsets, const int64_t* tile_base, const float* depth, const uint8_t* rgb,
+                        const int64_t* tile_offsets, const int64_t* tile_base, const float* depth, const float* disp,
+                        const uint8_t* rgb,
                         const int32_t* cam_model, const double* cam_params, const double* world_from_cam,
                         double* out, void* stream);
 

@@ -12,6 +12,13 @@ What it restates, and how:
   starts at 1, a trial with fewer inliers is skipped, one with equal inliers and a lower R^2 is skipped,
   ``max_trials = min(max_trials, _dynamic_max_trials(n_best, n, 2, 0.99))`` after each kept trial, stop once
   ``n_trials_ >= max_trials``; the final model is LinearRegression on the best inlier set.
+* ``pairwise_sum_f32`` / ``mean_f32``: numpy's float32 ``np.mean`` (``pairwise_sum`` of ``loops_utils.h``, then one
+  float32 division by float32(n)), which ``_preprocess_data`` uses for the float32 offsets of ``LinearRegression``.
+  This restatement is the rule ``dd_final_kernel`` follows for its means; ``test_dense_depth_oracle.py`` checks it
+  bitwise against ``np.mean``.
+* Errors: ``frame_samples`` and ``ransac_fit`` raise what the reference loop and sklearn 1.9 raise, in their order:
+  "Too few points", "Ill-posed scene", the ``residual_threshold`` parameter error of a NaN threshold (an empty sample
+  set or any NaN target), ``min_samples`` (one sample), then "Input X contains infinity" (a +inf disparity).
 * ``sample_pairs``: ``sklearn.utils.random.sample_without_replacement(n, 2, random_state)``, whose method depends on
   the ratio 2 / n: n = 2 returns [0, 1] without a draw (reservoir sampling), 2 / n in (0.01, 0.99) is
   ``permutation(n)[:2]``, and 2 / n <= 0.01 is tracking selection (``randint(n)`` until unseen).
@@ -27,6 +34,8 @@ What it restates, and how:
 """
 from __future__ import annotations
 
+import warnings
+
 import numpy as np
 import scipy.linalg
 
@@ -37,6 +46,45 @@ DEPTH_MAX = 1 / DISPARITY_MIN
 DEPTH_MIN = 1 / DISPARITY_MAX
 THRES_RATIO = 30
 MAX_TRIALS = 20000
+
+
+NAN_THRESHOLD_ERROR = ("The 'residual_threshold' parameter of RANSACRegressor must be a float in the range [0.0, inf) "
+                       "or None. Got {!r} instead.")
+MIN_SAMPLES_ERROR = "`min_samples` may not be larger than number of samples: n_samples = %d."
+INF_X_ERROR = "Input X contains infinity or a value too large for dtype('float32')."
+PAIRWISE_BLOCK = 128                                  # numpy's PW_BLOCKSIZE
+
+
+def pairwise_sum_f32(a):
+    """numpy's float32 pairwise sum of a contiguous vector, operation by operation: below 8 elements, 0 plus each in
+    order; up to 128, eight accumulators seeded with a[0..7] and stepped by 8 to n - n % 8, combined as
+    ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)), then the tail in order; above, split at n2 = n//2 - (n//2) % 8 and recurse."""
+    a = np.asarray(a, dtype=f32).reshape(-1)
+    n = len(a)
+    if n < 8:
+        s = f32(0)
+        for v in a:
+            s = f32(s + v)
+        return s
+    if n <= PAIRWISE_BLOCK:
+        m = n - n % 8
+        r = a[:m].reshape(-1, 8)
+        acc = r[0].copy()
+        for row in r[1:]:
+            acc = acc + row
+        s = ((acc[0] + acc[1]) + (acc[2] + acc[3])) + ((acc[4] + acc[5]) + (acc[6] + acc[7]))
+        for v in a[m:]:
+            s = f32(s + v)
+        return f32(s)
+    n2 = n // 2
+    n2 -= n2 % 8
+    return f32(pairwise_sum_f32(a[:n2]) + pairwise_sum_f32(a[n2:]))
+
+
+def mean_f32(a):
+    """np.mean of a float32 vector: the pairwise sum over float32(n), both float32."""
+    a = np.asarray(a, dtype=f32).reshape(-1)
+    return f32(pairwise_sum_f32(a) / f32(len(a)))
 
 
 def dynamic_max_trials(n_inliers, n_samples, min_samples=2, probability=0.99):
@@ -115,8 +163,12 @@ def ransac_fit(X, y, threshold, seed, max_trials=MAX_TRIALS, return_debug=False)
     X = np.asarray(X, dtype=f32)
     y = np.asarray(y, dtype=np.float64)
     n = len(X)
+    if np.isnan(threshold):                           # parameter validation comes first in fit
+        raise ValueError(NAN_THRESHOLD_ERROR.format(threshold))
     if 2 > n:
-        raise ValueError("`min_samples` may not be larger than number of samples: n_samples = %d." % n)
+        raise ValueError(MIN_SAMPLES_ERROR % n)
+    if np.isinf(X).any():                             # validate_data of the first trial's predict
+        raise ValueError(INF_X_ERROR)
     rs = np.random.RandomState(seed)
     n_best, score_best, mask_best, c_best = 1, -np.inf, None, None
     n_trials, mt = 0, max_trials
@@ -152,6 +204,27 @@ def ransac_fit(X, y, threshold, seed, max_trials=MAX_TRIALS, return_debug=False)
     return out
 
 
+def tie_fixture(k=3):
+    """Two groups of k samples at interleaved, distinct float32 x (group 0 at 1, 3, 5, ..., group 1 at 2, 4, ...) with
+    targets exactly 0.25 and 0.75 -> (X, y, threshold = median / 30, group [2k]).  A trial within a group fits the
+    horizontal line through it with zero residuals, so its R^2 takes the SStot == 0 branch (1.0): the two groups tie in
+    count and score, and RANSACRegressor keeps the later one.  Asserted here: every within-group pair has exactly its
+    group as inliers and every mixed pair fewer than k inliers, so no other trial can take part in the tie."""
+    X = np.concatenate([1 + 2 * np.arange(k), 2 + 2 * np.arange(k)]).astype(f32)
+    y = np.repeat([0.25, 0.75], k)
+    group = np.repeat([0, 1], k)
+    th = np.median(y) / THRES_RATIO
+    for i in range(2 * k):
+        for j in range(i + 1, 2 * k):
+            c, b = fit_two(X[i], X[j], y[i], y[j])
+            res = (y - predict(X, c, b)) ** 2
+            if group[i] == group[j]:
+                assert (res[group == group[i]] == 0).all() and (res <= th).sum() == k
+            else:
+                assert (res <= th).sum() < k
+    return X, y, th, group
+
+
 def frame_samples(disp_map, sparse_uvd):
     """utils.py:662-695 -> (X float32, y float64, threshold).  Raises the reference's ValueErrors."""
     sparse_uvd = np.array(sparse_uvd)
@@ -165,7 +238,9 @@ def frame_samples(disp_map, sparse_uvd):
     pos = sampled > 0
     X = sampled[pos]
     y = 1 / np.clip(sparse_uvd[:, -1][pos], DEPTH_MIN, DEPTH_MAX)
-    threshold = np.median(y) / THRES_RATIO
+    with np.errstate(invalid="ignore"), warnings.catch_warnings():
+        warnings.simplefilter("ignore", RuntimeWarning)   # the median of no sample is NaN, which ransac_fit rejects
+        threshold = np.median(y) / THRES_RATIO
     if threshold <= 0:
         raise ValueError("Ill-posed scene for depth alignment")
     return X, y, threshold

@@ -2,12 +2,16 @@
 
 Per frame the RANSAC decisions are exact: n_trials, n_inliers and the inlier mask, because the trial kernel computes
 sklearn's float32 two-sample fit bitwise (oracle.fit_two == sgelsd) and the residuals in the same float64 operations.
-The final fit on the inliers sums in float64 where sklearn sums in float32 and runs sgelsd, so scale and shift agree
-to a few float32 ulps (rtol 2e-6, plus the cancellation of ym - xm * c for the shift).  Given the same scale and shift,
-the rescaled disparity and depth are bitwise equal, so the maps are compared after the oracle's rescale with the
-kernel's scale / shift.  The decisions are only exact away from ties, so the oracle side asserts its margins."""
+The final fit on the inliers takes numpy's float32 means bitwise (oracle.mean_f32) and then solves the centred
+least squares in float64 where sklearn runs sgelsd in float32, so the scale agrees to a few float32 ulps (rtol 2e-6).
+With equal means, shift = ym - xm * c differs only through c: two roundings of the product and two of the difference
+give |d shift| <= |xm| |d c| + 4u (|ym| + |xm c|), u = 2^-24, which is the shift's bar (SHIFT_ULPS = 4).  Given the
+same scale and shift, the rescaled disparity and depth are bitwise equal, so the maps are compared after the oracle's
+rescale with the kernel's scale / shift.  The decisions are only exact away from ties, so the oracle side asserts its
+margins."""
 import glob
 import os
+import re
 
 import numpy as np
 import pytest
@@ -18,6 +22,21 @@ from vggsfm_b200.reconstruction import Camera, Image, Reconstruction, Rigid3d, R
 
 pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+SCALE_RTOL = 2e-6
+SHIFT_ULPS = 4
+U32 = 2.0 ** -24
+
+
+def check_fit(scale, shift, X, y, r, label=""):
+    """The kernel's final scale / shift against the oracle's fit on the same inlier mask -> shift error / bar."""
+    m = r["inlier_mask"]
+    xm, ym = float(O.mean_f32(X[m])), float(O.mean_f32(y[m]))
+    c = float(r["coef"])
+    assert abs(float(scale) - c) <= SCALE_RTOL * abs(c), (label, float(scale), c)
+    bar = abs(xm) * abs(float(scale) - c) + SHIFT_ULPS * U32 * (abs(ym) + abs(xm * c))
+    err = abs(float(shift) - float(r["intercept"]))
+    assert err <= bar, (label, float(shift), float(r["intercept"]), bar)
+    return err / bar if bar > 0 else 0.0
 
 
 def _scene(rng, shapes, n_samples, ratio, model="SIMPLE_PINHOLE", sky=0.05):
@@ -48,6 +67,7 @@ def _check(rec, sparse, disp, rgb, seeds, visual=False, model="SIMPLE_PINHOLE", 
     orig = {k: v.copy() for k, v in disp.items()}
     depth, pts, dbg = dense_depth.align_dense_depth_maps(rec, sparse, disp, rgb, visual, seeds=seeds,
                                                          return_debug=True, **kw)
+    worst = 0.0
     for f, nm in enumerate(sparse):
         X, y, th = O.frame_samples(orig[nm], sparse[nm])
         np.testing.assert_array_equal(dbg["x"][f], X)
@@ -59,9 +79,7 @@ def _check(rec, sparse, disp, rgb, seeds, visual=False, model="SIMPLE_PINHOLE", 
         assert dbg["n_trials"][f] == r["n_trials"], nm
         assert dbg["n_inliers"][f] == r["n_inliers"], nm
         np.testing.assert_array_equal(dbg["inlier_mask"][f], r["inlier_mask"])
-        np.testing.assert_allclose(dbg["scale"][f], r["coef"], rtol=2e-6)
-        ym = np.float32(y[r["inlier_mask"]].astype(np.float32).mean())
-        np.testing.assert_allclose(dbg["shift"][f], r["intercept"], rtol=0, atol=4e-7 * (abs(ym) + abs(r["coef"])))
+        worst = max(worst, check_fit(dbg["scale"][f], dbg["shift"][f], X, y, r, nm))
         dref, depref, valid = O.apply_scale(orig[nm], dbg["scale"][f], dbg["shift"][f])
         np.testing.assert_array_equal(depth[nm].view(np.uint32), depref.view(np.uint32))
         np.testing.assert_array_equal(disp[nm].view(np.uint32), dref.view(np.uint32))
@@ -83,6 +101,7 @@ def _check(rec, sparse, disp, rgb, seeds, visual=False, model="SIMPLE_PINHOLE", 
                 xy = np.column_stack([xx.ravel(), yy.ravel()])[valid.ravel()]
                 np.testing.assert_allclose(nrm, O.cam_from_img(model, cam.params, xy), atol=1e-9)
                 np.testing.assert_allclose(cam.img_from_cam(nrm), xy, atol=1e-6)
+    print(f"largest shift error / bar: {worst:.3g}")
     return dbg
 
 
@@ -144,7 +163,9 @@ def test_rounding_clip_and_limits(cuda_dev):
     _check(rec, sparse, disp, rgb, rng.integers(0, 2**31, 2))
 
 
-def test_errors_before_launch(cuda_dev):
+def test_reference_errors_before_launch(cuda_dev):
+    """The reference's errors and messages, raised before any RANSAC launch.  Samples that all fall out of bounds leave
+    no kept sample: np.median of it is NaN, and sklearn rejects the NaN residual_threshold."""
     rng = np.random.default_rng(3)
     rec, sparse, disp, rgb = _scene(rng, [(30, 40)], 50, 0.9)
     nm = list(sparse)[0]
@@ -152,7 +173,7 @@ def test_errors_before_launch(cuda_dev):
         dense_depth.align_dense_depth_maps(rec, {nm: np.zeros((0, 3))}, disp, rgb)
     out_of_bounds = sparse[nm].copy()
     out_of_bounds[:, 0] = -5
-    with pytest.raises(ValueError, match="min_samples"):
+    with pytest.raises(ValueError, match=re.escape(O.NAN_THRESHOLD_ERROR.format(np.float64(np.nan)))):
         dense_depth.align_dense_depth_maps(rec, {nm: out_of_bounds}, disp, rgb)
     with pytest.raises(TypeError):
         dense_depth.align_dense_depth_maps(rec, sparse, {nm: disp[nm].astype(np.float64)}, rgb)

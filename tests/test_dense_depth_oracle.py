@@ -77,6 +77,102 @@ def test_errors_of_the_reference():
     assert th == np.median(np.array([0.5, 0.25])) / 30 == (0.5 + 0.25) / 2 / 30
 
 
+PAIRWISE_SIZES = list(range(1, 300)) + [1000, 4095, 4096, 8191, 8192, 8193, 20000, 100003]
+
+
+def test_pairwise_mean_is_numpy_bitwise():
+    """The restatement of numpy's float32 pairwise sum is what dd_final_kernel computes; a numpy whose summation
+    changes fails here first."""
+    rng = np.random.default_rng(7)
+    for n in PAIRWISE_SIZES:
+        for a in (rng.uniform(0, 0.05, n) + 1000, rng.lognormal(0, 3, n), rng.normal(0, 1, n)):
+            a = a.astype(f32)
+            got = O.mean_f32(a)
+            assert got.view(np.uint32) == np.mean(a).view(np.uint32), n
+            assert got.view(np.uint32) == a.reshape(n, 1).mean(axis=0)[0].view(np.uint32), n
+            assert O.pairwise_sum_f32(a).view(np.uint32) == np.add.reduce(a).view(np.uint32), n
+
+
+def _reference_frame(disp_map, sparse_uvd, seed):
+    """utils.py:662-707 with live sklearn (random_state pinned) -> (coef, intercept, n_trials, inlier_mask)."""
+    sk = pytest.importorskip("sklearn.linear_model")
+    sparse_uvd = np.array(sparse_uvd)
+    if len(sparse_uvd) <= 0:
+        raise ValueError("Too few points for depth alignment")
+    ww, hh = disp_map.shape
+    int_uv = np.round(sparse_uvd[:, :2]).astype(int)
+    mask = (int_uv[:, 0] >= 0) & (int_uv[:, 0] < hh) & (int_uv[:, 1] >= 0) & (int_uv[:, 1] < ww)
+    sparse_uvd, int_uv = sparse_uvd[mask], int_uv[mask]
+    sampled = disp_map[int_uv[:, 1], int_uv[:, 0]]
+    pos = sampled > 0
+    X = sampled[pos].reshape(-1, 1)
+    y = 1 / np.clip(sparse_uvd[:, -1][pos], O.DEPTH_MIN, O.DEPTH_MAX)
+    th = np.median(y) / 30
+    if th <= 0:
+        raise ValueError("Ill-posed scene for depth alignment")
+    r = sk.RANSACRegressor(sk.LinearRegression(), min_samples=2, residual_threshold=th, max_trials=20000,
+                           loss="squared_error", random_state=np.random.RandomState(seed)).fit(X, y)
+    return r.estimator_.coef_[0], r.estimator_.intercept_, r.n_trials_, r.inlier_mask_
+
+
+def _error_frames():
+    """(name, disparity map, uvd) of frames that fail, each at a different check of the reference's order."""
+    disp = np.full((6, 8), 0.5, f32)
+    disp[0, 0], disp[0, 1], disp[0, 2], disp[0, 3] = np.inf, np.nan, 0, -1
+    good = np.array([[4, 3, 2.0], [5, 4, 3.0], [6, 2, 2.5], [2, 5, 4.0], [3, 1, 1.5]])
+    return [
+        ("no point", disp, np.zeros((0, 3))),
+        ("all out of bounds", disp, good - [20, 0, 0]),
+        ("no positive disparity", disp, np.array([[1, 0, 2.0], [2, 0, 3.0], [3, 0, 4.0], [2.4, 0, 1.0]])),
+        ("NaN depth", disp, np.vstack([good, [[5, 5, np.nan]]])),
+        ("NaN depth and +inf disparity", disp, np.vstack([good, [[0, 0, 2.0], [5, 5, np.nan]]])),
+        ("one sample", disp, np.array([[4, 3, 2.0], [1, 0, 2.0], [-9, 0, 1.0]])),
+        ("one sample at +inf disparity", disp, np.array([[0, 0, 2.0], [1, 0, 2.0]])),
+        ("+inf disparity", disp, np.vstack([good, [[0.4, 0.3, 2.0]]])),
+    ]
+
+
+ERROR_OF_FRAME = {"no point": "Too few points", "all out of bounds": "residual_threshold",
+                  "no positive disparity": "residual_threshold", "NaN depth": "residual_threshold",
+                  "NaN depth and +inf disparity": "residual_threshold", "one sample": "min_samples",
+                  "one sample at +inf disparity": "min_samples", "+inf disparity": "infinity"}
+
+
+@pytest.mark.filterwarnings("ignore::RuntimeWarning")     # numpy's median of an empty sample set
+@pytest.mark.parametrize("case", [c[0] for c in _error_frames()])
+def test_errors_match_sklearn_in_order(case):
+    _, disp, uvd = next(c for c in _error_frames() if c[0] == case)
+    with pytest.raises(ValueError) as ref:
+        _reference_frame(disp, uvd, 0)
+    with pytest.raises(ValueError) as got:
+        X, y, th = O.frame_samples(disp, uvd)
+        O.ransac_fit(X, y, th, 0)
+    assert str(got.value) == str(ref.value)
+    assert ERROR_OF_FRAME[case] in str(ref.value)
+
+
+def test_exact_tie_keeps_the_later_trial_like_sklearn():
+    """Two groups tie exactly in count and R^2; sklearn keeps the later one, and the dynamic stop ends the run at
+    ceil(log 0.01 / log 0.75) = 17 trials.  Among the seeds, both groups win, and in some runs the earlier winner is
+    replaced by the later group."""
+    sk = pytest.importorskip("sklearn.linear_model")
+    X, y, th, group = O.tie_fixture(3)
+    winners, replaced = set(), 0
+    for seed in range(40):
+        o = O.ransac_fit(X, y, th, seed, return_debug=True)
+        ref = sk.RANSACRegressor(sk.LinearRegression(), min_samples=2, residual_threshold=th, max_trials=20000,
+                                 loss="squared_error", random_state=np.random.RandomState(seed)).fit(X[:, None], y)
+        assert ref.n_trials_ == o["n_trials"] == 17
+        np.testing.assert_array_equal(ref.inlier_mask_, o["inlier_mask"])
+        assert o["coef"] == ref.estimator_.coef_[0] == 0 and o["intercept"] == ref.estimator_.intercept_
+        s = o["debug"]["samples"]
+        within = [group[a] for a, b in s if group[a] == group[b]]
+        assert o["inlier_mask"].sum() == 3 and (group[o["inlier_mask"]] == within[-1]).all()
+        winners.add(within[-1])
+        replaced += len(set(within)) == 2
+    assert winners == {0, 1} and replaced > 0
+
+
 def _golden_frames(path):
     z = np.load(path)
     F = len(z["seeds"])

@@ -190,7 +190,7 @@ def lib() -> ctypes.CDLL:
     L.vgg_depth_ransac_finish.argtypes = [ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, cs, vp]
     L.vgg_depth_tile_pixels.argtypes = []
     L.vgg_depth_apply.argtypes = [ci, i64, vp, vp, vp, vp, vp, vp, vp, vp]
-    L.vgg_depth_unproject.argtypes = [ci, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.vgg_depth_unproject.argtypes = [ci, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     _lib = L
     return L
 

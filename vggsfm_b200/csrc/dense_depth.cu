@@ -236,6 +236,116 @@ __global__ void dd_resolve_kernel(int R, const int32_t* __restrict__ offsets, co
   running[f] = s.n_trials < s.max_trials;
 }
 
+// numpy's float32 pairwise sum (oracle.pairwise_sum_f32), over the inliers of a frame in index order, of x and of
+// float32(y) at once.  One thread reads its inliers sequentially from their original positions.
+constexpr int PW_BLOCK = 128;              // numpy's PW_BLOCKSIZE
+
+struct InlierReader {
+  const float* x;
+  const double* y;
+  const uint8_t* mask;
+  int i;
+  __device__ float2 next() {
+    while (!mask[i]) ++i;
+    const float2 v = make_float2(x[i], (float)y[i]);
+    ++i;
+    return v;
+  }
+};
+
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+
+__device__ float2 pairwise_leaf(InlierReader& r, int n) {
+  if (n < 8) {
+    float2 s = make_float2(0.f, 0.f);
+    for (int k = 0; k < n; ++k) s = add2(s, r.next());
+    return s;
+  }
+  float2 acc[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) acc[j] = r.next();
+  const int m = n - n % 8;
+  for (int k = 8; k < m; k += 8)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[j] = add2(acc[j], r.next());
+  float2 s = add2(add2(add2(acc[0], acc[1]), add2(acc[2], acc[3])), add2(add2(acc[4], acc[5]), add2(acc[6], acc[7])));
+  for (int k = m; k < n; ++k) s = add2(s, r.next());
+  return s;
+}
+
+__device__ __forceinline__ int pairwise_split(int n) { return n / 2 - (n / 2) % 8; }
+
+// the recursion below a node; D bounds its depth statically (a split leaves at least 64 elements on each side, so 24
+// levels below the top 8 cover every int count)
+template <int D>
+__device__ __noinline__ float2 pairwise_sum(InlierReader& r, int n) {
+  if (n <= PW_BLOCK) return pairwise_leaf(r, n);
+  const int n2 = pairwise_split(n);
+  const float2 a = pairwise_sum<D - 1>(r, n2);
+  return add2(a, pairwise_sum<D - 1>(r, n - n2));
+}
+template <>
+__device__ __noinline__ float2 pairwise_sum<0>(InlierReader& r, int n) { return pairwise_leaf(r, n); }
+
+// Both float32 sums of the m inliers (mask already written by this CTA).  The top 8 levels of numpy's tree are spread
+// over the 256 threads: thread t takes the node of path t (most significant bit first); a node that is already a leaf
+// goes to its leftmost path and the others stay empty.  A prefix over the mask finds where each node's first inlier
+// lies, each thread sums its subtree, and the 256 results are combined back up the same 8 levels.
+__device__ float2 inlier_sums(const float* x, const double* y, const uint8_t* mask, int n, int m) {
+  static_assert(DD_THREADS == 256, "one thread per node of the top 8 levels");
+  __shared__ int start[DD_THREADS], first[DD_THREADS], warp_cnt[DD_THREADS / 32];
+  __shared__ float2 part[DD_THREADS];
+  const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
+  int a = 0, len = m;
+  for (int d = 7; d >= 0; --d) {
+    const int bit = (t >> d) & 1;
+    if (len > PW_BLOCK) {
+      const int n2 = pairwise_split(len);
+      if (bit) { a += n2; len -= n2; } else { len = n2; }
+    } else if (bit) {
+      a += len; len = 0;
+    }
+  }
+  start[t] = a;                            // non-decreasing in t; an empty node sits just before the next one
+  __syncthreads();
+  int carry = 0;
+  for (int base = 0; base < n; base += DD_THREADS) {
+    const int i = base + t;
+    const bool in = i < n && mask[i];
+    const unsigned bal = __ballot_sync(0xffffffffu, in);
+    if (lane == 0) warp_cnt[wid] = __popc(bal);
+    __syncthreads();
+    int p = carry + __popc(bal & ((1u << lane) - 1u)), total = 0;
+    for (int w = 0; w < DD_THREADS / 32; ++w) { p += w < wid ? warp_cnt[w] : 0; total += warp_cnt[w]; }
+    if (in) {
+      int lo = 0, hi = DD_THREADS - 1;     // the last node starting at or before p
+      while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (start[mid] <= p) lo = mid; else hi = mid - 1;
+      }
+      if (start[lo] == p) first[lo] = i;
+    }
+    carry += total;
+    __syncthreads();
+  }
+  float2 v = make_float2(0.f, 0.f);
+  if (len > 0) {
+    InlierReader r{x, y, mask, first[t]};
+    v = pairwise_sum<24>(r, len);
+  }
+  part[t] = v;
+  start[t] = len;
+  __syncthreads();
+  for (int h = 1; h < DD_THREADS; h <<= 1) {
+    if ((t & (2 * h - 1)) == 0 && start[t + h] > 0) {
+      part[t] = add2(part[t], part[t + h]);
+      start[t] += start[t + h];
+    }
+    __syncthreads();
+  }
+  return part[0];
+}
+
 __global__ void __launch_bounds__(DD_THREADS) dd_final_kernel(
     const int32_t* __restrict__ offsets, const float* __restrict__ x, const double* __restrict__ y,
     const double* __restrict__ thresh, const DdState* __restrict__ st, float* __restrict__ scale,
@@ -247,21 +357,20 @@ __global__ void __launch_bounds__(DD_THREADS) dd_final_kernel(
   const DdState s = st[f];
   const double th = thresh[f];
   int cnt = 0;
-  double sx = 0.0, sy = 0.0;
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const bool in = s.has_best && sq_residual(x[o + i], y[o + i], s.c, s.b) <= th;
     mask[o + i] = in;
-    if (in) { ++cnt; sx += x[o + i]; sy += (float)y[o + i]; }
+    cnt += in;
   }
   cnt = block_sum(cnt, redi);
-  sx = block_sum(sx, redd);
-  sy = block_sum(sy, redd);
   if (!s.has_best || cnt == 0) {
     if (threadIdx.x == 0) { scale[f] = 0.f; shift[f] = 0.f; n_trials[f] = s.n_trials; n_inliers[f] = s.has_best ? 0 : -1; }
     return;
   }
-  // LinearRegression on the inliers: float32 means, float32 centring, the 1-column least squares accumulated in float64
-  const float xm = (float)(sx / cnt), ym = (float)(sy / cnt);
+  // LinearRegression on the inliers: numpy's float32 means (bitwise), float32 centring, then the 1-column least
+  // squares accumulated in float64 where sgelsd works in float32
+  const float2 sum = inlier_sums(x + o, y + o, mask + o, n, cnt);
+  const float xm = __fdiv_rn(sum.x, __int2float_rn(cnt)), ym = __fdiv_rn(sum.y, __int2float_rn(cnt));
   double sxy = 0.0, sxx = 0.0;
   for (int i = threadIdx.x; i < n; i += blockDim.x)
     if (mask[o + i]) {
@@ -290,7 +399,7 @@ __device__ __forceinline__ int frame_tile(const int64_t* tile_offsets, int F, in
 }
 
 // numpy: disp[nz] = disp[nz] * scale + shift with float32 scale / shift (float32 ops); keep 0 < disp <= 10000;
-// depth = float32(1 / disp), 0 elsewhere
+// depth = float32(1 / disp), 0 elsewhere and where 1 / disp overflows (a kept disparity below 2^-128)
 __global__ void __launch_bounds__(DD_THREADS) dd_apply_kernel(
     int F, const int64_t* __restrict__ map_offsets, const int64_t* __restrict__ tile_offsets,
     const float* __restrict__ scale, const float* __restrict__ shift, float* __restrict__ disp,
@@ -311,7 +420,8 @@ __global__ void __launch_bounds__(DD_THREADS) dd_apply_kernel(
       const bool ok = d > 0.f && d <= 10000.f;
       if (!ok) d = 0.f;
       disp[base + p] = d;
-      depth[base + p] = ok ? __fdiv_rn(1.f, d) : 0.f;
+      const float inv = __fdiv_rn(1.f, d);           // the reference zeroes a depth that overflows to +inf
+      depth[base + p] = ok && inv != INFINITY ? inv : 0.f;
       cnt += ok;
     }
   }
@@ -359,8 +469,8 @@ __device__ __forceinline__ double rowdot(const double* R, double p0, double p1, 
 __global__ void __launch_bounds__(DD_THREADS) dd_unproject_kernel(
     int F, const int64_t* __restrict__ map_offsets, const int32_t* __restrict__ map_hw,
     const int64_t* __restrict__ tile_offsets, const int64_t* __restrict__ tile_base, const float* __restrict__ depth,
-    const uint8_t* __restrict__ rgb, const int32_t* __restrict__ cam_model, const double* __restrict__ cam_params,
-    const double* __restrict__ world_from_cam, double* __restrict__ out) {
+    const float* __restrict__ disp, const uint8_t* __restrict__ rgb, const int32_t* __restrict__ cam_model,
+    const double* __restrict__ cam_params, const double* __restrict__ world_from_cam, double* __restrict__ out) {
   __shared__ int warp_cnt[DD_THREADS / 32];
   const int64_t tile = blockIdx.x;
   const int f = frame_tile(tile_offsets, F, tile);
@@ -379,8 +489,9 @@ __global__ void __launch_bounds__(DD_THREADS) dd_unproject_kernel(
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   for (int k = 0; k < DD_TILE / DD_THREADS; ++k) {
     const int64_t p = p0 + k * DD_THREADS + threadIdx.x;
-    const float d = p < npix ? depth[base + p] : 0.f;
-    const bool ok = d != 0.f;
+    // the reference's valid_depth_mask is the rescaled disparity's: a kept pixel whose depth is 0 is still a point
+    const bool ok = p < npix && disp[base + p] != 0.f;
+    const float d = ok ? depth[base + p] : 0.f;
     const unsigned bal = __ballot_sync(0xffffffffu, ok);
     __syncthreads();
     if (lane == 0) warp_cnt[wid] = __popc(bal);
@@ -507,13 +618,13 @@ int vgg_depth_apply(int F, int64_t n_tiles, const int64_t* map_offsets, const in
 }
 
 int vgg_depth_unproject(int F, int64_t n_tiles, const int64_t* map_offsets, const int32_t* map_hw,
-                        const int64_t* tile_offsets, const int64_t* tile_base, const float* depth, const uint8_t* rgb,
-                        const int32_t* cam_model, const double* cam_params, const double* world_from_cam,
-                        double* out, void* stream) {
+                        const int64_t* tile_offsets, const int64_t* tile_base, const float* depth, const float* disp,
+                        const uint8_t* rgb, const int32_t* cam_model, const double* cam_params,
+                        const double* world_from_cam, double* out, void* stream) {
   VGG_REQUIRE(F >= 0 && n_tiles >= 0 && n_tiles < (1ll << 31), "bad frame or tile count");
   if (F == 0 || n_tiles == 0) return 0;
   dd_unproject_kernel<<<(unsigned)n_tiles, DD_THREADS, 0, (cudaStream_t)stream>>>(
-      F, map_offsets, map_hw, tile_offsets, tile_base, depth, rgb, cam_model, cam_params, world_from_cam, out);
+      F, map_offsets, map_hw, tile_offsets, tile_base, depth, disp, rgb, cam_model, cam_params, world_from_cam, out);
   VGG_LAUNCH_CHECK();
   return 0;
 }

@@ -199,6 +199,32 @@ def _pinned(n, dtype):
     return torch.empty(n, dtype=dtype, pin_memory=True)
 
 
+NAN_THRESHOLD_ERROR = ("The 'residual_threshold' parameter of RANSACRegressor must be a float in the range [0.0, inf) "
+                       "or None. Got np.float64(nan) instead.")
+MIN_SAMPLES_ERROR = "`min_samples` may not be larger than number of samples: n_samples = %d."
+INF_X_ERROR = "Input X contains infinity or a value too large for dtype('float32')."
+
+
+def _raise_first_error(uvds, stats):
+    """The reference's error for the first failing frame, in its order of checks: no sparse point, a non-positive
+    threshold, a NaN threshold (no kept sample, or a NaN target: sklearn's parameter check), one kept sample, then a
+    +inf disparity (sklearn's input check).  ``stats`` rows: kept samples, NaN targets, infinite disparities and the
+    threshold, per frame.  The reference has rescaled the earlier frames' disparities in place by then; this raises
+    before any frame is touched."""
+    cnt, nan_y, inf_x, thresh = stats
+    for f in range(len(uvds)):
+        if len(uvds[f]) <= 0:
+            raise ValueError("Too few points for depth alignment")
+        if thresh[f] <= 0:
+            raise ValueError("Ill-posed scene for depth alignment")
+        if cnt[f] == 0 or nan_y[f] > 0:
+            raise ValueError(NAN_THRESHOLD_ERROR)
+        if cnt[f] < 2:
+            raise ValueError(MIN_SAMPLES_ERROR % cnt[f])
+        if inf_x[f] > 0:
+            raise ValueError(INF_X_ERROR)
+
+
 def align_dense_depth_maps(reconstruction, sparse_depth, disp_dict, original_images, visual_dense_point_cloud=False,
                            *, seeds=None, device="cuda", memory_budget=8 << 30, return_debug=False):
     """vggsfm/utils/utils.py:635-770, same arguments and return ``(depth_dict, unproj_dense_points3D)``.
@@ -215,9 +241,6 @@ def align_dense_depth_maps(reconstruction, sparse_depth, disp_dict, original_ima
     names = list(sparse_depth)
     F = len(names)
     uvds = [np.asarray(sparse_depth[nm], dtype=np.float64).reshape(-1, 3) for nm in names]
-    for u in uvds:
-        if len(u) <= 0:
-            raise ValueError("Too few points for depth alignment")
     maps = [disp_dict[nm] for nm in names]
     for nm, m in zip(names, maps):
         if not (isinstance(m, np.ndarray) and m.dtype == np.float32 and m.ndim == 2):
@@ -267,20 +290,16 @@ def align_dense_depth_maps(reconstruction, sparse_depth, disp_dict, original_ima
         fids.append(fid_d[k].long() + int(idx[0]))
     x, y, fid = torch.cat(xs), torch.cat(ys), torch.cat(fids)
     counts = torch.bincount(fid, minlength=F)
-    cnt_host = counts.cpu().numpy()
-    for f in range(F):
-        if cnt_host[f] < 2:
-            raise ValueError("`min_samples` may not be larger than number of samples: n_samples = %d."
-                             % cnt_host[f])
     offsets = torch.zeros(F + 1, dtype=torch.int32, device=device)
     offsets[1:] = torch.cumsum(counts, 0).to(torch.int32)
 
-    # 2. threshold = np.median(y) / 30, then RANSAC on every frame at once
+    # 2. threshold = np.median(y) / 30, then the reference's checks, then RANSAC on every frame at once
     thresh = torch.empty(F, dtype=torch.float64, device=device)
     _lib.check(L.vgg_depth_median(F, _ptr(offsets), _ptr(y), float(THRES_RATIO), _ptr(thresh), stream),
                "vgg_depth_median")
-    if bool((thresh <= 0).any()):
-        raise ValueError("Ill-posed scene for depth alignment")
+    nan_y = torch.bincount(fid, weights=torch.isnan(y).to(torch.float64), minlength=F)
+    inf_x = torch.bincount(fid, weights=torch.isinf(x).to(torch.float64), minlength=F)
+    _raise_first_error(uvds, torch.stack([counts.to(torch.float64), nan_y, inf_x, thresh]).cpu().numpy())
     scale, shift, n_trials, n_inl, mask = _ransac(offsets, x, y, thresh, seeds, device)
     if bool((n_inl < 0).any()):
         raise ValueError("RANSAC could not find a valid consensus set. All `max_trials` iterations were skipped "
@@ -327,8 +346,8 @@ def align_dense_depth_maps(reconstruction, sparse_depth, disp_dict, original_ima
             out = torch.empty(6 * M, dtype=torch.float64, device=device)
             model_d, params_d, wfc_d = (torch.from_numpy(a).to(device) for a in (model, params, wfc))
             _lib.check(L.vgg_depth_unproject(B, n_tiles, _ptr(moff_d), _ptr(hw), _ptr(toff_d), _ptr(tbase),
-                                             _ptr(depth), _ptr(rgb), _ptr(model_d), _ptr(params_d), _ptr(wfc_d),
-                                             _ptr(out), stream), "vgg_depth_unproject")
+                                             _ptr(depth), _ptr(disp), _ptr(rgb), _ptr(model_d), _ptr(params_d),
+                                             _ptr(wfc_d), _ptr(out), stream), "vgg_depth_unproject")
             out_host = _pinned(6 * M, torch.float64)
             out_host.copy_(out)
             on = out_host.numpy()
