@@ -122,13 +122,13 @@ def project(poses, intr, points, model):
 def residuals_and_jacobians(poses, intr, points, uv, mask, model):
     """Per-observation residual r[S,N,2] and Jacobians wrt the camera tangent block
     (all 8 columns: delta(3), t(3), f, k) and the point: Jc[S,N,2,8], Jp[S,N,2,3].
-    Masked-out observations give zeros."""
+    Masked-out observations give exact zeros, selected with np.where rather than multiplied by the mask: their uv,
+    their point and their camera may be NaN or inf (ba_blocks_ref.c skips them, csrc/ba_obs.h selects)."""
     S, N = mask.shape
     R = poses[:, :, :3]
     t = poses[:, :, 3]
     RX = np.einsum("sij,nj->sni", R, points)
     p = RX + t[:, None, :]
-    m = mask.astype(np.float64)
     pz = np.where(mask, p[..., 2], 1.0)
     iz = 1.0 / pz
     u = p[..., 0] * iz
@@ -139,7 +139,7 @@ def residuals_and_jacobians(poses, intr, points, uv, mask, model):
     k = intr[:, 3][:, None] if model == SIMPLE_RADIAL else np.zeros((S, 1))
     r2 = u * u + v * v
     d = 1.0 + k * r2
-    res = np.stack([f * d * u + cx - uv[..., 0], f * d * v + cy - uv[..., 1]], axis=-1) * m[..., None]
+    res = np.stack([f * d * u + cx - uv[..., 0], f * d * v + cy - uv[..., 1]], axis=-1)
 
     # d(uhat,vhat)/d(u,v) = f * A
     a00 = f * (d + 2.0 * k * u * u)
@@ -153,7 +153,6 @@ def residuals_and_jacobians(poses, intr, points, uv, mask, model):
     Jproj[..., 1, 0] = a01 * iz
     Jproj[..., 1, 1] = a11 * iz
     Jproj[..., 1, 2] = -(a01 * u + a11 * v) * iz
-    Jproj *= m[..., None, None]
 
     Jp = np.einsum("snij,sjk->snik", Jproj, R)
     Jc = np.zeros((S, N, 2, 8))
@@ -163,12 +162,13 @@ def residuals_and_jacobians(poses, intr, points, uv, mask, model):
     Jc[..., 1] = 2.0 * (a3[..., None] * Jproj[..., 0] - a1[..., None] * Jproj[..., 2])
     Jc[..., 2] = 2.0 * (-a2[..., None] * Jproj[..., 0] + a1[..., None] * Jproj[..., 1])
     Jc[..., 3:6] = Jproj
-    Jc[..., 0, 6] = d * u * m
-    Jc[..., 1, 6] = d * v * m
+    Jc[..., 0, 6] = d * u
+    Jc[..., 1, 6] = d * v
     if model == SIMPLE_RADIAL:
-        Jc[..., 0, 7] = f * u * r2 * m
-        Jc[..., 1, 7] = f * v * r2 * m
-    return res, Jc, Jp
+        Jc[..., 0, 7] = f * u * r2
+        Jc[..., 1, 7] = f * v * r2
+    keep = mask[..., None, None]
+    return np.where(mask[..., None], res, 0.0), np.where(keep, Jc, 0.0), np.where(keep, Jp, 0.0)
 
 
 def build_blocks(poses, intr, points, uv, mask, model, mode, point_const=None):
@@ -180,7 +180,7 @@ def build_blocks(poses, intr, points, uv, mask, model, mode, point_const=None):
     ni = n_intr(model)
     res, Jc8, Jp = residuals_and_jacobians(poses, intr, points, uv, mask, model)
     if point_const is not None:
-        Jp = Jp * (~point_const)[None, :, None, None]
+        Jp = np.where(np.asarray(point_const, dtype=bool)[None, :, None, None], 0.0, Jp)
     Jc = Jc8[..., :dc]
     out = {
         "cost": 0.5 * float(np.sum(res * res)),
@@ -247,9 +247,9 @@ def build_blocks_c(poses, intr, points, uv, mask, model, mode, point_const=None)
 
 
 def cost_only(poses, intr, points, uv, mask, model):
-    uvh, _ = project(poses, intr, points, model)
-    r = (uvh - uv) * mask[..., None]
-    r = np.where(mask[..., None], r, 0.0)
+    with np.errstate(invalid="ignore", over="ignore"):
+        uvh, _ = project(poses, intr, points, model)
+        r = np.where(mask[..., None], uvh - uv, 0.0)
     return 0.5 * float(np.sum(r * r))
 
 
@@ -275,20 +275,25 @@ def exp_so3(phi):
 
 
 def apply_step(poses, intr, points, d_cam, d_shared, d_pts, model, mode):
-    """x (+) delta in the tangent parameterisation above.  d_cam [S,dc], d_shared [ns], d_pts [N,3]."""
+    """x (+) delta in the tangent parameterisation above.  d_cam [S,dc], d_shared [ns], d_pts [N,3].  A parameter whose
+    step is exactly zero is copied (as cam_update_kernel / point_step_kernel do), so a constant or unobserved one comes
+    back as given even when it is NaN or inf."""
     ni = n_intr(model)
+    add = lambda x, d: np.where(d == 0.0, x, x + d)
     new_poses = poses.copy()
-    new_poses[:, :, :3] = exp_so3(2.0 * d_cam[:, 0:3]) @ poses[:, :, :3]
-    new_poses[:, :, 3] = poses[:, :, 3] + d_cam[:, 3:6]
+    rot = np.any(d_cam[:, 0:3] != 0.0, axis=1)[:, None, None]
+    with np.errstate(invalid="ignore"):
+        new_poses[:, :, :3] = np.where(rot, exp_so3(2.0 * d_cam[:, 0:3]) @ poses[:, :, :3], poses[:, :, :3])
+    new_poses[:, :, 3] = add(poses[:, :, 3], d_cam[:, 3:6])
     new_intr = intr.copy()
     cols = [0, 3][:ni]
     if mode == INTR_PER_FRAME:
         for j, c in enumerate(cols):
-            new_intr[:, c] += d_cam[:, 6 + j]
+            new_intr[:, c] = add(intr[:, c], d_cam[:, 6 + j])
     elif mode == INTR_SHARED:
         for j, c in enumerate(cols):
-            new_intr[:, c] += d_shared[j]
-    return new_poses, new_intr, points + d_pts
+            new_intr[:, c] = add(intr[:, c], d_shared[j])
+    return new_poses, new_intr, add(points, d_pts)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -383,12 +388,20 @@ def lm_solve(poses, intr, points, uv, mask, model, mode, param_const=None, point
     S, N = mask.shape
     dc, ns = dims(model, mode)
     D = S * dc + ns
+    ar = allreduce.sum if allreduce is not None else (lambda a: a)
+    armax = allreduce.max if allreduce is not None else (lambda a: a)
     if param_const is None:
         param_const = default_param_const(S, model, mode)
     if point_const is None:
         point_const = np.zeros(N, dtype=bool)
-    ar = allreduce.sum if allreduce is not None else (lambda a: a)
-    armax = allreduce.max if allreduce is not None else (lambda a: a)
+    # A point that no valid observation sees, and every camera parameter of a frame that sees nothing, is not in Ceres'
+    # problem: constant here whatever the flags say, so that its values (NaN or inf allowed) reach neither |x| nor the step.
+    # Frames are summed over track shards (a frame is in the problem if any shard sees it).
+    mask = np.asarray(mask, dtype=bool)
+    point_const = np.asarray(point_const, dtype=bool) | ~mask.any(axis=0)
+    frame_seen = np.asarray(ar(mask.any(axis=1).astype(np.float64))) != 0.0
+    param_const = np.asarray(param_const, dtype=bool).copy()
+    param_const[:S * dc] |= np.repeat(~frame_seen, dc)
     free_c = ~param_const
 
     def evaluate(poses, intr, points):
@@ -484,7 +497,7 @@ def lm_solve(poses, intr, points, uv, mask, model, mode, param_const=None, point
         d_p = np.einsum("nij,nj->ni", M, np.einsum("nji,nj->ni", M, ypt))
         # ---- model cost change: 0.5*(delta^T D^2 delta - delta^T g)  (== -(J d)^T (f + J d/2))
         dps = d_p / np.where(sc_p == 0, 1.0, sc_p)
-        pt_terms = np.array([np.sum(dps * dps * dpp / radius * (~point_const)[:, None]) - np.sum(d_p * blk["g_p"]),
+        pt_terms = np.array([np.sum(np.where(point_const[:, None], 0.0, dps * dps * dpp / radius)) - np.sum(d_p * blk["g_p"]),
                              np.sum(d_p * d_p)])
         pt_terms = ar(pt_terms)
         quad = np.sum(dcs * dcs * dcc / radius * free_c) - np.sum(d_c * gc_glob) + pt_terms[0]

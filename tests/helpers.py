@@ -40,6 +40,29 @@ def banded_ba_case(S, N, camera_type, mode, life, seed=0, mask_seed=0):
     return c
 
 
+def hidden_case(S, N, cam, mode, seed, point_value, uv_value, n_hidden=3, hidden_frame=None, case=None):
+    """(problem with hidden values, its clean twin, hidden point indices).  The hidden points' columns are masked out
+    entirely; a third of the other masked slots get uv_value; hidden_frame (if given) loses every observation and gets a
+    NaN pose.  case: start from this ba_case / banded_ba_case instead of a new ba_case (S, N, cam, mode unused)."""
+    c = ba_case(S, N, cam, mode, seed=seed) if case is None else case
+    mask = c["mask"].copy()
+    rng = np.random.default_rng(seed)
+    hidden = rng.choice(N, size=n_hidden, replace=False)
+    mask[:, hidden] = False
+    if hidden_frame is not None:
+        mask[hidden_frame] = False
+    clean = dict(c, mask=mask, uv=np.where(mask[..., None], c["uv"], 0.0), points=c["points"].copy())
+    clean["points"][hidden] = [0.0, 0.0, 1.0]
+    dirty = dict(clean, uv=clean["uv"].copy(), points=clean["points"].copy(), poses=c["poses"].copy())
+    dirty["points"][hidden] = point_value
+    off = np.argwhere(~mask)
+    pick = off[rng.uniform(size=len(off)) < 1.0 / 3.0]
+    dirty["uv"][pick[:, 0], pick[:, 1]] = uv_value
+    if hidden_frame is not None:
+        dirty["poses"][hidden_frame] = np.nan
+    return dirty, clean, hidden
+
+
 def to_dev(a, dev, dtype=None):
     import torch
     t = torch.from_numpy(np.ascontiguousarray(a))

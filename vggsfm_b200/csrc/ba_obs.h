@@ -16,14 +16,15 @@ struct BlkCfg {
   static constexpr int KR = DC + NPACK + 6 * NS;   // per-frame camera record length
 };
 
-// One observation, branch-free: residual and Jacobian columns, all scaled by the validity mask (an invalid
-// observation computes on a safe depth and contributes exact zeros).  jc: delta(3), t(3), f, k; jx: point(3).
+// One observation, branch-free: residual and Jacobian columns.  An invalid observation computes on a safe depth and its
+// outputs are SELECTED to exact zeros, never multiplied by the mask: its uv, its point and its camera are then free to be
+// anything, NaN and inf included (a point or a frame that no valid observation sees is not in the problem, and 0 * NaN
+// would put it back).  jc: delta(3), t(3), f, k; jx: point(3).
 // cam: R (row-major 3x4 with t), f, cx, cy, k at cam[0], cam[cs], ..., cam[15 cs]; pc: the point is held constant.
 template <int MODEL>
 __device__ __forceinline__ void obs_math(const double* cam, int cs, double X0, double X1, double X2, bool pc, float ox,
                                          float oy, bool valid, double* jc0, double* jc1, double* jx0, double* jx1,
                                          double& rx, double& ry) {
-  const double m = valid ? 1.0 : 0.0;
   const double R00 = cam[0 * cs], R01 = cam[1 * cs], R02 = cam[2 * cs], t0_ = cam[3 * cs];
   const double R10 = cam[4 * cs], R11 = cam[5 * cs], R12 = cam[6 * cs], t1_ = cam[7 * cs];
   const double R20 = cam[8 * cs], R21 = cam[9 * cs], R22 = cam[10 * cs], t2_ = cam[11 * cs];
@@ -38,7 +39,7 @@ __device__ __forceinline__ void obs_math(const double* cam, int cs, double X0, d
   const double u = px * iz, w_ = py * iz;
   const double r2 = u * u + w_ * w_;
   const double d = 1.0 + kk * r2;
-  rx = valid ? (fo * d * u + cx - (double)ox) : 0.0;            // select, not multiply: ox/oy of a masked slot may be anything
+  rx = valid ? (fo * d * u + cx - (double)ox) : 0.0;
   ry = valid ? (fo * d * w_ + cy - (double)oy) : 0.0;
   double a00, a01, a11;
   if (MODEL == VGG_SIMPLE_RADIAL) {
@@ -48,25 +49,25 @@ __device__ __forceinline__ void obs_math(const double* cam, int cs, double X0, d
   } else {
     a00 = fo; a01 = 0.0; a11 = fo;
   }
-  // Jproj (2x3) = f*A * iz*[[1,0,-u],[0,1,-v]], masked
-  const double izm = iz * m;
-  const double j00 = a00 * izm, j01 = a01 * izm, j02 = -(a00 * u + a01 * w_) * izm;
-  const double j10 = a01 * izm, j11 = a11 * izm, j12 = -(a01 * u + a11 * w_) * izm;
-  const double b1 = 2.0 * a1, b2 = 2.0 * a2, b3 = 2.0 * a3;
+  // Jproj (2x3) = f*A * iz*[[1,0,-u],[0,1,-v]] and the rotated point, selected to zero for an invalid observation: the
+  // products below are then exact zeros whatever the point and the camera hold
+  const double j00 = valid ? a00 * iz : 0.0, j01 = valid ? a01 * iz : 0.0, j02 = valid ? -(a00 * u + a01 * w_) * iz : 0.0;
+  const double j10 = valid ? a01 * iz : 0.0, j11 = valid ? a11 * iz : 0.0, j12 = valid ? -(a01 * u + a11 * w_) * iz : 0.0;
+  const double b1 = valid ? 2.0 * a1 : 0.0, b2 = valid ? 2.0 * a2 : 0.0, b3 = valid ? 2.0 * a3 : 0.0;
   jc0[0] = b2 * j02 - b3 * j01;  jc1[0] = b2 * j12 - b3 * j11;
   jc0[1] = b3 * j00 - b1 * j02;  jc1[1] = b3 * j10 - b1 * j12;
   jc0[2] = b1 * j01 - b2 * j00;  jc1[2] = b1 * j11 - b2 * j10;
   jc0[3] = j00; jc0[4] = j01; jc0[5] = j02;
   jc1[3] = j10; jc1[4] = j11; jc1[5] = j12;
-  jc0[6] = m * d * u;            jc1[6] = m * d * w_;
-  jc0[7] = m * fo * u * r2;      jc1[7] = m * fo * w_ * r2;
-  const double mq = pc ? 0.0 : 1.0;                              // constant point: no point columns
-  jx0[0] = mq * (j00 * R00 + j01 * R10 + j02 * R20);
-  jx0[1] = mq * (j00 * R01 + j01 * R11 + j02 * R21);
-  jx0[2] = mq * (j00 * R02 + j01 * R12 + j02 * R22);
-  jx1[0] = mq * (j10 * R00 + j11 * R10 + j12 * R20);
-  jx1[1] = mq * (j10 * R01 + j11 * R11 + j12 * R21);
-  jx1[2] = mq * (j10 * R02 + j11 * R12 + j12 * R22);
+  jc0[6] = valid ? d * u : 0.0;            jc1[6] = valid ? d * w_ : 0.0;
+  jc0[7] = valid ? fo * u * r2 : 0.0;      jc1[7] = valid ? fo * w_ * r2 : 0.0;
+  const bool vp = valid && !pc;                                  // constant point: no point columns
+  jx0[0] = vp ? j00 * R00 + j01 * R10 + j02 * R20 : 0.0;
+  jx0[1] = vp ? j00 * R01 + j01 * R11 + j02 * R21 : 0.0;
+  jx0[2] = vp ? j00 * R02 + j01 * R12 + j02 * R22 : 0.0;
+  jx1[0] = vp ? j10 * R00 + j11 * R10 + j12 * R20 : 0.0;
+  jx1[1] = vp ? j10 * R01 + j11 * R11 + j12 * R21 : 0.0;
+  jx1[2] = vp ? j10 * R02 + j11 * R12 + j12 * R22 : 0.0;
 }
 
 // one entry of the coupling block W = J_c^T J_p: row i of the camera columns (6 + intrinsics), point column c

@@ -528,14 +528,19 @@ __global__ void __launch_bounds__(BS_W * 32) backsub_kernel(
   }
 }
 
-// d_p = M M^T (-(g_p + w)); candidate = X + d_p; scal[2] += sum dps^2 dpp/r - d_p.g_p; scal[3] += |d_p|^2
+// d_p = M M^T (-(g_p + w)); candidate = X + d_p; scal[2] += sum dps^2 dpp/r - d_p.g_p; scal[3] += |d_p|^2.  A constant
+// point (point_const: given constant, or seen by no valid observation) is SELECTED out: its step and both terms are
+// exact zeros and its candidate is X bit for bit, whatever wacc, g_p and sc_p hold for it (M = 0 alone would give
+// 0 * NaN = NaN for a point whose coordinates are not in the problem).
 __global__ void point_step_kernel(int N, const double* __restrict__ M, const double* __restrict__ g_p,
                                   const double* __restrict__ wacc, const double* __restrict__ sc_p,
-                                  const double* __restrict__ dpp, const double* __restrict__ X, double radius,
-                                  double* __restrict__ Xc, double* __restrict__ scal) {
+                                  const double* __restrict__ dpp, const uint8_t* __restrict__ point_const,
+                                  const double* __restrict__ X, double radius, double* __restrict__ Xc,
+                                  double* __restrict__ scal) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   double a = 0, b = 0;
   if (n < N) {
+    const bool pc = point_const && point_const[n];
     const double* m = M + (size_t)n * 9;
     const double g0 = g_p[n * 3], g1 = g_p[n * 3 + 1], g2 = g_p[n * 3 + 2];
     const double y0 = -(g0 + wacc[n * 3]), y1 = -(g1 + wacc[n * 3 + 1]), y2 = -(g2 + wacc[n * 3 + 2]);
@@ -546,14 +551,14 @@ __global__ void point_step_kernel(int N, const double* __restrict__ M, const dou
     const double d0 = m[0] * t0 + m[1] * t1 + m[2] * t2;
     const double d1 = m[4] * t1 + m[5] * t2;
     const double d2 = m[8] * t2;
-    Xc[n * 3] = X[n * 3] + d0;
-    Xc[n * 3 + 1] = X[n * 3 + 1] + d1;
-    Xc[n * 3 + 2] = X[n * 3 + 2] + d2;
+    Xc[n * 3] = pc ? X[n * 3] : X[n * 3] + d0;
+    Xc[n * 3 + 1] = pc ? X[n * 3 + 1] : X[n * 3 + 1] + d1;
+    Xc[n * 3 + 2] = pc ? X[n * 3 + 2] : X[n * 3 + 2] + d2;
     const double s0 = sc_p[n * 3], s1 = sc_p[n * 3 + 1], s2 = sc_p[n * 3 + 2];
     const double e0 = d0 / s0, e1 = d1 / s1, e2 = d2 / s2;
-    a = (e0 * e0 * dpp[n * 3] + e1 * e1 * dpp[n * 3 + 1] + e2 * e2 * dpp[n * 3 + 2]) / radius -
-        (d0 * g0 + d1 * g1 + d2 * g2);
-    b = d0 * d0 + d1 * d1 + d2 * d2;
+    a = pc ? 0.0 : (e0 * e0 * dpp[n * 3] + e1 * e1 * dpp[n * 3 + 1] + e2 * e2 * dpp[n * 3 + 2]) / radius -
+                       (d0 * g0 + d1 * g1 + d2 * g2);
+    b = pc ? 0.0 : d0 * d0 + d1 * d1 + d2 * d2;
   }
   a = warp_sum(a); b = warp_sum(b);
   if ((threadIdx.x & 31) == 0) {
@@ -562,7 +567,9 @@ __global__ void point_step_kernel(int N, const double* __restrict__ M, const dou
   }
 }
 
-// candidate cameras: R <- Exp(2 delta) R, t <- t + dt, intrinsics
+// candidate cameras: R <- Exp(2 delta) R, t <- t + dt, intrinsics.  A parameter whose step is exactly zero (a constant
+// one, and every parameter of a frame that no valid observation sees) is copied, so that it comes back bit for bit as
+// given even when it is NaN or inf.
 __global__ void cam_update_kernel(int S, int dc, int ns, int model, const double* __restrict__ d_c,
                                   const double* __restrict__ poses, const double* __restrict__ intr,
                                   double* __restrict__ poses_c, double* __restrict__ intr_c) {
@@ -581,6 +588,7 @@ __global__ void cam_update_kernel(int S, int dc, int ns, int model, const double
     b = (1.0 - cos(th)) / th2;
   }
   // E = I + a K + b K^2
+  const bool rot = p0 != 0.0 || p1 != 0.0 || p2 != 0.0;
   double E[9];
   E[0] = 1.0 + b * (-(p1 * p1 + p2 * p2)); E[1] = -a * p2 + b * p0 * p1;           E[2] = a * p1 + b * p0 * p2;
   E[3] = a * p2 + b * p0 * p1;             E[4] = 1.0 + b * (-(p0 * p0 + p2 * p2)); E[5] = -a * p0 + b * p1 * p2;
@@ -590,19 +598,17 @@ __global__ void cam_update_kernel(int S, int dc, int ns, int model, const double
 #pragma unroll
   for (int i = 0; i < 3; ++i)
 #pragma unroll
-    for (int j = 0; j < 3; ++j) Q[i * 4 + j] = E[i * 3] * P[j] + E[i * 3 + 1] * P[4 + j] + E[i * 3 + 2] * P[8 + j];
-  Q[3] = P[3] + d[3];
-  Q[7] = P[7] + d[4];
-  Q[11] = P[11] + d[5];
+    for (int j = 0; j < 3; ++j)
+      Q[i * 4 + j] = rot ? E[i * 3] * P[j] + E[i * 3 + 1] * P[4 + j] + E[i * 3 + 2] * P[8 + j] : P[i * 4 + j];
+  Q[3] = d[3] != 0.0 ? P[3] + d[3] : P[3];
+  Q[7] = d[4] != 0.0 ? P[7] + d[4] : P[7];
+  Q[11] = d[5] != 0.0 ? P[11] + d[5] : P[11];
   const int ni = (model == VGG_SIMPLE_PINHOLE) ? 1 : 2;
   double f = intr[s * 4], k = intr[s * 4 + 3];
-  if (dc > 6) {
-    f += d[6];
-    if (ni > 1) k += d[7];
-  } else if (ns > 0) {
-    const double* dsh = d_c + (size_t)S * dc;
-    f += dsh[0];
-    if (ni > 1) k += dsh[1];
+  const double* di = dc > 6 ? d + 6 : d_c + (size_t)S * dc;   // per-frame or shared intrinsics step
+  if (dc > 6 || ns > 0) {
+    if (di[0] != 0.0) f += di[0];
+    if (ni > 1 && di[1] != 0.0) k += di[1];
   }
   intr_c[s * 4] = f;
   intr_c[s * 4 + 1] = intr[s * 4 + 1];
@@ -765,8 +771,9 @@ int launch_backsub(const vgg_ba_problem* p, const double* d_c, double* wacc, con
   return VGG_OK;
 }
 int launch_point_step(int N, const double* M, const double* g_p, const double* wacc, const double* sc_p,
-                      const double* dpp, const double* X, double radius, double* Xc, double* scal, cudaStream_t st) {
-  point_step_kernel<<<(N + 127) / 128, 128, 0, st>>>(N, M, g_p, wacc, sc_p, dpp, X, radius, Xc, scal);
+                      const double* dpp, const uint8_t* point_const, const double* X, double radius, double* Xc,
+                      double* scal, cudaStream_t st) {
+  point_step_kernel<<<(N + 127) / 128, 128, 0, st>>>(N, M, g_p, wacc, sc_p, dpp, point_const, X, radius, Xc, scal);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }

@@ -45,7 +45,8 @@ int launch_cam_step(int D, const double* dcs, size_t dcs_stride, const double* s
                     cudaStream_t st);
 int launch_backsub(const vgg_ba_problem* p, const double* d_c, double* wacc, const int* fg_tracks, cudaStream_t st);
 int launch_point_step(int N, const double* M, const double* g_p, const double* wacc, const double* sc_p,
-                      const double* dpp, const double* X, double radius, double* Xc, double* scal, cudaStream_t st);
+                      const double* dpp, const uint8_t* point_const, const double* X, double radius, double* Xc,
+                      double* scal, cudaStream_t st);
 int launch_cam_update(int S, int dc, int ns, int model, const double* d_c, const double* poses, const double* intr,
                       double* poses_c, double* intr_c, cudaStream_t st);
 int launch_extract_gvec(int S, int dc, int ns, int KR, const double* camrec, const double* shared_in, double* gvec,
@@ -173,6 +174,7 @@ struct Layout {
   double *packed;    // [24] scalars gathered for the host
   double *chol_diag;
   int *dev_info;
+  uint8_t *pconst, *point_const;   // [Dpad], [N]: the solve's constant flags (observed_kernel / effective_const_kernel)
   size_t bytes;
 };
 
@@ -212,6 +214,8 @@ static int make_layout(int S, int N, int model, int mode, void* base, size_t cap
   L->packed = c.take<double>(32);
   L->chol_diag = c.take<double>(chol_workspace_doubles(L->D + 1));
   L->dev_info = c.take<int>(4);
+  L->pconst = c.take<uint8_t>(L->Dpad);
+  L->point_const = c.take<uint8_t>((size_t)N);
   L->bytes = align_up(c.off, 256);
   if (base && c.off > cap) {
     set_error("workspace too small: need %zu bytes, have %zu", c.off, cap);
@@ -307,6 +311,35 @@ __global__ void __launch_bounds__(256) frame_point_range_kernel(int S, int N, co
     out[2 * s] = s_lo[0];
     out[2 * s + 1] = s_hi[0];
   }
+}
+
+// Which points and frames at least one valid observation sees: point_seen[n] = 1 / frame_seen[s] = 1.0 (both zeroed
+// beforehand; frame_seen is a double so that track shards can sum it with the small all-reduce).  grid.y takes the frames
+// in chunks of OBS_FRAMES, one lane per point, so the mask reads are coalesced.
+constexpr int OBS_FRAMES = 16;
+__global__ void __launch_bounds__(256) observed_kernel(int S, int N, const uint8_t* __restrict__ mask,
+                                                       uint8_t* __restrict__ point_seen, double* __restrict__ frame_seen) {
+  const int n = blockIdx.x * 256 + threadIdx.x;
+  const int s0 = blockIdx.y * OBS_FRAMES, s1 = min(S, s0 + OBS_FRAMES);
+  bool seen = false;
+  for (int s = s0; s < s1; ++s) {
+    const bool m = n < N && mask[(size_t)s * N + n] != 0;
+    seen = seen || m;
+    if (__any_sync(0xffffffffu, m) && (threadIdx.x & 31) == 0) frame_seen[s] = 1.0;
+  }
+  if (seen) point_seen[n] = 1;
+}
+
+// The constant flags the solve runs with: a point that no valid observation sees, and every camera parameter of a frame
+// that sees nothing, count as constant whatever the caller's flags say.  Ceres leaves such blocks out of the problem, so
+// they must not reach |x| (parameter tolerance), the step or the gradient norm -- their values may be NaN or inf.
+// point_const holds point_seen on entry and is rewritten in place.
+__global__ void effective_const_kernel(int S, int N, int dc, int D, const uint8_t* __restrict__ param_const,
+                                       const uint8_t* __restrict__ user_point_const, const double* __restrict__ frame_seen,
+                                       uint8_t* __restrict__ pconst, uint8_t* __restrict__ point_const) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < D) pconst[i] = param_const[i] || (i < S * dc && frame_seen[i / dc] == 0.0);
+  if (i < N) point_const[i] = (user_point_const && user_point_const[i]) || !point_const[i];
 }
 
 // Per 128-column row block of Zt: the 64-row k-block range outside which the block is exactly zero (Zt row 3n+c belongs to
@@ -630,6 +663,13 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     fab.epoch = &fabric_epochs[fabric->peer_base[fabric->rank]];
     fab.err = L.dev_info + 2;
   }
+  // the constant flags of this solve (unobserved points and frames added); every kernel below reads these, not the
+  // caller's.  Frames are summed over track shards: a frame is in the problem if any rank sees it.
+  const vgg_ba_problem* const caller = prob;
+  vgg_ba_problem pe = *prob;
+  pe.param_const = L.pconst;
+  pe.point_const = L.point_const;
+  prob = &pe;
   BandPlan band;
   if ((rc = compute_band_hint(prob, dc, D, L.Dpad, L.Kpad, allreduce != nullptr || fabric != nullptr, st, &band))) return rc;
   g_band_last = band;
@@ -643,6 +683,17 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     if (allreduce) return allreduce(ar_user, vec, count, op, st);
     return VGG_OK;
   };
+
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.point_const, 0, (size_t)N, st));
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.small, 0, sizeof(double) * (8 + (size_t)L.Dpad), st));
+  observed_kernel<<<dim3((N + 255) / 256, (S + OBS_FRAMES - 1) / OBS_FRAMES), 256, 0, st>>>(S, N, pe.mask, L.point_const,
+                                                                                           L.small + 8);
+  VGG_LAUNCH_CHECK();
+  if ((rc = reduce_small(L.small, 8 + (size_t)L.Dpad, 0))) return rc;
+  effective_const_kernel<<<(std::max(D, N) + 255) / 256, 256, 0, st>>>(S, N, dc, D, caller->param_const,
+                                                                       caller->point_const, L.small + 8, L.pconst,
+                                                                       L.point_const);
+  VGG_LAUNCH_CHECK();
 
   EventPair evs;
   VGG_CUDA_CHECK(cudaEventCreate(&evs.a));
@@ -789,8 +840,8 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
                               opt.max_lm_diagonal, L.d_c, L.scal, st)))
       return rc;
     if ((rc = launch_backsub(&pcur, L.d_c, L.wacc, band.dev.fg_tracks, st))) return rc;
-    if ((rc = launch_point_step(N, L.M, L.blk[cur].g_p, L.wacc, L.sc_p, L.dpp, L.points[cur], radius, L.points[cand],
-                                L.scal, st)))
+    if ((rc = launch_point_step(N, L.M, L.blk[cur].g_p, L.wacc, L.sc_p, L.dpp, pe.point_const, L.points[cur], radius,
+                                L.points[cand], L.scal, st)))
       return rc;
     if ((rc = launch_cam_update(S, dc, ns, prob->camera_model, L.d_c, L.poses[cur], L.intr[cur], L.poses[cand],
                                 L.intr[cand], st)))
