@@ -5,7 +5,8 @@
 Profiles one `lm_solve` of bench.py's C3 problem (after one warm-up solve) and prints, per panel step b (median over
 the factorisations of the solve, plus the last factorisation in full):
   grid      CTAs of chol_panel_kernel b
-  panel     start to end of the panel kernel (us)
+  panel     start to end of the panel kernel (us); a kernel starts with its first CTA, so panel CTAs that wait for an
+            SM held by update CTAs lengthen this column, not the gap
   gap       end of panel b to start of panel b+1 (us)
   upd@start chol_update_kernel launches still running when panel b starts, and how long the last of them still runs
 The factorisation span is the first panel's start to the end of the last chol_* kernel before the next factorisation.

@@ -12,8 +12,9 @@
 //                       (16, 20, ... 32 rows) is chosen per panel such that the 1 + chunks CTAs fit on the device's SMs
 //                       in one wave: a second wave would repeat the whole POTRF128 on the critical path.
 //   chol_update_kernel  A22 -= P P^T on 64x64 tiles for block columns >= k+2, on low-priority side streams; one K half of
-//                       both operands in shared memory at a time (68 KB) so that its CTAs run NEXT TO the panel CTAs of
-//                       the following step (<= 155 KB with xr <= 20) on the same SMs.
+//                       both operands in shared memory at a time (68 KB).  Its grids are capped at what the SMs hold at
+//                       once and walk their tiles grid-stride, so no update CTA is left queued when the next panel's
+//                       CTAs are: those go first (graph node priorities) onto whichever SMs free up.
 // Every MMA is mma.sync.m16n8k16.f64 (dmma_m16n8k16, full FP64 tensor rate on sm_90; m8n8k4 runs at half of it).
 // The whole launch sequence is captured once per (matrix, order) into a CUDA graph.  Matrices of fewer than three blocks
 // are factored in program order (no fused update, no side streams), launched directly.
@@ -609,8 +610,11 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
   }
 }
 
-// A[t0.., t0..] -= P P^T (lower part), P = A[t0.., k0..k0+127]: one 64 x 64 tile (bi, bj), bj <= bi, per CTA; 8 warps
-// 2 x 4, warp tile 32 x 16 = two m16 x two n8 DMMA tiles.  Which tiles (tile columns counted from t0):
+// A[t0.., t0..] -= P P^T (lower part), P = A[t0.., k0..k0+127]: 64 x 64 tiles (bi, bj), bj <= bi, tile t of the mode's
+// list for t = blockIdx.x, blockIdx.x + gridDim.x, ... < ntiles (the fused schedule caps the grid at what the SMs
+// hold at once and lets each CTA walk several tiles, see chol_enqueue); 8 warps 2 x 4, warp tile 32 x 16 = two m16 x
+// two n8 DMMA tiles.
+// Which tiles (tile columns counted from t0):
 //   CU_ALL   every tile (the program-order schedule of matrices with fewer than three blocks)
 //   CU_NEXT  tile columns 2 and 3 = block column k+2, which the fused panel kernel of the next step is adding into at
 //            the same time: f64 REDs
@@ -623,15 +627,22 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
 // whole step and the trailing update ran after them, not beside them -- the factorisation took the SUM of all its kernels.
 constexpr int CUD = 68;
 enum { CU_ALL = 0, CU_NEXT = 1, CU_REST = 2 };
-__global__ void __launch_bounds__(C_THREADS, 2) chol_update_kernel(int n, int lda, int k0, int t0, int mode,
+__global__ void __launch_bounds__(C_THREADS, 2) chol_update_kernel(int n, int lda, int k0, int t0, int mode, int ntiles,
                                                                     double* __restrict__ A, int band_end, int arrow_lo,
                                                                     int all_red) {
   extern __shared__ __align__(16) double cu_smem[];
   double* As = cu_smem;                         // [64][CUD]
   double* Bs = cu_smem + CT * CUD;              // [64][CUD]
-  int bi, bj;
-  {
-    const int t = blockIdx.x;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  // banded matrices: 64-row tile v of the ACTIVE rows -- the band part [t0, band_end) first, then the arrow part
+  // [arrow_lo, n) (band_end = n: the plain dense mapping)
+  const int T1v = band_end >= n ? (1 << 30) : (band_end - t0) / 64;
+  auto vrow = [&](int v) { return v < T1v ? t0 + v * 64 : arrow_lo + (v - T1v) * 64; };
+  const int wm = warp / 4, wn = warp % 4;
+  const int g = lane >> 2, q = lane & 3;
+#pragma unroll 1
+  for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    int bi, bj;
     if (mode == CU_NEXT) {
       const int T = (max(0, min(band_end, n) - t0) + 63) / 64 + (band_end >= n ? 0 : (n - arrow_lo + 63) / 64);
       if (t < T - 2) { bi = 2 + t; bj = 2; }
@@ -645,86 +656,79 @@ __global__ void __launch_bounds__(C_THREADS, 2) chol_update_kernel(int n, int ld
       bi += skip;
       bj += skip;
     }
-  }
-  const bool diag = bi == bj;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  // banded matrices: 64-row tile v of the ACTIVE rows -- the band part [t0, band_end) first, then the arrow part
-  // [arrow_lo, n) (band_end = n: the plain dense mapping)
-  const int T1v = band_end >= n ? (1 << 30) : (band_end - t0) / 64;
-  auto vrow = [&](int v) { return v < T1v ? t0 + v * 64 : arrow_lo + (v - T1v) * 64; };
-  const int ri = vrow(bi), rj = vrow(bj);
-  const double* bs = diag ? As : Bs;
-  const int wm = warp / 4, wn = warp % 4;
-  const int g = lane >> 2, q = lane & 3;
-  double c[2][2][4];
+    const bool diag = bi == bj;
+    const int ri = vrow(bi), rj = vrow(bj);
+    const double* bs = diag ? As : Bs;
+    double c[2][2][4];
 #pragma unroll
-  for (int i = 0; i < 2; ++i)
+    for (int i = 0; i < 2; ++i)
 #pragma unroll
-    for (int j = 0; j < 2; ++j) c[i][j][0] = c[i][j][1] = c[i][j][2] = c[i][j][3] = 0.0;
-  const double* arow = As + (wm * 32 + g) * CUD + q;
-  const double* brow = bs + (wn * 16 + g) * CUD + q;
+      for (int j = 0; j < 2; ++j) c[i][j][0] = c[i][j][1] = c[i][j][2] = c[i][j][3] = 0.0;
+    const double* arow = As + (wm * 32 + g) * CUD + q;
+    const double* brow = bs + (wn * 16 + g) * CUD + q;
 #pragma unroll 1
-  for (int half = 0; half < 2; ++half) {
-    if (half) __syncthreads();                      // everyone is done with the first half's fragments
-    // panel rows, row-major (k contiguous)
-    for (int e = tid; e < 2 * CT * 16; e += C_THREADS) {
-      const int row = e >> 4, ch = (e & 15) * 4;     // 4 doubles (two 16-byte chunks) per thread-step
-      const bool isA = row < CT;
-      if (!isA && diag) continue;
-      const int grow = isA ? ri + row : rj + (row - CT);
-      double* dst = (isA ? As + row * CUD : Bs + (row - CT) * CUD) + ch;
-      if (grow < n) {
-        const double* src = A + (size_t)grow * lda + k0 + half * 64 + ch;
-        cp_async16(dst, src);
-        cp_async16(dst + 2, src + 2);
-      } else {
-        *reinterpret_cast<double2*>(dst) = make_double2(0.0, 0.0);
-        *reinterpret_cast<double2*>(dst + 2) = make_double2(0.0, 0.0);
+    for (int half = 0; half < 2; ++half) {
+      if (half || t != (int)blockIdx.x) __syncthreads();   // everyone is done with the previous half's fragments
+      // panel rows, row-major (k contiguous)
+      for (int e = tid; e < 2 * CT * 16; e += C_THREADS) {
+        const int row = e >> 4, ch = (e & 15) * 4;     // 4 doubles (two 16-byte chunks) per thread-step
+        const bool isA = row < CT;
+        if (!isA && diag) continue;
+        const int grow = isA ? ri + row : rj + (row - CT);
+        double* dst = (isA ? As + row * CUD : Bs + (row - CT) * CUD) + ch;
+        if (grow < n) {
+          const double* src = A + (size_t)grow * lda + k0 + half * 64 + ch;
+          cp_async16(dst, src);
+          cp_async16(dst + 2, src + 2);
+        } else {
+          *reinterpret_cast<double2*>(dst) = make_double2(0.0, 0.0);
+          *reinterpret_cast<double2*>(dst + 2) = make_double2(0.0, 0.0);
+        }
+      }
+      cp_async_commit();
+      cp_async_wait<0>();
+      __syncthreads();
+#pragma unroll 2
+      for (int kk = 0; kk < 64; kk += 16) {
+        double a[2][8], b[2][4];
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int e = 0; e < 8; ++e) a[i][e] = arow[(i * 16 + 8 * (e & 1)) * CUD + kk + 4 * (e >> 1)];
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) b[j][e] = brow[j * 8 * CUD + kk + 4 * e];
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int j = 0; j < 2; ++j) dmma_m16n8k16(c[i][j], a[i], b[j]);
       }
     }
-    cp_async_commit();
-    cp_async_wait<0>();
-    __syncthreads();
-#pragma unroll 2
-    for (int kk = 0; kk < 64; kk += 16) {
-      double a[2][8], b[2][4];
+    const bool red = all_red || mode == CU_NEXT || (mode == CU_REST && bj < 6);
 #pragma unroll
-      for (int i = 0; i < 2; ++i)
+    for (int i = 0; i < 2; ++i) {
 #pragma unroll
-        for (int e = 0; e < 8; ++e) a[i][e] = arow[(i * 16 + 8 * (e & 1)) * CUD + kk + 4 * (e >> 1)];
+      for (int h = 0; h < 2; ++h) {
+        const int r = ri + wm * 32 + i * 16 + g + 8 * h;
+        if (r >= n) continue;
 #pragma unroll
-      for (int j = 0; j < 2; ++j)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) b[j][e] = brow[j * 8 * CUD + kk + 4 * e];
-#pragma unroll
-      for (int i = 0; i < 2; ++i)
-#pragma unroll
-        for (int j = 0; j < 2; ++j) dmma_m16n8k16(c[i][j], a[i], b[j]);
-    }
-  }
-  const bool red = all_red || mode == CU_NEXT || (mode == CU_REST && bj < 6);
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int r = ri + wm * 32 + i * 16 + g + 8 * h;
-      if (r >= n) continue;
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int col = rj + wn * 16 + j * 8 + 2 * q;
-        if (col > r) continue;                         // lower triangle only (col <= r < n)
-        double* p = A + (size_t)r * lda + col;
-        const double v0 = c[i][j][2 * h], v1 = c[i][j][2 * h + 1];
-        if (red) {
-          atomicAdd(p, -v0);
-          if (col + 1 <= r) atomicAdd(p + 1, -v1);
-        } else if (col + 1 <= r) {
-          double2 v = *reinterpret_cast<double2*>(p);
-          v.x -= v0;
-          v.y -= v1;
-          *reinterpret_cast<double2*>(p) = v;
-        } else {
-          *p -= v0;
+        for (int j = 0; j < 2; ++j) {
+          const int col = rj + wn * 16 + j * 8 + 2 * q;
+          if (col > r) continue;                         // lower triangle only (col <= r < n)
+          double* p = A + (size_t)r * lda + col;
+          const double v0 = c[i][j][2 * h], v1 = c[i][j][2 * h + 1];
+          if (red) {
+            atomicAdd(p, -v0);
+            if (col + 1 <= r) atomicAdd(p + 1, -v1);
+          } else if (col + 1 <= r) {
+            double2 v = *reinterpret_cast<double2*>(p);
+            v.x -= v0;
+            v.y -= v1;
+            *reinterpret_cast<double2*>(p) = v;
+          } else {
+            *p -= v0;
+          }
         }
       }
     }
@@ -741,9 +745,14 @@ size_t chol_workspace_doubles(int n) {
 
 namespace {
 
+// Kernel roles of the fused schedule, each with its own graph-node priority
+enum { CR_PANEL = 0, CR_NEXT = 1, CR_REST = 2 };
+
 struct CholStreams {
   cudaStream_t side_lo = nullptr, side_mid = nullptr, cap = nullptr;
   cudaEvent_t ev_col = nullptr, ev_upd[2] = {nullptr, nullptr}, ev_bulk[3] = {nullptr, nullptr, nullptr};
+  int prio[3] = {0, 0, 0};          // per role: panel steps the greatest, U1 in the middle, U2 the least
+  int launched[3] = {0, 0, 0};      // per role: kernels captured into the graph being built
   bool ready = false;
 };
 
@@ -752,9 +761,13 @@ int chol_streams(CholStreams** out) {
   if (!s.ready) {
     int lo = 0, hi = 0;
     VGG_CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    // lo = least, hi = greatest priority.  The critical chain (panel steps) is captured on `cap` at the greatest
-    // priority; the fused schedule's bulk updates go to side_lo at the least, so that a panel CTA is placed as soon as
-    // an SM has room for it instead of queueing behind the remaining update CTAs.
+    // lo = least, hi = greatest priority.  The critical chain (panel steps) is captured on `cap`, the bulk updates
+    // on side_mid / side_lo; every captured launch carries its role's priority explicitly (chol_launch), and the
+    // graph is instantiated with node priorities, so that a panel CTA waiting for an SM is placed before any queued
+    // update CTA.
+    s.prio[CR_PANEL] = hi;
+    s.prio[CR_NEXT] = (lo + hi) / 2;
+    s.prio[CR_REST] = lo;
     VGG_CUDA_CHECK(cudaStreamCreateWithPriority(&s.side_lo, cudaStreamNonBlocking, lo));
     VGG_CUDA_CHECK(cudaStreamCreateWithPriority(&s.side_mid, cudaStreamNonBlocking, (lo + hi) / 2));
     VGG_CUDA_CHECK(cudaStreamCreateWithPriority(&s.cap, cudaStreamNonBlocking, hi));
@@ -788,6 +801,23 @@ int chol_set_attrs() {
                                       (int)(sizeof(double) * 2 * CT * CUD)));
   done = true;
   return VGG_OK;
+}
+
+// Launch of one kernel of the fused schedule with its role's priority as a launch attribute: stream capture records
+// it on the graph node, where cudaGraphInstantiateFlagUseNodePriority makes it count.
+template <typename... Params, typename... Args>
+cudaError_t chol_launch(void (*kernel)(Params...), int grid, size_t smem, cudaStream_t st, int priority, Args... args) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributePriority;
+  attr[0].val.priority = priority;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(C_THREADS);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, kernel, args...);
 }
 
 // Ride-along rows per panel CTA for `rows` rows below the diagonal block (in `segs` separately chunked ranges): the
@@ -832,8 +862,13 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
     const int below2 = band_end >= n ? 0 : n - arrow_lo;
     const int xr = chol_panel_rows(below1, below2, &chunks);
     const size_t smem_p = sizeof(double) * (CB + xr) * CLD;
-    const int fuse = lookahead ? 1 : 0;
-    chol_panel_kernel<<<1 + chunks, C_THREADS, smem_p, st>>>(n, lda, k0, A, Ldiag, info, flags, fuse, band_end, arrow_lo, xr);
+    if (lookahead) {
+      VGG_CUDA_CHECK(chol_launch(chol_panel_kernel, 1 + chunks, smem_p, st, cs->prio[CR_PANEL], n, lda, k0, A, Ldiag, info,
+                                 flags, 1, band_end, arrow_lo, xr));
+      ++cs->launched[CR_PANEL];
+    } else {
+      chol_panel_kernel<<<1 + chunks, C_THREADS, smem_p, st>>>(n, lda, k0, A, Ldiag, info, flags, 0, band_end, arrow_lo, xr);
+    }
     VGG_LAUNCH_CHECK();
     return VGG_OK;
   };
@@ -843,7 +878,7 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
     for (int b = 0; b + 1 < nblk; ++b) {
       const int k0 = b * CB, t0 = k0 + CB;
       const int T = (n - t0 + CT - 1) / CT;
-      chol_update_kernel<<<T * (T + 1) / 2, C_THREADS, smem_u, st>>>(n, lda, k0, t0, CU_ALL, A, n, n, 0);
+      chol_update_kernel<<<T * (T + 1) / 2, C_THREADS, smem_u, st>>>(n, lda, k0, t0, CU_ALL, T * (T + 1) / 2, A, n, n, 0);
       VGG_LAUNCH_CHECK();
       if ((rc = panel(b + 1))) return rc;
     }
@@ -852,6 +887,19 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
   // U1 gets one step of slack at medium priority, U2 two steps at the lowest.  r02: as ONE kernel with one step of
   // slack the update of the first six panels did not fit next to the following step and 0.15 ms of it showed up on the
   // critical path.
+  // Update grids are capped so that they are placed whole when they start: U1 at most sms / 8 CTAs, U2 at most the
+  // rest of what the SMs hold at once (two update CTAs per SM), each CTA walking every gridDim-th tile of its list.
+  // With one CTA per tile (595 CTAs after panel 0 at C3) update CTAs were still queued when the next panel kernel
+  // became ready; each SM that an update CTA left took the next queued update CTA, so the panel CTAs, which need
+  // most of an SM, waited for the update queue to run dry: 27 us before step 1, 145 us over steps 0-9.  With capped
+  // grids nothing is queued behind the running update CTAs, and the graph's node priorities put the panel CTAs
+  // ahead of any update CTAs that are queued at the same time.  Factorisation span at C3 (tools/chol_timeline.py; H100
+  // 80GB HBM3, 700 W power limit, 1980 MHz):
+  // 951 us with one CTA per tile, 886 us with the update grids capped at one CTA per SM (more tiles per CTA: the
+  // SMs free up later), 864 us at two per SM; without node priorities capped grids take 1004 us.  The split follows
+  // the tile counts of the first (largest) step at C3, 67 and 528 tiles.
+  const int sms = chol_sms();
+  const int budget_u1 = std::max(1, sms / 8), budget_u2 = std::max(1, 2 * sms - budget_u1);
   bool have_u1[2] = {false, false}, have_u2[3] = {false, false, false};
   for (int b = 0; b + 1 < nblk; ++b) {
     const int k0 = b * CB, t0 = k0 + CB;
@@ -868,13 +916,19 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
       VGG_CUDA_CHECK(cudaStreamWaitEvent(cs->side_mid, cs->ev_col, 0));
       // U2(b-2) still writes block column b+2 with plain read-modify-writes (only its first block column uses REDs)
       if (b >= 2 && have_u2[(b - 2) % 3]) VGG_CUDA_CHECK(cudaStreamWaitEvent(cs->side_mid, cs->ev_bulk[(b - 2) % 3], 0));
-      chol_update_kernel<<<n_u1, C_THREADS, smem_u, cs->side_mid>>>(n, lda, k0, t0, CU_NEXT, A, band_end, arrow_lo, all_red);
+      const int g1 = std::min(n_u1, budget_u1);
+      VGG_CUDA_CHECK(chol_launch(chol_update_kernel, g1, smem_u, cs->side_mid, cs->prio[CR_NEXT], n, lda, k0, t0,
+                                 (int)CU_NEXT, n_u1, A, band_end, arrow_lo, all_red));
+      ++cs->launched[CR_NEXT];
       VGG_LAUNCH_CHECK();
       VGG_CUDA_CHECK(cudaEventRecord(cs->ev_upd[b & 1], cs->side_mid));
       have_u1[b & 1] = true;
       if (n_u2 > 0) {
         VGG_CUDA_CHECK(cudaStreamWaitEvent(cs->side_lo, cs->ev_col, 0));
-        chol_update_kernel<<<n_u2, C_THREADS, smem_u, cs->side_lo>>>(n, lda, k0, t0, CU_REST, A, band_end, arrow_lo, all_red);
+        const int g2 = std::min(n_u2, budget_u2);
+        VGG_CUDA_CHECK(chol_launch(chol_update_kernel, g2, smem_u, cs->side_lo, cs->prio[CR_REST], n, lda, k0, t0,
+                                   (int)CU_REST, n_u2, A, band_end, arrow_lo, all_red));
+        ++cs->launched[CR_REST];
         VGG_LAUNCH_CHECK();
         VGG_CUDA_CHECK(cudaEventRecord(cs->ev_bulk[b % 3], cs->side_lo));
         have_u2[b % 3] = true;
@@ -890,6 +944,32 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
     if (have_u1[i]) VGG_CUDA_CHECK(cudaStreamWaitEvent(st, cs->ev_upd[i], 0));
   for (int i = 0; i < 3; ++i)
     if (have_u2[i]) VGG_CUDA_CHECK(cudaStreamWaitEvent(st, cs->ev_bulk[i], 0));
+  return VGG_OK;
+}
+
+// Every kernel node of the captured factorisation graph must carry its role's priority: count the nodes per priority
+// against the launches per role (the three priorities are distinct on any device with more than two levels).
+int chol_check_priorities(cudaGraph_t graph, const CholStreams* cs) {
+  size_t nn = 0;
+  VGG_CUDA_CHECK(cudaGraphGetNodes(graph, nullptr, &nn));
+  std::vector<cudaGraphNode_t> nodes(nn);
+  VGG_CUDA_CHECK(cudaGraphGetNodes(graph, nodes.data(), &nn));
+  int count[3] = {0, 0, 0}, kernels = 0;
+  for (cudaGraphNode_t node : nodes) {
+    cudaGraphNodeType ty;
+    VGG_CUDA_CHECK(cudaGraphNodeGetType(node, &ty));
+    if (ty != cudaGraphNodeTypeKernel) continue;
+    ++kernels;
+    cudaLaunchAttributeValue v;
+    VGG_CUDA_CHECK(cudaGraphKernelNodeGetAttribute(node, cudaLaunchAttributePriority, &v));
+    for (int r = 0; r < 3; ++r) count[r] += v.priority == cs->prio[r];
+  }
+  const bool distinct = cs->prio[CR_PANEL] != cs->prio[CR_NEXT] && cs->prio[CR_NEXT] != cs->prio[CR_REST];
+  VGG_REQUIRE(kernels == cs->launched[CR_PANEL] + cs->launched[CR_NEXT] + cs->launched[CR_REST],
+              "cholesky graph: kernel nodes do not match the captured launches");
+  VGG_REQUIRE(!distinct || (count[CR_PANEL] == cs->launched[CR_PANEL] && count[CR_NEXT] == cs->launched[CR_NEXT] &&
+                            count[CR_REST] == cs->launched[CR_REST]),
+              "cholesky graph: a kernel node lost its priority");
   return VGG_OK;
 }
 
@@ -925,6 +1005,7 @@ int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, cons
   if (it == cache.end()) {
     const long long launches_before = g_launch_count;
     cudaGraph_t graph = nullptr;
+    cs->launched[CR_PANEL] = cs->launched[CR_NEXT] = cs->launched[CR_REST] = 0;
     VGG_CUDA_CHECK(cudaStreamBeginCapture(cs->cap, cudaStreamCaptureModeThreadLocal));
     rc = chol_enqueue(n, lda, A, Ldiag, info, flags, end_blk, arrow_blk, cs->cap, cs, true);
     const cudaError_t ce = cudaStreamEndCapture(cs->cap, &graph);
@@ -935,8 +1016,15 @@ int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, cons
     }
     VGG_CUDA_CHECK(ce);
     cudaGraphExec_t exec = nullptr;
-    VGG_CUDA_CHECK(cudaGraphInstantiate(&exec, graph, 0));
+    const cudaError_t ie = cudaGraphInstantiate(&exec, graph, cudaGraphInstantiateFlagUseNodePriority);
+    // the priorities are what keeps the panel chain ahead of the updates: read them back from the graph's nodes
+    if (ie == cudaSuccess) rc = chol_check_priorities(graph, cs);
     cudaGraphDestroy(graph);
+    VGG_CUDA_CHECK(ie);
+    if (rc) {
+      cudaGraphExecDestroy(exec);
+      return rc;
+    }
     if (cache.size() > 8) {
       for (auto& kv : cache) cudaGraphExecDestroy(kv.second);
       cache.clear();
