@@ -118,7 +118,8 @@ int vgg_ba_workspace_bytes(int S, int N, int camera_model, int intr_mode, size_t
  * Outputs (all double): cost[1]; camrec[S,KR] = per frame (g_c[dc] | H_cc upper-packed | H_cs[6,ns]);
  * g_p[N,3]; H_pp[N,6] (xx,xy,xz,yy,yz,zz); W[N, pitch, 3] track-major coupling blocks J_c^T J_p with
  * row = s*dc+i (shared-intrinsics rows at S*dc..) and pitch = D rounded up to even, D = S*dc+ns;
- * shared[8] = (g_s[2], H_ss xx,xy,yy).  KR = vgg_ba_camrec_len().  The last int argument is the number of
+ * shared[8] = (g_s[2], H_ss xx,xy,yy).  KR = vgg_ba_camrec_len().  W = NULL runs the variant of the LM solve,
+ * which computes everything else and stores no coupling block.  The last int argument is the number of
  * tracks each warp walks: 0 = choose, otherwise a positive multiple of 4 (the observation loads of a warp are
  * vectorised over 4 tracks); any other value returns VGG_EINVAL before anything is launched. */
 int vgg_ba_camrec_len(int camera_model, int intr_mode);

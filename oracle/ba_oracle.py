@@ -41,7 +41,9 @@ LM control (lm_solve), as the CUDA loop (csrc/ba_solve.cu) must follow it:
     termination, parameters unchanged).  Ceres gives a candidate that fails to evaluate the cost DBL_MAX, which
     rejects the step; here a non-finite candidate cost also makes rho non-finite and rejects it, but the CUDA loop
     counts it as an invalid step.  No input with a finite initial cost and float32 observations was found that makes
-    the candidate cost non-finite, so that branch has no test (tests/test_ba_lm_edges_gpu.py).
+    the candidate cost non-finite, so that branch has no test (tests/test_ba_lm_edges_gpu.py).  A point block whose
+    damped 3x3 Cholesky fails (a one-view point at radius >= 1e14) makes the CUDA step invalid, where Ceres inverts the
+    block explicitly (DESIGN.md section 4.2); lm_solve here raises numpy's LinAlgError on it.
 """
 from __future__ import annotations
 

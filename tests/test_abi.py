@@ -83,6 +83,15 @@ def test_build_blocks_rejects_unaligned_tracks_per_warp():
         rc = L.vgg_ba_build_blocks(ctypes.byref(p), *[o.ctypes.data for o in outs], tpw, None)
         assert rc == -1, tpw                                         # VGG_EINVAL
         assert b"tracks_per_warp" in L.vgg_last_error()
+    # W = NULL selects the LM solve's variant (no coupling blocks stored): it passes the pointer check and meets the
+    # same tracks_per_warp check; any other null output is still refused
+    no_w = [o.ctypes.data for o in outs]
+    no_w[4] = None
+    assert L.vgg_ba_build_blocks(ctypes.byref(p), *no_w, 6, None) == -1
+    assert b"tracks_per_warp" in L.vgg_last_error()
+    no_w[0] = None
+    assert L.vgg_ba_build_blocks(ctypes.byref(p), *no_w, 0, None) == -1
+    assert b"null pointer" in L.vgg_last_error()
     assert all(np.array_equal(a, b) for a, b in zip(outs, sentinel))
 
 

@@ -32,7 +32,8 @@ EXPORTS = [
 
 # development probes (csrc/dev_probes.h): exported, not part of the public header
 DEV_EXPORTS = ["vgg_dev_blocks_timing", "vgg_dev_blocks_last_ms", "vgg_dev_chol128_probe", "vgg_dev_syrk_f64", "vgg_dev_syrk_f64_band", "vgg_dev_syrk_ozaki_band", "vgg_dev_trsv_probe", "vgg_dev_cholesky_band",
-               "vgg_dev_last_band_hint", "vgg_dev_msac_trace", "vgg_dev_relative_pose_counts"]
+               "vgg_dev_last_band_hint", "vgg_dev_msac_trace", "vgg_dev_relative_pose_counts",
+               "vgg_dev_build_blocks_band", "vgg_dev_schur_build", "vgg_dev_syrk_work_list"]
 
 
 class BAProblem(ctypes.Structure):
@@ -152,6 +153,9 @@ def lib() -> ctypes.CDLL:
     L.vgg_dev_syrk_f64_band.argtypes = L.vgg_dev_syrk_f64.argtypes + [vp, ci]
     L.vgg_dev_trsv_probe.argtypes = [ci, ci, vp, vp, cs, vp, vp]
     L.vgg_dev_last_band_hint.argtypes = [vp, vp, vp, vp, vp]
+    L.vgg_dev_build_blocks_band.argtypes = L.vgg_ba_build_blocks.argtypes[:-1] + [vp, ci, vp]
+    L.vgg_dev_schur_build.argtypes = [ctypes.POINTER(BAProblem)] + [vp] * 5 + [cd] * 3 + [ci, ci, vp, cs] + [vp] * 8
+    L.vgg_dev_syrk_work_list.argtypes = [ci, ci, vp, ci, ci, vp, ci, ctypes.POINTER(ci)]
     L.vgg_syrk_ozaki.argtypes = [ci, ci, vp, vp, ci, vp, cs, vp]
     L.vgg_dev_syrk_ozaki_band.argtypes = L.vgg_syrk_ozaki.argtypes + [vp, ci]
     L.vgg_cholesky_lower.argtypes = [ci, ci, vp, vp, cs, ctypes.POINTER(ci), vp]

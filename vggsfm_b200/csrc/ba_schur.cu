@@ -706,13 +706,24 @@ struct SyrkF64State {
 };
 thread_local SyrkF64State g_sf;
 
+// the work list of launch_syrk for nworkers persistent CTAs (ranges: the band hint, empty = dense)
+static std::vector<SyrkWork> syrk_f64_work(int Kpad, int Dpad, const std::vector<int>& ranges, int nworkers) {
+  const int nb = Dpad / SF_BM, KB = (Kpad + 63) / 64;
+  // equal-length items, longest first: the CTAs of a wave advance through k together, so Zt is read from HBM about
+  // once and from L2 by the other tiles of its column block
+  std::vector<SyrkWork> work;
+  build_work_list<SyrkWork>({1}, syrk_tile_jobs(nb, ranges), KB, nworkers, KB, 1,
+                            [](const SyrkTileJob& j, int, int k0, int k1) { return SyrkWork{j.bi, j.bj, k0, k1}; }, &work);
+  return work;
+}
+
 // Cmat -= Zt^T Zt: Zt [Kpad][Dpad] (Dpad % 128 == 0, Kpad % 16 == 0), Cmat [Dpad][Dpad] row-major, LOWER triangle (or
 // the fabric destinations of fd / mc_off, see syrk_red_upper).  kb_ranges: [lo, hi) k-block range per 128-column row
 // block of Zt outside which the block is exactly zero (csrc/ba_solve.cu, compute_band_hint); any other size = dense.
 int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc_off, const std::vector<int>& kb_ranges,
                 const FabricDev& fd, cudaStream_t st) {
   VGG_REQUIRE(Dpad % SF_BM == 0 && Kpad % SF_BK == 0, "syrk: Dpad must be a multiple of 128 and Kpad of 16");
-  const int nb = Dpad / SF_BM, KB = (Kpad + 63) / 64;
+  const int nb = Dpad / SF_BM;
   SyrkF64State& hs = g_sf;
   const std::vector<int> ranges = (int)kb_ranges.size() == 2 * nb ? kb_ranges : std::vector<int>();
   int dev = 0;
@@ -720,11 +731,7 @@ int launch_syrk(int Kpad, int Dpad, const double* Zt, double* Cmat, ptrdiff_t mc
   if (hs.dev != dev || hs.Kpad != Kpad || hs.Dpad != Dpad || hs.ranges != ranges) {
     VGG_CUDA_CHECK(cudaDeviceGetAttribute(&hs.sms, cudaDevAttrMultiProcessorCount, dev));
     VGG_CUDA_CHECK(cudaFuncSetAttribute(syrk_f64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SF_SMEM_BYTES));
-    // equal-length items, longest first: the CTAs of a wave advance through k together, so Zt is read from HBM about
-    // once and from L2 by the other tiles of its column block
-    std::vector<SyrkWork> work;
-    build_work_list<SyrkWork>({1}, syrk_tile_jobs(nb, ranges), KB, hs.sms, KB, 1,
-                              [](const SyrkTileJob& j, int, int k0, int k1) { return SyrkWork{j.bi, j.bj, k0, k1}; }, &work);
+    const std::vector<SyrkWork> work = syrk_f64_work(Kpad, Dpad, ranges, hs.sms);
     // a kernel in flight (on any stream) may still read the previous list
     VGG_CUDA_CHECK(cudaDeviceSynchronize());
     if (hs.dev != dev || work.size() > hs.work_cap) {
@@ -813,6 +820,28 @@ int vgg_dev_syrk_f64_band(int Kpad, int Dpad, const double* Zt, double* Cmat, vo
   VGG_REQUIRE(Zt && Cmat && Kpad > 0 && Dpad > 0 && (ranges || count <= 0), "bad argument");
   return launch_syrk(Kpad, Dpad, Zt, Cmat, 0, std::vector<int>(ranges, ranges + std::max(count, 0)), FabricDev{},
                      static_cast<cudaStream_t>(stream));
+}
+
+/* development probe (csrc/dev_probes.h): the work list launch_syrk builds for nworkers CTAs, host only */
+int vgg_dev_syrk_work_list(int Kpad, int Dpad, const int* ranges, int count, int nworkers, int* items, int cap,
+                           int* nwork) {
+  using namespace vgg;
+  VGG_REQUIRE(Kpad > 0 && Kpad % SF_BK == 0 && Dpad > 0 && Dpad % SF_BM == 0 && nworkers > 0 && nwork &&
+                  (ranges || count <= 0),
+              "bad argument");
+  std::vector<int> r(ranges, ranges + std::max(count, 0));
+  if ((int)r.size() != 2 * (Dpad / SF_BM)) r.clear();
+  const std::vector<SyrkWork> work = syrk_f64_work(Kpad, Dpad, r, nworkers);
+  *nwork = (int)work.size();
+  if (!items) return VGG_OK;
+  VGG_REQUIRE((int)work.size() <= cap, "work list longer than cap");
+  for (size_t i = 0; i < work.size(); ++i) {
+    items[4 * i] = work[i].bi;
+    items[4 * i + 1] = work[i].bj;
+    items[4 * i + 2] = work[i].kb0;
+    items[4 * i + 3] = work[i].kb1;
+  }
+  return VGG_OK;
 }
 
 }  // extern "C"

@@ -281,8 +281,8 @@ struct BandPlan {
   std::vector<int> kb_ranges, end_blk, kb_rows, fg_tracks;
   BandDev dev{nullptr};
 };
-// the plan of the most recent solve on this thread (vgg_dev_last_band_hint): the tests compare it with
-// oracle/band_oracle.py
+// the plan of the most recent solve or vgg_dev_schur_build on this thread (vgg_dev_last_band_hint): the tests compare it
+// with oracle/band_oracle.py
 static thread_local BandPlan g_band_last;
 
 // first / last visible point of every frame (N / -1 when the frame sees nothing): the band structure of sequential
@@ -464,10 +464,12 @@ static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad
 
 // Schur complement of blk onto AR (Sraw, rhs, hdiag, gvec) at the given radius; p: the problem at the state blk was
 // evaluated at (z_build rebuilds the coupling blocks from it); fd: where the SYRK epilogue sends each row block in a
-// fabric solve, fab: that solve's fabric (null otherwise)
+// fabric solve, fab: that solve's fabric (null otherwise); syrk = false stops after z_build (vgg_dev_schur_build with
+// Zt filled with a NaN sentinel: the SYRK adds every non-zero product, so sentinels left in the padding columns
+// [D, Dpad) would send it past the reduced system's rows)
 static int schur_build(const Layout& L, const vgg_ba_problem& p, const BlockSet& b, const BandPlan& band,
                        const FabricDev& fd, double radius, double min_diag, double max_diag, cudaStream_t st,
-                       ptrdiff_t mc_off = 0, Fabric* fab = nullptr) {
+                       ptrdiff_t mc_off = 0, Fabric* fab = nullptr, bool syrk = true) {
   int rc;
   double* Sraw = L.AR;
   double* rhs = L.AR + (size_t)L.D * L.Dpad;
@@ -481,7 +483,7 @@ static int schur_build(const Layout& L, const vgg_ba_problem& p, const BlockSet&
   if (fab && (rc = fab->barrier(st))) return rc;
   if ((rc = launch_assemble_hc(L.S, L.dc, L.ns, L.KR, L.Dpad, b.camrec, b.shared, Sraw, rhs, hdiag, gvec, mc_off, st))) return rc;
   if ((rc = launch_z_build(&p, L.Dpad, L.M, L.q, L.Zt, rhs, mc_off, band.dev.fg_tracks, st))) return rc;
-  if ((rc = launch_syrk(L.Kpad, L.Dpad, L.Zt, Sraw, mc_off, band.kb_ranges, fd, st))) return rc;
+  if (syrk && (rc = launch_syrk(L.Kpad, L.Dpad, L.Zt, Sraw, mc_off, band.kb_ranges, fd, st))) return rc;
   // ... and all reductions must have landed before anyone reads its copy
   if (fab && (rc = fab->barrier(st))) return rc;
   return VGG_OK;
@@ -533,11 +535,34 @@ int vgg_ba_workspace_bytes(int S, int N, int camera_model, int intr_mode, size_t
 
 int vgg_ba_build_blocks(const vgg_ba_problem* prob, double* cost, double* camrec, double* g_p, double* H_pp, double* W,
                         double* shared_out, int tracks_per_warp, void* stream) {
-  VGG_REQUIRE(prob && cost && camrec && g_p && H_pp && W && shared_out, "null pointer");
+  return vgg_dev_build_blocks_band(prob, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, nullptr, 0, stream);
+}
+
+/* development probe (csrc/dev_probes.h): vgg_ba_build_blocks with the band table of the solve's block kernel */
+int vgg_dev_build_blocks_band(const vgg_ba_problem* prob, double* cost, double* camrec, double* g_p, double* H_pp,
+                              double* W, double* shared_out, int tracks_per_warp, const int* fg_tracks, int count,
+                              void* stream) {
+  VGG_REQUIRE(prob && cost && camrec && g_p && H_pp && shared_out, "null pointer");
   // a warp's first track t0 = chunk * tracks_per_warp + 4k is the 16-byte (uv) / 4-byte (mask) cp.async offset
   VGG_REQUIRE(tracks_per_warp >= 0 && tracks_per_warp % 4 == 0, "tracks_per_warp must be 0 (choose) or a multiple of 4");
+  VGG_REQUIRE(!fg_tracks || count == 2 * ((prob->S + 31) / 32), "fg_tracks needs 2 entries per group of 32 frames");
+  cudaStream_t st = (cudaStream_t)stream;
   g_launch_count = 0;
-  return ba_build_blocks(prob, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, nullptr, (cudaStream_t)stream);
+  static thread_local int* tdev = nullptr;
+  static thread_local int tcap = 0;
+  if (fg_tracks) {
+    // a launch of an earlier call, on any stream, may still read the table
+    VGG_CUDA_CHECK(cudaDeviceSynchronize());
+    if (tcap < count) {
+      if (tdev) cudaFree(tdev);
+      tdev = nullptr;
+      VGG_CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&tdev), sizeof(int) * (size_t)count));
+      tcap = count;
+    }
+    VGG_CUDA_CHECK(cudaMemcpyAsync(tdev, fg_tracks, sizeof(int) * (size_t)count, cudaMemcpyHostToDevice, st));
+    VGG_CUDA_CHECK(cudaStreamSynchronize(st));           // pageable source
+  }
+  return ba_build_blocks(prob, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks ? tdev : nullptr, st);
 }
 
 int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double* g_p, const double* H_pp,
@@ -564,6 +589,44 @@ int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double*
   VGG_CUDA_CHECK(cudaMemcpyAsync(Sraw, L.AR, sizeof(double) * (size_t)L.D * L.Dpad, cudaMemcpyDeviceToDevice, st));
   VGG_CUDA_CHECK(cudaMemcpyAsync(rhs, L.AR + (size_t)L.D * L.Dpad, sizeof(double) * L.Dpad, cudaMemcpyDeviceToDevice, st));
   if (Dpad_out) *Dpad_out = L.Dpad;
+  return VGG_OK;
+}
+
+/* development probe (csrc/dev_probes.h): schur_build as the LM loop runs it, with its intermediate buffers */
+int vgg_dev_schur_build(const vgg_ba_problem* prob, const double* camrec, const double* g_p, const double* H_pp,
+                        const double* shared_in, const double* scale_p, double radius, double min_diag, double max_diag,
+                        int banded, int zt_nan, void* workspace, size_t ws_bytes, double* M, double* q, double* dpp,
+                        double* scal, double* Zt, double* Sraw, double* rhs, void* stream) {
+  VGG_REQUIRE(prob && camrec && g_p && H_pp && shared_in && scale_p && workspace, "null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  g_launch_count = 0;
+  Layout L;
+  int rc = make_layout(prob->S, prob->N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L);
+  if (rc) return rc;
+  BandPlan band;
+  if (banded && (rc = compute_band_hint(prob, L.dc, L.D, L.Dpad, L.Kpad, false, st, &band))) return rc;
+  g_band_last = band;
+  BlockSet b;
+  b.cost = nullptr;
+  b.camrec = const_cast<double*>(camrec);
+  b.g_p = const_cast<double*>(g_p);
+  b.H_pp = const_cast<double*>(H_pp);
+  b.shared = const_cast<double*>(shared_in);
+  VGG_CUDA_CHECK(cudaMemcpyAsync(L.sc_p, scale_p, sizeof(double) * (size_t)L.N * 3, cudaMemcpyDeviceToDevice, st));
+  // all-ones bytes: a NaN, so that the entries z_build writes can be told from the ones it leaves
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.Zt, zt_nan ? 0xff : 0, sizeof(double) * (size_t)L.Kpad * L.Dpad, st));
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.scal, 0, sizeof(double) * 16, st));
+  if ((rc = schur_build(L, *prob, b, band, FabricDev{}, radius, min_diag, max_diag, st, 0, nullptr, !zt_nan))) return rc;
+  auto out = [&](double* dst, const double* src, size_t n) -> int {
+    if (dst) VGG_CUDA_CHECK(cudaMemcpyAsync(dst, src, sizeof(double) * n, cudaMemcpyDeviceToDevice, st));
+    return VGG_OK;
+  };
+  const size_t N = (size_t)L.N;
+  if ((rc = out(M, L.M, 9 * N)) || (rc = out(q, L.q, 3 * N)) || (rc = out(dpp, L.dpp, 3 * N)) ||
+      (rc = out(scal, L.scal, 16)) || (rc = out(Zt, L.Zt, (size_t)L.Kpad * L.Dpad)) ||
+      (rc = out(Sraw, L.AR, (size_t)L.D * L.Dpad)) || (rc = out(rhs, L.AR + (size_t)L.D * L.Dpad, L.Dpad)))
+    return rc;
+  VGG_CUDA_CHECK(cudaStreamSynchronize(st));
   return VGG_OK;
 }
 

@@ -31,8 +31,8 @@ int vgg_dev_syrk_ozaki_band(int Kpad, int Dpad, const double* Zt, double* Cmat, 
  * 64 rows: entry, diagonal block loaded, inverse ready, every x_j consumed, x_b published, right-hand side ready). */
 int vgg_dev_trsv_probe(int n, int lda, const double* A_dev, const double* y_dev, size_t y_stride, double* x_dev,
                        long long* stamps_host);
-/* Band hint of the most recent vgg_ba_solve on the calling thread (csrc/ba_solve.cu, compute_band_hint).
- * meta_host[0..7] = {SYRK k-range hint active, factorisation band set, device tables for
+/* Band hint of the most recent vgg_ba_solve (or vgg_dev_schur_build) on the calling thread (csrc/ba_solve.cu,
+ * compute_band_hint).  meta_host[0..7] = {SYRK k-range hint active, factorisation band set, device tables for
  * ba_blocks / z_build / backsub made, nb (128-column row blocks), KB (64-row k blocks), frame groups of 32, arrow_blk, 0}.
  * Each non-null array receives its table if it was made: rb_range[2 nb], end_blk[nb], kb_rows[2 KB],
  * fg_tracks[2 groups]. */
@@ -51,6 +51,34 @@ int vgg_dev_msac_trace(int B, int N, int max_iterations, int min_iterations, con
 int vgg_dev_relative_pose_counts(int B, int N, const void* points1, const void* points2, int points_are_f64,
                                  const double* fmat, double width, double height, double* R_out, double* t_out,
                                  double* E_out, int32_t* counts_dev, void* stream);
+
+/* vgg_ba_build_blocks with the band table of the LM solve's block kernel: fg_tracks_host[2g], [2g+1] = the track range
+ * [lo, hi) outside which frame group g (32 frames) sees nothing (count = 2 * ceil(S/32); NULL, 0 = dense).  With a
+ * table and tracks_per_warp = 0 the kernel runs the banded sizing of the solve (64 tracks per warp; the warps whose
+ * track chunk misses their group's range return at once).  W = NULL runs the solve's variant, which stores no W.
+ * The table goes to a device buffer that the next call with a table rewrites after a device synchronise. */
+int vgg_dev_build_blocks_band(const vgg_ba_problem* prob, double* cost, double* camrec, double* g_p, double* H_pp,
+                              double* W, double* shared, int tracks_per_warp, const int* fg_tracks_host, int count,
+                              void* stream);
+/* One schur_build of the LM loop (csrc/ba_solve.cu) at the given state, Jacobi point scales (device [N,3]) and radius:
+ * point_prep, assemble_hc, z_build, syrk_f64 with the launchers of the solve.  banded = 0: dense plan; otherwise the
+ * plan compute_band_hint makes from prob->mask (then also reported by vgg_dev_last_band_hint).  zt_nan = 1 fills Zt
+ * with all-ones bytes (a NaN) instead of zeros before z_build, so the entries it writes can be told from the ones it
+ * leaves; the SYRK is then not run (it adds every non-zero product, so a sentinel left in the padding columns would
+ * reach rows beyond the reduced system) and Sraw holds assemble_hc's camera blocks only.  Each non-null device output
+ * receives a copy: M [N,9] (row-major upper triangular), q [N,3], dpp [N,3], scal [16] (scal[6] = points whose 3x3
+ * factorisation failed), Zt [Kpad,Dpad], Sraw [D,Dpad] (lower triangle valid), rhs [Dpad]; Kpad = 3N rounded up to 16, Dpad as in
+ * vgg_ba_schur.  workspace as vgg_ba_workspace_bytes.  Waits for the device. */
+int vgg_dev_schur_build(const vgg_ba_problem* prob, const double* camrec, const double* g_p, const double* H_pp,
+                        const double* shared, const double* scale_p, double radius, double min_diag, double max_diag,
+                        int banded, int zt_nan, void* workspace, size_t ws_bytes, double* M, double* q, double* dpp,
+                        double* scal, double* Zt, double* Sraw, double* rhs, void* stream);
+/* The work list of the Schur SYRK (csrc/ba_schur.cu launch_syrk, csrc/syrk_work.h) for nworkers persistent CTAs, on
+ * the host, no launch: items_host[4w..4w+3] = (bi, bj, kb0, kb1) of item w (upper tile bi <= bj, k blocks [kb0, kb1)
+ * of 64 rows), in the order CTAs take them (item w goes to CTA w mod nworkers).  ranges_host / count: the band hint of
+ * vgg_dev_syrk_f64_band.  *nwork = the length; items_host = NULL only queries it, otherwise cap must cover it. */
+int vgg_dev_syrk_work_list(int Kpad, int Dpad, const int* ranges_host, int count, int nworkers, int* items_host,
+                           int cap, int* nwork);
 
 #ifdef __cplusplus
 }
