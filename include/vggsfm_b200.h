@@ -87,7 +87,10 @@ typedef struct vgg_ba_summary {
 #define VGG_BA_FAILURE 5
 
 /* Sum/max all-reduce hook over track shards (one process per GPU).  `buf` is a device pointer
- * inside the caller's workspace; op 0 = sum, 1 = max, on `stream`.  NULL = single GPU. */
+ * inside the caller's workspace; op 0 = sum, 1 = max, on `stream`.  NULL = single GPU.
+ * Every rank makes the same sequence of calls and takes the same decisions.  The solve needs N > 0: a rank whose
+ * shard holds no track passes N = 16 padding tracks with an all-zero mask (any finite uv and points, e.g. (0, 0, 1))
+ * instead, which add nothing to any reduction (vggsfm_b200/bundle_adjustment.py lm_solve does this). */
 typedef int (*vgg_allreduce_fn)(void* user, double* buf, size_t count, int op, void* stream);
 
 /* Fused reduction over NVLink/NVSwitch: the reduced camera system [D x Dpad | rhs | diag | g] lives in symmetric

@@ -360,6 +360,14 @@ def _x_norm(poses, intr, points, S, dc, ns, param_const, point_const):
     image whose block is not constant (a block held partly constant through a SubsetManifold, e.g. the second image's
     translation or a camera with a fixed principal point, is still non-constant), camera parameter blocks (f,cx,cy[,k])
     unless no intrinsic is refined, free points. [3P-memory]"""
+    cams, pts = _x_norm_parts(poses, intr, points, S, dc, ns, param_const, point_const)
+    return np.sqrt(cams + pts)
+
+
+def _x_norm_parts(poses, intr, points, S, dc, ns, param_const, point_const):
+    """(camera part, point part) of |x|^2.  With track shards the camera part is the same on every rank and the point
+    part covers this rank's points only: it has to be summed over the ranks before |x| is formed, or each rank tests
+    the parameter tolerance against its own |x| and the ranks may stop at different iterations."""
     pc = np.asarray(param_const, dtype=bool)
     ni = dc - 6 if ns == 0 else ns
     nparam = 3 + (1 if ni == 2 else 0) if ni else 0
@@ -375,8 +383,7 @@ def _x_norm(poses, intr, points, S, dc, ns, param_const, point_const):
     if ns and not pc[S * dc:].all():
         tot += float(np.sum(intr[0][:3] ** 2)) + (float(intr[0][3] ** 2) if ns == 2 else 0.0)
     free = ~np.asarray(point_const, dtype=bool)
-    tot += float(np.sum(points[free] ** 2))
-    return np.sqrt(tot)
+    return tot, float(np.sum(points[free] ** 2))
 
 
 def lm_solve(poses, intr, points, uv, mask, model, mode, param_const=None, point_const=None,
@@ -499,8 +506,10 @@ def lm_solve(poses, intr, points, uv, mask, model, mode, param_const=None, point
         d_p = np.einsum("nij,nj->ni", M, np.einsum("nji,nj->ni", M, ypt))
         # ---- model cost change: 0.5*(delta^T D^2 delta - delta^T g)  (== -(J d)^T (f + J d/2))
         dps = d_p / np.where(sc_p == 0, 1.0, sc_p)
+        # the point part of |x|^2 rides in the same reduction (a rank-local |x| would split the ranks' decisions)
+        x_cams, x_pts = _x_norm_parts(poses, intr, points, S, dc, ns, param_const, point_const)
         pt_terms = np.array([np.sum(np.where(point_const[:, None], 0.0, dps * dps * dpp / radius)) - np.sum(d_p * blk["g_p"]),
-                             np.sum(d_p * d_p)])
+                             np.sum(d_p * d_p), x_pts])
         pt_terms = ar(pt_terms)
         quad = np.sum(dcs * dcs * dcc / radius * free_c) - np.sum(d_c * gc_glob) + pt_terms[0]
         model_change = 0.5 * quad
@@ -523,7 +532,7 @@ def lm_solve(poses, intr, points, uv, mask, model, mode, param_const=None, point
         step_norm = float(np.sqrt(np.sum(d_c * d_c) + pt_terms[1]))
         cost_change = cost - c_cost
         rho = cost_change / model_change
-        x_norm = _x_norm(poses, intr, points, S, dc, ns, param_const, point_const)
+        x_norm = np.sqrt(x_cams + pt_terms[2])
         rec = {"it": it, "cost": cost, "candidate_cost": c_cost, "model_change": model_change, "rho": rho,
                "radius": radius, "step_norm": step_norm, "cost_change": cost_change, "x_norm": x_norm, "outcome": 0}
         if trace is not None:

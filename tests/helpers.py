@@ -40,6 +40,14 @@ def banded_ba_case(S, N, camera_type, mode, life, seed=0, mask_seed=0):
     return c
 
 
+def far_points_first_case():
+    """ba_case(8, 128, SIMPLE_PINHOLE, INTR_CONST, seed=2) with the tracks sorted by descending |X|: over 2 track shards
+    the first holds the far points, and each shard's own points give an |x| well below the true one"""
+    c = ba_case(8, 128, "SIMPLE_PINHOLE", bo.INTR_CONST, seed=2)
+    order = np.argsort(-np.linalg.norm(c["points"], axis=1), kind="stable")
+    return dict(c, points=c["points"][order].copy(), uv=c["uv"][:, order].copy(), mask=c["mask"][:, order].copy())
+
+
 def hidden_case(S, N, cam, mode, seed, point_value, uv_value, n_hidden=3, hidden_frame=None, case=None):
     """(problem with hidden values, its clean twin, hidden point indices).  The hidden points' columns are masked out
     entirely; a third of the other masked slots get uv_value; hidden_frame (if given) loses every observation and gets a

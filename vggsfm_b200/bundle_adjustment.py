@@ -197,12 +197,22 @@ class Summary:
 def lm_solve(uv, mask, poses, intr, points, model, mode, param_const=None, point_const=None,
              options: Optional[BAOptions] = None, allreduce=None, want_trace=False) -> Summary:
     """In-place Levenberg-Marquardt on device tensors (vgg_ba_solve).  `allreduce` is a
-    vggsfm_b200.dist.AllReduceHook for track-sharded multi-GPU runs."""
+    vggsfm_b200.dist.AllReduceHook for track-sharded multi-GPU runs.  A rank whose shard holds no track (N = 0:
+    shard_range gives empty tail shards when the tracks are few) still takes part in every reduction: it solves 16
+    masked-out padding tracks, as bundle_adjustment() pads, and leaves its empty `points` untouched."""
     L = _lib.lib()
     S, N = mask.shape
     dev = uv.device
     if param_const is None:
         param_const = default_param_const(S, model, mode, dev)
+    if N == 0:
+        n = pad_tracks(1)
+        uv = torch.zeros(S, n, 2, dtype=torch.float32, device=dev)
+        mask = torch.zeros(S, n, dtype=torch.uint8, device=dev)
+        points = torch.zeros(n, 3, dtype=torch.float64, device=dev)
+        points[:, 2] = 1.0
+        point_const = torch.ones(n, dtype=torch.uint8, device=dev)
+        N = n
     opt = options or default_options()
     ws = workspace(S, N, model, mode, dev)
     p = _problem(uv, mask, poses, intr, points, model, mode, param_const, point_const)

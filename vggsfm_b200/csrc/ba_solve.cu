@@ -65,24 +65,28 @@ int launch_fabric_allreduce(const FabricDev& fd, size_t flags_off, size_t mail_o
                             unsigned long long epoch, double* vec, int count, int max_slot, int* err, cudaStream_t st);
 
 // gathers the accept/reject scalars into one 24-double record so the host reads them with ONE copy:
-// [0..7] = scal[0..7], [8..15] = small[0..7], [16] = factorisation info, [17] = substitution info, [18] = |x|^2
+// [0..7] = scal[0..7], [8..15] = small[0..7], [16] = factorisation info, [17] = substitution info, [18] = camera part of |x|^2
+// (its point part is small[5], summed over the ranks)
 __global__ void pack_scalars_kernel(const double* __restrict__ scal, const double* __restrict__ small,
                                     const int* __restrict__ info, double* __restrict__ out) {
   const int i = threadIdx.x;
   if (i < 8) out[i] = scal[i];
   else if (i < 16) out[i] = small[i - 8];
   else if (i < 18) out[i] = (double)info[i - 16];
-  else if (i == 18) out[i] = scal[8];              // |x|^2 (xnorm_kernel), 0 unless parameter_tolerance > 0
+  else if (i == 18) out[i] = scal[8];              // camera part of |x|^2 (xnorm_kernel), 0 unless parameter_tolerance > 0
   else if (i == 19) out[i] = (double)info[2];      // a cross-rank barrier of csrc/fabric.cu timed out
 }
 
 // |x|^2 of Ceres' reduced program in ambient coordinates (ParameterToleranceReached: step_norm <= tol * (|x| + tol)):
 // unit quaternion + translation of every image whose block is not constant, non-constant camera blocks (f,cx,cy[,k]),
-// free points.  Only launched when parameter_tolerance > 0 (COLMAP's BA default is 0).  One CTA; out[0] = |x|^2.
+// free points.  Only launched when parameter_tolerance > 0 (COLMAP's BA default is 0).  One CTA; the camera part goes to
+// cam_out[0], the point part to pts_out[0]: with track shards the cameras are the same on every rank but the points are
+// this rank's, so the point part has to be summed over the ranks before |x| is formed.
 __global__ void xnorm_kernel(int S, int N, int dc, int ns, int model, const uint8_t* __restrict__ pconst,
                              const uint8_t* __restrict__ point_const, const double* __restrict__ poses,
-                             const double* __restrict__ intr, const double* __restrict__ pts, double* __restrict__ out) {
-  double acc = 0.0;
+                             const double* __restrict__ intr, const double* __restrict__ pts,
+                             double* __restrict__ cam_out, double* __restrict__ pts_out) {
+  double acc = 0.0, acc_p = 0.0;
   const int np = model == VGG_SIMPLE_RADIAL ? 4 : 3;
   for (int s = threadIdx.x; s < S; s += blockDim.x) {
     const uint8_t* c = pconst + (size_t)s * dc;
@@ -106,17 +110,24 @@ __global__ void xnorm_kernel(int S, int N, int dc, int ns, int model, const uint
   }
   for (int n = threadIdx.x; n < N; n += blockDim.x) {
     if (point_const && point_const[n]) continue;
-    acc += pts[3 * (size_t)n] * pts[3 * (size_t)n] + pts[3 * (size_t)n + 1] * pts[3 * (size_t)n + 1] +
-           pts[3 * (size_t)n + 2] * pts[3 * (size_t)n + 2];
+    acc_p += pts[3 * (size_t)n] * pts[3 * (size_t)n] + pts[3 * (size_t)n + 1] * pts[3 * (size_t)n + 1] +
+             pts[3 * (size_t)n + 2] * pts[3 * (size_t)n + 2];
   }
-  __shared__ double red[32];
+  __shared__ double red[2][32];
   acc = warp_sum(acc);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+  acc_p = warp_sum(acc_p);
+  if ((threadIdx.x & 31) == 0) {
+    red[0][threadIdx.x >> 5] = acc;
+    red[1][threadIdx.x >> 5] = acc_p;
+  }
   __syncthreads();
   if (threadIdx.x < 32) {
-    double v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.0;
-    v = warp_sum(v);
-    if (threadIdx.x == 0) out[0] = v;
+    const bool in = threadIdx.x < (blockDim.x >> 5);
+    const double v = warp_sum(in ? red[0][threadIdx.x] : 0.0), vp = warp_sum(in ? red[1][threadIdx.x] : 0.0);
+    if (threadIdx.x == 0) {
+      cam_out[0] = v;
+      pts_out[0] = vp;
+    }
   }
 }
 
@@ -916,6 +927,14 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + 1, L.scal + 2, sizeof(double) * 2, cudaMemcpyDeviceToDevice, st));
     VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + 3, L.scal + 6, sizeof(double), cudaMemcpyDeviceToDevice, st));
     if ((rc = launch_extract_gvec(S, dc, ns, L.KR, L.blk[cand].camrec, L.blk[cand].shared, L.small + 8, st))) return rc;
+    if (opt.parameter_tolerance > 0.0) {
+      // |x|^2 of the current state: the camera part (replicated) stays in scal[8], the point part (this rank's points)
+      // joins the small all-reduce in slot 5, which both paths sum; |x| is formed from the two after the reduction, so
+      // every rank tests the parameter tolerance against the same |x|
+      xnorm_kernel<<<1, 1024, 0, st>>>(S, N, dc, ns, prob->camera_model, prob->param_const, prob->point_const,
+                                        L.poses[cur], L.intr[cur], L.points[cur], L.scal + 8, L.small + 5);
+      VGG_LAUNCH_CHECK();
+    }
     if (fab.on) {
       // one in-kernel all-reduce for everything: the point-gradient max rides in slot 4 (max), the rest is summed
       if ((rc = launch_gradmax(D, N, L.small + 8, prob->param_const, L.blk[cand].g_p, prob->point_const, L.scal, st))) return rc;
@@ -928,13 +947,6 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
       if (allreduce && (rc = allreduce(ar_user, L.small, 8 + (size_t)L.Dpad, 0, st))) return rc;
       if ((rc = launch_gradmax(D, N, L.small + 8, prob->param_const, L.blk[cand].g_p, prob->point_const, L.scal, st))) return rc;
       if (allreduce && (rc = allreduce(ar_user, L.scal + 5, 1, 1, st))) return rc;
-    }
-    if (opt.parameter_tolerance > 0.0) {
-      // |x| of THIS rank's points + the replicated cameras; with track shards the point part is a partial sum, which
-      // only makes the test stricter by under-estimating |x| (parameter_tolerance is 0 in every COLMAP preset)
-      xnorm_kernel<<<1, 1024, 0, st>>>(S, N, dc, ns, prob->camera_model, prob->param_const, prob->point_const,
-                                        L.poses[cur], L.intr[cur], L.points[cur], L.scal + 8);
-      VGG_LAUNCH_CHECK();
     }
     if ((rc = read_scalars())) return rc;
     const int h_info[2] = {(int)h_scal[16], (int)h_scal[17]};
@@ -968,8 +980,9 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     const double rho = cost_change / model_change;
     if (tr) tr[4] = rho;
     // Ceres ParameterToleranceReached(): step_norm <= tol * (|x| + tol), |x| over the non-constant blocks in ambient
-    // coordinates (h_scal[18], xnorm_kernel; only evaluated when the tolerance is non-zero -- COLMAP's default is 0)
-    const double x_norm = opt.parameter_tolerance > 0.0 ? sqrt(h_scal[18]) : 0.0;
+    // coordinates (xnorm_kernel: cameras h_scal[18] + points summed over the ranks h_scal[13] = small[5]; only evaluated
+    // when the tolerance is non-zero -- COLMAP's default is 0)
+    const double x_norm = opt.parameter_tolerance > 0.0 ? sqrt(h_scal[18] + h_scal[13]) : 0.0;
     if (step_norm <= opt.parameter_tolerance * (x_norm + opt.parameter_tolerance)) {
       summary->termination = VGG_BA_CONVERGENCE_PARAMETER;
       break;
