@@ -160,6 +160,42 @@ int vgg_syrk_ozaki(int Kpad, int Dpad, const double* Zt, double* Cmat, int slice
 int vgg_ba_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt, void* workspace,
                  size_t ws_bytes, vgg_allreduce_fn allreduce, void* allreduce_user,
                  vgg_ba_summary* summary, double* trace, void* stream);
+
+/* Linear solver of the LM loop.  vgg_ba_solve always runs DENSE_SCHUR (the reduced camera system is formed and factored);
+ * vgg_ba_solve_iterative runs ITERATIVE_SCHUR: preconditioned conjugate gradients on the reduced system without forming
+ * it (SCHUR_JACOBI preconditioner: one block per rotation, translation and camera-intrinsics parameter block), Ceres'
+ * ConjugateGradientsSolver as LevenbergMarquardtStrategy calls it (x0 = 0, stop when i (Q_i - Q_{i-1}) / Q_i < eta and
+ * i >= min, residual reset every 10 iterations; the first iteration always runs, so max 0 behaves as 1).  Its memory is
+ * O(S N) for the caller's observation grid plus O(S + N) workspace: no [D x D] matrix. */
+#define VGG_BA_DENSE_SCHUR 0
+#define VGG_BA_ITERATIVE_SCHUR 1
+typedef struct vgg_ba_linear_solver {
+  int32_t type;                          /* VGG_BA_*_SCHUR */
+  int32_t min_linear_solver_iterations;  /* >= 0 */
+  int32_t max_linear_solver_iterations;  /* >= min */
+  double eta;                            /* > 0: the q-tolerance of the truncated Newton step */
+} vgg_ba_linear_solver;
+
+/* CG termination (cg_trace column 1): SUCCESS (zeta < eta, or |b| = 0), NO_CONVERGENCE (max iterations: the step is
+ * used), FAILURE (zero or infinite rho, beta or alpha, p'q <= 0, or a preconditioner block that is not positive definite:
+ * the LM step is invalid). */
+#define VGG_CG_SUCCESS 0
+#define VGG_CG_NO_CONVERGENCE 1
+#define VGG_CG_FAILURE 2
+
+/* Ceres' defaults: DENSE_SCHUR, 0, 500, 0.1. */
+void vgg_ba_default_linear_solver(vgg_ba_linear_solver* lin);
+/* Workspace of vgg_ba_solve_iterative: no Schur operand, no reduced system, no factorisation workspace. */
+int vgg_ba_workspace_bytes_iterative(int S, int N, int camera_model, int intr_mode, size_t* bytes);
+/* vgg_ba_solve with lin->type = VGG_BA_ITERATIVE_SCHUR, on one GPU (no all-reduce hook, no fabric).  `trace` as for
+ * vgg_ba_solve; `cg_trace` is a HOST array [max_num_iterations, 4] or NULL: per LM iteration the CG iterations, the CG
+ * termination (VGG_CG_*), the last zeta and |r| / |b|.  The model change of the inexact step is
+ * -(J d)^T (f + J d / 2), evaluated per observation.  Returns VGG_EINVAL before any launch for another lin->type,
+ * min < 0, max < min or eta not positive and finite. */
+int vgg_ba_solve_iterative(const vgg_ba_problem* prob, const vgg_ba_options* opt, const vgg_ba_linear_solver* lin,
+                           void* workspace, size_t ws_bytes, vgg_ba_summary* summary, double* trace, double* cg_trace,
+                           void* stream);
+
 int vgg_ba_reduced_system_doubles(int S, int camera_model, int intr_mode, size_t* doubles);
 int vgg_ba_fabric_doubles(int S, int camera_model, int intr_mode, size_t* doubles);
 int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt, void* workspace,

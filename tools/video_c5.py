@@ -167,6 +167,38 @@ def run(frames=1000, new_per_window=512, joint_every=6, seed=0, dev=None, verbos
             "trajectory_length": float(np.linalg.norm(Cg[-1] - Cg[0])), "store_points": store.num_points}
 
 
+def final_problem_arrays(frames=1000, new_per_window=512, seed=0, dev=None):
+    """The last joint BA of the sequence as device tensors (tracks [S,P,2] float32, masks [S,P] bool, points [P,3],
+    extrinsics [S,3,4], K [1,3,3]), ground truth + noise, points seen in >= 3 frames.  The [S,P] grid is filled on the
+    device window by window, so the host never holds it (a 2500-frame sequence at 2048 new points per window is 6 GB)."""
+    dev = dev or torch.device("cuda:0")
+    sc = make_video_scene(F=frames, new_per_window=new_per_window, seed=seed)
+    rng = np.random.default_rng(seed + 2)
+    P = sc.points3d.shape[0]
+    uv = torch.zeros(frames, P, 2, dtype=torch.float32, device=dev)
+    ok = torch.zeros(frames, P, dtype=torch.bool, device=dev)
+    for w in range(sc.num_windows()):
+        ids = np.nonzero(sc.birth == w)[0]
+        f0, f1 = int(sc.first_frame[ids[0]]), int(sc.last_frame[ids[0]])
+        u, o = sc.observe(ids, f0, f1)
+        it = torch.from_numpy(ids).to(dev)
+        uv[f0:f1, it] = torch.from_numpy(np.ascontiguousarray(u, dtype=np.float32)).to(dev)
+        ok[f0:f1, it] = torch.from_numpy(np.ascontiguousarray(o)).to(dev)
+    keep = (ok.sum(0) >= 3).cpu().numpy()
+    w = rng.normal(size=(frames, 3))
+    w = w / np.linalg.norm(w, axis=1, keepdims=True) * np.deg2rad(0.2)
+    extr = sc.extrinsics.copy()
+    extr[:, :, :3] = _exp_so3(w) @ extr[:, :, :3]
+    extr[:, :, 3] += rng.normal(size=(frames, 3)) * 0.005
+    pts = sc.points3d[keep] + rng.normal(size=(int(keep.sum()), 3)) * 0.01
+    K = torch.tensor([[[sc.focal, 0.0, sc.pp[0]], [0.0, sc.focal, sc.pp[1]], [0.0, 0.0, 1.0]]], dtype=torch.float64, device=dev)
+    kt = torch.from_numpy(keep).to(dev)
+    tracks, masks = uv[:, kt].contiguous(), ok[:, kt].contiguous()
+    del uv, ok
+    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    return tracks, masks, T(pts), T(extr), K
+
+
 def final_problem(frames=1000, new_per_window=512, seed=0, dev=None, reps=1, shuffle=False):
     """Only the LAST joint BA of the sequence, built directly from the synthetic scene (ground truth + noise instead of
     the sequential estimates): the problem the launch lists and the multi-GPU leg look at."""

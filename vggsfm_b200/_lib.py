@@ -17,6 +17,7 @@ EXPORTS = [
     "vgg_ba_default_options", "vgg_ba_dims", "vgg_ba_workspace_bytes", "vgg_ba_camrec_len",
     "vgg_ba_build_blocks", "vgg_ba_schur", "vgg_cholesky_lower", "vgg_ba_solve",
     "vgg_ba_reduced_system_doubles", "vgg_ba_fabric_doubles", "vgg_ba_solve_fabric",
+    "vgg_ba_default_linear_solver", "vgg_ba_workspace_bytes_iterative", "vgg_ba_solve_iterative",
     "vgg_pose_default_options", "vgg_pose_refinement", "vgg_pnp_workspace_bytes", "vgg_absolute_pose_estimation", "vgg_syrk_ozaki_workspace_bytes", "vgg_syrk_ozaki",
     "vgg_tri_workspace_bytes", "vgg_triangulate_tracks", "vgg_triangulate_by_pair", "vgg_filter_points3d",
     "vgg_project_points", "vgg_normalize_tracks", "vgg_undistort_simple_radial",
@@ -33,7 +34,7 @@ EXPORTS = [
 # development probes (csrc/dev_probes.h): exported, not part of the public header
 DEV_EXPORTS = ["vgg_dev_blocks_timing", "vgg_dev_blocks_last_ms", "vgg_dev_chol128_probe", "vgg_dev_syrk_f64", "vgg_dev_syrk_f64_band", "vgg_dev_syrk_ozaki_band", "vgg_dev_trsv_probe", "vgg_dev_cholesky_band",
                "vgg_dev_last_band_hint", "vgg_dev_msac_trace", "vgg_dev_relative_pose_counts",
-               "vgg_dev_build_blocks_band", "vgg_dev_schur_build", "vgg_dev_syrk_work_list"]
+               "vgg_dev_build_blocks_band", "vgg_dev_schur_build", "vgg_dev_syrk_work_list", "vgg_dev_pcg_probe"]
 
 
 class BAProblem(ctypes.Structure):
@@ -61,6 +62,13 @@ class BAOptions(ctypes.Structure):
         ("min_relative_decrease", ctypes.c_double),
         ("min_lm_diagonal", ctypes.c_double),
         ("max_lm_diagonal", ctypes.c_double),
+    ]
+
+
+class BALinearSolver(ctypes.Structure):
+    _fields_ = [
+        ("type", ctypes.c_int32), ("min_linear_solver_iterations", ctypes.c_int32),
+        ("max_linear_solver_iterations", ctypes.c_int32), ("eta", ctypes.c_double),
     ]
 
 
@@ -140,6 +148,12 @@ def lib() -> ctypes.CDLL:
     L.vgg_ba_fabric_doubles.argtypes = [ci, ci, ci, ctypes.POINTER(cs)]
     L.vgg_ba_solve_fabric.argtypes = [ctypes.POINTER(BAProblem), ctypes.POINTER(BAOptions), vp, cs, ALLREDUCE_FN, vp,
                                       ctypes.POINTER(BAFabric), ctypes.POINTER(BASummary), vp, vp]
+    L.vgg_ba_default_linear_solver.argtypes = [ctypes.POINTER(BALinearSolver)]
+    L.vgg_ba_default_linear_solver.restype = None
+    L.vgg_ba_workspace_bytes_iterative.argtypes = [ci, ci, ci, ci, ctypes.POINTER(cs)]
+    L.vgg_ba_solve_iterative.argtypes = [ctypes.POINTER(BAProblem), ctypes.POINTER(BAOptions),
+                                         ctypes.POINTER(BALinearSolver), vp, cs, ctypes.POINTER(BASummary), vp, vp, vp]
+    L.vgg_dev_pcg_probe.argtypes = [ctypes.POINTER(BAProblem)] + [vp] * 6 + [cd] * 3 + [vp, vp, cs] + [vp] * 5
     L.vgg_pose_default_options.argtypes = [ctypes.POINTER(PoseOptions)]
     L.vgg_pose_default_options.restype = None
     L.vgg_pose_refinement.argtypes = [ci, ci, ci, vp, vp, vp, vp, vp, vp, ctypes.POINTER(PoseOptions), vp, vp, vp, vp]

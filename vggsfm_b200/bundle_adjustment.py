@@ -17,13 +17,16 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import BAOptions, BAProblem, BASummary
+from ._lib import BALinearSolver, BAOptions, BAProblem, BASummary
 
 SIMPLE_PINHOLE = 0
 SIMPLE_RADIAL = 1
 INTR_CONST = 0
 INTR_PER_FRAME = 1
 INTR_SHARED = 2
+
+LINEAR_SOLVER_TYPES = {"DENSE_SCHUR": 0, "ITERATIVE_SCHUR": 1}
+CG_TERMINATION = {0: "SUCCESS", 1: "NO_CONVERGENCE", 2: "FAILURE"}
 
 TERMINATION = {0: "NO_CONVERGENCE", 1: "CONVERGENCE_GRADIENT", 2: "CONVERGENCE_FUNCTION",
                3: "CONVERGENCE_PARAMETER", 4: "MIN_TRUST_REGION_RADIUS", 5: "FAILURE_INVALID_STEPS"}
@@ -84,17 +87,38 @@ def default_param_const(S: int, model: int, mode: int, device, refine_focal_leng
     return c.to(device)
 
 
+def linear_solver(linear_solver_type="DENSE_SCHUR", min_linear_solver_iterations=0, max_linear_solver_iterations=500,
+                  eta=0.1) -> BALinearSolver:
+    """Ceres' linear-solver options of the LM loop (defaults: Ceres' own).  ITERATIVE_SCHUR runs preconditioned CG on the
+    reduced camera system without forming it (SCHUR_JACOBI), for problems whose dense reduced system does not fit."""
+    if linear_solver_type not in LINEAR_SOLVER_TYPES:
+        raise ValueError(f"linear_solver_type must be one of {sorted(LINEAR_SOLVER_TYPES)}, not {linear_solver_type!r}")
+    lin = BALinearSolver()
+    _lib.lib().vgg_ba_default_linear_solver(ctypes.byref(lin))
+    lin.type = LINEAR_SOLVER_TYPES[linear_solver_type]
+    lin.min_linear_solver_iterations = int(min_linear_solver_iterations)
+    lin.max_linear_solver_iterations = int(max_linear_solver_iterations)
+    lin.eta = float(eta)
+    return lin
+
+
+def workspace_bytes(S: int, N: int, model: int, mode: int, iterative: bool = False) -> int:
+    """Bytes of the solve's workspace: vgg_ba_workspace_bytes (direct) or vgg_ba_workspace_bytes_iterative."""
+    nbytes = ctypes.c_size_t()
+    fn = _lib.lib().vgg_ba_workspace_bytes_iterative if iterative else _lib.lib().vgg_ba_workspace_bytes
+    _lib.check(fn(S, N, model, mode, ctypes.byref(nbytes)), fn.__name__)
+    return nbytes.value
+
+
 _ws_cache: dict = {}
 
 
-def workspace(S: int, N: int, model: int, mode: int, device) -> torch.Tensor:
-    key = (S, N, model, mode, str(device))
+def workspace(S: int, N: int, model: int, mode: int, device, iterative: bool = False) -> torch.Tensor:
+    key = (S, N, model, mode, str(device), iterative)
     ws = _ws_cache.get(key)
     if ws is None:
-        nbytes = ctypes.c_size_t()
         with torch.cuda.device(device):
-            _lib.check(_lib.lib().vgg_ba_workspace_bytes(S, N, model, mode, ctypes.byref(nbytes)),
-                       "vgg_ba_workspace_bytes")
+            nbytes = ctypes.c_size_t(workspace_bytes(S, N, model, mode, iterative))
         if len(_ws_cache) > 4:
             _ws_cache.clear()
         ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)
@@ -190,16 +214,26 @@ class Summary:
     device_ms: float
     kernel_launches: int
     trace: Optional[torch.Tensor] = None
+    linear_solver: str = "DENSE_SCHUR"
+    cg_iterations: int = 0                    # CG iterations over all LM iterations (ITERATIVE_SCHUR)
+    cg_trace: Optional[torch.Tensor] = None   # [iterations, 4]: CG iterations, termination (CG_TERMINATION), zeta, |r|/|b|
     alive: Optional[torch.Tensor] = None      # [P'] points the negative-depth filter kept (bundle_adjustment only)
     mask: Optional[torch.Tensor] = None       # [S,P'] observations that were in the problem (bundle_adjustment only)
 
 
 def lm_solve(uv, mask, poses, intr, points, model, mode, param_const=None, point_const=None,
-             options: Optional[BAOptions] = None, allreduce=None, want_trace=False) -> Summary:
+             options: Optional[BAOptions] = None, allreduce=None, want_trace=False, linear_solver_type="DENSE_SCHUR",
+             min_linear_solver_iterations=0, max_linear_solver_iterations=500, eta=0.1) -> Summary:
     """In-place Levenberg-Marquardt on device tensors (vgg_ba_solve).  `allreduce` is a
     vggsfm_b200.dist.AllReduceHook for track-sharded multi-GPU runs.  A rank whose shard holds no track (N = 0:
     shard_range gives empty tail shards when the tracks are few) still takes part in every reduction: it solves 16
-    masked-out padding tracks, as bundle_adjustment() pads, and leaves its empty `points` untouched."""
+    masked-out padding tracks, as bundle_adjustment() pads, and leaves its empty `points` untouched.
+    linear_solver_type="ITERATIVE_SCHUR" solves each step by PCG (vgg_ba_solve_iterative) with the three CG options;
+    it runs on one GPU only, so it raises ValueError together with `allreduce`."""
+    lin = linear_solver(linear_solver_type, min_linear_solver_iterations, max_linear_solver_iterations, eta)
+    iterative = linear_solver_type == "ITERATIVE_SCHUR"
+    if iterative and allreduce is not None:
+        raise ValueError("ITERATIVE_SCHUR runs on one GPU: it takes no all-reduce hook or fabric")
     L = _lib.lib()
     S, N = mask.shape
     dev = uv.device
@@ -214,15 +248,20 @@ def lm_solve(uv, mask, poses, intr, points, model, mode, param_const=None, point
         point_const = torch.ones(n, dtype=torch.uint8, device=dev)
         N = n
     opt = options or default_options()
-    ws = workspace(S, N, model, mode, dev)
+    ws = workspace(S, N, model, mode, dev, iterative=True) if iterative else workspace(S, N, model, mode, dev)
     p = _problem(uv, mask, poses, intr, points, model, mode, param_const, point_const)
     summ = BASummary()
     trace = torch.zeros(max(1, opt.max_num_iterations), 8, dtype=torch.float64) if want_trace else None
+    cg_trace = torch.zeros(max(1, opt.max_num_iterations), 4, dtype=torch.float64) if iterative else None
     cb = allreduce.bind(ws) if allreduce is not None else _lib.ALLREDUCE_FN()
     fabric = getattr(allreduce, "fabric", None)
     with torch.cuda.device(dev):
         st = torch.cuda.current_stream().cuda_stream
-        if fabric is not None:
+        if iterative:
+            rc = L.vgg_ba_solve_iterative(ctypes.byref(p), ctypes.byref(opt), ctypes.byref(lin), ws.data_ptr(),
+                                          ws.numel(), ctypes.byref(summ),
+                                          trace.data_ptr() if trace is not None else None, cg_trace.data_ptr(), st)
+        elif fabric is not None:
             fs = fabric.struct()
             rc = L.vgg_ba_solve_fabric(ctypes.byref(p), ctypes.byref(opt), ws.data_ptr(), ws.numel(), cb, None,
                                        ctypes.byref(fs), ctypes.byref(summ),
@@ -230,10 +269,14 @@ def lm_solve(uv, mask, poses, intr, points, model, mode, param_const=None, point
         else:
             rc = L.vgg_ba_solve(ctypes.byref(p), ctypes.byref(opt), ws.data_ptr(), ws.numel(), cb, None,
                                 ctypes.byref(summ), trace.data_ptr() if trace is not None else None, st)
-    _lib.check(rc, "vgg_ba_solve")
-    return Summary(summ.iterations, summ.successful, TERMINATION.get(summ.termination, "?"), summ.initial_cost,
-                   summ.final_cost, summ.final_radius, summ.device_ms, summ.kernel_launches,
-                   trace[:summ.iterations] if trace is not None else None)
+    _lib.check(rc, "vgg_ba_solve_iterative" if iterative else "vgg_ba_solve")
+    out = Summary(summ.iterations, summ.successful, TERMINATION.get(summ.termination, "?"), summ.initial_cost,
+                  summ.final_cost, summ.final_radius, summ.device_ms, summ.kernel_launches,
+                  trace[:summ.iterations] if trace is not None else None, linear_solver_type)
+    if iterative:
+        out.cg_trace = cg_trace[:summ.iterations]
+        out.cg_iterations = int(out.cg_trace[:, 0].sum().item())
+    return out
 
 
 # --------------------------------------------------------------------------------------------------
@@ -286,14 +329,21 @@ def bundle_adjustment(points3d, extrinsics, intrinsics, extra_params, tracks, ma
                       camera_type="SIMPLE_PINHOLE", options: Optional[BAOptions] = None, max_points3D_val=3000.0,
                       allreduce=None, want_trace=False, refine_focal_length=True, refine_extra_params=True,
                       const_pose=None, const_points=None, gauge=True, do_normalize=True, filter_reconstruction=True,
-                      drop_negative_depth=True):
+                      drop_negative_depth=True, linear_solver_type="DENSE_SCHUR", min_linear_solver_iterations=0,
+                      max_linear_solver_iterations=500, eta=0.1):
     """Tensor-in / tensor-out equivalent of batch_matrix_to_pycolmap + pycolmap.bundle_adjustment +
     filter_reconstruction + pycolmap_to_batch_matrix (triangulation.py:1033-1063).
 
     points3d [P,3], extrinsics [S,3,4], intrinsics [S,3,3], extra_params [S,1]|None, tracks [S,P,2],
     masks [S,P] bool -- CUDA tensors.  Returns (points3D [P',3] f64, extrinsics [S,3,4] f64,
-    intrinsics [S,3,3] f64, extra_params [S,1]|None, valid_idx [P'], Summary)."""
+    intrinsics [S,3,3] f64, extra_params [S,1]|None, valid_idx [P'], Summary).  linear_solver_type and the CG options
+    as lm_solve (ITERATIVE_SCHUR with `allreduce` raises ValueError before anything runs)."""
     model = camera_model_id(camera_type)
+    lin_kw = dict(linear_solver_type=linear_solver_type, min_linear_solver_iterations=min_linear_solver_iterations,
+                  max_linear_solver_iterations=max_linear_solver_iterations, eta=eta)
+    linear_solver(**lin_kw)
+    if linear_solver_type == "ITERATIVE_SCHUR" and allreduce is not None:
+        raise ValueError("ITERATIVE_SCHUR runs on one GPU: it takes no all-reduce hook or fabric")
     dev = tracks.device
     if not tracks.is_cuda:
         raise RuntimeError("vggsfm_b200.bundle_adjustment needs CUDA tensors (no CPU fallback)")
@@ -337,7 +387,7 @@ def bundle_adjustment(points3d, extrinsics, intrinsics, extra_params, tracks, ma
     pc = torch.ones(Pp, dtype=torch.uint8, device=dev)
     pc[:P] = point_const.to(torch.uint8)
     param_const = default_param_const(S, model, mode, dev, refine_focal_length, refine_extra_params, gauge, const_pose)
-    summary = lm_solve(uv, mk, poses, intr, X, model, mode, param_const, pc, options, allreduce, want_trace)
+    summary = lm_solve(uv, mk, poses, intr, X, model, mode, param_const, pc, options, allreduce, want_trace, **lin_kw)
     pts = X[:P]
     if do_normalize:
         poses, pts = normalize(poses, pts, 10.0, 0.1, 0.9, alive)   # BundleAdjustmentController::Run
@@ -384,15 +434,20 @@ def _revert_negative_focal(extr_new, K_new, extra_new, extr_old, K_old, extra_ol
 
 
 def global_BA(triangulated_points, valid_tracks, pred_tracks, inlier_mask, extrinsics, intrinsics, extra_params,
-              image_size, shared_camera=False, camera_type="SIMPLE_PINHOLE", allreduce=None):
+              image_size, shared_camera=False, camera_type="SIMPLE_PINHOLE", allreduce=None,
+              linear_solver_type="DENSE_SCHUR", min_linear_solver_iterations=0, max_linear_solver_iterations=200,
+              eta=0.1):
     """vggsfm/utils/triangulation.py:1020-1073 with the same arguments and return tuple
-    (points3D_opt, extrinsics, intrinsics, extra_params, reconstruction)."""
+    (points3D_opt, extrinsics, intrinsics, extra_params, reconstruction).  The linear-solver options are
+    bundle_adjustment()'s; max_linear_solver_iterations defaults to the 200 of prepare_ba_options."""
     BA_points = triangulated_points[valid_tracks]
     BA_tracks = pred_tracks[:, valid_tracks]
     BA_inlier_masks = inlier_mask[valid_tracks].transpose(0, 1)
     pts, extr, K, extra, valid_idx, summary = bundle_adjustment(
         BA_points, extrinsics, intrinsics, extra_params, BA_tracks, BA_inlier_masks, shared_camera=shared_camera,
-        camera_type=camera_type, options=prepare_ba_options(), allreduce=allreduce)
+        camera_type=camera_type, options=prepare_ba_options(), allreduce=allreduce,
+        linear_solver_type=linear_solver_type, min_linear_solver_iterations=min_linear_solver_iterations,
+        max_linear_solver_iterations=max_linear_solver_iterations, eta=eta)
     extr, K, extra = _revert_negative_focal(extr, K, extra, extrinsics, intrinsics, extra_params)
     rec = _reconstruction(pts, extr, K, extra, BA_tracks[:, valid_idx], summary.mask, image_size, camera_type,
                           shared_camera, summary, summary.alive)
@@ -448,11 +503,12 @@ def get_valid_frame_mask(intrinsics, extrinsics, extra_params, scale):
 def iterative_global_BA(pred_tracks, intrinsics, extrinsics, pred_vis, pred_score, valid_tracks, points3D_opt,
                         image_size, shared_camera=False, min_valid_track_length=2, max_reproj_error=1,
                         ba_options=None, lastBA=False, camera_type="SIMPLE_PINHOLE", extra_params=None,
-                        allreduce=None):
+                        allreduce=None, linear_solver_type="DENSE_SCHUR", min_linear_solver_iterations=0,
+                        max_linear_solver_iterations=200, eta=0.1):
     """vggsfm/utils/triangulation.py:1076-1209: re-triangulate (128 hypotheses) -> keep the last BA's points for
     already-valid tracks -> reprojection/triangle filter -> BA (default options) -> filter again -> compaction.
     Same arguments; returns (points3D_opt, extrinsics, intrinsics, extra_params, valid_tracks, BA_inlier_masks,
-    reconstruction)."""
+    reconstruction).  The linear-solver options are bundle_adjustment()'s (max 200 as in prepare_ba_options)."""
     from . import triangulation as tri
     tn = tri.cam_from_img(pred_tracks, intrinsics, extra_params)
     best_points, best_num, best_mask = tri.triangulate_tracks(extrinsics, tn, track_vis=pred_vis, track_score=pred_score,
@@ -466,7 +522,9 @@ def iterative_global_BA(pred_tracks, intrinsics, extrinsics, pred_vis, pred_scor
     BA_inlier_masks = filtered[:, valid_tracks]
     pts, extr, K, extra, valid_idx, summary = bundle_adjustment(
         BA_points, extrinsics, intrinsics, extra_params, BA_tracks, BA_inlier_masks, shared_camera=shared_camera,
-        camera_type=camera_type, options=ba_options or default_options(), allreduce=allreduce)
+        camera_type=camera_type, options=ba_options or default_options(), allreduce=allreduce,
+        linear_solver_type=linear_solver_type, min_linear_solver_iterations=min_linear_solver_iterations,
+        max_linear_solver_iterations=max_linear_solver_iterations, eta=eta)
     rec = _reconstruction(pts, extr, K, extra, BA_tracks[:, valid_idx], summary.mask, image_size, camera_type,
                           shared_camera, summary, summary.alive)        # the BA'd, filter_reconstruction'd object (:1146)
     if valid_idx.numel() != BA_points.shape[0]:

@@ -1,0 +1,44 @@
+// The iterative (PCG) linear solver of the LM loop, csrc/ba_pcg.cu; used by csrc/ba_solve.cu.
+#pragma once
+#include "common.cuh"
+
+namespace vgg {
+
+constexpr int PCG_CHUNK = 10;             // CG iterations queued between two reads of the done flag
+constexpr int PCG_RESET_PERIOD = 10;      // Ceres' residual_reset_period: r = b - A x every 10th iteration
+constexpr int PCG_STATE_DOUBLES = 32;
+
+// slots of the CG state (PcgBuffers::cg); [0..4] are what the host reads after each LM iteration
+enum : int {
+  CG_MODEL_CHANGE = 0, CG_ITERS = 1, CG_TERM = 2, CG_ZETA = 3, CG_RREL = 4, CG_DONE = 5, CG_RHO = 6, CG_BETA = 7,
+  CG_ALPHA = 8, CG_Q0 = 9, CG_BB = 10, CG_PRE_FAIL = 11,
+  CG_ACC = 16,              // [16..19] per-kernel partial sums (reset by the kernel's last CTA)
+  CG_TICKET_SLOT = 24,      // unsigned counter of the kernel's finished CTAs
+};
+
+// Device buffers of one solve (all [Dpad] unless noted), carved by make_layout in csrc/ba_solve.cu.
+struct PcgBuffers {
+  double *rhs, *hdiag, *gvec;   // reduced right-hand side (unscaled), diag(H_cc), camera gradient
+  double *x, *r, *z, *q, *u;    // CG vectors; u = Dc v, the operand of the Schur part of the matvec
+  double *p[2];                 // search direction, alternating between iterations
+  double *acc, *pinv;           // [9 * pcg_blocks]: sum Z_b Z_b^T, inverted preconditioner blocks
+  double *cg;                   // [PCG_STATE_DOUBLES] scalars, termination and the model change
+};
+
+int pcg_blocks(int S, int ns);
+int launch_pcg_assemble(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
+                        const double* M, const double* q, const PcgBuffers& B, const int* fg_tracks, cudaStream_t st);
+int launch_pcg_init(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
+                    const double* sc_c, double radius, double min_diag, double max_diag, const PcgBuffers& B,
+                    double* bvec, cudaStream_t st);
+int launch_pcg_matvec(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
+                      const double* M, const double* sc_c, const double* hdiag, double radius, double min_diag,
+                      double max_diag, int pmode, const double* p_old, double* p_new, const PcgBuffers& B,
+                      const int* fg_tracks, cudaStream_t st);
+int pcg_run(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
+            const double* M, const double* sc_c, double radius, double min_diag, double max_diag,
+            const vgg_ba_linear_solver& lin, const PcgBuffers& B, double* bvec, const int* fg_tracks, cudaStream_t st);
+int launch_pcg_model_change(const vgg_ba_problem* p, const double* M, const double* g_p, const double* wacc,
+                            const double* d_c, const int* fg_tracks, double* cg, cudaStream_t st);
+
+}  // namespace vgg

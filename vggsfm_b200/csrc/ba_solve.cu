@@ -8,6 +8,7 @@
 #include <string.h>
 #include <map>
 #include <vector>
+#include "ba_pcg.h"
 #include "common.cuh"
 #include "dev_probes.h"
 
@@ -66,15 +67,18 @@ int launch_fabric_allreduce(const FabricDev& fd, size_t flags_off, size_t mail_o
 
 // gathers the accept/reject scalars into one 24-double record so the host reads them with ONE copy:
 // [0..7] = scal[0..7], [8..15] = small[0..7], [16] = factorisation info, [17] = substitution info, [18] = camera part of |x|^2
-// (its point part is small[5], summed over the ranks)
+// (its point part is small[5], summed over the ranks); iterative solves add [20..24] = cg[0..4] (model change, CG
+// iterations, CG termination, zeta, |r| / |b|)
 __global__ void pack_scalars_kernel(const double* __restrict__ scal, const double* __restrict__ small,
-                                    const int* __restrict__ info, double* __restrict__ out) {
+                                    const int* __restrict__ info, const double* __restrict__ cg,
+                                    double* __restrict__ out) {
   const int i = threadIdx.x;
   if (i < 8) out[i] = scal[i];
   else if (i < 16) out[i] = small[i - 8];
   else if (i < 18) out[i] = (double)info[i - 16];
   else if (i == 18) out[i] = scal[8];              // camera part of |x|^2 (xnorm_kernel), 0 unless parameter_tolerance > 0
   else if (i == 19) out[i] = (double)info[2];      // a cross-rank barrier of csrc/fabric.cu timed out
+  else if (i < 25 && cg) out[i] = cg[i - 20];
 }
 
 // |x|^2 of Ceres' reduced program in ambient coordinates (ParameterToleranceReached: step_norm <= tol * (|x| + tol)):
@@ -186,10 +190,13 @@ struct Layout {
   double *chol_diag;
   int *dev_info;
   uint8_t *pconst, *point_const;   // [Dpad], [N]: the solve's constant flags (observed_kernel / effective_const_kernel)
+  PcgBuffers pcg;                  // iterative layout only (Zt, AR and chol_diag are then null)
   size_t bytes;
 };
 
-static int make_layout(int S, int N, int model, int mode, void* base, size_t cap, Layout* L) {
+// iterative: the layout of vgg_ba_solve_iterative -- the same buffers without the Schur operand Zt, the reduced system
+// AR and the factorisation workspace, plus the O(D) vectors of csrc/ba_pcg.cu
+static int make_layout(int S, int N, int model, int mode, void* base, size_t cap, Layout* L, bool iterative = false) {
   int dc, ns, KR;
   if (dims_of(model, mode, &dc, &ns, &KR) != VGG_OK) {
     set_error("bad camera_model/intr_mode");
@@ -218,15 +225,24 @@ static int make_layout(int S, int N, int model, int mode, void* base, size_t cap
   L->wacc = c.take<double>((size_t)N * 3);
   L->d_c = c.take<double>(L->Dpad);
   L->bvec = c.take<double>(L->Dpad);
-  L->Zt = c.take<double>((size_t)L->Kpad * L->Dpad);
-  L->AR = c.take<double>((size_t)L->D * L->Dpad + 3 * (size_t)L->Dpad);
+  L->Zt = iterative ? nullptr : c.take<double>((size_t)L->Kpad * L->Dpad);
+  L->AR = iterative ? nullptr : c.take<double>((size_t)L->D * L->Dpad + 3 * (size_t)L->Dpad);
   L->small = c.take<double>(8 + (size_t)L->Dpad);
   L->scal = c.take<double>(16);
   L->packed = c.take<double>(32);
-  L->chol_diag = c.take<double>(chol_workspace_doubles(L->D + 1));
+  L->chol_diag = iterative ? nullptr : c.take<double>(chol_workspace_doubles(L->D + 1));
   L->dev_info = c.take<int>(4);
   L->pconst = c.take<uint8_t>(L->Dpad);
   L->point_const = c.take<uint8_t>((size_t)N);
+  L->pcg = PcgBuffers{};
+  if (iterative) {
+    PcgBuffers& B = L->pcg;
+    for (double** v : {&B.rhs, &B.hdiag, &B.gvec, &B.x, &B.r, &B.z, &B.q, &B.u, &B.p[0], &B.p[1]})
+      *v = c.take<double>(L->Dpad);
+    B.acc = c.take<double>(9 * (size_t)pcg_blocks(S, ns));
+    B.pinv = c.take<double>(9 * (size_t)pcg_blocks(S, ns));
+    B.cg = c.take<double>(PCG_STATE_DOUBLES);
+  }
   L->bytes = align_up(c.off, 256);
   if (base && c.off > cap) {
     set_error("workspace too small: need %zu bytes, have %zu", c.off, cap);
@@ -695,9 +711,14 @@ int vgg_ba_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, void*
   return vgg_ba_solve_fabric(prob, opt_in, workspace, ws_bytes, allreduce, ar_user, nullptr, summary, trace, stream);
 }
 
-int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, void* workspace, size_t ws_bytes,
-                        vgg_allreduce_fn allreduce, void* ar_user, const vgg_ba_fabric* fabric, vgg_ba_summary* summary,
-                        double* trace, void* stream) {
+// The LM loop of both linear solvers: lin = null solves the reduced camera system directly (DENSE_SCHUR: schur_build,
+// Cholesky, backward substitution), otherwise by PCG (csrc/ba_pcg.cu, ITERATIVE_SCHUR, single GPU: allreduce and
+// fabric null).  Everything else -- point step, camera update, candidate evaluation, accept / reject and the radius
+// rules -- is the same code for both; the iterative solve takes Ceres' model change -(J d)^T (f + J d / 2) instead of
+// the exact-solve identity 0.5 * quad.
+static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, const vgg_ba_linear_solver* lin,
+                    void* workspace, size_t ws_bytes, vgg_allreduce_fn allreduce, void* ar_user,
+                    const vgg_ba_fabric* fabric, vgg_ba_summary* summary, double* trace, double* cg_trace, void* stream) {
   VGG_REQUIRE(prob && workspace && summary, "null pointer");
   VGG_REQUIRE(prob->uv && prob->mask && prob->param_const && prob->poses && prob->intr && prob->points, "null problem array");
   cudaStream_t st = (cudaStream_t)stream;
@@ -713,7 +734,7 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
   }
   const int D = S * dc + ns;
   Layout L;
-  int rc = make_layout(S, N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L);
+  int rc = make_layout(S, N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L, lin != nullptr);
   if (rc) return rc;
   const size_t ar_count = (size_t)D * L.Dpad + 3 * (size_t)L.Dpad;
   // fabric mode: the reduced system lives in symmetric (peer-mapped) memory and is reduced by the producing kernels
@@ -751,6 +772,12 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
   double* rhs = L.AR + (size_t)D * L.Dpad;
   double* hdiag = rhs + L.Dpad;
   double* gvec = hdiag + L.Dpad;
+  if (lin) {
+    Sraw = nullptr;
+    rhs = L.pcg.rhs;
+    hdiag = L.pcg.hdiag;
+    gvec = L.pcg.gvec;
+  }
   // sum (and one max slot) of a small vector over the ranks: in-kernel over the fabric, else through the host hook
   auto reduce_small = [&](double* vec, size_t count, int op) -> int {
     if (fab.on) return fab.allreduce(vec, (int)count, op == 1 ? 0 : -1, st);
@@ -779,7 +806,7 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
   VGG_CUDA_CHECK(cudaMemcpyAsync(L.poses[0], prob->poses, sizeof(double) * (size_t)S * 12, cudaMemcpyDeviceToDevice, st));
   VGG_CUDA_CHECK(cudaMemcpyAsync(L.intr[0], prob->intr, sizeof(double) * (size_t)S * 4, cudaMemcpyDeviceToDevice, st));
   VGG_CUDA_CHECK(cudaMemcpyAsync(L.points[0], prob->points, sizeof(double) * (size_t)N * 3, cudaMemcpyDeviceToDevice, st));
-  VGG_CUDA_CHECK(cudaMemsetAsync(L.Zt, 0, sizeof(double) * (size_t)L.Kpad * L.Dpad, st));
+  if (!lin) VGG_CUDA_CHECK(cudaMemsetAsync(L.Zt, 0, sizeof(double) * (size_t)L.Kpad * L.Dpad, st));
   VGG_CUDA_CHECK(cudaMemsetAsync(L.d_c, 0, sizeof(double) * L.Dpad, st));
 
   // the problem at state `which` (buffer set of the current state or the candidate)
@@ -806,9 +833,10 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
   }
   VGG_CUDA_CHECK(cudaMemsetAsync(L.dev_info, 0, sizeof(int) * 4, st));
   auto read_scalars = [&]() -> int {
-    pack_scalars_kernel<<<1, 32, 0, st>>>(L.scal, L.small, L.dev_info, L.packed);
+    pack_scalars_kernel<<<1, 32, 0, st>>>(L.scal, L.small, L.dev_info, L.pcg.cg, L.packed);
     VGG_LAUNCH_CHECK();
-    VGG_CUDA_CHECK(cudaMemcpyAsync(h_scal, L.packed, sizeof(double) * 24, cudaMemcpyDeviceToHost, st));   // [0..19] used
+    // [0..19] used, [20..24] by the iterative solve
+    VGG_CUDA_CHECK(cudaMemcpyAsync(h_scal, L.packed, sizeof(double) * (lin ? 28 : 24), cudaMemcpyDeviceToHost, st));
     VGG_CUDA_CHECK(cudaStreamSynchronize(st));
     return VGG_OK;
   };
@@ -868,46 +896,68 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
       fd = fab.at(off);
     }
     const vgg_ba_problem pcur = state(cur);
-    if ((rc = schur_build(L, pcur, L.blk[cur], band, fd, radius, opt.min_lm_diagonal, opt.max_lm_diagonal, st, mc_off,
-                          fab.on ? &fab : nullptr)))
-      return rc;
-    // every row block is complete on its owner: pull the others (matrix rows 0..D incl. the rhs row, then hdiag, gvec)
-    if (fab.on && (rc = launch_fabric_gather(fd, D + 3, D + 1, D, L.Dpad, st))) return rc;
-    if (allreduce && !mc_off && (rc = allreduce(ar_user, L.AR, ar_count, 0, st))) return rc;
-    if (!have_scale_c) {
-      if ((rc = launch_jacobi_scale_cams(D, hdiag, L.sc_c, opt.jacobi_scaling, st))) return rc;
-      have_scale_c = true;
-    }
-    if ((rc = launch_scale_damp(D, L.Dpad, Sraw, rhs, hdiag, L.sc_c, prob->param_const, radius, opt.min_lm_diagonal,
-                                opt.max_lm_diagonal, L.bvec, st)))
-      return rc;
-    // Factor the reduced system with the in-repo blocked Cholesky (csrc/chol.cu) on the row-major LOWER triangle of the
-    // BORDERED matrix of order D+1 -- scale_damp put the scaled right-hand side into row D, so the factorisation leaves
-    // y = L^-1 b there (and, mirrored like every panel, in column D): the forward substitution costs nothing and only the
-    // backward substitution L^T x = y remains.  (cuSOLVER potrf on the same matrix took 1.05 ms at n = 2403, this 0.93.)
-    if ((rc = chol_lower_inplace(D + 1, L.Dpad, Sraw, L.chol_diag, L.dev_info, band.end_blk, band.arrow_blk, st))) return rc;
-    // Backward substitution on U = L^T (the row-major upper triangle), y = column D of the buffer.
     const double* dcs = L.bvec;
     size_t dcs_stride = 1;
-    {
-      VGG_CUDA_CHECK(cudaMemsetAsync(L.dev_info + 1, 0, sizeof(int), st));
-      if (D > 7000) {                                 // beyond the own kernel's one co-resident wave of D/64 CTAs
-        cublasHandle_t cb = get_cublas();
-        if (!cb || cublasSetStream(cb, st) != CUBLAS_STATUS_SUCCESS) {
-          set_error("cublasCreate / cublasSetStream failed");
-          return VGG_ESOLVER;
+    if (lin) {
+      // point blocks as schur_build prepares them, then the reduced right-hand side and the Schur-Jacobi blocks in one
+      // pass over the observations, and CG on the implicit reduced system (csrc/ba_pcg.cu)
+      const BlockSet& b = L.blk[cur];
+      if ((rc = launch_point_prep(N, b.H_pp, b.g_p, L.sc_p, pcur.point_const, radius, opt.min_lm_diagonal,
+                                  opt.max_lm_diagonal, L.M, L.q, L.dpp, L.scal, st)))
+        return rc;
+      if ((rc = launch_pcg_assemble(&pcur, dc, ns, L.KR, b.camrec, b.shared, L.M, L.q, L.pcg, band.dev.fg_tracks, st)))
+        return rc;
+      if (!have_scale_c) {
+        if ((rc = launch_jacobi_scale_cams(D, hdiag, L.sc_c, opt.jacobi_scaling, st))) return rc;
+        have_scale_c = true;
+      }
+      if ((rc = launch_pcg_init(&pcur, dc, ns, L.KR, b.camrec, b.shared, L.sc_c, radius, opt.min_lm_diagonal,
+                                opt.max_lm_diagonal, L.pcg, L.bvec, st)))
+        return rc;
+      if ((rc = pcg_run(&pcur, dc, ns, L.KR, b.camrec, b.shared, L.M, L.sc_c, radius, opt.min_lm_diagonal,
+                        opt.max_lm_diagonal, *lin, L.pcg, L.bvec, band.dev.fg_tracks, st)))
+        return rc;
+      dcs = L.pcg.x;
+    } else {
+      if ((rc = schur_build(L, pcur, L.blk[cur], band, fd, radius, opt.min_lm_diagonal, opt.max_lm_diagonal, st, mc_off,
+                            fab.on ? &fab : nullptr)))
+        return rc;
+      // every row block is complete on its owner: pull the others (matrix rows 0..D incl. the rhs row, then hdiag, gvec)
+      if (fab.on && (rc = launch_fabric_gather(fd, D + 3, D + 1, D, L.Dpad, st))) return rc;
+      if (allreduce && !mc_off && (rc = allreduce(ar_user, L.AR, ar_count, 0, st))) return rc;
+      if (!have_scale_c) {
+        if ((rc = launch_jacobi_scale_cams(D, hdiag, L.sc_c, opt.jacobi_scaling, st))) return rc;
+        have_scale_c = true;
+      }
+      if ((rc = launch_scale_damp(D, L.Dpad, Sraw, rhs, hdiag, L.sc_c, prob->param_const, radius, opt.min_lm_diagonal,
+                                  opt.max_lm_diagonal, L.bvec, st)))
+        return rc;
+      // Factor the reduced system with the in-repo blocked Cholesky (csrc/chol.cu) on the row-major LOWER triangle of the
+      // BORDERED matrix of order D+1 -- scale_damp put the scaled right-hand side into row D, so the factorisation leaves
+      // y = L^-1 b there (and, mirrored like every panel, in column D): the forward substitution costs nothing and only the
+      // backward substitution L^T x = y remains.  (cuSOLVER potrf on the same matrix took 1.05 ms at n = 2403, this 0.93.)
+      if ((rc = chol_lower_inplace(D + 1, L.Dpad, Sraw, L.chol_diag, L.dev_info, band.end_blk, band.arrow_blk, st))) return rc;
+      // Backward substitution on U = L^T (the row-major upper triangle), y = column D of the buffer.
+      {
+        VGG_CUDA_CHECK(cudaMemsetAsync(L.dev_info + 1, 0, sizeof(int), st));
+        if (D > 7000) {                                 // beyond the own kernel's one co-resident wave of D/64 CTAs
+          cublasHandle_t cb = get_cublas();
+          if (!cb || cublasSetStream(cb, st) != CUBLAS_STATUS_SUCCESS) {
+            set_error("cublasCreate / cublasSetStream failed");
+            return VGG_ESOLVER;
+          }
+          if (cublasDtrsv(cb, CUBLAS_FILL_MODE_LOWER, CUBLAS_OP_T, CUBLAS_DIAG_NON_UNIT, D, Sraw, L.Dpad, Sraw + D, L.Dpad) !=
+              CUBLAS_STATUS_SUCCESS) {
+            set_error("cublasDtrsv failed to launch");
+            return VGG_ESOLVER;
+          }
+          g_launch_count += 1;
+          dcs = Sraw + D;
+          dcs_stride = (size_t)L.Dpad;
+        } else {
+          // own backward substitution (csrc/trsv.cu): one launch, block rows chained through the solution itself
+          if ((rc = launch_trsv_upper(D, L.Dpad, Sraw, Sraw + D, (size_t)L.Dpad, L.bvec, nullptr, st))) return rc;
         }
-        if (cublasDtrsv(cb, CUBLAS_FILL_MODE_LOWER, CUBLAS_OP_T, CUBLAS_DIAG_NON_UNIT, D, Sraw, L.Dpad, Sraw + D, L.Dpad) !=
-            CUBLAS_STATUS_SUCCESS) {
-          set_error("cublasDtrsv failed to launch");
-          return VGG_ESOLVER;
-        }
-        g_launch_count += 1;
-        dcs = Sraw + D;
-        dcs_stride = (size_t)L.Dpad;
-      } else {
-        // own backward substitution (csrc/trsv.cu): one launch, block rows chained through the solution itself
-        if ((rc = launch_trsv_upper(D, L.Dpad, Sraw, Sraw + D, (size_t)L.Dpad, L.bvec, nullptr, st))) return rc;
       }
     }
     if ((rc = launch_cam_step(D, dcs, dcs_stride, L.sc_c, hdiag, gvec, prob->param_const, radius, opt.min_lm_diagonal,
@@ -919,6 +969,8 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
       return rc;
     if ((rc = launch_cam_update(S, dc, ns, prob->camera_model, L.d_c, L.poses[cur], L.intr[cur], L.poses[cand],
                                 L.intr[cand], st)))
+      return rc;
+    if (lin && (rc = launch_pcg_model_change(&pcur, L.M, L.blk[cur].g_p, L.wacc, L.d_c, band.dev.fg_tracks, L.pcg.cg, st)))
       return rc;
     if ((rc = eval(cand))) return rc;
     // point-side model terms join the candidate cost in the small all-reduce
@@ -954,12 +1006,17 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
     const double c_cost = h_scal[8];
     const double quad = h_scal[0] + h_scal[9];
     const double step_norm = sqrt(h_scal[1] + h_scal[10]);
-    const double model_change = 0.5 * quad;
+    const double model_change = lin ? h_scal[20] : 0.5 * quad;
     if (h_scal[19] != 0.0) {
       set_error("fabric barrier timed out: a peer rank did not arrive");
       return VGG_ECUDA;
     }
-    const bool solver_bad = h_info[0] != 0 || h_info[1] != 0 || h_scal[7] > 0 || h_scal[11] > 0;
+    const bool solver_bad = h_info[0] != 0 || h_info[1] != 0 || h_scal[7] > 0 || h_scal[11] > 0 ||
+                            (lin && h_scal[22] == VGG_CG_FAILURE);
+    if (lin && cg_trace) {
+      double* ct = cg_trace + (size_t)(it - 1) * 4;
+      ct[0] = h_scal[21]; ct[1] = h_scal[22]; ct[2] = h_scal[23]; ct[3] = h_scal[24];
+    }
     double* tr = trace ? trace + (size_t)(it - 1) * 8 : nullptr;
     if (tr) {
       tr[0] = it; tr[1] = cost; tr[2] = c_cost; tr[3] = model_change; tr[4] = 0; tr[5] = radius; tr[6] = step_norm; tr[7] = 0;
@@ -1024,6 +1081,81 @@ int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in
   summary->final_radius = radius;
   summary->device_ms = ms;
   summary->kernel_launches = g_launch_count;
+  return VGG_OK;
+}
+
+int vgg_ba_solve_fabric(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, void* workspace, size_t ws_bytes,
+                        vgg_allreduce_fn allreduce, void* ar_user, const vgg_ba_fabric* fabric, vgg_ba_summary* summary,
+                        double* trace, void* stream) {
+  return lm_solve(prob, opt_in, nullptr, workspace, ws_bytes, allreduce, ar_user, fabric, summary, trace, nullptr, stream);
+}
+
+void vgg_ba_default_linear_solver(vgg_ba_linear_solver* lin) {
+  lin->type = VGG_BA_DENSE_SCHUR;
+  lin->min_linear_solver_iterations = 0;
+  lin->max_linear_solver_iterations = 500;
+  lin->eta = 0.1;
+}
+
+int vgg_ba_workspace_bytes_iterative(int S, int N, int camera_model, int intr_mode, size_t* bytes) {
+  VGG_REQUIRE(S > 0 && N > 0 && bytes, "S, N must be positive");
+  Layout L;
+  const int rc = make_layout(S, N, camera_model, intr_mode, nullptr, 0, &L, true);
+  if (rc) return rc;
+  *bytes = L.bytes;
+  return VGG_OK;
+}
+
+int vgg_ba_solve_iterative(const vgg_ba_problem* prob, const vgg_ba_options* opt, const vgg_ba_linear_solver* lin,
+                           void* workspace, size_t ws_bytes, vgg_ba_summary* summary, double* trace, double* cg_trace,
+                           void* stream) {
+  VGG_REQUIRE(lin && lin->type == VGG_BA_ITERATIVE_SCHUR, "vgg_ba_solve_iterative needs lin->type = VGG_BA_ITERATIVE_SCHUR");
+  VGG_REQUIRE(lin->min_linear_solver_iterations >= 0 &&
+                  lin->max_linear_solver_iterations >= lin->min_linear_solver_iterations && lin->eta > 0.0 &&
+                  isfinite(lin->eta),
+              "linear solver options: need 0 <= min <= max iterations and a positive finite eta");
+  return lm_solve(prob, opt, lin, workspace, ws_bytes, nullptr, nullptr, nullptr, summary, trace, cg_trace, stream);
+}
+
+/* development probe (csrc/dev_probes.h): the preparation of the iterative solve and one product of its reduced
+ * operator, at the given blocks, scales and radius, with the flags of prob taken as the solve's effective ones */
+int vgg_dev_pcg_probe(const vgg_ba_problem* prob, const double* camrec, const double* g_p, const double* H_pp,
+                      const double* shared_in, const double* scale_p, const double* scale_c, double radius,
+                      double min_diag, double max_diag, const double* x_in, void* workspace, size_t ws_bytes,
+                      double* y_out, double* b_out, double* pinv_out, double* state_out, void* stream) {
+  VGG_REQUIRE(prob && camrec && g_p && H_pp && shared_in && scale_p && scale_c && x_in && workspace, "null pointer");
+  VGG_REQUIRE(prob->param_const, "null param_const");
+  cudaStream_t st = (cudaStream_t)stream;
+  g_launch_count = 0;
+  Layout L;
+  int rc = make_layout(prob->S, prob->N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L, true);
+  if (rc) return rc;
+  const int D = L.D;
+  VGG_CUDA_CHECK(cudaMemcpyAsync(L.sc_p, scale_p, sizeof(double) * (size_t)L.N * 3, cudaMemcpyDeviceToDevice, st));
+  VGG_CUDA_CHECK(cudaMemcpyAsync(L.sc_c, scale_c, sizeof(double) * (size_t)D, cudaMemcpyDeviceToDevice, st));
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.scal, 0, sizeof(double) * 16, st));
+  if ((rc = launch_point_prep(L.N, H_pp, g_p, L.sc_p, prob->point_const, radius, min_diag, max_diag, L.M, L.q, L.dpp,
+                              L.scal, st)))
+    return rc;
+  if ((rc = launch_pcg_assemble(prob, L.dc, L.ns, L.KR, camrec, shared_in, L.M, L.q, L.pcg, nullptr, st))) return rc;
+  if ((rc = launch_pcg_init(prob, L.dc, L.ns, L.KR, camrec, shared_in, L.sc_c, radius, min_diag, max_diag, L.pcg, L.bvec,
+                            st)))
+    return rc;
+  if (state_out)
+    VGG_CUDA_CHECK(cudaMemcpyAsync(state_out, L.pcg.cg, sizeof(double) * PCG_STATE_DOUBLES, cudaMemcpyDeviceToDevice, st));
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.pcg.cg + CG_DONE, 0, sizeof(double), st));   // the product runs whatever init decided
+  VGG_CUDA_CHECK(cudaMemcpyAsync(L.pcg.x, x_in, sizeof(double) * (size_t)D, cudaMemcpyDeviceToDevice, st));
+  if ((rc = launch_pcg_matvec(prob, L.dc, L.ns, L.KR, camrec, shared_in, L.M, L.sc_c, L.pcg.hdiag, radius, min_diag,
+                              max_diag, 0, nullptr, nullptr, L.pcg, nullptr, st)))
+    return rc;
+  auto out = [&](double* dst, const double* src, size_t n) -> int {
+    if (dst) VGG_CUDA_CHECK(cudaMemcpyAsync(dst, src, sizeof(double) * n, cudaMemcpyDeviceToDevice, st));
+    return VGG_OK;
+  };
+  if ((rc = out(y_out, L.pcg.q, D)) || (rc = out(b_out, L.bvec, D)) ||
+      (rc = out(pinv_out, L.pcg.pinv, 9 * (size_t)pcg_blocks(prob->S, L.ns))))
+    return rc;
+  VGG_CUDA_CHECK(cudaStreamSynchronize(st));
   return VGG_OK;
 }
 

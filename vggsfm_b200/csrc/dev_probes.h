@@ -80,6 +80,17 @@ int vgg_dev_schur_build(const vgg_ba_problem* prob, const double* camrec, const 
 int vgg_dev_syrk_work_list(int Kpad, int Dpad, const int* ranges_host, int count, int nworkers, int* items_host,
                            int cap, int* nwork);
 
+/* The iterative solve's preparation at the given blocks (as vgg_ba_schur takes them), point scales scale_p [N,3], camera
+ * scales scale_c [D] and radius, with prob->param_const / point_const taken as the solve's effective flags; then one
+ * product y = A x of the scaled, damped reduced operator (csrc/ba_pcg.cu).  Outputs (device, each may be NULL): y_out [D],
+ * b_out [D] (scaled right-hand side, pinned entries 0), pinv_out [9 * (3 S + (ns > 0))] (the inverted Schur-Jacobi
+ * blocks, row-major 3x3: rotation, translation, intrinsics of each frame, then the shared block), state_out [32] (the CG
+ * state after its initialisation).  workspace from vgg_ba_workspace_bytes_iterative. */
+int vgg_dev_pcg_probe(const vgg_ba_problem* prob, const double* camrec, const double* g_p, const double* H_pp,
+                      const double* shared_in, const double* scale_p, const double* scale_c, double radius,
+                      double min_diag, double max_diag, const double* x_in, void* workspace, size_t ws_bytes,
+                      double* y_out, double* b_out, double* pinv_out, double* state_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

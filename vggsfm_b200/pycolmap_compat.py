@@ -41,6 +41,9 @@ class _SolverOptions:
         self.parameter_tolerance = 0.0
         self.max_num_iterations = 100
         self.max_linear_solver_iterations = 200
+        self.min_linear_solver_iterations = 0
+        self.linear_solver_type = "DENSE_SCHUR"      # or "ITERATIVE_SCHUR" (PCG, for problems the dense solve cannot hold)
+        self.eta = 0.1
         self.minimizer_progress_to_stdout = False
         self.num_threads = -1
 
@@ -55,11 +58,14 @@ class BundleAdjustmentOptions:
         self.print_summary = False
 
     def _native(self):
+        """(vgg_ba_options, the linear-solver keywords of bundle_adjustment.bundle_adjustment)."""
         o = _ba.default_options()
         so = self.solver_options
         o.function_tolerance, o.gradient_tolerance, o.parameter_tolerance = so.function_tolerance, so.gradient_tolerance, so.parameter_tolerance
         o.max_num_iterations = int(so.max_num_iterations)
-        return o
+        lin = dict(linear_solver_type=so.linear_solver_type, min_linear_solver_iterations=int(so.min_linear_solver_iterations),
+                   max_linear_solver_iterations=int(so.max_linear_solver_iterations), eta=float(so.eta))
+        return o, lin
 
 
 class BundleAdjustmentConfig:
@@ -147,14 +153,15 @@ def bundle_adjustment(reconstruction, options=None):
     """``pycolmap.bundle_adjustment(reconstruction, options)``: COLMAP's BundleAdjustmentController on the CUDA LM
     (gauge, negative-depth filter, Normalize(10)) -- in place on the object, like pycolmap."""
     options = options or BundleAdjustmentOptions()
+    native, lin = options._native()
     d = _dense(reconstruction)
     dev = _dev()
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
     pts, extr, K, extra, valid_idx, summ = _ba.bundle_adjustment(
         t(d["xyz"]), t(d["extr"]), t(d["K"]), t(d["extra"]) if d["extra"] is not None else None, t(d["tracks"]), t(d["masks"]),
-        shared_camera=d["shared"], camera_type=d["camera_type"], options=options._native(), max_points3D_val=float("inf"),
+        shared_camera=d["shared"], camera_type=d["camera_type"], options=native, max_points3D_val=float("inf"),
         refine_focal_length=options.refine_focal_length, refine_extra_params=options.refine_extra_params,
-        filter_reconstruction=False)
+        filter_reconstruction=False, **lin)
     _write_back(reconstruction, d, pts, extr, K, extra, valid_idx, summ.alive)
     reconstruction.summary = summ
     return summ

@@ -87,7 +87,8 @@ def window_bundle_adjustment(window_points_all, extrinsics, intrinsics, extra_pa
 
 
 def joint_BA(points3D, extrinsics, intrinsics, extra_params, tracks, masks, camera_type="SIMPLE_PINHOLE", reproj_error=2.0,
-             tri_angle=1.5, normalize=True):
+             tri_angle=1.5, normalize=True, linear_solver_type="DENSE_SCHUR", min_linear_solver_iterations=0,
+             max_linear_solver_iterations=500, eta=0.1):
     """Tensor form of VideoRunner.joint_BA (video_runner.py:494-541): all frames so far, all points, ONE shared
     camera, default Ceres options through the COLMAP controller (gauge + negative-depth filter + Normalize), then the
     2 px / 1.5 degree point filter and a second normalisation.  The runner keeps this state in its point_dict /
@@ -98,7 +99,9 @@ def joint_BA(points3D, extrinsics, intrinsics, extra_params, tracks, masks, came
     valid_points [P]) -- filtered observations are cleared in `masks`, deleted points are False in `valid_points`.
     The observation filter is the reference's own filter_all_points3D rule (reprojection <= reproj_error and positive
     depth per observation, >= 2 survivors, one camera pair with >= tri_angle), which is what COLMAP's
-    ObservationManager.filter_all_points3D + filter_observations_with_negative_depth compute [3P-memory]."""
+    ObservationManager.filter_all_points3D + filter_observations_with_negative_depth compute [3P-memory].
+    linear_solver_type="ITERATIVE_SCHUR" (and the CG options of bundle_adjustment.lm_solve) solves long sequences whose
+    dense reduced camera system does not fit in memory."""
     S, P = masks.shape
     K = intrinsics.expand(S, -1, -1)
     ex = extra_params.expand(S, -1) if extra_params is not None else None
@@ -108,7 +111,9 @@ def joint_BA(points3D, extrinsics, intrinsics, extra_params, tracks, masks, came
     global last_joint_summary
     pts_o, extr, K_o, ex_o, valid_idx, summary = ba.bundle_adjustment(
         pts, poses, K, ex, tracks, masks, shared_camera=True, camera_type=camera_type, options=ba.default_options(),
-        filter_reconstruction=False)
+        filter_reconstruction=False, linear_solver_type=linear_solver_type,
+        min_linear_solver_iterations=min_linear_solver_iterations,
+        max_linear_solver_iterations=max_linear_solver_iterations, eta=eta)
     last_joint_summary = summary
     out = pts.clone()
     out[valid_idx] = pts_o
@@ -216,12 +221,16 @@ class SceneStore:
         self.set_extrinsics(start_idx, extrinsics)
 
     def joint_bundle_adjustment(self, start_idx, end_idx, intrinsics, extra_params, camera_type="SIMPLE_PINHOLE",
-                                reproj_error=2.0, tri_angle=1.5, normalize=True):
+                                reproj_error=2.0, tri_angle=1.5, normalize=True, linear_solver_type="DENSE_SCHUR",
+                                min_linear_solver_iterations=0, max_linear_solver_iterations=500, eta=0.1):
         """VideoRunner.joint_BA (:494-541) on the store: dense view -> joint_BA (CUDA) -> store rebuilt from the result.
-        Returns the refined shared (intrinsics [1,3,3], extra_params [1,1]|None)."""
+        Returns the refined shared (intrinsics [1,3,3], extra_params [1,1]|None).  Linear-solver options as joint_BA."""
         xyz, tracks, masks, extr = self.dense(start_idx, end_idx)
         pts, extr, K, ex, new_masks, valid = joint_BA(xyz, extr, intrinsics, extra_params, tracks, masks, camera_type=camera_type,
-                                                      reproj_error=reproj_error, tri_angle=tri_angle, normalize=normalize)
+                                                      reproj_error=reproj_error, tri_angle=tri_angle, normalize=normalize,
+                                                      linear_solver_type=linear_solver_type,
+                                                      min_linear_solver_iterations=min_linear_solver_iterations,
+                                                      max_linear_solver_iterations=max_linear_solver_iterations, eta=eta)
         self.replace_from_ba(start_idx, pts, extr, tracks, new_masks, valid)
         return K.float(), (ex.float() if ex is not None else None)
 
