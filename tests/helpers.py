@@ -48,6 +48,13 @@ def far_points_first_case():
     return dict(c, points=c["points"][order].copy(), uv=c["uv"][:, order].copy(), mask=c["mask"][:, order].copy())
 
 
+def shuffled_twin(c, seed=0):
+    """c with its points in a fixed random order: the same problem, but every frame's visible points span the whole
+    track axis, so the band detection of vgg_ba_solve finds nothing to skip and the solve takes its dense path"""
+    perm = np.random.default_rng(seed).permutation(c["mask"].shape[1])
+    return dict(c, points=c["points"][perm].copy(), uv=c["uv"][:, perm].copy(), mask=c["mask"][:, perm].copy())
+
+
 def hidden_case(S, N, cam, mode, seed, point_value, uv_value, n_hidden=3, hidden_frame=None, case=None):
     """(problem with hidden values, its clean twin, hidden point indices).  The hidden points' columns are masked out
     entirely; a third of the other masked slots get uv_value; hidden_frame (if given) loses every observation and gets a

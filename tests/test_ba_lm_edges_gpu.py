@@ -45,7 +45,7 @@ import pytest
 
 from oracle import ba_oracle as bo
 from tests.helpers import (ba_case, backward_error, banded_ba_case, recovered_step, reference_system,
-                           rotation_angle_deg, to_dev)
+                           rotation_angle_deg, shuffled_twin, to_dev)
 
 pytestmark = pytest.mark.gpu
 
@@ -388,15 +388,14 @@ def _big_case(name):
 
 @pytest.mark.parametrize("name,band", [("1000x2048", None), ("1001x2048", None), ("1001x6000", None),
                                        ("1001x6000", "0")])
-def test_big_step_backward_error(cuda_dev, monkeypatch, name, band):
-    """one LM step at D = 7000 / 7007 in the full damped system (test_lm_step_gpu.py's backward error <= 1e-12)"""
+def test_big_step_backward_error(cuda_dev, name, band):
+    """one LM step at D = 7000 / 7007 in the full damped system (test_lm_step_gpu.py's backward error <= 1e-12); band
+    "0": the banded case's shuffled twin, which takes the dense path"""
     import torch
     from vggsfm_b200 import bundle_adjustment as ba
-    if band is None:
-        monkeypatch.delenv("VGG_BAND", raising=False)
-    else:
-        monkeypatch.setenv("VGG_BAND", band)
     c = _big_case(name)
+    if band == "0":
+        c = shuffled_twin(c)
     S, N = c["mask"].shape
     model, mode = c["model"], c["mode"]
     dc, ns = bo.dims(model, mode)
@@ -418,15 +417,14 @@ def test_big_step_backward_error(cuda_dev, monkeypatch, name, band):
     assert not d_c[pc].any()
     eta = backward_error(ref, d_c / ref["sc_c"], u_c / ref["sc_c"], d_p / ref["sc_p"], u_p / ref["sc_p"])
     c_cost = bo.cost_only(*new, c["uv"], c["mask"], model)
-    print(f"big step {name} VGG_BAND={band}: D = {S * dc + ns}, eta = {eta:.2e}, "
+    print(f"big step {name}{' shuffled' if band == '0' else ''}: D = {S * dc + ns}, eta = {eta:.2e}, "
           f"candidate cost {abs(tr[0, 2] / c_cost - 1):.1e}")
     assert eta <= 1e-12, (name, eta)
     assert abs(tr[0, 2] - c_cost) <= 1e-12 * c_cost
 
 
-def test_big_trajectory(cuda_dev, monkeypatch):
+def test_big_trajectory(cuda_dev):
     """3 LM iterations at D = 7007 (cuBLAS back-substitution in every one) against the oracle"""
-    monkeypatch.delenv("VGG_BAND", raising=False)
     _, _, s, _ = _solve(_big_case("1001x2048"), max_num_iterations=3, check_margins=False,
                         label="1001x2048 D = 7007, 3 iterations")
     assert s.iterations == 3 and s.successful >= 1

@@ -189,11 +189,10 @@ def test_point_step_matches_stored_W(cuda_dev, S, N, cam, mode):
     _one_step_check(c, pconst, param_const, cuda_dev, f"{S}x{N} {cam} mode {mode}")
 
 
-def test_banded_skip_regions_stay_zero(cuda_dev, monkeypatch):
-    """a sequential problem with the band hint on (VGG_BAND unset): the solve's step against the reduced system of the
-    stored W (a Zt region the band skip left wrong moves the camera step off it); then, through vgg_ba_schur (dense),
-    exact zeros between frames without a common point"""
-    monkeypatch.delenv("VGG_BAND", raising=False)
+def test_banded_skip_regions_stay_zero(cuda_dev):
+    """a sequential problem with the band hint on: the solve's step against the reduced system of the stored W (a Zt
+    region the band skip left wrong moves the camera step off it); then, through vgg_ba_schur (dense), exact zeros
+    between frames without a common point"""
     c = banded_ba_case(160, 2050, "SIMPLE_RADIAL", bo.INTR_SHARED, life=24, seed=41)
     S, N = c["mask"].shape
     pconst = np.zeros(N, dtype=bool)

@@ -8,7 +8,7 @@ Bars, applied to every successful call (derivations in oracle/chol_oracle.py):
   3. where the pivot is known (diagonal matrices, the first row of a diagonal block) L_jj is within 4 ulps of
      sqrt(a_jj) for the first pivot of a leaf pair and 9 for the second;
   4. info is never INT_MAX (a stalled hand-off between CTAs) -- asserted on every call.
-Cases: orders across the one-block / program-order / lookahead boundaries and every leaf, sub-panel and panel boundary;
+Cases: orders across the one-block / two-block / captured-graph boundaries and every leaf, sub-panel and panel boundary;
 failing pivots (negative, NaN, subnormal, +inf, two of them, both of a pair, in band and arrow) at every leaf position
 class of the first, a middle and the last block, each followed by a good matrix on the same buffer; graded scales whose
 pivot pairs leave the two-pivot range; ill-conditioned and nearly dependent pairs; the bordered matrix of the LM loop;
@@ -306,7 +306,7 @@ def _band_case():
 
 
 def test_representative_set_graph(cuda_dev):
-    """257 (program order), 2403, 4500 (second wave) and a band + arrow matrix under bars 1 and 2, with a failure and
+    """257 (the smallest captured order), 2403, 4500 (second wave) and a band + arrow matrix under bars 1 and 2, with a failure and
     a recovery on each buffer"""
     for n in (257, 2403, 4500):
         s = Slot(n)

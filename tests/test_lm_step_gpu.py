@@ -14,8 +14,9 @@ coupling block or observation gives eta of 1e-4 or more; rounding gives about 1e
 the model change and the step norm the solver reported (trace columns 3 and 6) at the recovered step, and the candidate
 cost (column 2) against the oracle's cost at the returned parameters.
 
-Banded (video-like) problems run with the band hint off (VGG_BAND=0) and on (unset); each run is checked against the
-oracle on its own, and the hint the solver computed is read back through a development probe and compared with
+Banded (video-like) problems run with the band hint on (points in creation order) and off (the same problem with its
+points in random order, which leaves the detection nothing to skip); each run is checked against the oracle on its
+own, and the hint the solver computed is read back through a development probe and compared with
 oracle/band_oracle.py table by table."""
 import ctypes
 
@@ -24,7 +25,7 @@ import pytest
 
 from oracle import ba_oracle as bo
 from oracle import band_oracle
-from tests.helpers import ba_case, backward_error, banded_ba_case, recovered_step, reference_system, to_dev
+from tests.helpers import ba_case, backward_error, banded_ba_case, recovered_step, reference_system, shuffled_twin, to_dev
 
 pytestmark = pytest.mark.gpu
 
@@ -63,16 +64,13 @@ def _band_record():
 
 
 def _check_band(c, band):
-    """banded problem: the hint the solver took equals band_oracle.band_tables; band None = dense expected"""
+    """banded problem: the hint the solver took equals band_oracle.band_tables; band None or "shuffled" = dense expected"""
     rec = _band_record()
-    if band is None:
+    if band in (None, "shuffled"):
         assert not (rec["active"] or rec["chol"] or rec["tables"]), rec
         return
     dc, ns = bo.dims(c["model"], c["mode"])
     t = band_oracle.band_tables(c["mask"], dc, ns)
-    if band == "0":
-        assert not (rec["active"] or rec["chol"] or rec["tables"]), rec
-        return
     assert rec["active"] and rec["chol"] and rec["tables"], rec
     assert np.array_equal(rec["rb_range"], t["rb_range"])
     assert np.array_equal(rec["end_blk"], t["end_blk"]) and rec["arrow_blk"] == t["arrow_blk"]
@@ -163,30 +161,26 @@ def _banded_case(name, mask_seed=0):
 
 
 @pytest.mark.parametrize("name", ["8x256", "64x1000", "45x700", "C3"])
-def test_dense_step_matches_oracle(cuda_dev, monkeypatch, name):
-    monkeypatch.delenv("VGG_BAND", raising=False)
+def test_dense_step_matches_oracle(cuda_dev, name):
     c, pc, ptc = _dense_case(name)
     _one_step(c, cuda_dev, pc, ptc, label=name)
     _check_band(c, None)
 
 
-@pytest.mark.parametrize("band", ["0", "1"])
+@pytest.mark.parametrize("band", ["shuffled", "1"])
 @pytest.mark.parametrize("name", ["160x4003", "130x2500", "128x2048"])
-def test_banded_step_matches_oracle(cuda_dev, monkeypatch, name, band):
-    """band "1" = VGG_BAND unset (hint on)"""
-    if band == "1":
-        monkeypatch.delenv("VGG_BAND", raising=False)
-    else:
-        monkeypatch.setenv("VGG_BAND", band)
+def test_banded_step_matches_oracle(cuda_dev, name, band):
+    """band "1": points in creation order (hint on); "shuffled": the shuffled twin (hint off)"""
     c = _banded_case(name)
-    _one_step(c, cuda_dev, label=f"{name} VGG_BAND={band}")
+    if band == "shuffled":
+        c = shuffled_twin(c)
+    _one_step(c, cuda_dev, label=f"{name} band hint {'on' if band == '1' else 'off (shuffled)'}")
     _check_band(c, band)
 
 
-def test_back_to_back_band_dense_band(cuda_dev, monkeypatch):
+def test_back_to_back_band_dense_band(cuda_dev):
     """One process, one workspace: banded, then dense, then banded with another mask (a new hint): the workspace cache,
     the SYRK work-list cache and the thread-local band tables must follow."""
-    monkeypatch.delenv("VGG_BAND", raising=False)
     c = _banded_case("160x4003", mask_seed=0)
     _one_step(c, cuda_dev, label="160x4003 first")
     _check_band(c, "1")

@@ -20,8 +20,7 @@ from oracle import ozaki_oracle as oz
 pytestmark = pytest.mark.gpu
 
 
-def _run(Z, s, dev, rg=None):
-    """rg: band hint (k-block range per 128-column row block of Z), None = dense"""
+def _run(Z, s, dev):
     import torch
     from vggsfm_b200 import _lib
     L = _lib.lib()
@@ -32,11 +31,8 @@ def _run(Z, s, dev, rg=None):
     _lib.check(L.vgg_syrk_ozaki_workspace_bytes(Kpad, Dpad, s, ctypes.byref(nb)), "vgg_syrk_ozaki_workspace_bytes")
     ws = torch.empty(nb.value, dtype=torch.uint8, device=dev)
     with torch.cuda.device(dev):
-        args = (Kpad, Dpad, Zt.data_ptr(), C.data_ptr(), s, ws.data_ptr(), ws.numel(), torch.cuda.current_stream().cuda_stream)
-        if rg is None:
-            _lib.check(L.vgg_syrk_ozaki(*args), "vgg_syrk_ozaki")
-        else:
-            _lib.check(L.vgg_dev_syrk_ozaki_band(*args, rg.ctypes.data, rg.size), "vgg_dev_syrk_ozaki_band")
+        _lib.check(L.vgg_syrk_ozaki(Kpad, Dpad, Zt.data_ptr(), C.data_ptr(), s, ws.data_ptr(), ws.numel(),
+                                    torch.cuda.current_stream().cuda_stream), "vgg_syrk_ozaki")
         torch.cuda.synchronize()
     full = C.cpu().numpy()
     del Zt, C, ws
@@ -156,38 +152,22 @@ def test_accumulates_and_flags_nonfinite(cuda_dev):
 
 
 def _banded(Dpad, KB, seed):
+    """a sequential problem's operand: row block rb is non-zero in k blocks [2 rb, 2 rb + 7) only, the last (the shared
+    camera's column) everywhere"""
     Z = _case(Dpad, KB * 64, seed)
     nb = Dpad // 128
-    rg = np.zeros((nb, 2), dtype=np.int32)
-    for rb in range(nb):
-        lo, hi = (0, KB) if rb == nb - 1 else (2 * rb, min(KB, 2 * rb + 7))        # last block: dense (the shared camera's column)
-        rg[rb] = (lo, hi)
+    for rb in range(nb - 1):
+        lo, hi = 2 * rb, min(KB, 2 * rb + 7)
         Z[:lo * 64, rb * 128:(rb + 1) * 128] = 0.0
         Z[hi * 64:, rb * 128:(rb + 1) * 128] = 0.0
-    return Z, rg
+    return Z
 
 
-def test_band_hint_skips_only_zero_blocks(cuda_dev):
-    """With the band hint (k-block range per 128-column row block outside which Zt is zero) the kernel skips tiles
-    whose ranges do not meet and shortens the rest: the result must equal the dense product of the same Z."""
-    Z, rg = _banded(1024, 24, 11)
-    dense = _run(Z, 7, cuda_dev)
-    got = _run(Z, 7, cuda_dev, rg)
-    _check(Z, dense, 7, cuda_dev, "band: dense")
-    _check(Z, got, 7, cuda_dev, "band: hint")
-    again = _run(Z, 7, cuda_dev)                       # and the cached plan goes back to dense without the hint
-    _check(Z, again, 7, cuda_dev, "band: dense again")
-
-
-def test_plan_cache_alternating_shapes(cuda_dev):
-    """The host plan is cached per (Kpad, Dpad, s, band hint): alternating them in one process must re-plan every
-    time the key changes and reuse nothing stale."""
-    Zb, rg = _banded(1024, 24, 12)
-    cases = {"a": (_case(256, 640, 21), 7), "b": (_case(384, 1040, 22), 5), "c": (_case(256, 700, 23), 4)}
-    for key in ["a", "b", "band", "a", "band-dense", "c", "band", "b", "c"]:
-        if key.startswith("band"):
-            got = _run(Zb, 7, cuda_dev, None if key == "band-dense" else rg)
-            _check(Zb, got, 7, cuda_dev, f"plan cache {key}")
-        else:
-            Z, s = cases[key]
-            _check(Z, _run(Z, s, cuda_dev), s, cuda_dev, f"plan cache {key}")
+def test_plan_cache_alternating_shapes_and_slice_counts(cuda_dev):
+    """The host plan is cached per (Kpad, Dpad, s): alternating them in one process must re-plan every time the key
+    changes and reuse nothing stale."""
+    cases = {"a": (_case(256, 640, 21), 7), "b": (_case(384, 1040, 22), 5), "c": (_case(256, 700, 23), 4),
+             "band": (_banded(1024, 24, 12), 7)}
+    for key in ["a", "b", "band", "a", "band", "c", "band", "b", "c"]:
+        Z, s = cases[key]
+        _check(Z, _run(Z, s, cuda_dev), s, cuda_dev, f"plan cache {key}")

@@ -19,36 +19,29 @@ def test_sequential_run_tracks_ground_truth(cuda_dev):
     assert out["camera_centre_rmse_vs_gt"] < 0.02 * out["trajectory_length"]
 
 
+def _band_hint_meta():
+    """{SYRK k-range hint, factorisation band, device tables} of the most recent solve (vgg_dev_last_band_hint)"""
+    import numpy as np
+    from vggsfm_b200 import _lib
+    meta = np.zeros(8, dtype=np.int32)
+    _lib.check(_lib.lib().vgg_dev_last_band_hint(meta.ctypes.data, None, None, None, None), "vgg_dev_last_band_hint")
+    return [bool(v) for v in meta[:3]]
+
+
 def test_band_hint_does_not_change_the_joint_ba(cuda_dev):
-    """The tile / k-range skipping of the tensor-core SYRK (band hint from the visibility mask, csrc/ba_solve.cu) must
-    leave the solve unchanged: same minimum (final cost to 1e-9 relative).  The iteration COUNT is not compared: the
-    last iterations of these solves sit on the gradient / function tolerance and the count moves by a few from run to
-    run in either mode (f64 RED order; tools/band_parity_check.py shows it)."""
+    """The band skipping (band hint from the visibility mask, csrc/ba_solve.cu: SYRK, Cholesky, ba_blocks, z_build and
+    backsub) must leave the solve unchanged.  The same problem with its points in random order is the dense twin: every
+    frame's [first, last] visible point then spans almost every track, so the detection must find nothing to skip.
+    Both reach the same minimum (final cost to 1e-9 relative).  The iteration COUNT is not compared: the last
+    iterations of these solves sit on the gradient / function tolerance and the count moves by a few from run to run
+    in either mode (f64 RED order)."""
     import video_c5
     from vggsfm_b200 import video
     res = {}
-    for band in ("0", "1"):               # dense / SYRK, Cholesky, ba_blocks, z_build and backsub skips
-        os.environ["VGG_BAND"] = band
-        try:
-            out = video_c5.final_problem(frames=320, new_per_window=128, dev=cuda_dev, reps=1)
-            res[band] = (out["lm_iterations"][0], float(video.last_joint_summary.final_cost))
-        finally:
-            os.environ.pop("VGG_BAND", None)
-    assert res["0"][0] > 5 and res["1"][0] > 5
-    assert abs(res["0"][1] - res["1"][1]) <= 1e-9 * abs(res["0"][1])
-
-
-def test_band_detection_is_safe_for_unordered_points(cuda_dev):
-    """Points in random order: every frame's [first, last] visible point spans almost everything, the hint must either
-    stay off or change nothing."""
-    import video_c5
-    from vggsfm_b200 import video
-    res = {}
-    for band in ("0", "1"):
-        os.environ["VGG_BAND"] = band
-        try:
-            video_c5.final_problem(frames=256, new_per_window=128, dev=cuda_dev, reps=1, shuffle=True)
-            res[band] = float(video.last_joint_summary.final_cost)
-        finally:
-            os.environ.pop("VGG_BAND", None)
-    assert abs(res["0"] - res["1"]) <= 1e-9 * abs(res["0"])
+    for shuffle in (False, True):
+        out = video_c5.final_problem(frames=320, new_per_window=128, dev=cuda_dev, reps=1, shuffle=shuffle)
+        res[shuffle] = (out["lm_iterations"][0], float(video.last_joint_summary.final_cost), _band_hint_meta())
+    assert res[False][2] == [True, True, True], res[False]          # in order: banded
+    assert res[True][2] == [False, False, False], res[True]         # shuffled: dense
+    assert res[False][0] > 5 and res[True][0] > 5
+    assert abs(res[False][1] - res[True][1]) <= 1e-9 * abs(res[True][1])

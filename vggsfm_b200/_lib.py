@@ -32,7 +32,7 @@ EXPORTS = [
 
 
 # development probes (csrc/dev_probes.h): exported, not part of the public header
-DEV_EXPORTS = ["vgg_dev_blocks_timing", "vgg_dev_blocks_last_ms", "vgg_dev_chol128_probe", "vgg_dev_syrk_f64", "vgg_dev_syrk_f64_band", "vgg_dev_syrk_ozaki_band", "vgg_dev_trsv_probe", "vgg_dev_cholesky_band",
+DEV_EXPORTS = ["vgg_dev_blocks_timing", "vgg_dev_blocks_last_ms", "vgg_dev_chol128_probe", "vgg_dev_syrk_f64", "vgg_dev_syrk_f64_band", "vgg_dev_trsv_probe", "vgg_dev_cholesky_band",
                "vgg_dev_last_band_hint", "vgg_dev_msac_trace", "vgg_dev_relative_pose_counts",
                "vgg_dev_build_blocks_band", "vgg_dev_schur_build", "vgg_dev_syrk_work_list", "vgg_dev_pcg_probe"]
 
@@ -171,7 +171,6 @@ def lib() -> ctypes.CDLL:
     L.vgg_dev_schur_build.argtypes = [ctypes.POINTER(BAProblem)] + [vp] * 5 + [cd] * 3 + [ci, ci, vp, cs] + [vp] * 8
     L.vgg_dev_syrk_work_list.argtypes = [ci, ci, vp, ci, ci, vp, ci, ctypes.POINTER(ci)]
     L.vgg_syrk_ozaki.argtypes = [ci, ci, vp, vp, ci, vp, cs, vp]
-    L.vgg_dev_syrk_ozaki_band.argtypes = L.vgg_syrk_ozaki.argtypes + [vp, ci]
     L.vgg_cholesky_lower.argtypes = [ci, ci, vp, vp, cs, ctypes.POINTER(ci), vp]
     L.vgg_dev_cholesky_band.argtypes = L.vgg_cholesky_lower.argtypes + [vp, ci, ci]
     L.vgg_tri_workspace_bytes.argtypes = [ci, ci, ci, ci, ctypes.POINTER(cs)]

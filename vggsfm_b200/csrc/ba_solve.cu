@@ -374,13 +374,11 @@ __global__ void effective_const_kernel(int S, int N, int dc, int D, const uint8_
 // the grid is (nearly) dense.  One small kernel + a 8 S byte read-back per solve.  *plan must come in empty (dense).
 static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad, int Kpad, bool multi_rank, cudaStream_t st,
                              BandPlan* plan) {
-  const char* env = getenv("VGG_BAND");                 // read per solve so that a test can compare both paths in one process
-  const bool off = env && env[0] == '0';
   const int S = prob->S, N = prob->N, nb = Dpad / 128, KB = (Kpad + 63) / 64;
   plan->nb = nb;
   plan->KB = KB;
   plan->ngroups = (S + 31) / 32;
-  if (off || nb < 6 || N < 1024) return VGG_OK;
+  if (nb < 6 || N < 1024) return VGG_OK;
   static thread_local int* dev = nullptr;
   static thread_local int cap = 0;
   if (cap < 2 * S) {

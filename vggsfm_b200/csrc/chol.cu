@@ -5,8 +5,8 @@
 //   chol_panel_kernel   EVERY CTA re-factors the 128x128 diagonal block in shared memory (cta_chol128 below) with its
 //                       own xr panel rows riding along, so no CTA waits for another one and the rows come out solved;
 //                       it writes them back together with their transpose (the upper triangle ends up holding L^T,
-//                       which is what the backward substitution kernel, csrc/trsv.cu, streams row by row), then --
-//                       fused schedule -- waits for the CTAs that own block row k+1, loads those 128 rows and applies
+//                       which is what the backward substitution kernel, csrc/trsv.cu, streams row by row), then
+//                       waits for the CTAs that own block row k+1, loads those 128 rows and applies
 //                       this panel's update to its own rows of block column k+1 with DMMA + f64 REDs.  The next panel
 //                       kernel follows on the same stream.  Each CTA needs a whole SM's worth of shared memory, so xr
 //                       (16, 20, ... 32 rows) is chosen per panel such that the 1 + chunks CTAs fit on the device's SMs
@@ -17,7 +17,7 @@
 //                       CTAs are: those go first (graph node priorities) onto whichever SMs free up.
 // Every MMA is mma.sync.m16n8k16.f64 (dmma_m16n8k16, full FP64 tensor rate on sm_90; m8n8k4 runs at half of it).
 // The whole launch sequence is captured once per (matrix, order) into a CUDA graph.  Matrices of fewer than three blocks
-// are factored in program order (no fused update, no side streams), launched directly.
+// have no trailing update beyond the fused one (panel kernels on one stream only) and are launched directly.
 #include <algorithm>
 #include <map>
 #include <vector>
@@ -417,7 +417,7 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol128_probe_kernel(const doubl
 // the other CTAs of this launch may still be loading the unfactored block; CTA 0 of the NEXT panel's launch moves it
 // into place (the last panel, a single CTA, writes its block directly).
 //
-// fuse != 0: the CTA then applies THIS panel's update to its own rows of the NEXT block column,
+// The CTA then applies THIS panel's update to its own rows of the NEXT block column,
 //   A[r0.., t0..t0+127] -= X P^T,   X = its solved rows,  P = L[t0..t0+127][k0..k0+127]  (block row k+1 of the panel),
 // so that column is complete when the kernel ends and the next panel kernel can follow directly (r02: the separate
 // critical-path update kernel and its two cross-stream graph edges cost ~12 us per panel step on top of the ~9 us the
@@ -431,7 +431,7 @@ constexpr int CHOL_INFO_STALLED = 0x7fffffff;
 __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda, int k0, double* __restrict__ A,
                                                                    double* __restrict__ Ldiag /*[nblk][128*128]*/,
                                                                    int* __restrict__ info, int* __restrict__ flags,
-                                                                   int fuse, int band_end, int arrow_lo, int xr) {
+                                                                   int band_end, int arrow_lo, int xr) {
   // Rows below the diagonal block that can be non-zero in this block column: [k0+128, band_end) and [arrow_lo, n)
   // (band_end = arrow_lo = n: everything, the dense case).  The CTAs cover exactly these rows, xr each; a chunk ends
   // early at the end of its range (nrows < xr), its remaining rows are zero.
@@ -518,12 +518,12 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
     const int c = e / nrows, r = e - c * nrows;
     if (c < nb) A[(size_t)(k0 + c) * lda + r0 + r] = Ts[r * CLD + c];
   }
-  if (!fuse) return;
 
   // ---- fused update of block column k+1 with this panel
   const int t0 = k0 + CB;
   // CTAs 1..nprod own block row k+1 (the band's first block, or the arrow block when it is the next one); a block
-  // row that is structurally zero in this column has no producers and there is nothing to subtract
+  // row that is structurally zero in this column has no producers and there is nothing to subtract, and the last
+  // panel has no CTA below its diagonal block
   const bool p_active = band_end > t0 || arrow_lo == t0;
   const int nprod = p_active ? min((CB + xr - 1) / xr, (int)gridDim.x - 1) : 0;
   if (nprod == 0) return;
@@ -611,11 +611,9 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
 }
 
 // A[t0.., t0..] -= P P^T (lower part), P = A[t0.., k0..k0+127]: 64 x 64 tiles (bi, bj), bj <= bi, tile t of the mode's
-// list for t = blockIdx.x, blockIdx.x + gridDim.x, ... < ntiles (the fused schedule caps the grid at what the SMs
-// hold at once and lets each CTA walk several tiles, see chol_enqueue); 8 warps 2 x 4, warp tile 32 x 16 = two m16 x
-// two n8 DMMA tiles.
-// Which tiles (tile columns counted from t0):
-//   CU_ALL   every tile (the program-order schedule of matrices with fewer than three blocks)
+// list for t = blockIdx.x, blockIdx.x + gridDim.x, ... < ntiles (the grid is capped at what the SMs hold at once and
+// each CTA walks several tiles, see chol_enqueue); 8 warps 2 x 4, warp tile 32 x 16 = two m16 x two n8 DMMA tiles.
+// Which tiles (tile columns counted from t0; columns 0 and 1 are the fused update of the panel kernel):
 //   CU_NEXT  tile columns 2 and 3 = block column k+2, which the fused panel kernel of the next step is adding into at
 //            the same time: f64 REDs
 //   CU_REST  tile columns >= 4 (REDs on 4 and 5: block column k+3 is shared with CU_NEXT of the next step)
@@ -626,7 +624,7 @@ __global__ void __launch_bounds__(C_THREADS, 1) chol_panel_kernel(int n, int lda
 // previous version (whole K resident, one CTA per SM): the panel kernel's latency-bound CTAs held their SMs for the
 // whole step and the trailing update ran after them, not beside them -- the factorisation took the SUM of all its kernels.
 constexpr int CUD = 68;
-enum { CU_ALL = 0, CU_NEXT = 1, CU_REST = 2 };
+enum { CU_NEXT, CU_REST };
 __global__ void __launch_bounds__(C_THREADS, 2) chol_update_kernel(int n, int lda, int k0, int t0, int mode, int ntiles,
                                                                     double* __restrict__ A, int band_end, int arrow_lo,
                                                                     int all_red) {
@@ -652,9 +650,8 @@ __global__ void __launch_bounds__(C_THREADS, 2) chol_update_kernel(int n, int ld
       while ((bi + 1) * (bi + 2) / 2 <= t) ++bi;
       while (bi * (bi + 1) / 2 > t) --bi;
       bj = t - bi * (bi + 1) / 2;
-      const int skip = mode == CU_REST ? 4 : 0;
-      bi += skip;
-      bj += skip;
+      bi += 4;
+      bj += 4;
     }
     const bool diag = bi == bj;
     const int ri = vrow(bi), rj = vrow(bj);
@@ -705,7 +702,7 @@ __global__ void __launch_bounds__(C_THREADS, 2) chol_update_kernel(int n, int ld
           for (int j = 0; j < 2; ++j) dmma_m16n8k16(c[i][j], a[i], b[j]);
       }
     }
-    const bool red = all_red || mode == CU_NEXT || (mode == CU_REST && bj < 6);
+    const bool red = all_red || bj < 6;              // CU_NEXT's tile columns 2, 3 and CU_REST's first block column
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
 #pragma unroll
@@ -834,17 +831,15 @@ int chol_panel_rows(int below1, int below2, int* chunks) {
   }
 }
 
-// The launch sequence on st (+ the side streams).
-//   lookahead (three or more blocks): step(b) = panel b + its fused update of block column b+1, on st back to back; the
-//     rest of panel b's trailing update runs on the side streams behind step(b): U1(b) = block column b+2 (CU_NEXT,
-//     needed by step(b+2)) and U2(b) = block columns >= b+3 (CU_REST, needed by step(b+3)).
-//   lookahead == false: everything on st in program order (one CU_ALL update per panel, no fused update).
+// The launch sequence on st (+ the side streams): step(b) = panel b + its fused update of block column b+1, on st back
+// to back; the rest of panel b's trailing update runs on the side streams behind step(b): U1(b) = block column b+2
+// (CU_NEXT, needed by step(b+2)) and U2(b) = block columns >= b+3 (CU_REST, needed by step(b+3)).  A matrix of fewer
+// than three blocks has neither: its panel kernels alone run, on st.
 int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags, const std::vector<int>& end_blk,
-                 int arrow_blk, cudaStream_t st, CholStreams* cs, bool lookahead) {
+                 int arrow_blk, cudaStream_t st, CholStreams* cs) {
   const int nblk = (n + CB - 1) / CB;
   const size_t smem_u = sizeof(double) * 2 * CT * CUD;
-  // the band structure is honoured by the lookahead schedule only; the program-order schedule treats the matrix as dense
-  const bool banded = lookahead && (int)end_blk.size() >= nblk && arrow_blk > 0;
+  const bool banded = (int)end_blk.size() >= nblk && arrow_blk > 0;
   auto band_rows = [&](int b, int* band_end, int* arrow_lo) {
     if (!banded) {
       *band_end = *arrow_lo = n;
@@ -862,28 +857,14 @@ int chol_enqueue(int n, int lda, double* A, double* Ldiag, int* info, int* flags
     const int below2 = band_end >= n ? 0 : n - arrow_lo;
     const int xr = chol_panel_rows(below1, below2, &chunks);
     const size_t smem_p = sizeof(double) * (CB + xr) * CLD;
-    if (lookahead) {
-      VGG_CUDA_CHECK(chol_launch(chol_panel_kernel, 1 + chunks, smem_p, st, cs->prio[CR_PANEL], n, lda, k0, A, Ldiag, info,
-                                 flags, 1, band_end, arrow_lo, xr));
-      ++cs->launched[CR_PANEL];
-    } else {
-      chol_panel_kernel<<<1 + chunks, C_THREADS, smem_p, st>>>(n, lda, k0, A, Ldiag, info, flags, 0, band_end, arrow_lo, xr);
-    }
+    VGG_CUDA_CHECK(chol_launch(chol_panel_kernel, 1 + chunks, smem_p, st, cs->prio[CR_PANEL], n, lda, k0, A, Ldiag, info,
+                               flags, band_end, arrow_lo, xr));
+    ++cs->launched[CR_PANEL];
     VGG_LAUNCH_CHECK();
     return VGG_OK;
   };
   int rc;
   if ((rc = panel(0))) return rc;
-  if (!lookahead) {
-    for (int b = 0; b + 1 < nblk; ++b) {
-      const int k0 = b * CB, t0 = k0 + CB;
-      const int T = (n - t0 + CT - 1) / CT;
-      chol_update_kernel<<<T * (T + 1) / 2, C_THREADS, smem_u, st>>>(n, lda, k0, t0, CU_ALL, T * (T + 1) / 2, A, n, n, 0);
-      VGG_LAUNCH_CHECK();
-      if ((rc = panel(b + 1))) return rc;
-    }
-    return VGG_OK;
-  }
   // U1 gets one step of slack at medium priority, U2 two steps at the lowest.  r02: as ONE kernel with one step of
   // slack the update of the first six panels did not fit next to the following step and 0.15 ms of it showed up on the
   // critical path.
@@ -994,7 +975,9 @@ int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, cons
   const int nblk = (n + CB - 1) / CB;
   CholStreams* cs = nullptr;
   if ((rc = chol_streams(&cs))) return rc;
-  if (nblk < 3) return chol_enqueue(n, lda, A, Ldiag, info, flags, end_blk, arrow_blk, st, cs, false);
+  // below three blocks the sequence is one or two panel kernels on st: no graph to capture.  Outside a graph the
+  // launches' priority attribute only ranks them against other streams' queued work.
+  if (nblk < 3) return chol_enqueue(n, lda, A, Ldiag, info, flags, end_blk, arrow_blk, st, cs);
   // one captured graph per (matrix, order): ~60 launches + events become a single cudaGraphLaunch
   typedef std::tuple<double*, int, int, int*, double*, unsigned long long> Key;
   static thread_local std::map<Key, cudaGraphExec_t> cache;
@@ -1007,7 +990,7 @@ int chol_lower_inplace(int n, int lda, double* A, double* Ldiag, int* info, cons
     cudaGraph_t graph = nullptr;
     cs->launched[CR_PANEL] = cs->launched[CR_NEXT] = cs->launched[CR_REST] = 0;
     VGG_CUDA_CHECK(cudaStreamBeginCapture(cs->cap, cudaStreamCaptureModeThreadLocal));
-    rc = chol_enqueue(n, lda, A, Ldiag, info, flags, end_blk, arrow_blk, cs->cap, cs, true);
+    rc = chol_enqueue(n, lda, A, Ldiag, info, flags, end_blk, arrow_blk, cs->cap, cs);
     const cudaError_t ce = cudaStreamEndCapture(cs->cap, &graph);
     g_launch_count = launches_before;
     if (rc) {

@@ -22,9 +22,6 @@ int vgg_dev_syrk_f64(int Kpad, int Dpad, const double* Zt, double* Cmat, void* s
  * NULL, 0 = dense). */
 int vgg_dev_syrk_f64_band(int Kpad, int Dpad, const double* Zt, double* Cmat, void* stream, const int* ranges_host,
                           int count);
-/* vgg_syrk_ozaki (csrc/syrk_i8.cu) with the band hint of vgg_dev_syrk_f64_band. */
-int vgg_dev_syrk_ozaki_band(int Kpad, int Dpad, const double* Zt, double* Cmat, int slices, void* workspace,
-                            size_t ws_bytes, void* stream, const int* ranges_host, int count);
 /* Backward substitution U x = y (csrc/trsv.cu).  A_dev: row-major upper triangle, lda columns (the strictly lower
  * triangle is never read); y_dev[i * y_stride] = y_i.  stamps_host == NULL: the launcher of the LM loop (sentinel fill +
  * kernel), then a device synchronise.  Otherwise the kernel alone with per-block-row timestamps (ns, 6 per block row of

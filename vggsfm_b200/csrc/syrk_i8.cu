@@ -21,7 +21,6 @@
 //                  FP64, scale by 2^(e_i+e_j) and RED into the lower triangle.
 // Work items (tile, order group, k range) are built on the host, longest first, and strided over the CTAs.
 #include "common.cuh"
-#include "dev_probes.h"
 #include "syrk_work.h"
 
 #include <algorithm>
@@ -90,12 +89,8 @@ __global__ void __launch_bounds__(512) oz_slice_kernel(int Kpad, int Dpad, int K
                                                        const double* __restrict__ Zt,
                                                        const unsigned long long* __restrict__ amax,
                                                        int* __restrict__ expo, double* __restrict__ pow2,
-                                                       int8_t* __restrict__ slices, size_t slice_stride,
-                                                       const int* __restrict__ kb_range /* [nb][2] or null */) {
+                                                       int8_t* __restrict__ slices, size_t slice_stride) {
   const int rb = blockIdx.x, kb = blockIdx.y;
-  // banded problems (csrc/ba_solve.cu computes the ranges from the visibility mask): outside [lo, hi) this row block of Z
-  // is zero and no work item reads its tile images
-  const bool skip = kb_range && (kb < kb_range[2 * rb] || kb >= kb_range[2 * rb + 1]);
   const int r = (threadIdx.x >> 5) * 8 + ((threadIdx.x & 31) >> 2), cphys = threadIdx.x & 3;
   const int c = cphys ^ ((r >> 1) & 3);
   const int d = rb * OZ_BM + r;
@@ -115,7 +110,6 @@ __global__ void __launch_bounds__(512) oz_slice_kernel(int Kpad, int Dpad, int K
     expo[d] = bad ? OZ_EXPO_BAD : e;
     pow2[d] = bad ? 0.0 : ldexp(1.0, e);
   }
-  if (skip) return;
   const int B = 8 * s - 2;
   const double scale = (bad || zero) ? 0.0 : __longlong_as_double((long long)(1023 + B - e) << 52);   // 2^(B-e), exact
   const unsigned long long bias = 0x0080808080808080ull >> (8 * (7 - s));
@@ -362,9 +356,6 @@ bool build_plan(int s, OzPlan* plan, int max_acc) {
 
 struct OzHostState {
   int Kpad = -1, Dpad = -1, slices = -1, sms = 0;
-  std::vector<int> ranges;        // k-block range per row block the cached work list was built for (empty: dense)
-  int* ranges_dev = nullptr;      // device copy for the slicing kernel
-  size_t ranges_cap = 0;
   OzPlan plan;
   std::vector<OzWork> work;
   OzWork* pinned = nullptr;       // page-locked copy of `work`, so the per-call upload is a true async copy
@@ -392,28 +383,14 @@ size_t oz_workspace_bytes(int Kpad, int Dpad, int s) {
 size_t syrk_i8_workspace_bytes(int Kpad, int Dpad, int slices) { return oz_workspace_bytes(Kpad, Dpad, slices); }
 
 // Sraw -= Zt^T Zt with s int8 slices.  Zt [Kpad][Dpad] (Dpad % 128 == 0), Cmat [Dpad][Dpad] row-major, LOWER triangle
-// written, same contract as launch_syrk.  kb_ranges: [lo, hi) k-block range per 128-column row block of Zt outside which
-// the block is exactly zero; any other size = dense.  Tiles whose two ranges do not intersect are skipped, the others
-// shortened.
-int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, int s, void* ws, size_t ws_bytes,
-                   const std::vector<int>& kb_ranges, cudaStream_t st) {
+// written, same contract as launch_syrk.
+int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, int s, void* ws, size_t ws_bytes, cudaStream_t st) {
   VGG_REQUIRE(Dpad % OZ_BM == 0, "syrk_i8: Dpad must be a multiple of 128");
   VGG_REQUIRE(ws_bytes >= oz_workspace_bytes(Kpad, Dpad, s), "syrk_i8: workspace too small");
   const int KB = (Kpad + OZ_BK - 1) / OZ_BK;
   const int nb = Dpad / OZ_BM;
   OzHostState& hs = g_oz;
-  const bool banded = (int)kb_ranges.size() == 2 * nb;
-  if (hs.Kpad != Kpad || hs.Dpad != Dpad || hs.slices != s || (banded ? hs.ranges != kb_ranges : !hs.ranges.empty())) {
-    hs.ranges = banded ? kb_ranges : std::vector<int>();
-    if (banded) {
-      if (hs.ranges_cap < hs.ranges.size()) {
-        if (hs.ranges_dev) cudaFree(hs.ranges_dev);
-        hs.ranges_cap = hs.ranges.size();
-        VGG_CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&hs.ranges_dev), sizeof(int) * hs.ranges_cap));
-      }
-      VGG_CUDA_CHECK(cudaMemcpyAsync(hs.ranges_dev, hs.ranges.data(), sizeof(int) * hs.ranges.size(), cudaMemcpyHostToDevice, st));
-      VGG_CUDA_CHECK(cudaStreamSynchronize(st));          // the source is pageable host memory; once per (re)plan
-    }
+  if (hs.Kpad != Kpad || hs.Dpad != Dpad || hs.slices != s) {
     VGG_REQUIRE(build_plan(s, &hs.plan, OZ_MAX_ACC), "syrk_i8: slices must be in [3,7]");
     int dev = 0;
     VGG_CUDA_CHECK(cudaGetDevice(&dev));
@@ -425,7 +402,7 @@ int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, int s, vo
       for (int g = 0; g < hs.plan.n_groups; ++g) pairs.push_back(hs.plan.g[g].n_pairs);
       // epilogue_cost: pair-kblock equivalents of one item's epilogue (order combination + REDs); OZ_MAX_ITEM_KB keeps
       // the int32 accumulators exact
-      build_work_list<OzWork>(pairs, syrk_tile_jobs(nb, hs.ranges), KB, hs.sms, OZ_MAX_ITEM_KB, 24,
+      build_work_list<OzWork>(pairs, syrk_tile_jobs(nb, {}), KB, hs.sms, OZ_MAX_ITEM_KB, 24,
                               [](const SyrkTileJob& j, int g, int k0, int k1) { return OzWork{j.bi, j.bj, g, k0, k1}; }, &hs.work);
     }
     if (hs.work.size() > hs.pinned_cap) {
@@ -456,8 +433,7 @@ int launch_syrk_i8(int Kpad, int Dpad, const double* Zt, double* Cmat, int s, vo
     oz_rowmax_kernel<<<dim3(Dpad / 128, ksplit), 128, 0, st>>>(Kpad, Dpad, k_per, Zt, amax);
     VGG_LAUNCH_CHECK();
   }
-  oz_slice_kernel<<<dim3(nb, KB), 512, 0, st>>>(Kpad, Dpad, KB, s, Zt, amax, expo, pow2, slices, slice_stride,
-                                                banded ? hs.ranges_dev : nullptr);
+  oz_slice_kernel<<<dim3(nb, KB), 512, 0, st>>>(Kpad, Dpad, KB, s, Zt, amax, expo, pow2, slices, slice_stride);
   VGG_LAUNCH_CHECK();
   const int grid = std::min(hs.sms, nwork);
   oz_syrk_kernel<<<grid, OZ_THREADS, OZ_SMEM_BYTES, st>>>(hs.plan, work_d, nwork, KB, slices, slice_stride, expo, pow2, Dpad,
@@ -479,17 +455,10 @@ int vgg_syrk_ozaki_workspace_bytes(int Kpad, int Dpad, int slices, size_t* bytes
 
 int vgg_syrk_ozaki(int Kpad, int Dpad, const double* Zt, double* Cmat, int slices, void* workspace, size_t ws_bytes,
                    void* stream) {
-  return vgg_dev_syrk_ozaki_band(Kpad, Dpad, Zt, Cmat, slices, workspace, ws_bytes, stream, nullptr, 0);
-}
-
-/* development probe (csrc/dev_probes.h): vgg_syrk_ozaki with a band hint */
-int vgg_dev_syrk_ozaki_band(int Kpad, int Dpad, const double* Zt, double* Cmat, int slices, void* workspace,
-                            size_t ws_bytes, void* stream, const int* ranges, int count) {
   using namespace vgg;
   g_launch_count = 0;
-  VGG_REQUIRE(Zt && Cmat && workspace && (ranges || count <= 0), "null pointer");
-  return launch_syrk_i8(Kpad, Dpad, Zt, Cmat, slices, workspace, ws_bytes,
-                        std::vector<int>(ranges, ranges + std::max(count, 0)), static_cast<cudaStream_t>(stream));
+  VGG_REQUIRE(Zt && Cmat && workspace, "null pointer");
+  return launch_syrk_i8(Kpad, Dpad, Zt, Cmat, slices, workspace, ws_bytes, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"
