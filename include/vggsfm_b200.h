@@ -47,6 +47,17 @@ int vgg_version(void);
 /* and the tensor<->Reconstruction marshalling around it (tensor_to_pycolmap.py:16-214).        */
 /* ------------------------------------------------------------------------------------------- */
 
+/* Robust loss of every observation (COLMAP's BundleAdjustmentOptions::loss_function_type, Ceres' TrivialLoss, SoftLOneLoss
+ * and CauchyLoss at loss_function_scale a).  With s = |r|^2 and b = a^2, an observation costs rho(s) / 2:
+ *   TRIVIAL  rho = s
+ *   SOFT_L1  rho = 2 b (sqrt(1 + s / b) - 1)
+ *   CAUCHY   rho = b log(1 + s / b)
+ * and, as Ceres' Corrector does for these losses (rho'' <= 0), its residual and Jacobian enter the normal equations
+ * scaled by sqrt(rho'(s)), rho' clamped below at DBL_MIN. */
+#define VGG_LOSS_TRIVIAL 0
+#define VGG_LOSS_SOFT_L1 1
+#define VGG_LOSS_CAUCHY 2
+
 typedef struct vgg_ba_problem {
   int32_t S, N;
   int32_t camera_model;        /* VGG_SIMPLE_* */
@@ -58,6 +69,11 @@ typedef struct vgg_ba_problem {
   double* poses;               /* [S,12] in/out */
   double* intr;                /* [S,4]  in/out */
   double* points;              /* [N,3]  in/out */
+  /* VGG_LOSS_* (0 = TRIVIAL, so a zero-initialised problem has the trivial loss) and its scale a in pixels: finite and
+   * > 0 for a robust loss, ignored for TRIVIAL.  Every BA entry point taking the problem returns VGG_EINVAL before any
+   * launch for another type or scale. */
+  int32_t loss_function_type;
+  double loss_function_scale;
 } vgg_ba_problem;
 
 /* Ceres solver options as COLMAP's BundleAdjustmentOptions sets them (triangulation_helpers.py:626-635). */

@@ -44,6 +44,7 @@ class BAProblem(ctypes.Structure):
         ("uv", ctypes.c_void_p), ("mask", ctypes.c_void_p),
         ("param_const", ctypes.c_void_p), ("point_const", ctypes.c_void_p),
         ("poses", ctypes.c_void_p), ("intr", ctypes.c_void_p), ("points", ctypes.c_void_p),
+        ("loss_function_type", ctypes.c_int32), ("loss_function_scale", ctypes.c_double),
     ]
 
 

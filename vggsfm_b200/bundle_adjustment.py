@@ -26,6 +26,8 @@ INTR_PER_FRAME = 1
 INTR_SHARED = 2
 
 LINEAR_SOLVER_TYPES = {"DENSE_SCHUR": 0, "ITERATIVE_SCHUR": 1}
+# COLMAP's BundleAdjustmentOptions::LossFunctionType (VGG_LOSS_* of include/vggsfm_b200.h)
+LOSS_FUNCTION_TYPES = {"TRIVIAL": 0, "SOFT_L1": 1, "CAUCHY": 2}
 CG_TERMINATION = {0: "SUCCESS", 1: "NO_CONVERGENCE", 2: "FAILURE"}
 
 TERMINATION = {0: "NO_CONVERGENCE", 1: "CONVERGENCE_GRADIENT", 2: "CONVERGENCE_FUNCTION",
@@ -126,7 +128,15 @@ def workspace(S: int, N: int, model: int, mode: int, device, iterative: bool = F
     return ws
 
 
-def _problem(uv, mask, poses, intr, points, model, mode, param_const, point_const):
+def loss_function_id(loss_function_type: str) -> int:
+    """VGG_LOSS_* of one of COLMAP's loss names: TRIVIAL, SOFT_L1 or CAUCHY."""
+    if loss_function_type not in LOSS_FUNCTION_TYPES:
+        raise ValueError(f"loss_function_type must be one of {sorted(LOSS_FUNCTION_TYPES)}, not {loss_function_type!r}")
+    return LOSS_FUNCTION_TYPES[loss_function_type]
+
+
+def _problem(uv, mask, poses, intr, points, model, mode, param_const, point_const, loss_function_type="TRIVIAL",
+             loss_function_scale=1.0):
     S, N = mask.shape
     assert uv.dtype == torch.float32 and uv.is_contiguous() and uv.shape == (S, N, 2)
     assert mask.dtype == torch.uint8 and mask.is_contiguous()
@@ -139,14 +149,18 @@ def _problem(uv, mask, poses, intr, points, model, mode, param_const, point_cons
     p.param_const = param_const.data_ptr() if param_const is not None else None
     p.point_const = point_const.data_ptr() if point_const is not None else None
     p.poses, p.intr, p.points = poses.data_ptr(), intr.data_ptr(), points.data_ptr()
+    p.loss_function_type = loss_function_id(loss_function_type)
+    p.loss_function_scale = float(loss_function_scale)
     return p
 
 
-def build_blocks(uv, mask, poses, intr, points, model, mode, point_const=None, tracks_per_warp=0):
+def build_blocks(uv, mask, poses, intr, points, model, mode, point_const=None, tracks_per_warp=0,
+                 loss_function_type="TRIVIAL", loss_function_scale=1.0):
     """One launch of the fused residual+Jacobian+block kernel (vgg_ba_build_blocks).  Returns a dict of
     device tensors: cost[1], camrec[S,KR], g_p[N,3], H_pp[N,6], W[N,pitch,3] (track-major, pitch = D rounded
     up to even), shared[8].  ``tracks_per_warp``: 0 lets the library choose; otherwise a positive multiple of 4
-    (the kernel loads the observations of 4 tracks at a time), anything else raises."""
+    (the kernel loads the observations of 4 tracks at a time), anything else raises.  With a robust loss the blocks
+    are those of the corrected residuals and Jacobians and the cost is 0.5 sum rho (as lm_solve)."""
     L = _lib.lib()
     S, N = mask.shape
     dc, ns = dims(model, mode)
@@ -169,7 +183,7 @@ def build_blocks(uv, mask, poses, intr, points, model, mode, point_const=None, t
         "W": torch.empty(N, (S * dc + ns + 1) // 2 * 2, 3, dtype=torch.float64, device=dev),
         "shared": view("shared", (8,)),
     }
-    p = _problem(uv, mask, poses, intr, points, model, mode, None, point_const)
+    p = _problem(uv, mask, poses, intr, points, model, mode, None, point_const, loss_function_type, loss_function_scale)
     with torch.cuda.device(dev):
         st = torch.cuda.current_stream().cuda_stream
         _lib.check(L.vgg_ba_build_blocks(ctypes.byref(p), out["cost"].data_ptr(), out["camrec"].data_ptr(),
@@ -179,9 +193,10 @@ def build_blocks(uv, mask, poses, intr, points, model, mode, point_const=None, t
 
 
 def schur(uv, mask, poses, intr, points, model, mode, blocks, scale_p, radius, min_diag=1e-6, max_diag=1e32,
-          point_const=None):
+          point_const=None, loss_function_type="TRIVIAL", loss_function_scale=1.0):
     """Schur complement of `blocks` (vgg_ba_schur; the coupling blocks are rebuilt from the observations and the
-    state, so blocks["W"] is not read).  Returns (Sraw[D,Dpad] lower-valid, rhs[D])."""
+    state, so blocks["W"] is not read; pass the loss `blocks` were built with).  Returns (Sraw[D,Dpad] lower-valid,
+    rhs[D])."""
     L = _lib.lib()
     S, N = mask.shape
     dc, ns = dims(model, mode)
@@ -191,7 +206,7 @@ def schur(uv, mask, poses, intr, points, model, mode, blocks, scale_p, radius, m
     ws = workspace(S, N, model, mode, dev)
     Sraw = torch.empty(D, Dpad, dtype=torch.float64, device=dev)
     rhs = torch.empty(Dpad, dtype=torch.float64, device=dev)
-    p = _problem(uv, mask, poses, intr, points, model, mode, None, point_const)
+    p = _problem(uv, mask, poses, intr, points, model, mode, None, point_const, loss_function_type, loss_function_scale)
     dpad = ctypes.c_int()
     with torch.cuda.device(dev):
         st = torch.cuda.current_stream().cuda_stream
@@ -223,13 +238,18 @@ class Summary:
 
 def lm_solve(uv, mask, poses, intr, points, model, mode, param_const=None, point_const=None,
              options: Optional[BAOptions] = None, allreduce=None, want_trace=False, linear_solver_type="DENSE_SCHUR",
-             min_linear_solver_iterations=0, max_linear_solver_iterations=500, eta=0.1) -> Summary:
+             min_linear_solver_iterations=0, max_linear_solver_iterations=500, eta=0.1, loss_function_type="TRIVIAL",
+             loss_function_scale=1.0) -> Summary:
     """In-place Levenberg-Marquardt on device tensors (vgg_ba_solve).  `allreduce` is a
     vggsfm_b200.dist.AllReduceHook for track-sharded multi-GPU runs.  A rank whose shard holds no track (N = 0:
     shard_range gives empty tail shards when the tracks are few) still takes part in every reduction: it solves 16
     masked-out padding tracks, as bundle_adjustment() pads, and leaves its empty `points` untouched.
     linear_solver_type="ITERATIVE_SCHUR" solves each step by PCG (vgg_ba_solve_iterative) with the three CG options;
-    it runs on one GPU only, so it raises ValueError together with `allreduce`."""
+    it runs on one GPU only, so it raises ValueError together with `allreduce`.
+    loss_function_type / loss_function_scale: COLMAP's BundleAdjustmentOptions loss (TRIVIAL, SOFT_L1 or CAUCHY at a
+    scale in pixels) on every observation; the costs of the summary are then 0.5 sum rho(|r|^2).  An unknown name raises
+    ValueError, a robust loss with a scale that is not finite and > 0 raises from the library before anything runs."""
+    loss_function_id(loss_function_type)
     lin = linear_solver(linear_solver_type, min_linear_solver_iterations, max_linear_solver_iterations, eta)
     iterative = linear_solver_type == "ITERATIVE_SCHUR"
     if iterative and allreduce is not None:
@@ -249,7 +269,8 @@ def lm_solve(uv, mask, poses, intr, points, model, mode, param_const=None, point
         N = n
     opt = options or default_options()
     ws = workspace(S, N, model, mode, dev, iterative=True) if iterative else workspace(S, N, model, mode, dev)
-    p = _problem(uv, mask, poses, intr, points, model, mode, param_const, point_const)
+    p = _problem(uv, mask, poses, intr, points, model, mode, param_const, point_const, loss_function_type,
+                 loss_function_scale)
     summ = BASummary()
     trace = torch.zeros(max(1, opt.max_num_iterations), 8, dtype=torch.float64) if want_trace else None
     cg_trace = torch.zeros(max(1, opt.max_num_iterations), 4, dtype=torch.float64) if iterative else None
@@ -330,15 +351,17 @@ def bundle_adjustment(points3d, extrinsics, intrinsics, extra_params, tracks, ma
                       allreduce=None, want_trace=False, refine_focal_length=True, refine_extra_params=True,
                       const_pose=None, const_points=None, gauge=True, do_normalize=True, filter_reconstruction=True,
                       drop_negative_depth=True, linear_solver_type="DENSE_SCHUR", min_linear_solver_iterations=0,
-                      max_linear_solver_iterations=500, eta=0.1):
+                      max_linear_solver_iterations=500, eta=0.1, loss_function_type="TRIVIAL", loss_function_scale=1.0):
     """Tensor-in / tensor-out equivalent of batch_matrix_to_pycolmap + pycolmap.bundle_adjustment +
     filter_reconstruction + pycolmap_to_batch_matrix (triangulation.py:1033-1063).
 
     points3d [P,3], extrinsics [S,3,4], intrinsics [S,3,3], extra_params [S,1]|None, tracks [S,P,2],
     masks [S,P] bool -- CUDA tensors.  Returns (points3D [P',3] f64, extrinsics [S,3,4] f64,
     intrinsics [S,3,3] f64, extra_params [S,1]|None, valid_idx [P'], Summary).  linear_solver_type and the CG options
-    as lm_solve (ITERATIVE_SCHUR with `allreduce` raises ValueError before anything runs)."""
+    as lm_solve (ITERATIVE_SCHUR with `allreduce` raises ValueError before anything runs), and so are
+    loss_function_type and loss_function_scale (COLMAP's BundleAdjustmentOptions defaults: TRIVIAL, 1.0)."""
     model = camera_model_id(camera_type)
+    loss_function_id(loss_function_type)
     lin_kw = dict(linear_solver_type=linear_solver_type, min_linear_solver_iterations=min_linear_solver_iterations,
                   max_linear_solver_iterations=max_linear_solver_iterations, eta=eta)
     linear_solver(**lin_kw)
@@ -387,7 +410,8 @@ def bundle_adjustment(points3d, extrinsics, intrinsics, extra_params, tracks, ma
     pc = torch.ones(Pp, dtype=torch.uint8, device=dev)
     pc[:P] = point_const.to(torch.uint8)
     param_const = default_param_const(S, model, mode, dev, refine_focal_length, refine_extra_params, gauge, const_pose)
-    summary = lm_solve(uv, mk, poses, intr, X, model, mode, param_const, pc, options, allreduce, want_trace, **lin_kw)
+    summary = lm_solve(uv, mk, poses, intr, X, model, mode, param_const, pc, options, allreduce, want_trace, **lin_kw,
+                       loss_function_type=loss_function_type, loss_function_scale=loss_function_scale)
     pts = X[:P]
     if do_normalize:
         poses, pts = normalize(poses, pts, 10.0, 0.1, 0.9, alive)   # BundleAdjustmentController::Run

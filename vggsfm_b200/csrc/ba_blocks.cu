@@ -121,13 +121,13 @@ __host__ __device__ inline size_t w_pitch(int D) { return (size_t)(D + (D & 1));
 // (WRITE_W = false) stores no W -- z_build and backsub rebuild each block from its observation (ba_obs.h) -- which
 // drops the staging buffers and the 24-double block from the live registers: it runs at BLK_NOW_CTAS CTAs per SM.
 constexpr int BLK_NOW_CTAS = 2;
-template <int MODEL, int MODE, bool WRITE_W, bool USE_TMA>
+template <int MODEL, int MODE, bool WRITE_W, bool USE_TMA, bool ROBUST>
 __global__ void __launch_bounds__(BT, WRITE_W ? (USE_TMA ? 2 : 3) : BLK_NOW_CTAS) ba_blocks_kernel(
     int S, int N, int tracks_per_warp, const float* __restrict__ uv, const uint8_t* __restrict__ mask,
     const double* __restrict__ poses, const double* __restrict__ intr, const double* __restrict__ points,
     const uint8_t* __restrict__ point_const, double* __restrict__ cost, double* __restrict__ camrec,
     double* __restrict__ g_p, double* __restrict__ H_pp, double* __restrict__ W, double* __restrict__ shared_out,
-    const int* __restrict__ fg_tracks) {
+    const int* __restrict__ fg_tracks, BaLoss loss) {
   using C = BlkCfg<MODEL, MODE>;
   constexpr int DC = C::DC, NS = C::NS, KR = C::KR;
   constexpr int NP = WRITE_W ? 9 + 3 * NS : 9;     // per-point reduced values: g_p 3, H_pp 6, W_s 3*NS
@@ -235,23 +235,26 @@ __global__ void __launch_bounds__(BT, WRITE_W ? (USE_TMA ? 2 : 3) : BLK_NOW_CTAS
       if (nA >= t_end) break;                                    // warp-uniform
       const bool hasB = nA + 1 < t_end;
       // ---- math for both tracks, registers only (overlaps the previous step's TMA read-out)
-      double jcA0[8], jcA1[8], jxA0[3], jxA1[3], rxA, ryA;
-      double jcB0[8], jcB1[8], jxB0[3], jxB1[3], rxB, ryB;
+      double jcA0[8], jcA1[8], jxA0[3], jxA1[3], rxA, ryA, cA;
+      double jcB0[8], jcB1[8], jxB0[3], jxB1[3], rxB, ryB, cB;
       {
         const float ox = k == 0 ? ca.x : cb.x, oy = k == 0 ? ca.y : cb.y;
         const bool valid = frame_ok && ((cm >> (8 * k)) & 0xffu) != 0;
         const double* xt = xw + ((nA - t_begin) & (XT - 1)) * 4;
         const double2 xa = *reinterpret_cast<const double2*>(xt), xb = *reinterpret_cast<const double2*>(xt + 2);
-        obs_math<MODEL>(pw + lane, 32, xa.x, xa.y, xb.x, xb.y != 0.0, ox, oy, valid, jcA0, jcA1, jxA0, jxA1, rxA, ryA);
+        obs_math<MODEL, ROBUST>(pw + lane, 32, xa.x, xa.y, xb.x, xb.y != 0.0, ox, oy, valid, jcA0, jcA1, jxA0, jxA1, rxA, ryA,
+                               loss, cA);
       }
       {
         const float ox = k == 0 ? ca.z : cb.z, oy = k == 0 ? ca.w : cb.w;
         const bool valid = hasB && frame_ok && ((cm >> (8 * (k + 1))) & 0xffu) != 0;
         const double* xt = xw + ((nA + 1 - t_begin) & (XT - 1)) * 4;
         const double2 xa = *reinterpret_cast<const double2*>(xt), xb = *reinterpret_cast<const double2*>(xt + 2);
-        obs_math<MODEL>(pw + lane, 32, xa.x, xa.y, xb.x, xb.y != 0.0, ox, oy, valid, jcB0, jcB1, jxB0, jxB1, rxB, ryB);
+        obs_math<MODEL, ROBUST>(pw + lane, 32, xa.x, xa.y, xb.x, xb.y != 0.0, ox, oy, valid, jcB0, jcB1, jxB0, jxB1, rxB, ryB,
+                               loss, cB);
       }
-      cost_acc += 0.5 * (rxA * rxA + ryA * ryA) + 0.5 * (rxB * rxB + ryB * ryB);
+      if constexpr (ROBUST) cost_acc += cA + cB;                   // 0.5 rho of each observation
+      else cost_acc += 0.5 * (rxA * rxA + ryA * ryA) + 0.5 * (rxB * rxB + ryB * ryB);
       // ---- both staging buffers must have been read out by the previous step's bulk stores
       if (WRITE_W && USE_TMA) {
         if (lane == 0) tma_store_wait_read<0>();
@@ -332,7 +335,7 @@ __global__ void __launch_bounds__(BT, WRITE_W ? (USE_TMA ? 2 : 3) : BLK_NOW_CTAS
   }
 }
 
-template <int MODEL, int MODE>
+template <int MODEL, int MODE, bool ROBUST>
 static int launch_blocks(const vgg_ba_problem* p, double* cost, double* camrec, double* g_p, double* H_pp,
                          double* W, double* shared_out, int tracks_per_warp, const int* fg_tracks, cudaStream_t stream,
                          bool outputs_zeroed) {
@@ -346,9 +349,9 @@ static int launch_blocks(const vgg_ba_problem* p, double* cost, double* camrec, 
                       sizeof(float) * BW * 2 * 32 * 12;
   const bool tma_ok = ((reinterpret_cast<uintptr_t>(W) & 15) == 0);
   const int ngroups = (S + 31) / 32;
-  const auto kern = !write_w ? ba_blocks_kernel<MODEL, MODE, false, false>
-                    : tma_ok ? ba_blocks_kernel<MODEL, MODE, true, true>
-                             : ba_blocks_kernel<MODEL, MODE, true, false>;
+  const auto kern = !write_w ? ba_blocks_kernel<MODEL, MODE, false, false, ROBUST>
+                    : tma_ok ? ba_blocks_kernel<MODEL, MODE, true, true, ROBUST>
+                             : ba_blocks_kernel<MODEL, MODE, true, false, ROBUST>;
   if (tracks_per_warp <= 0 && fg_tracks) {
     // banded (sequential) problems: most (frame group, track chunk) warps return at once, so the chunks must be small
     // enough for the few that do not to spread over the machine (r02 launch list at 1000 frames x 32 k points: with the
@@ -368,7 +371,7 @@ static int launch_blocks(const vgg_ba_problem* p, double* cost, double* camrec, 
       cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
       // the occupancy query needs the opt-in shared-memory limit in place (r02: without it the query returned 0, the
       // grid was sized for ONE CTA per SM and the 400 x 4096 launch ran as a single wave of 147 CTAs, half the warps)
-      const auto qk = write_w ? ba_blocks_kernel<MODEL, MODE, true, true> : kern;
+      const auto qk = write_w ? ba_blocks_kernel<MODEL, MODE, true, true, ROBUST> : kern;
       cudaFuncSetAttribute(qk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, qk, BT, smem);
       if (per_sm < 1) per_sm = 1;
@@ -416,7 +419,7 @@ static int launch_blocks(const vgg_ba_problem* p, double* cost, double* camrec, 
   if (g_blocks_timing) VGG_CUDA_CHECK(cudaEventRecord(g_blocks_ev[0], stream));
   VGG_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<grid, BT, smem, stream>>>(S, N, tracks_per_warp, p->uv, p->mask, p->poses, p->intr, p->points, p->point_const,
-                                   cost, camrec, g_p, H_pp, W, shared_out, fg_tracks);
+                                   cost, camrec, g_p, H_pp, W, shared_out, fg_tracks, ba_loss_of(p));
   VGG_LAUNCH_CHECK();
   if (g_blocks_timing) VGG_CUDA_CHECK(cudaEventRecord(g_blocks_ev[1], stream));
   return VGG_OK;
@@ -426,14 +429,21 @@ int ba_build_blocks(const vgg_ba_problem* p, double* cost, double* camrec, doubl
                     double* shared_out, int tracks_per_warp, const int* fg_tracks, cudaStream_t stream,
                     bool outputs_zeroed) {
   const int key = p->camera_model * 3 + p->intr_mode;
+  const bool robust = p->loss_function_type != VGG_LOSS_TRIVIAL;
+#define VGG_BLK(M, I)                                                                                                  \
+  return robust ? launch_blocks<M, I, true>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks,     \
+                                            stream, outputs_zeroed)                                                    \
+                : launch_blocks<M, I, false>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks,    \
+                                             stream, outputs_zeroed)
   switch (key) {
-    case 0: return launch_blocks<0, 0>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks, stream, outputs_zeroed);
-    case 1: return launch_blocks<0, 1>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks, stream, outputs_zeroed);
-    case 2: return launch_blocks<0, 2>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks, stream, outputs_zeroed);
-    case 3: return launch_blocks<1, 0>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks, stream, outputs_zeroed);
-    case 4: return launch_blocks<1, 1>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks, stream, outputs_zeroed);
-    case 5: return launch_blocks<1, 2>(p, cost, camrec, g_p, H_pp, W, shared_out, tracks_per_warp, fg_tracks, stream, outputs_zeroed);
+    case 0: VGG_BLK(0, 0);
+    case 1: VGG_BLK(0, 1);
+    case 2: VGG_BLK(0, 2);
+    case 3: VGG_BLK(1, 0);
+    case 4: VGG_BLK(1, 1);
+    case 5: VGG_BLK(1, 2);
   }
+#undef VGG_BLK
   set_error("bad camera_model/intr_mode %d/%d", p->camera_model, p->intr_mode);
   return VGG_EINVAL;
 }

@@ -3,6 +3,7 @@
 // in the solve; the kernels that use it rebuild it from the observation with this one function, so every copy of a
 // block is the same arithmetic.
 #pragma once
+#include <float.h>
 #include "common.cuh"
 
 namespace vgg {
@@ -16,15 +17,29 @@ struct BlkCfg {
   static constexpr int KR = DC + NPACK + 6 * NS;   // per-frame camera record length
 };
 
+// Robust loss of a problem as the kernels take it (vgg_ba_problem.loss_function_type / _scale): SOFT_L1 or CAUCHY, b = a^2,
+// c = 1 / b.  The kernels of the trivial loss are separate instantiations (ROBUST = false) that never read it.
+struct BaLoss {
+  int type;
+  double b, c;
+};
+inline BaLoss ba_loss_of(const vgg_ba_problem* p) {
+  const double a = p->loss_function_scale;
+  return BaLoss{p->loss_function_type, a * a, 1.0 / (a * a)};
+}
+
 // One observation, branch-free: residual and Jacobian columns.  An invalid observation computes on a safe depth and its
 // outputs are SELECTED to exact zeros, never multiplied by the mask: its uv, its point and its camera are then free to be
 // anything, NaN and inf included (a point or a frame that no valid observation sees is not in the problem, and 0 * NaN
 // would put it back).  jc: delta(3), t(3), f, k; jx: point(3).
 // cam: R (row-major 3x4 with t), f, cx, cy, k at cam[0], cam[cs], ..., cam[15 cs]; pc: the point is held constant.
-template <int MODEL>
+// cost: the observation's term of the cost, rho(s) / 2 with s = rx^2 + ry^2.  ROBUST: Ceres' Corrector for a loss with
+// rho'' <= 0 (SOFT_L1 and CAUCHY everywhere), i.e. residual and Jacobian scaled by sqrt(rho'), so that every block and
+// product built from them below is the robust one.  An invalid observation has s = 0, rho' = 1: still exact zeros.
+template <int MODEL, bool ROBUST>
 __device__ __forceinline__ void obs_math(const double* cam, int cs, double X0, double X1, double X2, bool pc, float ox,
                                          float oy, bool valid, double* jc0, double* jc1, double* jx0, double* jx1,
-                                         double& rx, double& ry) {
+                                         double& rx, double& ry, const BaLoss& loss, double& cost) {
   const double R00 = cam[0 * cs], R01 = cam[1 * cs], R02 = cam[2 * cs], t0_ = cam[3 * cs];
   const double R10 = cam[4 * cs], R11 = cam[5 * cs], R12 = cam[6 * cs], t1_ = cam[7 * cs];
   const double R20 = cam[8 * cs], R21 = cam[9 * cs], R22 = cam[10 * cs], t2_ = cam[11 * cs];
@@ -68,6 +83,38 @@ __device__ __forceinline__ void obs_math(const double* cam, int cs, double X0, d
   jx1[0] = vp ? j10 * R00 + j11 * R10 + j12 * R20 : 0.0;
   jx1[1] = vp ? j10 * R01 + j11 * R11 + j12 * R21 : 0.0;
   jx1[2] = vp ? j10 * R02 + j11 * R12 + j12 * R22 : 0.0;
+  if constexpr (!ROBUST) {
+    cost = 0.5 * (rx * rx + ry * ry);
+  } else {
+    // rho in forms without cancellation (the same functions as Ceres' b log(1 + s c) and 2 b (sqrt(1 + s c) - 1)), so
+    // that a large scale reduces to the trivial loss to rounding; rho' = max(DBL_MIN, 1 / (1 + s c)) resp.
+    // max(DBL_MIN, 1 / sqrt(1 + s c)).  One uniform branch per launch: the loss type is the same for every thread.
+    const double s = rx * rx + ry * ry;
+    const double x = s * loss.c;
+    double rho, rho1;
+    if (loss.type == VGG_LOSS_CAUCHY) {
+      rho = loss.b * log1p(x);
+      rho1 = fmax(DBL_MIN, 1.0 / (1.0 + x));
+    } else {
+      const double t = sqrt(1.0 + x);
+      rho = t < 2.0 ? 2.0 * s / (1.0 + t) : 2.0 * loss.b * (t - 1.0);
+      rho1 = fmax(DBL_MIN, 1.0 / t);
+    }
+    cost = 0.5 * rho;
+    const double k = sqrt(rho1);
+    rx *= k;
+    ry *= k;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      jc0[i] *= k;
+      jc1[i] *= k;
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      jx0[i] *= k;
+      jx1[i] *= k;
+    }
+  }
 }
 
 // one entry of the coupling block W = J_c^T J_p: row i of the camera columns (6 + intrinsics), point column c

@@ -104,12 +104,12 @@ __host__ __device__ __forceinline__ void pcg_block_rows(int b, int S, int dc, in
 // Same CTA shape as z_build (ba_schur.cu): PJ_NT tracks per CTA, warps over the 32-frame groups, one lane per frame; a
 // lane keeps its frame's sums in registers over the CTA's tracks and adds them once.
 constexpr int PJ_NT = 8, PJ_W = 4;
-template <int MODEL, int MODE>
+template <int MODEL, int MODE, bool ROBUST>
 __global__ void __launch_bounds__(PJ_W * 32) pcg_rhs_jacobi_kernel(
     int S, int N, const float* __restrict__ uv, const uint8_t* __restrict__ mask, const double* __restrict__ poses,
     const double* __restrict__ intr, const double* __restrict__ points, const uint8_t* __restrict__ point_const,
     const double* __restrict__ M, const double* __restrict__ q, double* __restrict__ rhs, double* __restrict__ acc,
-    const int* __restrict__ fg_tracks) {
+    const int* __restrict__ fg_tracks, BaLoss loss) {
   using C = BlkCfg<MODEL, MODE>;
   constexpr int DC = C::DC, NS = C::NS;
   constexpr int NI = DC - 6, NIU = NI * (NI + 1) / 2;
@@ -160,8 +160,9 @@ __global__ void __launch_bounds__(PJ_W * 32) pcg_rhs_jacobi_kernel(
       const float2 ob = frame_ok ? uv2[o] : make_float2(0.f, 0.f);
       const double* pt = s_pt[t];
       const double* m = pt + 4;
-      double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry;
-      obs_math<MODEL>(pw + lane, 32, pt[0], pt[1], pt[2], pt[3] != 0.0, ob.x, ob.y, valid, jc0, jc1, jx0, jx1, rx, ry);
+      double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry, oc;
+      obs_math<MODEL, ROBUST>(pw + lane, 32, pt[0], pt[1], pt[2], pt[3] != 0.0, ob.x, ob.y, valid, jc0, jc1, jx0, jx1,
+                              rx, ry, loss, oc);
       double z[DC][3];
 #pragma unroll
       for (int i = 0; i < DC; ++i) {
@@ -435,13 +436,13 @@ __global__ void __launch_bounds__(256) pcg_hcc_kernel(int S, int dc, int ns, int
 // frames in turn.  Pass 1 (as backsub): w_n = sum_s W_sn^T u_s; then t_n = M_n M_n^T w_n; pass 2: the frame's
 // sum over the CTA's tracks of W_sn t_n, one warp reduce-scatter and one f64 RED per (CTA, frame parameter).
 constexpr int PS_W = 16;
-template <int MODEL, int MODE>
+template <int MODEL, int MODE, bool ROBUST>
 __global__ void __launch_bounds__(PS_W * 32) pcg_schur_kernel(
     int S, int N, const float* __restrict__ uv, const uint8_t* __restrict__ mask, const double* __restrict__ poses,
     const double* __restrict__ intr, const double* __restrict__ points, const uint8_t* __restrict__ point_const,
     const double* __restrict__ M, const double* __restrict__ sc, const uint8_t* __restrict__ pconst,
     const double* __restrict__ u, double* __restrict__ q, const int* __restrict__ fg_tracks,
-    const double* __restrict__ cg) {
+    const double* __restrict__ cg, BaLoss loss) {
   if (cg[CG_DONE] != 0.0) return;
   using C = BlkCfg<MODEL, MODE>;
   constexpr int DC = C::DC, NS = C::NS;
@@ -475,8 +476,8 @@ __global__ void __launch_bounds__(PS_W * 32) pcg_schur_kernel(
     __syncwarp();
     if (lane < 16) cam[lane] = lane < 12 ? poses[(size_t)s * 12 + lane] : intr[(size_t)s * 4 + (lane - 12)];
     __syncwarp();
-    double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry;
-    obs_math<MODEL>(cam, 1, X0, X1, X2, pc, ob.x, ob.y, valid, jc0, jc1, jx0, jx1, rx, ry);
+    double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry, oc;
+    obs_math<MODEL, ROBUST>(cam, 1, X0, X1, X2, pc, ob.x, ob.y, valid, jc0, jc1, jx0, jx1, rx, ry, loss, oc);
     const double* d = u + (size_t)s * DC;
 #pragma unroll
     for (int i = 0; i < DC; ++i) {
@@ -532,8 +533,8 @@ __global__ void __launch_bounds__(PS_W * 32) pcg_schur_kernel(
     __syncwarp();
     if (lane < 16) cam[lane] = lane < 12 ? poses[(size_t)s * 12 + lane] : intr[(size_t)s * 4 + (lane - 12)];
     __syncwarp();
-    double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry;
-    obs_math<MODEL>(cam, 1, X0, X1, X2, pc, ob.x, ob.y, valid, jc0, jc1, jx0, jx1, rx, ry);
+    double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry, oc;
+    obs_math<MODEL, ROBUST>(cam, 1, X0, X1, X2, pc, ob.x, ob.y, valid, jc0, jc1, jx0, jx1, rx, ry, loss, oc);
     double a8[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i)
@@ -667,12 +668,12 @@ __global__ void __launch_bounds__(256) pcg_update_kernel(int S, int dc, int ns, 
 // Ceres' model change of a step: -(J d)^T (f + J d / 2) summed over the observations, d = (d_c, d_p) unscaled; d_p is
 // recomputed from M, g_p and wacc with point_step's arithmetic (bit for bit the step the candidate took).  One lane per
 // track, warps over the frames, as backsub.
-template <int MODEL, int MODE>
+template <int MODEL, int MODE, bool ROBUST>
 __global__ void __launch_bounds__(PS_W * 32) pcg_model_change_kernel(
     int S, int N, const float* __restrict__ uv, const uint8_t* __restrict__ mask, const double* __restrict__ poses,
     const double* __restrict__ intr, const double* __restrict__ points, const uint8_t* __restrict__ point_const,
     const double* __restrict__ M, const double* __restrict__ g_p, const double* __restrict__ wacc,
-    const double* __restrict__ d_c, const int* __restrict__ fg_tracks, double* __restrict__ out) {
+    const double* __restrict__ d_c, const int* __restrict__ fg_tracks, double* __restrict__ out, BaLoss loss) {
   using C = BlkCfg<MODEL, MODE>;
   constexpr int DC = C::DC, NS = C::NS;
   __shared__ double s_cam[PS_W][16];
@@ -713,8 +714,8 @@ __global__ void __launch_bounds__(PS_W * 32) pcg_model_change_kernel(
     __syncwarp();
     if (lane < 16) cam[lane] = lane < 12 ? poses[(size_t)s * 12 + lane] : intr[(size_t)s * 4 + (lane - 12)];
     __syncwarp();
-    double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry;
-    obs_math<MODEL>(cam, 1, X0, X1, X2, pc, ob.x, ob.y, valid, jc0, jc1, jx0, jx1, rx, ry);
+    double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry, oc;
+    obs_math<MODEL, ROBUST>(cam, 1, X0, X1, X2, pc, ob.x, ob.y, valid, jc0, jc1, jx0, jx1, rx, ry, loss, oc);
     if (!valid) continue;
     const double* d = d_c + (size_t)s * DC;
     double e0 = jx0[0] * d0 + jx0[1] * d1 + jx0[2] * d2, e1 = jx1[0] * d0 + jx1[1] * d1 + jx1[2] * d2;
@@ -744,16 +745,19 @@ __global__ void __launch_bounds__(PS_W * 32) pcg_model_change_kernel(
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-#define VGG_PICK_PCG_KERNEL(kern, tmpl, p)                \
-  decltype(&tmpl<0, 0>) kern = nullptr;                   \
-  switch ((p)->camera_model * 3 + (p)->intr_mode) {       \
-    case 0: kern = tmpl<0, 0>; break;                     \
-    case 1: kern = tmpl<0, 1>; break;                     \
-    case 2: kern = tmpl<0, 2>; break;                     \
-    case 3: kern = tmpl<1, 0>; break;                     \
-    case 4: kern = tmpl<1, 1>; break;                     \
-    case 5: kern = tmpl<1, 2>; break;                     \
-  }                                                       \
+#define VGG_PICK_PCG_KERNEL(kern, tmpl, p)                                                          \
+  decltype(&tmpl<0, 0, false>) kern = nullptr;                                                      \
+  {                                                                                                 \
+    const bool robust = (p)->loss_function_type != VGG_LOSS_TRIVIAL;                               \
+    switch ((p)->camera_model * 3 + (p)->intr_mode) {                                               \
+      case 0: kern = robust ? tmpl<0, 0, true> : tmpl<0, 0, false>; break;                           \
+      case 1: kern = robust ? tmpl<0, 1, true> : tmpl<0, 1, false>; break;                           \
+      case 2: kern = robust ? tmpl<0, 2, true> : tmpl<0, 2, false>; break;                           \
+      case 3: kern = robust ? tmpl<1, 0, true> : tmpl<1, 0, false>; break;                           \
+      case 4: kern = robust ? tmpl<1, 1, true> : tmpl<1, 1, false>; break;                           \
+      case 5: kern = robust ? tmpl<1, 2, true> : tmpl<1, 2, false>; break;                           \
+    }                                                                                               \
+  }                                                                                                 \
   VGG_REQUIRE(kern, "bad camera_model/intr_mode")
 
 int pcg_blocks(int S, int ns) { return 3 * S + (ns > 0 ? 1 : 0); }
@@ -767,7 +771,7 @@ int launch_pcg_assemble(const vgg_ba_problem* p, int dc, int ns, int KR, const d
   VGG_PICK_PCG_KERNEL(kern, pcg_rhs_jacobi_kernel, p);
   const int nw = std::min(PJ_W, (p->S + 31) / 32);
   kern<<<(p->N + PJ_NT - 1) / PJ_NT, nw * 32, 0, st>>>(p->S, p->N, p->uv, p->mask, p->poses, p->intr, p->points,
-                                                        p->point_const, M, q, B.rhs, B.acc, fg_tracks);
+                                                        p->point_const, M, q, B.rhs, B.acc, fg_tracks, ba_loss_of(p));
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
@@ -797,7 +801,7 @@ int launch_pcg_matvec(const vgg_ba_problem* p, int dc, int ns, int KR, const dou
   VGG_PICK_PCG_KERNEL(kern, pcg_schur_kernel, p);
   const int nw = std::min(PS_W, p->S);
   kern<<<(p->N + 31) / 32, nw * 32, 0, st>>>(p->S, p->N, p->uv, p->mask, p->poses, p->intr, p->points, p->point_const,
-                                             M, sc_c, p->param_const, B.u, B.q, fg_tracks, B.cg);
+                                             M, sc_c, p->param_const, B.u, B.q, fg_tracks, B.cg, ba_loss_of(p));
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
@@ -875,7 +879,8 @@ int launch_pcg_model_change(const vgg_ba_problem* p, const double* M, const doub
   const int nw = std::min(PS_W, p->S);
   VGG_CUDA_CHECK(cudaMemsetAsync(cg + CG_MODEL_CHANGE, 0, sizeof(double), st));
   kern<<<(p->N + 31) / 32, nw * 32, 0, st>>>(p->S, p->N, p->uv, p->mask, p->poses, p->intr, p->points, p->point_const,
-                                             M, g_p, wacc, d_c, fg_tracks, cg + CG_MODEL_CHANGE);
+                                             M, g_p, wacc, d_c, fg_tracks, cg + CG_MODEL_CHANGE,
+                                             ba_loss_of(p));
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }

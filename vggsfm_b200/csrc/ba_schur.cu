@@ -172,12 +172,12 @@ __global__ void assemble_hc_kernel(int S, int dc, int ns, int KR, int Dpad, cons
 // written: the mask is fixed during a solve and Zt is zeroed once before it, so they hold the zero they would get.
 constexpr int ZB_NT = 8;     // tracks per CTA
 constexpr int ZB_W = 4;      // warps per CTA
-template <int MODEL, int MODE>
+template <int MODEL, int MODE, bool ROBUST>
 __global__ void __launch_bounds__(ZB_W * 32) z_build_kernel(
     int S, int N, int Dpad, const float* __restrict__ uv, const uint8_t* __restrict__ mask,
     const double* __restrict__ poses, const double* __restrict__ intr, const double* __restrict__ points,
     const uint8_t* __restrict__ point_const, const double* __restrict__ M, const double* __restrict__ q,
-    double* __restrict__ Zt, double* __restrict__ rhs, ptrdiff_t mc_off, const int* __restrict__ fg_tracks) {
+    double* __restrict__ Zt, double* __restrict__ rhs, ptrdiff_t mc_off, const int* __restrict__ fg_tracks, BaLoss loss) {
   using C = BlkCfg<MODEL, MODE>;
   constexpr int DC = C::DC, NS = C::NS;
   constexpr int ZR = 32 * DC;                      // Zt columns of one frame group
@@ -226,8 +226,9 @@ __global__ void __launch_bounds__(ZB_W * 32) z_build_kernel(
       const float2 ob = frame_ok ? uv2[o] : make_float2(0.f, 0.f);
       const double* pt = s_pt[t];
       const double* m = pt + 4;                    // M upper triangular (row-major), then q
-      double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry;
-      obs_math<MODEL>(pw + lane, 32, pt[0], pt[1], pt[2], pt[3] != 0.0, ob.x, ob.y, valid, jc0, jc1, jx0, jx1, rx, ry);
+      double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry, oc;
+      obs_math<MODEL, ROBUST>(pw + lane, 32, pt[0], pt[1], pt[2], pt[3] != 0.0, ob.x, ob.y, valid, jc0, jc1, jx0, jx1,
+                              rx, ry, loss, oc);
 #pragma unroll
       for (int i = 0; i < DC; ++i) {
         const double w0 = w_entry(jc0, jc1, jx0, jx1, i, 0), w1 = w_entry(jc0, jc1, jx0, jx1, i, 1),
@@ -464,11 +465,11 @@ __global__ void cam_step_kernel(int D, const double* __restrict__ dcs, size_t dc
 // warps of a CTA take the frames in turn (a frame's camera and step are broadcasts) and add up at the end.  Frames in
 // which none of the CTA's tracks is visible (band skip of sequential problems, or all masked) are passed over.
 constexpr int BS_W = 16;     // warps per CTA
-template <int MODEL, int MODE>
+template <int MODEL, int MODE, bool ROBUST>
 __global__ void __launch_bounds__(BS_W * 32) backsub_kernel(
     int S, int N, const float* __restrict__ uv, const uint8_t* __restrict__ mask, const double* __restrict__ poses,
     const double* __restrict__ intr, const double* __restrict__ points, const uint8_t* __restrict__ point_const,
-    const double* __restrict__ d_c, double* __restrict__ wacc, const int* __restrict__ fg_tracks) {
+    const double* __restrict__ d_c, double* __restrict__ wacc, const int* __restrict__ fg_tracks, BaLoss loss) {
   using C = BlkCfg<MODEL, MODE>;
   constexpr int DC = C::DC, NS = C::NS;
   __shared__ double s_cam[BS_W][16];
@@ -498,8 +499,8 @@ __global__ void __launch_bounds__(BS_W * 32) backsub_kernel(
     __syncwarp();
     if (lane < 16) cam[lane] = lane < 12 ? poses[(size_t)s * 12 + lane] : intr[(size_t)s * 4 + (lane - 12)];
     __syncwarp();
-    double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry;
-    obs_math<MODEL>(cam, 1, X0, X1, X2, pc, ob.x, ob.y, valid, jc0, jc1, jx0, jx1, rx, ry);
+    double jc0[8], jc1[8], jx0[3], jx1[3], rx, ry, oc;
+    obs_math<MODEL, ROBUST>(cam, 1, X0, X1, X2, pc, ob.x, ob.y, valid, jc0, jc1, jx0, jx1, rx, ry, loss, oc);
     const double* d = d_c + (size_t)s * DC;
 #pragma unroll
     for (int i = 0; i < DC; ++i) {
@@ -675,16 +676,19 @@ int launch_assemble_hc(int S, int dc, int ns, int KR, int Dpad, const double* ca
   return VGG_OK;
 }
 // the instantiation of a bundle-adjustment kernel template for the problem's camera model and intrinsics mode
-#define VGG_PICK_BA_KERNEL(kern, tmpl, p)                 \
-  decltype(&tmpl<0, 0>) kern = nullptr;                   \
-  switch ((p)->camera_model * 3 + (p)->intr_mode) {       \
-    case 0: kern = tmpl<0, 0>; break;                     \
-    case 1: kern = tmpl<0, 1>; break;                     \
-    case 2: kern = tmpl<0, 2>; break;                     \
-    case 3: kern = tmpl<1, 0>; break;                     \
-    case 4: kern = tmpl<1, 1>; break;                     \
-    case 5: kern = tmpl<1, 2>; break;                     \
-  }                                                       \
+#define VGG_PICK_BA_KERNEL(kern, tmpl, p)                                                          \
+  decltype(&tmpl<0, 0, false>) kern = nullptr;                                                      \
+  {                                                                                                 \
+    const bool robust = (p)->loss_function_type != VGG_LOSS_TRIVIAL;                               \
+    switch ((p)->camera_model * 3 + (p)->intr_mode) {                                               \
+      case 0: kern = robust ? tmpl<0, 0, true> : tmpl<0, 0, false>; break;                           \
+      case 1: kern = robust ? tmpl<0, 1, true> : tmpl<0, 1, false>; break;                           \
+      case 2: kern = robust ? tmpl<0, 2, true> : tmpl<0, 2, false>; break;                           \
+      case 3: kern = robust ? tmpl<1, 0, true> : tmpl<1, 0, false>; break;                           \
+      case 4: kern = robust ? tmpl<1, 1, true> : tmpl<1, 1, false>; break;                           \
+      case 5: kern = robust ? tmpl<1, 2, true> : tmpl<1, 2, false>; break;                           \
+    }                                                                                               \
+  }                                                                                                 \
   VGG_REQUIRE(kern, "bad camera_model/intr_mode")
 
 int launch_z_build(const vgg_ba_problem* p, int Dpad, const double* M, const double* q, double* Zt, double* rhs,
@@ -692,7 +696,7 @@ int launch_z_build(const vgg_ba_problem* p, int Dpad, const double* M, const dou
   VGG_PICK_BA_KERNEL(kern, z_build_kernel, p);
   const int nw = std::min(ZB_W, (p->S + 31) / 32);
   kern<<<(p->N + ZB_NT - 1) / ZB_NT, nw * 32, 0, st>>>(p->S, p->N, Dpad, p->uv, p->mask, p->poses, p->intr, p->points,
-                                                        p->point_const, M, q, Zt, rhs, mc_off, fg_tracks);
+                                                        p->point_const, M, q, Zt, rhs, mc_off, fg_tracks, ba_loss_of(p));
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
@@ -773,7 +777,7 @@ int launch_backsub(const vgg_ba_problem* p, const double* d_c, double* wacc, con
   VGG_PICK_BA_KERNEL(kern, backsub_kernel, p);
   const int nw = std::min(BS_W, p->S);
   kern<<<(p->N + 31) / 32, nw * 32, 0, st>>>(p->S, p->N, p->uv, p->mask, p->poses, p->intr, p->points, p->point_const,
-                                             d_c, wacc, fg_tracks);
+                                             d_c, wacc, fg_tracks, ba_loss_of(p));
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }

@@ -156,6 +156,18 @@ static double* pinned_scalars() {
   return h;
 }
 
+// The problem's robust loss: an unknown type, or a robust one whose scale a is not finite and > 0 with a^2 a normal
+// number (so that b = a^2 and c = 1 / b are finite and nonzero), is VGG_EINVAL before anything is launched.
+static int check_loss(const vgg_ba_problem* p) {
+  const int t = p->loss_function_type;
+  const double a = p->loss_function_scale;
+  VGG_REQUIRE(t == VGG_LOSS_TRIVIAL || t == VGG_LOSS_SOFT_L1 || t == VGG_LOSS_CAUCHY,
+              "loss_function_type must be VGG_LOSS_TRIVIAL, VGG_LOSS_SOFT_L1 or VGG_LOSS_CAUCHY");
+  VGG_REQUIRE(t == VGG_LOSS_TRIVIAL || (isfinite(a) && a > 0.0 && isnormal(a * a)),
+              "loss_function_scale of a robust loss must be finite and > 0 (a^2 a normal double)");
+  return VGG_OK;
+}
+
 static int dims_of(int model, int mode, int* dc, int* ns, int* KR) {
   if (model != VGG_SIMPLE_PINHOLE && model != VGG_SIMPLE_RADIAL) return VGG_EINVAL;
   const int ni = model == VGG_SIMPLE_PINHOLE ? 1 : 2;
@@ -521,7 +533,7 @@ using namespace vgg;
 extern "C" {
 
 const char* vgg_last_error(void) { return g_err; }
-int vgg_version(void) { return 100; }
+int vgg_version(void) { return 101; }
 
 void vgg_ba_default_options(vgg_ba_options* o) {
   memset(o, 0, sizeof(*o));
@@ -568,6 +580,7 @@ int vgg_dev_build_blocks_band(const vgg_ba_problem* prob, double* cost, double* 
                               double* W, double* shared_out, int tracks_per_warp, const int* fg_tracks, int count,
                               void* stream) {
   VGG_REQUIRE(prob && cost && camrec && g_p && H_pp && shared_out, "null pointer");
+  if (const int rc = check_loss(prob)) return rc;
   // a warp's first track t0 = chunk * tracks_per_warp + 4k is the 16-byte (uv) / 4-byte (mask) cp.async offset
   VGG_REQUIRE(tracks_per_warp >= 0 && tracks_per_warp % 4 == 0, "tracks_per_warp must be 0 (choose) or a multiple of 4");
   VGG_REQUIRE(!fg_tracks || count == 2 * ((prob->S + 31) / 32), "fg_tracks needs 2 entries per group of 32 frames");
@@ -595,6 +608,7 @@ int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double*
                  double max_diag, void* workspace, size_t ws_bytes, double* Sraw, double* rhs, int* Dpad_out,
                  void* stream) {
   VGG_REQUIRE(prob && workspace && Sraw && rhs, "null pointer");
+  if (const int rc = check_loss(prob)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   g_launch_count = 0;
   Layout L;
@@ -623,6 +637,7 @@ int vgg_dev_schur_build(const vgg_ba_problem* prob, const double* camrec, const 
                         int banded, int zt_nan, void* workspace, size_t ws_bytes, double* M, double* q, double* dpp,
                         double* scal, double* Zt, double* Sraw, double* rhs, void* stream) {
   VGG_REQUIRE(prob && camrec && g_p && H_pp && shared_in && scale_p && workspace, "null pointer");
+  if (const int rc = check_loss(prob)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   g_launch_count = 0;
   Layout L;
@@ -719,6 +734,7 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
                     const vgg_ba_fabric* fabric, vgg_ba_summary* summary, double* trace, double* cg_trace, void* stream) {
   VGG_REQUIRE(prob && workspace && summary, "null pointer");
   VGG_REQUIRE(prob->uv && prob->mask && prob->param_const && prob->poses && prob->intr && prob->points, "null problem array");
+  if (const int rc = check_loss(prob)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   g_launch_count = 0;
   vgg_ba_options opt;
@@ -1123,6 +1139,7 @@ int vgg_dev_pcg_probe(const vgg_ba_problem* prob, const double* camrec, const do
                       double* y_out, double* b_out, double* pinv_out, double* state_out, void* stream) {
   VGG_REQUIRE(prob && camrec && g_p && H_pp && shared_in && scale_p && scale_c && x_in && workspace, "null pointer");
   VGG_REQUIRE(prob->param_const, "null param_const");
+  if (const int rc = check_loss(prob)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   g_launch_count = 0;
   Layout L;

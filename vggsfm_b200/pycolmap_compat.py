@@ -16,6 +16,8 @@ libvggsfm_b200.so on the current CUDA device; objects live on the host like pyco
 """
 from __future__ import annotations
 
+import enum
+
 import numpy as np
 import torch
 
@@ -48,9 +50,18 @@ class _SolverOptions:
         self.num_threads = -1
 
 
+class LossFunctionType(enum.Enum):
+    """COLMAP's BundleAdjustmentOptions::LossFunctionType: the robust loss on every reprojection residual."""
+    TRIVIAL = 0
+    SOFT_L1 = 1
+    CAUCHY = 2
+
+
 class BundleAdjustmentOptions:
     def __init__(self):
         self.solver_options = _SolverOptions()
+        self.loss_function_type = LossFunctionType.TRIVIAL
+        self.loss_function_scale = 1.0                 # pixels
         self.refine_focal_length = True
         self.refine_principal_point = False
         self.refine_extra_params = True
@@ -58,13 +69,16 @@ class BundleAdjustmentOptions:
         self.print_summary = False
 
     def _native(self):
-        """(vgg_ba_options, the linear-solver keywords of bundle_adjustment.bundle_adjustment)."""
+        """(vgg_ba_options, the linear-solver and loss keywords of bundle_adjustment.bundle_adjustment)."""
         o = _ba.default_options()
         so = self.solver_options
         o.function_tolerance, o.gradient_tolerance, o.parameter_tolerance = so.function_tolerance, so.gradient_tolerance, so.parameter_tolerance
         o.max_num_iterations = int(so.max_num_iterations)
         lin = dict(linear_solver_type=so.linear_solver_type, min_linear_solver_iterations=int(so.min_linear_solver_iterations),
                    max_linear_solver_iterations=int(so.max_linear_solver_iterations), eta=float(so.eta))
+        lt = self.loss_function_type
+        lin.update(loss_function_type=lt.name if isinstance(lt, LossFunctionType) else str(lt),
+                   loss_function_scale=float(self.loss_function_scale))
         return o, lin
 
 
