@@ -203,14 +203,33 @@ typedef struct vgg_ba_linear_solver {
 void vgg_ba_default_linear_solver(vgg_ba_linear_solver* lin);
 /* Workspace of vgg_ba_solve_iterative: no Schur operand, no reduced system, no factorisation workspace. */
 int vgg_ba_workspace_bytes_iterative(int S, int N, int camera_model, int intr_mode, size_t* bytes);
-/* vgg_ba_solve with lin->type = VGG_BA_ITERATIVE_SCHUR, on one GPU (no all-reduce hook, no fabric).  `trace` as for
- * vgg_ba_solve; `cg_trace` is a HOST array [max_num_iterations, 4] or NULL: per LM iteration the CG iterations, the CG
- * termination (VGG_CG_*), the last zeta and |r| / |b|.  The model change of the inexact step is
+/* vgg_ba_solve with lin->type = VGG_BA_ITERATIVE_SCHUR on one GPU: vgg_ba_solve_iterative_sharded without a hook.
+ * `trace` as for vgg_ba_solve; `cg_trace` is a HOST array [max_num_iterations, 4] or NULL: per LM iteration the CG
+ * iterations, the CG termination (VGG_CG_*), the last zeta and |r| / |b|.  The model change of the inexact step is
  * -(J d)^T (f + J d / 2), evaluated per observation.  Returns VGG_EINVAL before any launch for another lin->type,
  * min < 0, max < min or eta not positive and finite. */
 int vgg_ba_solve_iterative(const vgg_ba_problem* prob, const vgg_ba_options* opt, const vgg_ba_linear_solver* lin,
                            void* workspace, size_t ws_bytes, vgg_ba_summary* summary, double* trace, double* cg_trace,
                            void* stream);
+/* ITERATIVE_SCHUR over track shards (one process per GPU, every rank with all S cameras and its own tracks), with the
+ * all-reduce hook's contract: every rank makes the same sequence of calls, and every `buf` lies inside the workspace
+ * (vgg_ba_workspace_bytes_iterative of the rank's own N).  Besides the reductions both solvers make once per solve (the
+ * frames any rank sees) and per candidate (cost, gradient and model terms, sum; the point-gradient maximum, max), the
+ * hook sums
+ *   - once per LM iteration, one region: the right-hand side, diag(H_cc), the camera gradient and the Schur-Jacobi
+ *     accumulators this rank's observations give, with a copy of its camera records (H_cc and g);
+ *   - once per CG matvec, the D-vector of the matvec's Schur part: one call per CG iteration, two on every 10th (the
+ *     residual reset).  The host queues CG iterations in chunks of 10 and reads the stop flag once per chunk, so the
+ *     calls of a queued iteration past the stop are made too (on a vector nobody reads);
+ *   - the model change of the step, in the candidate's small reduction (no call of its own).
+ * The CG's scalars are sums in a fixed order, so every rank holds the same CG state, stops at the same iteration and
+ * ends with bit-identical cameras; CG iterations, termination and zeta (cg_trace) are the same on every rank.  allreduce
+ * NULL is vgg_ba_solve_iterative.  There is no fabric variant.  A rank without tracks passes 16 masked padding tracks
+ * (vgg_allreduce_fn).  VGG_EINVAL before any launch as vgg_ba_solve_iterative. */
+int vgg_ba_solve_iterative_sharded(const vgg_ba_problem* prob, const vgg_ba_options* opt,
+                                   const vgg_ba_linear_solver* lin, void* workspace, size_t ws_bytes,
+                                   vgg_allreduce_fn allreduce, void* allreduce_user, vgg_ba_summary* summary,
+                                   double* trace, double* cg_trace, void* stream);
 
 int vgg_ba_reduced_system_doubles(int S, int camera_model, int intr_mode, size_t* doubles);
 int vgg_ba_fabric_doubles(int S, int camera_model, int intr_mode, size_t* doubles);

@@ -18,6 +18,7 @@ EXPORTS = [
     "vgg_ba_build_blocks", "vgg_ba_schur", "vgg_cholesky_lower", "vgg_ba_solve",
     "vgg_ba_reduced_system_doubles", "vgg_ba_fabric_doubles", "vgg_ba_solve_fabric",
     "vgg_ba_default_linear_solver", "vgg_ba_workspace_bytes_iterative", "vgg_ba_solve_iterative",
+    "vgg_ba_solve_iterative_sharded",
     "vgg_pose_default_options", "vgg_pose_refinement", "vgg_pnp_workspace_bytes", "vgg_absolute_pose_estimation", "vgg_syrk_ozaki_workspace_bytes", "vgg_syrk_ozaki",
     "vgg_tri_workspace_bytes", "vgg_triangulate_tracks", "vgg_triangulate_by_pair", "vgg_filter_points3d",
     "vgg_project_points", "vgg_normalize_tracks", "vgg_undistort_simple_radial",
@@ -154,6 +155,9 @@ def lib() -> ctypes.CDLL:
     L.vgg_ba_workspace_bytes_iterative.argtypes = [ci, ci, ci, ci, ctypes.POINTER(cs)]
     L.vgg_ba_solve_iterative.argtypes = [ctypes.POINTER(BAProblem), ctypes.POINTER(BAOptions),
                                          ctypes.POINTER(BALinearSolver), vp, cs, ctypes.POINTER(BASummary), vp, vp, vp]
+    L.vgg_ba_solve_iterative_sharded.argtypes = [ctypes.POINTER(BAProblem), ctypes.POINTER(BAOptions),
+                                                 ctypes.POINTER(BALinearSolver), vp, cs, ALLREDUCE_FN, vp,
+                                                 ctypes.POINTER(BASummary), vp, vp, vp]
     L.vgg_dev_pcg_probe.argtypes = [ctypes.POINTER(BAProblem)] + [vp] * 6 + [cd] * 3 + [vp, vp, cs] + [vp] * 5
     L.vgg_pose_default_options.argtypes = [ctypes.POINTER(PoseOptions)]
     L.vgg_pose_default_options.restype = None

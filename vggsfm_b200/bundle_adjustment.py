@@ -236,6 +236,20 @@ class Summary:
     mask: Optional[torch.Tensor] = None       # [S,P'] observations that were in the problem (bundle_adjustment only)
 
 
+def check_allreduce(allreduce, linear_solver_type="DENSE_SCHUR"):
+    """ValueError, before anything runs, for a hook lm_solve cannot use: an object without a callable ``bind``, or a hook
+    with a fabric attached together with ITERATIVE_SCHUR (the fabric reduces the dense reduced system, which the
+    iterative solve never forms)."""
+    if allreduce is None:
+        return
+    if not callable(getattr(allreduce, "bind", None)):
+        raise ValueError(f"allreduce must be an all-reduce hook with a bind(workspace) method "
+                         f"(vggsfm_b200.dist.AllReduceHook), not {type(allreduce).__name__}")
+    if linear_solver_type == "ITERATIVE_SCHUR" and getattr(allreduce, "fabric", None) is not None:
+        raise ValueError("ITERATIVE_SCHUR reduces through the all-reduce hook, not a fabric: pass AllReduceHook() "
+                         "without a fabric")
+
+
 def lm_solve(uv, mask, poses, intr, points, model, mode, param_const=None, point_const=None,
              options: Optional[BAOptions] = None, allreduce=None, want_trace=False, linear_solver_type="DENSE_SCHUR",
              min_linear_solver_iterations=0, max_linear_solver_iterations=500, eta=0.1, loss_function_type="TRIVIAL",
@@ -244,16 +258,18 @@ def lm_solve(uv, mask, poses, intr, points, model, mode, param_const=None, point
     vggsfm_b200.dist.AllReduceHook for track-sharded multi-GPU runs.  A rank whose shard holds no track (N = 0:
     shard_range gives empty tail shards when the tracks are few) still takes part in every reduction: it solves 16
     masked-out padding tracks, as bundle_adjustment() pads, and leaves its empty `points` untouched.
-    linear_solver_type="ITERATIVE_SCHUR" solves each step by PCG (vgg_ba_solve_iterative) with the three CG options;
-    it runs on one GPU only, so it raises ValueError together with `allreduce`.
+    linear_solver_type="ITERATIVE_SCHUR" solves each step by PCG (vgg_ba_solve_iterative_sharded) with the three CG
+    options, on one GPU or, with `allreduce`, over track shards: every rank sums its assembly once per LM iteration and
+    the Schur part of every CG matvec through the hook, and all ranks take the same CG and LM decisions.  A hook with a
+    fabric attached raises ValueError with ITERATIVE_SCHUR, and so does an object without a callable ``bind``, before
+    anything runs.
     loss_function_type / loss_function_scale: COLMAP's BundleAdjustmentOptions loss (TRIVIAL, SOFT_L1 or CAUCHY at a
     scale in pixels) on every observation; the costs of the summary are then 0.5 sum rho(|r|^2).  An unknown name raises
     ValueError, a robust loss with a scale that is not finite and > 0 raises from the library before anything runs."""
     loss_function_id(loss_function_type)
     lin = linear_solver(linear_solver_type, min_linear_solver_iterations, max_linear_solver_iterations, eta)
     iterative = linear_solver_type == "ITERATIVE_SCHUR"
-    if iterative and allreduce is not None:
-        raise ValueError("ITERATIVE_SCHUR runs on one GPU: it takes no all-reduce hook or fabric")
+    check_allreduce(allreduce, linear_solver_type)
     L = _lib.lib()
     S, N = mask.shape
     dev = uv.device
@@ -279,9 +295,10 @@ def lm_solve(uv, mask, poses, intr, points, model, mode, param_const=None, point
     with torch.cuda.device(dev):
         st = torch.cuda.current_stream().cuda_stream
         if iterative:
-            rc = L.vgg_ba_solve_iterative(ctypes.byref(p), ctypes.byref(opt), ctypes.byref(lin), ws.data_ptr(),
-                                          ws.numel(), ctypes.byref(summ),
-                                          trace.data_ptr() if trace is not None else None, cg_trace.data_ptr(), st)
+            rc = L.vgg_ba_solve_iterative_sharded(ctypes.byref(p), ctypes.byref(opt), ctypes.byref(lin), ws.data_ptr(),
+                                                  ws.numel(), cb, None, ctypes.byref(summ),
+                                                  trace.data_ptr() if trace is not None else None, cg_trace.data_ptr(),
+                                                  st)
         elif fabric is not None:
             fs = fabric.struct()
             rc = L.vgg_ba_solve_fabric(ctypes.byref(p), ctypes.byref(opt), ws.data_ptr(), ws.numel(), cb, None,
@@ -358,15 +375,15 @@ def bundle_adjustment(points3d, extrinsics, intrinsics, extra_params, tracks, ma
     points3d [P,3], extrinsics [S,3,4], intrinsics [S,3,3], extra_params [S,1]|None, tracks [S,P,2],
     masks [S,P] bool -- CUDA tensors.  Returns (points3D [P',3] f64, extrinsics [S,3,4] f64,
     intrinsics [S,3,3] f64, extra_params [S,1]|None, valid_idx [P'], Summary).  linear_solver_type and the CG options
-    as lm_solve (ITERATIVE_SCHUR with `allreduce` raises ValueError before anything runs), and so are
+    as lm_solve (ITERATIVE_SCHUR runs over track shards through `allreduce` too; a hook with a fabric raises ValueError
+    with it before anything runs), and so are
     loss_function_type and loss_function_scale (COLMAP's BundleAdjustmentOptions defaults: TRIVIAL, 1.0)."""
     model = camera_model_id(camera_type)
     loss_function_id(loss_function_type)
     lin_kw = dict(linear_solver_type=linear_solver_type, min_linear_solver_iterations=min_linear_solver_iterations,
                   max_linear_solver_iterations=max_linear_solver_iterations, eta=eta)
     linear_solver(**lin_kw)
-    if linear_solver_type == "ITERATIVE_SCHUR" and allreduce is not None:
-        raise ValueError("ITERATIVE_SCHUR runs on one GPU: it takes no all-reduce hook or fabric")
+    check_allreduce(allreduce, linear_solver_type)
     dev = tracks.device
     if not tracks.is_cuda:
         raise RuntimeError("vggsfm_b200.bundle_adjustment needs CUDA tensors (no CPU fallback)")

@@ -10,7 +10,8 @@
 //   pcg_rhs_jacobi     one pass over the observations: rhs += sum Z q and, per parameter block, sum Z_b Z_b^T
 //                      (rotation, translation, per-frame intrinsics, shared intrinsics: Ceres' blocks)
 //   pcg_init           per block: A_bb scaled and damped, inverted by a 3x3 Cholesky; b, x = 0, r = b, z = P r, rho
-//   pcg_hcc / pcg_schur   q = A v: the camera-Hessian part per parameter row, then the Schur part per track CTA
+//   pcg_hcc / pcg_schur   q = A v: the camera-Hessian part per parameter row, then the Schur part per track CTA into its
+//                      own vector qs, which pcg_alpha (or pcg_update after the residual reset) adds to q
 //   pcg_alpha / pcg_xstep / pcg_update   the CG scalars and vectors
 //   pcg_model_change   Ceres' model change -(J d)^T (f + J d / 2) of the inexact step, per observation
 //
@@ -18,6 +19,13 @@
 // The CG scalars and its termination live on the device (pcg_state): every CG kernel returns at once when the state's
 // done flag is set, and the host launches iterations in chunks of PCG_CHUNK, reading the flag once per chunk while the
 // next chunk is already queued.
+//
+// Track shards (an all-reduce hook): each rank holds every camera and its own tracks, so what a rank builds from its
+// observations is a partial sum -- the camera records, rhs / hdiag / gvec / acc of the assembly, the Schur part qs of
+// every matvec and the model change.  The hook sums the assembly once per LM iteration (csrc/ba_solve.cu) and qs once per
+// matvec (pcg_iteration); everything else in the CG is computed from summed data only.  Its scalars are sums over CTAs
+// taken in a fixed order (reduce_fixed), so every rank forms the same bits, takes the same CG decisions and queues the
+// same hook calls.  The single-GPU solve runs the same kernels without the hook.
 #include <stddef.h>
 #include <algorithm>
 #include "ba_obs.h"
@@ -29,10 +37,12 @@ namespace vgg {
 
 __device__ __forceinline__ bool zero_or_inf(double v) { return v == 0.0 || isinf(v); }
 
-// Sum of up to 4 per-thread values over the CTA, added to acc[0..K) with one atomic each by thread 0; returns true in
-// every thread of the CTA that finished last (all other CTAs' atomics are visible to it).
+// Sum of up to 3 per-thread values over the grid in a fixed order: each CTA adds its threads by warp shuffles and then
+// its warps in index order into its own slots[K * blockIdx.x + k]; the CTA that finishes last adds the slots in CTA order
+// into out[].  The bits depend on the inputs and the grid shape only, not on which CTA finishes first, so ranks holding
+// the same data form the same sums.  Returns true in thread 0 of the last CTA, the only thread whose out[] is set.
 template <int K>
-__device__ bool reduce_and_ticket(const double (&v)[K], double* acc, unsigned* ticket) {
+__device__ bool reduce_fixed(const double (&v)[K], double* slots, unsigned* ticket, double (&out)[K]) {
   __shared__ double red[K][32];
   __shared__ bool last;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
@@ -47,19 +57,21 @@ __device__ bool reduce_and_ticket(const double (&v)[K], double* acc, unsigned* t
     for (int k = 0; k < K; ++k) {
       double s = 0.0;
       for (int w = 0; w < nw; ++w) s += red[k][w];
-      atomicAdd(&acc[k], s);
+      slots[(size_t)blockIdx.x * K + k] = s;
     }
     __threadfence();
     last = atomicAdd(ticket, 1u) == gridDim.x - 1;
   }
   __syncthreads();
-  if (last) __threadfence();
-  return last;
-}
-__device__ __forceinline__ double take_acc(double* p) {
-  const double v = atomicAdd(p, 0.0);
-  *p = 0.0;
-  return v;
+  if (!last || threadIdx.x != 0) return false;
+  __threadfence();
+#pragma unroll
+  for (int k = 0; k < K; ++k) out[k] = 0.0;
+  for (unsigned b = 0; b < gridDim.x; ++b)
+#pragma unroll
+    for (int k = 0; k < K; ++k) out[k] += __ldcg(slots + (size_t)b * K + k);
+  *ticket = 0u;
+  return true;
 }
 __device__ __forceinline__ void finish(double* cg, double term) {
   cg[CG_TERM] = term;
@@ -276,7 +288,7 @@ __global__ void pcg_init_kernel(int S, int dc, int ns, int KR, const double* __r
                                 const double* __restrict__ sc, const uint8_t* __restrict__ pconst, double radius,
                                 double min_diag, double max_diag, double* __restrict__ pinv, double* __restrict__ bvec,
                                 double* __restrict__ x, double* __restrict__ r, double* __restrict__ z,
-                                double* __restrict__ cg) {
+                                double* __restrict__ cg, double* __restrict__ slots) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   const int nblk = 3 * S + (ns > 0 ? 1 : 0);
   double part[3] = {0.0, 0.0, 0.0};       // r.z, |b|^2, failed blocks
@@ -341,9 +353,9 @@ __global__ void pcg_init_kernel(int S, int dc, int ns, int KR, const double* __r
     }
     part[2] = bad ? 1.0 : 0.0;
   }
-  if (reduce_and_ticket<3>(part, cg + CG_ACC, reinterpret_cast<unsigned*>(cg + CG_TICKET_SLOT)) && threadIdx.x == 0) {
-    const double rho = take_acc(cg + CG_ACC), bsq = take_acc(cg + CG_ACC + 1), fails = take_acc(cg + CG_ACC + 2);
-    *reinterpret_cast<unsigned*>(cg + CG_TICKET_SLOT) = 0u;
+  double sum[3];
+  if (reduce_fixed<3>(part, slots, reinterpret_cast<unsigned*>(cg + CG_TICKET_SLOT), sum)) {
+    const double rho = sum[0], bsq = sum[1], fails = sum[2];
     cg[CG_BB] = bsq;
     cg[CG_Q0] = 0.0;
     cg[CG_BETA] = 0.0;
@@ -375,7 +387,8 @@ __global__ void __launch_bounds__(256) pcg_hcc_kernel(int S, int dc, int ns, int
                                                       double max_diag, int pmode, const double* __restrict__ z,
                                                       const double* __restrict__ p_old, const double* __restrict__ x,
                                                       double* __restrict__ p_new, double* __restrict__ u,
-                                                      double* __restrict__ q, const double* __restrict__ cg) {
+                                                      double* __restrict__ q, double* __restrict__ qs,
+                                                      const double* __restrict__ cg) {
   if (cg[CG_DONE] != 0.0) return;
   const double beta = cg[CG_BETA];
   const bool pm = pmode != 0;
@@ -400,6 +413,7 @@ __global__ void __launch_bounds__(256) pcg_hcc_kernel(int S, int dc, int ns, int
     if (pm) p_new[i] = v;
     u[i] = pin ? 0.0 : sc[i] * v;
     q[i] = pin ? v : sc[i] * y + damp * v;
+    qs[i] = 0.0;
     return;
   }
   // shared-intrinsics rows: H_ss u_s + sum over frames of H_cs^T u_c
@@ -429,10 +443,11 @@ __global__ void __launch_bounds__(256) pcg_hcc_kernel(int S, int dc, int ns, int
     if (pm) p_new[i] = v;
     u[i] = pin ? 0.0 : sc[i] * v;
     q[i] = pin ? v : sc[i] * y + damp * v;
+    qs[i] = 0.0;
   }
 }
 
-// q[row] -= sc[row] (sum_n Z_n Z_n^T u)[row] for free rows.  A CTA owns 32 tracks (one lane each); its warps take the
+// qs[row] -= sc[row] (sum_n Z_n Z_n^T u)[row] for free rows (qs zeroed by pcg_hcc; q = its part + qs).  A CTA owns 32 tracks (one lane each); its warps take the
 // frames in turn.  Pass 1 (as backsub): w_n = sum_s W_sn^T u_s; then t_n = M_n M_n^T w_n; pass 2: the frame's
 // sum over the CTA's tracks of W_sn t_n, one warp reduce-scatter and one f64 RED per (CTA, frame parameter).
 constexpr int PS_W = 16;
@@ -441,7 +456,7 @@ __global__ void __launch_bounds__(PS_W * 32) pcg_schur_kernel(
     int S, int N, const float* __restrict__ uv, const uint8_t* __restrict__ mask, const double* __restrict__ poses,
     const double* __restrict__ intr, const double* __restrict__ points, const uint8_t* __restrict__ point_const,
     const double* __restrict__ M, const double* __restrict__ sc, const uint8_t* __restrict__ pconst,
-    const double* __restrict__ u, double* __restrict__ q, const int* __restrict__ fg_tracks,
+    const double* __restrict__ u, double* __restrict__ qs, const int* __restrict__ fg_tracks,
     const double* __restrict__ cg, BaLoss loss) {
   if (cg[CG_DONE] != 0.0) return;
   using C = BlkCfg<MODEL, MODE>;
@@ -548,7 +563,7 @@ __global__ void __launch_bounds__(PS_W * 32) pcg_schur_kernel(
     const double r = warp_reduce_scatter<8>(a8, lane);
     if (lane < DC) {
       const size_t row = (size_t)s * DC + lane;
-      if (!pconst[row] && r != 0.0) atomicAdd(&q[row], -sc[row] * r);
+      if (!pconst[row] && r != 0.0) atomicAdd(&qs[row], -sc[row] * r);
     }
   }
   if (NS > 0) {
@@ -564,20 +579,26 @@ __global__ void __launch_bounds__(PS_W * 32) pcg_schur_kernel(
       double v = 0.0;
       for (int k = 0; k < nw; ++k) v += s_acc[j][k][0];
       const size_t row = (size_t)S * DC + j;
-      if (!pconst[row] && v != 0.0) atomicAdd(&q[row], -sc[row] * v);
+      if (!pconst[row] && v != 0.0) atomicAdd(&qs[row], -sc[row] * v);
     }
   }
 }
 
-// pq = p.q; alpha = rho / pq.  p'q <= 0 (indefinite), an infinite p'q, or a zero or infinite alpha fail the solve.
-__global__ void __launch_bounds__(256) pcg_alpha_kernel(int D, const double* __restrict__ p, const double* __restrict__ q,
-                                                        double* __restrict__ cg) {
+// q += qs (the matvec's Schur part, summed over the ranks); pq = p.q; alpha = rho / pq.  p'q <= 0 (indefinite), an
+// infinite p'q, or a zero or infinite alpha fail the solve.
+__global__ void __launch_bounds__(256) pcg_alpha_kernel(int D, const double* __restrict__ p, double* __restrict__ q,
+                                                        const double* __restrict__ qs, double* __restrict__ cg,
+                                                        double* __restrict__ slots) {
   if (cg[CG_DONE] != 0.0) return;
   double part[1] = {0.0};
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < D; i += gridDim.x * blockDim.x) part[0] += p[i] * q[i];
-  if (reduce_and_ticket<1>(part, cg + CG_ACC, reinterpret_cast<unsigned*>(cg + CG_TICKET_SLOT)) && threadIdx.x == 0) {
-    *reinterpret_cast<unsigned*>(cg + CG_TICKET_SLOT) = 0u;
-    const double pq = take_acc(cg + CG_ACC);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < D; i += gridDim.x * blockDim.x) {
+    const double qi = q[i] + qs[i];
+    q[i] = qi;
+    part[0] += p[i] * qi;
+  }
+  double sum[1];
+  if (reduce_fixed<1>(part, slots, reinterpret_cast<unsigned*>(cg + CG_TICKET_SLOT), sum)) {
+    const double pq = sum[0];
     const double alpha = cg[CG_RHO] / pq;
     cg[CG_ALPHA] = alpha;
     if (pq <= 0.0 || isinf(pq) || zero_or_inf(alpha)) {
@@ -596,14 +617,15 @@ __global__ void pcg_xstep_kernel(int D, const double* __restrict__ p, double* __
 }
 
 // End of CG iteration i, one thread per preconditioner block: x += alpha p, r -= alpha q (reset: x already stepped,
-// r = b - q with q = A x); z = P r; the last CTA forms Q1 = -x.(b + r), zeta = i (Q1 - Q0) / Q1 and the next rho and beta,
+// r = b - q with q = A x, its Schur part still in qs); z = P r; the last CTA forms Q1 = -x.(b + r), zeta = i (Q1 - Q0) / Q1 and the next rho and beta,
 // in Ceres' order: zeta < eta with i >= min succeeds, then i >= max stops without convergence, then a zero or infinite
 // rho or beta of iteration i + 1 fails.
 __global__ void __launch_bounds__(256) pcg_update_kernel(int S, int dc, int ns, int reset, const double* __restrict__ pinv,
                                                          const double* __restrict__ bvec, const double* __restrict__ p,
-                                                         const double* __restrict__ q, double* __restrict__ x,
-                                                         double* __restrict__ r, double* __restrict__ z, double eta,
-                                                         int min_it, int max_it, double* __restrict__ cg) {
+                                                         const double* __restrict__ q, const double* __restrict__ qs,
+                                                         double* __restrict__ x, double* __restrict__ r,
+                                                         double* __restrict__ z, double eta, int min_it, int max_it,
+                                                         double* __restrict__ cg, double* __restrict__ slots) {
   if (cg[CG_DONE] != 0.0) return;
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   const int nblk = 3 * S + (ns > 0 ? 1 : 0);
@@ -617,7 +639,7 @@ __global__ void __launch_bounds__(256) pcg_update_kernel(int S, int dc, int ns, 
       const int k = r0 + i;
       double xi = x[k], ri;
       if (reset) {
-        ri = bvec[k] - q[k];
+        ri = bvec[k] - (q[k] + qs[k]);
       } else {
         xi += alpha * p[k];
         x[k] = xi;
@@ -636,9 +658,9 @@ __global__ void __launch_bounds__(256) pcg_update_kernel(int S, int dc, int ns, 
       part[0] += rr[i] * zi;
     }
   }
-  if (reduce_and_ticket<3>(part, cg + CG_ACC, reinterpret_cast<unsigned*>(cg + CG_TICKET_SLOT)) && threadIdx.x == 0) {
-    *reinterpret_cast<unsigned*>(cg + CG_TICKET_SLOT) = 0u;
-    const double rho = take_acc(cg + CG_ACC), Q1 = take_acc(cg + CG_ACC + 1), rsq = take_acc(cg + CG_ACC + 2);
+  double sum[3];
+  if (reduce_fixed<3>(part, slots, reinterpret_cast<unsigned*>(cg + CG_TICKET_SLOT), sum)) {
+    const double rho = sum[0], Q1 = sum[1], rsq = sum[2];
     const double i = cg[CG_ITERS] + 1.0;
     cg[CG_ITERS] = i;
     const double zeta = i * (Q1 - cg[CG_Q0]) / Q1;
@@ -667,7 +689,7 @@ __global__ void __launch_bounds__(256) pcg_update_kernel(int S, int dc, int ns, 
 // ------------------------------------------------------------------------------------------------
 // Ceres' model change of a step: -(J d)^T (f + J d / 2) summed over the observations, d = (d_c, d_p) unscaled; d_p is
 // recomputed from M, g_p and wacc with point_step's arithmetic (bit for bit the step the candidate took).  One lane per
-// track, warps over the frames, as backsub.
+// track, warps over the frames, as backsub.  With track shards this is the rank's part, summed with the candidate's cost.
 template <int MODEL, int MODE, bool ROBUST>
 __global__ void __launch_bounds__(PS_W * 32) pcg_model_change_kernel(
     int S, int N, const float* __restrict__ uv, const uint8_t* __restrict__ mask, const double* __restrict__ poses,
@@ -762,6 +784,12 @@ __global__ void __launch_bounds__(PS_W * 32) pcg_model_change_kernel(
 
 int pcg_blocks(int S, int ns) { return 3 * S + (ns > 0 ? 1 : 0); }
 
+// K partials per CTA of the fixed-order reductions: 3 per CTA of pcg_init / pcg_update, 1 per CTA of pcg_alpha
+static int pcg_alpha_ctas(int D) { return std::min(132, (D + 255) / 256); }
+size_t pcg_slot_doubles(int S, int dc, int ns) {
+  return (size_t)std::max(3 * ((pcg_blocks(S, ns) + 255) / 256), pcg_alpha_ctas(S * dc + ns));
+}
+
 int launch_pcg_assemble(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
                         const double* M, const double* q, const PcgBuffers& B, const int* fg_tracks, cudaStream_t st) {
   const int D = p->S * dc + ns;
@@ -783,7 +811,7 @@ int launch_pcg_init(const vgg_ba_problem* p, int dc, int ns, int KR, const doubl
   VGG_CUDA_CHECK(cudaMemsetAsync(B.cg, 0, sizeof(double) * PCG_STATE_DOUBLES, st));
   pcg_init_kernel<<<(nblk + 255) / 256, 256, 0, st>>>(p->S, dc, ns, KR, camrec, shared_in, B.acc, B.rhs, B.hdiag, sc_c,
                                                       p->param_const, radius, min_diag, max_diag, B.pinv, bvec, B.x,
-                                                      B.r, B.z, B.cg);
+                                                      B.r, B.z, B.cg, B.slots);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
@@ -796,21 +824,34 @@ int launch_pcg_matvec(const vgg_ba_problem* p, int dc, int ns, int KR, const dou
   const int nrow = p->S * dc;
   pcg_hcc_kernel<<<(nrow + 255) / 256 + (ns > 0 ? 1 : 0), 256, 0, st>>>(
       p->S, dc, ns, KR, camrec, shared_in, hdiag, sc_c, p->param_const, radius, min_diag, max_diag, pmode, B.z, p_old,
-      B.x, p_new, B.u, B.q, B.cg);
+      B.x, p_new, B.u, B.q, B.qs, B.cg);
   VGG_LAUNCH_CHECK();
   VGG_PICK_PCG_KERNEL(kern, pcg_schur_kernel, p);
   const int nw = std::min(PS_W, p->S);
   kern<<<(p->N + 31) / 32, nw * 32, 0, st>>>(p->S, p->N, p->uv, p->mask, p->poses, p->intr, p->points, p->point_const,
-                                             M, sc_c, p->param_const, B.u, B.q, fg_tracks, B.cg, ba_loss_of(p));
+                                             M, sc_c, p->param_const, B.u, B.qs, fg_tracks, B.cg, ba_loss_of(p));
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
 
-// One CG iteration i (1-based); iteration i reads p[(i + 1) & 1] and writes p[i & 1].
+// q += qs outside the CG (vgg_dev_pcg_probe: the whole product of one matvec)
+__global__ void pcg_combine_kernel(int D, double* __restrict__ q, const double* __restrict__ qs) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < D) q[i] += qs[i];
+}
+int launch_pcg_combine(int D, double* q, const double* qs, cudaStream_t st) {
+  pcg_combine_kernel<<<(D + 255) / 256, 256, 0, st>>>(D, q, qs);
+  VGG_LAUNCH_CHECK();
+  return VGG_OK;
+}
+
+// One CG iteration i (1-based); iteration i reads p[(i + 1) & 1] and writes p[i & 1].  With a hook, the Schur part qs
+// of each matvec is summed over the ranks before pcg_alpha (or pcg_update after the reset) adds it to q: one hook call
+// per iteration, two on the reset iteration.
 static int pcg_iteration(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
                          const double* M, const double* sc_c, double radius, double min_diag, double max_diag,
                          const vgg_ba_linear_solver& lin, const PcgBuffers& B, double* bvec, const int* fg_tracks,
-                         int i, cudaStream_t st) {
+                         PcgHook hook, int i, cudaStream_t st) {
   int rc;
   const int D = p->S * dc + ns;
   const int nblk = pcg_blocks(p->S, ns);
@@ -819,7 +860,8 @@ static int pcg_iteration(const vgg_ba_problem* p, int dc, int ns, int KR, const 
   if ((rc = launch_pcg_matvec(p, dc, ns, KR, camrec, shared_in, M, sc_c, B.hdiag, radius, min_diag, max_diag, 1, p_old,
                               p_new, B, fg_tracks, st)))
     return rc;
-  pcg_alpha_kernel<<<std::min(132, (D + 255) / 256), 256, 0, st>>>(D, p_new, B.q, B.cg);
+  if (hook.fn && (rc = hook.fn(hook.user, B.qs, (size_t)D, 0, st))) return rc;
+  pcg_alpha_kernel<<<pcg_alpha_ctas(D), 256, 0, st>>>(D, p_new, B.q, B.qs, B.cg, B.slots);
   VGG_LAUNCH_CHECK();
   const bool reset = i % PCG_RESET_PERIOD == 0;
   if (reset) {
@@ -828,20 +870,23 @@ static int pcg_iteration(const vgg_ba_problem* p, int dc, int ns, int KR, const 
     if ((rc = launch_pcg_matvec(p, dc, ns, KR, camrec, shared_in, M, sc_c, B.hdiag, radius, min_diag, max_diag, 0,
                                 nullptr, nullptr, B, fg_tracks, st)))
       return rc;
+    if (hook.fn && (rc = hook.fn(hook.user, B.qs, (size_t)D, 0, st))) return rc;
   }
-  pcg_update_kernel<<<(nblk + 255) / 256, 256, 0, st>>>(p->S, dc, ns, reset ? 1 : 0, B.pinv, bvec, p_new, B.q, B.x, B.r,
-                                                        B.z, lin.eta, lin.min_linear_solver_iterations,
-                                                        lin.max_linear_solver_iterations, B.cg);
+  pcg_update_kernel<<<(nblk + 255) / 256, 256, 0, st>>>(p->S, dc, ns, reset ? 1 : 0, B.pinv, bvec, p_new, B.q, B.qs, B.x,
+                                                        B.r, B.z, lin.eta, lin.min_linear_solver_iterations,
+                                                        lin.max_linear_solver_iterations, B.cg, B.slots);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
 
 // The CG loop after launch_pcg_init: chunks of PCG_CHUNK iterations; the done flag of chunk c is copied to the host
 // behind it and read only after chunk c + 1 has been queued, so the GPU does not wait for the host between chunks.
-// Iterations past the end are kernels that return at once.  The solution is B.x.
+// Iterations past the end are kernels that return at once (and hook calls that sum a vector nobody reads: the done flag
+// is the same on every rank, so every rank queues the same chunks).  The solution is B.x.
 int pcg_run(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
             const double* M, const double* sc_c, double radius, double min_diag, double max_diag,
-            const vgg_ba_linear_solver& lin, const PcgBuffers& B, double* bvec, const int* fg_tracks, cudaStream_t st) {
+            const vgg_ba_linear_solver& lin, const PcgBuffers& B, double* bvec, const int* fg_tracks, PcgHook hook,
+            cudaStream_t st) {
   static thread_local double* h_flag = nullptr;
   static thread_local cudaEvent_t ev[2] = {nullptr, nullptr};
   if (!h_flag) {
@@ -858,7 +903,7 @@ int pcg_run(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camre
   auto queue_chunk = [&](int c) -> int {
     for (int j = 1; j <= PCG_CHUNK; ++j)
       if ((rc = pcg_iteration(p, dc, ns, KR, camrec, shared_in, M, sc_c, radius, min_diag, max_diag, lin, B, bvec,
-                              fg_tracks, c * PCG_CHUNK + j, st)))
+                              fg_tracks, hook, c * PCG_CHUNK + j, st)))
         return rc;
     VGG_CUDA_CHECK(cudaMemcpyAsync(h_flag + (c & 1), B.cg + CG_DONE, sizeof(double), cudaMemcpyDeviceToHost, st));
     VGG_CUDA_CHECK(cudaEventRecord(ev[c & 1], st));
@@ -874,13 +919,12 @@ int pcg_run(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camre
 }
 
 int launch_pcg_model_change(const vgg_ba_problem* p, const double* M, const double* g_p, const double* wacc,
-                            const double* d_c, const int* fg_tracks, double* cg, cudaStream_t st) {
+                            const double* d_c, const int* fg_tracks, double* out, cudaStream_t st) {
   VGG_PICK_PCG_KERNEL(kern, pcg_model_change_kernel, p);
   const int nw = std::min(PS_W, p->S);
-  VGG_CUDA_CHECK(cudaMemsetAsync(cg + CG_MODEL_CHANGE, 0, sizeof(double), st));
+  VGG_CUDA_CHECK(cudaMemsetAsync(out, 0, sizeof(double), st));
   kern<<<(p->N + 31) / 32, nw * 32, 0, st>>>(p->S, p->N, p->uv, p->mask, p->poses, p->intr, p->points, p->point_const,
-                                             M, g_p, wacc, d_c, fg_tracks, cg + CG_MODEL_CHANGE,
-                                             ba_loss_of(p));
+                                             M, g_p, wacc, d_c, fg_tracks, out, ba_loss_of(p));
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }

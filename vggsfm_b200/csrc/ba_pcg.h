@@ -8,24 +8,38 @@ constexpr int PCG_CHUNK = 10;             // CG iterations queued between two re
 constexpr int PCG_RESET_PERIOD = 10;      // Ceres' residual_reset_period: r = b - A x every 10th iteration
 constexpr int PCG_STATE_DOUBLES = 32;
 
-// slots of the CG state (PcgBuffers::cg); [0..4] are what the host reads after each LM iteration
+// slots of the CG state (PcgBuffers::cg); [1..4] are what the host reads after each LM iteration (slot 0 is unused: the
+// model change goes to the small all-reduce of the candidate, launch_pcg_model_change)
 enum : int {
-  CG_MODEL_CHANGE = 0, CG_ITERS = 1, CG_TERM = 2, CG_ZETA = 3, CG_RREL = 4, CG_DONE = 5, CG_RHO = 6, CG_BETA = 7,
+  CG_ITERS = 1, CG_TERM = 2, CG_ZETA = 3, CG_RREL = 4, CG_DONE = 5, CG_RHO = 6, CG_BETA = 7,
   CG_ALPHA = 8, CG_Q0 = 9, CG_BB = 10, CG_PRE_FAIL = 11,
-  CG_ACC = 16,              // [16..19] per-kernel partial sums (reset by the kernel's last CTA)
-  CG_TICKET_SLOT = 24,      // unsigned counter of the kernel's finished CTAs
+  CG_TICKET_SLOT = 24,      // unsigned counter of the kernel's finished CTAs (reset by the last one)
 };
 
-// Device buffers of one solve (all [Dpad] unless noted), carved by make_layout in csrc/ba_solve.cu.
+// Device buffers of one solve (all [Dpad] unless noted), carved by make_layout in csrc/ba_solve.cu.  With track shards
+// the partial sums of a rank are rhs | hdiag | gvec | acc | shared | camrec, carved back to back from `rhs` on:
+// [rhs, rhs + red_doubles) is the one region the all-reduce hook sums once per LM iteration.
 struct PcgBuffers {
   double *rhs, *hdiag, *gvec;   // reduced right-hand side (unscaled), diag(H_cc), camera gradient
+  double *acc;                  // [9 * pcg_blocks]: sum Z_b Z_b^T of the Schur-Jacobi blocks
+  double *shared, *camrec;      // [8], [S * KR]: copy of the camera records (H_cc, g) summed with the above
+  size_t red_doubles;
   double *x, *r, *z, *q, *u;    // CG vectors; u = Dc v, the operand of the Schur part of the matvec
+  double *qs;                   // Schur part of the matvec (summed over the ranks before it joins q)
   double *p[2];                 // search direction, alternating between iterations
-  double *acc, *pinv;           // [9 * pcg_blocks]: sum Z_b Z_b^T, inverted preconditioner blocks
-  double *cg;                   // [PCG_STATE_DOUBLES] scalars, termination and the model change
+  double *pinv;                 // [9 * pcg_blocks]: inverted preconditioner blocks
+  double *cg;                   // [PCG_STATE_DOUBLES] scalars and termination
+  double *slots;                // [pcg_slot_doubles]: per-CTA partials of the fixed-order CG reductions
+};
+
+// the all-reduce hook of a track-sharded solve (fn null: one GPU)
+struct PcgHook {
+  vgg_allreduce_fn fn;
+  void* user;
 };
 
 int pcg_blocks(int S, int ns);
+size_t pcg_slot_doubles(int S, int dc, int ns);
 int launch_pcg_assemble(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
                         const double* M, const double* q, const PcgBuffers& B, const int* fg_tracks, cudaStream_t st);
 int launch_pcg_init(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
@@ -35,10 +49,12 @@ int launch_pcg_matvec(const vgg_ba_problem* p, int dc, int ns, int KR, const dou
                       const double* M, const double* sc_c, const double* hdiag, double radius, double min_diag,
                       double max_diag, int pmode, const double* p_old, double* p_new, const PcgBuffers& B,
                       const int* fg_tracks, cudaStream_t st);
+int launch_pcg_combine(int D, double* q, const double* qs, cudaStream_t st);
 int pcg_run(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
             const double* M, const double* sc_c, double radius, double min_diag, double max_diag,
-            const vgg_ba_linear_solver& lin, const PcgBuffers& B, double* bvec, const int* fg_tracks, cudaStream_t st);
+            const vgg_ba_linear_solver& lin, const PcgBuffers& B, double* bvec, const int* fg_tracks, PcgHook hook,
+            cudaStream_t st);
 int launch_pcg_model_change(const vgg_ba_problem* p, const double* M, const double* g_p, const double* wacc,
-                            const double* d_c, const int* fg_tracks, double* cg, cudaStream_t st);
+                            const double* d_c, const int* fg_tracks, double* out, cudaStream_t st);
 
 }  // namespace vgg

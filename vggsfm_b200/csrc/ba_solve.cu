@@ -67,8 +67,8 @@ int launch_fabric_allreduce(const FabricDev& fd, size_t flags_off, size_t mail_o
 
 // gathers the accept/reject scalars into one 24-double record so the host reads them with ONE copy:
 // [0..7] = scal[0..7], [8..15] = small[0..7], [16] = factorisation info, [17] = substitution info, [18] = camera part of |x|^2
-// (its point part is small[5], summed over the ranks); iterative solves add [20..24] = cg[0..4] (model change, CG
-// iterations, CG termination, zeta, |r| / |b|)
+// (its point part is small[5], summed over the ranks); iterative solves add [20..24] = cg[0..4] (unused, CG iterations,
+// CG termination, zeta, |r| / |b|) and their model change in small[6] (so [14], summed over the ranks)
 __global__ void pack_scalars_kernel(const double* __restrict__ scal, const double* __restrict__ small,
                                     const int* __restrict__ info, const double* __restrict__ cg,
                                     double* __restrict__ out) {
@@ -207,7 +207,8 @@ struct Layout {
 };
 
 // iterative: the layout of vgg_ba_solve_iterative -- the same buffers without the Schur operand Zt, the reduced system
-// AR and the factorisation workspace, plus the O(D) vectors of csrc/ba_pcg.cu
+// AR and the factorisation workspace, plus the O(S + N) buffers of csrc/ba_pcg.cu: its O(D) vectors, the Schur-Jacobi
+// blocks, a copy of the camera records (summed over track shards) and the per-CTA slots of its fixed-order reductions
 static int make_layout(int S, int N, int model, int mode, void* base, size_t cap, Layout* L, bool iterative = false) {
   int dc, ns, KR;
   if (dims_of(model, mode, &dc, &ns, &KR) != VGG_OK) {
@@ -249,11 +250,16 @@ static int make_layout(int S, int N, int model, int mode, void* base, size_t cap
   L->pcg = PcgBuffers{};
   if (iterative) {
     PcgBuffers& B = L->pcg;
-    for (double** v : {&B.rhs, &B.hdiag, &B.gvec, &B.x, &B.r, &B.z, &B.q, &B.u, &B.p[0], &B.p[1]})
-      *v = c.take<double>(L->Dpad);
+    // the region the hook sums once per LM iteration, back to back: rhs | hdiag | gvec | acc | shared | camrec
+    for (double** v : {&B.rhs, &B.hdiag, &B.gvec}) *v = c.take<double>(L->Dpad);
     B.acc = c.take<double>(9 * (size_t)pcg_blocks(S, ns));
+    B.shared = c.take<double>(8);
+    B.camrec = c.take<double>((size_t)S * KR);
+    B.red_doubles = (size_t)(B.camrec + (size_t)S * KR - B.rhs);
+    for (double** v : {&B.x, &B.r, &B.z, &B.q, &B.qs, &B.u, &B.p[0], &B.p[1]}) *v = c.take<double>(L->Dpad);
     B.pinv = c.take<double>(9 * (size_t)pcg_blocks(S, ns));
     B.cg = c.take<double>(PCG_STATE_DOUBLES);
+    B.slots = c.take<double>(pcg_slot_doubles(S, dc, ns));
   }
   L->bytes = align_up(c.off, 256);
   if (base && c.off > cap) {
@@ -533,7 +539,7 @@ using namespace vgg;
 extern "C" {
 
 const char* vgg_last_error(void) { return g_err; }
-int vgg_version(void) { return 101; }
+int vgg_version(void) { return 102; }
 
 void vgg_ba_default_options(vgg_ba_options* o) {
   memset(o, 0, sizeof(*o));
@@ -725,8 +731,9 @@ int vgg_ba_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, void*
 }
 
 // The LM loop of both linear solvers: lin = null solves the reduced camera system directly (DENSE_SCHUR: schur_build,
-// Cholesky, backward substitution), otherwise by PCG (csrc/ba_pcg.cu, ITERATIVE_SCHUR, single GPU: allreduce and
-// fabric null).  Everything else -- point step, camera update, candidate evaluation, accept / reject and the radius
+// Cholesky, backward substitution), otherwise by PCG (csrc/ba_pcg.cu, ITERATIVE_SCHUR: fabric null; with an allreduce
+// hook the assembly is summed once per LM iteration and the Schur part of every matvec once per CG matvec, and the
+// model change joins the candidate's small all-reduce).  Everything else -- point step, camera update, candidate evaluation, accept / reject and the radius
 // rules -- is the same code for both; the iterative solve takes Ceres' model change -(J d)^T (f + J d / 2) instead of
 // the exact-solve identity 0.5 * quad.
 static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, const vgg_ba_linear_solver* lin,
@@ -780,7 +787,10 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
   pe.point_const = L.point_const;
   prob = &pe;
   BandPlan band;
-  if ((rc = compute_band_hint(prob, dc, D, L.Dpad, L.Kpad, allreduce != nullptr || fabric != nullptr, st, &band))) return rc;
+  // the iterative solve factors nothing: each rank's band tables describe its own tracks, which is all its kernels read
+  if ((rc = compute_band_hint(prob, dc, D, L.Dpad, L.Kpad, !lin && (allreduce != nullptr || fabric != nullptr), st,
+                              &band)))
+    return rc;
   g_band_last = band;
   double* Sraw = L.AR;
   double* rhs = L.AR + (size_t)D * L.Dpad;
@@ -821,6 +831,9 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
   VGG_CUDA_CHECK(cudaMemcpyAsync(L.intr[0], prob->intr, sizeof(double) * (size_t)S * 4, cudaMemcpyDeviceToDevice, st));
   VGG_CUDA_CHECK(cudaMemcpyAsync(L.points[0], prob->points, sizeof(double) * (size_t)N * 3, cudaMemcpyDeviceToDevice, st));
   if (!lin) VGG_CUDA_CHECK(cudaMemsetAsync(L.Zt, 0, sizeof(double) * (size_t)L.Kpad * L.Dpad, st));
+  // the padding of the summed region (alignment gaps, rows past D) is never written: zero it once, so the sums over the
+  // ranks add zeros there
+  if (lin) VGG_CUDA_CHECK(cudaMemsetAsync(L.pcg.rhs, 0, sizeof(double) * L.pcg.red_doubles, st));
   VGG_CUDA_CHECK(cudaMemsetAsync(L.d_c, 0, sizeof(double) * L.Dpad, st));
 
   // the problem at state `which` (buffer set of the current state or the candidate)
@@ -921,15 +934,27 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
         return rc;
       if ((rc = launch_pcg_assemble(&pcur, dc, ns, L.KR, b.camrec, b.shared, L.M, L.q, L.pcg, band.dev.fg_tracks, st)))
         return rc;
+      // track shards: the assembly and a copy of the camera records are this rank's partial sums, summed in one call.
+      // The copy, not L.blk[cur] itself: after a rejected step cur is evaluated again and would be summed twice.
+      const double* camrec = b.camrec;
+      const double* shared_in = b.shared;
+      if (allreduce) {
+        VGG_CUDA_CHECK(cudaMemcpyAsync(L.pcg.shared, b.shared, sizeof(double) * 8, cudaMemcpyDeviceToDevice, st));
+        VGG_CUDA_CHECK(cudaMemcpyAsync(L.pcg.camrec, b.camrec, sizeof(double) * (size_t)S * L.KR, cudaMemcpyDeviceToDevice,
+                                       st));
+        if ((rc = allreduce(ar_user, L.pcg.rhs, L.pcg.red_doubles, 0, st))) return rc;
+        camrec = L.pcg.camrec;
+        shared_in = L.pcg.shared;
+      }
       if (!have_scale_c) {
         if ((rc = launch_jacobi_scale_cams(D, hdiag, L.sc_c, opt.jacobi_scaling, st))) return rc;
         have_scale_c = true;
       }
-      if ((rc = launch_pcg_init(&pcur, dc, ns, L.KR, b.camrec, b.shared, L.sc_c, radius, opt.min_lm_diagonal,
+      if ((rc = launch_pcg_init(&pcur, dc, ns, L.KR, camrec, shared_in, L.sc_c, radius, opt.min_lm_diagonal,
                                 opt.max_lm_diagonal, L.pcg, L.bvec, st)))
         return rc;
-      if ((rc = pcg_run(&pcur, dc, ns, L.KR, b.camrec, b.shared, L.M, L.sc_c, radius, opt.min_lm_diagonal,
-                        opt.max_lm_diagonal, *lin, L.pcg, L.bvec, band.dev.fg_tracks, st)))
+      if ((rc = pcg_run(&pcur, dc, ns, L.KR, camrec, shared_in, L.M, L.sc_c, radius, opt.min_lm_diagonal,
+                        opt.max_lm_diagonal, *lin, L.pcg, L.bvec, band.dev.fg_tracks, PcgHook{allreduce, ar_user}, st)))
         return rc;
       dcs = L.pcg.x;
     } else {
@@ -984,11 +1009,13 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
     if ((rc = launch_cam_update(S, dc, ns, prob->camera_model, L.d_c, L.poses[cur], L.intr[cur], L.poses[cand],
                                 L.intr[cand], st)))
       return rc;
-    if (lin && (rc = launch_pcg_model_change(&pcur, L.M, L.blk[cur].g_p, L.wacc, L.d_c, band.dev.fg_tracks, L.pcg.cg, st)))
-      return rc;
     if ((rc = eval(cand))) return rc;
-    // point-side model terms join the candidate cost in the small all-reduce
+    // point-side model terms join the candidate cost in the small all-reduce, and so does the iterative solve's model
+    // change (small[6]: each rank's observations)
     VGG_CUDA_CHECK(cudaMemsetAsync(L.small, 0, sizeof(double) * (8 + (size_t)L.Dpad), st));
+    if (lin && (rc = launch_pcg_model_change(&pcur, L.M, L.blk[cur].g_p, L.wacc, L.d_c, band.dev.fg_tracks, L.small + 6,
+                                             st)))
+      return rc;
     VGG_CUDA_CHECK(cudaMemcpyAsync(L.small, L.blk[cand].cost, sizeof(double), cudaMemcpyDeviceToDevice, st));
     VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + 1, L.scal + 2, sizeof(double) * 2, cudaMemcpyDeviceToDevice, st));
     VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + 3, L.scal + 6, sizeof(double), cudaMemcpyDeviceToDevice, st));
@@ -1020,7 +1047,7 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
     const double c_cost = h_scal[8];
     const double quad = h_scal[0] + h_scal[9];
     const double step_norm = sqrt(h_scal[1] + h_scal[10]);
-    const double model_change = lin ? h_scal[20] : 0.5 * quad;
+    const double model_change = lin ? h_scal[14] : 0.5 * quad;
     if (h_scal[19] != 0.0) {
       set_error("fabric barrier timed out: a peer rank did not arrive");
       return VGG_ECUDA;
@@ -1123,12 +1150,21 @@ int vgg_ba_workspace_bytes_iterative(int S, int N, int camera_model, int intr_mo
 int vgg_ba_solve_iterative(const vgg_ba_problem* prob, const vgg_ba_options* opt, const vgg_ba_linear_solver* lin,
                            void* workspace, size_t ws_bytes, vgg_ba_summary* summary, double* trace, double* cg_trace,
                            void* stream) {
+  return vgg_ba_solve_iterative_sharded(prob, opt, lin, workspace, ws_bytes, nullptr, nullptr, summary, trace, cg_trace,
+                                        stream);
+}
+
+int vgg_ba_solve_iterative_sharded(const vgg_ba_problem* prob, const vgg_ba_options* opt,
+                                   const vgg_ba_linear_solver* lin, void* workspace, size_t ws_bytes,
+                                   vgg_allreduce_fn allreduce, void* allreduce_user, vgg_ba_summary* summary,
+                                   double* trace, double* cg_trace, void* stream) {
   VGG_REQUIRE(lin && lin->type == VGG_BA_ITERATIVE_SCHUR, "vgg_ba_solve_iterative needs lin->type = VGG_BA_ITERATIVE_SCHUR");
   VGG_REQUIRE(lin->min_linear_solver_iterations >= 0 &&
                   lin->max_linear_solver_iterations >= lin->min_linear_solver_iterations && lin->eta > 0.0 &&
                   isfinite(lin->eta),
               "linear solver options: need 0 <= min <= max iterations and a positive finite eta");
-  return lm_solve(prob, opt, lin, workspace, ws_bytes, nullptr, nullptr, nullptr, summary, trace, cg_trace, stream);
+  return lm_solve(prob, opt, lin, workspace, ws_bytes, allreduce, allreduce_user, nullptr, summary, trace, cg_trace,
+                  stream);
 }
 
 /* development probe (csrc/dev_probes.h): the preparation of the iterative solve and one product of its reduced
@@ -1163,6 +1199,7 @@ int vgg_dev_pcg_probe(const vgg_ba_problem* prob, const double* camrec, const do
   if ((rc = launch_pcg_matvec(prob, L.dc, L.ns, L.KR, camrec, shared_in, L.M, L.sc_c, L.pcg.hdiag, radius, min_diag,
                               max_diag, 0, nullptr, nullptr, L.pcg, nullptr, st)))
     return rc;
+  if ((rc = launch_pcg_combine(D, L.pcg.q, L.pcg.qs, st))) return rc;
   auto out = [&](double* dst, const double* src, size_t n) -> int {
     if (dst) VGG_CUDA_CHECK(cudaMemcpyAsync(dst, src, sizeof(double) * n, cudaMemcpyDeviceToDevice, st));
     return VGG_OK;

@@ -6,6 +6,11 @@ and the Schur products are local; the reduced system [D x Dpad | rhs | diag | g]
 ranks once per LM iteration (NCCL over NVLink / NVSwitch), after which every rank factors the same
 small system redundantly and back-substitutes its own points.  A second, tiny all-reduce carries the
 candidate cost and gradient so all ranks take the same accept/reject decision.
+
+With linear_solver_type="ITERATIVE_SCHUR" nothing dense is reduced: AllReduceHook (without a fabric) sums the
+assembled right-hand side, diagonal, gradient, preconditioner accumulators and camera records once per LM iteration and
+one D-vector, the Schur part of the CG's matrix-vector product, per CG iteration; the CG's scalars are fixed-order
+sums of summed data, so every rank takes the same CG decisions and makes the same sequence of hook calls.
 """
 from __future__ import annotations
 

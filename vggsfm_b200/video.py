@@ -88,7 +88,7 @@ def window_bundle_adjustment(window_points_all, extrinsics, intrinsics, extra_pa
 
 def joint_BA(points3D, extrinsics, intrinsics, extra_params, tracks, masks, camera_type="SIMPLE_PINHOLE", reproj_error=2.0,
              tri_angle=1.5, normalize=True, linear_solver_type="DENSE_SCHUR", min_linear_solver_iterations=0,
-             max_linear_solver_iterations=500, eta=0.1):
+             max_linear_solver_iterations=500, eta=0.1, allreduce=None):
     """Tensor form of VideoRunner.joint_BA (video_runner.py:494-541): all frames so far, all points, ONE shared
     camera, default Ceres options through the COLMAP controller (gauge + negative-depth filter + Normalize), then the
     2 px / 1.5 degree point filter and a second normalisation.  The runner keeps this state in its point_dict /
@@ -101,7 +101,9 @@ def joint_BA(points3D, extrinsics, intrinsics, extra_params, tracks, masks, came
     depth per observation, >= 2 survivors, one camera pair with >= tri_angle), which is what COLMAP's
     ObservationManager.filter_all_points3D + filter_observations_with_negative_depth compute [3P-memory].
     linear_solver_type="ITERATIVE_SCHUR" (and the CG options of bundle_adjustment.lm_solve) solves long sequences whose
-    dense reduced camera system does not fit in memory."""
+    dense reduced camera system does not fit in memory.  `allreduce` (vggsfm_b200.dist.AllReduceHook) runs the BA over
+    track shards with either linear solver: every rank passes all frames and its own slice of the points (normalize
+    reads the cameras only, and the point filter is per point, so the rest of the call is the rank's own)."""
     S, P = masks.shape
     K = intrinsics.expand(S, -1, -1)
     ex = extra_params.expand(S, -1) if extra_params is not None else None
@@ -113,7 +115,7 @@ def joint_BA(points3D, extrinsics, intrinsics, extra_params, tracks, masks, came
         pts, poses, K, ex, tracks, masks, shared_camera=True, camera_type=camera_type, options=ba.default_options(),
         filter_reconstruction=False, linear_solver_type=linear_solver_type,
         min_linear_solver_iterations=min_linear_solver_iterations,
-        max_linear_solver_iterations=max_linear_solver_iterations, eta=eta)
+        max_linear_solver_iterations=max_linear_solver_iterations, eta=eta, allreduce=allreduce)
     last_joint_summary = summary
     out = pts.clone()
     out[valid_idx] = pts_o
