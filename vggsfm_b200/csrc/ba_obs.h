@@ -124,3 +124,19 @@ __device__ __forceinline__ double w_entry(const double* jc0, const double* jc1, 
 }
 
 }  // namespace vgg
+
+// the instantiation of a bundle-adjustment kernel template for the problem's camera model and intrinsics mode
+#define VGG_PICK_BA_KERNEL(kern, tmpl, p)                                                          \
+  decltype(&tmpl<0, 0, false>) kern = nullptr;                                                      \
+  {                                                                                                 \
+    const bool robust = (p)->loss_function_type != VGG_LOSS_TRIVIAL;                               \
+    switch ((p)->camera_model * 3 + (p)->intr_mode) {                                               \
+      case 0: kern = robust ? tmpl<0, 0, true> : tmpl<0, 0, false>; break;                           \
+      case 1: kern = robust ? tmpl<0, 1, true> : tmpl<0, 1, false>; break;                           \
+      case 2: kern = robust ? tmpl<0, 2, true> : tmpl<0, 2, false>; break;                           \
+      case 3: kern = robust ? tmpl<1, 0, true> : tmpl<1, 0, false>; break;                           \
+      case 4: kern = robust ? tmpl<1, 1, true> : tmpl<1, 1, false>; break;                           \
+      case 5: kern = robust ? tmpl<1, 2, true> : tmpl<1, 2, false>; break;                           \
+    }                                                                                               \
+  }                                                                                                 \
+  VGG_REQUIRE(kern, "bad camera_model/intr_mode")

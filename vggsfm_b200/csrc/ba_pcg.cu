@@ -767,21 +767,6 @@ __global__ void __launch_bounds__(PS_W * 32) pcg_model_change_kernel(
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-#define VGG_PICK_PCG_KERNEL(kern, tmpl, p)                                                          \
-  decltype(&tmpl<0, 0, false>) kern = nullptr;                                                      \
-  {                                                                                                 \
-    const bool robust = (p)->loss_function_type != VGG_LOSS_TRIVIAL;                               \
-    switch ((p)->camera_model * 3 + (p)->intr_mode) {                                               \
-      case 0: kern = robust ? tmpl<0, 0, true> : tmpl<0, 0, false>; break;                           \
-      case 1: kern = robust ? tmpl<0, 1, true> : tmpl<0, 1, false>; break;                           \
-      case 2: kern = robust ? tmpl<0, 2, true> : tmpl<0, 2, false>; break;                           \
-      case 3: kern = robust ? tmpl<1, 0, true> : tmpl<1, 0, false>; break;                           \
-      case 4: kern = robust ? tmpl<1, 1, true> : tmpl<1, 1, false>; break;                           \
-      case 5: kern = robust ? tmpl<1, 2, true> : tmpl<1, 2, false>; break;                           \
-    }                                                                                               \
-  }                                                                                                 \
-  VGG_REQUIRE(kern, "bad camera_model/intr_mode")
-
 int pcg_blocks(int S, int ns) { return 3 * S + (ns > 0 ? 1 : 0); }
 
 // K partials per CTA of the fixed-order reductions: 3 per CTA of pcg_init / pcg_update, 1 per CTA of pcg_alpha
@@ -790,46 +775,44 @@ size_t pcg_slot_doubles(int S, int dc, int ns) {
   return (size_t)std::max(3 * ((pcg_blocks(S, ns) + 255) / 256), pcg_alpha_ctas(S * dc + ns));
 }
 
-int launch_pcg_assemble(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
-                        const double* M, const double* q, const PcgBuffers& B, const int* fg_tracks, cudaStream_t st) {
-  const int D = p->S * dc + ns;
-  VGG_CUDA_CHECK(cudaMemsetAsync(B.acc, 0, sizeof(double) * 9 * (size_t)pcg_blocks(p->S, ns), st));
-  pcg_hc_kernel<<<(D + 255) / 256, 256, 0, st>>>(p->S, dc, ns, KR, camrec, shared_in, B.rhs, B.hdiag, B.gvec);
+int launch_pcg_assemble(const PcgOp& op, const double* q, const PcgBuffers& B, cudaStream_t st) {
+  const vgg_ba_problem* p = op.p;
+  const int D = p->S * op.dc + op.ns;
+  VGG_CUDA_CHECK(cudaMemsetAsync(B.acc, 0, sizeof(double) * 9 * (size_t)pcg_blocks(p->S, op.ns), st));
+  pcg_hc_kernel<<<(D + 255) / 256, 256, 0, st>>>(p->S, op.dc, op.ns, op.KR, op.camrec, op.shared_in, B.rhs, B.hdiag, B.gvec);
   VGG_LAUNCH_CHECK();
-  VGG_PICK_PCG_KERNEL(kern, pcg_rhs_jacobi_kernel, p);
+  VGG_PICK_BA_KERNEL(kern, pcg_rhs_jacobi_kernel, p);
   const int nw = std::min(PJ_W, (p->S + 31) / 32);
   kern<<<(p->N + PJ_NT - 1) / PJ_NT, nw * 32, 0, st>>>(p->S, p->N, p->uv, p->mask, p->poses, p->intr, p->points,
-                                                        p->point_const, M, q, B.rhs, B.acc, fg_tracks, ba_loss_of(p));
+                                                        p->point_const, op.M, q, B.rhs, B.acc, op.fg_tracks, ba_loss_of(p));
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
 
-int launch_pcg_init(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
-                    const double* sc_c, double radius, double min_diag, double max_diag, const PcgBuffers& B,
-                    double* bvec, cudaStream_t st) {
-  const int nblk = pcg_blocks(p->S, ns);
+int launch_pcg_init(const PcgOp& op, const PcgBuffers& B, double* bvec, cudaStream_t st) {
+  const int S = op.p->S, nblk = pcg_blocks(S, op.ns);
   VGG_CUDA_CHECK(cudaMemsetAsync(B.cg, 0, sizeof(double) * PCG_STATE_DOUBLES, st));
-  pcg_init_kernel<<<(nblk + 255) / 256, 256, 0, st>>>(p->S, dc, ns, KR, camrec, shared_in, B.acc, B.rhs, B.hdiag, sc_c,
-                                                      p->param_const, radius, min_diag, max_diag, B.pinv, bvec, B.x,
-                                                      B.r, B.z, B.cg, B.slots);
+  pcg_init_kernel<<<(nblk + 255) / 256, 256, 0, st>>>(S, op.dc, op.ns, op.KR, op.camrec, op.shared_in, B.acc, B.rhs,
+                                                      B.hdiag, op.sc_c, op.p->param_const, op.radius, op.min_diag,
+                                                      op.max_diag, B.pinv, bvec, B.x, B.r, B.z, B.cg, B.slots);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
 
 // q = A v (pmode: v = z + beta p_old, stored to p_new; otherwise v = x)
-int launch_pcg_matvec(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
-                      const double* M, const double* sc_c, const double* hdiag, double radius, double min_diag,
-                      double max_diag, int pmode, const double* p_old, double* p_new, const PcgBuffers& B,
-                      const int* fg_tracks, cudaStream_t st) {
-  const int nrow = p->S * dc;
-  pcg_hcc_kernel<<<(nrow + 255) / 256 + (ns > 0 ? 1 : 0), 256, 0, st>>>(
-      p->S, dc, ns, KR, camrec, shared_in, hdiag, sc_c, p->param_const, radius, min_diag, max_diag, pmode, B.z, p_old,
-      B.x, p_new, B.u, B.q, B.qs, B.cg);
+int launch_pcg_matvec(const PcgOp& op, int pmode, const double* p_old, double* p_new, const PcgBuffers& B,
+                      cudaStream_t st) {
+  const vgg_ba_problem* p = op.p;
+  const int nrow = p->S * op.dc;
+  pcg_hcc_kernel<<<(nrow + 255) / 256 + (op.ns > 0 ? 1 : 0), 256, 0, st>>>(
+      p->S, op.dc, op.ns, op.KR, op.camrec, op.shared_in, B.hdiag, op.sc_c, p->param_const, op.radius, op.min_diag,
+      op.max_diag, pmode, B.z, p_old, B.x, p_new, B.u, B.q, B.qs, B.cg);
   VGG_LAUNCH_CHECK();
-  VGG_PICK_PCG_KERNEL(kern, pcg_schur_kernel, p);
+  VGG_PICK_BA_KERNEL(kern, pcg_schur_kernel, p);
   const int nw = std::min(PS_W, p->S);
   kern<<<(p->N + 31) / 32, nw * 32, 0, st>>>(p->S, p->N, p->uv, p->mask, p->poses, p->intr, p->points, p->point_const,
-                                             M, sc_c, p->param_const, B.u, B.qs, fg_tracks, B.cg, ba_loss_of(p));
+                                             op.M, op.sc_c, p->param_const, B.u, B.qs, op.fg_tracks, B.cg,
+                                             ba_loss_of(p));
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
@@ -845,35 +828,29 @@ int launch_pcg_combine(int D, double* q, const double* qs, cudaStream_t st) {
   return VGG_OK;
 }
 
-// One CG iteration i (1-based); iteration i reads p[(i + 1) & 1] and writes p[i & 1].  With a hook, the Schur part qs
-// of each matvec is summed over the ranks before pcg_alpha (or pcg_update after the reset) adds it to q: one hook call
-// per iteration, two on the reset iteration.
-static int pcg_iteration(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
-                         const double* M, const double* sc_c, double radius, double min_diag, double max_diag,
-                         const vgg_ba_linear_solver& lin, const PcgBuffers& B, double* bvec, const int* fg_tracks,
-                         PcgHook hook, int i, cudaStream_t st) {
+// One CG iteration i (1-based); iteration i reads p[(i + 1) & 1] and writes p[i & 1].  With track shards, the Schur
+// part qs of each matvec is summed over the ranks before pcg_alpha (or pcg_update after the reset) adds it to q: one
+// reduction per iteration, two on the reset iteration.
+static int pcg_iteration(const PcgOp& op, const vgg_ba_linear_solver& lin, const PcgBuffers& B, double* bvec,
+                         const Ranks& ranks, int i, cudaStream_t st) {
   int rc;
-  const int D = p->S * dc + ns;
-  const int nblk = pcg_blocks(p->S, ns);
+  const int S = op.p->S, D = S * op.dc + op.ns;
+  const int nblk = pcg_blocks(S, op.ns);
   double* p_new = B.p[i & 1];
   const double* p_old = B.p[(i + 1) & 1];
-  if ((rc = launch_pcg_matvec(p, dc, ns, KR, camrec, shared_in, M, sc_c, B.hdiag, radius, min_diag, max_diag, 1, p_old,
-                              p_new, B, fg_tracks, st)))
-    return rc;
-  if (hook.fn && (rc = hook.fn(hook.user, B.qs, (size_t)D, 0, st))) return rc;
+  if ((rc = launch_pcg_matvec(op, 1, p_old, p_new, B, st))) return rc;
+  if ((rc = ranks.sum(B.qs, (size_t)D))) return rc;
   pcg_alpha_kernel<<<pcg_alpha_ctas(D), 256, 0, st>>>(D, p_new, B.q, B.qs, B.cg, B.slots);
   VGG_LAUNCH_CHECK();
   const bool reset = i % PCG_RESET_PERIOD == 0;
   if (reset) {
     pcg_xstep_kernel<<<(D + 255) / 256, 256, 0, st>>>(D, p_new, B.x, B.cg);
     VGG_LAUNCH_CHECK();
-    if ((rc = launch_pcg_matvec(p, dc, ns, KR, camrec, shared_in, M, sc_c, B.hdiag, radius, min_diag, max_diag, 0,
-                                nullptr, nullptr, B, fg_tracks, st)))
-      return rc;
-    if (hook.fn && (rc = hook.fn(hook.user, B.qs, (size_t)D, 0, st))) return rc;
+    if ((rc = launch_pcg_matvec(op, 0, nullptr, nullptr, B, st))) return rc;
+    if ((rc = ranks.sum(B.qs, (size_t)D))) return rc;
   }
-  pcg_update_kernel<<<(nblk + 255) / 256, 256, 0, st>>>(p->S, dc, ns, reset ? 1 : 0, B.pinv, bvec, p_new, B.q, B.qs, B.x,
-                                                        B.r, B.z, lin.eta, lin.min_linear_solver_iterations,
+  pcg_update_kernel<<<(nblk + 255) / 256, 256, 0, st>>>(S, op.dc, op.ns, reset ? 1 : 0, B.pinv, bvec, p_new, B.q, B.qs,
+                                                        B.x, B.r, B.z, lin.eta, lin.min_linear_solver_iterations,
                                                         lin.max_linear_solver_iterations, B.cg, B.slots);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
@@ -881,11 +858,9 @@ static int pcg_iteration(const vgg_ba_problem* p, int dc, int ns, int KR, const 
 
 // The CG loop after launch_pcg_init: chunks of PCG_CHUNK iterations; the done flag of chunk c is copied to the host
 // behind it and read only after chunk c + 1 has been queued, so the GPU does not wait for the host between chunks.
-// Iterations past the end are kernels that return at once (and hook calls that sum a vector nobody reads: the done flag
-// is the same on every rank, so every rank queues the same chunks).  The solution is B.x.
-int pcg_run(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
-            const double* M, const double* sc_c, double radius, double min_diag, double max_diag,
-            const vgg_ba_linear_solver& lin, const PcgBuffers& B, double* bvec, const int* fg_tracks, PcgHook hook,
+// Iterations past the end are kernels that return at once (and reductions of a vector nobody reads: the done flag is
+// the same on every rank, so every rank queues the same chunks).  The solution is B.x.
+int pcg_run(const PcgOp& op, const vgg_ba_linear_solver& lin, const PcgBuffers& B, double* bvec, const Ranks& ranks,
             cudaStream_t st) {
   static thread_local double* h_flag = nullptr;
   static thread_local cudaEvent_t ev[2] = {nullptr, nullptr};
@@ -894,17 +869,16 @@ int pcg_run(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camre
     VGG_CUDA_CHECK(cudaEventCreateWithFlags(&ev[0], cudaEventDisableTiming));
     VGG_CUDA_CHECK(cudaEventCreateWithFlags(&ev[1], cudaEventDisableTiming));
   }
-  VGG_CUDA_CHECK(cudaMemsetAsync(B.p[0], 0, sizeof(double) * (size_t)(p->S * dc + ns), st));
-  VGG_CUDA_CHECK(cudaMemsetAsync(B.p[1], 0, sizeof(double) * (size_t)(p->S * dc + ns), st));
+  const size_t D = (size_t)(op.p->S * op.dc + op.ns);
+  VGG_CUDA_CHECK(cudaMemsetAsync(B.p[0], 0, sizeof(double) * D, st));
+  VGG_CUDA_CHECK(cudaMemsetAsync(B.p[1], 0, sizeof(double) * D, st));
   // Ceres' loop runs its first iteration before it tests max_num_iterations
   const int max_it = std::max(1, lin.max_linear_solver_iterations);
   const int nchunks = (max_it + PCG_CHUNK - 1) / PCG_CHUNK;
   int rc;
   auto queue_chunk = [&](int c) -> int {
     for (int j = 1; j <= PCG_CHUNK; ++j)
-      if ((rc = pcg_iteration(p, dc, ns, KR, camrec, shared_in, M, sc_c, radius, min_diag, max_diag, lin, B, bvec,
-                              fg_tracks, hook, c * PCG_CHUNK + j, st)))
-        return rc;
+      if ((rc = pcg_iteration(op, lin, B, bvec, ranks, c * PCG_CHUNK + j, st))) return rc;
     VGG_CUDA_CHECK(cudaMemcpyAsync(h_flag + (c & 1), B.cg + CG_DONE, sizeof(double), cudaMemcpyDeviceToHost, st));
     VGG_CUDA_CHECK(cudaEventRecord(ev[c & 1], st));
     return VGG_OK;
@@ -920,7 +894,7 @@ int pcg_run(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camre
 
 int launch_pcg_model_change(const vgg_ba_problem* p, const double* M, const double* g_p, const double* wacc,
                             const double* d_c, const int* fg_tracks, double* out, cudaStream_t st) {
-  VGG_PICK_PCG_KERNEL(kern, pcg_model_change_kernel, p);
+  VGG_PICK_BA_KERNEL(kern, pcg_model_change_kernel, p);
   const int nw = std::min(PS_W, p->S);
   VGG_CUDA_CHECK(cudaMemsetAsync(out, 0, sizeof(double), st));
   kern<<<(p->N + 31) / 32, nw * 32, 0, st>>>(p->S, p->N, p->uv, p->mask, p->poses, p->intr, p->points, p->point_const,

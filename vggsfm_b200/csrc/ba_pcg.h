@@ -1,6 +1,6 @@
 // The iterative (PCG) linear solver of the LM loop, csrc/ba_pcg.cu; used by csrc/ba_solve.cu.
 #pragma once
-#include "common.cuh"
+#include "ba_lm.h"
 
 namespace vgg {
 
@@ -32,27 +32,23 @@ struct PcgBuffers {
   double *slots;                // [pcg_slot_doubles]: per-CTA partials of the fixed-order CG reductions
 };
 
-// the all-reduce hook of a track-sharded solve (fn null: one GPU)
-struct PcgHook {
-  vgg_allreduce_fn fn;
-  void* user;
+// the reduced operator of one LM iteration: the state, its camera records, point blocks M, camera scales and damping
+struct PcgOp {
+  const vgg_ba_problem* p;
+  int dc, ns, KR;
+  const double *camrec, *shared_in, *M, *sc_c;
+  double radius, min_diag, max_diag;
+  const int* fg_tracks;
 };
 
 int pcg_blocks(int S, int ns);
 size_t pcg_slot_doubles(int S, int dc, int ns);
-int launch_pcg_assemble(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
-                        const double* M, const double* q, const PcgBuffers& B, const int* fg_tracks, cudaStream_t st);
-int launch_pcg_init(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
-                    const double* sc_c, double radius, double min_diag, double max_diag, const PcgBuffers& B,
-                    double* bvec, cudaStream_t st);
-int launch_pcg_matvec(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
-                      const double* M, const double* sc_c, const double* hdiag, double radius, double min_diag,
-                      double max_diag, int pmode, const double* p_old, double* p_new, const PcgBuffers& B,
-                      const int* fg_tracks, cudaStream_t st);
+int launch_pcg_assemble(const PcgOp& op, const double* q, const PcgBuffers& B, cudaStream_t st);
+int launch_pcg_init(const PcgOp& op, const PcgBuffers& B, double* bvec, cudaStream_t st);
+int launch_pcg_matvec(const PcgOp& op, int pmode, const double* p_old, double* p_new, const PcgBuffers& B,
+                      cudaStream_t st);
 int launch_pcg_combine(int D, double* q, const double* qs, cudaStream_t st);
-int pcg_run(const vgg_ba_problem* p, int dc, int ns, int KR, const double* camrec, const double* shared_in,
-            const double* M, const double* sc_c, double radius, double min_diag, double max_diag,
-            const vgg_ba_linear_solver& lin, const PcgBuffers& B, double* bvec, const int* fg_tracks, PcgHook hook,
+int pcg_run(const PcgOp& op, const vgg_ba_linear_solver& lin, const PcgBuffers& B, double* bvec, const Ranks& ranks,
             cudaStream_t st);
 int launch_pcg_model_change(const vgg_ba_problem* p, const double* M, const double* g_p, const double* wacc,
                             const double* d_c, const int* fg_tracks, double* out, cudaStream_t st);

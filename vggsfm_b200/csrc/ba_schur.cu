@@ -15,6 +15,7 @@
 #include <stddef.h>
 #include <algorithm>
 #include <vector>
+#include "ba_lm.h"
 #include "ba_obs.h"
 #include "common.cuh"
 #include "dev_probes.h"
@@ -88,7 +89,7 @@ __global__ void point_prep_kernel(int N, const double* __restrict__ H_pp, const 
   bad = bad || !(t22 > 0.0);
   const double l22 = sqrt(t22);
   if (bad) {
-    atomicAdd(&scal[6], 1.0);
+    atomicAdd(&scal[SCAL_PT_FAIL], 1.0);
 #pragma unroll
     for (int i = 0; i < 9; ++i) Mo[i] = 0.0;
     q[n * 3] = q[n * 3 + 1] = q[n * 3 + 2] = 0.0;
@@ -436,7 +437,7 @@ __global__ void scale_damp_kernel(int D, int Dpad, double* __restrict__ A, const
   }
 }
 
-// d_c = sc * dcs ; scal[0] += sum dcs^2 dcc/r (free) - d_c.g ; scal[1] += |d_c|^2 ; scal[7] non-finite flag
+// d_c = sc * dcs ; the camera slots of scal (csrc/ba_lm.h): the model term, |d_c|^2 and the non-finite count
 __global__ void cam_step_kernel(int D, const double* __restrict__ dcs, size_t dcs_stride, const double* __restrict__ sc,
                                 const double* __restrict__ hdiag, const double* __restrict__ gvec,
                                 const uint8_t* __restrict__ pconst, double radius, double min_diag, double max_diag,
@@ -454,9 +455,9 @@ __global__ void cam_step_kernel(int D, const double* __restrict__ dcs, size_t dc
   }
   a = warp_sum(a); b = warp_sum(b); bad = warp_sum(bad);
   if ((threadIdx.x & 31) == 0) {
-    atomicAdd(&scal[0], a);
-    atomicAdd(&scal[1], b);
-    if (bad > 0) atomicAdd(&scal[7], bad);
+    atomicAdd(&scal[SCAL_CAM_QUAD], a);
+    atomicAdd(&scal[SCAL_CAM_STEP2], b);
+    if (bad > 0) atomicAdd(&scal[SCAL_CAM_BAD], bad);
   }
 }
 
@@ -529,10 +530,10 @@ __global__ void __launch_bounds__(BS_W * 32) backsub_kernel(
   }
 }
 
-// d_p = M M^T (-(g_p + w)); candidate = X + d_p; scal[2] += sum dps^2 dpp/r - d_p.g_p; scal[3] += |d_p|^2.  A constant
-// point (point_const: given constant, or seen by no valid observation) is SELECTED out: its step and both terms are
-// exact zeros and its candidate is X bit for bit, whatever wacc, g_p and sc_p hold for it (M = 0 alone would give
-// 0 * NaN = NaN for a point whose coordinates are not in the problem).
+// d_p = M M^T (-(g_p + w)); candidate = X + d_p; scal[SCAL_PT_QUAD] += sum dps^2 dpp/r - d_p.g_p,
+// scal[SCAL_PT_STEP2] += |d_p|^2.  A constant point (point_const: given constant, or seen by no valid observation) is
+// SELECTED out: its step and both terms are exact zeros and its candidate is X bit for bit, whatever wacc, g_p and sc_p
+// hold for it (M = 0 alone would give 0 * NaN = NaN for a point whose coordinates are not in the problem).
 __global__ void point_step_kernel(int N, const double* __restrict__ M, const double* __restrict__ g_p,
                                   const double* __restrict__ wacc, const double* __restrict__ sc_p,
                                   const double* __restrict__ dpp, const uint8_t* __restrict__ point_const,
@@ -563,8 +564,8 @@ __global__ void point_step_kernel(int N, const double* __restrict__ M, const dou
   }
   a = warp_sum(a); b = warp_sum(b);
   if ((threadIdx.x & 31) == 0) {
-    atomicAdd(&scal[2], a);
-    atomicAdd(&scal[3], b);
+    atomicAdd(&scal[SCAL_PT_QUAD], a);
+    atomicAdd(&scal[SCAL_PT_STEP2], b);
   }
 }
 
@@ -626,9 +627,9 @@ __global__ void extract_gvec_kernel(int S, int dc, int ns, int KR, const double*
   gvec[i] = (i < S * dc) ? camrec[(size_t)(i / dc) * KR + (i % dc)] : shared_in[i - S * dc];
 }
 
-// scal[4] = max |gvec| over free parameters, scal[5] = max |g_p| over variable points.  The maximum is taken over the
-// bit patterns: non-negative doubles order like them, and fabs(NaN) is a positive NaN, which orders above +inf -- so a
-// NaN gradient entry gives a NaN max-norm (that never passes gradient_tolerance) where fmax would drop it.
+// scal[SCAL_GMAX_C] = max |gvec| over free parameters, scal[SCAL_GMAX_P] = max |g_p| over variable points, taken over
+// the bit patterns: non-negative doubles order like them, and fabs(NaN) is a positive NaN, which orders above +inf --
+// so a NaN gradient entry gives a NaN max-norm (that never passes gradient_tolerance) where fmax would drop it.
 __global__ void gradmax_kernel(int D, int N, const double* __restrict__ gvec, const uint8_t* __restrict__ pconst,
                                const double* __restrict__ g_p, const uint8_t* __restrict__ point_const,
                                double* __restrict__ scal) {
@@ -642,8 +643,8 @@ __global__ void gradmax_kernel(int D, int N, const double* __restrict__ gvec, co
     mp = max(mp, __shfl_xor_sync(0xffffffffu, mp, off));
   }
   if ((threadIdx.x & 31) == 0) {
-    atomicMax(reinterpret_cast<unsigned long long*>(&scal[4]), mc);
-    atomicMax(reinterpret_cast<unsigned long long*>(&scal[5]), mp);
+    atomicMax(reinterpret_cast<unsigned long long*>(&scal[SCAL_GMAX_C]), mc);
+    atomicMax(reinterpret_cast<unsigned long long*>(&scal[SCAL_GMAX_P]), mp);
   }
 }
 
@@ -675,22 +676,6 @@ int launch_assemble_hc(int S, int dc, int ns, int KR, int Dpad, const double* ca
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }
-// the instantiation of a bundle-adjustment kernel template for the problem's camera model and intrinsics mode
-#define VGG_PICK_BA_KERNEL(kern, tmpl, p)                                                          \
-  decltype(&tmpl<0, 0, false>) kern = nullptr;                                                      \
-  {                                                                                                 \
-    const bool robust = (p)->loss_function_type != VGG_LOSS_TRIVIAL;                               \
-    switch ((p)->camera_model * 3 + (p)->intr_mode) {                                               \
-      case 0: kern = robust ? tmpl<0, 0, true> : tmpl<0, 0, false>; break;                           \
-      case 1: kern = robust ? tmpl<0, 1, true> : tmpl<0, 1, false>; break;                           \
-      case 2: kern = robust ? tmpl<0, 2, true> : tmpl<0, 2, false>; break;                           \
-      case 3: kern = robust ? tmpl<1, 0, true> : tmpl<1, 0, false>; break;                           \
-      case 4: kern = robust ? tmpl<1, 1, true> : tmpl<1, 1, false>; break;                           \
-      case 5: kern = robust ? tmpl<1, 2, true> : tmpl<1, 2, false>; break;                           \
-    }                                                                                               \
-  }                                                                                                 \
-  VGG_REQUIRE(kern, "bad camera_model/intr_mode")
-
 int launch_z_build(const vgg_ba_problem* p, int Dpad, const double* M, const double* q, double* Zt, double* rhs,
                    ptrdiff_t mc_off, const int* fg_tracks, cudaStream_t st) {
   VGG_PICK_BA_KERNEL(kern, z_build_kernel, p);

@@ -8,6 +8,7 @@
 #include <string.h>
 #include <map>
 #include <vector>
+#include "ba_lm.h"
 #include "ba_pcg.h"
 #include "common.cuh"
 #include "dev_probes.h"
@@ -65,20 +66,17 @@ int launch_fabric_gather(const FabricDev& fd, int nrows, int nmat, int ncols_vec
 int launch_fabric_allreduce(const FabricDev& fd, size_t flags_off, size_t mail_off, int mail_len, int parity,
                             unsigned long long epoch, double* vec, int count, int max_slot, int* err, cudaStream_t st);
 
-// gathers the accept/reject scalars into one 24-double record so the host reads them with ONE copy:
-// [0..7] = scal[0..7], [8..15] = small[0..7], [16] = factorisation info, [17] = substitution info, [18] = camera part of |x|^2
-// (its point part is small[5], summed over the ranks); iterative solves add [20..24] = cg[0..4] (unused, CG iterations,
-// CG termination, zeta, |r| / |b|) and their model change in small[6] (so [14], summed over the ranks)
+// gathers the accept/reject scalars into one record (csrc/ba_lm.h) so the host reads them with ONE copy
 __global__ void pack_scalars_kernel(const double* __restrict__ scal, const double* __restrict__ small,
                                     const int* __restrict__ info, const double* __restrict__ cg,
                                     double* __restrict__ out) {
   const int i = threadIdx.x;
-  if (i < 8) out[i] = scal[i];
-  else if (i < 16) out[i] = small[i - 8];
-  else if (i < 18) out[i] = (double)info[i - 16];
-  else if (i == 18) out[i] = scal[8];              // camera part of |x|^2 (xnorm_kernel), 0 unless parameter_tolerance > 0
-  else if (i == 19) out[i] = (double)info[2];      // a cross-rank barrier of csrc/fabric.cu timed out
-  else if (i < 25 && cg) out[i] = cg[i - 20];
+  if (i < VGG_REC(small)) out[i] = scal[i];
+  else if (i < VGG_REC(chol_info)) out[i] = small[i - VGG_REC(small)];
+  else if (i <= VGG_REC(trsv_info)) out[i] = (double)info[i - VGG_REC(chol_info)];   // INFO_CHOL, INFO_TRSV
+  else if (i == VGG_REC(xnorm_c)) out[i] = scal[SCAL_XNORM_C];
+  else if (i == VGG_REC(fabric_timeout)) out[i] = (double)info[INFO_FABRIC];
+  else if (i < (int)(sizeof(LmRecord) / sizeof(double)) && cg) out[i] = cg[i - VGG_REC(cg)];
 }
 
 // |x|^2 of Ceres' reduced program in ambient coordinates (ParameterToleranceReached: step_norm <= tol * (|x| + tol)):
@@ -144,14 +142,13 @@ struct EventPair {
   }
 };
 
-// max of the camera and point gradient max-norms; a NaN in either (gradmax_kernel keeps them) stays NaN, so that a NaN
-// gradient is never taken for convergence
-static double grad_max_norm(double gc, double gp) { return isnan(gc) || isnan(gp) ? NAN : fmax(gc, gp); }
-
 static double* pinned_scalars() {
   static thread_local double* h = nullptr;
   if (!h) {
-    if (cudaHostAlloc(reinterpret_cast<void**>(&h), sizeof(double) * 32, cudaHostAllocDefault) != cudaSuccess) h = nullptr;
+    if (cudaHostAlloc(reinterpret_cast<void**>(&h), sizeof(double) * REC_CAP, cudaHostAllocDefault) != cudaSuccess) {
+      h = nullptr;
+      set_error("cudaHostAlloc for the scalar read-back failed");
+    }
   }
   return h;
 }
@@ -168,17 +165,21 @@ static int check_loss(const vgg_ba_problem* p) {
   return VGG_OK;
 }
 
-static int dims_of(int model, int mode, int* dc, int* ns, int* KR) {
-  if (model != VGG_SIMPLE_PINHOLE && model != VGG_SIMPLE_RADIAL) return VGG_EINVAL;
+// sizes of S frames and N points; Dpad leaves >= 2 spare slots after D (row D: the bordered right-hand side)
+struct Dims {
+  int dc, ns, KR, D, Dpad, Kpad;
+};
+static int dims_of(int model, int mode, int S, int N, Dims* d) {
+  VGG_REQUIRE((model == VGG_SIMPLE_PINHOLE || model == VGG_SIMPLE_RADIAL) &&
+                  (mode == VGG_INTR_CONST || mode == VGG_INTR_PER_FRAME || mode == VGG_INTR_SHARED),
+              "bad camera_model/intr_mode");
   const int ni = model == VGG_SIMPLE_PINHOLE ? 1 : 2;
-  int d, n;
-  if (mode == VGG_INTR_CONST) { d = 6; n = 0; }
-  else if (mode == VGG_INTR_PER_FRAME) { d = 6 + ni; n = 0; }
-  else if (mode == VGG_INTR_SHARED) { d = 6; n = ni; }
-  else return VGG_EINVAL;
-  if (dc) *dc = d;
-  if (ns) *ns = n;
-  if (KR) *KR = d + d * (d + 1) / 2 + 6 * n;
+  d->dc = mode == VGG_INTR_PER_FRAME ? 6 + ni : 6;
+  d->ns = mode == VGG_INTR_SHARED ? ni : 0;
+  d->KR = d->dc + d->dc * (d->dc + 1) / 2 + 6 * d->ns;
+  d->D = S * d->dc + d->ns;
+  d->Dpad = (int)align_up((size_t)d->D + 2, 128);
+  d->Kpad = (int)align_up((size_t)3 * N, 16);
   return VGG_OK;
 }
 
@@ -190,15 +191,15 @@ static int dims_of(int model, int mode, int* dc, int* ns, int* KR) {
 struct BlockSet {
   double *cost, *camrec, *g_p, *H_pp, *shared;
 };
-struct Layout {
-  int S, N, dc, ns, KR, D, Dpad, Kpad;
+struct Layout : Dims {
+  int S, N;
   BlockSet blk[2];
   double *poses[2], *intr[2], *points[2];
   double *sc_c, *sc_p, *M, *q, *dpp, *wacc, *d_c, *bvec, *Zt;
-  double *AR;        // [D*Dpad | rhs Dpad | hdiag Dpad | gvec Dpad]  (one all-reduce)
-  double *small;     // [8 scalars | gvec_candidate Dpad]           (one small all-reduce)
-  double *scal;      // [16]
-  double *packed;    // [24] scalars gathered for the host
+  double *AR;        // the reduced system (reduced_view)
+  double *small;     // [SMALL_VEC + Dpad]: the candidate's all-reduce (csrc/ba_lm.h)
+  double *scal;      // [SCAL_DOUBLES]
+  double *packed;    // [REC_CAP]: the record the host reads
   double *chol_diag;
   int *dev_info;
   uint8_t *pconst, *point_const;   // [Dpad], [N]: the solve's constant flags (observed_kernel / effective_const_kernel)
@@ -210,15 +211,10 @@ struct Layout {
 // AR and the factorisation workspace, plus the O(S + N) buffers of csrc/ba_pcg.cu: its O(D) vectors, the Schur-Jacobi
 // blocks, a copy of the camera records (summed over track shards) and the per-CTA slots of its fixed-order reductions
 static int make_layout(int S, int N, int model, int mode, void* base, size_t cap, Layout* L, bool iterative = false) {
-  int dc, ns, KR;
-  if (dims_of(model, mode, &dc, &ns, &KR) != VGG_OK) {
-    set_error("bad camera_model/intr_mode");
-    return VGG_EINVAL;
-  }
-  L->S = S; L->N = N; L->dc = dc; L->ns = ns; L->KR = KR;
-  L->D = S * dc + ns;
-  L->Dpad = (int)align_up((size_t)L->D + 2, 128);      // >= 2 spare slots after D (row D: the bordered right-hand side)
-  L->Kpad = (int)align_up((size_t)3 * N, 16);
+  if (const int rc = dims_of(model, mode, S, N, L)) return rc;
+  const int KR = L->KR, dc = L->dc, ns = L->ns;
+  L->S = S;
+  L->N = N;
   Carver c(base, cap);
   for (int b = 0; b < 2; ++b) {
     L->blk[b].cost = c.take<double>(8);
@@ -239,12 +235,12 @@ static int make_layout(int S, int N, int model, int mode, void* base, size_t cap
   L->d_c = c.take<double>(L->Dpad);
   L->bvec = c.take<double>(L->Dpad);
   L->Zt = iterative ? nullptr : c.take<double>((size_t)L->Kpad * L->Dpad);
-  L->AR = iterative ? nullptr : c.take<double>((size_t)L->D * L->Dpad + 3 * (size_t)L->Dpad);
-  L->small = c.take<double>(8 + (size_t)L->Dpad);
-  L->scal = c.take<double>(16);
-  L->packed = c.take<double>(32);
+  L->AR = iterative ? nullptr : c.take<double>(reduced_doubles(L->D, L->Dpad));
+  L->small = c.take<double>(SMALL_VEC + (size_t)L->Dpad);
+  L->scal = c.take<double>(SCAL_DOUBLES);
+  L->packed = c.take<double>(REC_CAP);
   L->chol_diag = iterative ? nullptr : c.take<double>(chol_workspace_doubles(L->D + 1));
-  L->dev_info = c.take<int>(4);
+  L->dev_info = c.take<int>(INFO_INTS);
   L->pconst = c.take<uint8_t>(L->Dpad);
   L->point_const = c.take<uint8_t>((size_t)N);
   L->pcg = PcgBuffers{};
@@ -286,7 +282,7 @@ struct FabricLayout {
 };
 static FabricLayout fabric_layout(int D, int Dpad) {
   FabricLayout f;
-  f.arc = align_up((size_t)D * Dpad + 3 * (size_t)Dpad, 256);
+  f.arc = align_up(reduced_doubles(D, Dpad), 256);
   f.mail_len = Dpad + 64;
   f.mail_off = 2 * f.arc;
   f.flags_off = align_up(f.mail_off + (size_t)2 * 8 * f.mail_len, 32);
@@ -297,9 +293,10 @@ static FabricLayout fabric_layout(int D, int Dpad) {
 // Run-time state of the fabric (csrc/fabric.cu): reduce-scatter + gather of the reduced system, in-kernel barriers and
 // small all-reduces -- no NCCL call and no host callback inside the LM loop.
 struct Fabric {
-  bool on = false;
   FabricDev base{};                 // peer[r] = base of rank r's symmetric allocation
   FabricLayout lay{};
+  double* ar_local = nullptr;       // this rank's copy of the symmetric allocation
+  ptrdiff_t mc_off = 0;             // multicast twin of a local address, minus the address
   unsigned long long* epoch = nullptr;
   int small_parity = 0;
   int* err = nullptr;
@@ -315,6 +312,28 @@ struct Fabric {
                                    max_slot, err, st);
   }
 };
+
+int Ranks::sum(double* vec, size_t count) const {
+  if (fab) return fab->allreduce(vec, (int)count, -1, st);
+  return fn ? fn(user, vec, count, 0, st) : VGG_OK;
+}
+int Ranks::max(double* slot) const {
+  if (fab) return fab->allreduce(slot, 1, 0, st);
+  return fn ? fn(user, slot, 1, 1, st) : VGG_OK;
+}
+template <class Gradmax>
+int Ranks::candidate(double* small, size_t count, double* scal, Gradmax gradmax) const {
+  int rc;
+  if (!fab) return (rc = sum(small, count)) || (rc = gradmax()) ? rc : max(scal + SCAL_GMAX_P);
+  // one in-kernel all-reduce: the point-gradient max rides in its max slot; the camera max is taken from the sum
+  if ((rc = gradmax())) return rc;
+  VGG_CUDA_CHECK(cudaMemcpyAsync(small + SMALL_GMAX_P, scal + SCAL_GMAX_P, sizeof(double), cudaMemcpyDeviceToDevice, st));
+  if ((rc = fab->allreduce(small, (int)count, SMALL_GMAX_P, st))) return rc;
+  VGG_CUDA_CHECK(cudaMemsetAsync(scal + SCAL_GMAX_C, 0, sizeof(double) * 2, st));
+  if ((rc = gradmax())) return rc;
+  VGG_CUDA_CHECK(cudaMemcpyAsync(scal + SCAL_GMAX_P, small + SMALL_GMAX_P, sizeof(double), cudaMemcpyDeviceToDevice, st));
+  return VGG_OK;
+}
 
 // The band structure of one solve (compute_band_hint), passed to the launchers that use it; empty / null = dense.
 //   kb_ranges             SYRK k-block range per 128-column row block of Zt (launch_syrk)
@@ -505,30 +524,56 @@ static int compute_band_hint(const vgg_ba_problem* prob, int dc, int D, int Dpad
   return VGG_OK;
 }
 
-// Schur complement of blk onto AR (Sraw, rhs, hdiag, gvec) at the given radius; p: the problem at the state blk was
-// evaluated at (z_build rebuilds the coupling blocks from it); fd: where the SYRK epilogue sends each row block in a
-// fabric solve, fab: that solve's fabric (null otherwise); syrk = false stops after z_build (vgg_dev_schur_build with
-// Zt filled with a NaN sentinel: the SYRK adds every non-zero product, so sentinels left in the padding columns
-// [D, Dpad) would send it past the reduced system's rows)
-static int schur_build(const Layout& L, const vgg_ba_problem& p, const BlockSet& b, const BandPlan& band,
-                       const FabricDev& fd, double radius, double min_diag, double max_diag, cudaStream_t st,
-                       ptrdiff_t mc_off = 0, Fabric* fab = nullptr, bool syrk = true) {
+// Schur complement of blk onto the reduced system R at the given radius; p: the problem at the state blk was evaluated
+// at (z_build rebuilds the coupling blocks from it); fd: where the SYRK epilogue sends each row block in a fabric solve,
+// fab: that solve's fabric (null otherwise); syrk = false stops after z_build (vgg_dev_schur_build with Zt filled with a
+// NaN sentinel: the SYRK adds every non-zero product, so sentinels left in the padding columns [D, Dpad) would send it
+// past the reduced system's rows)
+static int schur_build(const Layout& L, const Reduced& R, const vgg_ba_problem& p, const BlockSet& b,
+                       const BandPlan& band, const FabricDev& fd, double radius, double min_diag, double max_diag,
+                       cudaStream_t st, Fabric* fab = nullptr, bool syrk = true) {
   int rc;
-  double* Sraw = L.AR;
-  double* rhs = L.AR + (size_t)L.D * L.Dpad;
-  double* hdiag = rhs + L.Dpad;
-  double* gvec = hdiag + L.Dpad;
+  const ptrdiff_t mc_off = fab ? fab->mc_off : 0;
   if ((rc = launch_point_prep(L.N, b.H_pp, b.g_p, L.sc_p, p.point_const, radius, min_diag, max_diag, L.M, L.q, L.dpp,
                               L.scal, st)))
     return rc;
-  VGG_CUDA_CHECK(cudaMemsetAsync(L.AR, 0, sizeof(double) * ((size_t)L.D * L.Dpad + 3 * (size_t)L.Dpad), st));
+  VGG_CUDA_CHECK(cudaMemsetAsync(R.S, 0, sizeof(double) * reduced_doubles(L.D, L.Dpad), st));
   // fabric mode: every rank's copy must be zero before anyone's reductions land in it
   if (fab && (rc = fab->barrier(st))) return rc;
-  if ((rc = launch_assemble_hc(L.S, L.dc, L.ns, L.KR, L.Dpad, b.camrec, b.shared, Sraw, rhs, hdiag, gvec, mc_off, st))) return rc;
-  if ((rc = launch_z_build(&p, L.Dpad, L.M, L.q, L.Zt, rhs, mc_off, band.dev.fg_tracks, st))) return rc;
-  if (syrk && (rc = launch_syrk(L.Kpad, L.Dpad, L.Zt, Sraw, mc_off, band.kb_ranges, fd, st))) return rc;
+  if ((rc = launch_assemble_hc(L.S, L.dc, L.ns, L.KR, L.Dpad, b.camrec, b.shared, R.S, R.rhs, R.hdiag, R.gvec, mc_off, st)))
+    return rc;
+  if ((rc = launch_z_build(&p, L.Dpad, L.M, L.q, L.Zt, R.rhs, mc_off, band.dev.fg_tracks, st))) return rc;
+  if (syrk && (rc = launch_syrk(L.Kpad, L.Dpad, L.Zt, R.S, mc_off, band.kb_ranges, fd, st))) return rc;
   // ... and all reductions must have landed before anyone reads its copy
   if (fab && (rc = fab->barrier(st))) return rc;
+  return VGG_OK;
+}
+
+// The one schur_build of vgg_ba_schur and vgg_dev_schur_build, into the buffers of *L.  band null: the dense plan, and
+// the last band plan is left alone; otherwise the plan of prob->mask when `banded`, recorded as the last one.
+static int schur_probe(const vgg_ba_problem* prob, const double* camrec, const double* g_p, const double* H_pp,
+                       const double* shared_in, const double* scale_p, double radius, double min_diag, double max_diag,
+                       BandPlan* band, bool banded, bool zt_nan, void* workspace, size_t ws_bytes, cudaStream_t st,
+                       Layout* L) {
+  if (const int rc = check_loss(prob)) return rc;
+  g_launch_count = 0;
+  int rc = make_layout(prob->S, prob->N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, L);
+  if (rc) return rc;
+  BandPlan dense;
+  if (band && banded && (rc = compute_band_hint(prob, L->dc, L->D, L->Dpad, L->Kpad, false, st, band))) return rc;
+  if (band) g_band_last = *band;
+  const BlockSet b{nullptr, const_cast<double*>(camrec), const_cast<double*>(g_p), const_cast<double*>(H_pp),
+                   const_cast<double*>(shared_in)};
+  VGG_CUDA_CHECK(cudaMemcpyAsync(L->sc_p, scale_p, sizeof(double) * (size_t)L->N * 3, cudaMemcpyDeviceToDevice, st));
+  // all-ones bytes: a NaN, so that the entries z_build writes can be told from the ones it leaves
+  VGG_CUDA_CHECK(cudaMemsetAsync(L->Zt, zt_nan ? 0xff : 0, sizeof(double) * (size_t)L->Kpad * L->Dpad, st));
+  VGG_CUDA_CHECK(cudaMemsetAsync(L->scal, 0, sizeof(double) * SCAL_DOUBLES, st));
+  return schur_build(*L, reduced_view(L->AR, L->D, L->Dpad), *prob, b, band ? *band : dense, FabricDev{}, radius,
+                     min_diag, max_diag, st, nullptr, !zt_nan);
+}
+
+static int copy_out(double* dst, const double* src, size_t n, cudaStream_t st) {
+  if (dst) VGG_CUDA_CHECK(cudaMemcpyAsync(dst, src, sizeof(double) * n, cudaMemcpyDeviceToDevice, st));
   return VGG_OK;
 }
 
@@ -558,22 +603,29 @@ void vgg_ba_default_options(vgg_ba_options* o) {
 }
 
 int vgg_ba_dims(int camera_model, int intr_mode, int* dc, int* ns) {
-  return dims_of(camera_model, intr_mode, dc, ns, nullptr);
+  Dims d;
+  if (const int rc = dims_of(camera_model, intr_mode, 0, 0, &d)) return rc;
+  if (dc) *dc = d.dc;
+  if (ns) *ns = d.ns;
+  return VGG_OK;
 }
 
 int vgg_ba_camrec_len(int camera_model, int intr_mode) {
-  int KR = 0;
-  if (dims_of(camera_model, intr_mode, nullptr, nullptr, &KR) != VGG_OK) return VGG_EINVAL;
-  return KR;
+  Dims d;
+  if (const int rc = dims_of(camera_model, intr_mode, 0, 0, &d)) return rc;
+  return d.KR;
+}
+
+static int workspace_bytes(int S, int N, int camera_model, int intr_mode, size_t* bytes, bool iterative) {
+  VGG_REQUIRE(S > 0 && N > 0 && bytes, "S, N must be positive");
+  Layout L;
+  const int rc = make_layout(S, N, camera_model, intr_mode, nullptr, 0, &L, iterative);
+  if (!rc) *bytes = L.bytes;
+  return rc;
 }
 
 int vgg_ba_workspace_bytes(int S, int N, int camera_model, int intr_mode, size_t* bytes) {
-  VGG_REQUIRE(S > 0 && N > 0 && bytes, "S, N must be positive");
-  Layout L;
-  const int rc = make_layout(S, N, camera_model, intr_mode, nullptr, 0, &L);
-  if (rc) return rc;
-  *bytes = L.bytes;
-  return VGG_OK;
+  return workspace_bytes(S, N, camera_model, intr_mode, bytes, false);
 }
 
 int vgg_ba_build_blocks(const vgg_ba_problem* prob, double* cost, double* camrec, double* g_p, double* H_pp, double* W,
@@ -614,25 +666,13 @@ int vgg_ba_schur(const vgg_ba_problem* prob, const double* camrec, const double*
                  double max_diag, void* workspace, size_t ws_bytes, double* Sraw, double* rhs, int* Dpad_out,
                  void* stream) {
   VGG_REQUIRE(prob && workspace && Sraw && rhs, "null pointer");
-  if (const int rc = check_loss(prob)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  g_launch_count = 0;
   Layout L;
-  int rc = make_layout(prob->S, prob->N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L);
+  int rc = schur_probe(prob, camrec, g_p, H_pp, shared_in, scale_p, radius, min_diag, max_diag, nullptr, false, false,
+                       workspace, ws_bytes, st, &L);
   if (rc) return rc;
-  BlockSet b;
-  b.cost = nullptr;
-  b.camrec = const_cast<double*>(camrec);
-  b.g_p = const_cast<double*>(g_p);
-  b.H_pp = const_cast<double*>(H_pp);
-  b.shared = const_cast<double*>(shared_in);
-  VGG_CUDA_CHECK(cudaMemcpyAsync(L.sc_p, scale_p, sizeof(double) * (size_t)L.N * 3, cudaMemcpyDeviceToDevice, st));
-  VGG_CUDA_CHECK(cudaMemsetAsync(L.Zt, 0, sizeof(double) * (size_t)L.Kpad * L.Dpad, st));
-  VGG_CUDA_CHECK(cudaMemsetAsync(L.scal, 0, sizeof(double) * 16, st));
-  rc = schur_build(L, *prob, b, BandPlan{}, FabricDev{}, radius, min_diag, max_diag, st);
-  if (rc) return rc;
-  VGG_CUDA_CHECK(cudaMemcpyAsync(Sraw, L.AR, sizeof(double) * (size_t)L.D * L.Dpad, cudaMemcpyDeviceToDevice, st));
-  VGG_CUDA_CHECK(cudaMemcpyAsync(rhs, L.AR + (size_t)L.D * L.Dpad, sizeof(double) * L.Dpad, cudaMemcpyDeviceToDevice, st));
+  const Reduced R = reduced_view(L.AR, L.D, L.Dpad);
+  if ((rc = copy_out(Sraw, R.S, (size_t)L.D * L.Dpad, st)) || (rc = copy_out(rhs, R.rhs, L.Dpad, st))) return rc;
   if (Dpad_out) *Dpad_out = L.Dpad;
   return VGG_OK;
 }
@@ -643,34 +683,18 @@ int vgg_dev_schur_build(const vgg_ba_problem* prob, const double* camrec, const 
                         int banded, int zt_nan, void* workspace, size_t ws_bytes, double* M, double* q, double* dpp,
                         double* scal, double* Zt, double* Sraw, double* rhs, void* stream) {
   VGG_REQUIRE(prob && camrec && g_p && H_pp && shared_in && scale_p && workspace, "null pointer");
-  if (const int rc = check_loss(prob)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  g_launch_count = 0;
   Layout L;
-  int rc = make_layout(prob->S, prob->N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L);
-  if (rc) return rc;
   BandPlan band;
-  if (banded && (rc = compute_band_hint(prob, L.dc, L.D, L.Dpad, L.Kpad, false, st, &band))) return rc;
-  g_band_last = band;
-  BlockSet b;
-  b.cost = nullptr;
-  b.camrec = const_cast<double*>(camrec);
-  b.g_p = const_cast<double*>(g_p);
-  b.H_pp = const_cast<double*>(H_pp);
-  b.shared = const_cast<double*>(shared_in);
-  VGG_CUDA_CHECK(cudaMemcpyAsync(L.sc_p, scale_p, sizeof(double) * (size_t)L.N * 3, cudaMemcpyDeviceToDevice, st));
-  // all-ones bytes: a NaN, so that the entries z_build writes can be told from the ones it leaves
-  VGG_CUDA_CHECK(cudaMemsetAsync(L.Zt, zt_nan ? 0xff : 0, sizeof(double) * (size_t)L.Kpad * L.Dpad, st));
-  VGG_CUDA_CHECK(cudaMemsetAsync(L.scal, 0, sizeof(double) * 16, st));
-  if ((rc = schur_build(L, *prob, b, band, FabricDev{}, radius, min_diag, max_diag, st, 0, nullptr, !zt_nan))) return rc;
-  auto out = [&](double* dst, const double* src, size_t n) -> int {
-    if (dst) VGG_CUDA_CHECK(cudaMemcpyAsync(dst, src, sizeof(double) * n, cudaMemcpyDeviceToDevice, st));
-    return VGG_OK;
-  };
+  int rc = schur_probe(prob, camrec, g_p, H_pp, shared_in, scale_p, radius, min_diag, max_diag, &band, banded, zt_nan,
+                       workspace, ws_bytes, st, &L);
+  if (rc) return rc;
+  const Reduced R = reduced_view(L.AR, L.D, L.Dpad);
   const size_t N = (size_t)L.N;
-  if ((rc = out(M, L.M, 9 * N)) || (rc = out(q, L.q, 3 * N)) || (rc = out(dpp, L.dpp, 3 * N)) ||
-      (rc = out(scal, L.scal, 16)) || (rc = out(Zt, L.Zt, (size_t)L.Kpad * L.Dpad)) ||
-      (rc = out(Sraw, L.AR, (size_t)L.D * L.Dpad)) || (rc = out(rhs, L.AR + (size_t)L.D * L.Dpad, L.Dpad)))
+  if ((rc = copy_out(M, L.M, 9 * N, st)) || (rc = copy_out(q, L.q, 3 * N, st)) ||
+      (rc = copy_out(dpp, L.dpp, 3 * N, st)) || (rc = copy_out(scal, L.scal, SCAL_DOUBLES, st)) ||
+      (rc = copy_out(Zt, L.Zt, (size_t)L.Kpad * L.Dpad, st)) || (rc = copy_out(Sraw, R.S, (size_t)L.D * L.Dpad, st)) ||
+      (rc = copy_out(rhs, R.rhs, L.Dpad, st)))
     return rc;
   VGG_CUDA_CHECK(cudaStreamSynchronize(st));
   return VGG_OK;
@@ -704,24 +728,18 @@ int vgg_dev_cholesky_band(int n, int lda, double* A, void* workspace, size_t ws_
 }
 
 int vgg_ba_reduced_system_doubles(int S, int camera_model, int intr_mode, size_t* doubles) {
-  int dc, ns;
-  if (!doubles || dims_of(camera_model, intr_mode, &dc, &ns, nullptr) != VGG_OK) {
-    set_error("bad camera_model/intr_mode");
-    return VGG_EINVAL;
-  }
-  const size_t D = (size_t)S * dc + ns, Dpad = align_up(D + 2, 128);
-  *doubles = D * Dpad + 3 * Dpad;
+  Dims d;
+  VGG_REQUIRE(doubles, "null pointer");
+  if (const int rc = dims_of(camera_model, intr_mode, S, 0, &d)) return rc;
+  *doubles = reduced_doubles(d.D, d.Dpad);
   return VGG_OK;
 }
 
 int vgg_ba_fabric_doubles(int S, int camera_model, int intr_mode, size_t* doubles) {
-  int dc, ns;
-  if (!doubles || dims_of(camera_model, intr_mode, &dc, &ns, nullptr) != VGG_OK) {
-    set_error("bad camera_model/intr_mode");
-    return VGG_EINVAL;
-  }
-  const int D = S * dc + ns;
-  *doubles = fabric_layout(D, (int)align_up((size_t)D + 2, 128)).total;
+  Dims d;
+  VGG_REQUIRE(doubles, "null pointer");
+  if (const int rc = dims_of(camera_model, intr_mode, S, 0, &d)) return rc;
+  *doubles = fabric_layout(d.D, d.Dpad).total;
   return VGG_OK;
 }
 
@@ -730,12 +748,204 @@ int vgg_ba_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, void*
   return vgg_ba_solve_fabric(prob, opt_in, workspace, ws_bytes, allreduce, ar_user, nullptr, summary, trace, stream);
 }
 
-// The LM loop of both linear solvers: lin = null solves the reduced camera system directly (DENSE_SCHUR: schur_build,
-// Cholesky, backward substitution), otherwise by PCG (csrc/ba_pcg.cu, ITERATIVE_SCHUR: fabric null; with an allreduce
-// hook the assembly is summed once per LM iteration and the Schur part of every matvec once per CG matvec, and the
-// model change joins the candidate's small all-reduce).  Everything else -- point step, camera update, candidate evaluation, accept / reject and the radius
-// rules -- is the same code for both; the iterative solve takes Ceres' model change -(J d)^T (f + J d / 2) instead of
-// the exact-solve identity 0.5 * quad.
+// a fabric solve's state from the caller's description; the barrier epoch lives as long as the allocation
+static int attach_fabric(const vgg_ba_fabric& f, const Layout& L, Fabric* fab) {
+  static thread_local std::map<const double*, unsigned long long> fabric_epochs;
+  VGG_REQUIRE(f.ar_doubles >= reduced_doubles(L.D, L.Dpad), "fabric buffer too small (vgg_ba_reduced_system_doubles)");
+  const FabricLayout lay = fabric_layout(L.D, L.Dpad);
+  VGG_REQUIRE(f.world > 1 && f.world <= 8 && f.peer_base[0] && f.total_doubles >= lay.total,
+              "fabric needs its peer table: world in 2..8, peer_base set, total_doubles >= vgg_ba_fabric_doubles");
+  fab->lay = lay;
+  fab->ar_local = f.ar_local;
+  fab->mc_off = f.ar_multicast - f.ar_local;
+  fab->base = FabricDev{f.world, f.rank, {}};
+  for (int r = 0; r < f.world; ++r) fab->base.peer[r] = f.peer_base[r];
+  fab->epoch = &fabric_epochs[f.peer_base[f.rank]];
+  fab->err = L.dev_info + INFO_FABRIC;
+  return VGG_OK;
+}
+
+// What the steps of one solve's LM loop share
+struct LmContext {
+  const Layout& L;
+  const vgg_ba_options& opt;
+  const BandPlan& band;
+  const Ranks& ranks;
+};
+
+// a linear step as cam_step reads it: the scaled camera step (entries stride apart), diag(H_cc) and the gradient
+struct LinStep {
+  const double *dcs, *hdiag, *gvec;
+  size_t stride;
+};
+
+// DENSE_SCHUR: schur_build, the exchange of the reduced system over the ranks, its scaled and damped bordered form, the
+// Cholesky and the backward substitution.  first: the camera Jacobi scale is taken from this hdiag.
+static int direct_step(const LmContext& c, const vgg_ba_problem& pcur, const BlockSet& b, int it, double radius,
+                       bool first, LinStep* out) {
+  const Layout& L = c.L;
+  const int D = L.D;
+  Fabric* fab = c.ranks.fab;
+  const cudaStream_t st = c.ranks.st;
+  int rc;
+  // a fabric solve alternates two copies of the reduced system (fabric_layout); fd: where the SYRK sends each row block
+  const size_t off = fab ? (size_t)(it & 1) * fab->lay.arc : 0;
+  const Reduced R = reduced_view(fab ? fab->ar_local + off : L.AR, D, L.Dpad);
+  const FabricDev fd = fab ? fab->at(off) : FabricDev{};
+  if ((rc = schur_build(L, R, pcur, b, c.band, fd, radius, c.opt.min_lm_diagonal, c.opt.max_lm_diagonal, st, fab)))
+    return rc;
+  // fabric: every row block is complete on its owner, pull the others (rows 0..D incl. the rhs row, hdiag, gvec)
+  if ((rc = fab ? launch_fabric_gather(fd, D + 3, D + 1, D, L.Dpad, st) : c.ranks.sum(R.S, reduced_doubles(D, L.Dpad))))
+    return rc;
+  if (first && (rc = launch_jacobi_scale_cams(D, R.hdiag, L.sc_c, c.opt.jacobi_scaling, st))) return rc;
+  if ((rc = launch_scale_damp(D, L.Dpad, R.S, R.rhs, R.hdiag, L.sc_c, pcur.param_const, radius, c.opt.min_lm_diagonal,
+                              c.opt.max_lm_diagonal, L.bvec, st)))
+    return rc;
+  // Factor the reduced system with the in-repo blocked Cholesky (csrc/chol.cu) on the row-major LOWER triangle of the
+  // BORDERED matrix of order D+1 -- scale_damp put the scaled right-hand side into row D, so the factorisation leaves
+  // y = L^-1 b there (and, mirrored like every panel, in column D): the forward substitution costs nothing and only the
+  // backward substitution L^T x = y remains.  (cuSOLVER potrf on the same matrix took 1.05 ms at n = 2403, this 0.93.)
+  if ((rc = chol_lower_inplace(D + 1, L.Dpad, R.S, L.chol_diag, L.dev_info + INFO_CHOL, c.band.end_blk, c.band.arrow_blk, st)))
+    return rc;
+  // Backward substitution on U = L^T (the row-major upper triangle), y = column D of the buffer: the own kernel
+  // (csrc/trsv.cu, block rows chained through the solution), cuBLAS beyond its one co-resident wave of D/64 CTAs.
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.dev_info + INFO_TRSV, 0, sizeof(int), st));
+  *out = LinStep{L.bvec, R.hdiag, R.gvec, 1};
+  if (D <= 7000) return launch_trsv_upper(D, L.Dpad, R.S, R.S + D, (size_t)L.Dpad, L.bvec, nullptr, st);
+  cublasHandle_t cb = get_cublas();
+  if (!cb || cublasSetStream(cb, st) != CUBLAS_STATUS_SUCCESS) {
+    set_error("cublasCreate / cublasSetStream failed");
+    return VGG_ESOLVER;
+  }
+  if (cublasDtrsv(cb, CUBLAS_FILL_MODE_LOWER, CUBLAS_OP_T, CUBLAS_DIAG_NON_UNIT, D, R.S, L.Dpad, R.S + D, L.Dpad) !=
+      CUBLAS_STATUS_SUCCESS) {
+    set_error("cublasDtrsv failed to launch");
+    return VGG_ESOLVER;
+  }
+  g_launch_count += 1;
+  *out = LinStep{R.S + D, R.hdiag, R.gvec, (size_t)L.Dpad};
+  return VGG_OK;
+}
+
+// ITERATIVE_SCHUR: the point blocks as schur_build prepares them, then the reduced right-hand side and the Schur-Jacobi
+// blocks in one pass over the observations, and CG on the implicit reduced system (csrc/ba_pcg.cu)
+static int iterative_step(const LmContext& c, const vgg_ba_linear_solver& lin, const vgg_ba_problem& pcur,
+                          const BlockSet& b, double radius, bool first, LinStep* out) {
+  const Layout& L = c.L;
+  const PcgBuffers& B = L.pcg;
+  const cudaStream_t st = c.ranks.st;
+  int rc;
+  if ((rc = launch_point_prep(L.N, b.H_pp, b.g_p, L.sc_p, pcur.point_const, radius, c.opt.min_lm_diagonal,
+                              c.opt.max_lm_diagonal, L.M, L.q, L.dpp, L.scal, st)))
+    return rc;
+  PcgOp op{&pcur, L.dc, L.ns, L.KR, b.camrec, b.shared, L.M, L.sc_c, radius, c.opt.min_lm_diagonal,
+           c.opt.max_lm_diagonal, c.band.dev.fg_tracks};
+  if ((rc = launch_pcg_assemble(op, L.q, B, st))) return rc;
+  // track shards: the assembly and a copy of the camera records are this rank's partial sums, summed in one call.
+  // The copy, not b itself: after a rejected step b is evaluated again and would be summed twice.
+  if (c.ranks.sharded()) {
+    VGG_CUDA_CHECK(cudaMemcpyAsync(B.shared, b.shared, sizeof(double) * 8, cudaMemcpyDeviceToDevice, st));
+    VGG_CUDA_CHECK(cudaMemcpyAsync(B.camrec, b.camrec, sizeof(double) * (size_t)L.S * L.KR, cudaMemcpyDeviceToDevice, st));
+    if ((rc = c.ranks.sum(B.rhs, B.red_doubles))) return rc;
+    op.camrec = B.camrec;
+    op.shared_in = B.shared;
+  }
+  if (first && (rc = launch_jacobi_scale_cams(L.D, B.hdiag, L.sc_c, c.opt.jacobi_scaling, st))) return rc;
+  if ((rc = launch_pcg_init(op, B, L.bvec, st)) || (rc = pcg_run(op, lin, B, L.bvec, c.ranks, st))) return rc;
+  *out = LinStep{B.x, B.hdiag, B.gvec, 1};
+  return VGG_OK;
+}
+
+// The candidate's record, summed over the ranks: its cost, the point-side model terms, the iterative solve's model
+// change, the point part of |x|^2 and the candidate's camera gradient, and from that the gradient max-norms
+static int reduce_candidate(const LmContext& c, const vgg_ba_problem& pcur, int cur, bool iterative) {
+  const Layout& L = c.L;
+  const BlockSet& bn = L.blk[cur ^ 1];
+  const cudaStream_t st = c.ranks.st;
+  const size_t count = SMALL_VEC + (size_t)L.Dpad;
+  int rc;
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.small, 0, sizeof(double) * count, st));
+  if (iterative && (rc = launch_pcg_model_change(&pcur, L.M, L.blk[cur].g_p, L.wacc, L.d_c, c.band.dev.fg_tracks,
+                                                 L.small + SMALL_MODEL_CHANGE, st)))
+    return rc;
+  VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + SMALL_COST, bn.cost, sizeof(double), cudaMemcpyDeviceToDevice, st));
+  VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + SMALL_PT_QUAD, L.scal + SCAL_PT_QUAD, sizeof(double) * 2, cudaMemcpyDeviceToDevice, st));
+  VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + SMALL_PT_FAIL, L.scal + SCAL_PT_FAIL, sizeof(double), cudaMemcpyDeviceToDevice, st));
+  if ((rc = launch_extract_gvec(L.S, L.dc, L.ns, L.KR, bn.camrec, bn.shared, L.small + SMALL_VEC, st))) return rc;
+  if (c.opt.parameter_tolerance > 0.0) {
+    // |x|^2 of the current state: the camera part stays in scal, the point part (this rank's points) is summed, so
+    // every rank tests the parameter tolerance against the same |x|
+    xnorm_kernel<<<1, 1024, 0, st>>>(L.S, L.N, L.dc, L.ns, pcur.camera_model, pcur.param_const, pcur.point_const,
+                                      pcur.poses, pcur.intr, pcur.points, L.scal + SCAL_XNORM_C, L.small + SMALL_XNORM_P);
+    VGG_LAUNCH_CHECK();
+  }
+  return c.ranks.candidate(L.small, count, L.scal, [&] {
+    return launch_gradmax(L.D, L.N, L.small + SMALL_VEC, pcur.param_const, bn.g_p, pcur.point_const, L.scal, st);
+  });
+}
+
+struct LmState {
+  double cost, radius, decrease_factor;
+  int invalid_steps;
+};
+
+// Ceres' TrustRegionMinimizer + LevenbergMarquardtStrategy rules on iteration it's record: updates s and the trace rows,
+// sets summary->termination when the solve stops, and returns true when the candidate becomes the state.
+static bool lm_decide(const LmRecord& r, const vgg_ba_options& opt, bool iterative, int it, LmState* s,
+                      vgg_ba_summary* summary, double* trace, double* cg_trace) {
+  const double c_cost = r.cost();
+  const double step_norm = sqrt(r.scal[SCAL_CAM_STEP2] + r.small[SMALL_PT_STEP2]);
+  // the iterative solve takes Ceres' model change -(J d)^T (f + J d / 2); 0.5 * quad holds for an exact solve only
+  const double model_change =
+      iterative ? r.small[SMALL_MODEL_CHANGE] : 0.5 * (r.scal[SCAL_CAM_QUAD] + r.small[SMALL_PT_QUAD]);
+  const bool solver_bad = r.chol_info != 0 || r.trsv_info != 0 || r.scal[SCAL_CAM_BAD] > 0 ||
+                          r.small[SMALL_PT_FAIL] > 0 || (iterative && r.cg[CG_TERM] == VGG_CG_FAILURE);
+  if (iterative && cg_trace) memcpy(cg_trace + (size_t)(it - 1) * 4, r.cg + CG_ITERS, sizeof(double) * 4);
+  double* tr = trace ? trace + (size_t)(it - 1) * 8 : nullptr;
+  if (tr) {
+    tr[0] = it; tr[1] = s->cost; tr[2] = c_cost; tr[3] = model_change; tr[4] = 0; tr[5] = s->radius; tr[6] = step_norm;
+    tr[7] = 0;
+  }
+  if (solver_bad || !(model_change > 0.0) || !isfinite(c_cost)) {
+    // Ceres: invalid step -> LevenbergMarquardtStrategy::StepIsInvalid
+    if (tr) tr[7] = 2;
+    if (++s->invalid_steps >= opt.max_num_consecutive_invalid_steps) summary->termination = VGG_BA_FAILURE;
+    else s->radius *= 0.5;
+    return false;
+  }
+  s->invalid_steps = 0;
+  const double cost_change = s->cost - c_cost;
+  const double rho = cost_change / model_change;
+  if (tr) tr[4] = rho;
+  // Ceres ParameterToleranceReached(): step_norm <= tol * (|x| + tol), |x| over the non-constant blocks in ambient
+  // coordinates (xnorm_kernel, only launched when the tolerance is non-zero -- COLMAP's default is 0)
+  const double x_norm = opt.parameter_tolerance > 0.0 ? sqrt(r.xnorm_c + r.small[SMALL_XNORM_P]) : 0.0;
+  if (step_norm <= opt.parameter_tolerance * (x_norm + opt.parameter_tolerance)) {
+    summary->termination = VGG_BA_CONVERGENCE_PARAMETER;
+    return false;
+  }
+  if (fabs(cost_change) <= opt.function_tolerance * s->cost) {
+    // Ceres 2.x TrustRegionMinimizer::Minimize returns from FunctionToleranceReached() before IsStepSuccessful() /
+    // HandleSuccessfulStep(): the candidate of the terminating iteration is discarded
+    summary->termination = VGG_BA_CONVERGENCE_FUNCTION;
+    return false;
+  }
+  if (!(rho > opt.min_relative_decrease)) {
+    s->radius = s->radius / s->decrease_factor;
+    s->decrease_factor *= 2.0;
+    return false;
+  }
+  s->cost = c_cost;
+  summary->successful++;
+  if (tr) tr[7] = 1;
+  s->radius = fmin(opt.max_trust_region_radius, s->radius / fmax(1.0 / 3.0, 1.0 - pow(2.0 * rho - 1.0, 3.0)));
+  s->decrease_factor = 2.0;
+  if (r.gmax() <= opt.gradient_tolerance) summary->termination = VGG_BA_CONVERGENCE_GRADIENT;
+  return true;
+}
+
+// The LM loop of both linear solvers: lin = null solves the reduced camera system directly (direct_step, DENSE_SCHUR),
+// otherwise by PCG (iterative_step, ITERATIVE_SCHUR; fabric null).  Everything else is the same code for both.
 static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, const vgg_ba_linear_solver* lin,
                     void* workspace, size_t ws_bytes, vgg_allreduce_fn allreduce, void* ar_user,
                     const vgg_ba_fabric* fabric, vgg_ba_summary* summary, double* trace, double* cg_trace, void* stream) {
@@ -747,38 +957,14 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
   vgg_ba_options opt;
   if (opt_in) opt = *opt_in;
   else vgg_ba_default_options(&opt);
-  const int S = prob->S, N = prob->N;
-  int dc, ns;
-  if (dims_of(prob->camera_model, prob->intr_mode, &dc, &ns, nullptr) != VGG_OK) {
-    set_error("bad camera_model/intr_mode");
-    return VGG_EINVAL;
-  }
-  const int D = S * dc + ns;
   Layout L;
-  int rc = make_layout(S, N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L, lin != nullptr);
+  int rc = make_layout(prob->S, prob->N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L, lin != nullptr);
   if (rc) return rc;
-  const size_t ar_count = (size_t)D * L.Dpad + 3 * (size_t)L.Dpad;
-  // fabric mode: the reduced system lives in symmetric (peer-mapped) memory and is reduced by the producing kernels
-  // (multimem operations for the small blocks, the SYRK's reduce-scatter for the rest); mc_off is the distance from a
-  // local address to its multicast twin
-  ptrdiff_t mc_off = 0;
+  const int S = L.S, N = L.N, D = L.D;
   Fabric fab;
-  static thread_local std::map<const double*, unsigned long long> fabric_epochs;
-  if (fabric && fabric->ar_local && fabric->ar_multicast) {
-    VGG_REQUIRE(fabric->ar_doubles >= ar_count, "fabric buffer too small (vgg_ba_reduced_system_doubles)");
-    const FabricLayout lay = fabric_layout(D, L.Dpad);
-    VGG_REQUIRE(fabric->world > 1 && fabric->world <= 8 && fabric->peer_base[0] && fabric->total_doubles >= lay.total,
-                "fabric needs its peer table: world in 2..8, peer_base set, total_doubles >= vgg_ba_fabric_doubles");
-    L.AR = fabric->ar_local;
-    mc_off = fabric->ar_multicast - fabric->ar_local;
-    fab.on = true;
-    fab.lay = lay;
-    fab.base.world = fabric->world;
-    fab.base.rank = fabric->rank;
-    for (int r = 0; r < fabric->world; ++r) fab.base.peer[r] = fabric->peer_base[r];
-    fab.epoch = &fabric_epochs[fabric->peer_base[fabric->rank]];
-    fab.err = L.dev_info + 2;
-  }
+  const bool fab_on = fabric && fabric->ar_local && fabric->ar_multicast;
+  if (fab_on && (rc = attach_fabric(*fabric, L, &fab))) return rc;
+  const Ranks ranks{fab_on ? &fab : nullptr, allreduce, ar_user, st};
   // the constant flags of this solve (unobserved points and frames added); every kernel below reads these, not the
   // caller's.  Frames are summed over track shards: a frame is in the problem if any rank sees it.
   const vgg_ba_problem* const caller = prob;
@@ -788,36 +974,22 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
   prob = &pe;
   BandPlan band;
   // the iterative solve factors nothing: each rank's band tables describe its own tracks, which is all its kernels read
-  if ((rc = compute_band_hint(prob, dc, D, L.Dpad, L.Kpad, !lin && (allreduce != nullptr || fabric != nullptr), st,
+  if ((rc = compute_band_hint(prob, L.dc, D, L.Dpad, L.Kpad, !lin && (allreduce != nullptr || fabric != nullptr), st,
                               &band)))
     return rc;
   g_band_last = band;
-  double* Sraw = L.AR;
-  double* rhs = L.AR + (size_t)D * L.Dpad;
-  double* hdiag = rhs + L.Dpad;
-  double* gvec = hdiag + L.Dpad;
-  if (lin) {
-    Sraw = nullptr;
-    rhs = L.pcg.rhs;
-    hdiag = L.pcg.hdiag;
-    gvec = L.pcg.gvec;
-  }
-  // sum (and one max slot) of a small vector over the ranks: in-kernel over the fabric, else through the host hook
-  auto reduce_small = [&](double* vec, size_t count, int op) -> int {
-    if (fab.on) return fab.allreduce(vec, (int)count, op == 1 ? 0 : -1, st);
-    if (allreduce) return allreduce(ar_user, vec, count, op, st);
-    return VGG_OK;
-  };
+  const LmContext c{L, opt, band, ranks};
+  const size_t small_count = SMALL_VEC + (size_t)L.Dpad;
 
   VGG_CUDA_CHECK(cudaMemsetAsync(L.point_const, 0, (size_t)N, st));
-  VGG_CUDA_CHECK(cudaMemsetAsync(L.small, 0, sizeof(double) * (8 + (size_t)L.Dpad), st));
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.small, 0, sizeof(double) * small_count, st));
   observed_kernel<<<dim3((N + 255) / 256, (S + OBS_FRAMES - 1) / OBS_FRAMES), 256, 0, st>>>(S, N, pe.mask, L.point_const,
-                                                                                           L.small + 8);
+                                                                                           L.small + SMALL_VEC);
   VGG_LAUNCH_CHECK();
-  if ((rc = reduce_small(L.small, 8 + (size_t)L.Dpad, 0))) return rc;
-  effective_const_kernel<<<(std::max(D, N) + 255) / 256, 256, 0, st>>>(S, N, dc, D, caller->param_const,
-                                                                       caller->point_const, L.small + 8, L.pconst,
-                                                                       L.point_const);
+  if ((rc = ranks.sum(L.small, small_count))) return rc;
+  effective_const_kernel<<<(std::max(D, N) + 255) / 256, 256, 0, st>>>(S, N, L.dc, D, caller->param_const,
+                                                                       caller->point_const, L.small + SMALL_VEC,
+                                                                       L.pconst, L.point_const);
   VGG_LAUNCH_CHECK();
 
   EventPair evs;
@@ -852,262 +1024,68 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
     VGG_CUDA_CHECK(cudaMemsetAsync(b.cost, 0, acc_bytes, st));
     return ba_build_blocks(&p, b.cost, b.camrec, b.g_p, b.H_pp, nullptr, b.shared, 0, band.dev.fg_tracks, st, true);
   };
-  // global cost + gradient max-norm of block set `which`; result lands in host h[0..2] = cost, gmax_c, gmax_p
-  double* h_scal = pinned_scalars();
-  if (!h_scal) {
-    set_error("cudaHostAlloc for the scalar read-back failed");
-    return VGG_ECUDA;
-  }
-  VGG_CUDA_CHECK(cudaMemsetAsync(L.dev_info, 0, sizeof(int) * 4, st));
-  auto read_scalars = [&]() -> int {
+  double* h_rec = pinned_scalars();
+  if (!h_rec) return VGG_ECUDA;
+  const LmRecord& rec = *reinterpret_cast<const LmRecord*>(h_rec);
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.dev_info, 0, sizeof(int) * INFO_INTS, st));
+  auto read_record = [&]() -> int {
     pack_scalars_kernel<<<1, 32, 0, st>>>(L.scal, L.small, L.dev_info, L.pcg.cg, L.packed);
     VGG_LAUNCH_CHECK();
-    // [0..19] used, [20..24] by the iterative solve
-    VGG_CUDA_CHECK(cudaMemcpyAsync(h_scal, L.packed, sizeof(double) * (lin ? 28 : 24), cudaMemcpyDeviceToHost, st));
+    VGG_CUDA_CHECK(cudaMemcpyAsync(h_rec, L.packed, sizeof(double) * (lin ? REC_DOUBLES_CG : REC_DOUBLES),
+                                   cudaMemcpyDeviceToHost, st));
     VGG_CUDA_CHECK(cudaStreamSynchronize(st));
-    return VGG_OK;
-  };
-  auto cost_and_gradient = [&](int which, double* cost_out, double* gmax_out) -> int {
-    const BlockSet& b = L.blk[which];
-    int r;
-    VGG_CUDA_CHECK(cudaMemsetAsync(L.small, 0, sizeof(double) * (8 + (size_t)L.Dpad), st));
-    VGG_CUDA_CHECK(cudaMemcpyAsync(L.small, b.cost, sizeof(double), cudaMemcpyDeviceToDevice, st));
-    if ((r = launch_extract_gvec(S, dc, ns, L.KR, b.camrec, b.shared, L.small + 8, st))) return r;
-    if ((r = reduce_small(L.small, 8 + (size_t)L.Dpad, 0))) return r;
-    VGG_CUDA_CHECK(cudaMemsetAsync(L.scal + 4, 0, sizeof(double) * 2, st));
-    if ((r = launch_gradmax(D, N, L.small + 8, prob->param_const, b.g_p, prob->point_const, L.scal, st))) return r;
-    if ((r = reduce_small(L.scal + 5, 1, 1))) return r;
-    if ((r = read_scalars())) return r;
-    if (h_scal[19] != 0.0) {
+    if (rec.fabric_timeout != 0.0) {
       set_error("fabric barrier timed out: a peer rank did not arrive");
       return VGG_ECUDA;
     }
-    *cost_out = h_scal[8];
-    *gmax_out = grad_max_norm(h_scal[4], h_scal[5]);
     return VGG_OK;
   };
 
+  // the initial cost and gradient max-norm, summed over the ranks
+  const BlockSet& b0 = L.blk[cur];
   if ((rc = eval(cur))) return rc;
-  if ((rc = launch_jacobi_scale_points(N, L.blk[cur].H_pp, L.sc_p, opt.jacobi_scaling, st))) return rc;
-  double cost = 0, gmax = 0;
-  if ((rc = cost_and_gradient(cur, &cost, &gmax))) return rc;
+  if ((rc = launch_jacobi_scale_points(N, b0.H_pp, L.sc_p, opt.jacobi_scaling, st))) return rc;
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.small, 0, sizeof(double) * small_count, st));
+  VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + SMALL_COST, b0.cost, sizeof(double), cudaMemcpyDeviceToDevice, st));
+  if ((rc = launch_extract_gvec(S, L.dc, L.ns, L.KR, b0.camrec, b0.shared, L.small + SMALL_VEC, st))) return rc;
+  if ((rc = ranks.sum(L.small, small_count))) return rc;
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.scal + SCAL_GMAX_C, 0, sizeof(double) * 2, st));
+  if ((rc = launch_gradmax(D, N, L.small + SMALL_VEC, prob->param_const, b0.g_p, prob->point_const, L.scal, st)) ||
+      (rc = ranks.max(L.scal + SCAL_GMAX_P)) || (rc = read_record()))
+    return rc;
 
+  LmState s{rec.cost(), opt.initial_trust_region_radius, 2.0, 0};
   memset(summary, 0, sizeof(*summary));
-  summary->initial_cost = cost;
-  summary->termination = VGG_BA_NO_CONVERGENCE;
-  double radius = opt.initial_trust_region_radius;
-  double decrease_factor = 2.0;
-  int it = 0, invalid_steps = 0;
+  summary->initial_cost = s.cost;
+  summary->termination = rec.gmax() <= opt.gradient_tolerance ? VGG_BA_CONVERGENCE_GRADIENT : VGG_BA_NO_CONVERGENCE;
+  int it = 0;
   bool have_scale_c = false;
-  bool done = gmax <= opt.gradient_tolerance;
-  if (done) summary->termination = VGG_BA_CONVERGENCE_GRADIENT;
 
-  while (!done) {
+  while (summary->termination == VGG_BA_NO_CONVERGENCE) {
     if (it >= opt.max_num_iterations) break;
-    if (radius < opt.min_trust_region_radius) {
+    if (s.radius < opt.min_trust_region_radius) {
       summary->termination = VGG_BA_MIN_TRUST_REGION;
       break;
     }
     ++it;
     const int cand = cur ^ 1;
-    VGG_CUDA_CHECK(cudaMemsetAsync(L.scal, 0, sizeof(double) * 16, st));
-    FabricDev fd{};
-    if (fab.on) {
-      // this iteration's copy of the reduced system (parity) and where the SYRK epilogue sends each row block
-      const size_t off = (size_t)(it & 1) * fab.lay.arc;
-      L.AR = fabric->ar_local + off;
-      Sraw = L.AR;
-      rhs = L.AR + (size_t)D * L.Dpad;
-      hdiag = rhs + L.Dpad;
-      gvec = hdiag + L.Dpad;
-      fd = fab.at(off);
-    }
+    VGG_CUDA_CHECK(cudaMemsetAsync(L.scal, 0, sizeof(double) * SCAL_DOUBLES, st));
     const vgg_ba_problem pcur = state(cur);
-    const double* dcs = L.bvec;
-    size_t dcs_stride = 1;
-    if (lin) {
-      // point blocks as schur_build prepares them, then the reduced right-hand side and the Schur-Jacobi blocks in one
-      // pass over the observations, and CG on the implicit reduced system (csrc/ba_pcg.cu)
-      const BlockSet& b = L.blk[cur];
-      if ((rc = launch_point_prep(N, b.H_pp, b.g_p, L.sc_p, pcur.point_const, radius, opt.min_lm_diagonal,
-                                  opt.max_lm_diagonal, L.M, L.q, L.dpp, L.scal, st)))
-        return rc;
-      if ((rc = launch_pcg_assemble(&pcur, dc, ns, L.KR, b.camrec, b.shared, L.M, L.q, L.pcg, band.dev.fg_tracks, st)))
-        return rc;
-      // track shards: the assembly and a copy of the camera records are this rank's partial sums, summed in one call.
-      // The copy, not L.blk[cur] itself: after a rejected step cur is evaluated again and would be summed twice.
-      const double* camrec = b.camrec;
-      const double* shared_in = b.shared;
-      if (allreduce) {
-        VGG_CUDA_CHECK(cudaMemcpyAsync(L.pcg.shared, b.shared, sizeof(double) * 8, cudaMemcpyDeviceToDevice, st));
-        VGG_CUDA_CHECK(cudaMemcpyAsync(L.pcg.camrec, b.camrec, sizeof(double) * (size_t)S * L.KR, cudaMemcpyDeviceToDevice,
-                                       st));
-        if ((rc = allreduce(ar_user, L.pcg.rhs, L.pcg.red_doubles, 0, st))) return rc;
-        camrec = L.pcg.camrec;
-        shared_in = L.pcg.shared;
-      }
-      if (!have_scale_c) {
-        if ((rc = launch_jacobi_scale_cams(D, hdiag, L.sc_c, opt.jacobi_scaling, st))) return rc;
-        have_scale_c = true;
-      }
-      if ((rc = launch_pcg_init(&pcur, dc, ns, L.KR, camrec, shared_in, L.sc_c, radius, opt.min_lm_diagonal,
-                                opt.max_lm_diagonal, L.pcg, L.bvec, st)))
-        return rc;
-      if ((rc = pcg_run(&pcur, dc, ns, L.KR, camrec, shared_in, L.M, L.sc_c, radius, opt.min_lm_diagonal,
-                        opt.max_lm_diagonal, *lin, L.pcg, L.bvec, band.dev.fg_tracks, PcgHook{allreduce, ar_user}, st)))
-        return rc;
-      dcs = L.pcg.x;
-    } else {
-      if ((rc = schur_build(L, pcur, L.blk[cur], band, fd, radius, opt.min_lm_diagonal, opt.max_lm_diagonal, st, mc_off,
-                            fab.on ? &fab : nullptr)))
-        return rc;
-      // every row block is complete on its owner: pull the others (matrix rows 0..D incl. the rhs row, then hdiag, gvec)
-      if (fab.on && (rc = launch_fabric_gather(fd, D + 3, D + 1, D, L.Dpad, st))) return rc;
-      if (allreduce && !mc_off && (rc = allreduce(ar_user, L.AR, ar_count, 0, st))) return rc;
-      if (!have_scale_c) {
-        if ((rc = launch_jacobi_scale_cams(D, hdiag, L.sc_c, opt.jacobi_scaling, st))) return rc;
-        have_scale_c = true;
-      }
-      if ((rc = launch_scale_damp(D, L.Dpad, Sraw, rhs, hdiag, L.sc_c, prob->param_const, radius, opt.min_lm_diagonal,
-                                  opt.max_lm_diagonal, L.bvec, st)))
-        return rc;
-      // Factor the reduced system with the in-repo blocked Cholesky (csrc/chol.cu) on the row-major LOWER triangle of the
-      // BORDERED matrix of order D+1 -- scale_damp put the scaled right-hand side into row D, so the factorisation leaves
-      // y = L^-1 b there (and, mirrored like every panel, in column D): the forward substitution costs nothing and only the
-      // backward substitution L^T x = y remains.  (cuSOLVER potrf on the same matrix took 1.05 ms at n = 2403, this 0.93.)
-      if ((rc = chol_lower_inplace(D + 1, L.Dpad, Sraw, L.chol_diag, L.dev_info, band.end_blk, band.arrow_blk, st))) return rc;
-      // Backward substitution on U = L^T (the row-major upper triangle), y = column D of the buffer.
-      {
-        VGG_CUDA_CHECK(cudaMemsetAsync(L.dev_info + 1, 0, sizeof(int), st));
-        if (D > 7000) {                                 // beyond the own kernel's one co-resident wave of D/64 CTAs
-          cublasHandle_t cb = get_cublas();
-          if (!cb || cublasSetStream(cb, st) != CUBLAS_STATUS_SUCCESS) {
-            set_error("cublasCreate / cublasSetStream failed");
-            return VGG_ESOLVER;
-          }
-          if (cublasDtrsv(cb, CUBLAS_FILL_MODE_LOWER, CUBLAS_OP_T, CUBLAS_DIAG_NON_UNIT, D, Sraw, L.Dpad, Sraw + D, L.Dpad) !=
-              CUBLAS_STATUS_SUCCESS) {
-            set_error("cublasDtrsv failed to launch");
-            return VGG_ESOLVER;
-          }
-          g_launch_count += 1;
-          dcs = Sraw + D;
-          dcs_stride = (size_t)L.Dpad;
-        } else {
-          // own backward substitution (csrc/trsv.cu): one launch, block rows chained through the solution itself
-          if ((rc = launch_trsv_upper(D, L.Dpad, Sraw, Sraw + D, (size_t)L.Dpad, L.bvec, nullptr, st))) return rc;
-        }
-      }
-    }
-    if ((rc = launch_cam_step(D, dcs, dcs_stride, L.sc_c, hdiag, gvec, prob->param_const, radius, opt.min_lm_diagonal,
-                              opt.max_lm_diagonal, L.d_c, L.scal, st)))
+    LinStep ls;
+    if ((rc = lin ? iterative_step(c, *lin, pcur, L.blk[cur], s.radius, !have_scale_c, &ls)
+                  : direct_step(c, pcur, L.blk[cur], it, s.radius, !have_scale_c, &ls)))
       return rc;
-    if ((rc = launch_backsub(&pcur, L.d_c, L.wacc, band.dev.fg_tracks, st))) return rc;
-    if ((rc = launch_point_step(N, L.M, L.blk[cur].g_p, L.wacc, L.sc_p, L.dpp, pe.point_const, L.points[cur], radius,
-                                L.points[cand], L.scal, st)))
+    have_scale_c = true;
+    if ((rc = launch_cam_step(D, ls.dcs, ls.stride, L.sc_c, ls.hdiag, ls.gvec, prob->param_const, s.radius,
+                              opt.min_lm_diagonal, opt.max_lm_diagonal, L.d_c, L.scal, st)) ||
+        (rc = launch_backsub(&pcur, L.d_c, L.wacc, band.dev.fg_tracks, st)) ||
+        (rc = launch_point_step(N, L.M, L.blk[cur].g_p, L.wacc, L.sc_p, L.dpp, prob->point_const, L.points[cur],
+                                s.radius, L.points[cand], L.scal, st)) ||
+        (rc = launch_cam_update(S, L.dc, L.ns, prob->camera_model, L.d_c, L.poses[cur], L.intr[cur], L.poses[cand],
+                                L.intr[cand], st)) ||
+        (rc = eval(cand)) || (rc = reduce_candidate(c, pcur, cur, lin != nullptr)) || (rc = read_record()))
       return rc;
-    if ((rc = launch_cam_update(S, dc, ns, prob->camera_model, L.d_c, L.poses[cur], L.intr[cur], L.poses[cand],
-                                L.intr[cand], st)))
-      return rc;
-    if ((rc = eval(cand))) return rc;
-    // point-side model terms join the candidate cost in the small all-reduce, and so does the iterative solve's model
-    // change (small[6]: each rank's observations)
-    VGG_CUDA_CHECK(cudaMemsetAsync(L.small, 0, sizeof(double) * (8 + (size_t)L.Dpad), st));
-    if (lin && (rc = launch_pcg_model_change(&pcur, L.M, L.blk[cur].g_p, L.wacc, L.d_c, band.dev.fg_tracks, L.small + 6,
-                                             st)))
-      return rc;
-    VGG_CUDA_CHECK(cudaMemcpyAsync(L.small, L.blk[cand].cost, sizeof(double), cudaMemcpyDeviceToDevice, st));
-    VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + 1, L.scal + 2, sizeof(double) * 2, cudaMemcpyDeviceToDevice, st));
-    VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + 3, L.scal + 6, sizeof(double), cudaMemcpyDeviceToDevice, st));
-    if ((rc = launch_extract_gvec(S, dc, ns, L.KR, L.blk[cand].camrec, L.blk[cand].shared, L.small + 8, st))) return rc;
-    if (opt.parameter_tolerance > 0.0) {
-      // |x|^2 of the current state: the camera part (replicated) stays in scal[8], the point part (this rank's points)
-      // joins the small all-reduce in slot 5, which both paths sum; |x| is formed from the two after the reduction, so
-      // every rank tests the parameter tolerance against the same |x|
-      xnorm_kernel<<<1, 1024, 0, st>>>(S, N, dc, ns, prob->camera_model, prob->param_const, prob->point_const,
-                                        L.poses[cur], L.intr[cur], L.points[cur], L.scal + 8, L.small + 5);
-      VGG_LAUNCH_CHECK();
-    }
-    if (fab.on) {
-      // one in-kernel all-reduce for everything: the point-gradient max rides in slot 4 (max), the rest is summed
-      if ((rc = launch_gradmax(D, N, L.small + 8, prob->param_const, L.blk[cand].g_p, prob->point_const, L.scal, st))) return rc;
-      VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + 4, L.scal + 5, sizeof(double), cudaMemcpyDeviceToDevice, st));
-      if ((rc = fab.allreduce(L.small, 8 + L.Dpad, 4, st))) return rc;
-      VGG_CUDA_CHECK(cudaMemsetAsync(L.scal + 4, 0, sizeof(double) * 2, st));
-      if ((rc = launch_gradmax(D, N, L.small + 8, prob->param_const, L.blk[cand].g_p, prob->point_const, L.scal, st))) return rc;
-      VGG_CUDA_CHECK(cudaMemcpyAsync(L.scal + 5, L.small + 4, sizeof(double), cudaMemcpyDeviceToDevice, st));
-    } else {
-      if (allreduce && (rc = allreduce(ar_user, L.small, 8 + (size_t)L.Dpad, 0, st))) return rc;
-      if ((rc = launch_gradmax(D, N, L.small + 8, prob->param_const, L.blk[cand].g_p, prob->point_const, L.scal, st))) return rc;
-      if (allreduce && (rc = allreduce(ar_user, L.scal + 5, 1, 1, st))) return rc;
-    }
-    if ((rc = read_scalars())) return rc;
-    const int h_info[2] = {(int)h_scal[16], (int)h_scal[17]};
-
-    const double c_cost = h_scal[8];
-    const double quad = h_scal[0] + h_scal[9];
-    const double step_norm = sqrt(h_scal[1] + h_scal[10]);
-    const double model_change = lin ? h_scal[14] : 0.5 * quad;
-    if (h_scal[19] != 0.0) {
-      set_error("fabric barrier timed out: a peer rank did not arrive");
-      return VGG_ECUDA;
-    }
-    const bool solver_bad = h_info[0] != 0 || h_info[1] != 0 || h_scal[7] > 0 || h_scal[11] > 0 ||
-                            (lin && h_scal[22] == VGG_CG_FAILURE);
-    if (lin && cg_trace) {
-      double* ct = cg_trace + (size_t)(it - 1) * 4;
-      ct[0] = h_scal[21]; ct[1] = h_scal[22]; ct[2] = h_scal[23]; ct[3] = h_scal[24];
-    }
-    double* tr = trace ? trace + (size_t)(it - 1) * 8 : nullptr;
-    if (tr) {
-      tr[0] = it; tr[1] = cost; tr[2] = c_cost; tr[3] = model_change; tr[4] = 0; tr[5] = radius; tr[6] = step_norm; tr[7] = 0;
-    }
-    if (solver_bad || !(model_change > 0.0) || !isfinite(c_cost)) {
-      // Ceres: invalid step -> LevenbergMarquardtStrategy::StepIsInvalid
-      ++invalid_steps;
-      if (tr) tr[7] = 2;
-      if (invalid_steps >= opt.max_num_consecutive_invalid_steps) {
-        summary->termination = VGG_BA_FAILURE;
-        break;
-      }
-      radius *= 0.5;
-      continue;
-    }
-    invalid_steps = 0;
-    const double cost_change = cost - c_cost;
-    const double rho = cost_change / model_change;
-    if (tr) tr[4] = rho;
-    // Ceres ParameterToleranceReached(): step_norm <= tol * (|x| + tol), |x| over the non-constant blocks in ambient
-    // coordinates (xnorm_kernel: cameras h_scal[18] + points summed over the ranks h_scal[13] = small[5]; only evaluated
-    // when the tolerance is non-zero -- COLMAP's default is 0)
-    const double x_norm = opt.parameter_tolerance > 0.0 ? sqrt(h_scal[18] + h_scal[13]) : 0.0;
-    if (step_norm <= opt.parameter_tolerance * (x_norm + opt.parameter_tolerance)) {
-      summary->termination = VGG_BA_CONVERGENCE_PARAMETER;
-      break;
-    }
-    const bool success = rho > opt.min_relative_decrease;
-    if (fabs(cost_change) <= opt.function_tolerance * cost) {
-      // Ceres 2.x TrustRegionMinimizer::Minimize returns from FunctionToleranceReached() before IsStepSuccessful() /
-      // HandleSuccessfulStep(): the candidate of the terminating iteration is discarded
-      summary->termination = VGG_BA_CONVERGENCE_FUNCTION;
-      break;
-    }
-    if (success) {
-      cur = cand;
-      cost = c_cost;
-      summary->successful++;
-      if (tr) tr[7] = 1;
-      radius = fmin(opt.max_trust_region_radius, radius / fmax(1.0 / 3.0, 1.0 - pow(2.0 * rho - 1.0, 3.0)));
-      decrease_factor = 2.0;
-      gmax = grad_max_norm(h_scal[4], h_scal[5]);
-      if (gmax <= opt.gradient_tolerance) {
-        summary->termination = VGG_BA_CONVERGENCE_GRADIENT;
-        break;
-      }
-    } else {
-      radius = radius / decrease_factor;
-      decrease_factor *= 2.0;
-    }
+    if (lm_decide(rec, opt, lin != nullptr, it, &s, summary, trace, cg_trace)) cur = cand;
   }
 
   VGG_CUDA_CHECK(cudaMemcpyAsync(prob->poses, L.poses[cur], sizeof(double) * (size_t)S * 12, cudaMemcpyDeviceToDevice, st));
@@ -1118,8 +1096,8 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
   float ms = 0;
   VGG_CUDA_CHECK(cudaEventElapsedTime(&ms, ev0, ev1));
   summary->iterations = it;
-  summary->final_cost = cost;
-  summary->final_radius = radius;
+  summary->final_cost = s.cost;
+  summary->final_radius = s.radius;
   summary->device_ms = ms;
   summary->kernel_launches = g_launch_count;
   return VGG_OK;
@@ -1139,12 +1117,7 @@ void vgg_ba_default_linear_solver(vgg_ba_linear_solver* lin) {
 }
 
 int vgg_ba_workspace_bytes_iterative(int S, int N, int camera_model, int intr_mode, size_t* bytes) {
-  VGG_REQUIRE(S > 0 && N > 0 && bytes, "S, N must be positive");
-  Layout L;
-  const int rc = make_layout(S, N, camera_model, intr_mode, nullptr, 0, &L, true);
-  if (rc) return rc;
-  *bytes = L.bytes;
-  return VGG_OK;
+  return workspace_bytes(S, N, camera_model, intr_mode, bytes, true);
 }
 
 int vgg_ba_solve_iterative(const vgg_ba_problem* prob, const vgg_ba_options* opt, const vgg_ba_linear_solver* lin,
@@ -1182,30 +1155,23 @@ int vgg_dev_pcg_probe(const vgg_ba_problem* prob, const double* camrec, const do
   int rc = make_layout(prob->S, prob->N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L, true);
   if (rc) return rc;
   const int D = L.D;
+  const PcgOp op{prob, L.dc, L.ns, L.KR, camrec, shared_in, L.M, L.sc_c, radius, min_diag, max_diag, nullptr};
   VGG_CUDA_CHECK(cudaMemcpyAsync(L.sc_p, scale_p, sizeof(double) * (size_t)L.N * 3, cudaMemcpyDeviceToDevice, st));
   VGG_CUDA_CHECK(cudaMemcpyAsync(L.sc_c, scale_c, sizeof(double) * (size_t)D, cudaMemcpyDeviceToDevice, st));
-  VGG_CUDA_CHECK(cudaMemsetAsync(L.scal, 0, sizeof(double) * 16, st));
+  VGG_CUDA_CHECK(cudaMemsetAsync(L.scal, 0, sizeof(double) * SCAL_DOUBLES, st));
   if ((rc = launch_point_prep(L.N, H_pp, g_p, L.sc_p, prob->point_const, radius, min_diag, max_diag, L.M, L.q, L.dpp,
                               L.scal, st)))
     return rc;
-  if ((rc = launch_pcg_assemble(prob, L.dc, L.ns, L.KR, camrec, shared_in, L.M, L.q, L.pcg, nullptr, st))) return rc;
-  if ((rc = launch_pcg_init(prob, L.dc, L.ns, L.KR, camrec, shared_in, L.sc_c, radius, min_diag, max_diag, L.pcg, L.bvec,
-                            st)))
-    return rc;
+  if ((rc = launch_pcg_assemble(op, L.q, L.pcg, st))) return rc;
+  if ((rc = launch_pcg_init(op, L.pcg, L.bvec, st))) return rc;
   if (state_out)
     VGG_CUDA_CHECK(cudaMemcpyAsync(state_out, L.pcg.cg, sizeof(double) * PCG_STATE_DOUBLES, cudaMemcpyDeviceToDevice, st));
   VGG_CUDA_CHECK(cudaMemsetAsync(L.pcg.cg + CG_DONE, 0, sizeof(double), st));   // the product runs whatever init decided
   VGG_CUDA_CHECK(cudaMemcpyAsync(L.pcg.x, x_in, sizeof(double) * (size_t)D, cudaMemcpyDeviceToDevice, st));
-  if ((rc = launch_pcg_matvec(prob, L.dc, L.ns, L.KR, camrec, shared_in, L.M, L.sc_c, L.pcg.hdiag, radius, min_diag,
-                              max_diag, 0, nullptr, nullptr, L.pcg, nullptr, st)))
-    return rc;
+  if ((rc = launch_pcg_matvec(op, 0, nullptr, nullptr, L.pcg, st))) return rc;
   if ((rc = launch_pcg_combine(D, L.pcg.q, L.pcg.qs, st))) return rc;
-  auto out = [&](double* dst, const double* src, size_t n) -> int {
-    if (dst) VGG_CUDA_CHECK(cudaMemcpyAsync(dst, src, sizeof(double) * n, cudaMemcpyDeviceToDevice, st));
-    return VGG_OK;
-  };
-  if ((rc = out(y_out, L.pcg.q, D)) || (rc = out(b_out, L.bvec, D)) ||
-      (rc = out(pinv_out, L.pcg.pinv, 9 * (size_t)pcg_blocks(prob->S, L.ns))))
+  if ((rc = copy_out(y_out, L.pcg.q, D, st)) || (rc = copy_out(b_out, L.bvec, D, st)) ||
+      (rc = copy_out(pinv_out, L.pcg.pinv, 9 * (size_t)pcg_blocks(prob->S, L.ns), st)))
     return rc;
   VGG_CUDA_CHECK(cudaStreamSynchronize(st));
   return VGG_OK;

@@ -63,8 +63,8 @@ int vgg_dev_build_blocks_band(const vgg_ba_problem* prob, double* cost, double* 
  * with all-ones bytes (a NaN) instead of zeros before z_build, so the entries it writes can be told from the ones it
  * leaves; the SYRK is then not run (it adds every non-zero product, so a sentinel left in the padding columns would
  * reach rows beyond the reduced system) and Sraw holds assemble_hc's camera blocks only.  Each non-null device output
- * receives a copy: M [N,9] (row-major upper triangular), q [N,3], dpp [N,3], scal [16] (scal[6] = points whose 3x3
- * factorisation failed), Zt [Kpad,Dpad], Sraw [D,Dpad] (lower triangle valid), rhs [Dpad]; Kpad = 3N rounded up to 16, Dpad as in
+ * receives a copy: M [N,9] (row-major upper triangular), q [N,3], dpp [N,3], scal [16] (slot SCAL_PT_FAIL = 6 of csrc/ba_lm.h:
+ * points whose 3x3 factorisation failed), Zt [Kpad,Dpad], Sraw [D,Dpad] (lower triangle valid), rhs [Dpad]; Kpad = 3N rounded up to 16, Dpad as in
  * vgg_ba_schur.  workspace as vgg_ba_workspace_bytes.  Waits for the device. */
 int vgg_dev_schur_build(const vgg_ba_problem* prob, const double* camrec, const double* g_p, const double* H_pp,
                         const double* shared, const double* scale_p, double radius, double min_diag, double max_diag,
