@@ -1,11 +1,12 @@
 """K track-shard ranks emulated by K host threads of one process, meeting at a barrier for every all-reduce.
 
-Each rank runs its own solve (the oracle's lm_solve or the CUDA lm_solve on its own stream and workspace).  Every
-reduction goes through RankGroup.reduce: the rank stashes its operand, passes the turn on and waits at a
-threading.Barrier whose action checks that all ranks arrived with the same (count, op) tag, sums the operands in rank
-order (op 0) or takes their maximum (op 1, NaN-propagating) and hands the result back to every rank.  A rank whose solve
-returns arrives once more with the tag "exit", so a rank that stops while the others ask for another reduction breaks
-the barrier at once (RankGroup.error says how the tags differed) instead of waiting for the timeout.
+Each rank runs its own solve (the oracle's lm_solve or the CUDA lm_solve on its own stream and workspace; run_shards
+gives each rank its shard of the tracks).  Every reduction goes through RankGroup.reduce: the rank stashes its operand,
+passes the turn on and waits at a threading.Barrier whose action checks that all ranks arrived with the same (count, op)
+tag, sums the operands in rank order (op 0) or takes their maximum (op 1, NaN-propagating) and hands the result back to
+every rank.  A rank whose solve returns arrives once more with the tag "exit", so a rank that stops while the others ask
+for another reduction breaks the barrier at once (RankGroup.error says how the tags differed) instead of waiting for the
+timeout.
 
 The turn is a lock that a rank holds whenever it runs anything but a barrier wait.  On the GPU this means that only one
 rank has work in flight at a time and every wait happens on the host after a stream synchronisation: two solves never
@@ -106,6 +107,29 @@ class RankGroup:
         for r in range(1, self.K):
             assert self.tags[r] == self.tags[0], ("reduction sequences differ", r, self.tags[r], self.tags[0])
         return results
+
+
+def run_shards(N, K, body, device=None, timeout=120.0):
+    """body(rank, lo, hi, hook) on K ranks, rank r on tracks shard_range(N, r, K) of N, with an OracleAllReduce hook,
+    or with device a DeviceAllReduce hook and its own stream.  Returns ([body's result per rank], group); no rank
+    thread is left alive."""
+    from vggsfm_b200.dist import shard_range
+    group = RankGroup(K, timeout=timeout)
+
+    def rank(r):
+        lo, hi = shard_range(N, r, K)
+        if device is None:
+            return body(r, lo, hi, OracleAllReduce(group, r))
+        import torch
+        st = torch.cuda.Stream(device=device)
+        with torch.cuda.stream(st):
+            out = body(r, lo, hi, DeviceAllReduce(group, r))
+            st.synchronize()
+        return out
+
+    res = group.run(rank)
+    assert not [t.name for t in threading.enumerate() if t.name.startswith("rank")]
+    return res, group
 
 
 class OracleAllReduce:

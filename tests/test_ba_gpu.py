@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from oracle import ba_oracle as bo
+from tests.ba_harness import check_same_solve, check_trajectory, device_solve, options, oracle_solve, relerr
 from tests.helpers import ba_case, to_dev, unpack_camrec, rotation_angle_deg
 
 pytestmark = pytest.mark.gpu
@@ -29,10 +30,6 @@ BLOCK_CASES = CASES + [
     (33, 130, "SIMPLE_RADIAL", bo.INTR_PER_FRAME),     # frame group 1 has nf = 1
     (70, 1001, "SIMPLE_PINHOLE", bo.INTR_SHARED),      # N % 4 != 0: scalar observation loads, several groups
 ]
-
-
-def relerr(a, b):
-    return np.abs(a - b).max() / max(1e-300, np.abs(b).max())
 
 
 @functools.lru_cache(maxsize=None)
@@ -136,35 +133,10 @@ def test_schur_matches_oracle(cuda_dev, S, N, cam, mode):
     (12, 200, "SIMPLE_RADIAL", bo.INTR_PER_FRAME),
 ])
 def test_lm_trajectory_matches_oracle(cuda_dev, S, N, cam, mode):
-    import torch
-    from vggsfm_b200 import bundle_adjustment as ba
-    c = ba_case(S, N, cam, mode, seed=11)
-    trace = []
-    opt = bo.LMOptions()
-    opt.max_num_iterations = 25
-    p_ref, i_ref, x_ref, summ = bo.lm_solve(c["poses"], c["intr"], c["points"], c["uv"], c["mask"], c["model"], mode,
-                                            options=opt, trace=trace)
-    dev = cuda_dev
-    poses, intr, pts = to_dev(c["poses"], dev), to_dev(c["intr"], dev), to_dev(c["points"], dev)
-    o = ba.default_options()
-    o.max_num_iterations = 25
-    s = ba.lm_solve(to_dev(c["uv"], dev, torch.float32), to_dev(c["mask"].astype(np.uint8), dev), poses, intr, pts,
-                    c["model"], mode, options=o, want_trace=True)
-    assert s.iterations == summ["iterations"]
-    assert s.successful == summ["successful"]
-    assert s.termination == summ["termination"]
-    tr = s.trace.numpy()
-    for k, ref in enumerate(trace):
-        if ref.get("invalid"):
-            continue
-        assert abs(tr[k, 2] - ref["candidate_cost"]) <= 1e-7 * max(1.0, ref["candidate_cost"]), (k, tr[k], ref)
-        assert abs(tr[k, 5] - ref["radius"]) <= 1e-6 * ref["radius"]
-    assert abs(s.final_cost - summ["final_cost"]) <= 1e-9 * summ["final_cost"]
-    assert rotation_angle_deg(poses.cpu().numpy()[:, :, :3], p_ref[:, :, :3]).max() < 1e-6      # degrees
-    assert np.abs(poses.cpu().numpy()[:, :, 3] - p_ref[:, :, 3]).max() < 1e-7
-    assert np.abs(pts.cpu().numpy() - x_ref).max() < 1e-7
-    assert np.abs(intr.cpu().numpy() - i_ref).max() < 1e-6
-    assert s.kernel_launches > 0
+    ref, got = _solve_both(ba_case(S, N, cam, mode, seed=11), cuda_dev, 25)
+    check_trajectory(got, ref)
+    check_same_solve(got, ref)
+    assert got["s"].kernel_launches > 0
 
 
 def test_bundle_adjustment_wrapper_matches_oracle(cuda_dev):
@@ -193,40 +165,10 @@ def test_bundle_adjustment_wrapper_matches_oracle(cuda_dev):
     assert np.abs(out[3].cpu().numpy() - ref[3]).max() < 1e-7
 
 
-def _solve_both(c, cuda_dev, max_it, use_c):
-    import torch
-    from vggsfm_b200 import bundle_adjustment as ba
-    trace = []
-    opt = bo.LMOptions()
-    opt.max_num_iterations = max_it
-    p_ref, i_ref, x_ref, summ = bo.lm_solve(c["poses"], c["intr"], c["points"], c["uv"], c["mask"], c["model"], c["mode"],
-                                            options=opt, trace=trace, use_c=use_c)
-    dev = cuda_dev
-    poses, intr, pts = to_dev(c["poses"], dev), to_dev(c["intr"], dev), to_dev(c["points"], dev)
-    o = ba.default_options()
-    o.max_num_iterations = max_it
-    s = ba.lm_solve(to_dev(c["uv"], dev, torch.float32), to_dev(c["mask"].astype(np.uint8), dev), poses, intr, pts,
-                    c["model"], c["mode"], options=o, want_trace=True)
-    return (p_ref, i_ref, x_ref, summ, trace), (poses.cpu().numpy(), intr.cpu().numpy(), pts.cpu().numpy(), s)
-
-
-def _assert_same_solve(ref, got, traj_tol=1e-7):
-    """Bars of VERDICT r01 task 1b: per-iterate candidate cost 1e-7 relative, rotation geodesic <= 1e-6 degrees,
-    translation / point L2 <= 1e-7."""
-    p_ref, i_ref, x_ref, summ, trace = ref
-    poses, intr, pts, s = got
-    assert s.iterations == summ["iterations"] and s.successful == summ["successful"] and s.termination == summ["termination"]
-    tr = s.trace.numpy()
-    for k, r in enumerate(trace):
-        if r.get("invalid"):
-            continue
-        assert abs(tr[k, 2] - r["candidate_cost"]) <= traj_tol * max(1.0, r["candidate_cost"]), (k, tr[k], r)
-        assert abs(tr[k, 5] - r["radius"]) <= 1e-6 * r["radius"]
-    assert abs(s.final_cost - summ["final_cost"]) <= 1e-9 * summ["final_cost"]
-    assert rotation_angle_deg(poses[:, :, :3], p_ref[:, :, :3]).max() <= 1e-6
-    assert np.linalg.norm(poses[:, :, 3] - p_ref[:, :, 3], axis=1).max() <= 1e-7
-    assert np.linalg.norm(pts - x_ref, axis=1).max() <= 1e-7
-    assert np.abs(intr - i_ref).max() <= 1e-6
+def _solve_both(c, cuda_dev, max_it, use_c=False):
+    """the oracle's and the GPU's solve of c with default options but max_num_iterations (tests/ba_harness.py)"""
+    o, opt = options(max_num_iterations=max_it)
+    return oracle_solve(c, opt=opt, use_c=use_c), device_solve(c, cuda_dev, options=o)
 
 
 def test_c2_full_solve_matches_oracle(cuda_dev):
@@ -234,8 +176,9 @@ def test_c2_full_solve_matches_oracle(cuda_dev):
     against the oracle (C/OpenMP Jacobians + numpy Schur/Cholesky)."""
     c = ba_case(50, 2048, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME, seed=2, invisible_frac=0.3)
     ref, got = _solve_both(c, cuda_dev, 100, use_c=bo._load_c() is not None)
-    assert got[3].termination == "CONVERGENCE_GRADIENT" and got[3].iterations >= 5
-    _assert_same_solve(ref, got)
+    assert got["s"].termination == "CONVERGENCE_GRADIENT" and got["s"].iterations >= 5
+    check_trajectory(got, ref)
+    check_same_solve(got, ref)
 
 
 def test_c3_bench_config_matches_oracle(cuda_dev):
@@ -244,8 +187,9 @@ def test_c3_bench_config_matches_oracle(cuda_dev):
     (wgmma Ozaki SYRK + the in-repo Cholesky) against the oracle."""
     c = ba_case(400, 4096, "SIMPLE_RADIAL", bo.INTR_SHARED, seed=0, invisible_frac=0.0)
     ref, got = _solve_both(c, cuda_dev, 3, use_c=bo._load_c() is not None)
-    assert got[3].iterations == 3
-    _assert_same_solve(ref, got)
+    assert got["s"].iterations == 3
+    check_trajectory(got, ref)
+    check_same_solve(got, ref)
 
 
 def test_c2_full_size_properties(cuda_dev):

@@ -5,8 +5,8 @@ or the pose of a frame that no valid observation sees (tests/helpers.py hidden_c
 them reach what it computes or returns, so every case here runs the problem with hidden values and its clean twin (the
 same problem with uv = 0, points at (0, 0, 1) and the original pose in those places) and holds the two to the bars the
 existing files use: blocks at 1e-10 (test_ba_gpu.py), the Schur complement at 1e-12 sqrt(S_ii S_jj), one LM step at a
-backward error of 1e-12 in the clean twin's damped system (test_lm_step_gpu.py), whole solves with identical decisions
-and costs within EPS_COST (test_ba_lm_edges_gpu.py).  Hidden parameters come back bit for bit as given.
+backward error of 1e-12 in the clean twin's damped system, whole solves with identical decisions and costs within
+EPS_COST (tests/ba_harness.py).  Hidden parameters come back bit for bit as given.
 
 bundle_adjustment() makes such input itself: a triangulated point with a NaN or a coordinate >= max_points3D_val is
 given no observations but keeps its coordinates (as pycolmap's input conversion drops them)."""
@@ -14,33 +14,22 @@ import numpy as np
 import pytest
 
 from oracle import ba_oracle as bo
-from tests.helpers import (backward_error, banded_ba_case, hidden_case, recovered_step, reference_system,
-                           rotation_angle_deg, to_dev, unpack_camrec)
+from tests.ba_harness import (EPS_COST, SHAPES, check_one_step, check_same_solve, device_args, device_solve,
+                              first_drop, options, oracle_solve, relerr)
+from tests.helpers import banded_ba_case, hidden_case, rotation_angle_deg, to_dev, unpack_camrec
 
 pytestmark = pytest.mark.gpu
 
 FLT_MAX = float(np.finfo(np.float32).max)
 MODES = [(cam, mode) for cam in ("SIMPLE_PINHOLE", "SIMPLE_RADIAL")
          for mode in (bo.INTR_CONST, bo.INTR_PER_FRAME, bo.INTR_SHARED)]
-EPS_COST = 1e-10                     # tests/test_ba_lm_edges_gpu.py
-RADIUS = 1e4
-
-
-def relerr(a, b):
-    return np.abs(a - b).max() / max(1e-300, np.abs(b).max())
-
-
-def _dev_problem(c, dev, point_const=None):
-    import torch
-    args = (to_dev(c["uv"], dev, torch.float32), to_dev(c["mask"].astype(np.uint8), dev), to_dev(c["poses"], dev),
-            to_dev(c["intr"], dev), to_dev(c["points"], dev), c["model"], c["mode"])
-    return args, (None if point_const is None else to_dev(point_const.astype(np.uint8), dev))
 
 
 def _blocks(c, dev, tracks_per_warp=0, point_const=None):
     import torch
     from vggsfm_b200 import bundle_adjustment as ba
-    args, pc = _dev_problem(c, dev, point_const)
+    args = device_args(c, dev)
+    pc = None if point_const is None else to_dev(point_const.astype(np.uint8), dev)
     out = ba.build_blocks(*args, point_const=pc, tracks_per_warp=tracks_per_warp)
     torch.cuda.synchronize()
     return args, {k: v.cpu().numpy() if hasattr(v, "cpu") else v for k, v in out.items()}, out
@@ -130,20 +119,10 @@ def test_schur_equals_clean_twin(cuda_dev, name):
 # LM solve
 # ------------------------------------------------------------------------------------------------------------------
 
-def _gpu_solve(c, dev, param_const=None, point_const=None, **kw):
-    import torch
-    from vggsfm_b200 import bundle_adjustment as ba
+def _gpu_solve(c, dev, **kw):
     S, N = c["mask"].shape
-    pc = bo.default_param_const(S, c["model"], c["mode"]) if param_const is None else param_const
-    ptc = np.zeros(N, dtype=bool) if point_const is None else point_const
-    o = ba.default_options()
-    for k, v in kw.items():
-        setattr(o, k, v)
-    (uv, mask, poses, intr, pts, model, mode), _ = _dev_problem(c, dev)
-    s = ba.lm_solve(uv, mask, poses, intr, pts, model, mode, param_const=to_dev(pc.astype(np.uint8), dev),
-                    point_const=to_dev(ptc.astype(np.uint8), dev), options=o, want_trace=True)
-    tr = s.trace.numpy() if s.iterations else np.zeros((0, 8))
-    return s, tr, (poses.cpu().numpy(), intr.cpu().numpy(), pts.cpu().numpy())
+    return device_solve(c, dev, param_const=bo.default_param_const(S, c["model"], c["mode"]),
+                        point_const=np.zeros(N, dtype=bool), options=options(**kw)[0])
 
 
 def _hidden_frames(c):
@@ -151,11 +130,11 @@ def _hidden_frames(c):
 
 
 def _assert_hidden_as_given(dirty, got, hidden):
-    assert np.array_equal(got[2][hidden].view(np.uint64), dirty["points"][hidden].view(np.uint64))
+    assert np.array_equal(got["points"][hidden].view(np.uint64), dirty["points"][hidden].view(np.uint64))
     hf = _hidden_frames(dirty)
-    assert np.array_equal(got[0][hf].view(np.uint64), dirty["poses"][hf].view(np.uint64))
+    assert np.array_equal(got["poses"][hf].view(np.uint64), dirty["poses"][hf].view(np.uint64))
     if dirty["mode"] != bo.INTR_SHARED:
-        assert np.array_equal(got[1][hf].view(np.uint64), dirty["intr"][hf].view(np.uint64))
+        assert np.array_equal(got["intr"][hf].view(np.uint64), dirty["intr"][hf].view(np.uint64))
 
 
 @pytest.mark.parametrize("name", ["dense 8x256", "dense 45x700", "banded 160x4003"])
@@ -174,62 +153,26 @@ def test_one_step_in_clean_twins_system(cuda_dev, name):
     S, N = clean["mask"].shape
     model, mode = clean["model"], clean["mode"]
     dc, ns = bo.dims(model, mode)
-    s, tr, new = _gpu_solve(dirty, cuda_dev, max_num_iterations=1, function_tolerance=0.0, gradient_tolerance=0.0,
-                            parameter_tolerance=0.0)
-    assert s.iterations == 1 and tr[0, 7] == 1 and tr[0, 5] == RADIUS, (name, tr)
-    _assert_hidden_as_given(dirty, new, hidden)
+    got = _gpu_solve(dirty, cuda_dev, max_num_iterations=1, function_tolerance=0.0, gradient_tolerance=0.0,
+                     parameter_tolerance=0.0)
+    _assert_hidden_as_given(dirty, got, hidden)
     hf = _hidden_frames(clean)
-    new = tuple(a.copy() for a in new)
-    new[0][hf] = clean["poses"][hf]
-    new[2][hidden] = clean["points"][hidden]
+    got = dict(got, poses=got["poses"].copy(), intr=got["intr"].copy(), points=got["points"].copy())
+    got["poses"][hf] = clean["poses"][hf]
+    got["points"][hidden] = clean["points"][hidden]
     if mode != bo.INTR_SHARED:
-        new[1][hf] = clean["intr"][hf]
+        got["intr"][hf] = clean["intr"][hf]
     point_const = ~clean["mask"].any(axis=0)
     param_const = bo.default_param_const(S, model, mode)
     param_const[:S * dc] |= np.repeat(~clean["mask"].any(axis=1), dc)
-    ref = reference_system(clean, param_const, point_const, RADIUS)
-    assert abs(s.initial_cost - ref["cost"]) <= 1e-12 * ref["cost"]
-    d_c, u_c, d_p, u_p = recovered_step((clean["poses"], clean["intr"], clean["points"]), new, S, dc, ns, model, mode)
-    assert not d_c[param_const].any() and not d_p[point_const].any()
-    dcs, ucs = d_c / ref["sc_c"], u_c / ref["sc_c"]
-    dps, ups = d_p / ref["sc_p"], u_p / ref["sc_p"]
-    eta = backward_error(ref, dcs, ucs, dps, ups)
-    quad = (np.sum(dcs * dcs * ref["dcc"] / RADIUS * ref["fc"]) - np.sum(d_c * ref["gc"]) +
-            np.sum(dps * dps * ref["dpp"] / RADIUS * ref["fp"][:, None]) - np.sum(d_p * ref["gp"]))
-    step_norm = np.sqrt(np.sum(d_c * d_c) + np.sum(d_p * d_p))
-    print(f"hidden-value step {name}: eta = {eta:.2e}")
-    assert eta <= 1e-12, (name, eta)
-    assert abs(tr[0, 3] - 0.5 * quad) <= 1e-10 * abs(0.5 * quad), (name, tr[0, 3], 0.5 * quad)
-    assert abs(tr[0, 6] - step_norm) <= 1e-10 * step_norm, (name, tr[0, 6], step_norm)
-
-
-SHAPES = [                                         # tests/test_ba_lm_edges_gpu.py
-    (8, 256, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME),
-    (10, 240, "SIMPLE_RADIAL", bo.INTR_SHARED),
-    (12, 200, "SIMPLE_RADIAL", bo.INTR_PER_FRAME),
-    (16, 300, "SIMPLE_PINHOLE", bo.INTR_SHARED),
-    (9, 220, "SIMPLE_RADIAL", bo.INTR_CONST),
-    (20, 300, "SIMPLE_PINHOLE", bo.INTR_CONST),
-]
-
-
-def _between(lo, hi):
-    assert 0 < lo < hi, (lo, hi)
-    return float(np.sqrt(lo * hi))
-
-
-def _first_drop(ratio, start):
-    for k in range(start, len(ratio)):
-        if ratio[k] < min(ratio[:k]):
-            return k, _between(ratio[k], min(ratio[:k]))
-    raise AssertionError(("no decision to place", ratio))
+    check_one_step(clean, got, param_const, point_const, label=f"hidden-value step {name}")
 
 
 def _compare_solves(dirty, clean, hidden, dev, label, **kw):
     """the problem with hidden values and its clean twin through the whole solve: identical decisions, costs within
-    EPS_COST, the visible parameters at the bars of test_ba_gpu.py, hidden parameters bit for bit as given"""
-    s_d, tr_d, got_d = _gpu_solve(dirty, dev, **kw)
-    s_c, tr_c, got_c = _gpu_solve(clean, dev, **kw)
+    EPS_COST, the visible parameters at the whole-solve bars, hidden parameters bit for bit as given"""
+    d, c = _gpu_solve(dirty, dev, **kw), _gpu_solve(clean, dev, **kw)
+    s_d, tr_d, s_c, tr_c = d["s"], d["trace"], c["s"], c["trace"]
     assert (s_d.termination, s_d.iterations, s_d.successful) == (s_c.termination, s_c.iterations, s_c.successful), \
         (label, s_d.termination, s_c.termination, s_d.iterations, s_c.iterations)
     assert [int(v) for v in tr_d[:, 7]] == [int(v) for v in tr_c[:, 7]], (label, tr_d[:, 7], tr_c[:, 7])
@@ -238,26 +181,18 @@ def _compare_solves(dirty, clean, hidden, dev, label, **kw):
         for col in (1, 2):
             assert abs(tr_d[k, col] - tr_c[k, col]) <= EPS_COST * max(tr_c[k, 1], tr_c[k, 2]), (label, k, tr_d[k], tr_c[k])
         assert tr_d[k, 5] == tr_c[k, 5] or abs(tr_d[k, 5] - tr_c[k, 5]) <= 1e-6 * tr_c[k, 5], (label, k)
-    assert abs(s_d.final_cost - s_c.final_cost) <= EPS_COST * s_c.final_cost
-    _assert_hidden_as_given(dirty, got_d, hidden)
+    _assert_hidden_as_given(dirty, d, hidden)
     keep = np.setdiff1d(np.arange(clean["mask"].shape[1]), hidden)
     fr = np.setdiff1d(np.arange(clean["mask"].shape[0]), _hidden_frames(clean))
-    assert rotation_angle_deg(got_d[0][fr, :, :3], got_c[0][fr, :, :3]).max() <= 1e-6, label
-    assert np.linalg.norm(got_d[0][fr, :, 3] - got_c[0][fr, :, 3], axis=1).max() <= 1e-7, label
-    assert np.linalg.norm(got_d[2][keep] - got_c[2][keep], axis=1).max() <= 1e-7, label
-    assert np.abs(got_d[1][fr] - got_c[1][fr]).max() <= 1e-6, label
+    check_same_solve(d, c, label, cost_bar=EPS_COST, frames=fr, points=keep)
     print(f"{label}: {s_d.termination} after {s_d.iterations} iterations ({s_d.successful} accepted)")
     return s_d
 
 
 def _probe(clean, iters):
     """the oracle's trace of the clean twin with every tolerance off"""
-    trace = []
-    opt = bo.LMOptions()
-    opt.max_num_iterations = iters
-    opt.gradient_tolerance = 0.0
-    bo.lm_solve(clean["poses"], clean["intr"], clean["points"], clean["uv"], clean["mask"], clean["model"],
-                clean["mode"], options=opt, trace=trace, use_c=bo._load_c() is not None)
+    _, opt = options(max_num_iterations=iters, gradient_tolerance=0.0)
+    trace = oracle_solve(clean, opt=opt, use_c=bo._load_c() is not None)["trace"]
     assert all(r["outcome"] != 2 for r in trace)
     return trace
 
@@ -270,7 +205,7 @@ def test_solve_function_tolerance(cuda_dev, shape):
     dirty, clean, hidden = hidden_case(S, N, cam, mode, 11, np.nan, np.inf, n_hidden=4)
     dirty["points"][hidden[0]] = np.inf
     trace = _probe(clean, 12)
-    at, ftol = _first_drop([abs(r["cost_change"]) / r["cost"] for r in trace], 2)
+    at, ftol = first_drop([abs(r["cost_change"]) / r["cost"] for r in trace], 2)
     s = _compare_solves(dirty, clean, hidden, cuda_dev, f"function {shape}", function_tolerance=ftol,
                         gradient_tolerance=0.0)
     assert s.termination == "CONVERGENCE_FUNCTION" and s.iterations == at + 1
@@ -283,7 +218,7 @@ def test_solve_parameter_tolerance(cuda_dev, shape):
     S, N, cam, mode = shape
     dirty, clean, hidden = hidden_case(S, N, cam, mode, 12, np.nan, np.nan, n_hidden=4)
     trace = _probe(clean, 12)
-    at, ptol = _first_drop([r["step_norm"] / r["x_norm"] for r in trace], 1)
+    at, ptol = first_drop([r["step_norm"] / r["x_norm"] for r in trace], 1)
     s = _compare_solves(dirty, clean, hidden, cuda_dev, f"parameter {shape}", parameter_tolerance=ptol,
                         gradient_tolerance=0.0)
     assert s.termination == "CONVERGENCE_PARAMETER" and s.iterations == at + 1

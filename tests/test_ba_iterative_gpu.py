@@ -13,8 +13,8 @@ rounding.  b gets the same bar with T_i = |sc_i| (|g_i| + sum |Z q|_i).  A dropp
 an entry by about one term, far above the bar.
 
 Whole solves reach the direct solver's final cost within 1e-9 relative; one LM step matches the oracle's CG iteration
-count and termination exactly, with every zeta of the oracle's CG at least 1e-6 from eta, so that no decision sits within
-rounding of its threshold."""
+count and termination exactly, with every zeta of the oracle's CG at least 1e-6 from eta and its rho outside its band
+(tests/ba_harness.py assert_clear), so that no decision sits within rounding of its threshold."""
 import ctypes
 
 import numpy as np
@@ -22,6 +22,7 @@ import pytest
 
 from oracle import ba_oracle as bo
 from oracle import ba_pcg_oracle as po
+from tests.ba_harness import assert_clear, device_solve, options, oracle_solve
 from tests.helpers import ba_case, banded_ba_case, to_dev
 
 pytestmark = pytest.mark.gpu
@@ -171,42 +172,23 @@ def test_operator_large(cuda_dev, name):
     _check_probe(c, cuda_dev)
 
 
-def _solve(c, dev, iterative, opt=None, pc=None, ptc=None, **lin):
-    import torch
-    from vggsfm_b200 import bundle_adjustment as ba
-    S, N = c["mask"].shape
-    t = lambda a, dt=None: to_dev(a, dev, dt)
-    poses, intr, pts = t(c["poses"].reshape(S, 3, 4)).clone(), t(c["intr"]).clone(), t(c["points"]).clone()
-    summ = ba.lm_solve(t(c["uv"], torch.float32), t(c["mask"], torch.uint8), poses, intr, pts, c["model"], c["mode"],
-                       t(pc, torch.uint8) if pc is not None else None, t(ptc, torch.uint8) if ptc is not None else None,
-                       options=opt, want_trace=True,
-                       linear_solver_type="ITERATIVE_SCHUR" if iterative else "DENSE_SCHUR", **lin)
-    return summ, poses, intr, pts
+def _solve(c, dev, iterative, opt=None, **lin):
+    return device_solve(c, dev, options=opt, linear_solver="ITERATIVE_SCHUR" if iterative else "DENSE_SCHUR", **lin)["s"]
 
 
 def _tight(max_it=100):
-    from vggsfm_b200 import bundle_adjustment as ba
-    o = ba.default_options()
-    o.function_tolerance = 1e-13
-    o.gradient_tolerance = 1e-10
-    o.max_num_iterations = max_it
-    return o
+    return options(function_tolerance=1e-13, gradient_tolerance=1e-10, max_num_iterations=max_it)[0]
 
 
 @pytest.mark.parametrize("name", ["C1", "C2"])
 def test_one_lm_step_matches_oracle(cuda_dev, name):
-    from vggsfm_b200 import bundle_adjustment as ba
     c = ba_case(8, 256, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME, seed=0) if name == "C1" else \
         ba_case(50, 2048, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME, seed=1)
-    o = ba.default_options()
-    o.max_num_iterations = 1
-    summ, *_ = _solve(c, cuda_dev, True, o)
-    trace, cgs = [], []
-    po.lm_solve(c["poses"], c["intr"], c["points"], c["uv"], c["mask"], c["model"], c["mode"],
-                options=bo.LMOptions(max_num_iterations=1), trace=trace, cg_traces=cgs)
-    cs = cgs[0]
-    margins = [abs(t["zeta"] - 0.1) for t in cs["trace"] if "zeta" in t]
-    assert min(margins) > 1e-6, "an oracle zeta sits within rounding of eta"
+    o, opt = options(max_num_iterations=1)
+    summ = _solve(c, cuda_dev, True, o)
+    ref = oracle_solve(c, opt=opt, linear_solver="ITERATIVE_SCHUR")
+    trace, cs = ref["trace"], ref["cg"][0]
+    assert_clear(trace, opt, cg=ref["cg"])
     got = summ.cg_trace[0].numpy()
     assert int(got[0]) == cs["summary"]["iterations"] and int(got[1]) == cs["summary"]["termination"]
     assert abs(got[2] - cs["summary"]["zeta"]) <= 1e-6 * max(1.0, abs(cs["summary"]["zeta"]))
@@ -229,11 +211,11 @@ def test_whole_solve_reaches_the_direct_minimum(cuda_dev, name, rel):
         c = ba_case(400, 4096, "SIMPLE_RADIAL", bo.INTR_SHARED, seed=0, invisible_frac=0.0)
     else:
         c = banded_ba_case(1000, 12000, "SIMPLE_PINHOLE", bo.INTR_SHARED, life=24, seed=7)
-    sd, *_ = _solve(c, cuda_dev, False, _tight())
+    sd = _solve(c, cuda_dev, False, _tight())
     # a CG solved to rounding (eta 1e-12): the same minimum as the direct solve.  With Ceres' eta = 0.1 the truncated
     # steps converge far more slowly on these problems (at C2 the oracle's own iterative LM is 2.5 % above the minimum
     # after 100 iterations, DESIGN 4.8), which says nothing about the kernels.
-    si, *_ = _solve(c, cuda_dev, True, _tight(), eta=1e-12, max_linear_solver_iterations=500)
+    si = _solve(c, cuda_dev, True, _tight(), eta=1e-12, max_linear_solver_iterations=500)
     print(f"{name}: direct {sd.final_cost:.12g} ({sd.iterations} it, {sd.termination}), iterative {si.final_cost:.12g} "
           f"({si.iterations} it, {si.termination}, {si.cg_iterations} CG it, {si.kernel_launches} launches)")
     assert si.termination != "FAILURE_INVALID_STEPS"
@@ -243,7 +225,7 @@ def test_whole_solve_reaches_the_direct_minimum(cuda_dev, name, rel):
 @pytest.mark.parametrize("mn,mx", [(0, 0), (0, 1), (0, 2), (1, 2), (2, 2), (0, 200), (2, 200), (200, 200)])
 def test_cg_iteration_limits(cuda_dev, mn, mx):
     c = ba_case(50, 2048, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME, seed=1)
-    summ, *_ = _solve(c, cuda_dev, True, _tight(4), min_linear_solver_iterations=mn, max_linear_solver_iterations=mx)
+    summ = _solve(c, cuda_dev, True, _tight(4), min_linear_solver_iterations=mn, max_linear_solver_iterations=mx)
     for it, term, *_ in summ.cg_trace.numpy():
         it, term = int(it), int(term)
         assert 1 <= it <= max(1, mx)

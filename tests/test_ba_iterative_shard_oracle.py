@@ -6,9 +6,9 @@ The ranks sum their parts of the reduced system in another order than the unshar
 a system that differs by rounding.  Decisions must match exactly: termination, LM iterations, the outcome of every
 iteration, and per LM iteration the CG iteration count and termination.  They are clear of rounding where the unsharded
 run places them away from their thresholds, which is asserted: every zeta of every CG iteration at least 1e-6 from eta,
-rho and the function-tolerance test outside the bands of test_ba_sharded_gpu.py (costs 1e-10, model change 1e-9
-relative).  Values: costs and model changes within 1e-9 relative, poses and points within 1e-8, intrinsics within 1e-8
-relative.  Every rank makes the same sequence of reductions (RankGroup.run).
+rho and the function-tolerance test outside their bands (tests/ba_harness.py assert_clear).  Values: costs and model
+changes within 1e-9 relative, poses and points within 1e-8, intrinsics within 1e-8 relative.  Every rank makes the
+same sequence of reductions (RankGroup.run).
 
 CG iterates are not forward stable: a rounding-level change of the system grows with the CG iteration count (at C1 the
 candidate cost of the 4th LM step, after 25 CG iterations, moves by 5e-7 relative between one and two ranks, and the
@@ -21,13 +21,10 @@ from oracle import ba_oracle as bo
 from oracle import ba_pcg_oracle as po
 from tests import ba_pcg_shard_oracle as so
 from tests.ba_loss_oracle import robust, with_outliers
-from tests.emulated_ranks import OracleAllReduce, RankGroup
+from tests.ba_harness import assert_clear
+from tests.emulated_ranks import run_shards
 from tests.helpers import ba_case
 from vggsfm_b200.dist import shard_range
-
-EPS_COST = 1e-10
-EPS_MODEL = 1e-9
-ETA = 0.1
 
 
 def _shard(c, lo, hi, ptc):
@@ -53,30 +50,7 @@ def _run(c, o, lo=0, hi=None, pc=None, ptc=None, allreduce=None, max_cg=500):
 
 
 def _sharded(c, K, o, **kw):
-    N = c["mask"].shape[1]
-    group = RankGroup(K)
-
-    def rank(r):
-        lo, hi = shard_range(N, r, K)
-        return _run(c, o, lo, hi, allreduce=OracleAllReduce(group, r), **kw)
-
-    return group.run(rank), group
-
-
-def _assert_clear(ref, o):
-    for cg in ref["cg"]:
-        for t in cg["trace"]:
-            if "zeta" in t:
-                assert abs(t["zeta"] - ETA) > 1e-6, ("zeta within its band of eta", t)
-    for t in ref["trace"]:
-        if t["outcome"] == 2:
-            continue
-        cost, cc, mc, rho = t["cost"], t["candidate_cost"], t["model_change"], t["rho"]
-        cc_bar = 2 * EPS_COST * max(cost, cc)
-        rho_bar = (cc_bar + abs(rho) * EPS_MODEL * abs(mc)) / abs(mc)
-        assert abs(rho - o.min_relative_decrease) > rho_bar, ("rho within its band", t, rho_bar)
-        if o.function_tolerance > 0:
-            assert abs(abs(cost - cc) - o.function_tolerance * cost) > cc_bar, ("cost change within its band", t)
+    return run_shards(c["mask"].shape[1], K, lambda r, lo, hi, hook: _run(c, o, lo, hi, allreduce=hook, **kw))
 
 
 def _cg_key(cgs):
@@ -130,7 +104,7 @@ def test_unsharded_restatement_is_the_pcg_oracle():
 def test_shards_match_unsharded(name, K):
     c, o = _case(name)
     ref = _run(c, o)
-    _assert_clear(ref, o)
+    assert_clear(ref["trace"], o, cg=ref["cg"])
     res, _ = _sharded(c, K, o)
     _check(res, ref, f"{name} K={K}")
 
@@ -141,7 +115,7 @@ def test_empty_shard():
     o = bo.LMOptions(max_num_iterations=3)
     assert shard_range(64, 2, 3) == (64, 64)
     ref = _run(c, o)
-    _assert_clear(ref, o)
+    assert_clear(ref["trace"], o, cg=ref["cg"])
     res, group = _sharded(c, 3, o)
     _check(res, ref, "empty shard")
     assert len(group.tags[2]) == len(group.tags[0]) > 3 * ref["s"]["iterations"]
@@ -163,7 +137,7 @@ def test_constant_and_unobserved(K):
     ptc[::11] = True
     o = bo.LMOptions(max_num_iterations=3)
     ref = _run(c, o, pc=pc, ptc=ptc)
-    _assert_clear(ref, o)
+    assert_clear(ref["trace"], o, cg=ref["cg"])
     assert np.abs(ref["poses"][4] - c["poses"][4]).max() > 1e-6
     res, _ = _sharded(c, K, o, pc=pc, ptc=ptc)
     _check(res, ref, f"constant / unobserved K={K}")
@@ -177,6 +151,6 @@ def test_cauchy(K):
     o = bo.LMOptions(max_num_iterations=3)
     with robust("CAUCHY", 1.0):
         ref = _run(c, o)
-        _assert_clear(ref, o)
+        assert_clear(ref["trace"], o, cg=ref["cg"])
         res, _ = _sharded(c, K, o)
     _check(res, ref, f"CAUCHY K={K}")

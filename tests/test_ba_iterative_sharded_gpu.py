@@ -2,14 +2,14 @@
 (tests/emulated_ranks.py), each with its own stream, shard, iterative workspace and DeviceAllReduce, against the
 unsharded iterative CUDA solve of the same problem.
 
-Every rank must take the unsharded run's decisions: the same termination, LM iterations and per-iteration outcome
-(trace column 7), and per LM iteration the same CG iteration count and CG termination (cg_trace columns 0 and 1).  The
-shard sum adds the same terms as the unsharded solve in another order, so the reduced system, and with it every CG
-scalar, moves by rounding only.  The decisions are clear of that rounding where the unsharded run places them away from
-their thresholds: _assert_clear checks rho and the function-tolerance test as test_ba_sharded_gpu.py does (costs 1e-10,
-model change 1e-9 relative), and every CG stop by SUCCESS has its last zeta at least 1e-6 relative below eta.  The zetas
-of the iterations before the stop are not in the trace; that no one of them sat within rounding of eta is what the
-exact match of the CG iteration counts checks.
+Every rank must take the unsharded run's decisions: the same termination, LM iterations and per-iteration outcome (trace
+column 7), and per LM iteration the same CG iteration count and CG termination (cg_trace columns 0 and 1).  The shard
+sum adds the same terms as the unsharded solve in another order, so the reduced system, and with it every CG scalar,
+moves by rounding only.  The decisions are clear of that rounding where the unsharded run places them away from their
+thresholds: assert_clear (tests/ba_harness.py) checks rho and the function-tolerance test as test_ba_sharded_gpu.py
+does, and every CG stop by SUCCESS has its last zeta at least 1e-6 below eta.  The zetas of the iterations before the
+stop are not in the trace; that no one of them sat within rounding of eta is what the exact match of the CG iteration
+counts checks.
 
 Values are not held to test_ba_sharded_gpu.py's bars (1e-9 / 1e-8): CG iterates are not forward stable, and a
 rounding-level change of the reduced system grows with the CG iteration count and then through the LM iterations that
@@ -30,117 +30,26 @@ agree within rounding, as in the direct path.  Every rank makes the same sequenc
 many as the chunk schedule says: three before the loop, and per LM iteration one for the assembly, eleven per queued
 CG chunk (ten matvecs and the residual reset's) and two for the candidate."""
 import ctypes
-import threading
 
 import numpy as np
 import pytest
 
 from oracle import ba_oracle as bo
-from tests.emulated_ranks import DeviceAllReduce, RankGroup
+from tests.ba_harness import assert_clear, device_solve, options, radius_bar, trace_rows
+from tests.emulated_ranks import run_shards
 from tests.helpers import ba_case, banded_ba_case, shuffled_twin, to_dev
 from vggsfm_b200.dist import shard_range
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("cuda_dev")]
 
+DEV = "cuda:0"
 COST_BAR = 1e-5
 PARAM_BAR = 1e-4
-EPS_COST = 1e-10
-EPS_MODEL = 1e-9
-ETA = 0.1
 CHUNK = 10
 
 
-@pytest.fixture(autouse=True)
-def per_thread_workspace(monkeypatch, cuda_dev):
-    """lm_solve takes its workspace from a per-process cache keyed by shape: ranks with equal shard sizes would share
-    one.  Each thread gets its own cache here (dropped with the thread)."""
-    from vggsfm_b200 import _lib
-    from vggsfm_b200 import bundle_adjustment as ba
-    local = threading.local()
-
-    def workspace(S, N, model, mode, device, iterative=False):
-        cache = local.__dict__.setdefault("cache", {})
-        key = (S, N, model, mode, str(device), iterative)
-        if key not in cache:
-            import torch
-            nbytes = ctypes.c_size_t()
-            fn = _lib.lib().vgg_ba_workspace_bytes_iterative if iterative else _lib.lib().vgg_ba_workspace_bytes
-            _lib.check(fn(S, N, model, mode, ctypes.byref(nbytes)), "workspace")
-            cache[key] = torch.empty(nbytes.value, dtype=torch.uint8, device=device)
-        return cache[key]
-
-    monkeypatch.setattr(ba, "workspace", workspace)
-    yield
-    assert not [t.name for t in threading.enumerate() if t.name.startswith("rank")]
-
-
-def _opts(**kw):
-    from vggsfm_b200 import bundle_adjustment as ba
-    o = ba.default_options()
-    for k, v in kw.items():
-        setattr(o, k, v)
-    return o
-
-
-def _solve(c, o, lo=0, hi=None, pc=None, ptc=None, allreduce=None, max_cg=500, loss=("TRIVIAL", 1.0)):
-    import torch
-    from vggsfm_b200 import bundle_adjustment as ba
-    dev = torch.device("cuda:0")
-    hi = c["mask"].shape[1] if hi is None else hi
-    poses, intr, pts = to_dev(c["poses"], dev), to_dev(c["intr"], dev), to_dev(c["points"][lo:hi], dev)
-    s = ba.lm_solve(to_dev(c["uv"][:, lo:hi], dev, torch.float32), to_dev(c["mask"][:, lo:hi].astype(np.uint8), dev),
-                    poses, intr, pts, c["model"], c["mode"],
-                    param_const=None if pc is None else to_dev(pc.astype(np.uint8), dev),
-                    point_const=None if ptc is None else to_dev(ptc[lo:hi].astype(np.uint8), dev), options=o,
-                    allreduce=allreduce, want_trace=True, linear_solver_type="ITERATIVE_SCHUR",
-                    max_linear_solver_iterations=max_cg, loss_function_type=loss[0], loss_function_scale=loss[1])
-    torch.cuda.current_stream().synchronize()
-    tr = s.trace.numpy().copy() if s.iterations else np.zeros((0, 8))
-    ct = s.cg_trace.numpy().copy() if s.iterations else np.zeros((0, 4))
-    return dict(poses=poses.cpu().numpy(), intr=intr.cpu().numpy(), points=pts.cpu().numpy(), s=s, trace=tr, cg=ct,
-                calls=allreduce.calls if allreduce is not None else 0, lo=lo, hi=hi)
-
-
-def _sharded(c, K, o, **kw):
-    import torch
-    N = c["mask"].shape[1]
-    group = RankGroup(K)
-
-    def rank(r):
-        lo, hi = shard_range(N, r, K)
-        st = torch.cuda.Stream(device=torch.device("cuda:0"))
-        with torch.cuda.stream(st):
-            return _solve(c, o, lo, hi, allreduce=DeviceAllReduce(group, r), **kw)
-
-    return group.run(rank)
-
-
-def _assert_clear(ref, o):
-    """no LM decision and no CG stop of the unsharded run lies within its rounding band (module docstring)"""
-    for row, cg in zip(ref["trace"], ref["cg"]):
-        if int(cg[1]) == 0 and cg[0] > 0:
-            assert ETA - cg[2] > 1e-6 * ETA, ("zeta within its band of eta", cg)
-        if row[7] == 2:
-            continue
-        cost, cc, mc, rho = row[1], row[2], row[3], row[4]
-        cc_bar = 2 * EPS_COST * max(cost, cc)
-        rho_bar = (cc_bar + abs(rho) * EPS_MODEL * abs(mc)) / abs(mc)
-        assert abs(rho - o.min_relative_decrease) > rho_bar, ("rho within its band", row, rho_bar)
-        if o.function_tolerance > 0:
-            assert abs(abs(cost - cc) - o.function_tolerance * cost) > cc_bar, ("cost change within its band", row)
-
-
-def _radius_bar(ref):
-    """test_ba_sharded_gpu.py's derived parameter bar: 1e-8 + sum over iterations of (radius bar) x (step norm)"""
-    rad, bar = 0.0, 1e-8
-    for row in ref["trace"]:
-        if row[7] == 2:
-            continue
-        bar += rad * row[6]
-        cc_bar = 2 * EPS_COST * max(row[1], row[2])
-        if row[7] == 1:
-            rad += 18 * (cc_bar + abs(row[4]) * EPS_MODEL * abs(row[3])) / abs(row[3])
-    return bar
+def _solve(c, o, max_cg=500, **kw):
+    return device_solve(c, DEV, options=o, linear_solver="ITERATIVE_SCHUR", max_linear_solver_iterations=max_cg, **kw)
 
 
 def expected_calls(cg, max_cg):
@@ -191,9 +100,10 @@ def _check(res, ref, label="", bar=1e-4, max_cg=500):
 
 def _run_case(c, K, o, label="", derived_bar=False, max_cg=500, **kw):
     ref = _solve(c, o, max_cg=max_cg, **kw)
-    _assert_clear(ref, o)
-    res = _sharded(c, K, o, max_cg=max_cg, **kw)
-    bar = max(PARAM_BAR, _radius_bar(ref)) if derived_bar else PARAM_BAR
+    assert_clear(trace_rows(ref["trace"]), o, cg=ref["cg"])
+    res, _ = run_shards(c["mask"].shape[1], K,
+                        lambda r, lo, hi, hook: _solve(c, o, max_cg, lo=lo, hi=hi, allreduce=hook, **kw), device=DEV)
+    bar = max(PARAM_BAR, radius_bar(trace_rows(ref["trace"]))) if derived_bar else PARAM_BAR
     _check(res, ref, label, bar, max_cg)
     return ref, res
 
@@ -203,7 +113,7 @@ def _run_case(c, K, o, label="", derived_bar=False, max_cg=500, **kw):
 @pytest.mark.parametrize("K", [2, 3, 8])
 def test_c2(K):
     c = ba_case(50, 2048, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME, seed=1)
-    _run_case(c, K, _opts(max_num_iterations=10), label=f"C2 K={K}")
+    _run_case(c, K, options(max_num_iterations=10)[0], label=f"C2 K={K}")
 
 
 @pytest.mark.parametrize("K", [2, 3, 8])
@@ -224,7 +134,7 @@ def test_banded(K, shuffled):
     c = banded_ba_case(160, 4003, "SIMPLE_RADIAL", bo.INTR_SHARED, life=24, seed=31)
     if shuffled:
         c = shuffled_twin(c)
-    _run_case(c, K, _opts(max_num_iterations=5), label=f"banded shuffled={shuffled} K={K}")
+    _run_case(c, K, options(max_num_iterations=5)[0], label=f"banded shuffled={shuffled} K={K}")
 
 
 PAIRS = [("SIMPLE_PINHOLE", bo.INTR_CONST), ("SIMPLE_PINHOLE", bo.INTR_PER_FRAME), ("SIMPLE_PINHOLE", bo.INTR_SHARED),
@@ -236,7 +146,7 @@ PAIRS = [("SIMPLE_PINHOLE", bo.INTR_CONST), ("SIMPLE_PINHOLE", bo.INTR_PER_FRAME
 def test_every_dims_layout(K, cam, mode):
     """five (dc, ns) layouts at 9 x 300; the sixth, SIMPLE_RADIAL with shared intrinsics, is C3's (module docstring)"""
     c = ba_case(9, 300, cam, mode, seed=5)
-    _run_case(c, K, _opts(max_num_iterations=3), label=f"9x300 {cam} mode={mode} K={K}")
+    _run_case(c, K, options(max_num_iterations=3)[0], label=f"9x300 {cam} mode={mode} K={K}")
 
 
 @pytest.mark.parametrize("K", [2, 3, 8])
@@ -248,7 +158,7 @@ def test_cauchy_with_outliers(K):
     bad = c["mask"] & (rng.random(c["mask"].shape) < 0.1)
     uv[bad] += rng.uniform(20, 60, (int(bad.sum()), 2)) * rng.choice([-1.0, 1.0], (int(bad.sum()), 2))
     c = dict(c, uv=uv)
-    _run_case(c, K, _opts(max_num_iterations=3), label=f"CAUCHY K={K}", loss=("CAUCHY", 1.0))
+    _run_case(c, K, options(max_num_iterations=3)[0], label=f"CAUCHY K={K}", loss=("CAUCHY", 1.0))
 
 
 @pytest.mark.parametrize("K", [2, 3, 8])
@@ -269,7 +179,8 @@ def test_constant_unobserved_and_hidden(K):
     pc = bo.default_param_const(10, c["model"], c["mode"], const_pose=const_pose)
     ptc = np.zeros(400, bool)
     ptc[::7] = True
-    ref, res = _run_case(c, K, _opts(max_num_iterations=3), label=f"edges K={K}", pc=pc, ptc=ptc)
+    ref, res = _run_case(c, K, options(max_num_iterations=3)[0], label=f"edges K={K}", param_const=pc,
+                         point_const=ptc)
     for x in res:
         assert np.all(np.isinf(x["poses"][6])) and np.array_equal(x["poses"][3], c["poses"][3])
         held = ptc[x["lo"]:x["hi"]] | ~mask[:, x["lo"]:x["hi"]].any(axis=0)
@@ -282,13 +193,13 @@ def test_empty_shard(N, K):
     spans = [shard_range(N, r, K) for r in range(K)]
     assert spans[-1][0] == spans[-1][1] == N
     c = ba_case(8, N, "SIMPLE_RADIAL", bo.INTR_PER_FRAME, seed=13)
-    _run_case(c, K, _opts(max_num_iterations=3), label=f"8x{N} K={K}")
+    _run_case(c, K, options(max_num_iterations=3)[0], label=f"8x{N} K={K}")
 
 
 def _ba(c, lo, hi, mask, o, hook=None):
     import torch
     from vggsfm_b200 import bundle_adjustment as ba
-    dev = torch.device("cuda:0")
+    dev = DEV
     pts, extr, K, ex, vidx, summ = ba.bundle_adjustment(
         to_dev(c["points"][lo:hi], dev), to_dev(c["poses"], dev), to_dev(c["K"], dev), to_dev(c["extra"], dev),
         to_dev(c["uv"][:, lo:hi], dev, torch.float32), to_dev(mask[:, lo:hi], dev), shared_camera=False,
@@ -302,24 +213,15 @@ def _ba(c, lo, hi, mask, o, hook=None):
 def test_bundle_adjustment_sharded(S, N, K):
     """bundle_adjustment(..., ITERATIVE_SCHUR, allreduce=hook) on track shards against the unsharded call, by global
     track index; at 8 x 100 over 8 ranks rank 6 keeps no valid track and rank 7 has none"""
-    import torch
     c = ba_case(S, N, "SIMPLE_RADIAL", bo.INTR_PER_FRAME, seed=17)
     mask = c["mask"].copy()
     if K == 8:
         lo, hi = shard_range(N, 6, K)
         mask[1:, lo:hi] = False
         mask[0, lo:hi] = True
-    o = _opts(max_num_iterations=3)
+    o = options(max_num_iterations=3)[0]
     ref = _ba(c, 0, N, mask, o)
-    group = RankGroup(K)
-
-    def rank(r):
-        lo, hi = shard_range(N, r, K)
-        st = torch.cuda.Stream(device=torch.device("cuda:0"))
-        with torch.cuda.stream(st):
-            return _ba(c, lo, hi, mask, o, DeviceAllReduce(group, r))
-
-    res = group.run(rank)
+    res, _ = run_shards(N, K, lambda r, lo, hi, hook: _ba(c, lo, hi, mask, o, hook), device=DEV)
     pos = {int(g): j for j, g in enumerate(ref[4])}
     assert sorted(np.concatenate([x[4] for x in res]).tolist()) == sorted(pos)
     for r, x in enumerate(res):
@@ -394,15 +296,7 @@ def test_joint_ba_2500_frames_two_ranks():
                ref.final_cost)
     del ref
     torch.cuda.empty_cache()
-    group = RankGroup(2)
-
-    def rank(r):
-        lo, hi = shard_range(P, r, 2)
-        st = torch.cuda.Stream(device=dev)
-        with torch.cuda.stream(st):
-            return run(lo, hi, DeviceAllReduce(group, r))
-
-    res = group.run(rank)
+    res, _ = run_shards(P, 2, lambda r, lo, hi, hook: run(lo, hi, hook), device=dev)
     print(f"2500 x {P}: {unsharded[0]} LM it, CG {unsharded[3][:, 0].tolist()}, cost {init:.6g} -> "
           f"{unsharded[4]:.6g}")
     for s in res:
@@ -430,7 +324,7 @@ def _nccl_worker(rank, world, port, q):
     poses, intr, pts = t(c["poses"]), t(c["intr"]), t(c["points"][lo:hi])
     hook = AllReduceHook()
     s = ba.lm_solve(t(c["uv"][:, lo:hi], torch.float32), t(c["mask"][:, lo:hi].astype(np.uint8)), poses, intr, pts,
-                    c["model"], c["mode"], options=_opts(max_num_iterations=8), allreduce=hook, want_trace=True,
+                    c["model"], c["mode"], options=options(max_num_iterations=8)[0], allreduce=hook, want_trace=True,
                     linear_solver_type="ITERATIVE_SCHUR")
     q.put((rank, poses.cpu().numpy(), intr.cpu().numpy(), pts.cpu().numpy(), s.iterations, s.final_cost,
            s.cg_trace.numpy().copy(), hook.calls))
@@ -460,7 +354,7 @@ def test_two_gpu_nccl():
         p.join(timeout=120)
         assert p.exitcode == 0
     c = ba_case(12, 512, "SIMPLE_RADIAL", bo.INTR_SHARED, seed=3)
-    ref = _solve(c, _opts(max_num_iterations=8))
+    ref = _solve(c, options(max_num_iterations=8)[0])
     for rank, poses, intr, pts, its, cost, cg, calls in res:
         lo, hi = shard_range(512, rank, 2)
         assert its == ref["s"].iterations and np.array_equal(cg[:, :2], ref["cg"][:, :2])

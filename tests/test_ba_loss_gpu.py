@@ -5,8 +5,9 @@ displaced by 20-80 px, so that the weights sqrt(rho') are far from 1.
 The bars are those of the trivial loss's tests, which the robust path shares kernel for kernel: blocks at 1e-10 relative
 and the Schur complement per entry at 1e-12 sqrt(S_ii S_jj) (test_ba_gpu.py); one LM step at backward error <= 1e-12 in
 the full damped system, initial and candidate cost within 1e-12, model change and step norm within 1e-10
-(test_lm_step_gpu.py); whole solves with termination, iterations and every iteration's outcome exact, and no decision
-of the oracle's run inside its rounding band (test_ba_lm_edges_gpu.py)."""
+(tests/ba_harness.py check_one_step); whole solves with termination, iterations and every iteration's outcome exact,
+and no decision of the oracle's run inside its rounding band; DENSE_SCHUR solves also with every iteration and the
+final state at the bars of tests/ba_harness.py check_decisions (final cost within EPS_COST)."""
 import ctypes
 
 import numpy as np
@@ -14,32 +15,19 @@ import pytest
 
 from oracle import ba_oracle as bo
 from tests import ba_loss_oracle as lo
-from tests.helpers import (ba_case, backward_error, banded_ba_case, hidden_case, recovered_step, reference_system,
-                           rotation_angle_deg, shuffled_twin, to_dev, unpack_camrec)
+from tests.ba_harness import (EPS_COST, SHAPES, assert_clear, check_decisions, check_one_step, check_outcomes,
+                              device_args, device_solve, options, oracle_solve, relerr)
+from tests.emulated_ranks import run_shards
+from tests.helpers import (ba_case, banded_ba_case, hidden_case, rotation_angle_deg, shuffled_twin, to_dev,
+                           unpack_camrec)
 
 pytestmark = pytest.mark.gpu
 
 LOSSES = [("SOFT_L1", 0.5), ("SOFT_L1", 1.0), ("SOFT_L1", 4.0), ("CAUCHY", 0.5), ("CAUCHY", 1.0), ("CAUCHY", 4.0)]
-SHAPES = [(8, 256, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME), (10, 240, "SIMPLE_RADIAL", bo.INTR_SHARED),
-          (12, 200, "SIMPLE_RADIAL", bo.INTR_PER_FRAME), (16, 300, "SIMPLE_PINHOLE", bo.INTR_SHARED),
-          (9, 220, "SIMPLE_RADIAL", bo.INTR_CONST), (20, 300, "SIMPLE_PINHOLE", bo.INTR_CONST)]
-RADIUS = 1e4
-EPS_COST = 1e-10
-EPS_MODEL = 1e-9
 
 
 def _case(S, N, cam, mode, seed=11, invisible_frac=0.2):
     return lo.with_outliers(ba_case(S, N, cam, mode, seed=seed, invisible_frac=invisible_frac), seed=seed + 100)
-
-
-def _args(c, dev):
-    import torch
-    return (to_dev(c["uv"], dev, torch.float32), to_dev(c["mask"].astype(np.uint8), dev), to_dev(c["poses"], dev),
-            to_dev(c["intr"], dev), to_dev(c["points"], dev), c["model"], c["mode"])
-
-
-def relerr(a, b):
-    return np.abs(a - b).max() / max(1e-300, np.abs(b).max())
 
 
 # ---- blocks and Schur complement ---------------------------------------------------------------------------------
@@ -72,7 +60,7 @@ def _check_blocks_and_schur(dev, c, pconst, loss, a):
     D = S * dc + ns
     kw = dict(loss_function_type=loss, loss_function_scale=a)
     ref = lo.build_blocks(c["poses"], c["intr"], c["points"], c["uv"], c["mask"], model, mode, pconst, **kw)
-    args = _args(c, dev)
+    args = device_args(c, dev)
     ptc = to_dev(pconst.astype(np.uint8), dev)
     out = ba.build_blocks(*args, point_const=ptc, **kw)
     torch.cuda.synchronize()
@@ -118,39 +106,12 @@ def _check_blocks_and_schur(dev, c, pconst, loss, a):
 # ---- one LM step -------------------------------------------------------------------------------------------------
 
 def _one_step(c, dev, loss, a, label=""):
-    import torch
-    from vggsfm_b200 import bundle_adjustment as ba
     S, N = c["mask"].shape
-    model, mode = c["model"], c["mode"]
-    dc, ns = bo.dims(model, mode)
-    param_const = bo.default_param_const(S, model, mode)
+    param_const = bo.default_param_const(S, c["model"], c["mode"])
     point_const = ~c["mask"].any(axis=0)
-    args = _args(c, dev)
-    o = ba.default_options()
-    o.max_num_iterations = 1
-    o.function_tolerance = o.gradient_tolerance = o.parameter_tolerance = 0.0
-    s = ba.lm_solve(*args, param_const=to_dev(param_const.astype(np.uint8), dev),
-                    point_const=to_dev(point_const.astype(np.uint8), dev), options=o, want_trace=True,
-                    loss_function_type=loss, loss_function_scale=a)
-    new = (args[2].cpu().numpy(), args[3].cpu().numpy(), args[4].cpu().numpy())
-    tr = s.trace.numpy()
-    assert s.iterations == 1 and tr[0, 7] == 1, (label, tr)
-    with lo.robust(loss, a):
-        ref = reference_system(c, param_const, point_const, RADIUS)
-    assert abs(s.initial_cost - ref["cost"]) <= 1e-12 * ref["cost"], (label, s.initial_cost, ref["cost"])
-    d_c, u_c, d_p, u_p = recovered_step((c["poses"], c["intr"], c["points"]), new, S, dc, ns, model, mode)
-    dcs, ucs, dps, ups = d_c / ref["sc_c"], u_c / ref["sc_c"], d_p / ref["sc_p"], u_p / ref["sc_p"]
-    eta = backward_error(ref, dcs, ucs, dps, ups)
-    quad = (np.sum(dcs * dcs * ref["dcc"] / RADIUS * ref["fc"]) - np.sum(d_c * ref["gc"]) +
-            np.sum(dps * dps * ref["dpp"] / RADIUS * ref["fp"][:, None]) - np.sum(d_p * ref["gp"]))
-    step_norm = np.sqrt(np.sum(d_c * d_c) + np.sum(d_p * d_p))
-    c_cost = lo.cost_only(*new, c["uv"], c["mask"], model, loss, a)
-    print(f"lm step {label}: eta = {eta:.2e}  model change {abs(tr[0, 3] / (0.5 * quad) - 1):.1e}  "
-          f"step norm {abs(tr[0, 6] / step_norm - 1):.1e}  candidate cost {abs(tr[0, 2] / c_cost - 1):.1e}")
-    assert eta <= 1e-12, label
-    assert abs(tr[0, 3] - 0.5 * quad) <= 1e-10 * abs(0.5 * quad), label
-    assert abs(tr[0, 6] - step_norm) <= 1e-10 * step_norm, label
-    assert abs(tr[0, 2] - c_cost) <= 1e-12 * c_cost, label
+    o, _ = options(max_num_iterations=1, function_tolerance=0.0, gradient_tolerance=0.0, parameter_tolerance=0.0)
+    got = device_solve(c, dev, param_const=param_const, point_const=point_const, options=o, loss=(loss, a))
+    check_one_step(c, got, param_const, point_const, loss=(loss, a), label=label)
 
 
 @pytest.mark.parametrize("loss,a", [("SOFT_L1", 1.0), ("CAUCHY", 0.5), ("CAUCHY", 4.0)])
@@ -169,49 +130,21 @@ def test_one_lm_step_banded(cuda_dev, loss):
 
 # ---- whole solves against the oracle's LM decisions --------------------------------------------------------------
 
-def _assert_clear(trace, o):
-    """no decision of the oracle's run lies within its rounding band (test_ba_lm_edges_gpu.py)"""
-    for r in trace:
-        if r["outcome"] == 2:
-            continue
-        mc, cost, cc = r["model_change"], r["cost"], r["candidate_cost"]
-        e_cc = 2 * EPS_COST * max(cost, cc)
-        e_rho = (e_cc + abs(r["rho"]) * EPS_MODEL * abs(mc)) / abs(mc)
-        assert abs(r["rho"] - o.min_relative_decrease) > e_rho, ("rho within its band", r)
-
-
 def _solve_both(c, dev, loss, a, iters, solver="DENSE_SCHUR"):
-    from vggsfm_b200 import bundle_adjustment as ba
-    S, N = c["mask"].shape
-    opt = bo.LMOptions(max_num_iterations=iters, function_tolerance=0.0, gradient_tolerance=0.0,
-                       parameter_tolerance=0.0)
-    trace = []
-    p_r, i_r, x_r, summ = lo.lm_solve(c["poses"], c["intr"], c["points"], c["uv"], c["mask"], c["model"], c["mode"],
-                                      linear_solver=solver.lower(), loss_function_type=loss, loss_function_scale=a,
-                                      options=opt, trace=trace)
-    _assert_clear(trace, opt)
-    args = _args(c, dev)
-    o = ba.default_options()
-    o.max_num_iterations = iters
-    o.function_tolerance = o.gradient_tolerance = o.parameter_tolerance = 0.0
-    s = ba.lm_solve(*args, options=o, want_trace=True, linear_solver_type=solver, loss_function_type=loss,
-                    loss_function_scale=a)
-    tr = s.trace.numpy()
-    assert s.termination == summ["termination"] and s.iterations == summ["iterations"]
-    assert s.successful == summ["successful"]
-    assert np.array_equal(tr[:, 7], [r["outcome"] for r in trace])
-    assert abs(s.initial_cost - summ["initial_cost"]) <= 1e-12 * summ["initial_cost"]
-    out = (args[2].cpu().numpy(), args[3].cpu().numpy(), args[4].cpu().numpy())
+    o, opt = options(max_num_iterations=iters, function_tolerance=0.0, gradient_tolerance=0.0, parameter_tolerance=0.0)
+    ref = oracle_solve(c, opt=opt, linear_solver=solver, loss=(loss, a))
+    got = device_solve(c, dev, options=o, linear_solver=solver, loss=(loss, a))
+    label = f"{c['mask'].shape} {solver} {loss} {a}"
     if solver == "DENSE_SCHUR":
-        assert abs(s.final_cost - summ["final_cost"]) <= EPS_COST * summ["final_cost"]
-        assert rotation_angle_deg(out[0][:, :, :3], p_r[:, :, :3]).max() < 1e-6
-        assert np.abs(out[2] - x_r).max() < 1e-6 * max(1.0, np.abs(x_r).max())
+        check_decisions(got, ref, opt, c, label=label, cost_bar=EPS_COST)
     else:
         # a truncated CG step ends at the first iteration with zeta < eta; the two CG runs may place that test on
         # either side at a close iteration, so the steps agree to the CG's truncation, not to rounding
         # (test_ba_iterative_gpu.py)
-        assert abs(s.final_cost - summ["final_cost"]) <= 1e-5 * summ["final_cost"]
-    return s, summ
+        assert_clear(ref["trace"], opt)
+        check_outcomes(got, ref, label)
+        assert abs(got["s"].final_cost - ref["s"]["final_cost"]) <= 1e-5 * ref["s"]["final_cost"]
+    return got["s"], ref["s"]
 
 
 @pytest.mark.parametrize("loss,a", [("SOFT_L1", 0.5), ("CAUCHY", 1.0), ("CAUCHY", 4.0)])
@@ -230,13 +163,10 @@ def test_iterative_solve_decisions_match_oracle(cuda_dev, shape, loss):
 
 # ---- edges ------------------------------------------------------------------------------------------------------
 
-def _run(c, dev, iters=5, **kw):
-    from vggsfm_b200 import bundle_adjustment as ba
-    args = _args(c, dev)
-    o = ba.default_options()
-    o.max_num_iterations = iters
-    s = ba.lm_solve(*args, options=o, want_trace=True, **kw)
-    return s, tuple(t.cpu().numpy() for t in args[2:5])
+def _run(c, dev, iters=5, loss=None):
+    """loss (type, scale) None: lm_solve's default loss"""
+    got = device_solve(c, dev, options=options(max_num_iterations=iters)[0], loss=loss)
+    return got["s"], (got["poses"], got["intr"], got["points"])
 
 
 @pytest.mark.parametrize("loss", ["SOFT_L1", "CAUCHY"])
@@ -246,9 +176,9 @@ def test_hidden_values_change_nothing(cuda_dev, loss):
         dirty, clean, hidden = hidden_case(10, 200, "SIMPLE_RADIAL", bo.INTR_PER_FRAME, 7, pv, uvv,
                                       case=_case(10, 200, "SIMPLE_RADIAL", bo.INTR_PER_FRAME, seed=7))
         clean = dict(clean, poses=dirty["poses"])
-        sd, xd = _run(dirty, cuda_dev, loss_function_type=loss)
-        sc, xc = _run(clean, cuda_dev, loss_function_type=loss)
-        s2, x2 = _run(clean, cuda_dev, loss_function_type=loss)
+        sd, xd = _run(dirty, cuda_dev, loss=(loss, 1.0))
+        sc, xc = _run(clean, cuda_dev, loss=(loss, 1.0))
+        s2, x2 = _run(clean, cuda_dev, loss=(loss, 1.0))
         # a hidden point is not in the problem: it comes back as given (NaN / inf in the dirty twin)
         assert np.array_equal(xd[2][hidden], dirty["points"][hidden], equal_nan=True)
         keep = np.setdiff1d(np.arange(xd[2].shape[0]), hidden)
@@ -272,7 +202,7 @@ def test_non_finite_residual_gives_invalid_steps(cuda_dev, loss):
     s_, n_ = np.argwhere(c["mask"])[5]
     c["uv"] = c["uv"].copy()
     c["uv"][s_, n_, 0] = np.inf
-    s, x = _run(c, cuda_dev, iters=20, loss_function_type=loss)
+    s, x = _run(c, cuda_dev, iters=20, loss=(loss, 1.0))
     assert s.termination in ("FAILURE_INVALID_STEPS", "MIN_TRUST_REGION_RADIUS") and s.successful == 0
     assert np.all(s.trace.numpy()[:, 7] == 2)
     assert not np.isfinite(s.initial_cost)
@@ -283,7 +213,7 @@ def test_non_finite_residual_gives_invalid_steps(cuda_dev, loss):
 def test_explicit_trivial_is_the_default(cuda_dev):
     c = _case(8, 256, "SIMPLE_RADIAL", bo.INTR_SHARED)
     sa, xa = _run(c, cuda_dev)
-    sb, xb = _run(c, cuda_dev, loss_function_type="TRIVIAL", loss_function_scale=7.0)
+    sb, xb = _run(c, cuda_dev, loss=("TRIVIAL", 7.0))
     sc, xc = _run(c, cuda_dev)
     if sa.final_cost == sc.final_cost and all(np.array_equal(u, v) for u, v in zip(xa, xc)):
         assert sb.final_cost == sa.final_cost and np.array_equal(sb.trace.numpy(), sa.trace.numpy())
@@ -297,7 +227,7 @@ def test_explicit_trivial_is_the_default(cuda_dev):
 def test_large_scale_is_trivial(cuda_dev, loss):
     c = _case(8, 256, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME)
     st, xt = _run(c, cuda_dev, iters=3)
-    sr, xr = _run(c, cuda_dev, iters=3, loss_function_type=loss, loss_function_scale=1e8)
+    sr, xr = _run(c, cuda_dev, iters=3, loss=(loss, 1e8))
     assert abs(sr.initial_cost - st.initial_cost) <= 1e-9 * st.initial_cost
     assert abs(sr.final_cost - st.final_cost) <= 1e-9 * st.final_cost
     assert np.array_equal(sr.trace.numpy()[:, 7], st.trace.numpy()[:, 7])
@@ -309,7 +239,7 @@ def test_cauchy_rejects_outliers(cuda_dev):
     c = lo.with_outliers(ba_case(20, 600, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME, seed=2, noise_px=0.3), frac=0.1, seed=3)
     gt = c["scene"].extrinsics[:, :, :3]
     st, xt = _run(c, cuda_dev, iters=50)
-    sr, xr = _run(c, cuda_dev, iters=50, loss_function_type="CAUCHY")
+    sr, xr = _run(c, cuda_dev, iters=50, loss=("CAUCHY", 1.0))
     rel = lambda R: R[1:] @ R[0].T                      # rotations relative to the first frame: free of the gauge
     et = np.median(rotation_angle_deg(rel(xt[0][:, :, :3]), rel(gt)))
     er = np.median(rotation_angle_deg(rel(xr[0][:, :, :3]), rel(gt)))
@@ -317,55 +247,22 @@ def test_cauchy_rejects_outliers(cuda_dev):
     assert er < 0.5 * et
 
 
-def test_sharded_cauchy_matches_unsharded(cuda_dev, monkeypatch):
+def test_sharded_cauchy_matches_unsharded(cuda_dev):
     """two and three emulated ranks (tests/emulated_ranks.py) with CAUCHY against the unsharded robust solve"""
-    import threading
-
-    import torch
-    from tests.emulated_ranks import DeviceAllReduce, RankGroup
-    from vggsfm_b200 import bundle_adjustment as ba
-    from vggsfm_b200.dist import shard_range
     c = _case(12, 512, "SIMPLE_RADIAL", bo.INTR_SHARED, seed=3)
-    N = c["mask"].shape[1]
-    ref, xref = _run(c, cuda_dev, iters=8, loss_function_type="CAUCHY")
-    # lm_solve takes its workspace from a per-process cache keyed by shape, which ranks with equal shards would share:
-    # each rank thread gets its own cache (as test_ba_sharded_gpu.py does), installed here on the main thread and
-    # restored by monkeypatch when the test ends
-    local = threading.local()
-
-    def workspace(S, N_, model, mode, device, iterative=False):
-        cache = local.__dict__.setdefault("cache", {})
-        key = (S, N_, model, mode, str(device), iterative)
-        if key not in cache:
-            cache[key] = torch.empty(ba.workspace_bytes(S, N_, model, mode, iterative), dtype=torch.uint8,
-                                     device=device)
-        return cache[key]
-
-    monkeypatch.setattr(ba, "workspace", workspace)
+    o, _ = options(max_num_iterations=8)
+    cauchy = ("CAUCHY", 1.0)
+    ref = device_solve(c, cuda_dev, options=o, loss=cauchy)
     for K in (2, 3):
-        group = RankGroup(K)
-
-        def rank(r):
-            lo_, hi_ = shard_range(N, r, K)
-            st = torch.cuda.Stream(device=cuda_dev)
-            with torch.cuda.stream(st):
-                sub = dict(c, uv=c["uv"][:, lo_:hi_], mask=c["mask"][:, lo_:hi_], points=c["points"][lo_:hi_])
-                args = _args(sub, cuda_dev)
-                o = ba.default_options()
-                o.max_num_iterations = 8
-                s = ba.lm_solve(*args, options=o, want_trace=True, allreduce=DeviceAllReduce(group, r),
-                                loss_function_type="CAUCHY")
-                torch.cuda.current_stream().synchronize()
-            return dict(s=s, poses=args[2].cpu().numpy(), points=args[4].cpu().numpy(), lo=lo_, hi=hi_)
-
-        res = group.run(rank)
+        res, _ = run_shards(c["mask"].shape[1], K, lambda r, lo_, hi_, hook: device_solve(
+            c, cuda_dev, lo_, hi_, options=o, allreduce=hook, loss=cauchy), device=cuda_dev)
         for x in res:
             s = x["s"]
-            assert s.termination == ref.termination and s.iterations == ref.iterations
-            assert np.array_equal(s.trace.numpy()[:, 7], ref.trace.numpy()[:, 7])
-            assert np.isclose(s.final_cost, ref.final_cost, rtol=1e-9, atol=0)
-            assert np.abs(x["poses"] - xref[0]).max() < 1e-8
-            assert np.abs(x["points"] - xref[2][x["lo"]:x["hi"]]).max() < 1e-8
+            assert s.termination == ref["s"].termination and s.iterations == ref["s"].iterations
+            assert np.array_equal(x["trace"][:, 7], ref["trace"][:, 7])
+            assert np.isclose(s.final_cost, ref["s"].final_cost, rtol=1e-9, atol=0)
+            assert np.abs(x["poses"] - ref["poses"]).max() < 1e-8
+            assert np.abs(x["points"] - ref["points"][x["lo"]:x["hi"]]).max() < 1e-8
 
 
 # ---- argument errors and the pycolmap-shaped options ---------------------------------------------------------------
@@ -377,7 +274,7 @@ def test_bad_loss_is_einval_before_any_launch(cuda_dev, ltype, scale):
     from vggsfm_b200 import bundle_adjustment as ba
     L = _lib.lib()
     c = _case(8, 256, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME)
-    uv, mask, poses, intr, pts, model, mode = _args(c, cuda_dev)
+    uv, mask, poses, intr, pts, model, mode = device_args(c, cuda_dev)
     S, N = mask.shape
     pc = ba.default_param_const(S, model, mode, cuda_dev)
     p = ba._problem(uv, mask, poses, intr, pts, model, mode, pc, None)
@@ -407,9 +304,9 @@ def test_unknown_loss_name_raises(cuda_dev):
     from vggsfm_b200 import bundle_adjustment as ba
     c = _case(8, 256, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME)
     with pytest.raises(ValueError):
-        ba.lm_solve(*_args(c, cuda_dev), loss_function_type="HUBER")
+        ba.lm_solve(*device_args(c, cuda_dev), loss_function_type="HUBER")
     with pytest.raises(ValueError):
-        ba.lm_solve(*_args(c, cuda_dev), loss_function_type="cauchy")
+        ba.lm_solve(*device_args(c, cuda_dev), loss_function_type="cauchy")
 
 
 def test_pycolmap_options_carry_the_loss(cuda_dev):

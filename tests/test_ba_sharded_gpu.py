@@ -2,150 +2,48 @@
 each with its own stream, shard and workspace, reducing through the solver's all-reduce hook.  This is the path
 `bench.py --gpus N` runs over NCCL; test_dist_gpu.py needs two GPUs and test_dist_gloo.py runs the oracle only.
 
-The reference is the unsharded CUDA solve of the same problem (and the float64 oracle where a decision is placed).
-Every rank must take the unsharded run's decisions: the same termination, iterations and per-iteration outcome (trace
-column 7).  Values use test_dist_gpu.py's bars: final cost within 1e-9 relative, candidate costs (trace column 2)
-within 1e-8 relative, poses and points within 1e-8, intrinsics within 1e-8 relative.  The sum over shards adds the
-same terms as the unsharded solve in another order, which moves the reduced system by rounding only; these bars hold
-while no decision lies within its rounding band, so every run stops by max_num_iterations or by a tolerance placed
-between two iterations, and _assert_clear checks on the unsharded trace that rho and the function-tolerance test are
-outside the bands of test_ba_lm_edges_gpu.py (cost 1e-10, model change 1e-9 relative).  Every rank must also make
-the same sequence of reductions (RankGroup.run), at least two per iteration, and hold the same cameras: bit-identical
-where the bordered reduced system fits one 128-wide Cholesky panel (D + 1 <= 128), since then every rank factors the
-same matrix with the same arithmetic.  Beyond one panel the trailing updates of csrc/chol.cu accumulate with atomicAdd,
-so two factorisations of the same matrix may differ in the last bits; there the cameras of the ranks agree within the
-same bars as against the unsharded run.
+The reference is the unsharded CUDA solve of the same problem (and the float64 oracle where a decision is placed). Every
+rank must take the unsharded run's decisions: the same termination, iterations and per-iteration outcome (trace column
+7).  Values use test_dist_gpu.py's bars: final cost within 1e-9 relative, candidate costs (trace column 2) within 1e-8
+relative, poses and points within 1e-8, intrinsics within 1e-8 relative.  The sum over shards adds the same terms as the
+unsharded solve in another order, which moves the reduced system by rounding only; these bars hold while no decision
+lies within its rounding band, so every run stops by max_num_iterations or by a tolerance placed between two iterations,
+and assert_clear checks on the unsharded trace that rho and the function-tolerance test are outside their bands
+(tests/ba_harness.py).  Every rank must also make the same sequence of reductions (RankGroup.run), at least two per
+iteration, and hold the same cameras: bit-identical where the bordered reduced system fits one 128-wide Cholesky panel
+(D + 1 <= 128), since then every rank factors the same matrix with the same arithmetic.  Beyond one panel the trailing
+updates of csrc/chol.cu accumulate with atomicAdd, so two factorisations of the same matrix may differ in the last bits;
+there the cameras of the ranks agree within the same bars as against the unsharded run.
 
 C3 (D = 2402, 10 iterations) widens the parameter bar by a derived term.  The shard sum evaluates the costs in another
-order, so rho of each step carries the rounding band e_rho of test_ba_lm_edges_gpu.py (costs 1e-10, model change 1e-9
-relative), and an accepted step multiplies the radius by a factor whose relative derivative in rho is at most 18: the
-radius of iteration k may differ by rad_k = sum of 18 e_rho over the accepted steps before it.  The LM step
-d = -(H + D/radius)^-1 g moves by at most |d| times the relative change of the radius, so the parameters may differ by
-1e-8 + sum_k rad_k |d_k| (trace column 6).  Measured on an H100 80GB HBM3: up to 7.9e-8 in a point at 8 ranks, varying
-between runs by a factor of about 5 (two unsharded runs agree to 3e-11)."""
-import ctypes
-import threading
-import time
-
+order, so rho of each step carries the rounding band e_rho of tests/ba_harness.py, and an accepted step multiplies the
+radius by a factor whose relative derivative in rho is at most 18: the radius of iteration k may differ by rad_k = sum
+of 18 e_rho over the accepted steps before it.  The LM step d = -(H + D/radius)^-1 g moves by at most |d| times the
+relative change of the radius, so the parameters may differ by 1e-8 + sum_k rad_k |d_k| (trace column 6).  Measured on
+an H100 80GB HBM3: up to 7.9e-8 in a point at 8 ranks, varying between runs by a factor of about 5 (two unsharded runs
+agree to 3e-11)."""
 import numpy as np
 import pytest
 
 from oracle import ba_oracle as bo
 from oracle import band_oracle
-from tests.emulated_ranks import DeviceAllReduce, RankGroup
+from tests.ba_harness import assert_clear, band_record, device_solve, options, radius_bar, trace_rows
+from tests.emulated_ranks import run_shards
 from tests.helpers import ba_case, banded_ba_case, far_points_first_case, to_dev
 from vggsfm_b200.dist import shard_range
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("cuda_dev")]
 
-EPS_COST = 1e-10
-EPS_MODEL = 1e-9
+DEV = "cuda:0"
 C3 = (400, 4096, "SIMPLE_RADIAL", bo.INTR_SHARED)
 
 
-@pytest.fixture(autouse=True)
-def per_thread_workspace(monkeypatch, cuda_dev):
-    """lm_solve takes its workspace from a per-process cache keyed by shape: ranks with equal shard sizes would share
-    one.  Each thread gets its own cache here (dropped with the thread)."""
-    from vggsfm_b200 import _lib
-    from vggsfm_b200 import bundle_adjustment as ba
-    local = threading.local()
+def _sharded(c, K, o, band=False, **kw):
+    """the solve on K emulated ranks: per rank device_solve's result (with the band hint it took)"""
+    def body(r, lo, hi, hook):
+        return dict(device_solve(c, DEV, lo, hi, options=o, allreduce=hook, **kw), band=band_record() if band else None)
 
-    def workspace(S, N, model, mode, device):
-        cache = local.__dict__.setdefault("cache", {})
-        key = (S, N, model, mode, str(device))
-        if key not in cache:
-            import torch
-            nbytes = ctypes.c_size_t()
-            _lib.check(_lib.lib().vgg_ba_workspace_bytes(S, N, model, mode, ctypes.byref(nbytes)), "workspace")
-            cache[key] = torch.empty(nbytes.value, dtype=torch.uint8, device=device)
-        return cache[key]
-
-    monkeypatch.setattr(ba, "workspace", workspace)
-    t0 = time.perf_counter()
-    yield
-    print(f"wall {time.perf_counter() - t0:.2f} s")
-    assert not [t.name for t in threading.enumerate() if t.name.startswith("rank")]
-
-
-def _opts(**kw):
-    from vggsfm_b200 import bundle_adjustment as ba
-    o = ba.default_options()
-    for k, v in kw.items():
-        setattr(o, k, v)
-    return o
-
-
-def _band_record():
-    """the band hint of the most recent solve on the calling thread (vgg_dev_last_band_hint)"""
-    from vggsfm_b200 import _lib
-    L = _lib.lib()
-    meta = np.zeros(8, dtype=np.int32)
-    _lib.check(L.vgg_dev_last_band_hint(meta.ctypes.data, None, None, None, None), "vgg_dev_last_band_hint")
-    rb = np.zeros((int(meta[3]), 2), np.int32)
-    _lib.check(L.vgg_dev_last_band_hint(meta.ctypes.data, rb.ctypes.data, None, None, None), "vgg_dev_last_band_hint")
-    return dict(active=int(meta[0]), chol=int(meta[1]), tables=int(meta[2]), rb_range=rb)
-
-
-def _solve(c, o, lo=0, hi=None, param_const=None, point_const=None, allreduce=None, band=False):
-    """lm_solve of tracks [lo, hi) on the current thread and stream; host copies of the results"""
-    import torch
-    from vggsfm_b200 import bundle_adjustment as ba
-    dev = torch.device("cuda:0")
-    hi = c["mask"].shape[1] if hi is None else hi
-    poses, intr, pts = to_dev(c["poses"], dev), to_dev(c["intr"], dev), to_dev(c["points"][lo:hi], dev)
-    pc = None if param_const is None else to_dev(param_const.astype(np.uint8), dev)
-    ptc = None if point_const is None else to_dev(point_const[lo:hi].astype(np.uint8), dev)
-    s = ba.lm_solve(to_dev(c["uv"][:, lo:hi], dev, torch.float32), to_dev(c["mask"][:, lo:hi].astype(np.uint8), dev),
-                    poses, intr, pts, c["model"], c["mode"], param_const=pc, point_const=ptc, options=o,
-                    allreduce=allreduce, want_trace=True)
-    torch.cuda.current_stream().synchronize()
-    tr = s.trace.numpy().copy() if s.iterations else np.zeros((0, 8))
-    return dict(poses=poses.cpu().numpy(), intr=intr.cpu().numpy(), points=pts.cpu().numpy(), s=s, trace=tr,
-                calls=allreduce.calls if allreduce is not None else 0, band=_band_record() if band else None)
-
-
-def _sharded(c, K, o, param_const=None, point_const=None, band=False):
-    """the solve on K emulated ranks; per rank the result of _solve plus its shard (lo, hi)"""
-    import torch
-    N = c["mask"].shape[1]
-    group = RankGroup(K)
-
-    def rank(r):
-        lo, hi = shard_range(N, r, K)
-        st = torch.cuda.Stream(device=torch.device("cuda:0"))
-        with torch.cuda.stream(st):
-            out = _solve(c, o, lo, hi, param_const, point_const, DeviceAllReduce(group, r), band)
-        return dict(out, lo=lo, hi=hi)
-
-    res = group.run(rank)
-    return res, group
-
-
-def _assert_clear(ref, o):
-    """no decision of the unsharded run lies within its rounding band (module docstring)"""
-    for row in ref["trace"]:
-        if row[7] == 2:
-            continue
-        cost, cc, mc, rho = row[1], row[2], row[3], row[4]
-        cc_bar = 2 * EPS_COST * max(cost, cc)
-        rho_bar = (cc_bar + abs(rho) * EPS_MODEL * abs(mc)) / abs(mc)
-        assert abs(rho - o.min_relative_decrease) > rho_bar, ("rho within its band", row, rho_bar)
-        if o.function_tolerance > 0:
-            assert abs(abs(cost - cc) - o.function_tolerance * cost) > cc_bar, ("cost change within its band", row)
-
-
-def _radius_bar(ref):
-    """1e-8 + sum over iterations of (radius bar) x (step norm), as derived in the module docstring"""
-    rad, bar = 0.0, 1e-8
-    for row in ref["trace"]:
-        if row[7] == 2:
-            continue
-        bar += rad * row[6]
-        cc_bar = 2 * EPS_COST * max(row[1], row[2])
-        if row[7] == 1:
-            rad += 18 * (cc_bar + abs(row[4]) * EPS_MODEL * abs(row[3])) / abs(row[3])
-    return bar
+    return run_shards(c["mask"].shape[1], K, body, device=DEV)
 
 
 def _single_panel(c):
@@ -180,10 +78,10 @@ def _check(res, ref, label="", bar=1e-8, exact_cameras=True):
 
 
 def _run_case(c, K, o, param_const=None, point_const=None, label="", derived_bar=False):
-    ref = _solve(c, o, param_const=param_const, point_const=point_const)
-    _assert_clear(ref, o)
-    res, group = _sharded(c, K, o, param_const, point_const)
-    bar = _radius_bar(ref) if derived_bar else 1e-8
+    ref = device_solve(c, DEV, options=o, param_const=param_const, point_const=point_const)
+    assert_clear(trace_rows(ref["trace"]), o)
+    res, group = _sharded(c, K, o, param_const=param_const, point_const=point_const)
+    bar = radius_bar(trace_rows(ref["trace"])) if derived_bar else 1e-8
     _check(res, ref, label, bar, _single_panel(c))
     if derived_bar:
         print(f"{label}: parameter bar {bar:.3g}")
@@ -196,8 +94,8 @@ def test_one_rank_through_the_hook():
     """K = 1: the hook 'sums' one term, so the solve through it is the solve without it.  Bit-identical when two runs
     without the hook are (the Jacobian kernels accumulate with float atomics, whose order may vary between runs)."""
     c = ba_case(8, 256, "SIMPLE_PINHOLE", bo.INTR_PER_FRAME, seed=11)
-    o = _opts(max_num_iterations=8)
-    a, b = _solve(c, o), _solve(c, o)
+    o = options(max_num_iterations=8)[0]
+    a, b = device_solve(c, DEV, options=o), device_solve(c, DEV, options=o)
     res, _ = _sharded(c, 1, o)
     x = dict(res[0])
     same = all(np.array_equal(a[k], b[k]) for k in ("poses", "intr", "points", "trace"))
@@ -206,14 +104,14 @@ def test_one_rank_through_the_hook():
         for k in ("poses", "intr", "points", "trace"):
             assert np.array_equal(x[k], a[k]), k
         assert x["s"].final_cost == a["s"].final_cost and x["s"].iterations == a["s"].iterations
-    _assert_clear(a, o)
+    assert_clear(trace_rows(a["trace"]), o)
     _check(res, a, "K=1")
 
 
 @pytest.mark.parametrize("K", [2, 3, 4, 8])
 def test_shards_match_unsharded(K):
     c = ba_case(12, 512, "SIMPLE_RADIAL", bo.INTR_SHARED, seed=3)
-    _run_case(c, K, _opts(max_num_iterations=8), label=f"12x512 K={K}")
+    _run_case(c, K, options(max_num_iterations=8)[0], label=f"12x512 K={K}")
 
 
 @pytest.mark.parametrize("mode", [bo.INTR_CONST, bo.INTR_PER_FRAME, bo.INTR_SHARED])
@@ -221,7 +119,7 @@ def test_shards_match_unsharded(K):
 def test_every_dims_layout(cam, mode):
     """every (dc, ns) layout of the reduced system and the small vector through the reductions"""
     c = ba_case(9, 300, cam, mode, seed=5)
-    _run_case(c, 3, _opts(max_num_iterations=6), label=f"9x300 {cam} mode={mode} K=3")
+    _run_case(c, 3, options(max_num_iterations=6)[0], label=f"9x300 {cam} mode={mode} K=3")
 
 
 @pytest.mark.parametrize("N,K", [(100, 8), (64, 3)])
@@ -231,7 +129,7 @@ def test_ragged_and_empty_shards(N, K):
     spans = [shard_range(N, r, K) for r in range(K)]
     assert spans[-1][0] == spans[-1][1] == N
     c = ba_case(8, N, "SIMPLE_RADIAL", bo.INTR_PER_FRAME, seed=13)
-    _run_case(c, K, _opts(max_num_iterations=6), label=f"8x{N} K={K}")
+    _run_case(c, K, options(max_num_iterations=6)[0], label=f"8x{N} K={K}")
 
 
 @pytest.mark.parametrize("mode", [bo.INTR_PER_FRAME, bo.INTR_SHARED])
@@ -245,7 +143,7 @@ def test_frame_seen_in_one_shard(mode):
     mask[5, hi:] = False
     assert mask[5, lo:hi].sum() >= 20
     c = dict(c, mask=mask)
-    ref, res = _run_case(c, K, _opts(max_num_iterations=6), label=f"frame seen by one shard, mode={mode}")
+    ref, res = _run_case(c, K, options(max_num_iterations=6)[0], label=f"frame seen by one shard, mode={mode}")
     moved = np.abs(ref["poses"][5] - c["poses"][5]).max()
     assert moved > 1e-6, moved
 
@@ -274,7 +172,7 @@ def test_gradient_max_decides():
     assert abs(tr[1]["gmax"] - g[top[-1]]) <= 1e-9 * g[top[-1]] and tr[0]["gmax"] > 10 * gtol
     order = np.concatenate([np.delete(np.arange(N), top[-1]), [top[-1]]])
     c = dict(c, points=c["points"][order].copy(), uv=c["uv"][:, order].copy(), mask=c["mask"][:, order].copy())
-    o = _opts(gradient_tolerance=gtol, function_tolerance=0.0, max_num_iterations=10)
+    o = options(gradient_tolerance=gtol, function_tolerance=0.0, max_num_iterations=10)[0]
     for K in (2, 4):
         ref, res = _run_case(c, K, o, param_const=pc, label=f"gradient K={K}")
         assert ref["s"].termination == "CONVERGENCE_GRADIENT" and ref["s"].iterations == 3, ref["s"]
@@ -295,7 +193,7 @@ def test_parameter_tolerance_over_shards(K, ptol):
     ratios = [t["step_norm"] / (ptol * (t["x_norm"] + ptol)) for t in tr if t["outcome"] != 2]
     assert summ["termination"] == "CONVERGENCE_PARAMETER" and ratios[-1] < 1.0 - 1e-6
     assert all(q > 1.0 + 1e-6 for q in ratios[:-1]), ratios
-    o = _opts(parameter_tolerance=ptol, gradient_tolerance=0.0, function_tolerance=0.0, max_num_iterations=20)
+    o = options(parameter_tolerance=ptol, gradient_tolerance=0.0, function_tolerance=0.0, max_num_iterations=20)[0]
     ref, res = _run_case(c, K, o, label=f"parameter tolerance {ptol} K={K}")
     assert ref["s"].termination == "CONVERGENCE_PARAMETER" and ref["s"].iterations == summ["iterations"], ref["s"]
     assert [int(v) for v in ref["trace"][:, 7]] == [t["outcome"] for t in tr]
@@ -311,8 +209,8 @@ def test_nan_observation_in_one_shard():
     uv = c["uv"].copy()
     uv[s, lo + n, 1] = np.nan
     c = dict(c, uv=uv)
-    o = _opts()
-    ref = _solve(c, o)
+    o = options()[0]
+    ref = device_solve(c, DEV, options=o)
     res, _ = _sharded(c, K, o)
     assert ref["s"].termination == "FAILURE_INVALID_STEPS"
     _check(res, ref, "NaN observation")
@@ -328,12 +226,12 @@ def test_banded_shards():
     Cholesky.  Both must agree."""
     c = banded_ba_case(128, 4096, "SIMPLE_RADIAL", bo.INTR_SHARED, life=20, seed=33)
     dc, ns = bo.dims(c["model"], c["mode"])
-    o = _opts(max_num_iterations=5)
-    ref = _solve(c, o, band=True)
-    b = ref["band"]
+    o = options(max_num_iterations=5)[0]
+    ref = device_solve(c, DEV, options=o)
+    b = band_record()
     assert b["active"] and b["chol"] and b["tables"], b
     assert b["rb_range"].shape[0] >= 6 and (128 * dc) // 128 >= 4
-    _assert_clear(ref, o)
+    assert_clear(trace_rows(ref["trace"]), o)
     K = 2
     res, _ = _sharded(c, K, o, band=True)
     for x in res:
@@ -352,9 +250,9 @@ def test_c3(K):
     benchmark's multi-GPU runs"""
     S, N, cam, mode = C3
     c = ba_case(S, N, cam, mode, seed=0, invisible_frac=0.0)
-    o = _opts(max_num_iterations=10)
+    o = options(max_num_iterations=10)[0]
     ref, res = _run_case(c, K, o, label=f"C3 K={K}", derived_bar=True)
-    again = _solve(c, o)
+    again = device_solve(c, DEV, options=o)
     print(f"C3 K={K}: largest difference to the unsharded run: poses "
           f"{max(np.abs(x['poses'] - ref['poses']).max() for x in res):.3g}, points "
           f"{max(np.abs(x['points'] - ref['points'][x['lo']:x['hi']]).max() for x in res):.3g}; "
@@ -363,28 +261,16 @@ def test_c3(K):
 
 
 def _ba_sharded(c, K, o, mask):
-    """bundle_adjustment() of every rank's track shard: per rank (points, extrinsics, K, extra, global valid index)"""
-    import torch
-    N = mask.shape[1]
-    group = RankGroup(K)
-    dev = torch.device("cuda:0")
-
-    def rank(r):
-        lo, hi = shard_range(N, r, K)
-        st = torch.cuda.Stream(device=dev)
-        with torch.cuda.stream(st):
-            hook = DeviceAllReduce(group, r)
-            out = _ba(c, lo, hi, mask, o, hook)
-            st.synchronize()
-        return out + (hook.calls,)
-
-    return group.run(rank)
+    """bundle_adjustment() of every rank's track shard: per rank (points, extrinsics, K, extra, global valid index,
+    iterations, termination, hook calls)"""
+    return run_shards(mask.shape[1], K, lambda r, lo, hi, hook: _ba(c, lo, hi, mask, o, hook) + (hook.calls,),
+                      device=DEV)[0]
 
 
 def _ba(c, lo, hi, mask, o, hook=None):
     import torch
     from vggsfm_b200 import bundle_adjustment as ba
-    dev = torch.device("cuda:0")
+    dev = DEV
     extra = to_dev(c["extra"], dev) if c["extra"] is not None else None
     pts, extr, K, ex, vidx, summ = ba.bundle_adjustment(
         to_dev(c["points"][lo:hi], dev), to_dev(c["poses"], dev), to_dev(c["K"], dev), extra,
@@ -406,7 +292,7 @@ def test_bundle_adjustment_sharded(S, N, K):
         assert (lo, hi) == (96, 100) and shard_range(N, 7, K) == (100, 100)
         mask[1:, lo:hi] = False
         mask[0, lo:hi] = True
-    o = _opts(max_num_iterations=6)
+    o = options(max_num_iterations=6)[0]
     ref = _ba(c, 0, N, mask, o)
     res = _ba_sharded(c, K, o, mask)
     pos = {int(g): j for j, g in enumerate(ref[4])}

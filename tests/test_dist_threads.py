@@ -12,45 +12,22 @@ import numpy as np
 import pytest
 
 from oracle import ba_oracle as bo
-from tests.emulated_ranks import OracleAllReduce, RankGroup, RanksFailed
+from tests.ba_harness import oracle_solve
+from tests.emulated_ranks import RankGroup, RanksFailed, run_shards
 from tests.helpers import far_points_first_case
 from vggsfm_b200.dist import shard_range
 
 
-def run_sharded(c, K, opt, point_const=None):
-    """the oracle's lm_solve on K emulated ranks: per rank (poses, intr, points, summary, trace)"""
-    N = c["mask"].shape[1]
-    group = RankGroup(K, timeout=60.0)
-
-    def rank(r):
-        lo, hi = shard_range(N, r, K)
-        tr = []
-        ptc = None if point_const is None else point_const[lo:hi]
-        out = bo.lm_solve(c["poses"], c["intr"], c["points"][lo:hi], c["uv"][:, lo:hi], c["mask"][:, lo:hi], c["model"],
-                          c["mode"], point_const=ptc, options=opt, trace=tr, allreduce=OracleAllReduce(group, r))
-        return out + (tr,)
-
-    return group.run(rank), group
-
-
-def options(**kw):
-    o = bo.LMOptions()
-    o.max_num_iterations = 20
-    o.function_tolerance = o.gradient_tolerance = 0.0
-    for k, v in kw.items():
-        setattr(o, k, v)
-    return o
-
-
-def check_against_unsharded(c, res, summ0, trace0):
-    for r, (p, i, x, summ, tr) in enumerate(res):
+def check_against_unsharded(res, ref):
+    for r, x in enumerate(res):
+        summ, summ0 = x["s"], ref["s"]
         assert summ["termination"] == summ0["termination"], (r, summ["termination"], summ0["termination"])
         assert summ["iterations"] == summ0["iterations"] and summ["successful"] == summ0["successful"], (r, summ)
-        assert [t["outcome"] for t in tr] == [t["outcome"] for t in trace0]
-        for t, t0 in zip(tr, trace0):
+        assert [t["outcome"] for t in x["trace"]] == [t["outcome"] for t in ref["trace"]]
+        for t, t0 in zip(x["trace"], ref["trace"]):
             assert abs(t["x_norm"] - t0["x_norm"]) <= 1e-12 * t0["x_norm"], (r, t["x_norm"], t0["x_norm"])
             assert abs(t["candidate_cost"] - t0["candidate_cost"]) <= 1e-9 * t0["candidate_cost"]
-        assert np.array_equal(p, res[0][0]) and np.array_equal(i, res[0][1])
+        assert np.array_equal(x["poses"], res[0]["poses"]) and np.array_equal(x["intr"], res[0]["intr"])
 
 
 @pytest.mark.parametrize("K,ptol", [(2, 0.0072), (2, 0.0054), (4, 0.0072)])
@@ -58,20 +35,21 @@ def test_parameter_tolerance_over_shards(K, ptol):
     """every rank stops where the unsharded solve stops; the tolerance lies strictly between two iterations of the
     unsharded trace (ratio step_norm / (ptol (|x| + ptol)) at least 1e-6 away from 1)"""
     c = far_points_first_case()
-    opt = options(parameter_tolerance=ptol)
-    trace0 = []
-    p0, i0, x0, summ0 = bo.lm_solve(c["poses"], c["intr"], c["points"], c["uv"], c["mask"], c["model"], c["mode"],
-                                    options=opt, trace=trace0)
+    opt = bo.LMOptions(max_num_iterations=20, function_tolerance=0.0, gradient_tolerance=0.0, parameter_tolerance=ptol)
+    ref = oracle_solve(c, opt=opt)
+    summ0 = ref["s"]
     assert summ0["termination"] == "CONVERGENCE_PARAMETER", summ0
-    ratios = [t["step_norm"] / (ptol * (t["x_norm"] + ptol)) for t in trace0 if t["outcome"] != 2]
+    ratios = [t["step_norm"] / (ptol * (t["x_norm"] + ptol)) for t in ref["trace"] if t["outcome"] != 2]
     assert all(abs(q - 1.0) > 1e-6 for q in ratios), ratios
     assert ratios[-1] < 1.0 and all(q > 1.0 for q in ratios[:-1]), ratios
-    res, group = run_sharded(c, K, opt)
-    check_against_unsharded(c, res, summ0, trace0)
+    res, group = run_shards(c["mask"].shape[1], K, lambda r, lo, hi, hook: oracle_solve(c, opt=opt, lo=lo, hi=hi,
+                                                                                           allreduce=hook),
+                            timeout=60.0)
+    check_against_unsharded(res, ref)
     assert len(group.tags[0]) >= 2 * summ0["iterations"]
-    for r, (p, i, x, summ, tr) in enumerate(res):
-        lo, hi = shard_range(c["mask"].shape[1], r, K)
-        assert np.abs(p - p0).max() < 1e-9 and np.abs(x - x0[lo:hi]).max() < 1e-9
+    for x in res:
+        assert np.abs(x["poses"] - ref["poses"]).max() < 1e-9
+        assert np.abs(x["points"] - ref["points"][x["lo"]:x["hi"]]).max() < 1e-9
 
 
 def test_local_x_norm_is_not_the_global_one():

@@ -18,18 +18,15 @@ Banded (video-like) problems run with the band hint on (points in creation order
 points in random order, which leaves the detection nothing to skip); each run is checked against the oracle on its
 own, and the hint the solver computed is read back through a development probe and compared with
 oracle/band_oracle.py table by table."""
-import ctypes
-
 import numpy as np
 import pytest
 
 from oracle import ba_oracle as bo
 from oracle import band_oracle
-from tests.helpers import ba_case, backward_error, banded_ba_case, recovered_step, reference_system, shuffled_twin, to_dev
+from tests.ba_harness import band_record, check_one_step, device_solve, options
+from tests.helpers import ba_case, banded_ba_case, shuffled_twin
 
 pytestmark = pytest.mark.gpu
-
-RADIUS = 1e4                # initial_trust_region_radius of the default options
 
 
 def _oracle_step(ref):
@@ -48,24 +45,9 @@ def _oracle_step(ref):
     return dcs, dps, ev[-1] / ev[0]
 
 
-def _band_record():
-    """the band hint of the most recent solve (vgg_dev_last_band_hint)"""
-    from vggsfm_b200 import _lib
-    L = _lib.lib()
-    meta = np.zeros(8, dtype=np.int32)
-    _lib.check(L.vgg_dev_last_band_hint(meta.ctypes.data, None, None, None, None), "vgg_dev_last_band_hint")
-    nb, KB, ng = int(meta[3]), int(meta[4]), int(meta[5])
-    rec = dict(active=bool(meta[0]), chol=bool(meta[1]), tables=bool(meta[2]), arrow_blk=int(meta[6]),
-               rb_range=np.zeros((nb, 2), np.int32), end_blk=np.zeros(nb, np.int32), kb_rows=np.zeros((KB, 2), np.int32),
-               fg_tracks=np.zeros((ng, 2), np.int32))
-    _lib.check(L.vgg_dev_last_band_hint(meta.ctypes.data, rec["rb_range"].ctypes.data, rec["end_blk"].ctypes.data,
-                                        rec["kb_rows"].ctypes.data, rec["fg_tracks"].ctypes.data), "vgg_dev_last_band_hint")
-    return rec
-
-
 def _check_band(c, band):
     """banded problem: the hint the solver took equals band_oracle.band_tables; band None or "shuffled" = dense expected"""
-    rec = _band_record()
+    rec = band_record()
     if band in (None, "shuffled"):
         assert not (rec["active"] or rec["chol"] or rec["tables"]), rec
         return
@@ -79,51 +61,21 @@ def _check_band(c, band):
 
 
 def _one_step(c, dev, param_const=None, point_const=None, label=""):
-    """run one LM iteration on the GPU and check it against the oracle's system; returns eta"""
-    import torch
-    from vggsfm_b200 import bundle_adjustment as ba
+    """run one LM iteration on the GPU and check it against the oracle's system (tests/ba_harness.py
+    check_one_step); prints the forward error against the oracle's own step"""
     S, N = c["mask"].shape
-    model, mode = c["model"], c["mode"]
-    dc, ns = bo.dims(model, mode)
     if param_const is None:
-        param_const = bo.default_param_const(S, model, mode)
+        param_const = bo.default_param_const(S, c["model"], c["mode"])
     if point_const is None:
         point_const = np.zeros(N, dtype=bool)
-    poses, intr, pts = to_dev(c["poses"], dev), to_dev(c["intr"], dev), to_dev(c["points"], dev)
-    o = ba.default_options()
-    o.max_num_iterations = 1
-    o.function_tolerance = o.gradient_tolerance = o.parameter_tolerance = 0.0
-    s = ba.lm_solve(to_dev(c["uv"], dev, torch.float32), to_dev(c["mask"].astype(np.uint8), dev), poses, intr, pts, model,
-                    mode, param_const=to_dev(param_const.astype(np.uint8), dev),
-                    point_const=to_dev(point_const.astype(np.uint8), dev), options=o, want_trace=True)
-    new = (poses.cpu().numpy(), intr.cpu().numpy(), pts.cpu().numpy())
-    tr = s.trace.numpy()
-    assert s.iterations == 1 and tr[0, 7] == 1, (label, tr)            # the step was accepted
-    assert tr[0, 5] == RADIUS
-
-    ref = reference_system(c, param_const, point_const, RADIUS)
-    assert abs(s.initial_cost - ref["cost"]) <= 1e-12 * ref["cost"], (label, s.initial_cost, ref["cost"])
-    d_c, u_c, d_p, u_p = recovered_step((c["poses"], c["intr"], c["points"]), new, S, dc, ns, model, mode)
-    assert not d_c[param_const].any() and not d_p[point_const].any()
-    dcs, ucs = d_c / ref["sc_c"], u_c / ref["sc_c"]
-    dps, ups = d_p / ref["sc_p"], u_p / ref["sc_p"]
-    eta = backward_error(ref, dcs, ucs, dps, ups)
-    # model change (oracle/ba_oracle.py lm_solve) and step norm at the recovered step
-    quad = (np.sum(dcs * dcs * ref["dcc"] / RADIUS * ref["fc"]) - np.sum(d_c * ref["gc"]) +
-            np.sum(dps * dps * ref["dpp"] / RADIUS * ref["fp"][:, None]) - np.sum(d_p * ref["gp"]))
-    model_change = 0.5 * quad
-    step_norm = np.sqrt(np.sum(d_c * d_c) + np.sum(d_p * d_p))
-    c_cost = bo.cost_only(*new, c["uv"], c["mask"], model)
-    ref_dcs, ref_dps, kappa = _oracle_step(ref)
+    o, _ = options(max_num_iterations=1, function_tolerance=0.0, gradient_tolerance=0.0, parameter_tolerance=0.0)
+    got = device_solve(c, dev, param_const=param_const, point_const=point_const, options=o)
+    step = check_one_step(c, got, param_const, point_const, label=label)
+    dcs, dps = step["dcs"], step["dps"]
+    ref_dcs, ref_dps, kappa = _oracle_step(step["ref"])
     fwd = max(np.abs(dcs - ref_dcs).max(), np.abs(dps - ref_dps).max()) / max(np.abs(ref_dcs).max(), np.abs(ref_dps).max())
-    print(f"lm step {label}: eta = {eta:.2e}  forward error vs oracle step = {fwd:.2e}  kappa2(reduced) = {kappa:.2e}  "
-          f"model change {abs(tr[0, 3] / model_change - 1):.1e}  step norm {abs(tr[0, 6] / step_norm - 1):.1e}  "
-          f"candidate cost {abs(tr[0, 2] / c_cost - 1):.1e}")
-    assert eta <= 1e-12, (label, eta)
-    assert abs(tr[0, 3] - model_change) <= 1e-10 * abs(model_change), (label, tr[0, 3], model_change)
-    assert abs(tr[0, 6] - step_norm) <= 1e-10 * step_norm, (label, tr[0, 6], step_norm)
-    assert abs(tr[0, 2] - c_cost) <= 1e-12 * c_cost, (label, tr[0, 2], c_cost)
-    return eta
+    print(f"lm step {label}: forward error vs oracle step = {fwd:.2e}  kappa2(reduced) = {kappa:.2e}")
+    return step["eta"]
 
 
 def _dense_case(name):

@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import ctypes
 import dataclasses
+import threading
 from typing import Optional
 
 import torch
@@ -112,19 +113,22 @@ def workspace_bytes(S: int, N: int, model: int, mode: int, iterative: bool = Fal
     return nbytes.value
 
 
-_ws_cache: dict = {}
+_ws_local = threading.local()
 
 
 def workspace(S: int, N: int, model: int, mode: int, device, iterative: bool = False) -> torch.Tensor:
+    """The solve's workspace, cached by shape per host thread, as the library's own caches are: two threads solving
+    the same shape (track-shard ranks in one process) never share one."""
+    cache = _ws_local.__dict__.setdefault("cache", {})
     key = (S, N, model, mode, str(device), iterative)
-    ws = _ws_cache.get(key)
+    ws = cache.get(key)
     if ws is None:
         with torch.cuda.device(device):
             nbytes = ctypes.c_size_t(workspace_bytes(S, N, model, mode, iterative))
-        if len(_ws_cache) > 4:
-            _ws_cache.clear()
+        if len(cache) > 4:
+            cache.clear()
         ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)
-        _ws_cache[key] = ws
+        cache[key] = ws
     return ws
 
 
