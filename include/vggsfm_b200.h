@@ -182,7 +182,8 @@ int vgg_ba_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt, void* wo
  * it (SCHUR_JACOBI preconditioner: one block per rotation, translation and camera-intrinsics parameter block), Ceres'
  * ConjugateGradientsSolver as LevenbergMarquardtStrategy calls it (x0 = 0, stop when i (Q_i - Q_{i-1}) / Q_i < eta and
  * i >= min, residual reset every 10 iterations; the first iteration always runs, so max 0 behaves as 1).  Its memory is
- * O(S N) for the caller's observation grid plus O(S + N) workspace: no [D x D] matrix. */
+ * O(S N) for the caller's observation grid (O(M) for an observation list, vgg_ba_solve_iterative_obs) plus O(S + N)
+ * workspace: no [D x D] matrix. */
 #define VGG_BA_DENSE_SCHUR 0
 #define VGG_BA_ITERATIVE_SCHUR 1
 typedef struct vgg_ba_linear_solver {
@@ -230,6 +231,39 @@ int vgg_ba_solve_iterative_sharded(const vgg_ba_problem* prob, const vgg_ba_opti
                                    const vgg_ba_linear_solver* lin, void* workspace, size_t ws_bytes,
                                    vgg_allreduce_fn allreduce, void* allreduce_user, vgg_ba_summary* summary,
                                    double* trace, double* cg_trace, void* stream);
+
+/* Observations as a list instead of the [S,N] grid: 9 B per grid cell become 20 B per observation (uv 8, frame 4,
+ * point 4, its frame_obs entry 4), so a video whose grid is almost all padding fits on one card.  Point-major: point n
+ * owns the list entries [track_start[n], track_start[n+1]), its frames strictly increasing (which excludes a second
+ * observation of one point in one frame); point[m] repeats the owner of entry m, so that the kernels that walk a frame
+ * find each observation's point without a search.  Frame-major view: frame s owns positions [frame_start[s],
+ * frame_start[s+1]) of frame_obs, which hold the list indices of its observations in ascending order.  Every listed
+ * observation is valid (there is no mask).  A point or a frame with an empty segment is constant whatever param_const
+ * and point_const say, and comes back bit for bit, NaN and inf included. */
+typedef struct vgg_ba_obs_list {
+  int64_t M;                   /* observations, 0 <= M < 2^30 (VGG_EINVAL beyond) */
+  const float* uv;             /* [M,2] pixels, point-major */
+  const int32_t* frame;        /* [M] frame of each observation, strictly increasing within a point */
+  const int32_t* point;        /* [M] point of each observation: n on [track_start[n], track_start[n+1]) */
+  const int32_t* track_start;  /* [N+1], track_start[0] = 0, track_start[N] = M, non-decreasing */
+  const int32_t* frame_start;  /* [S+1], frame_start[0] = 0, frame_start[S] = M, non-decreasing */
+  const int32_t* frame_obs;    /* [M] list indices of frame s at [frame_start[s], frame_start[s+1]), ascending */
+} vgg_ba_obs_list;
+/* Workspace of vgg_ba_solve_iterative_obs: vgg_ba_workspace_bytes_iterative's plus 3 doubles per point; O(S + N), the
+ * list itself is the caller's memory. */
+int vgg_ba_workspace_bytes_obs(int S, int N, int camera_model, int intr_mode, size_t* bytes);
+/* vgg_ba_solve_iterative_sharded on an observation list: the same ITERATIVE_SCHUR (SCHUR_JACOBI), loss, constant sets,
+ * hook contract and determinism rule; each rank passes the list of its own tracks.  prob->uv and prob->mask must be
+ * NULL, lin->type VGG_BA_ITERATIVE_SCHUR.  The list is checked once per solve by one kernel and one read of its flag
+ * word before the LM loop: VGG_EINVAL (with vgg_last_error naming the failed checks) unless track_start and frame_start
+ * have the ends and order above, every point[m] is the owner of entry m, every frame lies in [0, S) and increases
+ * strictly within its point, and every frame_obs entry is an observation of its segment's frame, strictly increasing
+ * within the segment.  Together these prove that frame_obs is the unique frame-major permutation of the list and that
+ * each frame's count of observations equals its segment's length. */
+int vgg_ba_solve_iterative_obs(const vgg_ba_problem* prob, const vgg_ba_obs_list* obs, const vgg_ba_options* opt,
+                               const vgg_ba_linear_solver* lin, void* workspace, size_t ws_bytes,
+                               vgg_allreduce_fn allreduce, void* allreduce_user, vgg_ba_summary* summary,
+                               double* trace, double* cg_trace, void* stream);
 
 int vgg_ba_reduced_system_doubles(int S, int camera_model, int intr_mode, size_t* doubles);
 int vgg_ba_fabric_doubles(int S, int camera_model, int intr_mode, size_t* doubles);
@@ -302,6 +336,16 @@ int vgg_filter_points3d(int S, int P, const double* points3d, const void* points
                         const double* extrinsics, const double* intrinsics9, const double* extra_params,
                         double max_reproj_error, double min_tri_angle_deg, int check_triangle, double hard_max,
                         uint8_t* out_valid, uint8_t* out_detail, void* workspace, size_t ws_bytes, void* stream);
+/* The point filter on an observation list (see vgg_ba_obs_list; only M, uv, frame and track_start are read): out_keep
+ * uint8 [M] = the observation reprojects within max_reproj_error at positive depth (the per-cell arithmetic of
+ * vgg_filter_points3d, bit for bit); out_valid uint8 [N] = at least two kept observations and one kept pair with a
+ * triangulation angle >= min_tri_angle_deg (COLMAP's ObservationManager::FilterAllPoints3D, which considers track
+ * elements only, where vgg_filter_points3d also counts an unobserved cell that reprojects within the bound).  An
+ * observation whose frame lies outside [0, S) is not kept.  workspace >= S*24 B. */
+int vgg_filter_observations(int S, int N, const vgg_ba_obs_list* obs, const double* points3d, const double* extrinsics,
+                            const double* intrinsics9, const double* extra_params, double max_reproj_error,
+                            double min_tri_angle_deg, uint8_t* out_keep, uint8_t* out_valid, void* workspace,
+                            size_t ws_bytes, void* stream);
 
 /* project_3D_points / img_from_cam (triangulation_helpers.py:311-395): out_points2d [S,P,2] and/or
  * out_points_cam [S,3,P] (either may be NULL). */

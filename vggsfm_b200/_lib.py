@@ -18,9 +18,10 @@ EXPORTS = [
     "vgg_ba_build_blocks", "vgg_ba_schur", "vgg_cholesky_lower", "vgg_ba_solve",
     "vgg_ba_reduced_system_doubles", "vgg_ba_fabric_doubles", "vgg_ba_solve_fabric",
     "vgg_ba_default_linear_solver", "vgg_ba_workspace_bytes_iterative", "vgg_ba_solve_iterative",
-    "vgg_ba_solve_iterative_sharded",
+    "vgg_ba_solve_iterative_sharded", "vgg_ba_workspace_bytes_obs", "vgg_ba_solve_iterative_obs",
     "vgg_pose_default_options", "vgg_pose_refinement", "vgg_pnp_workspace_bytes", "vgg_absolute_pose_estimation", "vgg_syrk_ozaki_workspace_bytes", "vgg_syrk_ozaki",
     "vgg_tri_workspace_bytes", "vgg_triangulate_tracks", "vgg_triangulate_by_pair", "vgg_filter_points3d",
+    "vgg_filter_observations",
     "vgg_project_points", "vgg_normalize_tracks", "vgg_undistort_simple_radial",
     "vgg_corr_pyramid_bytes", "vgg_corr_build_pyramid", "vgg_corr_sample", "vgg_sample_features4d",
     "vgg_corr_tc_supported", "vgg_corr_tc_bytes", "vgg_corr_tc_build", "vgg_corr_tc_sample",
@@ -82,6 +83,11 @@ class BASummary(ctypes.Structure):
         ("final_radius", ctypes.c_double), ("device_ms", ctypes.c_double),
         ("kernel_launches", ctypes.c_int64),
     ]
+
+
+class BAObsList(ctypes.Structure):
+    _fields_ = [("M", ctypes.c_int64), ("uv", ctypes.c_void_p), ("frame", ctypes.c_void_p), ("point", ctypes.c_void_p),
+                ("track_start", ctypes.c_void_p), ("frame_start", ctypes.c_void_p), ("frame_obs", ctypes.c_void_p)]
 
 
 class BAFabric(ctypes.Structure):
@@ -158,6 +164,10 @@ def lib() -> ctypes.CDLL:
     L.vgg_ba_solve_iterative_sharded.argtypes = [ctypes.POINTER(BAProblem), ctypes.POINTER(BAOptions),
                                                  ctypes.POINTER(BALinearSolver), vp, cs, ALLREDUCE_FN, vp,
                                                  ctypes.POINTER(BASummary), vp, vp, vp]
+    L.vgg_ba_workspace_bytes_obs.argtypes = [ci, ci, ci, ci, ctypes.POINTER(cs)]
+    L.vgg_ba_solve_iterative_obs.argtypes = [ctypes.POINTER(BAProblem), ctypes.POINTER(BAObsList),
+                                             ctypes.POINTER(BAOptions), ctypes.POINTER(BALinearSolver), vp, cs,
+                                             ALLREDUCE_FN, vp, ctypes.POINTER(BASummary), vp, vp, vp]
     L.vgg_dev_pcg_probe.argtypes = [ctypes.POINTER(BAProblem)] + [vp] * 6 + [cd] * 3 + [vp, vp, cs] + [vp] * 5
     L.vgg_pose_default_options.argtypes = [ctypes.POINTER(PoseOptions)]
     L.vgg_pose_default_options.restype = None
@@ -182,6 +192,7 @@ def lib() -> ctypes.CDLL:
     L.vgg_triangulate_tracks.argtypes = [ci, ci, vp, vp, vp, vp, vp, ci, ci, cd, cd, vp, vp, vp, vp, cs, vp]
     L.vgg_triangulate_by_pair.argtypes = [ci, ci, vp, vp, vp, vp, vp, vp, cs, vp]
     L.vgg_filter_points3d.argtypes = [ci, ci, vp, vp, ci, vp, vp, vp, cd, cd, ci, cd, vp, vp, vp, cs, vp]
+    L.vgg_filter_observations.argtypes = [ci, ci, ctypes.POINTER(BAObsList), vp, vp, vp, vp, cd, cd, vp, vp, vp, cs, vp]
     L.vgg_project_points.argtypes = [ci, ci, vp, vp, vp, vp, vp, vp, vp]
     L.vgg_normalize_tracks.argtypes = [ci, ci, vp, vp, vp, ci, vp, vp]
     L.vgg_undistort_simple_radial.argtypes = [ci, ci, vp, vp, ci, cd, cd, vp, ctypes.POINTER(ci), vp, cs, vp]

@@ -105,10 +105,13 @@ def linear_solver(linear_solver_type="DENSE_SCHUR", min_linear_solver_iterations
     return lin
 
 
-def workspace_bytes(S: int, N: int, model: int, mode: int, iterative: bool = False) -> int:
-    """Bytes of the solve's workspace: vgg_ba_workspace_bytes (direct) or vgg_ba_workspace_bytes_iterative."""
+def workspace_bytes(S: int, N: int, model: int, mode: int, iterative: bool = False, obs: bool = False) -> int:
+    """Bytes of the solve's workspace: vgg_ba_workspace_bytes (direct), vgg_ba_workspace_bytes_iterative, or with obs
+    vgg_ba_workspace_bytes_obs (the iterative solve on an observation list)."""
     nbytes = ctypes.c_size_t()
-    fn = _lib.lib().vgg_ba_workspace_bytes_iterative if iterative else _lib.lib().vgg_ba_workspace_bytes
+    L = _lib.lib()
+    fn = L.vgg_ba_workspace_bytes_obs if obs else L.vgg_ba_workspace_bytes_iterative if iterative else \
+        L.vgg_ba_workspace_bytes
     _lib.check(fn(S, N, model, mode, ctypes.byref(nbytes)), fn.__name__)
     return nbytes.value
 
@@ -116,15 +119,15 @@ def workspace_bytes(S: int, N: int, model: int, mode: int, iterative: bool = Fal
 _ws_local = threading.local()
 
 
-def workspace(S: int, N: int, model: int, mode: int, device, iterative: bool = False) -> torch.Tensor:
+def workspace(S: int, N: int, model: int, mode: int, device, iterative: bool = False, obs: bool = False) -> torch.Tensor:
     """The solve's workspace, cached by shape per host thread, as the library's own caches are: two threads solving
     the same shape (track-shard ranks in one process) never share one."""
     cache = _ws_local.__dict__.setdefault("cache", {})
-    key = (S, N, model, mode, str(device), iterative)
+    key = (S, N, model, mode, str(device), iterative, obs)
     ws = cache.get(key)
     if ws is None:
         with torch.cuda.device(device):
-            nbytes = ctypes.c_size_t(workspace_bytes(S, N, model, mode, iterative))
+            nbytes = ctypes.c_size_t(workspace_bytes(S, N, model, mode, iterative, obs))
         if len(cache) > 4:
             cache.clear()
         ws = torch.empty(nbytes.value, dtype=torch.uint8, device=device)
@@ -238,6 +241,7 @@ class Summary:
     cg_trace: Optional[torch.Tensor] = None   # [iterations, 4]: CG iterations, termination (CG_TERMINATION), zeta, |r|/|b|
     alive: Optional[torch.Tensor] = None      # [P'] points the negative-depth filter kept (bundle_adjustment only)
     mask: Optional[torch.Tensor] = None       # [S,P'] observations that were in the problem (bundle_adjustment only)
+    keep: Optional[torch.Tensor] = None       # [M] observations that were in the problem (bundle_adjustment_obs only)
 
 
 def check_allreduce(allreduce, linear_solver_type="DENSE_SCHUR"):
@@ -318,6 +322,108 @@ def lm_solve(uv, mask, poses, intr, points, model, mode, param_const=None, point
     if iterative:
         out.cg_trace = cg_trace[:summ.iterations]
         out.cg_iterations = int(out.cg_trace[:, 0].sum().item())
+    return out
+
+
+@dataclasses.dataclass
+class ObsList:
+    """An observation list as vgg_ba_solve_iterative_obs takes it (include/vggsfm_b200.h vgg_ba_obs_list), device
+    tensors: uv [M,2] f32, frame / point [M] and frame_obs [M] i32 point-major, track_start [N+1], frame_start [S+1];
+    order [M]: entry i of the list is the caller's observation order[i]."""
+    uv: torch.Tensor
+    frame: torch.Tensor
+    point: torch.Tensor
+    track_start: torch.Tensor
+    frame_start: torch.Tensor
+    frame_obs: torch.Tensor
+    order: torch.Tensor
+
+    def struct(self) -> "_lib.BAObsList":
+        return _lib.BAObsList(self.uv.shape[0], self.uv.data_ptr(), self.frame.data_ptr(), self.point.data_ptr(),
+                              self.track_start.data_ptr(), self.frame_start.data_ptr(), self.frame_obs.data_ptr())
+
+
+def obs_list(obs_uv, obs_frame, obs_point, S: int, N: int) -> ObsList:
+    """The list of COO observations (obs_uv [M,2], obs_frame [M], obs_point [M], any order) on S frames and N points:
+    sorted point-major by (point, frame), with its track segments and its frame-major permutation (stable sorts).
+    ValueError for shapes, indices outside [0, S) x [0, N), or a second observation of one point in one frame."""
+    M = obs_frame.shape[0]
+    if obs_uv.shape != (M, 2) or obs_frame.shape != (M,) or obs_point.shape != (M,):
+        raise ValueError(f"observations must be obs_uv [M,2], obs_frame [M], obs_point [M]; got "
+                         f"{tuple(obs_uv.shape)}, {tuple(obs_frame.shape)}, {tuple(obs_point.shape)}")
+    if M >= 2 ** 30:
+        raise ValueError(f"at most 2^30 - 1 observations, not {M}")
+    dev = obs_uv.device
+    fr, pt = obs_frame.to(dev, torch.int64), obs_point.to(dev, torch.int64)
+    if M and (fr.min() < 0 or fr.max() >= S or pt.min() < 0 or pt.max() >= N):
+        raise ValueError(f"observation frames must lie in [0, {S}) and points in [0, {N})")
+    key, order = torch.sort(pt * S + fr, stable=True)
+    if M > 1 and bool((key[1:] == key[:-1]).any()):
+        raise ValueError("a point is observed twice in one frame (duplicate (point, frame) observations)")
+    fr, pt = fr[order], pt[order]
+    zero = torch.zeros(1, dtype=torch.int64, device=dev)
+    track_start = torch.cat([zero, torch.cumsum(torch.bincount(pt, minlength=N), 0)])
+    frame_start = torch.cat([zero, torch.cumsum(torch.bincount(fr, minlength=S), 0)])
+    frame_obs = torch.sort(fr, stable=True).indices
+    i32 = lambda t: t.to(torch.int32).contiguous()
+    return ObsList(obs_uv[order].to(torch.float32).contiguous(), i32(fr), i32(pt), i32(track_start), i32(frame_start),
+                   i32(frame_obs), order)
+
+
+def lm_solve_obs(obs_uv, obs_frame, obs_point, poses, intr, points, model, mode, param_const=None, point_const=None,
+                 options: Optional[BAOptions] = None, allreduce=None, want_trace=False, min_linear_solver_iterations=0,
+                 max_linear_solver_iterations=500, eta=0.1, loss_function_type="TRIVIAL",
+                 loss_function_scale=1.0) -> Summary:
+    """lm_solve with ITERATIVE_SCHUR on observations given as a list instead of the [S, N] grid
+    (vgg_ba_solve_iterative_obs): COO (obs_uv [M,2], obs_frame [M], obs_point [M]) in any order, each one valid; memory
+    O(M) for the list and O(S + N) for the workspace.  The CG options, loss, allreduce (each rank passes the observations
+    of its own tracks) and trace are lm_solve's.  A point or frame without observations is constant and comes back bit
+    for bit.  ValueError (obs_list) for malformed observations."""
+    loss_function_id(loss_function_type)
+    lin = linear_solver("ITERATIVE_SCHUR", min_linear_solver_iterations, max_linear_solver_iterations, eta)
+    check_allreduce(allreduce, "ITERATIVE_SCHUR")
+    L = _lib.lib()
+    S, N = poses.shape[0], points.shape[0]
+    dev = poses.device
+    if param_const is None:
+        param_const = default_param_const(S, model, mode, dev)
+    if N == 0:
+        if obs_frame.shape[0] > 0:
+            raise ValueError("observations given for a problem without points")
+        # a rank without tracks: padding points without observations (constant), as lm_solve pads
+        N = pad_tracks(1)
+        points = torch.zeros(N, 3, dtype=torch.float64, device=dev)
+        points[:, 2] = 1.0
+        point_const = None
+    lst = obs_list(obs_uv, obs_frame, obs_point, S, N)
+    opt = options or default_options()
+    ws = workspace(S, N, model, mode, dev, iterative=True, obs=True)
+    p = BAProblem()                      # no grid: uv = mask = NULL
+    p.S, p.N, p.camera_model, p.intr_mode = S, N, model, mode
+    p.uv, p.mask = None, None
+    p.param_const = param_const.data_ptr()
+    p.point_const = point_const.data_ptr() if point_const is not None else None
+    for t in (poses, intr, points):
+        assert t.dtype == torch.float64 and t.is_contiguous() and t.is_cuda
+    p.poses, p.intr, p.points = poses.data_ptr(), intr.data_ptr(), points.data_ptr()
+    p.loss_function_type = loss_function_id(loss_function_type)
+    p.loss_function_scale = float(loss_function_scale)
+    ol = lst.struct()
+    summ = BASummary()
+    trace = torch.zeros(max(1, opt.max_num_iterations), 8, dtype=torch.float64) if want_trace else None
+    cg_trace = torch.zeros(max(1, opt.max_num_iterations), 4, dtype=torch.float64)
+    cb = allreduce.bind(ws) if allreduce is not None else _lib.ALLREDUCE_FN()
+    with torch.cuda.device(dev):
+        st = torch.cuda.current_stream().cuda_stream
+        rc = L.vgg_ba_solve_iterative_obs(ctypes.byref(p), ctypes.byref(ol), ctypes.byref(opt), ctypes.byref(lin),
+                                          ws.data_ptr(), ws.numel(), cb, None, ctypes.byref(summ),
+                                          trace.data_ptr() if trace is not None else None, cg_trace.data_ptr(), st)
+    _lib.check(rc, "vgg_ba_solve_iterative_obs")
+    out = Summary(summ.iterations, summ.successful, TERMINATION.get(summ.termination, "?"), summ.initial_cost,
+                  summ.final_cost, summ.final_radius, summ.device_ms, summ.kernel_launches,
+                  trace[:summ.iterations] if trace is not None else None, "ITERATIVE_SCHUR")
+    out.cg_trace = cg_trace[:summ.iterations]
+    out.cg_iterations = int(out.cg_trace[:, 0].sum().item())
     return out
 
 
@@ -451,6 +557,88 @@ def bundle_adjustment(points3d, extrinsics, intrinsics, extra_params, tracks, ma
 
 
 run_ba = bundle_adjustment   # the name BASELINE.json's north_star uses for this call
+
+
+def bundle_adjustment_obs(points3d, extrinsics, intrinsics, extra_params, obs_uv, obs_frame, obs_point,
+                          shared_camera=False, camera_type="SIMPLE_PINHOLE", options: Optional[BAOptions] = None,
+                          max_points3D_val=3000.0, allreduce=None, want_trace=False, refine_focal_length=True,
+                          refine_extra_params=True, const_pose=None, const_points=None, gauge=True, do_normalize=True,
+                          filter_reconstruction=True, drop_negative_depth=True, min_linear_solver_iterations=0,
+                          max_linear_solver_iterations=500, eta=0.1, loss_function_type="TRIVIAL",
+                          loss_function_scale=1.0):
+    """bundle_adjustment with ITERATIVE_SCHUR on observations given as a list (COO obs_uv [M,2], obs_frame [M],
+    obs_point [M] into points3d [P,3], any order) instead of the [S,P] grid, with the same COLMAP wrapper semantics:
+    points with >= 2 observations kept and renumbered in id order, the max_points3D_val clamp, the negative-depth filter
+    per observation, the gauge, the constant sets and both normalisations.  Returns bundle_adjustment's tuple
+    (points3D [P',3], extrinsics, intrinsics, extra_params, valid_idx [P'], Summary); Summary.alive is as there and
+    Summary.keep [M] bool (in the caller's order) replaces Summary.mask: the observations that were in the problem."""
+    model = camera_model_id(camera_type)
+    loss_function_id(loss_function_type)
+    linear_solver("ITERATIVE_SCHUR", min_linear_solver_iterations, max_linear_solver_iterations, eta)
+    check_allreduce(allreduce, "ITERATIVE_SCHUR")
+    dev = obs_uv.device
+    if not obs_uv.is_cuda:
+        raise RuntimeError("vggsfm_b200.bundle_adjustment_obs needs CUDA tensors (no CPU fallback)")
+    S, P0 = extrinsics.shape[0], points3d.shape[0]
+    fr, pt = obs_frame.to(dev, torch.int64), obs_point.to(dev, torch.int64)
+    M = fr.shape[0]
+    if M and (pt.min() < 0 or pt.max() >= P0 or fr.min() < 0 or fr.max() >= S):
+        raise ValueError(f"observation frames must lie in [0, {S}) and points in [0, {P0})")
+    count = torch.bincount(pt, minlength=P0)
+    valid_idx = torch.nonzero(count >= 2).flatten()                  # tensor_to_pycolmap.py:62-64
+    new_id = torch.full((P0,), -1, dtype=torch.int64, device=dev)
+    new_id[valid_idx] = torch.arange(valid_idx.numel(), device=dev)
+    pts = points3d.double()[valid_idx].contiguous()
+    P = pts.shape[0]
+    cp = new_id[pt]
+    m = (cp >= 0) & (pts < max_points3D_val).all(dim=1)[cp.clamp(min=0)]   # tensor_to_pycolmap.py:131-133
+    poses = extrinsics.double().contiguous().clone()
+    intr = torch.zeros(S, 4, dtype=torch.float64, device=dev)
+    intr[:, 0] = intrinsics[:, 0, 0]
+    intr[:, 1] = intrinsics[:, 0, 2]
+    intr[:, 2] = intrinsics[:, 1, 2]
+    if model == SIMPLE_RADIAL:
+        intr[:, 3] = extra_params[:, 0]
+    if shared_camera:
+        mode = INTR_SHARED
+        intr[:] = intr[0].clone()
+    else:
+        mode = INTR_PER_FRAME
+    if not (refine_focal_length or refine_extra_params):
+        mode = INTR_CONST
+    cpc = cp.clamp(min=0)
+    if drop_negative_depth:                                          # filter_negative_depth, per observation
+        depth = (poses[fr, 2, :3] * pts[cpc]).sum(dim=1) + poses[fr, 2, 3]
+        bad = m & ~(depth >= torch.finfo(torch.float64).eps)
+        length = torch.bincount(cpc[m], minlength=P)
+        nbad = torch.bincount(cpc[bad], minlength=P)
+        alive = (nbad == 0) | ((length - nbad) >= 2)
+        m = m & ~bad & alive[cpc]
+    else:
+        alive = torch.ones(P, dtype=torch.bool, device=dev)
+    point_const = torch.bincount(cpc[m], minlength=P) == 0
+    if const_points is not None:
+        point_const = point_const | const_points[valid_idx]
+    param_const = default_param_const(S, model, mode, dev, refine_focal_length, refine_extra_params, gauge, const_pose)
+    X = pts.clone()
+    summary = lm_solve_obs(obs_uv[m], fr[m], cpc[m], poses, intr, X, model, mode, param_const,
+                           point_const.to(torch.uint8), options, allreduce, want_trace, min_linear_solver_iterations,
+                           max_linear_solver_iterations, eta, loss_function_type, loss_function_scale)
+    pts = X
+    if do_normalize:
+        poses, pts = normalize(poses, pts, 10.0, 0.1, 0.9, alive)   # BundleAdjustmentController::Run
+        if filter_reconstruction:
+            poses, pts = normalize(poses, pts, 5.0, 0.1, 0.9, alive)    # filter_reconstruction (triangulation.py:1217)
+    pts = torch.where(alive[:, None], pts, torch.zeros_like(pts))
+    summary.alive, summary.keep = alive, m
+    K = torch.zeros(S, 3, 3, dtype=torch.float64, device=dev)
+    K[:, 0, 0] = intr[:, 0]
+    K[:, 1, 1] = intr[:, 0]
+    K[:, 0, 2] = intr[:, 1]
+    K[:, 1, 2] = intr[:, 2]
+    K[:, 2, 2] = 1.0
+    extra_out = intr[:, 3:4].clone() if model == SIMPLE_RADIAL else None
+    return pts, poses, K, extra_out, valid_idx, summary
 
 
 # --------------------------------------------------------------------------------------------------

@@ -44,39 +44,6 @@ constexpr int TB = 4;            // tracks per prefetch batch (32 B of uv per la
 constexpr int XT = 32;           // tracks per shared-memory point tile (one per lane)
 constexpr int PVS = 33;          // row stride of the per-point scratch (odd: conflict-free column sums)
 
-// ---- compile-time layout of the per-frame camera record: g_c[DC] | H_cc upper-packed | H_cs[6][NS] ----
-__host__ __device__ constexpr int pack_row(int dc, int p) {
-  int i = 0;
-  while (p >= dc - i) { p -= dc - i; ++i; }
-  return i;
-}
-__host__ __device__ constexpr int pack_col(int dc, int p) {
-  int i = 0;
-  while (p >= dc - i) { p -= dc - i; ++i; }
-  return i + p;
-}
-
-template <int DC, int NS, int K, int KR>
-__device__ __forceinline__ void cam_accumulate_one(double (&acc)[KR], const double* jc0, const double* jc1, double rx,
-                                                   double ry) {
-  constexpr int NPACK = DC * (DC + 1) / 2;
-  if constexpr (K < DC) {
-    acc[K] = fma(jc0[K], rx, fma(jc1[K], ry, acc[K]));
-  } else if constexpr (K < DC + NPACK) {
-    constexpr int i = pack_row(DC, K - DC), j = pack_col(DC, K - DC);
-    acc[K] = fma(jc0[i], jc0[j], fma(jc1[i], jc1[j], acc[K]));
-  } else {
-    constexpr int q = K - DC - NPACK;
-    constexpr int i = q / (NS > 0 ? NS : 1), j = q % (NS > 0 ? NS : 1);
-    acc[K] = fma(jc0[i], jc0[6 + j], fma(jc1[i], jc1[6 + j], acc[K]));
-  }
-}
-template <int DC, int NS, int KR, int... K>
-__device__ __forceinline__ void cam_accumulate(double (&acc)[KR], const double* jc0, const double* jc1, double rx,
-                                               double ry, std::integer_sequence<int, K...>) {
-  (cam_accumulate_one<DC, NS, K, KR>(acc, jc0, jc1, rx, ry), ...);
-}
-
 // coupling block (DC rows x 3, 16-byte stores into the staging buffer; only when W is written) and per-point values
 // (scratch column)
 template <int DC, int NS, int WB, bool WRITE_W>

@@ -18,7 +18,8 @@ enum : int {
   SMALL_COST = 0, SMALL_PT_QUAD = 1, SMALL_PT_STEP2 = 2, SMALL_PT_FAIL = 3, SMALL_GMAX_P = 4, SMALL_XNORM_P = 5,
   SMALL_MODEL_CHANGE = 6, SMALL_VEC = 8,
 };
-enum : int { INFO_CHOL = 0, INFO_TRSV = 1, INFO_FABRIC = 2, INFO_INTS = 4 };   // int info[INFO_INTS]
+// int info[INFO_INTS]; INFO_LIST: the flag word of an observation list's check (before the loop)
+enum : int { INFO_CHOL = 0, INFO_TRSV = 1, INFO_FABRIC = 2, INFO_LIST = 3, INFO_INTS = 4 };
 
 // The record pack_scalars_kernel gathers for the host's one read per iteration (cg: the CG state of csrc/ba_pcg.h).
 // The host reads REC_DOUBLES of it, REC_DOUBLES_CG in an iterative solve, into a buffer of REC_CAP.

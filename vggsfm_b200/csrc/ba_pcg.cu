@@ -781,6 +781,7 @@ int launch_pcg_assemble(const PcgOp& op, const double* q, const PcgBuffers& B, c
   VGG_CUDA_CHECK(cudaMemsetAsync(B.acc, 0, sizeof(double) * 9 * (size_t)pcg_blocks(p->S, op.ns), st));
   pcg_hc_kernel<<<(D + 255) / 256, 256, 0, st>>>(p->S, op.dc, op.ns, op.KR, op.camrec, op.shared_in, B.rhs, B.hdiag, B.gvec);
   VGG_LAUNCH_CHECK();
+  if (op.obs) return launch_list_rhs_jacobi(op, q, B, st);
   VGG_PICK_BA_KERNEL(kern, pcg_rhs_jacobi_kernel, p);
   const int nw = std::min(PJ_W, (p->S + 31) / 32);
   kern<<<(p->N + PJ_NT - 1) / PJ_NT, nw * 32, 0, st>>>(p->S, p->N, p->uv, p->mask, p->poses, p->intr, p->points,
@@ -808,6 +809,7 @@ int launch_pcg_matvec(const PcgOp& op, int pmode, const double* p_old, double* p
       p->S, op.dc, op.ns, op.KR, op.camrec, op.shared_in, B.hdiag, op.sc_c, p->param_const, op.radius, op.min_diag,
       op.max_diag, pmode, B.z, p_old, B.x, p_new, B.u, B.q, B.qs, B.cg);
   VGG_LAUNCH_CHECK();
+  if (op.obs) return launch_list_schur(op, B, st);
   VGG_PICK_BA_KERNEL(kern, pcg_schur_kernel, p);
   const int nw = std::min(PS_W, p->S);
   kern<<<(p->N + 31) / 32, nw * 32, 0, st>>>(p->S, p->N, p->uv, p->mask, p->poses, p->intr, p->points, p->point_const,

@@ -30,6 +30,14 @@ struct PcgBuffers {
   double *pinv;                 // [9 * pcg_blocks]: inverted preconditioner blocks
   double *cg;                   // [PCG_STATE_DOUBLES] scalars and termination
   double *slots;                // [pcg_slot_doubles]: per-CTA partials of the fixed-order CG reductions
+  double *tp;                   // [N * 3]: t_n = M_n M_n^T W_n^T u of the list matvec's point pass (list solve only)
+};
+
+// A validated vgg_ba_obs_list (csrc/ba_list.cu), M < 2^30: point-major uv / frame / point, frame-major frame_obs
+struct ObsList {
+  int M;
+  const float2* uv;
+  const int *frame, *point, *track_start, *frame_start, *frame_obs;
 };
 
 // the reduced operator of one LM iteration: the state, its camera records, point blocks M, camera scales and damping
@@ -39,6 +47,7 @@ struct PcgOp {
   const double *camrec, *shared_in, *M, *sc_c;
   double radius, min_diag, max_diag;
   const int* fg_tracks;
+  const ObsList* obs;           // the observation list, or null: the problem's grid
 };
 
 int pcg_blocks(int S, int ns);
@@ -52,5 +61,17 @@ int pcg_run(const PcgOp& op, const vgg_ba_linear_solver& lin, const PcgBuffers& 
             cudaStream_t st);
 int launch_pcg_model_change(const vgg_ba_problem* p, const double* M, const double* g_p, const double* wacc,
                             const double* d_c, const int* fg_tracks, double* out, cudaStream_t st);
+
+// the same steps on an observation list (csrc/ba_list.cu); *bad (zeroed by the caller) gets a non-zero word of
+// LIST_BAD_* bits for a malformed list
+int launch_list_validate(int S, int N, const ObsList& L, int* bad, cudaStream_t st);
+int launch_list_observed(int S, int N, const ObsList& L, uint8_t* point_seen, double* frame_seen, cudaStream_t st);
+int launch_list_blocks(const vgg_ba_problem* p, const ObsList& L, double* cost, double* camrec, double* g_p,
+                       double* H_pp, double* shared_out, cudaStream_t st);
+int launch_list_rhs_jacobi(const PcgOp& op, const double* q, const PcgBuffers& B, cudaStream_t st);
+int launch_list_schur(const PcgOp& op, const PcgBuffers& B, cudaStream_t st);
+int launch_list_backsub(const vgg_ba_problem* p, const ObsList& L, const double* d_c, double* wacc, cudaStream_t st);
+int launch_list_model_change(const vgg_ba_problem* p, const ObsList& L, const double* M, const double* g_p,
+                             const double* wacc, const double* d_c, double* out, cudaStream_t st);
 
 }  // namespace vgg

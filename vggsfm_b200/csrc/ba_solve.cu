@@ -209,8 +209,10 @@ struct Layout : Dims {
 
 // iterative: the layout of vgg_ba_solve_iterative -- the same buffers without the Schur operand Zt, the reduced system
 // AR and the factorisation workspace, plus the O(S + N) buffers of csrc/ba_pcg.cu: its O(D) vectors, the Schur-Jacobi
-// blocks, a copy of the camera records (summed over track shards) and the per-CTA slots of its fixed-order reductions
-static int make_layout(int S, int N, int model, int mode, void* base, size_t cap, Layout* L, bool iterative = false) {
+// blocks, a copy of the camera records (summed over track shards) and the per-CTA slots of its fixed-order reductions.
+// list: the iterative layout of vgg_ba_solve_iterative_obs, which adds the point pass's [N, 3] of the list matvec.
+static int make_layout(int S, int N, int model, int mode, void* base, size_t cap, Layout* L, bool iterative = false,
+                       bool list = false) {
   if (const int rc = dims_of(model, mode, S, N, L)) return rc;
   const int KR = L->KR, dc = L->dc, ns = L->ns;
   L->S = S;
@@ -256,6 +258,7 @@ static int make_layout(int S, int N, int model, int mode, void* base, size_t cap
     B.pinv = c.take<double>(9 * (size_t)pcg_blocks(S, ns));
     B.cg = c.take<double>(PCG_STATE_DOUBLES);
     B.slots = c.take<double>(pcg_slot_doubles(S, dc, ns));
+    B.tp = list ? c.take<double>((size_t)N * 3) : nullptr;
   }
   L->bytes = align_up(c.off, 256);
   if (base && c.off > cap) {
@@ -616,10 +619,11 @@ int vgg_ba_camrec_len(int camera_model, int intr_mode) {
   return d.KR;
 }
 
-static int workspace_bytes(int S, int N, int camera_model, int intr_mode, size_t* bytes, bool iterative) {
+static int workspace_bytes(int S, int N, int camera_model, int intr_mode, size_t* bytes, bool iterative,
+                           bool list = false) {
   VGG_REQUIRE(S > 0 && N > 0 && bytes, "S, N must be positive");
   Layout L;
-  const int rc = make_layout(S, N, camera_model, intr_mode, nullptr, 0, &L, iterative);
+  const int rc = make_layout(S, N, camera_model, intr_mode, nullptr, 0, &L, iterative, list);
   if (!rc) *bytes = L.bytes;
   return rc;
 }
@@ -771,6 +775,7 @@ struct LmContext {
   const vgg_ba_options& opt;
   const BandPlan& band;
   const Ranks& ranks;
+  const ObsList* obs;     // the observation list of a list solve, else null (the problem's grid)
 };
 
 // a linear step as cam_step reads it: the scaled camera step (entries stride apart), diag(H_cc) and the gradient
@@ -839,7 +844,7 @@ static int iterative_step(const LmContext& c, const vgg_ba_linear_solver& lin, c
                               c.opt.max_lm_diagonal, L.M, L.q, L.dpp, L.scal, st)))
     return rc;
   PcgOp op{&pcur, L.dc, L.ns, L.KR, b.camrec, b.shared, L.M, L.sc_c, radius, c.opt.min_lm_diagonal,
-           c.opt.max_lm_diagonal, c.band.dev.fg_tracks};
+           c.opt.max_lm_diagonal, c.band.dev.fg_tracks, c.obs};
   if ((rc = launch_pcg_assemble(op, L.q, B, st))) return rc;
   // track shards: the assembly and a copy of the camera records are this rank's partial sums, summed in one call.
   // The copy, not b itself: after a rejected step b is evaluated again and would be summed twice.
@@ -865,8 +870,11 @@ static int reduce_candidate(const LmContext& c, const vgg_ba_problem& pcur, int 
   const size_t count = SMALL_VEC + (size_t)L.Dpad;
   int rc;
   VGG_CUDA_CHECK(cudaMemsetAsync(L.small, 0, sizeof(double) * count, st));
-  if (iterative && (rc = launch_pcg_model_change(&pcur, L.M, L.blk[cur].g_p, L.wacc, L.d_c, c.band.dev.fg_tracks,
-                                                 L.small + SMALL_MODEL_CHANGE, st)))
+  if (iterative &&
+      (rc = c.obs ? launch_list_model_change(&pcur, *c.obs, L.M, L.blk[cur].g_p, L.wacc, L.d_c, L.small + SMALL_MODEL_CHANGE,
+                                             st)
+                  : launch_pcg_model_change(&pcur, L.M, L.blk[cur].g_p, L.wacc, L.d_c, c.band.dev.fg_tracks,
+                                            L.small + SMALL_MODEL_CHANGE, st)))
     return rc;
   VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + SMALL_COST, bn.cost, sizeof(double), cudaMemcpyDeviceToDevice, st));
   VGG_CUDA_CHECK(cudaMemcpyAsync(L.small + SMALL_PT_QUAD, L.scal + SCAL_PT_QUAD, sizeof(double) * 2, cudaMemcpyDeviceToDevice, st));
@@ -944,13 +952,45 @@ static bool lm_decide(const LmRecord& r, const vgg_ba_options& opt, bool iterati
   return true;
 }
 
+// The checks of vgg_ba_solve_iterative_obs on a list (csrc/ba_list.cu list_validate_kernel): one kernel, one read of
+// its flag word (dev_flag, a zeroed int of the workspace)
+static int check_list(int S, int N, const ObsList& ol, int* dev_flag, cudaStream_t st) {
+  int rc;
+  if ((rc = launch_list_validate(S, N, ol, dev_flag, st))) return rc;
+  int bad = 0;
+  VGG_CUDA_CHECK(cudaMemcpyAsync(&bad, dev_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+  VGG_CUDA_CHECK(cudaStreamSynchronize(st));
+  if (bad) {
+    set_error("malformed observation list:%s%s%s%s%s%s", bad & 1 ? " track_start (ends or order)" : "",
+              bad & 2 ? " point[] (not the owner of its track segment)" : "", bad & 4 ? " frame outside [0, S)" : "",
+              bad & 8 ? " frames not strictly increasing within a point" : "",
+              bad & 16 ? " frame_start (ends or order)" : "",
+              bad & 32 ? " frame_obs (not its segment's frame, or not strictly increasing)" : "");
+    return VGG_EINVAL;
+  }
+  return VGG_OK;
+}
+
 // The LM loop of both linear solvers: lin = null solves the reduced camera system directly (direct_step, DENSE_SCHUR),
 // otherwise by PCG (iterative_step, ITERATIVE_SCHUR; fabric null).  Everything else is the same code for both.
+// list: the observations as a list (ITERATIVE_SCHUR only; prob->uv and prob->mask null), checked before the loop.
 static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, const vgg_ba_linear_solver* lin,
                     void* workspace, size_t ws_bytes, vgg_allreduce_fn allreduce, void* ar_user,
-                    const vgg_ba_fabric* fabric, vgg_ba_summary* summary, double* trace, double* cg_trace, void* stream) {
+                    const vgg_ba_fabric* fabric, vgg_ba_summary* summary, double* trace, double* cg_trace, void* stream,
+                    const vgg_ba_obs_list* list = nullptr) {
   VGG_REQUIRE(prob && workspace && summary, "null pointer");
-  VGG_REQUIRE(prob->uv && prob->mask && prob->param_const && prob->poses && prob->intr && prob->points, "null problem array");
+  VGG_REQUIRE(prob->param_const && prob->poses && prob->intr && prob->points, "null problem array");
+  if (list) {
+    VGG_REQUIRE(!prob->uv && !prob->mask, "a list solve takes no grid: prob->uv and prob->mask must be NULL");
+    VGG_REQUIRE(lin && !fabric, "the observation list runs ITERATIVE_SCHUR only");
+    // 2^30: the kernels' 32-bit list indices stay clear of overflow after any loop or grid stride
+    VGG_REQUIRE(list->M >= 0 && list->M < ((int64_t)1 << 30), "observation list: need 0 <= M < 2^30");
+    VGG_REQUIRE(list->track_start && list->frame_start &&
+                    (list->M == 0 || (list->uv && list->frame && list->point && list->frame_obs)),
+                "observation list: null array");
+  } else {
+    VGG_REQUIRE(prob->uv && prob->mask, "null problem array");
+  }
   if (const int rc = check_loss(prob)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   g_launch_count = 0;
@@ -958,8 +998,17 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
   if (opt_in) opt = *opt_in;
   else vgg_ba_default_options(&opt);
   Layout L;
-  int rc = make_layout(prob->S, prob->N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L, lin != nullptr);
+  int rc = make_layout(prob->S, prob->N, prob->camera_model, prob->intr_mode, workspace, ws_bytes, &L, lin != nullptr,
+                       list != nullptr);
   if (rc) return rc;
+  ObsList ol{};
+  if (list) {
+    ol = ObsList{(int)list->M, reinterpret_cast<const float2*>(list->uv), list->frame, list->point, list->track_start,
+                 list->frame_start, list->frame_obs};
+    VGG_CUDA_CHECK(cudaMemsetAsync(L.dev_info, 0, sizeof(int) * INFO_INTS, st));
+    if ((rc = check_list(prob->S, prob->N, ol, L.dev_info + INFO_LIST, st))) return rc;
+  }
+  const ObsList* obs = list ? &ol : nullptr;
   const int S = L.S, N = L.N, D = L.D;
   Fabric fab;
   const bool fab_on = fabric && fabric->ar_local && fabric->ar_multicast;
@@ -973,19 +1022,24 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
   pe.point_const = L.point_const;
   prob = &pe;
   BandPlan band;
-  // the iterative solve factors nothing: each rank's band tables describe its own tracks, which is all its kernels read
-  if ((rc = compute_band_hint(prob, L.dc, D, L.Dpad, L.Kpad, !lin && (allreduce != nullptr || fabric != nullptr), st,
-                              &band)))
+  // the iterative solve factors nothing: each rank's band tables describe its own tracks, which is all its kernels read.
+  // A list solve has no grid to skip: its kernels walk the observations only.
+  if (!list && (rc = compute_band_hint(prob, L.dc, D, L.Dpad, L.Kpad, !lin && (allreduce != nullptr || fabric != nullptr),
+                                       st, &band)))
     return rc;
   g_band_last = band;
-  const LmContext c{L, opt, band, ranks};
+  const LmContext c{L, opt, band, ranks, obs};
   const size_t small_count = SMALL_VEC + (size_t)L.Dpad;
 
   VGG_CUDA_CHECK(cudaMemsetAsync(L.point_const, 0, (size_t)N, st));
   VGG_CUDA_CHECK(cudaMemsetAsync(L.small, 0, sizeof(double) * small_count, st));
-  observed_kernel<<<dim3((N + 255) / 256, (S + OBS_FRAMES - 1) / OBS_FRAMES), 256, 0, st>>>(S, N, pe.mask, L.point_const,
-                                                                                           L.small + SMALL_VEC);
-  VGG_LAUNCH_CHECK();
+  if (obs) {
+    if ((rc = launch_list_observed(S, N, *obs, L.point_const, L.small + SMALL_VEC, st))) return rc;
+  } else {
+    observed_kernel<<<dim3((N + 255) / 256, (S + OBS_FRAMES - 1) / OBS_FRAMES), 256, 0, st>>>(S, N, pe.mask, L.point_const,
+                                                                                             L.small + SMALL_VEC);
+    VGG_LAUNCH_CHECK();
+  }
   if ((rc = ranks.sum(L.small, small_count))) return rc;
   effective_const_kernel<<<(std::max(D, N) + 255) / 256, 256, 0, st>>>(S, N, L.dc, D, caller->param_const,
                                                                        caller->point_const, L.small + SMALL_VEC,
@@ -1022,6 +1076,7 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
     // cost | shared | camrec | g_p | H_pp are carved back to back: one memset covers all accumulators
     const size_t acc_bytes = reinterpret_cast<char*>(b.H_pp + (size_t)N * 6) - reinterpret_cast<char*>(b.cost);
     VGG_CUDA_CHECK(cudaMemsetAsync(b.cost, 0, acc_bytes, st));
+    if (obs) return launch_list_blocks(&p, *obs, b.cost, b.camrec, b.g_p, b.H_pp, b.shared, st);
     return ba_build_blocks(&p, b.cost, b.camrec, b.g_p, b.H_pp, nullptr, b.shared, 0, band.dev.fg_tracks, st, true);
   };
   double* h_rec = pinned_scalars();
@@ -1078,7 +1133,8 @@ static int lm_solve(const vgg_ba_problem* prob, const vgg_ba_options* opt_in, co
     have_scale_c = true;
     if ((rc = launch_cam_step(D, ls.dcs, ls.stride, L.sc_c, ls.hdiag, ls.gvec, prob->param_const, s.radius,
                               opt.min_lm_diagonal, opt.max_lm_diagonal, L.d_c, L.scal, st)) ||
-        (rc = launch_backsub(&pcur, L.d_c, L.wacc, band.dev.fg_tracks, st)) ||
+        (rc = obs ? launch_list_backsub(&pcur, *obs, L.d_c, L.wacc, st)
+                  : launch_backsub(&pcur, L.d_c, L.wacc, band.dev.fg_tracks, st)) ||
         (rc = launch_point_step(N, L.M, L.blk[cur].g_p, L.wacc, L.sc_p, L.dpp, prob->point_const, L.points[cur],
                                 s.radius, L.points[cand], L.scal, st)) ||
         (rc = launch_cam_update(S, L.dc, L.ns, prob->camera_model, L.d_c, L.poses[cur], L.intr[cur], L.poses[cand],
@@ -1127,17 +1183,36 @@ int vgg_ba_solve_iterative(const vgg_ba_problem* prob, const vgg_ba_options* opt
                                         stream);
 }
 
-int vgg_ba_solve_iterative_sharded(const vgg_ba_problem* prob, const vgg_ba_options* opt,
-                                   const vgg_ba_linear_solver* lin, void* workspace, size_t ws_bytes,
-                                   vgg_allreduce_fn allreduce, void* allreduce_user, vgg_ba_summary* summary,
-                                   double* trace, double* cg_trace, void* stream) {
+static int check_iterative(const vgg_ba_linear_solver* lin) {
   VGG_REQUIRE(lin && lin->type == VGG_BA_ITERATIVE_SCHUR, "vgg_ba_solve_iterative needs lin->type = VGG_BA_ITERATIVE_SCHUR");
   VGG_REQUIRE(lin->min_linear_solver_iterations >= 0 &&
                   lin->max_linear_solver_iterations >= lin->min_linear_solver_iterations && lin->eta > 0.0 &&
                   isfinite(lin->eta),
               "linear solver options: need 0 <= min <= max iterations and a positive finite eta");
+  return VGG_OK;
+}
+
+int vgg_ba_solve_iterative_sharded(const vgg_ba_problem* prob, const vgg_ba_options* opt,
+                                   const vgg_ba_linear_solver* lin, void* workspace, size_t ws_bytes,
+                                   vgg_allreduce_fn allreduce, void* allreduce_user, vgg_ba_summary* summary,
+                                   double* trace, double* cg_trace, void* stream) {
+  if (const int rc = check_iterative(lin)) return rc;
   return lm_solve(prob, opt, lin, workspace, ws_bytes, allreduce, allreduce_user, nullptr, summary, trace, cg_trace,
                   stream);
+}
+
+int vgg_ba_workspace_bytes_obs(int S, int N, int camera_model, int intr_mode, size_t* bytes) {
+  return workspace_bytes(S, N, camera_model, intr_mode, bytes, true, true);
+}
+
+int vgg_ba_solve_iterative_obs(const vgg_ba_problem* prob, const vgg_ba_obs_list* obs, const vgg_ba_options* opt,
+                               const vgg_ba_linear_solver* lin, void* workspace, size_t ws_bytes,
+                               vgg_allreduce_fn allreduce, void* allreduce_user, vgg_ba_summary* summary,
+                               double* trace, double* cg_trace, void* stream) {
+  VGG_REQUIRE(obs, "null observation list");
+  if (const int rc = check_iterative(lin)) return rc;
+  return lm_solve(prob, opt, lin, workspace, ws_bytes, allreduce, allreduce_user, nullptr, summary, trace, cg_trace,
+                  stream, obs);
 }
 
 /* development probe (csrc/dev_probes.h): the preparation of the iterative solve and one product of its reduced

@@ -17,6 +17,7 @@
 // early-exit search instead of a table.  Minimal HBM traffic: S*N*(16+2) B in, N*(24+8+S) B out.
 // All arithmetic is float64 like the reference's real pipeline (triangulator.py:91).
 #include "common.cuh"
+#include "tri_obs.h"
 
 namespace vgg {
 
@@ -153,19 +154,6 @@ __device__ __forceinline__ double tri_angle_deg(const double* c1, const double* 
   t = fmin(t, kPi - t);       // fmin drops NaN like torch.min? torch.min propagates NaN: handled by caller (>= false)
   if (c != c) t = c;
   return t * (180.0 / kPi);
-}
-
-// |cos| of the angle at X between two centres; returns 2 when the reference's guard gives angle 0
-__device__ __forceinline__ double tri_cos_abs(const double* c1, const double* c2, double X0, double X1, double X2) {
-  const double b0 = c1[0] - c2[0], b1 = c1[1] - c2[1], b2 = c1[2] - c2[2];
-  const double base2 = b0 * b0 + b1 * b1 + b2 * b2;
-  const double u0 = X0 - c1[0], u1 = X1 - c1[1], u2 = X2 - c1[2];
-  const double w0 = X0 - c2[0], w1 = X1 - c2[1], w2 = X2 - c2[2];
-  const double r1 = u0 * u0 + u1 * u1 + u2 * u2;
-  const double r2 = w0 * w0 + w1 * w1 + w2 * w2;
-  const double den = 2.0 * sqrt(r1 * r2);
-  if (den <= 1e-12) return 2.0;
-  return fabs((r1 + r2 - base2) / den);    // NaN propagates -> comparison false
 }
 
 struct TriParams {
@@ -550,30 +538,9 @@ __global__ void __launch_bounds__(256) filter_points_kernel(
   for (int w = 0; w < W; ++w) {
     const int s = w * 32 + lane;
     bool inl = false;
-    if (s < S) {
-      const double* Pm = cams + (size_t)s * 12;
-      const double p0 = Pm[0] * X0 + Pm[1] * X1 + Pm[2] * X2 + Pm[3];
-      const double p1 = Pm[4] * X0 + Pm[5] * X1 + Pm[6] * X2 + Pm[7];
-      const double p2 = Pm[8] * X0 + Pm[9] * X1 + Pm[10] * X2 + Pm[11];
-      double u = p0 / p2, v = p1 / p2;
-      if (extra) {
-        const double k = extra[s];
-        const double rad = k * (u * u + v * v);
-        const double du = u * rad, dv = v * rad;
-        u = u + du; v = v + dv;
-      }
-      const double* Km = K + (size_t)s * 9;
-      double x = Km[0] * u + Km[1] * v + Km[2];
-      double y = Km[3] * u + Km[4] * v + Km[5];
-      if (x != x) x = 0.0;                       // nan_to_num(nan=0); +-inf -> +-max
-      if (y != y) y = 0.0;
-      x = fmin(fmax(x, -1.7976931348623157e308), 1.7976931348623157e308);
-      y = fmin(fmax(y, -1.7976931348623157e308), 1.7976931348623157e308);
-      const double dx = x - (double)uv[((size_t)s * P + pidx) * 2], dy = y - (double)uv[((size_t)s * P + pidx) * 2 + 1];
-      double e2 = dx * dx + dy * dy;
-      if (p2 <= 0.0) e2 = 1e6;
-      inl = e2 <= max_err2;
-    }
+    if (s < S)
+      inl = filter_err2(cams, K, extra, s, X0, X1, X2, uv[((size_t)s * P + pidx) * 2],
+                        uv[((size_t)s * P + pidx) * 2 + 1]) <= max_err2;
     const uint32_t word = __ballot_sync(0xffffffffu, inl);
     if (lane == 0) bits[w] = word;
     cnt += __popc(word);
@@ -609,6 +576,43 @@ __global__ void __launch_bounds__(256) filter_points_kernel(
       detail[(size_t)s * P + pidx] = d ? 1 : 0;
     }
   }
+}
+
+// The point filter on an observation list (vgg_filter_observations), warp per point over its track segment
+// [track_start[n], track_start[n+1]): keep[m] = the observation reprojects within the bound at positive depth
+// (filter_err2, the grid filter's arithmetic); valid[n] = at least two kept observations and one kept pair whose
+// triangulation angle is at least the minimum (COLMAP's ObservationManager::FilterAllPoints3D, which considers the
+// track's elements only; the grid filter also counts an unobserved cell that happens to reproject within the bound)
+__global__ void __launch_bounds__(256) filter_obs_list_kernel(
+    int S, int N, const float* __restrict__ uv, const int* __restrict__ frame, const int* __restrict__ track_start,
+    const double* __restrict__ X, const double* __restrict__ cams, const double* __restrict__ centers,
+    const double* __restrict__ K, const double* __restrict__ extra, double max_err2, double cos_min_tri,
+    uint8_t* __restrict__ keep, uint8_t* __restrict__ valid) {
+  const int lane = threadIdx.x & 31, n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (n >= N) return;
+  const double X0 = X[(size_t)n * 3], X1 = X[(size_t)n * 3 + 1], X2 = X[(size_t)n * 3 + 2];
+  const int m0 = track_start[n], m1 = track_start[n + 1];
+  int cnt = 0;
+  for (int b = m0; b < m1; b += 32) {
+    const int m = b + lane;
+    const int s = m < m1 ? frame[m] : -1;
+    const bool inl = s >= 0 && s < S &&
+                     filter_err2(cams, K, extra, s, X0, X1, X2, uv[(size_t)m * 2], uv[(size_t)m * 2 + 1]) <= max_err2;
+    if (m < m1) keep[m] = inl ? 1 : 0;
+    cnt += __popc(__ballot_sync(0xffffffffu, inl));
+  }
+  __syncwarp();
+  bool tri_ok = false;
+  if (cnt >= 2)
+    for (int a = m0; a < m1 && !tri_ok; ++a) {
+      if (!keep[a]) continue;
+      const double* ca = centers + (size_t)frame[a] * 3;
+      bool found = false;
+      for (int b = a + 1 + lane; b < m1; b += 32)
+        if (keep[b] && tri_cos_abs(ca, centers + (size_t)frame[b] * 3, X0, X1, X2) <= cos_min_tri) found = true;
+      tri_ok = __any_sync(0xffffffffu, found);
+    }
+  if (lane == 0) valid[n] = (cnt >= 2 && tri_ok) ? 1 : 0;
 }
 
 // project_3D_points (triangulation_helpers.py:311-395): out[S,P,2], cam[S,3,P]
@@ -847,6 +851,29 @@ int vgg_filter_points3d(int S, int P, const double* points3d, const void* points
     filter_points_kernel<float><<<(P + 7) / 8, 256, smem, st>>>(S, P, points3d, (const float*)points2d, extrinsics, centers,
                                                                 intrinsics9, extra_params, e2, cosmin, check_triangle, hard_max,
                                                                 out_valid, out_detail);
+  VGG_LAUNCH_CHECK();
+  return VGG_OK;
+}
+
+int vgg_filter_observations(int S, int N, const vgg_ba_obs_list* obs, const double* points3d, const double* extrinsics,
+                            const double* intrinsics9, const double* extra_params, double max_reproj_error,
+                            double min_tri_angle_deg, uint8_t* out_keep, uint8_t* out_valid, void* workspace,
+                            size_t ws_bytes, void* stream) {
+  VGG_REQUIRE(obs && points3d && extrinsics && intrinsics9 && out_keep && out_valid && workspace && obs->track_start,
+              "null pointer");
+  VGG_REQUIRE(S >= 1 && N >= 0 && ws_bytes >= (size_t)S * 24, "bad sizes");
+  VGG_REQUIRE(obs->M >= 0 && obs->M < ((int64_t)1 << 30) && (obs->M == 0 || (obs->uv && obs->frame)),
+              "observation list: need 0 <= M < 2^30 and its uv and frame arrays");
+  cudaStream_t st = (cudaStream_t)stream;
+  g_launch_count = 0;
+  if (N == 0) return VGG_OK;
+  double* centers = reinterpret_cast<double*>(workspace);
+  proj_centers_kernel<<<(S + 127) / 128, 128, 0, st>>>(S, extrinsics, centers);
+  VGG_LAUNCH_CHECK();
+  filter_obs_list_kernel<<<(N + 7) / 8, 256, 0, st>>>(S, N, obs->uv, obs->frame, obs->track_start, points3d, extrinsics,
+                                                      centers, intrinsics9, extra_params,
+                                                      max_reproj_error * max_reproj_error,
+                                                      cos(min_tri_angle_deg * (kPi / 180.0)), out_keep, out_valid);
   VGG_LAUNCH_CHECK();
   return VGG_OK;
 }

@@ -177,6 +177,38 @@ def filter_all_points3D(points3D, points2D, extrinsics, intrinsics, extra_params
     return valid.bool(), (detail.bool() if detail is not None else None)
 
 
+def filter_observations(points3D, obs_uv, obs_frame, obs_point, extrinsics, intrinsics, extra_params=None,
+                        max_reproj_error=4, min_tri_angle=1.5):
+    """filter_all_points3D on observations given as a list (COO obs_uv [M,2], obs_frame [M], obs_point [M] into
+    points3D [P,3], any order) instead of the [S,P] grid (vgg_filter_observations).  Returns (keep [M] bool in the
+    caller's order: reprojection error <= max_reproj_error at positive depth, valid [P] bool: >= 2 kept observations
+    and one kept pair with a triangulation angle >= min_tri_angle degrees).  The per-observation arithmetic is the grid
+    filter's; unlike the grid filter, an unobserved frame never counts (COLMAP's FilterAllPoints3D)."""
+    from . import bundle_adjustment as ba
+    _need_cuda(obs_uv, "obs_uv")
+    L = _lib.lib()
+    S, P = extrinsics.shape[0], points3D.shape[0]
+    dev = obs_uv.device
+    lst = ba.obs_list(obs_uv, obs_frame, obs_point, S, P)
+    M = lst.frame.shape[0]
+    keep_l = torch.zeros(M, dtype=torch.uint8, device=dev)
+    valid = torch.zeros(P, dtype=torch.uint8, device=dev)
+    X = _f64c(points3D)
+    E = _f64c(extrinsics.reshape(S, 12))
+    K = _f64c(intrinsics.reshape(S, 9))
+    ex = _f64c(extra_params[:, 0]) if extra_params is not None else None
+    ws = torch.empty(S * 24 + 64, dtype=torch.uint8, device=dev)
+    ol = lst.struct()
+    with torch.cuda.device(dev):
+        _lib.check(L.vgg_filter_observations(S, P, ctypes.byref(ol), X.data_ptr(), E.data_ptr(), K.data_ptr(),
+                                             ex.data_ptr() if ex is not None else None, float(max_reproj_error),
+                                             float(min_tri_angle), keep_l.data_ptr(), valid.data_ptr(), ws.data_ptr(),
+                                             ws.numel(), _stream(dev)), "vgg_filter_observations")
+    keep = torch.zeros(M, dtype=torch.bool, device=dev)
+    keep[lst.order] = keep_l.bool()
+    return keep, valid.bool()
+
+
 def project_3D_points(points3D, extrinsics, intrinsics=None, extra_params=None, return_points_cam=False, default=0,
                       only_points_cam=False):
     """vggsfm/utils/triangulation_helpers.py:311-355: points2D [S,P,2] (and points_cam [S,3,P])."""

@@ -88,7 +88,7 @@ def window_bundle_adjustment(window_points_all, extrinsics, intrinsics, extra_pa
 
 def joint_BA(points3D, extrinsics, intrinsics, extra_params, tracks, masks, camera_type="SIMPLE_PINHOLE", reproj_error=2.0,
              tri_angle=1.5, normalize=True, linear_solver_type="DENSE_SCHUR", min_linear_solver_iterations=0,
-             max_linear_solver_iterations=500, eta=0.1, allreduce=None):
+             max_linear_solver_iterations=500, eta=0.1, allreduce=None, options=None):
     """Tensor form of VideoRunner.joint_BA (video_runner.py:494-541): all frames so far, all points, ONE shared
     camera, default Ceres options through the COLMAP controller (gauge + negative-depth filter + Normalize), then the
     2 px / 1.5 degree point filter and a second normalisation.  The runner keeps this state in its point_dict /
@@ -103,7 +103,8 @@ def joint_BA(points3D, extrinsics, intrinsics, extra_params, tracks, masks, came
     linear_solver_type="ITERATIVE_SCHUR" (and the CG options of bundle_adjustment.lm_solve) solves long sequences whose
     dense reduced camera system does not fit in memory.  `allreduce` (vggsfm_b200.dist.AllReduceHook) runs the BA over
     track shards with either linear solver: every rank passes all frames and its own slice of the points (normalize
-    reads the cameras only, and the point filter is per point, so the rest of the call is the rank's own)."""
+    reads the cameras only, and the point filter is per point, so the rest of the call is the rank's own).  options: the
+    BA's BAOptions (default: bundle_adjustment.default_options())."""
     S, P = masks.shape
     K = intrinsics.expand(S, -1, -1)
     ex = extra_params.expand(S, -1) if extra_params is not None else None
@@ -112,8 +113,8 @@ def joint_BA(points3D, extrinsics, intrinsics, extra_params, tracks, masks, came
         poses, pts = ba.normalize(poses, pts, 5.0, 0.1, 0.9)                             # :503-504
     global last_joint_summary
     pts_o, extr, K_o, ex_o, valid_idx, summary = ba.bundle_adjustment(
-        pts, poses, K, ex, tracks, masks, shared_camera=True, camera_type=camera_type, options=ba.default_options(),
-        filter_reconstruction=False, linear_solver_type=linear_solver_type,
+        pts, poses, K, ex, tracks, masks, shared_camera=True, camera_type=camera_type,
+        options=options or ba.default_options(), filter_reconstruction=False, linear_solver_type=linear_solver_type,
         min_linear_solver_iterations=min_linear_solver_iterations,
         max_linear_solver_iterations=max_linear_solver_iterations, eta=eta, allreduce=allreduce)
     last_joint_summary = summary
@@ -131,6 +132,57 @@ def joint_BA(points3D, extrinsics, intrinsics, extra_params, tracks, masks, came
     if normalize:
         extr, out = ba.normalize(extr, out, 5.0, 0.1, 0.9, valid_points)                 # :513-514
     return out, extr, K_o[:1].clone(), (ex_o[:1].clone() if ex_o is not None else None), new_masks, valid_points
+
+
+def joint_BA_obs(points3D, extrinsics, intrinsics, extra_params, obs_uv, obs_frame, obs_point,
+                 camera_type="SIMPLE_PINHOLE", reproj_error=2.0, tri_angle=1.5, normalize=True,
+                 min_linear_solver_iterations=0, max_linear_solver_iterations=500, eta=0.1, allreduce=None, options=None):
+    """joint_BA with ITERATIVE_SCHUR on the observations as a list -- the form VideoRunner.joint_BA hands COLMAP, each
+    point carrying its track (video_runner.py:494-541) -- instead of the [S,P] grid: COO obs_uv [M,2], obs_frame [M],
+    obs_point [M] into points3D [P,3].  bundle_adjustment_obs, then the point filter on the list
+    (triangulation.filter_observations: reprojection <= reproj_error at positive depth per observation, >= 2 survivors,
+    one surviving pair with >= tri_angle) and the second normalisation.  Returns (points3D [P,3], extrinsics [S,3,4],
+    intrinsics [1,3,3], extra_params [1,1]|None, keep [M] bool, valid_points [P]) -- keep is the list form of
+    joint_BA's masks.  options: the BA's BAOptions (default: bundle_adjustment.default_options())."""
+    S, P = extrinsics.shape[0], points3D.shape[0]
+    K = intrinsics.expand(S, -1, -1)
+    ex = extra_params.expand(S, -1) if extra_params is not None else None
+    poses, pts = extrinsics.double(), points3D.double()
+    if normalize:
+        poses, pts = ba.normalize(poses, pts, 5.0, 0.1, 0.9)                             # :503-504
+    global last_joint_summary
+    pts_o, extr, K_o, ex_o, valid_idx, summary = ba.bundle_adjustment_obs(
+        pts, poses, K, ex, obs_uv, obs_frame, obs_point, shared_camera=True, camera_type=camera_type,
+        options=options or ba.default_options(), filter_reconstruction=False,
+        min_linear_solver_iterations=min_linear_solver_iterations,
+        max_linear_solver_iterations=max_linear_solver_iterations, eta=eta, allreduce=allreduce)
+    last_joint_summary = summary
+    out = pts.clone()
+    out[valid_idx] = pts_o
+    keep, ok_tri = tri.filter_observations(out, obs_uv, obs_frame, obs_point, extr, K_o, extra_params=ex_o,
+                                           max_reproj_error=reproj_error, min_tri_angle=tri_angle)
+    in_problem = torch.zeros(P, dtype=torch.bool, device=out.device)
+    in_problem[valid_idx] = True
+    op = obs_point.to(out.device, torch.int64)
+    keep = keep & in_problem[op]
+    valid_points = (torch.bincount(op[keep], minlength=P) >= 2) & ok_tri
+    keep = keep & valid_points[op]
+    if normalize:
+        extr, out = ba.normalize(extr, out, 5.0, 0.1, 0.9, valid_points)                 # :513-514
+    return out, extr, K_o[:1].clone(), (ex_o[:1].clone() if ex_o is not None else None), keep, valid_points
+
+
+# The grid path's peak device memory in SceneStore.joint_bundle_adjustment, as a multiple of the 9 S P bytes of its
+# [S,P] grid (uv 8 B + mask 1 B per cell): 3.01 measured on an H100 80GB HBM3 (700 W) by tools/ba_obs_bench.py on the
+# 2500-frame joint BA (tools/video_c5.py final_problem_arrays(2500, 2048): the grid's 7.2 GB plus 14.5 GB the call
+# allocates beside it), rounded up; see DESIGN 4.10.
+GRID_PEAK_MULTIPLE = 3.1
+
+
+def grid_fits(S, P, device) -> bool:
+    """whether the grid path of a joint BA over S frames and P points fits on `device`: GRID_PEAK_MULTIPLE x 9 S P
+    bytes within the device's total memory"""
+    return GRID_PEAK_MULTIPLE * 9.0 * S * P <= torch.cuda.get_device_properties(device).total_memory
 
 
 class SceneStore:
@@ -222,17 +274,56 @@ class SceneStore:
         self.has_extri[:] = False
         self.set_extrinsics(start_idx, extrinsics)
 
+    def observations(self, start_idx, end_idx):
+        """The observations of frames [start, end) as a list: (xyz [P,3] f64, obs_uv [M,2] f32, obs_frame [M] (relative
+        to start), obs_point [M], extrinsics [S,3,4])."""
+        sel = (self.obs_frame >= start_idx) & (self.obs_frame < end_idx)
+        return (self.xyz.double(), self.obs_uv[sel], self.obs_frame[sel] - start_idx, self.obs_point[sel],
+                self.extri[start_idx:end_idx].clone())
+
+    def replace_from_obs(self, start_idx, points3D, extrinsics, obs_uv, obs_frame, obs_point, keep_obs, keep):
+        """replace_from_ba on the list form of the BA's result: points `keep` [P] survive and are renumbered in id
+        order, their observations are the list entries `keep_obs` [M] (obs_frame relative to start_idx), stored in the
+        (frame, point) order replace_from_ba gives them; visibilities become 1, xyz is stored as float32."""
+        new_id = torch.cumsum(keep.long(), 0) - 1
+        self.xyz = points3D[keep].float()
+        self.rgb = self.rgb[keep]
+        op = obs_point.to(torch.int64)
+        sel = keep_obs & keep[op]
+        f, p, uv = obs_frame[sel].to(torch.int64), new_id[op[sel]], obs_uv[sel]
+        order = torch.sort(f * max(1, self.num_points) + p).indices
+        self.obs_point = p[order]
+        self.obs_frame = f[order] + start_idx
+        self.obs_uv = uv[order].float()
+        self.obs_vis = torch.ones(order.numel(), dtype=torch.float32, device=self.device)
+        self.has_extri[:] = False
+        self.set_extrinsics(start_idx, extrinsics)
+
     def joint_bundle_adjustment(self, start_idx, end_idx, intrinsics, extra_params, camera_type="SIMPLE_PINHOLE",
                                 reproj_error=2.0, tri_angle=1.5, normalize=True, linear_solver_type="DENSE_SCHUR",
-                                min_linear_solver_iterations=0, max_linear_solver_iterations=500, eta=0.1):
+                                min_linear_solver_iterations=0, max_linear_solver_iterations=500, eta=0.1,
+                                options=None):
         """VideoRunner.joint_BA (:494-541) on the store: dense view -> joint_BA (CUDA) -> store rebuilt from the result.
-        Returns the refined shared (intrinsics [1,3,3], extra_params [1,1]|None).  Linear-solver options as joint_BA."""
+        Returns the refined shared (intrinsics [1,3,3], extra_params [1,1]|None).  Linear-solver options as joint_BA.
+        With ITERATIVE_SCHUR a problem whose grid does not fit on the device (grid_fits) takes the observation list
+        instead (joint_BA_obs, replace_from_obs); every problem that fits runs the grid path.  options: the BA's
+        BAOptions (default: bundle_adjustment.default_options())."""
+        S, P = end_idx - start_idx, self.num_points
+        if linear_solver_type == "ITERATIVE_SCHUR" and not grid_fits(S, P, self.device):
+            xyz, uv, fr, pt, extr = self.observations(start_idx, end_idx)
+            pts, extr, K, ex, keep_obs, valid = joint_BA_obs(
+                xyz, extr, intrinsics, extra_params, uv, fr, pt, camera_type=camera_type, reproj_error=reproj_error,
+                tri_angle=tri_angle, normalize=normalize, min_linear_solver_iterations=min_linear_solver_iterations,
+                max_linear_solver_iterations=max_linear_solver_iterations, eta=eta, options=options)
+            self.replace_from_obs(start_idx, pts, extr, uv, fr, pt, keep_obs, valid)
+            return K.float(), (ex.float() if ex is not None else None)
         xyz, tracks, masks, extr = self.dense(start_idx, end_idx)
         pts, extr, K, ex, new_masks, valid = joint_BA(xyz, extr, intrinsics, extra_params, tracks, masks, camera_type=camera_type,
                                                       reproj_error=reproj_error, tri_angle=tri_angle, normalize=normalize,
                                                       linear_solver_type=linear_solver_type,
                                                       min_linear_solver_iterations=min_linear_solver_iterations,
-                                                      max_linear_solver_iterations=max_linear_solver_iterations, eta=eta)
+                                                      max_linear_solver_iterations=max_linear_solver_iterations, eta=eta,
+                                                      options=options)
         self.replace_from_ba(start_idx, pts, extr, tracks, new_masks, valid)
         return K.float(), (ex.float() if ex is not None else None)
 
